@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- call-graph DAGs/sec (forward + backward + optimizer step) on B200, per the driver contract.
+"""bench.py -- call-graph DAGs/sec (forward + backward + optimizer step) on NVIDIA H100 GPUs.
 
   python bench.py --gpus N --steps K --warmup W            # this repository's CUDA path
+  python bench.py ... --dump-outputs DIR                    # + what the timed path computed in its last step, as .npy
   python bench.py --impl reference --gpus N --steps K ...   # reference-semantics CPU path (oracle) on host cores
 
 Workload (BASELINE.json configs[1]): Alibaba-trace-shaped synthetic batch, 256 DAGs x 200 nodes / 600 edges,
@@ -12,7 +13,7 @@ train.PeerAdam, with one NCCL all-reduce of the flat gradient as the fallback).
 Arms and JSON keys beyond the base contract:
   value         train.GraphedTrainStep on 8 rotating RESIDENT batches: index build + forward + pinball loss +
                 backward replayed from one CUDA graph per batch buffer, then the (fused) Adam  [PERT_BENCH_GRAPH=0:
-                eager train.fused_train_step]; CUDA events around exactly K steps, max over ranks
+                eager train.fused_train_step]; CUDA events around exactly K = --steps steps, max over ranks
   e2e           the same step fed from pinned HOST batches: data.DevicePrefetcher (one H2D copy per step on a side
                 stream, one step ahead) + graph replay + Adam + every step's loss read back (train.AsyncLossReader)
   e2e_dropin    the reference's own loop body (pert_gnn.py:219-250) around the drop-in model, unchanged: pinned host
@@ -20,7 +21,7 @@ Arms and JSON keys beyond the base contract:
   kernels       per-kernel in-step times: CUDA events recorded by the engine (PertProbe) around one kernel family per
                 step, in eagerly issued train steps run right after the timed region
   roofline      the kernel family with the largest share of the step: algorithmic bytes / its in-step time against
-                the measured HBM peak (MEASURED_PEAKS.json); traffic = DRAM bytes from the committed ncu capture
+                the HBM peak (MEASURED_PEAKS.json when present, else the H100 SXM data-sheet 3.35 TB/s)
   scatter_max   the BASELINE metric kernel ([E,64] -> [N,64] segment-max): trains of launches over rotating buffers
                 larger than L2 (and the single-launch-after-flush time)
   cpu_baseline  the oracle (torch restatement of the reference's PyG 2.4.0 ops) on this box's host cores, thread
@@ -52,7 +53,7 @@ def _peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -314,18 +315,6 @@ def cpu_baseline(cfg, budget_s=25.0):
 _BENCH_CFG = 2
 
 
-def ncu_traffic(kernel):
-    """DRAM bytes per launch (read + write) of a kernel family from the committed ncu --set full capture
-    (profiles/r1_traffic.json, cfg2 shapes only); None when there is no capture for it."""
-    if _BENCH_CFG != 2:
-        return None
-    try:
-        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r2_traffic.json")) as f:
-            return json.load(f).get(kernel)
-    except (OSError, ValueError):
-        return None
-
-
 def scatter_max_bench(batch_dev, H, peak_gbs, iters=40):
     """BASELINE metric kernel: segment-max of msg[E,H] (CSR order) -> out[N,H].
 
@@ -340,7 +329,7 @@ def scatter_max_bench(batch_dev, H, peak_gbs, iters=40):
     N, E = batch_dev.x.size(0), batch_dev.edge_index.size(1)
     gi = build_index(batch_dev.edge_index, N)
     bytes_alg = 4 * E * H + 4 * (N + 1) + 4 * N * H
-    ROT = max(4, int(3 * (160 << 20) // max(bytes_alg, 1)) + 1)     # >= 3 x 160 MB of distinct data in rotation
+    ROT = max(4, int(3 * (160 << 20) // max(bytes_alg, 1)) + 1)     # >= 3 x 160 MB of distinct data (L2: 50 MB)
     TRAIN = 2 * ROT
     msgs = [torch.randn(E, H, device="cuda") for _ in range(ROT)]
     outs = [torch.empty(N, H, device="cuda") for _ in range(ROT)]
@@ -375,7 +364,7 @@ def scatter_max_bench(batch_dev, H, peak_gbs, iters=40):
     t_single, t_train = statistics.median(single), statistics.median(train)
     ach = bytes_alg / t_train / 1e9
     return {"kernel": "k_segreduce_stream<max> [E,H]->[N,H] (TMA bulk + mbarrier pipeline)", "bound": "hbm",
-            "achieved": ach, "peak": peak_gbs, "unit": "GB/s", "frac": ach / peak_gbs, "traffic": ncu_traffic("scatter_max"),
+            "achieved": ach, "peak": peak_gbs, "unit": "GB/s", "frac": ach / peak_gbs,
             "algorithmic_bytes": bytes_alg, "us_per_launch": t_train * 1e6,
             "protocol": f"{TRAIN} back-to-back launches over {ROT} distinct msg/out buffer pairs "
                         f"({ROT * bytes_alg >> 20} MB > L2), event pair around the train, median of 10",
@@ -394,34 +383,32 @@ def _workload_string(cfg, B):
             f"num_layers={c['num_layers']}, fwd+bwd+Adam")
 
 
-def timed_blocks(run_block, K, barrier, world, dev, min_region_s=0.6, max_blocks=300, min_blocks=5):
-    """Times R blocks of EXACTLY K steps each (barrier + synchronize on both sides of every block, CUDA events around
-    it, max over ranks per block) and returns (median seconds per block, list of block seconds).  R is chosen so that
-    the whole timed region lasts >= min_region_s: a 13 ms region (20 steps of 0.67 ms) gives NVML no samples and lets
-    one scheduler hiccup move the headline by percents."""
+def timed_blocks(run_block, K, barrier, world, dev):
+    """Times ONE block of exactly K steps (barrier + synchronize on both sides, CUDA events around it, max over
+    ranks) and returns (seconds, [seconds])."""
     import torch.distributed as dist
 
-    def one():
-        barrier()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        run_block(K)
-        e1.record()
-        barrier()
-        return e0.elapsed_time(e1) * 1e-3
+    barrier()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    run_block(K)
+    e1.record()
+    barrier()
+    sec = e0.elapsed_time(e1) * 1e-3
+    if world > 1:
+        t = torch.tensor([sec], device=dev)
+        dist.all_reduce(t, op=dist.ReduceOp.MAX)
+        sec = float(t)
+    return sec, [sec]
 
-    est = one()
-    if world > 1:
-        t = torch.tensor([est], device=dev)
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        est = float(t)
-    R = int(min(max_blocks, max(min_blocks, -(-min_region_s // max(est, 1e-6)))))
-    secs = [one() for _ in range(R)]
-    if world > 1:
-        t = torch.tensor(secs, device=dev)
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        secs = t.tolist()
-    return statistics.median(secs), secs
+
+def dump_outputs(out_dir, named):
+    """Writes every array of `named` as out_dir/<name>.npy in float32 (what the timed path handed its caller)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in named.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 def first_step_parity(model, batch_host, dev, tau=0.5):
@@ -546,6 +533,9 @@ def run_b200(args, rank, world, local_rank):
     t_wall = time.perf_counter()
     secs, blocks = timed_blocks(resident_block, args.steps, barrier, world, dev)
     t_wall = time.perf_counter() - t_wall
+    if args.dump_outputs and rank == 0:
+        # the last timed step's loss, and the parameters and gradients it left in the flat buffers
+        dump_outputs(args.dump_outputs, {"loss": state["loss"], "params": fp.flat, "grads": fp.grad})
     launches_per_step = (ops.LAUNCHES["n"] - l0) / max(1, state["i"] - s0)
     clocks = sampler.stop() if rank == 0 else None
     peer_phases = opt.phase_times_us(reset=True) if hasattr(opt, "phase_times_us") and world > 1 else None
@@ -592,7 +582,7 @@ def run_b200(args, rank, world, local_rank):
             st2["i"] += 1
 
     dropin_block(args.warmup)
-    secs2, _ = timed_blocks(dropin_block, args.steps, barrier, world, dev, min_region_s=0.3, max_blocks=40)
+    secs2, _ = timed_blocks(dropin_block, args.steps, barrier, world, dev)
     e2e_val = world * B * args.steps / secs2
 
     # ---- end-to-end through the fused public API: pinned host batch -> device -> graph-replayed step -> loss read-back
@@ -642,8 +632,8 @@ def run_b200(args, rank, world, local_rank):
     }
     names = {"tconv_fwd": "fused conv forward (csrc/tconv_tile.cu)",
              "tconv_bwd": "fused conv backward: target pass + source pass (csrc/tconv_tile.cu, 2 launches)",
-             "gemm_fwd": "k_gemm_nt_tma (node linears, tcgen05 3xTF32, TMA-tiled)",
-             "gemm_dgrad": "k_gemm_nt_tma (data gradient)", "gemm_wgrad": "k_gemm_tn_tma (weight + bias gradient)"}
+             "gemm_fwd": "k_gemm_nt_wg (node linears, wgmma 3xTF32)",
+             "gemm_dgrad": "k_gemm_nt_wg (data gradient)", "gemm_wgrad": "k_gemm_tn_wg (weight + bias gradient)"}
     kernels = {}
     for name, ts in kern.items():
         ts = [t for t in ts if t == t]
@@ -658,10 +648,7 @@ def run_b200(args, rank, world, local_rank):
         top = max(kernels, key=lambda k: kernels[k]["ms_per_step"])
         ach = kernels[top]["GBs"]
         roof = {"kernel": names[top], "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s",
-                "frac": ach / peak, "traffic": ncu_traffic(top),
-                "traffic_source": "committed ncu --set full capture of this command (profiles/r2_traffic.json), "
-                                  "NOT measured in this run; below the algorithmic bytes when outputs stay dirty in L2",
-                "peak_source": peak_kind, "algorithmic_bytes": alg[top],
+                "frac": ach / peak, "peak_source": peak_kind, "algorithmic_bytes": alg[top],
                 "us_per_launch": kernels[top]["us_per_launch"],
                 "share_of_step": kernels[top]["ms_per_step"] / (1e3 * secs / args.steps),
                 "how": "CUDA event pair recorded by the engine around the launch(es) inside eagerly issued train "
@@ -678,12 +665,10 @@ def run_b200(args, rank, world, local_rank):
                    "step_issue": ("CUDA-graph replay per batch buffer (index build + forward + loss + backward), eager "
                                   f"all-reduce + Adam; {gstep.replays} replays, capture_error={gstep.capture_error}")
                    if use_graph else "eager fused_train_step (5 C calls per step)",
-                   "timing": f"{len(blocks)} blocks of exactly {args.steps} steps, each bracketed by barrier + "
-                             "synchronize and a CUDA event pair, max over ranks per block; value = median block "
-                             f"(min {min(blocks) * 1e3:.3f} / max {max(blocks) * 1e3:.3f} ms per block, timed region "
-                             f"{sum(blocks):.2f} s)",
+                   "timing": f"one block of exactly {args.steps} steps bracketed by barrier + synchronize and a "
+                             f"CUDA event pair, max over ranks (timed region {sum(blocks):.2f} s)",
                    "l2": f"rotating {N_ROT} distinct resident batches; ~{(n_convs * 8 * Nn * H * 4) >> 20} MB of "
-                         "activations written+read per step (> 126 MB L2 for cfg2+): no explicit flush in the step "
+                         "activations written+read per step (> 50 MB L2 for cfg2+): no explicit flush in the step "
                          "loop; scatter_max is timed with an explicit 512 MB L2 flush"},
         "roofline": roof, "scatter_max": smx, "kernels": kernels, "cpu_baseline": base,
         "e2e_dropin": {"value": e2e_val, "unit": "DAGs/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4,
@@ -698,8 +683,7 @@ def run_b200(args, rank, world, local_rank):
                               "(train.AsyncLossReader: 4-byte D2H + event behind each step, consumed one step later)"},
         "gpu_launches": int(round(launches_per_step * args.steps)),
         "gpu_launches_how": "kernels launched per step through the C-ABI (counted at every binding call: the engine's "
-                            "launch list mirrored from csrc/engine.cu + index build + loss + Adam) x steps of one block; "
-                            "cross-check: profiles/r2_launches_step.csv (ncu launch list of the same command)",
+                            "launch list mirrored from csrc/engine.cu + index build + loss + Adam) x timed steps",
         "wall_s": t_wall, "clocks": clocks, "final_loss": float(loss), "parity_first_step": parity,
         "peer": peer_phases, "cfg4": cfg4, "cfg2_jittered": cfg2j, "pert_pipeline": pert_pipe,
     }
@@ -739,8 +723,8 @@ def run_extra_block(args, rank, world, dev, barrier, make_optimizer, cfg, per_gp
     barrier()
     if hasattr(opt, "phase_times_us"):
         opt.phase_times_us(reset=True)
-    K = max(5, min(args.steps, 20))
-    secs, blocks = timed_blocks(block, K, barrier, world, dev, min_region_s=0.4, max_blocks=60)
+    K = args.steps
+    secs, blocks = timed_blocks(block, K, barrier, world, dev)
     phases = opt.phase_times_us(reset=True) if hasattr(opt, "phase_times_us") and world > 1 else None
     if hasattr(opt, "check"):
         opt.check()
@@ -803,8 +787,8 @@ def run_pert_pipeline_block(args, dev, barrier):
 
     epoch_block(5)
     barrier()
-    K = max(5, min(args.steps, 20))
-    secs, blocks = timed_blocks(epoch_block, K, barrier, 1, dev, min_region_s=0.3, max_blocks=40)
+    K = args.steps
+    secs, blocks = timed_blocks(epoch_block, K, barrier, 1, dev)
     store.check()
     res = [store.assemble(ids[i * B:(i + 1) * B]) for i in range(3)]
     gstep = GraphedTrainStep(model, opt, 0.5, None)
@@ -817,7 +801,7 @@ def run_pert_pipeline_block(args, dev, barrier):
 
     block(7)
     barrier()
-    secs2, blocks2 = timed_blocks(block, K, barrier, 1, dev, min_region_s=0.3, max_blocks=40)
+    secs2, blocks2 = timed_blocks(block, K, barrier, 1, dev)
     Nn, Ee = int(res[0].x.size(0)), int(res[0].edge_index.size(1))
     return {"workload": f"PERT-exact synthetic: {B} traces per step, one PERT graph each (60-72 calls: nodes = 2 calls + "
                         "distinct ms, edges = 4 calls), 64-dim, num_layers=3, fwd+bwd+Adam",
@@ -845,6 +829,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity-check", action="store_true")
     ap.add_argument("--no-cfg4", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss, parameters and gradients as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     global _BENCH_CFG
     _BENCH_CFG = args.cfg

@@ -1,4 +1,4 @@
-/* libpertgnn -- C-ABI of the B200 (sm_100a) hot path of PERT-GNN.
+/* libpertgnn -- C-ABI of the H100 (sm_90a) hot path of PERT-GNN.
  *
  * The reference (handasontam/PERT-GNN-KDD23) is pure Python on top of torch_geometric 2.4.0 and has no
  * FFI of its own; the "interface each entry point replaces" is therefore the Python/PyG call the
@@ -17,15 +17,15 @@
  *     (PERT_ERR_*).  Never throws, never exits.  Out-of-range indices found ON THE DEVICE are
  *     reported by writing PERT_ERR_RANGE into the optional device word `status`;
  *   - library-owned state (all of it; none of it is data): (1) a per-device ring of 8192 self-resetting tile-ticket
- *     counters for the dynamically scheduled tensor-core GEMMs -- every launch takes the next slot (host atomic), so
- *     concurrent launches on different streams / threads / captured graphs do not share a counter unless 8192 GEMM
+ *     counters for the dynamically scheduled graph-tile kernels -- every launch takes the next slot (host atomic), so
+ *     concurrent launches on different streams / threads / captured graphs do not share a counter unless 8192 such
  *     launches separate them while the first is still running; (2) per device, one auxiliary non-blocking stream and
  *     two events the step engine (pert_model_forward/backward) uses to run independent small kernels beside the main
  *     chain (fork/join by events, capture-safe; PERT_ENGINE_FORK=0 disables); the host-side issue of engine calls on
  *     one device is serialised by a mutex, so engines driven from several host threads / streams stay correct (their
- *     side work shares that one auxiliary stream); (3) the cached
- *     cuTensorMapEncodeTiled driver entry point; (4) environment switches read once (debug / measurement A/B only):
- *     PERT_GEMM_TC, PERT_GEMM_TMA, PERT_GEMM_TN_ACC, PERT_TCONV_TILE, PERT_TCONV_VPL, PERT_TCONV_VPL_BWD,
+ *     side work shares that one auxiliary stream); (3) the SM count of
+ *     each device, read once; (4) environment switches read once (debug / measurement A/B only):
+ *     PERT_GEMM_TC, PERT_TCONV_TILE, PERT_TCONV_VPL, PERT_TCONV_VPL_BWD,
  *     PERT_TILE_LIST, PERT_BN_FUSE, PERT_ENGINE_FORK, PERT_PEER_MODE.
  *     With that, operator-level calls are re-entrant and thread-safe across streams;
  *   - rows of float matrices must be 16-byte aligned (ld % 4 == 0, base pointer 16-byte aligned)

@@ -1,10 +1,10 @@
-"""Generates tests/golden/node_depth_*.npz by RUNNING THE REFERENCE's own code (run in the build container only:
-needs /root/reference).  Row A9 of SURVEY.md section 8a -- the one piece of the hot-path scope whose reference
+"""Generates tests/golden/node_depth_*.npz by RUNNING THE REFERENCE's own code (needs a checkout of
+handasontam/PERT-GNN-KDD23 named by the environment variable PERT_GNN_REFERENCE).  Row A9 of SURVEY.md section 8a -- the one piece of the hot-path scope whose reference
 implementation is pure Python/numpy and importable here:
   misc.DFS.dfs_min_node_depth (misc.py:59-63), GraphConstruct.build_adj_list (:107-111),
   GraphConstruct.get_node_depth (:113-136), GraphConstruct.get_node_features (:144-175),
   and the torch.tensor(node_depth, dtype=torch.long) cast of misc.py:215 / :368.
-Usage:  python oracle/gen_golden.py
+Usage:  PERT_GNN_REFERENCE=<checkout> python oracle/gen_golden.py
 """
 import os
 import sys
@@ -13,7 +13,7 @@ import numpy as np
 import pandas as pd
 import torch
 
-REF = "/root/reference"
+REF = os.environ.get("PERT_GNN_REFERENCE", "")
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
 
 

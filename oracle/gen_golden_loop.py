@@ -1,6 +1,7 @@
-"""Generates tests/golden/ref_loop.npz by RUNNING THE REFERENCE's own code (build container only: needs /root/reference).
+"""Generates tests/golden/ref_loop.npz by RUNNING THE REFERENCE's own code (needs a checkout of
+handasontam/PERT-GNN-KDD23 named by the environment variable PERT_GNN_REFERENCE).
 
-What runs, from /root/reference/pert_gnn.py itself (oracle/ref_loop.py extracts the function definitions at run time):
+What runs, from the reference's pert_gnn.py itself (oracle/ref_loop.py extracts the function definitions at run time):
   get_data_list -> get_entry_data -> get_x / get_cat_X / get_edge_index / ... (:40-188)  on synthetic processed/ artefacts
   get_data_loader (:196-210), train (:213-251), test (:254-294)                            for EPOCHS epochs
 with `torch_geometric` = compat/ shim (Data, DataLoader) and `model` = the CPU oracle (oracle/model_oracle.py; PyG
@@ -9,7 +10,7 @@ itself is not installable, see DESIGN.md section 6).  Stored:
     pattern_num_nodes, pattern_probs, entry_id, y)  -> pins the device pattern store + feature join (SURVEY N1 / N4);
   * the batch composition of every step (the train loader shuffles), the initial weights, and per epoch the values
     train() / test() returned  -> pins the drop-in loop and the eval metrics (X1 / N3) end to end.
-Usage:  python oracle/gen_golden_loop.py
+Usage:  PERT_GNN_REFERENCE=<checkout> python oracle/gen_golden_loop.py
 """
 import os
 import sys
@@ -65,7 +66,7 @@ def run(model_factory=None, device="cpu", artifacts=None, init_state=None):
 
 
 def main():
-    assert ref_loop.available(), "needs /root/reference"
+    assert ref_loop.available(), "set PERT_GNN_REFERENCE to a checkout of handasontam/PERT-GNN-KDD23"
     r = run()
     out = {"epochs": r["epochs"], "n_traces": np.int64(len(r["data_list"])),
            "model_args": np.array([r["model_args"][0], r["model_args"][1][0], *r["model_args"][2:7]], dtype=np.int64),

@@ -1,14 +1,14 @@
-"""Generates tests/golden/ref_pert.npz by RUNNING THE REFERENCE's GraphConstruct (build container only: needs
-/root/reference and pandas).
+"""Generates tests/golden/ref_pert.npz by RUNNING THE REFERENCE's GraphConstruct (needs pandas and a checkout
+of handasontam/PERT-GNN-KDD23 named by the environment variable PERT_GNN_REFERENCE).
 
 For every table of synthetic.make_span_tables(SEED) it builds the DataFrame preprocess.py:296-318 would pass and calls,
-from /root/reference/misc.py itself:
+from the reference's misc.py itself:
   GraphConstruct.__init__  -> get_root_spanID (:138-142) and drop_wrong_edges (:87-105)
   get_pert_edge_index      -> edge_index, edge_attr, node_depth, sorted_span_id          (:221-370)
   get_span_edge_index      -> edge_index, node_depth, edge_attr, sorted_unique_ms        (:190-219)
 Stored per trace t: the surviving row indices (`t{t}_keep`), the root (`t{t}_root`) and the four outputs.  The raw
 tables are regenerated from the seed by the tests (synthetic.make_span_tables is deterministic).
-Usage:  python oracle/gen_golden_pert.py
+Usage:  PERT_GNN_REFERENCE=<checkout> python oracle/gen_golden_pert.py
 """
 import importlib.util
 import os
@@ -29,7 +29,7 @@ COLS = ("timestamp", "rpcid", "um", "interface", "dm", "rpctype", "rt", "endTime
 
 
 def load_reference_misc():
-    spec = importlib.util.spec_from_file_location("_ref_misc", "/root/reference/misc.py")
+    spec = importlib.util.spec_from_file_location("_ref_misc", os.path.join(os.environ["PERT_GNN_REFERENCE"], "misc.py"))
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
     return mod

@@ -2,7 +2,7 @@
 pert_gnn_kdd23_b200/ imports this file.
 
 Restates, in plain Python loops (small cases only):
-  get_root_ms        <- /root/reference/misc.py:138-142  (GraphConstruct.get_root_spanID)
+  get_root_ms        <- misc.py:138-142  (GraphConstruct.get_root_spanID)
   drop_wrong_edges   <- misc.py:87-105
   span_graph         <- misc.py:190-219 (get_span_edge_index)
   pert_graph         <- misc.py:221-319 (get_pert_edge_index: stage chains, call / return edges in time order)

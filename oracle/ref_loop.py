@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE (not product): runs the REFERENCE'S OWN sample assembly and train / test loop.
 
-`/root/reference/pert_gnn.py` is a script (argparse + file loads at import time), so it cannot be imported; this
+The reference's `pert_gnn.py` is a script (argparse + file loads at import time), so it cannot be imported; this
 harness parses it with `ast`, takes the function definitions it needs VERBATIM FROM THE FILE AT RUN TIME (nothing is
 copied into this repository) --
 
@@ -14,8 +14,8 @@ copied into this repository) --
 `compat/` shim (`Data`, `DataLoader`).  So the reference's loop body really executes against the shim's
 Data/Batch/DataLoader surface; the model is whatever the caller passes (the CPU oracle when generating goldens).
 
-Only usable where /root/reference exists (the build container); the GPU box uses the committed fixture
-tests/golden/ref_loop.npz produced by oracle/gen_golden_loop.py.
+Only usable with a checkout of handasontam/PERT-GNN-KDD23 named by the environment variable PERT_GNN_REFERENCE; the
+tests use the committed fixture tests/golden/ref_loop.npz produced by oracle/gen_golden_loop.py.
 """
 import ast
 import itertools
@@ -28,7 +28,7 @@ import numpy as np
 import pandas as pd
 import torch
 
-REF_FILE = "/root/reference/pert_gnn.py"
+REF_FILE = os.path.join(os.environ.get("PERT_GNN_REFERENCE", ""), "pert_gnn.py")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 FUNCS = ("get_x", "get_all_runtimes_id_probs", "get_edge_attr", "get_pattern_num_nodes", "get_cat_X",
@@ -37,7 +37,7 @@ FUNCS = ("get_x", "get_all_runtimes_id_probs", "get_edge_attr", "get_pattern_num
 
 
 def available():
-    return os.path.exists(REF_FILE)
+    return bool(os.environ.get("PERT_GNN_REFERENCE")) and os.path.exists(REF_FILE)
 
 
 def _shim_modules():

@@ -1,2 +1,2 @@
-"""pert_gnn_kdd23_b200 -- B200-native hot path of PERT-GNN (see DESIGN.md)."""
+"""pert_gnn_kdd23_b200 -- H100-native hot path of PERT-GNN (see DESIGN.md)."""
 __version__ = "0.1.0"

@@ -1,11 +1,24 @@
-// Shared device/host helpers for libpertgnn (sm_100a only).
+// Shared device/host helpers for libpertgnn (sm_90a: H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../../include/pertgnn.h"  // prototypes + PERT_ERR_* (keeps definitions and ABI header in sync)
 
-#define PERT_NUM_SMS 148          // B200: 2 dies x 74 SMs
+// SM count of the current device (H100 SXM: 132, H100 PCIe: 114), read once per device.  Persistent grids are sized
+// to it, and the peer all-reduce needs all of its CTAs co-resident, so it must not be a compile-time guess.
+static inline int pert_num_sms() {
+  static int sms[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 1;
+  if (sms[dev] <= 0) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 1;
+    sms[dev] = n;
+  }
+  return sms[dev];
+}
+#define PERT_NUM_SMS pert_num_sms()
 
 #define PERT_LAUNCH_CHECK()                          \
   do {                                               \

@@ -483,9 +483,7 @@ std::mutex& engine_mutex() {
   static std::mutex m;
   return m;
 }
-// Graph-aligned tile lists (csrc/tconv_tile.cu:k_build_tiles) are OFF by default: measured on B200 (round 2,
-// profiles/r2_tile_list_ab.md) the fixed T-node tiles win on every BASELINE shape -- uniform cfg2 0.649 vs 0.690 ms/step,
-// cfg2 with +-20 % graph sizes 0.721 vs 0.804, power-law cfg3 1.331 vs 1.388 -- because a fixed tiling has the minimal
+// Graph-aligned tile lists (csrc/tconv_tile.cu:k_build_tiles) are OFF by default: fixed T-node tiles have the minimal
 // number of tiles (one wave of CTAs at cfg2) and the global-gather variant that cut graphs need is only ~10 % slower
 // than the all-in-tile variant, while whole-graph tiles cost a packing kernel per batch and more, unevenly filled
 // tiles.  PERT_TILE_LIST=1 turns them on.

@@ -234,7 +234,7 @@ inline bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
 }  // namespace
 
-// tensor-core (tcgen05, 3xTF32) kernels of gemm_tc.cu; PERT_ERR_UNSUPPORTED => exact-fp32 SIMT kernels below
+// tensor-core (wgmma, 3xTF32) kernels of gemm_tc.cu; PERT_ERR_UNSUPPORTED => exact-fp32 SIMT kernels below
 int pert_gemm_nt_tc(const float* A, int lda, int a_cb, long long a_cbs, const float* B, int ldb, const float* bias,
                     float* C, int ldc, int c_cb, long long c_cbs, long long M, int Nc, int K, int relu,
                     cudaStream_t st);

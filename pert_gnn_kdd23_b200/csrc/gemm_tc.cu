@@ -1,412 +1,230 @@
-// Tensor-core path of the dense node linears: tcgen05.mma kind::tf32 with 3xTF32 split accumulation.
+// Tensor-core path of the dense node linears on Hopper: wgmma (m64nNk8, kind tf32) with 3xTF32 split accumulation.
 //
 // The linears need fp32-level accuracy (1e-4 after 3-5 layers + BatchNorm), which single-pass TF32 (10-bit
-// mantissa) does not give.  Every fp32 operand x is split into hi = nearest tf32 of x and lo = x - hi (see tf32_hi); the product is accumulated in fp32 (TMEM) as  hi*hi + lo*hi + hi*lo  (the dropped lo*lo term is
-// ~2^-22 relative), three MMAs per K-step on the 5th-generation tensor cores (tests: test_linear_* at 2e-6).
+// mantissa) does not give.  Every fp32 operand x is split into hi = nearest tf32 of x and lo = x - hi (see tf32_hi);
+// the product is accumulated in fp32 registers as  hi*hi + lo*hi + hi*lo  (the dropped lo*lo term is ~2^-22
+// relative), three wgmmas per K-step (tests: test_linear_* at 2e-6).
 //
-// Operand staging (validated by csrc/dev/umma_probe*.cu on B200):
-//   A (activations):  thread = row; the row's K-chunk goes global -> registers (16-byte loads) -> split ->
-//       tcgen05.st into TMEM (A-from-TMEM MMA form: lane = row, one 32-bit column per K element).  No smem, no TMA
-//       descriptor; the split is free.  (MN-major smem operands are NOT usable for 32-bit types without the special
-//       128B_BASE32B swizzle -- probed, returns zeros -- so the weight-gradient kernel also feeds A through TMEM and
-//       transposes B while filling shared memory.)
+// Operand staging:
+//   A (activations / the transposed operand of the weight gradient): global -> registers in the wgmma A-fragment
+//       layout -> split.  A thread of warp w holds rows 16w + g and 16w + g + 8 (g = lane / 4) and K columns t, t + 4
+//       (t = lane % 4) of every K-step of 8.  The K order inside a step is free as long as B uses the same one, so the
+//       forward kernel gives thread t the four CONTIGUOUS columns 4t..4t+3 of a 16-column chunk (one 16-byte load per
+//       row and chunk: columns 4t, 4t+1 feed step 0, 4t+2, 4t+3 step 1) and permutes the weights to match
+//       (nt_logical_k).  The weight-gradient kernel permutes M instead: fragment rows g / g + 8 are the adjacent
+//       output rows 2g / 2g + 1, so a thread reads two of them with one 8-byte load.
 //   B:  shared memory, no-swizzle K-major canonical layout (8-row x 16-byte core matrices, LBO = 128 B between
-//       K-adjacent core matrices, SBO between N-adjacent), split hi/lo.
-//   D:  fp32 accumulator in TMEM; epilogue tcgen05.ld (lane = row).
+//       K-adjacent core matrices, SBO between N-adjacent ones), split hi/lo.
+//   D:  fp32 accumulators in registers (fragment: row g / g + 8, columns 8j + 2t, 8j + 2t + 1).
 //
-// Two generations of kernels live in this file (all persistent, one CTA per SM, warp-specialised, mbarrier pipelines):
-//   k_gemm_nt_tma / k_gemm_tn_tma (further down) -- the production path: a loader warp moves the operands with TMA
-//       (2-D tensor-map copies with 128-byte swizzle for the forward / data-gradient A tiles, large 1-D bulk copies
-//       for the weight-gradient chunks) into a multi-stage shared-memory ring, tiles / chunks are handed out by
-//       self-resetting ticket counters, and the forward epilogue leaves through TMA tensor stores.
-//   k_gemm_nt_tc / k_gemm_tn_tc -- the first generation (converter warps fetch their operands with LDG); still the
-//       path for operands the TMA kernels do not accept (strided rows) and for PERT_GEMM_TMA=0:
-//   NT (forward / data gradient, C[M,Nc] = A[M,K] . B[Nc,K]^T (+bias)):
-//       warps 0-3 load+split A chunks into TMEM stage s | warp 4 issues the MMAs (one thread) | warps 5-8 drain the
-//       accumulator stage (TMEM -> registers -> +bias -> global) while the next tile is being multiplied.
-//   TN (weight gradient, C[Mc,Nc] += A[R,Mc]^T . B[R,Nc], split over R, REDG.128 accumulation):
-//       warps 0-3 load A columns (coalesced across lanes) into TMEM | warps 4-7 transpose the B chunk into the K-major
-//       smem layout (bank-conflict-free 8x4 patches) | warp 8 issues the MMAs.
-// These GEMMs are memory-bound by shape (K <= 256): A read once, C written once; measured bounds in DESIGN.md section 3.
+//   k_gemm_nt_wg (forward / data gradient, C[M,Nc] = A[M,K] . B[Nc,K]^T (+bias)): persistent, two warpgroups per
+//       CTA, each owns 64-row tiles; the [BN, K] weight block is resident in shared memory (hi + lo), the next
+//       16-column A chunk is in flight while the current one is multiplied.
+//   k_gemm_tn_wg (weight gradient, C[Mc,Nc] += A[R,Mc]^T . B[R,Nc], split over R, vector red.global accumulation):
+//       two warpgroups cover 128 output rows; the CTA transposes 32-row chunks of B into a double-buffered K-major
+//       stage while the previous chunk is multiplied.  The tensor-core accumulation truncates, an error that grows
+//       with the length of the running sum, so every TN_FLUSH chunks the register accumulators are added (round to
+//       nearest) into per-thread partial sums in shared memory and restarted from zero.
+// These GEMMs are memory-bound by shape (K <= 256): A read once, C written once.
 #include "common.cuh"
 #include <atomic>
-#include <cuda.h>
 #include <stdlib.h>
 
 namespace {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// wgmma shared-memory matrix descriptor (sm_90): start address, LBO, SBO in 16-byte units; base offset 0,
+// layout type 0 (no swizzle)
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3fff);
   d |= (uint64_t)((lbo >> 4) & 0x3fff) << 16;
   d |= (uint64_t)((sbo >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version 1 (sm_100); base_offset 0, lbo_mode 0, SWIZZLE_NONE
   return d;
 }
-__device__ __forceinline__ uint32_t make_idesc(int M, int N) {
-  // c_format F32 (1<<4), a/b format TF32 (2<<7, 2<<10), K-major both, N>>3 at bit 17, M>>4 at bit 24
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(phase)
-        : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
+// D[64 x 32] += A[64 x 8] (registers) . B[32 x 8]^T (descriptor)
+__device__ __forceinline__ void wgmma_n32(float* d, const uint32_t* a, uint64_t b) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(
-          taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
+      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b)
       : "memory");
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+// D[64 x 16] += A[64 x 8] . B[16 x 8]^T
+__device__ __forceinline__ void wgmma_n16(float* d, const uint32_t* a, uint64_t b) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
+      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b)
       : "memory");
 }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+
 // Round-to-nearest split with integer ops: hi = (bits + 0x1000) & 0xffffe000 (nearest tf32, ties away from zero; two
-// full-rate ALU instructions -- cvt.rna.tf32.f32 runs on the quarter-rate conversion pipe and cost the converter
-// warps 8 us per weight-gradient launch at cfg2), lo = x - hi (exact in fp32, |lo| <= 2^-11 |x|, either sign; the
-// tensor core drops its low 13 bits: <= 2^-21 |x|, sign-symmetric).  A truncating hi (x & 0xffffe000) makes lo
-// one-signed and the dropped bits a one-sided residual that does not average out over 10^4..10^5-term sums.
+// full-rate ALU instructions instead of the quarter-rate cvt.rna.tf32.f32), lo = x - hi (exact in fp32,
+// |lo| <= 2^-11 |x|, either sign; the tensor core drops its low 13 bits: <= 2^-21 |x|, sign-symmetric).  A truncating
+// hi (x & 0xffffe000) makes lo one-signed and the dropped bits a one-sided residual that does not average out over
+// 10^4..10^5-term sums.
 __device__ __forceinline__ uint32_t tf32_hi(float x) { return (__float_as_uint(x) + 0x1000u) & 0xffffe000u; }
 __device__ __forceinline__ uint32_t tf32_lo(float x, uint32_t hi) { return __float_as_uint(x - __uint_as_float(hi)); }
 
-#ifdef PERT_TC_TRACE
-__device__ long long g_trace[6][32][4];   // [role][tile or chunk][event] clock64 stamps of CTA (0,0)
-__device__ unsigned long long g_cta_t[512][2];   // per-CTA globaltimer at entry / exit
-__device__ __forceinline__ unsigned long long gtimer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
+__device__ __forceinline__ void split4(const float (&v)[4], uint32_t (&h)[4], uint32_t (&l)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    h[i] = tf32_hi(v[i]);
+    l[i] = tf32_lo(v[i], h[i]);
+  }
 }
-#define CTA_T(ev)                                                                                            \
-  do {                                                                                                       \
-    if (threadIdx.x == 0) g_cta_t[blockIdx.y * gridDim.x + blockIdx.x][ev] = gtimer();                      \
-  } while (0)
-#define TRACE(role, it, ev)                                                                                  \
-  do {                                                                                                       \
-    if (blockIdx.x == 0 && blockIdx.y == 0 && (threadIdx.x & 31) == 0 && (it) < 32) g_trace[role][it][ev] = clock64(); \
-  } while (0)
-#else
-#define TRACE(role, it, ev)
-#define CTA_T(ev)
-#endif
 
-constexpr int TC_THREADS = 288;  // 4 producer warps + 1 MMA warp + 4 consumer warps
-constexpr int KC = 64;           // K elements per A stage (TMEM columns per hi / lo half)
-constexpr int D_COL = 0;         // accumulator stages at columns 0 and 128
-constexpr int A_COL = 256;       // A stages at 256 + s*128 (hi: +0, lo: +64)
-constexpr int TMEM_COLS = 512;
+// One K-step of 8 over all BN columns: hi*hi + lo*hi + hi*lo.  bhi / blo: shared addresses of the step's first core
+// matrix; 32 columns (four 8-row core-matrix groups) further is 4 * SBO.
+template <int BN>
+__device__ __forceinline__ void mma_step(float* d, const uint32_t (&ah)[4], const uint32_t (&al)[4], uint32_t bhi,
+                                         uint32_t blo, uint32_t sbo) {
+  constexpr int N32 = BN / 32;
+#pragma unroll
+  for (int j = 0; j < N32; ++j) {
+    const uint64_t dh = make_desc(bhi + j * 4 * sbo, 128, sbo), dl = make_desc(blo + j * 4 * sbo, 128, sbo);
+    wgmma_n32(d + 16 * j, ah, dh);
+    wgmma_n32(d + 16 * j, al, dh);
+    wgmma_n32(d + 16 * j, ah, dl);
+  }
+  if (BN % 32) {
+    const uint64_t dh = make_desc(bhi + N32 * 4 * sbo, 128, sbo), dl = make_desc(blo + N32 * 4 * sbo, 128, sbo);
+    wgmma_n16(d + 16 * N32, ah, dh);
+    wgmma_n16(d + 16 * N32, al, dh);
+    wgmma_n16(d + 16 * N32, ah, dl);
+  }
+}
+
+// Local column of accumulator register i (fragment of the n32 / n16 pieces: 4 registers per 8 columns)
+__device__ __forceinline__ int acc_col(int i, int t) { return (i >> 2) * 8 + 2 * t + (i & 1); }
+
+constexpr int WG_THREADS = 256;   // two warpgroups
+constexpr int SMEM_MAX = 226 * 1024;
 
 struct NtArgs {
   const float* A;
   int lda, a_cb;
   long long a_cbs;
+  long long a_pz;      // plane stride of A (gridDim.z > 1: plane z multiplies A + z * a_pz by columns z*K.. of B)
   const float* B;
   int ldb;
   const float* bias;
   float* C;
   int ldc, c_cb;
   long long c_cbs;
-  int M, Nc, K, BN, relu;
-  int reduce;          // TMA kernel: leave through cp.reduce.async.bulk (+=) instead of a plain store
-  int kplanes;         // > 1: gridDim.z column blocks of A, each a K-wide GEMM against its own K-slice of B
-  unsigned int* ctr;   // this launch's ticket counters (one per blockIdx.y), see ticket_slot()
+  int M, Nc, K, relu;
+  int reduce;          // 1: accumulate into C with vector red.global (planes), bias from plane 0 only
 };
 
-struct NtBars {
-  uint64_t a_full[2], a_empty[2], d_full[2], d_empty[2];
-};
+// logical K position (inside the weight operand) of physical column p: see the operand staging notes above
+__device__ __forceinline__ int nt_logical_k(int p, int K16) {
+  if (p < K16) {
+    const int r = p & 15;
+    return (p & ~15) + ((r >> 1) & 1) * 8 + (r >> 2) + (r & 1) * 4;
+  }
+  const int r = p - K16;                          // trailing 8 columns (K % 16 == 8): thread t holds 2t, 2t + 1
+  return K16 + (r >> 1) + (r & 1) * 4;
+}
 
-// grid: (persistent over 128-row tiles, Nc / BN); one CTA per SM
-__global__ void __launch_bounds__(TC_THREADS, 1) k_gemm_nt_tc(NtArgs g) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ uint32_t s_tmem;
-  __shared__ __align__(8) NtBars bars;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) TRACE(3, 1, 0);
-  CTA_T(0);
-  const int K = g.K, BN = g.BN;
-  const int n0 = blockIdx.y * BN;
-  const uint32_t LBO = 128, SBO = (uint32_t)(K / 4) * 128;
-  const int kq = K / 4;
+// grid: (persistent over 128-row tile pairs, Nc / BN, planes)
+template <int BN>
+__global__ void __launch_bounds__(WG_THREADS, 1) k_gemm_nt_wg(NtArgs g) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int tid = threadIdx.x, wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31, gq = lane >> 2, tq = lane & 3;
+  const int K = g.K, Kp = (K + 7) & ~7, K16 = K & ~15;
+  const int n0 = blockIdx.y * BN, kz = blockIdx.z;
+  const uint32_t SBO = (uint32_t)(Kp / 4) * 128;
   unsigned char* sBhi = smem;
-  unsigned char* sBlo = smem + (size_t)BN * K * 4;
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)),
-                 "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  if (tid == 0) {
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&bars.a_full[s], 128);
-      mbar_init(&bars.a_empty[s], 1);
-      mbar_init(&bars.d_full[s], 1);
-      mbar_init(&bars.d_empty[s], 128);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  fence_before();
-  __syncthreads();
-  fence_after();
-  const uint32_t tmem = s_tmem;
-  if (tid == 0) TRACE(3, 1, 1);
-  const int mtiles = (g.M + 127) / 128;
-  const int nchunks = (K + KC - 1) / KC;
+  unsigned char* sBlo = smem + (size_t)BN * Kp * 4;
+  const float* Bp = g.B + (size_t)kz * K;
+  const float* Ap = g.A + (size_t)kz * g.a_pz;
 
-  if (warp < 4) {
-    // ================= A producer: global -(coalesced)-> smem -(row per thread)-> hi/lo -> TMEM stage ==========
-    // A thread owns one TMEM lane (= row), but a warp reading 32 different rows per instruction costs 32 L1 tag
-    // lookups for 16 useful bytes each (r1 ncu: L1 at 71 %, DRAM at 5 %).  So the chunk [128 rows x 256 B] is first
-    // read with fully coalesced 16-byte loads (16 lanes per row) into a staging buffer, XOR-swizzled so that both the
-    // row-major writes and the row-per-thread reads are bank-conflict free.
-    const uint32_t lane_off = (uint32_t)(warp * 32) << 16;
-    unsigned char* stA = smem + (size_t)BN * K * 8;          // 32 KB: 128 rows x 16 chunks of 16 B
-    const int c16 = tid & 15, rsub = tid >> 4;               // coalesced phase: chunk within the row, row within a pass of 8
-    uint32_t stage = 0, ph = 0;
-    int tr_i = 0;
-    float4 va[KC / 4], vr[KC / 4];                           // va: loads in flight (next chunk); vr: this thread's row
-    auto issue = [&](int mt, int ch) {
-      const int k0 = ch * KC;
-      const int kw = min(KC, K - k0);
-      const float* base = g.A + (size_t)(k0 / g.a_cb) * g.a_cbs + (k0 % g.a_cb);   // a chunk never straddles blocks
-      const int row0 = mt * 128;
-#pragma unroll
-      for (int it = 0; it < 16; ++it) {
-        const int r = it * 8 + rsub;
-        va[it] = (row0 + r < g.M && c16 * 4 < kw) ? ldg4(base + (size_t)(row0 + r) * g.lda + c16 * 4) : f4zero();
-      }
-    };
-    int mt = blockIdx.x, ch = 0;
-    bool have = mt < mtiles;
-    if (have) issue(mt, ch);
-    while (have) {
-      TRACE(0, tr_i, 0);
-      const int kw = min(KC, K - ch * KC);
-      asm volatile("bar.sync 1, 128;" ::: "memory");         // previous chunk's row reads are done
-#pragma unroll
-      for (int it = 0; it < 16; ++it) {
-        const int r = it * 8 + rsub;
-        *reinterpret_cast<float4*>(stA + r * 256 + (((c16 & 8) | ((c16 ^ r) & 7)) << 4)) = va[it];
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      TRACE(0, tr_i, 1);
-      // the next chunk's loads fly while this one is split and written to TMEM
-      // (the shared-memory reads go first: LDS queues in order behind global loads in the memory pipe)
-#pragma unroll
-      for (int q = 0; q < KC / 4; ++q)
-        vr[q] = *reinterpret_cast<const float4*>(stA + tid * 256 + (((q & 8) | ((q ^ tid) & 7)) << 4));
-      int nmt = mt, nch = ch + 1;
-      if (nch == nchunks) { nch = 0; nmt += gridDim.x; }
-      const bool nhave = nmt < mtiles;
-      if (nhave) issue(nmt, nch);
-      mbar_wait(&bars.a_empty[stage], ph ^ 1);
-      fence_after();
-      TRACE(0, tr_i, 2);
-      const uint32_t t_hi = tmem + lane_off + A_COL + stage * 128;
-#pragma unroll
-      for (int grp = 0; grp < KC / 16; ++grp) {
-        if (grp * 16 < kw) {
-          uint32_t hi[16], lo[16];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float4 v = vr[grp * 4 + q];
-            hi[q * 4 + 0] = tf32_hi(v.x); lo[q * 4 + 0] = tf32_lo(v.x, hi[q * 4 + 0]);
-            hi[q * 4 + 1] = tf32_hi(v.y); lo[q * 4 + 1] = tf32_lo(v.y, hi[q * 4 + 1]);
-            hi[q * 4 + 2] = tf32_hi(v.z); lo[q * 4 + 2] = tf32_lo(v.z, hi[q * 4 + 2]);
-            hi[q * 4 + 3] = tf32_hi(v.w); lo[q * 4 + 3] = tf32_lo(v.w, hi[q * 4 + 3]);
-          }
-          tmem_st16(t_hi + grp * 16, hi);
-          tmem_st16(t_hi + KC + grp * 16, lo);
-        }
-      }
-      tmem_wait_st();
-      fence_before();
-      mbar_arrive(&bars.a_full[stage]);
-      TRACE(0, tr_i, 3);
-      ++tr_i;
-      stage ^= 1;
-      if (stage == 0) ph ^= 1;
-      mt = nmt; ch = nch; have = nhave;
-    }
-  } else {
-    // ---- B (weights) -> smem, split hi/lo, canonical K-major (warps 4-8, once per CTA, while the A producers already stream)
-    // lane -> (n % 8, kc % 4): a warp's 16-byte stores cover 8 consecutive core-matrix rows (128 contiguous bytes)
-    // per quarter-warp -- conflict-free; (consecutive lanes along kc would all land 128 B apart in the same 4 banks)
-    {
-      const int t = tid - 128, w = t >> 5, nlo = lane & 7, klo = lane >> 3;
-      const int kqb = (kq + 3) / 4, nblk8 = (BN / 8) * kqb;
-      for (int b0 = w; b0 < nblk8; b0 += 8 * 5) {              // 8 independent 16-byte loads in flight per thread
-        float4 v[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const int b = b0 + u * 5;
-          const int n = (b / kqb) * 8 + nlo, kc = (b % kqb) * 4 + klo;
-          v[u] = (b < nblk8 && kc < kq && n0 + n < g.Nc) ? ldg4(g.B + (size_t)(n0 + n) * g.ldb + kc * 4) : f4zero();
-        }
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const int b = b0 + u * 5;
-          const int n = (b / kqb) * 8 + nlo, kc = (b % kqb) * 4 + klo;
-          if (b < nblk8 && kc < kq) {
-            uint4 h, l;
-            h.x = tf32_hi(v[u].x); h.y = tf32_hi(v[u].y); h.z = tf32_hi(v[u].z); h.w = tf32_hi(v[u].w);
-            l.x = tf32_lo(v[u].x, h.x); l.y = tf32_lo(v[u].y, h.y); l.z = tf32_lo(v[u].z, h.z); l.w = tf32_lo(v[u].w, h.w);
-            const size_t off = (size_t)(n >> 3) * SBO + (n & 7) * 16 + (size_t)kc * LBO;
-            *reinterpret_cast<uint4*>(sBhi + off) = h;
-            *reinterpret_cast<uint4*>(sBlo + off) = l;
-          }
-        }
-      }
-    }
-    fence_async_smem();                                      // generic-proxy smem writes -> visible to the MMA (async proxy)
-    asm volatile("bar.sync 3, 160;" ::: "memory");
-  if (warp == 4) {
-    // ================= MMA issuer (one thread) =================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(128, BN);
-      const uint32_t bhi0 = smem_u32(sBhi), blo0 = smem_u32(sBlo);
-      uint32_t stage = 0, ph = 0, ds = 0, dph = 0;
-      int tr_i = 0;
-      for (int mt = blockIdx.x; mt < mtiles; mt += gridDim.x, ++tr_i) {
-        mbar_wait(&bars.d_empty[ds], dph ^ 1);
-        fence_after();
-        TRACE(1, tr_i, 0);
-        const uint32_t t_d = tmem + D_COL + ds * 128;
-        for (int ch = 0; ch < nchunks; ++ch) {
-          const int k0 = ch * KC;
-          const int kw = min(KC, K - k0);
-          mbar_wait(&bars.a_full[stage], ph);
-          fence_after();
-          TRACE(1, tr_i, 1);
-          const uint32_t t_hi = tmem + A_COL + stage * 128;
-          for (int s = 0; s < kw / 8; ++s) {
-            const uint32_t koff = (uint32_t)((k0 >> 3) + s) * 2 * LBO;   // 8 K-elements = two 16-byte core columns
-            const uint64_t bhi = make_desc(bhi0 + koff, LBO, SBO);
-            const uint64_t blo = make_desc(blo0 + koff, LBO, SBO);
-            mma_ts(t_d, t_hi + s * 8, bhi, idesc, (ch | s) ? 1u : 0u);
-            mma_ts(t_d, t_hi + KC + s * 8, bhi, idesc, 1u);
-            mma_ts(t_d, t_hi + s * 8, blo, idesc, 1u);
-          }
-          mma_commit(&bars.a_empty[stage]);
-          stage ^= 1;
-          if (stage == 0) ph ^= 1;
-        }
-        mma_commit(&bars.d_full[ds]);
-        TRACE(1, tr_i, 2);
-        ds ^= 1;
-        if (ds == 0) dph ^= 1;
-      }
-    }
-    __syncwarp();
-  } else {
-    // ================= epilogue: accumulator stage -> registers -> (+bias, relu) -> global =================
-    // The TMEM read is row-per-thread; the global write is made coalesced through a swizzled 16 KB slab
-    // (128 rows x 32 columns): row-per-thread STS.128, then 8 lanes per row / 4 rows per warp store 128-byte lines.
-    const int q4 = warp & 3;                       // TMEM lane quarter this warp may access
-    const uint32_t lane_off = (uint32_t)(q4 * 32) << 16;
-    const int et = (warp - 5) * 32 + lane;         // 0..127 among the epilogue threads
-    const int trow = q4 * 32 + lane;               // tile row owned in TMEM
-    unsigned char* stD = smem + (size_t)BN * K * 8 + 32 * 1024;
-    const int c8 = et & 7, rsub = et >> 3;         // coalesced phase: 16-byte chunk within the 128-byte row, row in a pass of 16
-    uint32_t ds = 0, dph = 0;
-    int tr_i = 0;
-    float4 bv[4];                                  // bias of this thread's 4 columns in each of the <= 4 slabs
-#pragma unroll
-    for (int sl = 0; sl < 4; ++sl) {
-      const int col = n0 + sl * 32 + c8 * 4;
-      bv[sl] = (g.bias && sl * 32 + c8 * 4 < BN && col < g.Nc) ? ldg4(g.bias + col) : f4zero();
-    }
-    for (int mt = blockIdx.x; mt < mtiles; mt += gridDim.x, ++tr_i) {
-      const int row0 = mt * 128;
-      TRACE(2, tr_i, 0);
-      mbar_wait(&bars.d_full[ds], dph);
-      fence_after();
-      TRACE(2, tr_i, 1);
-      const uint32_t t_d = tmem + lane_off + D_COL + ds * 128;
-#pragma unroll
-      for (int sl = 0; sl < 4; ++sl) {
-        const int c0 = sl * 32;
-        if (c0 >= BN) break;
-        uint32_t r0[16], r1[16];
-        tmem_ld16(t_d + c0, r0);
-        tmem_ld16(t_d + c0 + 16, r1);              // columns >= BN of the 128-column stage are never stored
-        tmem_wait_ld();
-        asm volatile("bar.sync 2, 128;" ::: "memory");   // previous slab fully drained
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          *reinterpret_cast<uint4*>(stD + trow * 128 + (((q ^ trow) & 7) << 4)) =
-              make_uint4(r0[q * 4], r0[q * 4 + 1], r0[q * 4 + 2], r0[q * 4 + 3]);
-          *reinterpret_cast<uint4*>(stD + trow * 128 + ((((q + 4) ^ trow) & 7) << 4)) =
-              make_uint4(r1[q * 4], r1[q * 4 + 1], r1[q * 4 + 2], r1[q * 4 + 3]);
-        }
-        asm volatile("bar.sync 2, 128;" ::: "memory");
-        const int col = n0 + c0 + c8 * 4;
-        if (c0 + c8 * 4 < BN && col < g.Nc) {
-          float* cbase = g.C + (size_t)(col / g.c_cb) * g.c_cbs + (col % g.c_cb);
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int r = it * 16 + rsub;
-            if (row0 + r < g.M) {
-              float4 o = *reinterpret_cast<const float4*>(stD + r * 128 + (((c8 ^ r) & 7) << 4));
-              o = f4add(o, bv[sl]);
-              if (g.relu) o = f4max(o, f4zero());
-              st4(cbase + (size_t)(row0 + r) * g.ldc, o);
-            }
-          }
-        }
-      }
-      fence_before();
-      mbar_arrive(&bars.d_empty[ds]);
-      TRACE(2, tr_i, 2);
-      ds ^= 1;
-      if (ds == 0) dph ^= 1;
-    }
+  // ---- weights [BN, K] -> shared memory once per CTA, split hi / lo, permuted K (nt_logical_k)
+  for (int i = tid; i < BN * Kp; i += WG_THREADS) {
+    const int n = i / Kp, p = i - n * Kp;
+    const float v = p < K ? __ldg(Bp + (size_t)(n0 + n) * g.ldb + p) : 0.f;
+    const int L = nt_logical_k(p, K16);
+    const uint32_t off = (uint32_t)(n >> 3) * SBO + (n & 7) * 16 + (L >> 2) * 128 + (L & 3) * 4;
+    const uint32_t h = tf32_hi(v);
+    *reinterpret_cast<uint32_t*>(sBhi + off) = h;
+    *reinterpret_cast<uint32_t*>(sBlo + off) = tf32_lo(v, h);
   }
-  }
-  fence_before();
+  fence_async_smem();                                // generic-proxy smem writes -> visible to wgmma (async proxy)
   __syncthreads();
-  if (tid == 0) TRACE(3, 1, 2);
-  CTA_T(1);
-  if (warp == 4) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS));
+
+  const uint32_t bhi0 = smem_u32(sBhi), blo0 = smem_u32(sBlo);
+  const int mtiles = (g.M + 63) / 64, nq = K16 / 16;
+  const bool add_bias = g.bias && kz == 0;
+  for (int mt = blockIdx.x * 2 + wg; mt < mtiles; mt += gridDim.x * 2) {
+    const int r0 = mt * 64 + w * 16 + gq, r1 = r0 + 8;
+    const bool ok0 = r0 < g.M, ok1 = r1 < g.M;
+    float d[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+    auto load = [&](int q, float4& v0, float4& v1) {
+      const int c = q * 16 + tq * 4;               // a 16-column chunk never straddles two column blocks
+      const float* base = Ap + (size_t)(c / g.a_cb) * g.a_cbs + (c % g.a_cb);
+      v0 = ok0 ? ldg4(base + (size_t)r0 * g.lda) : f4zero();
+      v1 = ok1 ? ldg4(base + (size_t)r1 * g.lda) : f4zero();
+    };
+    float4 v0, v1;
+    if (nq > 0) load(0, v0, v1);
+    for (int q = 0; q < nq; ++q) {
+      uint32_t ah0[4], al0[4], ah1[4], al1[4];
+      split4({v0.x, v1.x, v0.y, v1.y}, ah0, al0);  // step 2q:     columns 4t, 4t+1 of rows g, g+8
+      split4({v0.z, v1.z, v0.w, v1.w}, ah1, al1);  // step 2q + 1: columns 4t+2, 4t+3
+      if (q + 1 < nq) load(q + 1, v0, v1);         // in flight while this chunk is multiplied
+      wgmma_fence();
+      mma_step<BN>(d, ah0, al0, bhi0 + (2 * q) * 256, blo0 + (2 * q) * 256, SBO);
+      mma_step<BN>(d, ah1, al1, bhi0 + (2 * q + 1) * 256, blo0 + (2 * q + 1) * 256, SBO);
+      wgmma_commit();
+      wgmma_wait0();                               // the A registers are rewritten next iteration
+    }
+    if (K16 < K) {                                 // trailing K-step of 8
+      const int c = K16 + tq * 2;
+      const float* base = Ap + (size_t)(c / g.a_cb) * g.a_cbs + (c % g.a_cb);
+      const float2 u0 = ok0 ? __ldg(reinterpret_cast<const float2*>(base + (size_t)r0 * g.lda)) : make_float2(0.f, 0.f);
+      const float2 u1 = ok1 ? __ldg(reinterpret_cast<const float2*>(base + (size_t)r1 * g.lda)) : make_float2(0.f, 0.f);
+      uint32_t ah[4], al[4];
+      split4({u0.x, u1.x, u0.y, u1.y}, ah, al);
+      wgmma_fence();
+      mma_step<BN>(d, ah, al, bhi0 + (K16 / 8) * 256, blo0 + (K16 / 8) * 256, SBO);
+      wgmma_commit();
+      wgmma_wait0();
+    }
+    // ---- epilogue: registers (+bias, relu) -> global, two adjacent columns per store
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+      const int col = n0 + (i / 16) * 32 + acc_col(i & 15, tq);
+      const int row = (i & 2) ? r1 : r0;
+      if (row >= g.M) continue;
+      float2 o = make_float2(d[i], d[i + 1]);
+      if (add_bias) {
+        o.x += __ldg(g.bias + col);
+        o.y += __ldg(g.bias + col + 1);
+      }
+      if (g.relu) o = make_float2(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f));
+      float2* p = reinterpret_cast<float2*>(g.C + (size_t)(col / g.c_cb) * g.c_cbs + (col % g.c_cb) + (size_t)row * g.ldc);
+      if (g.reduce) atomicAdd(p, o);
+      else *p = o;
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------
-constexpr int RC = 64;   // reduction rows (nodes) per chunk == K of one pipeline stage
+constexpr int RC = 32;   // reduction rows (nodes) per chunk == K of one stage
+constexpr int TN_FLUSH = 1;   // chunks per register partial sum of the weight gradient
 
 struct TnArgs {
   const float* A;   // [R, Mc] blocked
@@ -416,886 +234,125 @@ struct TnArgs {
   int ldb;
   float* C;         // [Mc, Nc], ldc
   int ldc;
-  float* colsum;    // optional [Mc]: += column sums of A (bias gradient), only by blockIdx.y's A producers
-  int R, Mc, Nc, NcP, rows_per_split;
-};
-struct TnBars {
-  uint64_t full[2], empty[2], done;
+  float* colsum;    // optional [Mc]: += column sums of A (bias gradient)
+  int R, Mc, Nc, rows_per_split;
 };
 
-// grid: (splits over R, Mc / 128); one CTA per SM.  NPMAX = upper bound of NcP / 8 (register budget of the B producer)
-template <int NPMAX>
-__global__ void __launch_bounds__(TC_THREADS, 1) k_gemm_tn_tc(TnArgs g) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ uint32_t s_tmem;
-  __shared__ __align__(8) TnBars bars;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) TRACE(3, 1, 0);
-  CTA_T(0);
-  const int NcP = g.NcP;
-  const uint32_t LBO = 128, SBO = (RC / 4) * 128;
-  const size_t stage_bytes = (size_t)NcP * RC * 4;      // one of hi / lo
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)),
-                 "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  if (tid == 0) {
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&bars.full[s], 256);
-      mbar_init(&bars.empty[s], 1);
-    }
-    mbar_init(&bars.done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  fence_before();
-  __syncthreads();
-  fence_after();
-  const uint32_t tmem = s_tmem;
-  if (tid == 0) TRACE(3, 1, 1);
+// grid: (splits over R, Mc / 128).  NCP = Nc rounded up to 16 (<= 160)
+template <int NCP>
+__global__ void __launch_bounds__(WG_THREADS, 1) k_gemm_tn_wg(TnArgs g) {
+  constexpr uint32_t SBO = (RC / 4) * 128;            // N-adjacent core-matrix groups of a stage
+  constexpr uint32_t HALF = (uint32_t)NCP * RC * 4;   // one of hi / lo of one stage
+  constexpr int NP = NCP / 8;                         // B items per thread: a warp item is 4 rows x 8 columns
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int tid = threadIdx.x, wg = tid >> 7, w = (tid >> 5) & 3, warp = tid >> 5, lane = tid & 31;
+  const int gq = lane >> 2, tq = lane & 3;
   const int r_begin = blockIdx.x * g.rows_per_split;
   const int r_end = min(g.R, r_begin + g.rows_per_split);
   const int nch = (r_end - r_begin + RC - 1) / RC;
+  // fragment rows g / g + 8 of this warp are output rows mb / mb + 1
+  const int mb = blockIdx.y * 128 + wg * 64 + w * 16 + 2 * gq;
+  const bool mok = mb < g.Mc;
+  const float* acol = g.A + (size_t)((mok ? mb : 0) / g.a_cb) * g.a_cbs + ((mok ? mb : 0) % g.a_cb);
+  const uint32_t s0 = smem_u32(smem);
+  float* part = reinterpret_cast<float*>(smem + 4 * HALF);   // [NCP / 2][256]: this thread's partial sums
+  bool parted = false;
 
-  if (warp < 4) {
-    // ================= A producer: column mcol over RC rows (coalesced across the warp) -> TMEM =================
-    const int mcol = blockIdx.y * 128 + tid;     // this thread's A column == D row
-    const bool mok = mcol < g.Mc;
-    const int mc = mok ? mcol : 0;
-    const float* acol = g.A + (size_t)(mc / g.a_cb) * g.a_cbs + (mc % g.a_cb);
-    const uint32_t lane_off = (uint32_t)(warp * 32) << 16;
-    uint32_t stage = 0, ph = 0;
-    float csum = 0.f;
-    // (a register double buffer -- next chunk's loads issued before this chunk is converted -- was measured SLOWER:
-    // the SM's global-load path is the limit here, 256 outstanding 128-byte requests already take ~2500 cycles to issue)
-    float av0[RC];
-    auto loadA = [&](float (&av)[RC], int c) {
-      const int r0 = r_begin + c * RC;
-      const float* p = acol + (size_t)r0 * g.lda;
+  float2 av[4][2];                                    // [K-step][row t / t + 4] x (row mb, mb + 1)
+  float bv[NP];
+  auto load = [&](int c) {
+    const int r0 = r_begin + c * RC;
 #pragma unroll
-      for (int i = 0; i < RC; ++i) av[i] = (mok && r0 + i < r_end) ? __ldg(p + (size_t)i * g.lda) : 0.f;
-    };
-    auto procA = [&](float (&av)[RC], int c) {
-      TRACE(0, c, 0);
+    for (int s = 0; s < 4; ++s)
 #pragma unroll
-      for (int i = 0; i < RC; ++i) csum += av[i];
-      mbar_wait(&bars.empty[stage], ph ^ 1);
-      fence_after();
-      TRACE(0, c, 1);
-      const uint32_t t_hi = tmem + lane_off + A_COL + stage * 128;
-#pragma unroll
-      for (int grp = 0; grp < RC / 16; ++grp) {
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          hi[i] = tf32_hi(av[grp * 16 + i]);
-          lo[i] = tf32_lo(av[grp * 16 + i], hi[i]);
-        }
-        tmem_st16(t_hi + grp * 16, hi);
-        tmem_st16(t_hi + RC + grp * 16, lo);
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + s * 8 + tq + 4 * h;
+        av[s][h] = (mok && r < r_end) ? __ldg(reinterpret_cast<const float2*>(acol + (size_t)r * g.lda))
+                                      : make_float2(0.f, 0.f);
       }
-      tmem_wait_st();
-      fence_before();
-      mbar_arrive(&bars.full[stage]);
-      TRACE(0, c, 2);
-      stage ^= 1;
-      if (stage == 0) ph ^= 1;
-    };
-    for (int c = 0; c < nch; ++c) {
-      loadA(av0, c);
-      procA(av0, c);
+#pragma unroll
+    for (int i = 0; i < NP; ++i) {
+      const int it = warp + 8 * i, r = (it & 7) * 4 + (lane & 3), n = (it >> 3) * 8 + (lane >> 2);
+      bv[i] = (r0 + r < r_end && n < g.Nc) ? __ldg(g.B + (size_t)(r0 + r) * g.ldb + n) : 0.f;
     }
-    if (g.colsum && mok && nch > 0) atomicAdd(g.colsum + mcol, csum);
-    // ---- epilogue: D -> REDG.128 into C
-    if (nch > 0) {
-      mbar_wait(&bars.done, 0);
-      fence_after();
-      TRACE(3, 0, 0);
-      for (int c0 = 0; c0 < NcP; c0 += 16) {
-        uint32_t r[16];
-        tmem_ld16(tmem + lane_off + D_COL + c0, r);
-        tmem_wait_ld();
-        if (mok) {
-          float* dst = g.C + (size_t)mcol * g.ldc + c0;
+  };
+  float d[NCP / 2];
 #pragma unroll
-          for (int q = 0; q < 4; ++q)
-            if (c0 + q * 4 < g.Nc)
-              red4(dst + q * 4, make_float4(__uint_as_float(r[q * 4]), __uint_as_float(r[q * 4 + 1]),
-                                            __uint_as_float(r[q * 4 + 2]), __uint_as_float(r[q * 4 + 3])));
-        }
-      }
-      TRACE(3, 0, 1);
+  for (int i = 0; i < NCP / 2; ++i) d[i] = 0.f;
+  float cs0 = 0.f, cs1 = 0.f;
+  if (nch > 0) load(0);
+  for (int c = 0; c < nch; ++c) {
+    // stage c & 1 was last read by the wgmmas of chunk c - 2, which every warpgroup waited for before the barrier of
+    // chunk c - 1
+    unsigned char* sh = smem + (size_t)(c & 1) * 2 * HALF;
+#pragma unroll
+    for (int i = 0; i < NP; ++i) {
+      const int it = warp + 8 * i;
+      const uint32_t off = (uint32_t)(it >> 3) * SBO + (lane >> 2) * 16 + (it & 7) * 128 + (lane & 3) * 4;
+      const uint32_t h = tf32_hi(bv[i]);
+      *reinterpret_cast<uint32_t*>(sh + off) = h;
+      *reinterpret_cast<uint32_t*>(sh + HALF + off) = tf32_lo(bv[i], h);
     }
-  } else if (warp < 8) {
-    // ================= B producer: [RC rows, Nc] -> smem stage, K-major (K = row), hi/lo =================
-    // lane -> (n % 8, r % 4): a warp store covers an 8 (n) x 4 (r) patch = 32 distinct banks
-    const int w = warp - 4;
-    const int ln = lane & 7, lr = lane >> 3;
-    const int npatch_n = NcP / 8;
-    uint32_t stage = 0, ph = 0;
-    // all of this thread's loads of a chunk are issued before anything is stored (a load -> STS loop would serialise
-    // one memory latency per element: the compiler cannot hoist loads over the shared-memory stores)
-    float xv0[RC / 16][NPMAX];
-    auto loadB = [&](float (&xv)[RC / 16][NPMAX], int c) {
-      const int r0 = r_begin + c * RC;
+    fence_async_smem();
+    __syncthreads();
+    uint32_t ah[4][4], al[4][4];
 #pragma unroll
-      for (int i = 0; i < RC / 16; ++i) {
-        const int r = (w + 4 * i) * 4 + lr;
-        const bool rok = r0 + r < r_end;
-        const float* brow = g.B + (size_t)(r0 + (rok ? r : 0)) * g.ldb;
-#pragma unroll
-        for (int np = 0; np < NPMAX; ++np) {
-          const int n = np * 8 + ln;
-          xv[i][np] = (rok && np < npatch_n && n < g.Nc) ? __ldg(brow + n) : 0.f;
-        }
-      }
-    };
-    auto procB = [&](float (&xv)[RC / 16][NPMAX], int c) {
-      TRACE(1, c, 0);
-      mbar_wait(&bars.empty[stage], ph ^ 1);
-      TRACE(1, c, 1);
-      unsigned char* sBhi = smem + (size_t)stage * 2 * stage_bytes;
-      unsigned char* sBlo = sBhi + stage_bytes;
-#pragma unroll
-      for (int i = 0; i < RC / 16; ++i) {
-        const int r = (w + 4 * i) * 4 + lr;
-        const size_t roff = (size_t)(r >> 2) * LBO + (r & 3) * 4;
-#pragma unroll
-        for (int np = 0; np < NPMAX; ++np) {
-          if (np < npatch_n) {
-            const float x = xv[i][np];
-            const uint32_t h = tf32_hi(x);
-            const size_t off = (size_t)np * SBO + ln * 16 + roff;
-            *reinterpret_cast<uint32_t*>(sBhi + off) = h;
-            *reinterpret_cast<uint32_t*>(sBlo + off) = tf32_lo(x, h);
-          }
-        }
-      }
-      fence_async_smem();
-      mbar_arrive(&bars.full[stage]);
-      TRACE(1, c, 2);
-      stage ^= 1;
-      if (stage == 0) ph ^= 1;
-    };
-    for (int c = 0; c < nch; ++c) {
-      loadB(xv0, c);
-      procB(xv0, c);
+    for (int s = 0; s < 4; ++s) {
+      split4({av[s][0].x, av[s][0].y, av[s][1].x, av[s][1].y}, ah[s], al[s]);
+      cs0 += av[s][0].x + av[s][1].x;
+      cs1 += av[s][0].y + av[s][1].y;
     }
-  } else {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(128, NcP);
-      uint32_t stage = 0, ph = 0;
-      for (int c = 0; c < nch; ++c) {
-        mbar_wait(&bars.full[stage], ph);
-        fence_after();
-        TRACE(2, c, 0);
-        const uint32_t bhi0 = smem_u32(smem + (size_t)stage * 2 * stage_bytes);
-        const uint32_t blo0 = bhi0 + (uint32_t)stage_bytes;
-        const uint32_t t_hi = tmem + A_COL + stage * 128;
+    if (c + 1 < nch) load(c + 1);                     // in flight while this chunk is multiplied
+    const uint32_t bhi = s0 + (uint32_t)(c & 1) * 2 * HALF, blo = bhi + HALF;
+    wgmma_fence();
 #pragma unroll
-        for (int s = 0; s < RC / 8; ++s) {
-          const uint32_t koff = (uint32_t)s * 2 * LBO;
-          const uint64_t bhi = make_desc(bhi0 + koff, LBO, SBO);
-          const uint64_t blo = make_desc(blo0 + koff, LBO, SBO);
-          mma_ts(tmem + D_COL, t_hi + s * 8, bhi, idesc, (c | s) ? 1u : 0u);
-          mma_ts(tmem + D_COL, t_hi + RC + s * 8, bhi, idesc, 1u);
-          mma_ts(tmem + D_COL, t_hi + s * 8, blo, idesc, 1u);
-        }
-        mma_commit(&bars.empty[stage]);
-        TRACE(2, c, 1);
-        stage ^= 1;
-        if (stage == 0) ph ^= 1;
+    for (int s = 0; s < 4; ++s) mma_step<NCP>(d, ah[s], al[s], bhi + s * 256, blo + s * 256, SBO);
+    wgmma_commit();
+    wgmma_wait0();
+    if (c % TN_FLUSH == TN_FLUSH - 1 && c + 1 < nch) {
+#pragma unroll
+      for (int i = 0; i < NCP / 2; ++i) {
+        part[i * WG_THREADS + tid] = parted ? part[i * WG_THREADS + tid] + d[i] : d[i];
+        d[i] = 0.f;
       }
-      if (nch > 0) mma_commit(&bars.done);
+      parted = true;
     }
-    __syncwarp();
   }
-  fence_before();
-  __syncthreads();
-  if (tid == 0) TRACE(3, 1, 2);
-  CTA_T(1);
-  if (warp == 8) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS));
+  if (nch == 0 || !mok) return;
+  if (parted)
+#pragma unroll
+    for (int i = 0; i < NCP / 2; ++i) d[i] += part[i * WG_THREADS + tid];
+  if (g.colsum) {
+    cs0 += __shfl_xor_sync(0xffffffffu, cs0, 1);
+    cs0 += __shfl_xor_sync(0xffffffffu, cs0, 2);
+    cs1 += __shfl_xor_sync(0xffffffffu, cs1, 1);
+    cs1 += __shfl_xor_sync(0xffffffffu, cs1, 2);
+    if (tq == 0) {
+      atomicAdd(g.colsum + mb, cs0);
+      atomicAdd(g.colsum + mb + 1, cs1);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < NCP / 2; i += 2) {
+    const int col = (i / 16) * 32 + acc_col(i & 15, tq);
+    if (col < g.Nc)
+      atomicAdd(reinterpret_cast<float2*>(g.C + (size_t)(mb + ((i & 2) ? 1 : 0)) * g.ldc + col),
+                make_float2(d[i], d[i + 1]));
+  }
 }
 
-
 // ---------------------------------------------------------------------------------------------------------
-// Weight gradient, TMA-fed: the same MMA scheme as k_gemm_tn_tc, but the operands reach the SM through a dedicated
-// loader warp issuing bulk copies (cp.async.bulk -> mbarrier complete_tx) into an NS-deep shared-memory ring,
-// so the bytes in flight per SM (NS x ~50 KB) no longer depend on how many loads the converter warps can keep
-// outstanding (the LDG path saturated at ~32 KB / 2500 cycles per SM), and the chunks are handed out dynamically
-// from a self-resetting global counter (static splits finished between 18 and 29 us on equal work).
-//   warp 9     loader: next chunk id <- atomicAdd; the chunk's rows of every column piece of A (a piece = pw columns
-//              inside one column block; with dense blocks, lda == pw, the piece is ONE contiguous 16 KB copy) and of
-//              B (one copy when ldb == Nc) -> ring stage.  Small copies are slow (measured ~70 cycles per 256-byte
-//              cp.async.bulk), so the per-row form is only the fallback for strided operands.
-//   warps 0-3  A converters: column t over the chunk's rows (LDS, conflict free) -> hi/lo -> TMEM
-//   warps 4-7  B converters: a lane reads 4 consecutive rows of one column (LDS.32, 32 lanes = 32 columns) and
-//              stores them as one 16-byte K-quad of the K-major operand stage (hi and lo)
-//   warp 8     MMA issuer
-// A chunk id >= nchunks is the stop sentinel; it travels through the ring and the operand stages.
-// Tile tickets: every launch of a dynamically scheduled GEMM draws its tickets from its OWN slot of a ring of
-// self-resetting device counters (8 counters per slot, one per blockIdx.y).  The host hands out slots round-robin
-// (atomic), so two launches that run concurrently on different streams -- or two replicas captured into different CUDA
-// graphs -- never share a counter unless TICKET_SLOTS launches were issued in between while the first was still running.
-// The CTA that draws the last ticket of a launch resets the counter, so a slot (also one baked into a captured graph)
-// is reusable as soon as its launch has finished.
+// Tile tickets (used by the graph-aligned conv kernels, csrc/tconv_tile.cu): every launch of a dynamically scheduled
+// kernel draws its tickets from its OWN slot of a ring of self-resetting device counters (8 counters per slot).  The
+// host hands out slots round-robin (atomic), so two launches that run concurrently on different streams -- or two
+// replicas captured into different CUDA graphs -- never share a counter unless TICKET_SLOTS launches were issued in
+// between while the first was still running.  The CTA that draws the last ticket of a launch resets the counter, so
+// a slot (also one baked into a captured graph) is reusable as soon as its launch has finished.
 constexpr int TICKET_SLOTS = 8192;
 __device__ unsigned int g_ticket_ring[TICKET_SLOTS * 8];
 
-__device__ __forceinline__ void mbar_arrive_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-
-constexpr int TMA_THREADS = 320;
-constexpr int RING_MAX = 4;
-struct TnTmaArgs {
-  const float* A;
-  int lda, a_cb;
-  long long a_cbs;
-  const float* B;
-  int ldb;
-  float* C;
-  int ldc;
-  float* colsum;
-  int R, Mc, Nc, NcP, nchunks, NS, pw, a_contig, b_contig;
-  unsigned int* ctr;   // this launch's ticket counters (see g_ticket_ring)
-  int nacc;            // TMEM accumulators the chunks rotate over (1..4)
-};
-struct TnTmaBars {
-  uint64_t ring_full[RING_MAX], ring_empty[RING_MAX], op_full[2], op_empty[2], done;
-  int ring_meta[RING_MAX], op_meta[2];
-};
-
-// GMAX: B-converter items (row quad x 32-column group) per warp = ceil((RCT / 4) * ceil(NcP / 32) / 4);
-// RCT: reduction rows per chunk (64; 32 when the 64-row operand + ring stages do not fit next to each other: Nc > 96)
-template <int GMAX, int RCT>
-__global__ void __launch_bounds__(TMA_THREADS, 1) k_gemm_tn_tma(TnTmaArgs g) {
-  constexpr int TN_A_COL = TMEM_COLS - 4 * RCT;            // two A stages (hi | lo, RCT columns each) at the top of TMEM
-  extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ uint32_t s_tmem;
-  __shared__ __align__(8) TnTmaBars bars;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  CTA_T(0);
-  const int NcP = g.NcP, NS = g.NS;
-  const uint32_t LBO = 128, SBO = (RCT / 4) * 128;
-  const size_t op_bytes = (size_t)NcP * RCT * 4;           // one of hi / lo of one operand stage
-  unsigned char* ring0 = smem + 4 * op_bytes;
-  const int a_stage = RCT * 512;
-  const int ring_bytes = a_stage + RCT * g.Nc * 4;
-  const int m0 = blockIdx.y * 128;
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)),
-                 "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  if (tid == 0) {
-    for (int s = 0; s < RING_MAX; ++s) {
-      mbar_init(&bars.ring_full[s], 1);
-      mbar_init(&bars.ring_empty[s], 256);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&bars.op_full[s], 256);
-      mbar_init(&bars.op_empty[s], 1);
-    }
-    mbar_init(&bars.done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  fence_before();
-  __syncthreads();
-  fence_after();
-  const uint32_t tmem = s_tmem;
-
-  if (warp == 9) {
-    // ================= loader =================
-    const int pw = g.pw, npieces = 128 / pw;
-    const int vcols = min(128, g.Mc - m0);                 // multiple of pw
-    uint32_t rs = 0, rph = 0;
-    while (true) {
-      unsigned int c = 0;
-      if (lane == 0) c = atomicAdd(&g.ctr[blockIdx.y], 1u);
-      c = __shfl_sync(0xffffffffu, c, 0);
-      mbar_wait(&bars.ring_empty[rs], rph ^ 1);
-      if (c >= (unsigned int)g.nchunks) {
-        if (lane == 0) {
-          if (c == (unsigned int)g.nchunks + gridDim.x - 1) g.ctr[blockIdx.y] = 0;   // last ticket of the launch
-          bars.ring_meta[rs] = -1;
-          mbar_arrive(&bars.ring_full[rs]);
-        }
-        break;
-      }
-      const int r0 = (int)c * RCT;
-      const int rows = min(RCT, g.R - r0);
-      unsigned char* sA = ring0 + (size_t)rs * ring_bytes;
-      unsigned char* sB = sA + a_stage;
-      if (lane == 0) {
-        bars.ring_meta[rs] = rows;
-        mbar_arrive_tx(&bars.ring_full[rs], (uint32_t)rows * (uint32_t)(vcols + g.Nc) * 4u);
-      }
-      __syncwarp();
-      // stage layout: A piece-major [npieces][RCT][pw], B [RCT][Nc]
-      if (g.a_contig) {
-        if (lane < npieces && lane * pw < vcols) {
-          const int col = m0 + lane * pw;
-          bulk_g2s(sA + (size_t)lane * RCT * pw * 4,
-                   g.A + (size_t)(col / g.a_cb) * g.a_cbs + (col % g.a_cb) + (size_t)r0 * g.lda, rows * pw * 4,
-                   &bars.ring_full[rs]);
-        }
-      } else {
-        for (int i = lane; i < rows * npieces; i += 32) {
-          const int p = i / rows, r = i - p * rows;
-          const int col = m0 + p * pw;
-          if (p * pw < vcols)
-            bulk_g2s(sA + ((size_t)p * RCT + r) * pw * 4,
-                     g.A + (size_t)(col / g.a_cb) * g.a_cbs + (col % g.a_cb) + (size_t)(r0 + r) * g.lda, pw * 4,
-                     &bars.ring_full[rs]);
-        }
-      }
-      if (g.b_contig) {
-        if (lane == 31) bulk_g2s(sB, g.B + (size_t)r0 * g.ldb, rows * g.Nc * 4, &bars.ring_full[rs]);
-      } else {
-        for (int r = lane; r < rows; r += 32)
-          bulk_g2s(sB + (size_t)r * g.Nc * 4, g.B + (size_t)(r0 + r) * g.ldb, g.Nc * 4, &bars.ring_full[rs]);
-      }
-      if (++rs == (uint32_t)NS) { rs = 0; rph ^= 1; }
-    }
-  } else if (warp < 4) {
-    // ================= A converters + epilogue =================
-    const int mcol = m0 + tid;
-    const bool mok = mcol < g.Mc;
-    const uint32_t lane_off = (uint32_t)(warp * 32) << 16;
-    const int a_off = (tid / g.pw) * RCT * g.pw + (tid % g.pw);   // piece-major stage layout
-    uint32_t rs = 0, rph = 0, stage = 0, ph = 0;
-    int nproc = 0;
-    float csum = 0.f;
-    while (true) {
-      mbar_wait(&bars.ring_full[rs], rph);
-      const int rows = bars.ring_meta[rs];
-      if (rows < 0) break;
-      const float* sA = reinterpret_cast<const float*>(ring0 + (size_t)rs * ring_bytes) + a_off;
-      float av[RCT];
-#pragma unroll
-      for (int i = 0; i < RCT; ++i) {
-        const float v = sA[i * g.pw];
-        av[i] = (mok && i < rows) ? v : 0.f;
-      }
-#pragma unroll
-      for (int i = 0; i < RCT; ++i) csum += av[i];
-      mbar_wait(&bars.op_empty[stage], ph ^ 1);
-      fence_after();
-      const uint32_t t_hi = tmem + lane_off + TN_A_COL + stage * (2 * RCT);
-#pragma unroll
-      for (int grp = 0; grp < RCT / 16; ++grp) {
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          hi[i] = tf32_hi(av[grp * 16 + i]);
-          lo[i] = tf32_lo(av[grp * 16 + i], hi[i]);
-        }
-        tmem_st16(t_hi + grp * 16, hi);
-        tmem_st16(t_hi + RCT + grp * 16, lo);
-      }
-      tmem_wait_st();
-      fence_before();
-      mbar_arrive(&bars.ring_empty[rs]);               // every staged value has been consumed
-      if (tid == 0) bars.op_meta[stage] = rows;
-      mbar_arrive(&bars.op_full[stage]);
-      ++nproc;
-      stage ^= 1;
-      if (stage == 0) ph ^= 1;
-      if (++rs == (uint32_t)NS) { rs = 0; rph ^= 1; }
-    }
-    mbar_wait(&bars.op_empty[stage], ph ^ 1);          // pass the stop sentinel on to the MMA warp
-    if (tid == 0) bars.op_meta[stage] = -1;
-    mbar_arrive(&bars.op_full[stage]);
-    if (g.colsum && mok && nproc > 0) atomicAdd(g.colsum + mcol, csum);
-    if (nproc > 0) {
-      mbar_wait(&bars.done, 0);
-      fence_after();
-      const int nused = nproc < g.nacc ? nproc : g.nacc;   // accumulators that received at least one chunk
-      for (int c0 = 0; c0 < NcP; c0 += 16) {
-        uint32_t r[16];
-        tmem_ld16(tmem + lane_off + D_COL + c0, r);
-        tmem_wait_ld();
-        for (int a = 1; a < nused; ++a) {                  // partial sums are combined with round-to-nearest adds
-          uint32_t r2[16];
-          tmem_ld16(tmem + lane_off + D_COL + a * NcP + c0, r2);
-          tmem_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(r2[i]));
-        }
-        if (mok) {
-          float* dst = g.C + (size_t)mcol * g.ldc + c0;
-#pragma unroll
-          for (int q = 0; q < 4; ++q)
-            if (c0 + q * 4 < g.Nc)
-              red4(dst + q * 4, make_float4(__uint_as_float(r[q * 4]), __uint_as_float(r[q * 4 + 1]),
-                                            __uint_as_float(r[q * 4 + 2]), __uint_as_float(r[q * 4 + 3])));
-        }
-      }
-    }
-  } else if (warp < 8) {
-    // ================= B converters: ring stage [rows, Nc] -> K-major (K = row) hi/lo operand stage =================
-    const int w = warp - 4;
-    const int ngrp = (NcP + 31) / 32, items = (RCT / 4) * ngrp;
-    uint32_t rs = 0, rph = 0, stage = 0, ph = 0;
-    while (true) {
-      mbar_wait(&bars.ring_full[rs], rph);
-      const int rows = bars.ring_meta[rs];
-      if (rows < 0) break;
-      const float* sBr = reinterpret_cast<const float*>(ring0 + (size_t)rs * ring_bytes + a_stage);
-      float xv[GMAX][4];
-#pragma unroll
-      for (int j = 0; j < GMAX; ++j) {
-        const int it = w + 4 * j;
-        const int rq = it / ngrp, n = (it - rq * ngrp) * 32 + lane;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int r = rq * 4 + q;
-          float v = 0.f;
-          if (it < items && n < g.Nc) v = sBr[r * g.Nc + n];
-          xv[j][q] = r < rows ? v : 0.f;
-        }
-      }
-      mbar_wait(&bars.op_empty[stage], ph ^ 1);
-      unsigned char* sBhi = smem + (size_t)stage * 2 * op_bytes;
-      unsigned char* sBlo = sBhi + op_bytes;
-#pragma unroll
-      for (int j = 0; j < GMAX; ++j) {
-        const int it = w + 4 * j;
-        const int rq = it / ngrp, n = (it - rq * ngrp) * 32 + lane;
-        if (it < items && n < NcP) {
-          uint4 h, l;
-          h.x = tf32_hi(xv[j][0]); h.y = tf32_hi(xv[j][1]); h.z = tf32_hi(xv[j][2]); h.w = tf32_hi(xv[j][3]);
-          l.x = tf32_lo(xv[j][0], h.x); l.y = tf32_lo(xv[j][1], h.y);
-          l.z = tf32_lo(xv[j][2], h.z); l.w = tf32_lo(xv[j][3], h.w);
-          const size_t off = (size_t)(n >> 3) * SBO + (n & 7) * 16 + (size_t)rq * LBO;
-          *reinterpret_cast<uint4*>(sBhi + off) = h;
-          *reinterpret_cast<uint4*>(sBlo + off) = l;
-        }
-      }
-      fence_async_smem();
-      mbar_arrive(&bars.ring_empty[rs]);
-      mbar_arrive(&bars.op_full[stage]);
-      stage ^= 1;
-      if (stage == 0) ph ^= 1;
-      if (++rs == (uint32_t)NS) { rs = 0; rph ^= 1; }
-    }
-    mbar_wait(&bars.op_empty[stage], ph ^ 1);
-    mbar_arrive(&bars.op_full[stage]);
-  } else {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(128, NcP);
-      uint32_t stage = 0, ph = 0;
-      int n = 0;
-      while (true) {
-        mbar_wait(&bars.op_full[stage], ph);
-        fence_after();
-        if (bars.op_meta[stage] < 0) break;
-        const uint32_t bhi0 = smem_u32(smem + (size_t)stage * 2 * op_bytes);
-        const uint32_t blo0 = bhi0 + (uint32_t)op_bytes;
-        const uint32_t t_hi = tmem + TN_A_COL + stage * (2 * RCT);
-        // Chunks rotate over nacc accumulators: the tensor core truncates every accumulation (round toward zero), a
-        // one-sided error that grows with the number of steps times the ulp of the running sum; nacc shorter, smaller
-        // partial sums divide it by nacc (the epilogue adds them with round-to-nearest).
-        const uint32_t d = tmem + D_COL + (uint32_t)(n % g.nacc) * NcP;
-#pragma unroll
-        for (int s = 0; s < RCT / 8; ++s) {
-          const uint32_t koff = (uint32_t)s * 2 * LBO;
-          const uint64_t bhi = make_desc(bhi0 + koff, LBO, SBO);
-          const uint64_t blo = make_desc(blo0 + koff, LBO, SBO);
-          mma_ts(d, t_hi + s * 8, bhi, idesc, (n >= g.nacc || s) ? 1u : 0u);
-          mma_ts(d, t_hi + RCT + s * 8, bhi, idesc, 1u);
-          mma_ts(d, t_hi + s * 8, blo, idesc, 1u);
-        }
-        mma_commit(&bars.op_empty[stage]);
-        ++n;
-        stage ^= 1;
-        if (stage == 0) ph ^= 1;
-      }
-      if (n > 0) mma_commit(&bars.done);
-    }
-    __syncwarp();
-  }
-  fence_before();
-  __syncthreads();
-  CTA_T(1);
-  if (warp == 8) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS));
-}
-
-
-// ---------------------------------------------------------------------------------------------------------
-// Forward / data-gradient GEMM, TMA-tiled: same roles and MMA scheme as k_gemm_nt_tc, but the A tiles are fetched by
-// a loader warp with 2-D tensor-map copies (cp.async.bulk.tensor, one [128 rows x 32 floats] box per 128-byte swizzle
-// span, SWIZZLE_128B) into an NS-deep ring, so the converter warps never issue global loads and their row-per-thread
-// 16-byte reads are bank-conflict free by the hardware swizzle (16-byte slot c of row r sits at slot c ^ (r & 7)).
-// Tiles are handed out dynamically from a self-resetting ticket counter (one per N block); the tile id travels with
-// the data: ring_meta -> a_meta -> d_meta, a negative id is the stop sentinel.
-// A is addressed as a 2-D tensor [row_blk * nblocks, a_cb] with pitch lda: column block b of a blocked operand starts at
-// tensor row b * row_blk (row_blk = a_cbs / lda), rows beyond M of a block alias the next block (their products are
-// never stored) and out-of-range columns / rows are zero-filled by the TMA unit.
-
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* tm, int x, int y, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-          smem_u32(dst)),
-      "l"(tm), "r"(x), "r"(y), "r"(smem_u32(bar))
-      : "memory");
-}
-
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, const void* src, int x, int y, int z) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%1, %2, %3}], [%4];" ::"l"(tm), "r"(x),
-               "r"(y), "r"(z), "r"(smem_u32(src))
-               : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* tm, const void* src, int x, int y, int z) {
-  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%1, %2, %3}], [%4];" ::"l"(tm),
-               "r"(x), "r"(y), "r"(z), "r"(smem_u32(src))
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-struct NtTmaBars {
-  uint64_t ring_full[RING_MAX], ring_empty[RING_MAX], a_full[2], a_empty[2], d_full[2], d_empty[2];
-  int ring_meta[RING_MAX], a_meta[2], d_meta[2];
-};
-
-__global__ void __launch_bounds__(TMA_THREADS, 1)
-    k_gemm_nt_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmC, NtArgs g, int NS,
-                  int row_blk) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ uint32_t s_tmem;
-  __shared__ __align__(16) float s_bias[128];
-  __shared__ __align__(8) NtTmaBars bars;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  CTA_T(0);
-  const int K = g.K, BN = g.BN;
-  const int n0 = blockIdx.y * BN;
-  const int kz = blockIdx.z;                                // K plane (column block of A) of this CTA
-  const int ctr_i = blockIdx.y + gridDim.y * kz;            // ticket counter of this (N block, K plane)
-  const uint32_t LBO = 128, SBO = (uint32_t)(K / 4) * 128;
-  const int kq = K / 4;
-  unsigned char* sBhi = smem;
-  unsigned char* sBlo = smem + (size_t)BN * K * 4;
-  // swizzle atoms need 1024-byte alignment in the shared address space
-  unsigned char* ring0 = smem + (size_t)BN * K * 8;
-  ring0 += (1024u - (smem_u32(ring0) & 1023u)) & 1023u;
-  unsigned char* stD = ring0 + (size_t)NS * 32 * 1024;
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)),
-                 "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  if (tid == 0) {
-    for (int s = 0; s < RING_MAX; ++s) {
-      mbar_init(&bars.ring_full[s], 1);
-      mbar_init(&bars.ring_empty[s], 128);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&bars.a_full[s], 128);
-      mbar_init(&bars.a_empty[s], 1);
-      mbar_init(&bars.d_full[s], 1);
-      mbar_init(&bars.d_empty[s], 128);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  fence_before();
-  __syncthreads();
-  fence_after();
-  const uint32_t tmem = s_tmem;
-  const int mtiles = (g.M + 127) / 128;
-  const int nchunks = (K + KC - 1) / KC;
-
-  if (warp == 9) {
-    // ================= loader (one thread) =================
-    if (lane == 0) {
-      uint32_t rs = 0, rph = 0;
-      int tr_i = 0;
-      while (true) {
-        const unsigned int c = atomicAdd(&g.ctr[ctr_i], 1u);
-        if (c >= (unsigned int)mtiles) {
-          if (c == (unsigned int)mtiles + gridDim.x - 1) g.ctr[ctr_i] = 0;   // last ticket of the launch
-          mbar_wait(&bars.ring_empty[rs], rph ^ 1);
-          bars.ring_meta[rs] = -1;
-          mbar_arrive(&bars.ring_full[rs]);
-          break;
-        }
-        for (int ch = 0; ch < nchunks; ++ch) {
-          const int k0 = ch * KC;
-          const int kw = min(KC, K - k0);
-          const int x0 = k0 % g.a_cb, y0 = (k0 / g.a_cb + kz) * row_blk + (int)c * 128;
-          TRACE(0, tr_i, 0);
-          mbar_wait(&bars.ring_empty[rs], rph ^ 1);
-          TRACE(0, tr_i, 1);
-          ++tr_i;
-          bars.ring_meta[rs] = (int)c;
-          unsigned char* st = ring0 + (size_t)rs * 32 * 1024;
-          const int nbox = kw > 32 ? 2 : 1;
-          mbar_arrive_tx(&bars.ring_full[rs], (uint32_t)nbox * 16384u);
-          tma_load_2d(st, &tmA, x0, y0, &bars.ring_full[rs]);
-          if (nbox == 2) tma_load_2d(st + 16384, &tmA, x0 + 32, y0, &bars.ring_full[rs]);
-          if (++rs == (uint32_t)NS) { rs = 0; rph ^= 1; }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp < 4) {
-    // ================= A converters: ring stage (swizzled rows) -> hi/lo -> TMEM stage =================
-    const uint32_t lane_off = (uint32_t)(warp * 32) << 16;
-    uint32_t rs = 0, rph = 0, stage = 0, ph = 0;
-    int ch = 0, tr_i = 0;
-    while (true) {
-      TRACE(1, tr_i, 0);
-      mbar_wait(&bars.ring_full[rs], rph);
-      const int mt = bars.ring_meta[rs];
-      if (mt < 0) break;
-      TRACE(1, tr_i, 1);
-      const int kw = min(KC, K - ch * KC);
-      const unsigned char* row = ring0 + (size_t)rs * 32 * 1024 + tid * 128;
-      float4 vr[KC / 4];
-#pragma unroll
-      for (int q = 0; q < KC / 4; ++q)
-        vr[q] = *reinterpret_cast<const float4*>(row + (q >> 3) * 16384 + (((q & 7) ^ (tid & 7)) << 4));
-      mbar_wait(&bars.a_empty[stage], ph ^ 1);
-      fence_after();
-      TRACE(1, tr_i, 2);
-      const uint32_t t_hi = tmem + lane_off + A_COL + stage * 128;
-#pragma unroll
-      for (int grp = 0; grp < KC / 16; ++grp) {
-        if (grp * 16 < kw) {
-          uint32_t hi[16], lo[16];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float4 v = vr[grp * 4 + q];
-            hi[q * 4 + 0] = tf32_hi(v.x); lo[q * 4 + 0] = tf32_lo(v.x, hi[q * 4 + 0]);
-            hi[q * 4 + 1] = tf32_hi(v.y); lo[q * 4 + 1] = tf32_lo(v.y, hi[q * 4 + 1]);
-            hi[q * 4 + 2] = tf32_hi(v.z); lo[q * 4 + 2] = tf32_lo(v.z, hi[q * 4 + 2]);
-            hi[q * 4 + 3] = tf32_hi(v.w); lo[q * 4 + 3] = tf32_lo(v.w, hi[q * 4 + 3]);
-          }
-          tmem_st16(t_hi + grp * 16, hi);
-          tmem_st16(t_hi + KC + grp * 16, lo);
-        }
-      }
-      tmem_wait_st();
-      fence_before();
-      mbar_arrive(&bars.ring_empty[rs]);
-      if (tid == 0) bars.a_meta[stage] = mt;
-      mbar_arrive(&bars.a_full[stage]);
-      TRACE(1, tr_i, 3);
-      ++tr_i;
-      if (++ch == nchunks) ch = 0;
-      stage ^= 1;
-      if (stage == 0) ph ^= 1;
-      if (++rs == (uint32_t)NS) { rs = 0; rph ^= 1; }
-    }
-    mbar_wait(&bars.a_empty[stage], ph ^ 1);
-    if (tid == 0) bars.a_meta[stage] = -1;
-    mbar_arrive(&bars.a_full[stage]);
-  } else {
-    // ---- B (weights) -> smem, split hi/lo, canonical K-major (warps 4-8, once per CTA, while A already streams)
-    {
-      const int t = tid - 128, w = t >> 5, nlo = lane & 7, klo = lane >> 3;
-      (void)t;
-      const int kqb = (kq + 3) / 4, nblk8 = (BN / 8) * kqb;
-      // block b = (n8, kb): 8 weight rows x 4 sixteen-byte K pieces; a warp takes blocks w, w+5, w+10, ... and walks
-      // (n8, kb) incrementally (no per-item integer division: this loop is on the MMA warp's critical path)
-      if (warp == 5) TRACE(5, 0, 0);
-      int n8 = w / kqb, kb = w - n8 * kqb;
-      for (int b0 = w; b0 < nblk8; b0 += 16 * 5) {
-        float4 v[16];   // 16 independent 16-byte loads in flight per thread
-        int n8l = n8, kbl = kb;
-#pragma unroll
-        for (int u = 0; u < 16; ++u) {
-          const int n = n8l * 8 + nlo, kc = kbl * 4 + klo;
-          v[u] = (b0 + u * 5 < nblk8 && kc < kq && n0 + n < g.Nc)
-                     ? ldg4(g.B + (size_t)(n0 + n) * g.ldb + (size_t)kz * K + kc * 4)
-                     : f4zero();
-          kbl += 5;
-          while (kbl >= kqb) { kbl -= kqb; ++n8l; }
-        }
-        if (warp == 5 && b0 == w) TRACE(5, 0, 1);
-#pragma unroll
-        for (int u = 0; u < 16; ++u) {
-          const int kc = kb * 4 + klo;
-          if (b0 + u * 5 < nblk8 && kc < kq) {
-            uint4 h, l;
-            h.x = tf32_hi(v[u].x); h.y = tf32_hi(v[u].y); h.z = tf32_hi(v[u].z); h.w = tf32_hi(v[u].w);
-            l.x = tf32_lo(v[u].x, h.x); l.y = tf32_lo(v[u].y, h.y); l.z = tf32_lo(v[u].z, h.z); l.w = tf32_lo(v[u].w, h.w);
-            const uint32_t off = (uint32_t)n8 * SBO + (uint32_t)nlo * 16 + (uint32_t)kc * LBO;
-            *reinterpret_cast<uint4*>(sBhi + off) = h;
-            *reinterpret_cast<uint4*>(sBlo + off) = l;
-          }
-          kb += 5;
-          while (kb >= kqb) { kb -= kqb; ++n8; }
-        }
-      }
-    }
-    if (warp == 5) TRACE(5, 0, 2);
-    if (tid - 128 < 128) {
-      const int c = tid - 128;
-      s_bias[c] = (g.bias && kz == 0 && c < BN && n0 + c < g.Nc) ? __ldg(g.bias + n0 + c) : 0.f;
-    }
-    fence_async_smem();
-    asm volatile("bar.sync 3, 160;" ::: "memory");
-    if (warp == 5) TRACE(5, 0, 3);
-    if (warp == 4) {
-      // ================= MMA issuer (one thread) =================
-      if (lane == 0) {
-        const uint32_t idesc = make_idesc(128, BN);
-        const uint32_t bhi0 = smem_u32(sBhi), blo0 = smem_u32(sBlo);
-        uint32_t stage = 0, ph = 0, ds = 0, dph = 0;
-        bool stop = false;
-        int tr_i = 0;
-        while (!stop) {
-          uint32_t t_d = 0;
-          for (int ch = 0; ch < nchunks; ++ch) {
-            const int k0 = ch * KC;
-            const int kw = min(KC, K - k0);
-            TRACE(2, tr_i, 0);
-            mbar_wait(&bars.a_full[stage], ph);
-            fence_after();
-            const int mt = bars.a_meta[stage];
-            if (mt < 0) { stop = true; break; }
-            TRACE(2, tr_i, 1);
-            if (ch == 0) {
-              mbar_wait(&bars.d_empty[ds], dph ^ 1);
-              fence_after();
-              bars.d_meta[ds] = mt;
-              __threadfence_block();
-              t_d = tmem + D_COL + ds * 128;
-            }
-            const uint32_t t_hi = tmem + A_COL + stage * 128;
-            for (int s = 0; s < kw / 8; ++s) {
-              const uint32_t koff = (uint32_t)((k0 >> 3) + s) * 2 * LBO;
-              const uint64_t bhi = make_desc(bhi0 + koff, LBO, SBO);
-              const uint64_t blo = make_desc(blo0 + koff, LBO, SBO);
-              mma_ts(t_d, t_hi + s * 8, bhi, idesc, (ch | s) ? 1u : 0u);
-              mma_ts(t_d, t_hi + KC + s * 8, bhi, idesc, 1u);
-              mma_ts(t_d, t_hi + s * 8, blo, idesc, 1u);
-            }
-            mma_commit(&bars.a_empty[stage]);
-            TRACE(2, tr_i, 2);
-            ++tr_i;
-            stage ^= 1;
-            if (stage == 0) ph ^= 1;
-          }
-          if (stop) break;
-          mma_commit(&bars.d_full[ds]);
-          ds ^= 1;
-          if (ds == 0) dph ^= 1;
-        }
-        mbar_wait(&bars.d_empty[ds], dph ^ 1);             // stop sentinel for the epilogue warps
-        bars.d_meta[ds] = -1;
-        __threadfence_block();
-        mbar_arrive(&bars.d_full[ds]);
-      }
-      __syncwarp();
-    } else {
-      // ================= epilogue: accumulator stage -> registers (+bias, relu) -> swizzled slab -> TMA store ======
-      // A thread owns one accumulator row.  Each epilogue WARP works on its own 32 rows: it writes their 32 columns
-      // of a slab into its 4 KB piece of shared memory in the 128-byte-swizzle pattern and its lane 0 hands the
-      // [32 x 32] box to the TMA unit (cp.async.bulk.tensor store) -- the global writes are asynchronous full lines,
-      // the warps never issue LDS/STG for them and never wait for each other (no CTA-level barrier in the loop; the
-      // thread-store version spent ~1200 cycles per slab, 4850 per 128x128 tile: the bottleneck of the forward GEMM).
-      // Two buffers per warp alternate; a buffer is rewritten only after the store that read it has drained.  The
-      // TMEM load of the next slab is in flight while the current one is written out.
-      const int q4 = warp & 3;
-      const uint32_t lane_off = (uint32_t)(q4 * 32) << 16;
-      unsigned char* wslab = stD + q4 * 4096;
-      uint32_t ds = 0, dph = 0;
-      uint32_t slab_ctr = 0;
-      int tr_i = 0;
-      const int nsl = (BN + 31) / 32;
-      while (true) {
-        TRACE(4, tr_i, 0);
-        mbar_wait(&bars.d_full[ds], dph);
-        fence_after();
-        const int mt = bars.d_meta[ds];
-        if (mt < 0) break;
-        TRACE(4, tr_i, 1);
-        const int row0 = mt * 128 + q4 * 32;
-        const uint32_t t_d = tmem + lane_off + D_COL + ds * 128;
-        uint32_t ra[2][2][16];                            // [buffer][column half][16 columns]
-        tmem_ld16(t_d, ra[0][0]);
-        tmem_ld16(t_d + 16, ra[0][1]);
-#pragma unroll
-        for (int sl = 0; sl < 4; ++sl) {
-          if (sl >= nsl) break;
-          const int c0 = sl * 32;
-          unsigned char* slab = wslab + (slab_ctr & 1) * 16384;
-          ++slab_ctr;
-          tmem_wait_ld();
-          if (sl + 1 < nsl) {
-            tmem_ld16(t_d + c0 + 32, ra[(sl + 1) & 1][0]);
-            tmem_ld16(t_d + c0 + 48, ra[(sl + 1) & 1][1]);
-          }
-          if (lane == 0) bulk_wait_read<1>();             // this warp's store from two slabs ago has read the buffer
-          __syncwarp();
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float4 bq = *reinterpret_cast<const float4*>(s_bias + c0 + q * 4);   // warp-uniform: broadcast
-            const uint32_t* rr = &ra[sl & 1][q >> 2][(q & 3) * 4];
-            float4 o = make_float4(__uint_as_float(rr[0]) + bq.x, __uint_as_float(rr[1]) + bq.y,
-                                   __uint_as_float(rr[2]) + bq.z, __uint_as_float(rr[3]) + bq.w);
-            if (g.relu) o = f4max(o, f4zero());
-            *reinterpret_cast<float4*>(slab + lane * 128 + (((q ^ lane) & 7) << 4)) = o;
-          }
-          fence_async_smem();                             // generic-proxy writes -> visible to the TMA (async proxy)
-          __syncwarp();
-          if (lane == 0) {
-            const int col = n0 + c0;
-            if (g.reduce) tma_reduce_add_3d(&tmC, slab, col % g.c_cb, row0, col / g.c_cb);
-            else tma_store_3d(&tmC, slab, col % g.c_cb, row0, col / g.c_cb);
-            bulk_commit();
-          }
-        }
-        // (the last tcgen05.wait::ld above covered every load of this accumulator stage)
-        fence_before();
-        mbar_arrive(&bars.d_empty[ds]);
-        TRACE(4, tr_i, 2);
-        ++tr_i;
-        ds ^= 1;
-        if (ds == 0) dph ^= 1;
-      }
-      if (lane == 0) bulk_wait_all();                     // all stores complete before the CTA (and its smem) goes away
-    }
-  }
-  fence_before();
-  __syncthreads();
-  CTA_T(1);
-  if (warp == 4) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS));
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qr) == cudaSuccess &&
-        qr == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
 inline bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+inline bool al8(const void* p) { return ((uintptr_t)p & 7) == 0; }
 // next ticket slot of the current device's ring (host side: one atomic increment per launch, thread-safe)
 static unsigned int* ticket_slot() {
   static std::atomic<unsigned int> next{0};
@@ -1309,22 +366,6 @@ static unsigned int* ticket_slot() {
   }
   return base + (size_t)(next.fetch_add(1u, std::memory_order_relaxed) % TICKET_SLOTS) * 8;
 }
-static bool tma_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("PERT_GEMM_TMA");
-    on = (e && e[0] == '0') ? 0 : 1;
-  }
-  return on == 1;
-}
-static bool tn_single_acc() {   // PERT_GEMM_TN_ACC=1: one weight-gradient accumulator (accuracy A/B)
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("PERT_GEMM_TN_ACC");
-    on = (e && e[0] == '1') ? 1 : 0;
-  }
-  return on == 1;
-}
 static bool tc_enabled() {
   static int on = -1;
   if (on < 0) {
@@ -1334,132 +375,109 @@ static bool tc_enabled() {
   return on == 1;
 }
 
+// grid size of a persistent launch: as many CTAs as fit on the device, shared by `parts` independent grid columns
+template <typename Kern>
+static int persistent_ctas(Kern kern, size_t smem, int parts, int* out) {
+  int occ = 0;
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, WG_THREADS, smem);
+  if (e != cudaSuccess) return (int)e;
+  const int n = PERT_NUM_SMS * (occ > 0 ? occ : 1) / parts;
+  *out = n > 0 ? n : 1;
+  return PERT_OK;
+}
+
+template <int BN>
+static int launch_nt(const NtArgs& g, int nblk, int kplanes, cudaStream_t st) {
+  const size_t smem = (size_t)BN * ((g.K + 7) & ~7) * 8;
+  auto kern = k_gemm_nt_wg<BN>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return (int)e;
+  int gx = 0;
+  int rc = persistent_ctas(kern, smem, nblk * kplanes, &gx);
+  if (rc) return rc;
+  const int pairs = (g.M + 127) / 128;
+  if (gx > pairs) gx = pairs;
+  kern<<<dim3(gx, nblk, kplanes), WG_THREADS, smem, st>>>(g);
+  return PERT_OK;
+}
+
 }  // namespace
 
 unsigned int* pert_ticket_slot() { return ticket_slot(); }
 
 // Returns PERT_ERR_UNSUPPORTED when the shape / layout is outside what the tensor-core kernels handle (the caller
 // then uses the exact-fp32 SIMT kernels of gemm.cu).
-static int gemm_nt_tc_impl(const float* A, int lda, int a_cb, long long a_cbs, const float* B, int ldb,
+static int gemm_nt_tc_impl(const float* A, int lda, int a_cb, long long a_cbs, long long a_pz, const float* B, int ldb,
                            const float* bias, float* C, int ldc, int c_cb, long long c_cbs, long long M, int Nc, int K,
-                           int relu, int reduce, int kplanes, cudaStream_t st);
+                           int relu, int kplanes, cudaStream_t st);
 
 int pert_gemm_nt_tc(const float* A, int lda, int a_cb, long long a_cbs, const float* B, int ldb, const float* bias,
                     float* C, int ldc, int c_cb, long long c_cbs, long long M, int Nc, int K, int relu,
                     cudaStream_t st) {
   if (!tc_enabled() || M < 1024) return PERT_ERR_UNSUPPORTED;
   // Deep K over a column-blocked A (the data gradient dX = [dq|dk|dv|ds] . W4 at H = 128: K = 512): the whole [BN, K]
-  // weight block (hi + lo) no longer fits in shared memory next to the ring unless BN is narrowed to 32, which re-reads
-  // A four times.  Instead run ONE PASS PER COLUMN BLOCK (plane): K' = a_cb, B' = the plane's K-slice of the weights
-  // (resident, BN = Nc), the first pass stores, the following ones leave through TMA reduce-add stores
-  // (cp.reduce.async.bulk.tensor .add.f32: the accumulation happens in L2).  A is read once, each accumulator sees
-  // K' / 8 * 3 truncating steps instead of K / 8 * 3 (accuracy), C is written nblocks times.
-  if (tma_enabled() && a_cb > 0 && a_cb < K && K % a_cb == 0 && !relu && a_cb % KC == 0 && Nc <= 128 &&
-      (size_t)Nc * K * 8 + 1024 + 1024 + 2 * 32 * 1024 + 32 * 1024 > 226 * 1024 &&
-      (size_t)Nc * a_cb * 8 + 1024 + 1024 + 2 * 32 * 1024 + 32 * 1024 <= 226 * 1024 && encode_tiled_fn()) {
-    const int nb = K / a_cb;
-    if (nb <= 8 && (c_cb <= 0 || c_cb >= Nc)) {
-      // all planes in ONE launch (gridDim.z = planes, each with its own resident K-slice of the weights and its own
-      // share of the SMs); C is zeroed first and every plane leaves through reduce-add stores
-      cudaError_t me = (ldc == Nc) ? cudaMemsetAsync(C, 0, (size_t)M * Nc * sizeof(float), st)
-                                   : cudaMemset2DAsync(C, (size_t)ldc * 4, 0, (size_t)Nc * 4, (size_t)M, st);
-      if (me != cudaSuccess) return (int)me;
-      int rc = gemm_nt_tc_impl(A, lda, a_cb, a_cbs, B, ldb, bias, C, ldc, c_cb, c_cbs, M, Nc, a_cb, 0, 1, nb, st);
-      if (rc != PERT_ERR_UNSUPPORTED) return rc;
-    }
-    for (int p = 0; p < nb; ++p) {
-      int rc = gemm_nt_tc_impl(A + (size_t)p * a_cbs, lda, 0, 0, B + (size_t)p * a_cb, ldb, p == 0 ? bias : nullptr, C,
-                               ldc, c_cb, c_cbs, M, Nc, a_cb, 0, p > 0 ? 1 : 0, 1, st);
-      if (rc != PERT_OK) return p == 0 ? rc : (rc == PERT_ERR_UNSUPPORTED ? PERT_ERR_BADARG : rc);
-    }
-    return PERT_OK;
+  // weight block (hi + lo) does not fit in shared memory unless BN is narrowed, which re-reads A once per N block.
+  // Instead every column block of A is a plane (gridDim.z) with its own resident K-slice of the weights; C is zeroed
+  // first and every plane accumulates into it (vector red.global), so A is read once.
+  if (a_cb > 0 && a_cb < K && K % a_cb == 0 && !relu && Nc <= 128 && (size_t)Nc * K * 8 > SMEM_MAX &&
+      (size_t)Nc * a_cb * 8 <= SMEM_MAX && K / a_cb <= 8 && (c_cb <= 0 || c_cb >= Nc)) {
+    cudaError_t me = (ldc == Nc) ? cudaMemsetAsync(C, 0, (size_t)M * Nc * sizeof(float), st)
+                                 : cudaMemset2DAsync(C, (size_t)ldc * 4, 0, (size_t)Nc * 4, (size_t)M, st);
+    if (me != cudaSuccess) return (int)me;
+    int rc = gemm_nt_tc_impl(A, lda, a_cb, 0, a_cbs, B, ldb, bias, C, ldc, c_cb, c_cbs, M, Nc, a_cb, 0, K / a_cb, st);
+    return rc == PERT_ERR_UNSUPPORTED ? PERT_ERR_BADARG : rc;   // C is already cleared: no fall-back from here
   }
-  return gemm_nt_tc_impl(A, lda, a_cb, a_cbs, B, ldb, bias, C, ldc, c_cb, c_cbs, M, Nc, K, relu, 0, 1, st);
+  return gemm_nt_tc_impl(A, lda, a_cb, a_cbs, 0, B, ldb, bias, C, ldc, c_cb, c_cbs, M, Nc, K, relu, 1, st);
 }
 
-static int gemm_nt_tc_impl(const float* A, int lda, int a_cb, long long a_cbs, const float* B, int ldb,
+static int gemm_nt_tc_impl(const float* A, int lda, int a_cb, long long a_cbs, long long a_pz, const float* B, int ldb,
                            const float* bias, float* C, int ldc, int c_cb, long long c_cbs, long long M, int Nc, int K,
-                           int relu, int reduce, int kplanes, cudaStream_t st) {
-  if (a_cb <= 0) { a_cb = K; a_cbs = 0; }
+                           int relu, int kplanes, cudaStream_t st) {
+  if (a_cb <= 0 || a_cb >= K) { a_cb = K; a_cbs = 0; }
   if (c_cb <= 0) { c_cb = Nc; c_cbs = 0; }
-  if (K % 8 || K > 1024 || Nc % 16 || lda % 4 || ldb % 4 || ldc % 4 || c_cb % 16 || a_cbs % 4 || c_cbs % 4 ||
-      !al16(A) || !al16(B) || !al16(C) || (bias && !al16(bias)))
+  if (K % 8 || K > 1024 || Nc % 16 || lda % 4 || ldc % 2 || c_cb % 16 || a_cbs % 4 || a_pz % 4 || c_cbs % 2 ||
+      !al16(A) || !al8(C) || M > 0x7fffffff)
     return PERT_ERR_UNSUPPORTED;
-  if (a_cb < K && a_cb % KC) return PERT_ERR_UNSUPPORTED;   // a K-chunk must not straddle two column blocks
-  // N block: <= 128 accumulator columns per CTA, Nc split into equal multiples of 16
-  // (the whole [BN, K] weight block is resident in shared memory, hi and lo: for a deep K -- the data gradient at
-  // H = 128 has K = 512 -- the block is narrowed until it fits, at the price of re-reading A once per N block)
-  int nblk = (Nc + 127) / 128;
-  size_t smem = 0;
-  int BN = 0;
+  if (a_cb < K && a_cb % 16) return PERT_ERR_UNSUPPORTED;   // a 16-column chunk must not straddle two column blocks
+  // N block: <= 128 accumulator columns per warpgroup, Nc split into equal multiples of 16 (the whole [BN, K] weight
+  // block is resident in shared memory, hi and lo: for a deep K it is narrowed until it fits, at the price of
+  // re-reading A once per N block)
+  const size_t Kp = (size_t)((K + 7) & ~7);
+  int nblk = (Nc + 127) / 128, BN = 0;
   for (;; ++nblk) {
     if (nblk > Nc / 16) return PERT_ERR_UNSUPPORTED;
     if (Nc % nblk || (Nc / nblk) % 16) continue;
     BN = Nc / nblk;
-    smem = (size_t)BN * K * 4 * 2 + 32 * 1024 + 16 * 1024;   // B hi/lo + A staging + D staging
-    // the TMA kernel needs 1 KB alignment slack + 2 ring stages + 2 x 16 KB store slabs next to B
-    const size_t need = tma_enabled() ? (size_t)BN * K * 8 + 1024 + 1024 + 2 * 32 * 1024 + 32 * 1024 : smem;
-    if (need <= 226 * 1024) break;
+    if ((size_t)BN * Kp * 8 <= SMEM_MAX) break;
   }
-  NtArgs g{A, lda, a_cb, a_cbs, B, ldb, bias, C, ldc, c_cb, c_cbs, (int)M, Nc, K, BN, relu, reduce, kplanes, nullptr};
-  const int mtiles_all = (int)((M + 127) / 128);
-  if (tma_enabled() && nblk <= 8 && encode_tiled_fn()) {
-    // TMA-tiled kernel: A as a 2-D tensor [nblocks * row_blk, a_cb] with pitch lda (see k_gemm_nt_tma)
-    const int nblocks = kplanes > 1 ? kplanes : (K + a_cb - 1) / a_cb;
-    const bool blocked = nblocks > 1;
-    const bool ok = (!blocked || (a_cbs % lda == 0 && a_cb % KC == 0)) && (size_t)lda * 4 % 16 == 0;
-    const size_t bbytes = ((size_t)BN * K * 8 + 1023) & ~(size_t)1023;
-    int NS = (int)((226 * 1024 - 1024 - (long long)bbytes - 32 * 1024) / (32 * 1024));
-    if (NS > RING_MAX) NS = RING_MAX;
-    if (ok && NS >= 2) {
-      const long long row_blk = blocked ? a_cbs / lda : 0;
-      CUtensorMap tm;
-      const cuuint64_t gdim[2] = {(cuuint64_t)(blocked ? a_cb : K),
-                                  (cuuint64_t)(blocked ? row_blk * (nblocks - 1) + M : M)};
-      const cuuint64_t gstr[1] = {(cuuint64_t)lda * 4};
-      const cuuint32_t box[2] = {32, 128};
-      const cuuint32_t estr[2] = {1, 1};
-      CUresult cr = encode_tiled_fn()(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)A, gdim, gstr, box, estr,
-                                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                      CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      // C as a 3-D tensor {columns of one block, rows, blocks}: stores clip at M and at the block width
-      CUtensorMap tc;
-      const int cblocks = (Nc + c_cb - 1) / c_cb;
-      const bool c_ok = (c_cb % 32 == 0 || cblocks == 1) && (BN % 32 == 0 || nblk == 1) && (cblocks == 1 || Nc % c_cb == 0);
-      if (cr == CUDA_SUCCESS && c_ok) {
-        const cuuint64_t cdim[3] = {(cuuint64_t)(cblocks > 1 ? c_cb : Nc), (cuuint64_t)M, (cuuint64_t)cblocks};
-        const cuuint64_t cstr[2] = {(cuuint64_t)ldc * 4, cblocks > 1 ? (cuuint64_t)c_cbs * 4 : (cuuint64_t)ldc * 4 * (cuuint64_t)M};
-        const cuuint32_t cbox[3] = {32, 32, 1};   // one box per epilogue warp
-        const cuuint32_t cest[3] = {1, 1, 1};
-        cr = encode_tiled_fn()(&tc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)C, cdim, cstr, cbox, cest,
-                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                               CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      } else if (cr == CUDA_SUCCESS) {
-        cr = CUDA_ERROR_NOT_SUPPORTED;
-      }
-      if (cr == CUDA_SUCCESS) {
-        const size_t smem2 = 1024 + bbytes + (size_t)NS * 32 * 1024 + 32 * 1024;
-        cudaError_t e2 = cudaFuncSetAttribute(k_gemm_nt_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
-        if (e2 != cudaSuccess) return (int)e2;
-        g.ctr = ticket_slot();
-        if (!g.ctr) return (int)cudaGetLastError();
-        if (nblk * kplanes > 8) return PERT_ERR_UNSUPPORTED;          // 8 ticket counters per slot
-        int gx2 = PERT_NUM_SMS / (nblk * kplanes);
-        if (gx2 < 1) gx2 = 1;
-        if (gx2 > mtiles_all) gx2 = mtiles_all;
-        k_gemm_nt_tma<<<dim3(gx2, nblk, kplanes), TMA_THREADS, smem2, st>>>(tm, tc, g, NS, (int)row_blk);
-        return PERT_OK;
-      }
-    }
+  NtArgs g{A, lda, a_cb, a_cbs, a_pz, B, ldb, bias, C, ldc, c_cb, c_cbs, (int)M, Nc, K, relu, kplanes > 1 ? 1 : 0};
+  switch (BN) {
+    case 16: return launch_nt<16>(g, nblk, kplanes, st);
+    case 32: return launch_nt<32>(g, nblk, kplanes, st);
+    case 48: return launch_nt<48>(g, nblk, kplanes, st);
+    case 64: return launch_nt<64>(g, nblk, kplanes, st);
+    case 80: return launch_nt<80>(g, nblk, kplanes, st);
+    case 96: return launch_nt<96>(g, nblk, kplanes, st);
+    case 112: return launch_nt<112>(g, nblk, kplanes, st);
+    case 128: return launch_nt<128>(g, nblk, kplanes, st);
   }
-  if (reduce || kplanes > 1) return PERT_ERR_UNSUPPORTED;   // only the TMA kernel has the reduce-add epilogue / K planes
-  cudaError_t e = cudaFuncSetAttribute(k_gemm_nt_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  return PERT_ERR_UNSUPPORTED;
+}
+
+template <int NCP>
+static int launch_tn(TnArgs g, int mblk, cudaStream_t st) {
+  const size_t smem = (size_t)NCP * RC * 4 * 2 * 2 + (size_t)NCP / 2 * WG_THREADS * 4;   // two stages (hi + lo), partials
+  auto kern = k_gemm_tn_wg<NCP>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;
-  const int mtiles = (int)((M + 127) / 128);
-  int gx = PERT_NUM_SMS / nblk;
-  if (gx < 1) gx = 1;
-  if (gx > mtiles) gx = mtiles;
-  k_gemm_nt_tc<<<dim3(gx, nblk), TC_THREADS, smem, st>>>(g);
+  int splits = 0;
+  int rc = persistent_ctas(kern, smem, mblk, &splits);
+  if (rc) return rc;
+  int rps = (g.R + splits - 1) / splits;
+  rps = (rps + RC - 1) / RC * RC;
+  splits = (g.R + rps - 1) / rps;
+  g.rows_per_split = rps;
+  kern<<<dim3(splits, mblk), WG_THREADS, smem, st>>>(g);
   return PERT_OK;
 }
 
@@ -1469,59 +487,24 @@ int pert_gemm_tn_tc(const float* A, int lda, int a_cb, long long a_cbs, const fl
   if (!tc_enabled() || R < 4096) return PERT_ERR_UNSUPPORTED;
   if (a_cb <= 0) { a_cb = Mc; a_cbs = 0; }
   if (b_cb > 0 && b_cb < Nc) return PERT_ERR_UNSUPPORTED;   // B must be a plain matrix
-  if (Nc % 4 || Nc > 160 || ldc % 4 || !al16(C)) return PERT_ERR_UNSUPPORTED;   // D: <= 256 TMEM columns; B-converter items
-  const int NcP = (Nc + 15) / 16 * 16;
+  // two adjacent output rows per thread (8-byte loads of A), two adjacent columns per vector reduction into C
+  if (Nc % 4 || Nc > 160 || Mc % 2 || a_cb % 2 || lda % 2 || a_cbs % 2 || ldc % 2 || !al8(A) || !al8(C) ||
+      R > 0x7fffffff)
+    return PERT_ERR_UNSUPPORTED;
+  (void)b_cbs;
+  TnArgs g{A, lda, a_cb, a_cbs, B, ldb, C, ldc, a_colsum, (int)R, Mc, Nc, 0};
   const int mblk = (Mc + 127) / 128;
-  if (tma_enabled() && mblk <= 8) {
-    // TMA-fed kernel: rows of A are copied in pieces of pw columns that never straddle a column block
-    const int pw = a_cb < 128 ? a_cb : 128;
-    const bool ok = pw >= 4 && 128 % pw == 0 && a_cb % pw == 0 && Mc % pw == 0 && lda % 4 == 0 && a_cbs % 4 == 0 &&
-                    ldb % 4 == 0 && al16(A) && al16(B);
-    // chunk depth: 64 reduction rows when two operand stages + >= 2 ring stages fit, else 32 (H = 128: Nc = 128 / 144)
-    int rc = 64;
-    size_t op = 0, ring = 0;
-    int NS = 0;
-    for (; rc >= 32; rc >>= 1) {
-      op = (size_t)NcP * rc * 4 * 2 * 2;
-      ring = (size_t)rc * 512 + (size_t)rc * Nc * 4;
-      NS = op < 226 * 1024 ? (int)((226 * 1024 - op) / ring) : 0;
-      if (NS >= 2) break;
-    }
-    if (NS > RING_MAX) NS = RING_MAX;
-    if (ok && NS >= 2) {
-      const int nchunks = (int)((R + rc - 1) / rc);
-      int gx = PERT_NUM_SMS / mblk;
-      if (gx < 1) gx = 1;
-      if (gx > nchunks) gx = nchunks;
-      int nacc = (TMEM_COLS - 4 * rc) / NcP;               // accumulators that fit below the A stages
-      nacc = nacc > 4 ? 4 : (nacc < 1 ? 1 : nacc);
-      if (tn_single_acc()) nacc = 1;
-      TnTmaArgs g{A,        lda, a_cb, a_cbs, B,   ldb,     C,  ldc, a_colsum,
-                  (int)R,   Mc,  Nc,   NcP,   nchunks, NS, pw, lda == pw ? 1 : 0, ldb == Nc ? 1 : 0, ticket_slot(), nacc};
-      if (!g.ctr) return (int)cudaGetLastError();
-      const size_t smem = op + ring * NS;
-      const int ngrp = (NcP + 31) / 32;
-      void (*kern)(TnTmaArgs) = nullptr;
-      if (rc == 64) kern = ngrp <= 2 ? k_gemm_tn_tma<8, 64> : (ngrp == 3 ? k_gemm_tn_tma<12, 64> : k_gemm_tn_tma<16, 64>);
-      else kern = ngrp <= 4 ? k_gemm_tn_tma<8, 32> : k_gemm_tn_tma<10, 32>;
-      if (rc == 64 && ngrp > 4) return PERT_ERR_UNSUPPORTED;
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return (int)e;
-      kern<<<dim3(gx, mblk), TMA_THREADS, smem, st>>>(g);
-      return PERT_OK;
-    }
+  switch ((Nc + 15) / 16) {
+    case 1: return launch_tn<16>(g, mblk, st);
+    case 2: return launch_tn<32>(g, mblk, st);
+    case 3: return launch_tn<48>(g, mblk, st);
+    case 4: return launch_tn<64>(g, mblk, st);
+    case 5: return launch_tn<80>(g, mblk, st);
+    case 6: return launch_tn<96>(g, mblk, st);
+    case 7: return launch_tn<112>(g, mblk, st);
+    case 8: return launch_tn<128>(g, mblk, st);
+    case 9: return launch_tn<144>(g, mblk, st);
+    case 10: return launch_tn<160>(g, mblk, st);
   }
-  if (Nc > 128) return PERT_ERR_UNSUPPORTED;   // the LDG-fed kernel below is instantiated for Nc <= 128 only
-  int splits = PERT_NUM_SMS / mblk;
-  if (splits < 1) splits = 1;
-  int rps = (int)((R + splits - 1) / splits);
-  rps = (rps + RC - 1) / RC * RC;
-  splits = (int)((R + rps - 1) / rps);
-  const size_t smem = (size_t)NcP * RC * 4 * 2 * 2;
-  TnArgs g{A, lda, a_cb, a_cbs, B, ldb, C, ldc, a_colsum, (int)R, Mc, Nc, NcP, rps};
-  auto kern = NcP <= 64 ? k_gemm_tn_tc<8> : k_gemm_tn_tc<16>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return (int)e;
-  kern<<<dim3(splits, mblk), TC_THREADS, smem, st>>>(g);
-  return PERT_OK;
+  return PERT_ERR_UNSUPPORTED;
 }

@@ -343,9 +343,8 @@ int pert_allreduce_adam(float* p, const float* g, float* m, float* v, long long 
   if (blocks < 1) blocks = 1;
   // the grid counter is monotonic: after `step` launches of `blocks` CTAs the last arrival reads step*blocks - 1
   a.arrive_target = (unsigned int)((unsigned long long)step * (unsigned long long)blocks - 1ull);
-  // measured on B200 (profiles/r2_bench_2gpu_{ag,rs}.json, r2_bench_8gpu.json): the reduce-scatter form pays a second
-  // flag round (~6-10 us) and wins it back only when the pulled volume shrinks enough: 0.670 vs 0.663 ms/step at 2
-  // GPUs, 0.675 vs 0.681 at 8 (cfg4: 2.336 vs 2.370).  PERT_PEER_MODE=ag|rs overrides (same value on every rank).
+  // the reduce-scatter form pays a second flag round and wins it back only when the pulled volume shrinks enough,
+  // i.e. at more than 4 ranks.  PERT_PEER_MODE=ag|rs overrides (same value on every rank).
   static int mode = -1;   // 0 auto, 1 all-gather form, 2 reduce-scatter form
   if (mode < 0) {
     const char* e = getenv("PERT_PEER_MODE");

@@ -16,8 +16,8 @@ namespace {
 
 constexpr int TN = 32;        // segments (nodes) per tile
 // ring geometry by row width: a tile of 32 segments at ~3 rows each is 12 / 24 / 48 KB for H = 32 / 64 / 128; the stage
-// must hold a tile with headroom (an oversized tile falls back to global loads), and 4 stages beat 3 when they fit
-// (same-box A/B at cfg2, H = 64: 3x64 KB 0.60, 4x48 KB 0.62, 5x40 KB 0.60 of the measured HBM peak)
+// must hold a tile with headroom (an oversized tile falls back to global loads), and 4 stages of 48 KB fit next to
+// each other in the 227 KB of shared memory an H100 block may use
 template <int LPR>
 struct Ring {
   static constexpr int STAGES = (LPR >= 32) ? 3 : 4;

@@ -625,8 +625,8 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
   if (HAS_E)
     for (int x = tid; x < a.n_rpc * H; x += NT) s_drpc[x] = 0.f;
   // Interface id `hot_if` (0: what the reference writes on every chain and return edge of a PERT graph, misc.py:247,289,
-  // i.e. 3 of 4 edges of real data) would serialise tens of thousands of REDG.128 on ONE 4H-byte row per layer (measured:
-  // a PERT-shaped batch ran 2x slower than a random one with twice the edges).  Its contributions stay in registers
+  // i.e. 3 of 4 edges of real data) would serialise tens of thousands of REDG.128 on ONE 4H-byte row per layer.  Its
+  // contributions stay in registers
   // and leave once per CTA (through the first row of tile A, which is dead after the tile loop: the geometry of cfg2
   // fits its 200-node graphs into a two-CTA tile with less than 256 bytes to spare).
   float4 hot[VPL];
@@ -955,8 +955,7 @@ int launch_bwd(const TileArgs& a0, long long N, long long E, long long B, bool h
   if (pd < 0 || ps < 0) return (int)cudaGetLastError();
   // VPL = 2 (H / 8 lanes per node, 256-thread CTAs) whenever two CTAs share an SM and the rpc sums still have a lane per
   // type (LPR >= RPC_FAST), i.e. H >= 64; else one vector per lane
-  // (measured r2: the two-vector variant HURTS the backward pair -- cfg2 61.3 vs 59.3 us, cfg3 148 vs 129 -- whose REDG
-  // and shared-memory atomics want the resident warps more than fewer instructions; forward gains 12 %.  So the
+  // (the backward pair's REDG and shared-memory atomics want the resident warps more than fewer instructions, so the
   // backward default stays one vector per lane; PERT_TCONV_VPL_BWD=2 selects the other for A/B.)
   static int bwd_v = -1;
   if (bwd_v < 0) {

@@ -14,7 +14,7 @@ collation rules (SURVEY.md section 8b):
 * 0-dim tensors are stacked into a 1-D tensor;
 * ``batch`` [N] int64 and ``ptr`` [B+1] int64 are added.
 
-B200 additions (not in PyG): ``Batch.pin_memory()`` stages the whole batch in ONE
+Additions (not in PyG): ``Batch.pin_memory()`` stages the whole batch in ONE
 pinned host slab and ``Batch.to(device, non_blocking=True)`` moves it with ONE
 H2D copy (the reference does one copy per attribute plus B tiny ones per step,
 pert_gnn.py:220-231); the per-attribute tensors on the device are views into

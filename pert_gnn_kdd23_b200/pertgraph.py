@@ -1,7 +1,7 @@
 """PERT-graph construction (SURVEY.md section 8f row N2): span rows of many traces -> the per-pattern graph tensors
 the reference stores in ``runtime2pertgraph_map`` (preprocess.py:350-371), built on the GPU.
 
-Reference: /root/reference/misc.py ``GraphConstruct``
+Reference: misc.py ``GraphConstruct``
   ``get_root_ms`` / ``drop_wrong_edges``  (misc.py:138-142 / :87-105)  row filters; host numpy, as in the reference
   ``build_span_graphs``                   (misc.py:190-219 + :113-175) CUDA: sorted unique ids + one edge per row
   ``build_pert_graphs``                   (misc.py:221-319 + :113-175) CUDA: csrc/pertgraph.cu builds the stage chains

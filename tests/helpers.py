@@ -109,9 +109,8 @@ def _check_one_grad(n, grad, ref, po, rtol, scale, n_convs):
         # = alpha_t (dalpha_t - sum alpha dalpha) cancels inside every target's neighbourhood (softmax shift invariance:
         # sum_t ds_t = 0, hence sum_j dk_j = 0), and dW_{q,k} = sum_nodes d{q,k} x^T sums 10^4..10^5 such terms: at
         # cfg3-5, conv 0, the result is as small as a few terms (conditioning kappa = sum|terms| / |result| ~ 10^2..10^4)
-        # and 500x below the step's largest gradient.  Every tcgen05 kind::tf32 accumulation truncates (round toward
-        # zero), which costs ~1e-5 of sum|terms| per GEMM (profiles/tn_accuracy_probe.py: 1e-5 vs 8e-7 for an fp32 FMA
-        # GEMM) in the weight gradient itself and ~1e-6 in the upstream data gradients that feed ds; kappa turns that
+        # and 500x below the step's largest gradient.  The 3xTF32 tensor-core GEMMs carry ~1e-6..1e-5 of sum|terms|
+        # (an fp32 FMA GEMM: ~1e-6) in the weight gradient itself and ~1e-6 in the upstream data gradients that feed ds; kappa turns that
         # into up to 1.5e-2 OF THESE TENSORS while it stays < 1e-5 of the step's gradient scale (DESIGN.md section 6).
         # Bar: the standard 1e-4 element-wise check (met at cfg1/cfg2 and for every layer >= 1); where kappa defeats it,
         # the absolute error must stay below 1e-5 of the largest gradient of the step and 2e-2 of the tensor.

@@ -1,6 +1,6 @@
 """-m gpu parity tests AT THE SIZES BASELINE.json NAMES, so that the kernels bench.py times are the kernels checked:
   * k_segreduce_stream (the BASELINE metric kernel; only dispatched for N >= 4096) at cfg2's real shape and around it;
-  * the tcgen05 / TMA GEMMs (NT forward into planes, data gradient out of blocked planes, TN weight gradient with the
+  * the wgmma GEMMs (NT forward into planes, data gradient out of blocked planes, TN weight gradient with the
     fused bias column sums; only dispatched for M >= 1024 / R >= 4096) at M, R in {4096, 51200, 102400} x H in {64,128};
   * the whole model (outputs, loss, every gradient, BN statistics) on the FULL cfg2 / cfg3 / cfg5 batches and a cfg4
     per-GPU shard, against the CPU oracle.
@@ -12,7 +12,7 @@ import pytest
 import torch
 
 from oracle import model_oracle
-from tests.helpers import (RTOL, assert_close, assert_grads_close, forward_args, make_batch, make_models)
+from tests.helpers import (RTOL, assert_close, forward_args, make_batch, make_models)
 
 pytestmark = pytest.mark.gpu
 
@@ -91,9 +91,8 @@ def _planes_case(M, K, H, seed):
     planes = ops.linear(xc, Wc, bc, out_blocks=4)
     gx, gW, gb = torch.autograd.grad(planes, (xc, Wc, bc), g.cuda())
     tag = f"M={M} K={K} H={H}"
-    # bars (norm-wise, against fp64): the tcgen05 kind::tf32 accumulator truncates (round toward zero) on every MMA, so
-    # the error grows with the number of accumulation steps 3*K/8 (measured r2: 6e-7 at K=64, 2.5e-6 at K=256, 5e-6 at
-    # K=512 -- DESIGN.md section 3); planes: K <= 144; dX: K = 4H; dW4: rows / CTA
+    # bars (norm-wise, against fp64): the 3xTF32 error grows with the number of accumulation steps 3*K/8
+    # (DESIGN.md section 3); planes: K <= 144; dX: K = 4H; dW4: rows / CTA
     for got, want, what, tol in ((planes.permute(1, 0, 2).reshape(M, 4 * H), ref, "planes", 2e-6),
                                  (gx, rx, "dX", 4e-6 if H <= 64 else 8e-6), (gW, rW, "dW4", 3e-5), (gb, rb, "db4", 2e-5)):
         assert_close(got, want, rtol=tol, what=f"{what} {tag}", norm_only=True)
@@ -131,15 +130,15 @@ def test_gemm_tn_fused_colsum(H):
 
 
 # ------------------------------------------------------------------ whole model at the real batch sizes
-def _full_parity(cfg, ng, tag, grad_rtol=RTOL):
+def _full_parity(cfg, ng, tag, grad_rtol=RTOL, batch=None):
     """Outputs, loss, every gradient and the BatchNorm statistics of the FULL batch against the oracle.
 
     Derivatives are compared ON THE SAME LINEAR PIECE of the network.  A batch of 10^5 nodes puts ~10^7 arguments through
     the BatchNorm ReLUs; a few dozen of them lie within the 1e-6 by which two fp32 implementations of the conv stack differ,
     and each such unit that lands on the other side of zero adds or removes one node's term from weight-gradient sums whose
-    result is ~sqrt(N) terms large -- 1e-3 of conv 0/1 gradients at cfg3-5 (measured: identical for the tcgen05, the exact
-    fp32 SIMT GEMMs and both families of conv kernels, while BatchNorm itself agrees with torch to 1e-7:
-    profiles/bn_probe.py), although every forward value agrees to 1e-6.  That is a property of fp32 evaluation of a
+    result is ~sqrt(N) terms large -- 1e-3 of conv 0/1 gradients at cfg3-5 (identical for the tensor-core, the exact
+    fp32 SIMT GEMMs and both families of conv kernels, while BatchNorm itself agrees with torch to 1e-7), although every
+    forward value agrees to 1e-6.  That is a property of fp32 evaluation of a
     piecewise-linear network, not of a kernel.  So the step ENGINE (what bench.py times) runs forward, the set of active ReLUs
     is read back from its saved activations (Engine.active_relus), and the oracle (fp32 = the reference path, fp64 =
     arbiter) is evaluated and differentiated with exactly those ReLUs active.  The free-running oracle (its own ReLUs) is
@@ -148,7 +147,7 @@ def _full_parity(cfg, ng, tag, grad_rtol=RTOL):
 
     from tests.helpers import assert_close_ref, assert_grads_close_ref
 
-    b = make_batch(cfg, ng)
+    b = make_batch(cfg, ng) if batch is None else batch
     a32 = forward_args(b)
     a64 = [t.double() if t.is_floating_point() else t for t in a32]
     oracle, model = make_models(cfg)
@@ -204,31 +203,21 @@ def test_model_cfg4_shard():
 
 
 def test_model_cfg5_full():
-    # 5 layers x 256,000 nodes x 128: outputs / loss / BN statistics at 1e-4; gradients at 2e-4 -- the truncating
-    # tensor-core accumulators (DESIGN.md section 3) compound over ten GEMM layers of backward: measured <= 8.4e-5
-    # (convs.3.lin_edge.weight; 1.9e-4 before the weight-gradient kernel rotated its chunks over several TMEM
-    # accumulators) where the exact-fp32 reference path itself is 1.3e-5 from fp64 -- the bar leaves the run-to-run
-    # spread of the float atomics (x1.5) above the measured value
+    # 5 layers x 256,000 nodes x 128: outputs / loss / BN statistics at 1e-4; gradients at 2e-4 -- the tensor-core
+    # GEMM errors (DESIGN.md section 3) compound over ten GEMM layers of backward, and the float atomics spread a
+    # run's worst value; the exact-fp32 reference path itself is 1.3e-5 from fp64
     _full_parity(5, None, "cfg5[256x1000]", grad_rtol=2e-4)
 
 
 def test_model_cfg2_jittered_sizes():
-    """cfg2 with graph sizes 200 +- 20 % (no tile is a whole number of equal graphs): the graph-aligned tiles."""
+    """cfg2 with graph sizes 200 +- 20 % (no tile is a whole number of equal graphs): the graph-aligned tiles.  Compared
+    like the other full-size batches, on the same linear piece (see _full_parity): the free-running fp32 oracle puts a
+    few BatchNorm ReLU arguments of this batch on the other side of zero depending on the host's summation order, which
+    moves conv 0/1 and embedding gradients by 1e-3..1e-2 for every GPU GEMM path alike."""
     from pert_gnn_kdd23_b200.data import Batch
     from pert_gnn_kdd23_b200.synthetic import make_data_list
 
-    oracle, model = make_models(2)
-    b = Batch.from_data_list(make_data_list(2, num_graphs=96, jitter=0.2))
-    oracle.train()
-    model.train()
-    go, lo = oracle(*forward_args(b))
-    gc, lc = model(*forward_args(b.to("cuda")))
-    assert_close(gc, go, what="cfg2j global_predict")
-    loss_o = model_oracle.torch_quantile_loss(b.y.float(), go.flatten(), 0.5)
-    loss_c = model_oracle.torch_quantile_loss(b.y.float().cuda(), gc.flatten(), 0.5)
-    loss_o.backward()
-    loss_c.backward()
-    assert_grads_close(model.named_parameters(), oracle.named_parameters(), RTOL, n_convs=len(model.convs))
+    _full_parity(2, None, "cfg2j[96]", batch=Batch.from_data_list(make_data_list(2, num_graphs=96, jitter=0.2)))
 
 
 # ------------------------------------------------------------------ eval path (pert_gnn.py:254-294) on device accumulators

@@ -1,6 +1,6 @@
 """PERT-graph construction (SURVEY N2) against the REFERENCE'S OWN GraphConstruct.
 
-tests/golden/ref_pert.npz holds what /root/reference/misc.py returned on synthetic.make_span_tables(11)
+tests/golden/ref_pert.npz holds what the reference's misc.py returned on synthetic.make_span_tables(11)
 (oracle/gen_golden_pert.py): surviving rows, root, and per trace the PERT graph (edge_index, edge_attr, node_depth,
 sorted_span_id) and the span graph (`--graph_type span`: edge_index, edge_attr, node_depth, sorted_unique_ms).
 CPU tests pin the oracle restatement and the host row filters to it; the gpu tests compare the CUDA builder

@@ -511,7 +511,8 @@ int pert_tconv_fwd(const float* q, const float* k, const float* v, const float* 
                    void* stream) {
   if (N < 0 || E < 0 || !q || !k || !v || !rowptr || !out) return PERT_ERR_BADARG;
   if (ld % 4 || ld_out % 4 || !aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out) ||
-      (s && !aligned16(s)) || (t_if && (!aligned16(t_if) || !aligned16(t_rpc) || !t_rpc || !csr_if || !csr_rpc)))
+      (s && !aligned16(s)) || (t_if && (!aligned16(t_if) || !aligned16(t_rpc) || !t_rpc)) ||
+      (t_if && E > 0 && (!csr_if || !csr_rpc)))   // an edgeless batch may pass null edge arrays
     return PERT_ERR_BADARG;
   if (N == 0) return PERT_OK;
   if (tile_enabled() && ld_out == H) {
@@ -546,8 +547,8 @@ int pert_tconv_bwd(const float* g, int ld_g, const float* q, const float* k, con
   if (ld % 4 || ld_g % 4 || ld_d % 4 || !aligned16(g) || !aligned16(q) || !aligned16(k) || !aligned16(v) ||
       !aligned16(dq) || !aligned16(dk) || !aligned16(dv))
     return PERT_ERR_BADARG;
-  if (t_if && (!t_rpc || !dt_if || !dt_rpc || !csr_if || !csr_rpc || !aligned16(dt_if) || !aligned16(dt_rpc)))
-    return PERT_ERR_BADARG;
+  if (t_if && (!t_rpc || !dt_if || !dt_rpc || !aligned16(dt_if) || !aligned16(dt_rpc))) return PERT_ERR_BADARG;
+  if (t_if && E > 0 && (!csr_if || !csr_rpc)) return PERT_ERR_BADARG;   // an edgeless batch may pass null edge arrays
   if (N == 0) return PERT_OK;
   if (tile_enabled() && ld_d == H) {
     int rt = pert_tile_bwd(g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, colptr, csc_pos, csc_dst, t_if, t_rpc,

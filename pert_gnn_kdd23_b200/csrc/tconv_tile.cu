@@ -93,10 +93,13 @@ constexpr int RPC_FAST = 8;   // fast path for n_rpc <= 8 (the reference data ha
 
 // dynamic smem layout shared by the three kernels (NA per-edge 4-byte arrays, kernel specific):
 //   [bar 16 B][tile A: T*H][tile B: T*H][rpc table (source pass only): n_rpc*H][row/col ptr slice: T+1][NA x ecap]
-// attribute ids are staged packed: interface id | rpc id << 22
+// attribute ids are staged packed: interface id | rpc id << 22.  Ids that do not fit (interface id >= 2^22, rpc id >=
+// 2^10) are seen while a tile is staged; that tile then ignores its staged edges and runs the global-gather variant, which
+// reads the two ids separately (so any int32 interface id is right, the common tile pays one compare per edge).
 #define PACK_ID(a, b) ((a) | ((b) << 22))
 #define ID_IF(x) ((x) & 0x3fffff)
 #define ID_RPC(x) ((int)((unsigned)(x) >> 22))
+__device__ __forceinline__ bool packable(int ia, int ib) { return (unsigned)ia < (1u << 22) && (unsigned)ib < (1u << 10); }
 struct Smem {
   uint64_t* bar;
   float *ta, *tb, *rpc;
@@ -282,17 +285,25 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
   for (bool first = true; next_tile(a, first, n0, nt); first = false, phase ^= 1) {
     stage_tiles<H, NT>(S, a.k, a.v, a.rowptr, n0, nt, tid);
     const int e_lo = S.ptr[0];
-    const int ne_s = min(S.ptr[nt] - e_lo, a.edge_cap);
-    int bad = 0;   // a staged neighbour outside this tile
-    for (int x = tid; x < ne_s; x += NT) {
+    const int ne_c = min(S.ptr[nt] - e_lo, a.edge_cap);
+    int bad = 0, wide = 0;   // a staged neighbour outside this tile / staged ids that do not pack
+    for (int x = tid; x < ne_c; x += NT) {
       const int nb_id = __ldg(a.csr_src + e_lo + x);
       S.e0[x] = nb_id;
       bad |= (unsigned)(nb_id - n0) >= (unsigned)nt;
-      if (HAS_E) S.e1[x] = PACK_ID(__ldg(a.csr_if + e_lo + x), __ldg(a.csr_rpc + e_lo + x));
+      if (HAS_E) {
+        const int ia = __ldg(a.csr_if + e_lo + x), ib = __ldg(a.csr_rpc + e_lo + x);
+        wide |= !packable(ia, ib);
+        S.e1[x] = PACK_ID(ia, ib);
+      }
     }
     // fast variant of the edge loops when every edge of the tile is staged and every neighbour row is in the tile
     // (whole-graph tiles): no global-memory fallbacks are compiled into it
-    const bool all_in = (__syncthreads_or(bad) == 0) && (S.ptr[nt] - e_lo <= a.edge_cap);
+    // (one barrier in the common case; a second one tells unpackable ids from neighbours outside the tile)
+    const bool any = __syncthreads_or(bad | wide) != 0;
+    const bool narrow = !(HAS_E && any && __syncthreads_or(wide));   // else every edge takes the global path
+    const int ne_s = narrow ? ne_c : 0;
+    const bool all_in = !any && (S.ptr[nt] - e_lo <= a.edge_cap);
     mbar_wait(S.bar, phase);
 
     // node slots are handed out in descending-degree order (S.ord); the q row is requested one node ahead, the skip row
@@ -328,26 +339,33 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
         for (int u = 0; u < VPL; ++u) acc[u] = f4zero();
         float m = -INFINITY, Z = 0.f;
         // software pipeline over edges: ids + table rows of edge t+1 are requested before edge t is consumed
-        int j = n0, id = 0;
+        int j = n0;
         float4 eif[VPL], erp[VPL];
 #pragma unroll
         for (int u = 0; u < VPL; ++u) eif[u] = erp[u] = f4zero();
         auto fetch = [&](int p, bool on) {
           j = n0;
-          id = 0;
+          int ia = 0, ib = 0;
           if (on) {
             const int le = p - e_lo;
             if (FAST || le < ne_s) {
               j = ldsi(sa.e0 + le * 4);
-              if (HAS_E) id = ldsi(sa.e1 + le * 4);
+              if (HAS_E) {
+                const int id = ldsi(sa.e1 + le * 4);
+                ia = ID_IF(id);
+                ib = ID_RPC(id);
+              }
             } else {
               j = __ldg(a.csr_src + p);
-              if (HAS_E) id = PACK_ID(__ldg(a.csr_if + p), __ldg(a.csr_rpc + p));
+              if (HAS_E) {
+                ia = __ldg(a.csr_if + p);
+                ib = __ldg(a.csr_rpc + p);
+              }
             }
           }
           if (HAS_E) {
-            ldrow(a.t_if, (size_t)ID_IF(id), eif);
-            ldrow(a.t_rpc, (size_t)ID_RPC(id), erp);
+            ldrow(a.t_if, (size_t)ia, eif);
+            ldrow(a.t_rpc, (size_t)ib, erp);
           }
         };
         fetch(p0, 0 < deg);
@@ -468,18 +486,26 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
   for (bool first = true; next_tile(a, first, n0, nt); first = false, phase ^= 1) {
     stage_tiles<H, NT>(S, a.k, a.v, a.rowptr, n0, nt, tid);
     const int e_lo = S.ptr[0];
-    const int ne_s = min(S.ptr[nt] - e_lo, a.edge_cap);
-    int bad = 0;   // a staged neighbour outside this tile
-    for (int x = tid; x < ne_s; x += NT) {
+    const int ne_c = min(S.ptr[nt] - e_lo, a.edge_cap);
+    int bad = 0, wide = 0;   // a staged neighbour outside this tile / staged ids that do not pack
+    for (int x = tid; x < ne_c; x += NT) {
       const int nb_id = __ldg(a.csr_src + e_lo + x);
       S.e0[x] = nb_id;
       bad |= (unsigned)(nb_id - n0) >= (unsigned)nt;
       S.f0[x] = __ldg(a.alpha + e_lo + x);
-      if (HAS_E) S.e1[x] = PACK_ID(__ldg(a.csr_if + e_lo + x), __ldg(a.csr_rpc + e_lo + x));
+      if (HAS_E) {
+        const int ia = __ldg(a.csr_if + e_lo + x), ib = __ldg(a.csr_rpc + e_lo + x);
+        wide |= !packable(ia, ib);
+        S.e1[x] = PACK_ID(ia, ib);
+      }
     }
     // fast variant of the edge loops when every edge of the tile is staged and every neighbour row is in the tile
     // (whole-graph tiles): no global-memory fallbacks are compiled into it
-    const bool all_in = (__syncthreads_or(bad) == 0) && (S.ptr[nt] - e_lo <= a.edge_cap);
+    // (one barrier in the common case; a second one tells unpackable ids from neighbours outside the tile)
+    const bool any = __syncthreads_or(bad | wide) != 0;
+    const bool narrow = !(HAS_E && any && __syncthreads_or(wide));   // else every edge takes the global path
+    const int ne_s = narrow ? ne_c : 0;
+    const bool all_in = !any && (S.ptr[nt] - e_lo <= a.edge_cap);
     mbar_wait(S.bar, phase);
 
     int slot = g0 + grp;
@@ -508,27 +534,34 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
         auto edge = [&](int p, bool on, int& j, float& al, float4 (&e)[VPL], int& rid) {
           j = n0;
           al = 0.f;
-          int id = 0;
+          int ia = 0, ib = 0;
           if (on) {
             const int le = p - e_lo;
             if (FAST || le < ne_s) {
               j = ldsi(sa.e0 + le * 4);
               al = ldsf(sa.f0 + le * 4);
-              if (HAS_E) id = ldsi(sa.e1 + le * 4);
+              if (HAS_E) {
+                const int id = ldsi(sa.e1 + le * 4);
+                ia = ID_IF(id);
+                ib = ID_RPC(id);
+              }
             } else {
               j = __ldg(a.csr_src + p);
               al = __ldg(a.alpha + p);
-              if (HAS_E) id = PACK_ID(__ldg(a.csr_if + p), __ldg(a.csr_rpc + p));
+              if (HAS_E) {
+                ia = __ldg(a.csr_if + p);
+                ib = __ldg(a.csr_rpc + p);
+              }
             }
           }
 #pragma unroll
           for (int u = 0; u < VPL; ++u) {
             e[u] = f4zero();
             if (HAS_E)
-              e[u] = f4add(ldg4(a.t_if + (size_t)ID_IF(id) * H + (lig + u * LPR) * 4),
-                           ldg4(a.t_rpc + ID_RPC(id) * H + (lig + u * LPR) * 4));
+              e[u] = f4add(ldg4(a.t_if + (size_t)ia * H + (lig + u * LPR) * 4),
+                           ldg4(a.t_rpc + ib * H + (lig + u * LPR) * 4));
           }
-          rid = ID_RPC(id);
+          rid = ib;
         };
         // ONE pass over the in-edges.  With d_t = <g_i, v_j + e_t> (shifted by the first edge's value c, which cancels
         // exactly: sum_t ds_t = 0), w_t = alpha_t (d_t - c) and dot = sum_t w_t:
@@ -638,21 +671,29 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
   for (bool first = true; next_tile(a, first, n0, nt); first = false, phase ^= 1) {
   stage_tiles<H, NT>(S, a.g, a.q, a.colptr, n0, nt, tid);   // targets of a node's out-edges live in the same graph
   const int c_lo = S.ptr[0];
-  const int ne_s = min(S.ptr[nt] - c_lo, a.edge_cap);
+  const int ne_c = min(S.ptr[nt] - c_lo, a.edge_cap);
   // per out-edge (CSC order): target, and through the CSR slot its alpha, ds and attribute ids
-  int bad = 0;   // a staged neighbour outside this tile
-  for (int x = tid; x < ne_s; x += NT) {
+  int bad = 0, wide = 0;   // a staged neighbour outside this tile / staged ids that do not pack
+  for (int x = tid; x < ne_c; x += NT) {
     const int p = __ldg(a.csc_pos + c_lo + x);
     const int nb_id = __ldg(a.csc_dst + c_lo + x);
     S.e0[x] = nb_id;
     bad |= (unsigned)(nb_id - n0) >= (unsigned)nt;
     S.f0[x] = __ldg(a.alpha + p);
     S.f1[x] = __ldg(a.dsp + p);
-    if (HAS_E) S.e1[x] = PACK_ID(__ldg(a.csr_if + p), __ldg(a.csr_rpc + p));
+    if (HAS_E) {
+      const int ia = __ldg(a.csr_if + p), ib = __ldg(a.csr_rpc + p);
+      wide |= !packable(ia, ib);
+      S.e1[x] = PACK_ID(ia, ib);
+    }
   }
   // fast variant of the edge loops when every edge of the tile is staged and every neighbour row is in the tile
   // (whole-graph tiles): no global-memory fallbacks are compiled into it
-  const bool all_in = (__syncthreads_or(bad) == 0) && (S.ptr[nt] - c_lo <= a.edge_cap);
+  // (one barrier in the common case; a second one tells unpackable ids from neighbours outside the tile)
+  const bool any = __syncthreads_or(bad | wide) != 0;
+  const bool narrow = !(HAS_E && any && __syncthreads_or(wide));   // else every edge takes the global path
+  const int ne_s = narrow ? ne_c : 0;
+  const bool all_in = !any && (S.ptr[nt] - c_lo <= a.edge_cap);
   mbar_wait(S.bar, phase);
 
   auto run = [&](auto fast_c) {
@@ -672,17 +713,24 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
       for (int t = 0; t < degmax; ++t) {
         const bool on = t < deg;
         const int c = c0 + t;
-        int i = n0, id = 0;
+        int i = n0, ia = 0, ib = 0;
         float al = 0.f, ds = 0.f;
         if (on) {
           const int le = c - c_lo;
           if (FAST || le < ne_s) {
             i = ldsi(sa.e0 + le * 4); al = ldsf(sa.f0 + le * 4); ds = ldsf(sa.f1 + le * 4);
-            if (HAS_E) id = ldsi(sa.e1 + le * 4);
+            if (HAS_E) {
+              const int id = ldsi(sa.e1 + le * 4);
+              ia = ID_IF(id);
+              ib = ID_RPC(id);
+            }
           } else {
             const int p = __ldg(a.csc_pos + c);
             i = __ldg(a.csc_dst + c); al = __ldg(a.alpha + p); ds = __ldg(a.dsp + p);
-            if (HAS_E) id = PACK_ID(__ldg(a.csr_if + p), __ldg(a.csr_rpc + p));
+            if (HAS_E) {
+              ia = __ldg(a.csr_if + p);
+              ib = __ldg(a.csr_rpc + p);
+            }
           }
         }
         const unsigned sl = (unsigned)(i - n0);
@@ -700,10 +748,10 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
           dv[u] = f4fma(al, gi, dv[u]);
           if (HAS_E && on) {
             const float4 de = f4fma(ds, qi, f4scale(al, gi));
-            if (ID_IF(id) == a.hot_if) hot[u] = f4add(hot[u], de);
-            else red4(a.dt_if + (size_t)ID_IF(id) * H + (lig + u * LPR) * 4, de);
+            if (ia == a.hot_if) hot[u] = f4add(hot[u], de);
+            else red4(a.dt_if + (size_t)ia * H + (lig + u * LPR) * 4, de);
             if (!a.rpc_ws) {                 // general path (n_rpc > RPC_FAST): privatised table, per-edge atomics
-              float* prp = s_drpc + ID_RPC(id) * H + (lig + u * LPR) * 4;
+              float* prp = s_drpc + ib * H + (lig + u * LPR) * 4;
               atomicAdd(prp + 0, de.x);
               atomicAdd(prp + 1, de.y);
               atomicAdd(prp + 2, de.z);
@@ -998,7 +1046,7 @@ int pert_tile_fwd(const float* q, const float* k, const float* v, const float* s
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if, const float* t_rpc,
                   int n_rpc, float* out, int ld_out, float* alpha, long long N, long long E, long long B, int H,
                   double* bn_acc, const PertTiles* tiles, cudaStream_t st) {
-  if (ld != H || ld_out != H || (t_if && ((size_t)n_rpc * H * 4 > 16 * 1024 || n_rpc > 1023)))
+  if (ld != H || ld_out != H || (t_if && (size_t)n_rpc * H * 4 > 16 * 1024))
     return PERT_ERR_UNSUPPORTED;
   TileArgs a{};
   a.q = q; a.k = k; a.v = v; a.s = s;
@@ -1018,7 +1066,7 @@ int pert_tile_bwd(const float* g_, int ld_g, const float* q, const float* k, con
                   const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha, float* dq, float* dk,
                   float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc, int n_rpc, long long N,
                   long long E, long long B, int H, const PertTiles* tiles, cudaStream_t st) {
-  if (ld != H || ld_g != H || ld_d != H || (t_if && ((size_t)n_rpc * H * 4 > 16 * 1024 || n_rpc > 1023)))
+  if (ld != H || ld_g != H || ld_d != H || (t_if && (size_t)n_rpc * H * 4 > 16 * 1024))
     return PERT_ERR_UNSUPPORTED;
   TileArgs a{};
   a.q = q; a.k = k; a.v = v; a.g = g_;

@@ -26,7 +26,7 @@
  *     side work shares that one auxiliary stream); (3) the SM count of
  *     each device, read once; (4) environment switches read once (debug / measurement A/B only):
  *     PERT_GEMM_TC, PERT_TCONV_TILE, PERT_TCONV_VPL, PERT_TCONV_VPL_BWD,
- *     PERT_TILE_LIST, PERT_BN_FUSE, PERT_ENGINE_FORK, PERT_PEER_MODE.
+ *     PERT_TILE_LIST, PERT_BN_FUSE, PERT_ENGINE_FORK, PERT_PEER_MODE, PERT_LINEAR_BWD_FUSED.
  *     With that, operator-level calls are re-entrant and thread-safe across streams;
  *   - rows of float matrices must be 16-byte aligned (ld % 4 == 0, base pointer 16-byte aligned)
  *     unless stated otherwise.
@@ -47,7 +47,7 @@ extern "C" {
 
 /* ABI version (major*1000 + minor).  2000: pert_tconv_bwd takes rpc_ws; node_depth / eval-metric entry points.
  * 2001: pert_pert_graph_count / pert_pert_graph_build.  2002: pert_allreduce_adam timing[5], reduce-scatter form.
- * 2003: pert_span_graph_count / pert_span_graph_build. */
+ * 2003: pert_span_graph_count / pert_span_graph_build.  2004: pert_linear_bwd_planes(_supported). */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -136,6 +136,21 @@ int pert_gemm_nt(const float* A, int lda, int a_cb, long long a_cbs, const float
 int pert_gemm_tn(const float* A, int lda, int a_cb, long long a_cbs, const float* B, int ldb, int b_cb,
                  long long b_cbs, float* C, int ldc, float* a_colsum, long long R, int Mc, int Nc, void* stream);
 int pert_colsum(const float* A, int lda, int a_cb, long long a_cbs, float* out, long long R, int Cc, void* stream);
+/* Backward of the plane-blocked node linear [q|k|v|skip] = X . W4^T + b4 in one pass over the gradient planes
+ * (tensor cores, 3xTF32; dY and X are read once):
+ *   dY: 4 planes [N, H] (row stride H, plane stride plane_stride);  X [N, K] (ldx);  W4t = W4^T [K, 4H] (ldw);
+ *   dW4 [4H, K] (ldw4) += dY^T . X;   db4 [4H] += colsum(dY);   dX[:, 0:Kd] (ldx_out) = dY . W4[:, 0:Kd] (written,
+ *   columns Kd.. untouched; bit-identical from run to run).
+ * PERT_ERR_BADARG for NULL pointers, negative sizes, Kd > K, a leading dimension shorter than its row or
+ * overlapping planes.  PERT_ERR_UNSUPPORTED (nothing launched: use pert_gemm_tn + pert_gemm_nt) unless H = 64,
+ * K in {64, 80}, Kd in {64, K}, N >= 4096, ldx == K, 16-byte aligned dY / X / dX rows, 8-byte aligned dW4 rows, and a
+ * cluster of 4 CTAs fits on the device; also with PERT_LINEAR_BWD_FUSED=0 or PERT_GEMM_TC=0.
+ * pert_linear_bwd_planes_supported: 1 if the shape, the switches and the current device qualify, else 0; operand
+ * alignment and ldx == K are the caller's to ensure (the engine's workspace always meets them). */
+int pert_linear_bwd_planes(const float* dY, long long plane_stride, const float* X, int ldx, const float* W4t, int ldw,
+                           float* dW4, int ldw4, float* db4, float* dX, int ldx_out, long long N, int H, int K, int Kd,
+                           void* stream);
+int pert_linear_bwd_planes_supported(long long N, int H, int K, int Kd);
 
 /* ---- embeddings / concat (model.py:87-97,108) -------------------------------------------------------
  * fwd: out[n,0:H] (=|+=) table[ids[n*id_stride]];  bwd: dtable[ids[n*id_stride]] += dy[n,0:H]. */
@@ -254,8 +269,9 @@ long long pert_model_workspace_offset(const PertModelDesc* desc, long long N, lo
  * Outputs: global_pred [B], local_pred [N] (NULL to skip). */
 /* Optional measurement probe: the engine records the two caller-created cudaEvent_t around ONE kernel family of ONE
  * layer, on the launching stream (bench.py: in-step duration of the dominant kernel).  kernel: 1 = fused conv forward,
- * 2 = fused conv backward (target + source pass), 3 = node-linear forward GEMM, 4 = weight-gradient GEMM,
- * 5 = data-gradient GEMM.  NULL = no probe. */
+ * 2 = fused conv backward (target + source pass), 3 = node-linear forward GEMM, 4 = weight-gradient GEMM (where the
+ * node-linear backward runs fused, pert_linear_bwd_planes: the whole backward, weight and data gradient),
+ * 5 = data-gradient GEMM (an empty interval right after 4 when fused).  NULL = no probe. */
 typedef struct PertProbe {
   int32_t kernel, layer;
   void* ev_start;

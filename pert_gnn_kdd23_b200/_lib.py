@@ -34,6 +34,8 @@ SIGNATURES = {
     "pert_gemm_nt": (I, [P, I, I, LL, P, I, P, P, I, I, LL, LL, I, I, I, I, P]),
     "pert_gemm_tn": (I, [P, I, I, LL, P, I, I, LL, P, I, P, LL, I, I, P]),
     "pert_colsum": (I, [P, I, I, LL, P, LL, I, P]),
+    "pert_linear_bwd_planes": (I, [P, LL, P, I, P, I, P, I, P, P, I, LL, I, I, I, P]),
+    "pert_linear_bwd_planes_supported": (I, [LL, I, I, I]),
     "pert_embedding_fwd": (I, [P, I, P, I, P, I, LL, I, I, P, P]),
     "pert_embedding_bwd": (I, [P, I, P, I, P, I, LL, I, P]),
     "pert_copy_cols": (I, [P, I, P, I, I, LL, P]),

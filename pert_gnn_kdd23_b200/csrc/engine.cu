@@ -774,13 +774,20 @@ int pert_model_backward(const PertModelDesc* d, const float* params, float* grad
       if (forked) table_grads(ax->s);
     }
     // weight / bias gradients of the fused node linear (packed), data gradient
+    // (conv 0: only the embedding columns [0, H) of dX0 are needed -- x and the pad columns carry no parameters)
+    const int Kd = l == 0 ? H : K;
     PROBE_START(4, l);
-    TRY(pert_gemm_tn(w.dplanes, H, H, N * (long long)H, w.x[l], K, 0, 0, w.dw4[l], K, w.db4[l], N, 4 * H, K, st));
+    int frc = pert_linear_bwd_planes(w.dplanes, N * (long long)H, w.x[l], K, w.w4t[l], 4 * H, w.dw4[l], K, w.db4[l],
+                                     w.dx, K, N, H, K, Kd, st);
+    if (frc == PERT_ERR_UNSUPPORTED)
+      TRY(pert_gemm_tn(w.dplanes, H, H, N * (long long)H, w.x[l], K, 0, 0, w.dw4[l], K, w.db4[l], N, 4 * H, K, st));
+    else if (frc != PERT_OK)
+      return frc;
     PROBE_STOP(4, l);
     PROBE_START(5, l);
-    // (conv 0: only the embedding columns [0, H) of dX0 are needed -- x and the pad columns carry no parameters)
-    TRY(pert_gemm_nt(w.dplanes, H, H, N * (long long)H, w.w4t[l], 4 * H, nullptr, w.dx, K, 0, 0, N, l == 0 ? H : K, 4 * H,
-                     0, 0, st));
+    if (frc == PERT_ERR_UNSUPPORTED)
+      TRY(pert_gemm_nt(w.dplanes, H, H, N * (long long)H, w.w4t[l], 4 * H, nullptr, w.dx, K, 0, 0, N, Kd, 4 * H, 0, 0,
+                       st));
     PROBE_STOP(5, l);
     if (l > 0) {
       // BN(+ReLU) backward of layer l-1: dx (grad wrt x[l]) -> g of conv l-1, into the skip plane

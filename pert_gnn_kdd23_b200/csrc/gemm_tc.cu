@@ -27,87 +27,11 @@
 //       nearest) into per-thread partial sums in shared memory and restarted from zero.
 // These GEMMs are memory-bound by shape (K <= 256): A read once, C written once.
 #include "common.cuh"
+#include "sm90.cuh"
 #include <atomic>
 #include <stdlib.h>
 
 namespace {
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-// wgmma shared-memory matrix descriptor (sm_90): start address, LBO, SBO in 16-byte units; base offset 0,
-// layout type 0 (no swizzle)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3fff);
-  d |= (uint64_t)((lbo >> 4) & 0x3fff) << 16;
-  d |= (uint64_t)((sbo >> 4) & 0x3fff) << 32;
-  return d;
-}
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-
-// D[64 x 32] += A[64 x 8] (registers) . B[32 x 8]^T (descriptor)
-__device__ __forceinline__ void wgmma_n32(float* d, const uint32_t* a, uint64_t b) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b)
-      : "memory");
-}
-// D[64 x 16] += A[64 x 8] . B[16 x 8]^T
-__device__ __forceinline__ void wgmma_n16(float* d, const uint32_t* a, uint64_t b) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b)
-      : "memory");
-}
-
-// Round-to-nearest split with integer ops: hi = (bits + 0x1000) & 0xffffe000 (nearest tf32, ties away from zero; two
-// full-rate ALU instructions instead of the quarter-rate cvt.rna.tf32.f32), lo = x - hi (exact in fp32,
-// |lo| <= 2^-11 |x|, either sign; the tensor core drops its low 13 bits: <= 2^-21 |x|, sign-symmetric).  A truncating
-// hi (x & 0xffffe000) makes lo one-signed and the dropped bits a one-sided residual that does not average out over
-// 10^4..10^5-term sums.
-__device__ __forceinline__ uint32_t tf32_hi(float x) { return (__float_as_uint(x) + 0x1000u) & 0xffffe000u; }
-__device__ __forceinline__ uint32_t tf32_lo(float x, uint32_t hi) { return __float_as_uint(x - __uint_as_float(hi)); }
-
-__device__ __forceinline__ void split4(const float (&v)[4], uint32_t (&h)[4], uint32_t (&l)[4]) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    h[i] = tf32_hi(v[i]);
-    l[i] = tf32_lo(v[i], h[i]);
-  }
-}
-
-// One K-step of 8 over all BN columns: hi*hi + lo*hi + hi*lo.  bhi / blo: shared addresses of the step's first core
-// matrix; 32 columns (four 8-row core-matrix groups) further is 4 * SBO.
-template <int BN>
-__device__ __forceinline__ void mma_step(float* d, const uint32_t (&ah)[4], const uint32_t (&al)[4], uint32_t bhi,
-                                         uint32_t blo, uint32_t sbo) {
-  constexpr int N32 = BN / 32;
-#pragma unroll
-  for (int j = 0; j < N32; ++j) {
-    const uint64_t dh = make_desc(bhi + j * 4 * sbo, 128, sbo), dl = make_desc(blo + j * 4 * sbo, 128, sbo);
-    wgmma_n32(d + 16 * j, ah, dh);
-    wgmma_n32(d + 16 * j, al, dh);
-    wgmma_n32(d + 16 * j, ah, dl);
-  }
-  if (BN % 32) {
-    const uint64_t dh = make_desc(bhi + N32 * 4 * sbo, 128, sbo), dl = make_desc(blo + N32 * 4 * sbo, 128, sbo);
-    wgmma_n16(d + 16 * N32, ah, dh);
-    wgmma_n16(d + 16 * N32, al, dh);
-    wgmma_n16(d + 16 * N32, ah, dl);
-  }
-}
-
-// Local column of accumulator register i (fragment of the n32 / n16 pieces: 4 registers per 8 columns)
-__device__ __forceinline__ int acc_col(int i, int t) { return (i >> 2) * 8 + 2 * t + (i & 1); }
 
 constexpr int WG_THREADS = 256;   // two warpgroups
 constexpr int SMEM_MAX = 226 * 1024;
@@ -126,16 +50,6 @@ struct NtArgs {
   int M, Nc, K, relu;
   int reduce;          // 1: accumulate into C with vector red.global (planes), bias from plane 0 only
 };
-
-// logical K position (inside the weight operand) of physical column p: see the operand staging notes above
-__device__ __forceinline__ int nt_logical_k(int p, int K16) {
-  if (p < K16) {
-    const int r = p & 15;
-    return (p & ~15) + ((r >> 1) & 1) * 8 + (r >> 2) + (r & 1) * 4;
-  }
-  const int r = p - K16;                          // trailing 8 columns (K % 16 == 8): thread t holds 2t, 2t + 1
-  return K16 + (r >> 1) + (r & 1) * 4;
-}
 
 // grid: (persistent over 128-row tile pairs, Nc / BN, planes)
 template <int BN>

@@ -196,10 +196,13 @@ class Engine:
         return self._pack_launches() + (L + 5) // 6 + self.desc.n_cat + 1 + 2 * L + (L - 1) + 1 + 1
 
     def launches_backward(self):
-        """head, pool, per conv (target pass, source pass, weight GEMM, data GEMM), per BatchNorm reduce + apply,
+        """head, pool, per conv (target pass, source pass, node-linear backward: one fused launch where
+        pert_linear_bwd_planes takes the shape, else weight GEMM + data GEMM), per BatchNorm reduce + apply,
         embedding scatters, edge-table gradients (3 layers per launch), unpack."""
-        L = self.n_convs
-        return 1 + 1 + 4 * L + 2 * (L - 1) + self.desc.n_cat + (L + 2) // 3 + self._pack_launches()
+        L, H, N = self.n_convs, self.desc.H, self._saved[8]
+        linear = sum(1 if self.lib.pert_linear_bwd_planes_supported(N, H, self.desc.k0 if l == 0 else H,
+                                                                     H) else 2 for l in range(L))
+        return 1 + 1 + 2 * L + linear + 2 * (L - 1) + self.desc.n_cat + (L + 2) // 3 + self._pack_launches()
 
     @_lib.on_device_of
     def forward(self, x, cat_X, entry_id, probs, pnn, batch, index: GraphIndex, training, probe=None,

@@ -112,6 +112,7 @@ class _LinearFn(torch.autograd.Function):
             y = torch.empty(M, Nc, device=x.device, dtype=torch.float32)
         gemm_nt_raw(x, weight, bias, y, relu=relu)
         ctx.relu = relu
+        ctx.out_blocks = out_blocks
         ctx.has_bias = bias is not None
         ctx.save_for_backward(x, weight, y if relu else None)
         return y
@@ -126,6 +127,23 @@ class _LinearFn(torch.autograd.Function):
             call("pert_relu_bwd", ptr(y), ptr(dy), dy.numel(), stream())
             LAUNCHES["n"] += 1
         dx = dw = db = None
+        M, K = x.size(-2), weight.size(1)
+        if (ctx.out_blocks == 4 and not ctx.relu and ctx.has_bias and all(ctx.needs_input_grad[:3]) and x.dim() == 2
+                and _lib.lib().pert_linear_bwd_planes_supported(M, weight.size(0) // 4, K, K)):
+            # one pass over the four gradient planes for dX, dW and db (csrc/linear_bwd.cu)
+            dx = torch.empty_like(x)
+            dw = torch.zeros_like(weight)
+            db = torch.zeros(weight.size(0), device=dy.device, dtype=torch.float32)
+            wt = weight.t().contiguous()
+            with _timed("linear_bwd_planes"):
+                rc = _lib.lib().pert_linear_bwd_planes(ptr(dy), dy.stride(0), ptr(x), x.stride(0), ptr(wt), wt.stride(0),
+                                                       ptr(dw), dw.stride(0), ptr(db), ptr(dx), dx.stride(0), M,
+                                                       weight.size(0) // 4, K, K, stream())
+            if rc == 0:
+                LAUNCHES["n"] += 1
+                return dx, dw, db, None, None
+            if rc != -2:                                      # -2: nothing launched, the GEMM pair below does it
+                _lib.check(rc, "pert_linear_bwd_planes")
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)
             wt = weight.t().contiguous()                      # [K,Nc]: B operand of dX = dY . W

@@ -325,6 +325,18 @@ static int gemm_nt_tc_impl(const float* A, int lda, int a_cb, long long a_cbs, l
                            const float* bias, float* C, int ldc, int c_cb, long long c_cbs, long long M, int Nc, int K,
                            int relu, int kplanes, cudaStream_t st);
 
+// Layout requirements of k_gemm_nt_wg, on the arguments of gemm_nt_tc_impl (K is the K of one plane).  A column block
+// that covers all of A or C is a plain matrix.
+static bool nt_tc_layout_ok(const float* A, int lda, int a_cb, long long a_cbs, long long a_pz, const float* C,
+                            int ldc, int c_cb, long long c_cbs, long long M, int Nc, int K) {
+  if (a_cb <= 0 || a_cb >= K) { a_cb = K; a_cbs = 0; }
+  if (c_cb <= 0) { c_cb = Nc; c_cbs = 0; }
+  if (K % 8 || K > 1024 || Nc % 16 || lda % 4 || ldc % 2 || c_cb % 16 || a_cbs % 4 || a_pz % 4 || c_cbs % 2 ||
+      !al16(A) || !al8(C) || M > 0x7fffffff)
+    return false;
+  return a_cb == K || a_cb % 16 == 0;   // a 16-column chunk must not straddle two column blocks
+}
+
 int pert_gemm_nt_tc(const float* A, int lda, int a_cb, long long a_cbs, const float* B, int ldb, const float* bias,
                     float* C, int ldc, int c_cb, long long c_cbs, long long M, int Nc, int K, int relu,
                     cudaStream_t st) {
@@ -332,14 +344,16 @@ int pert_gemm_nt_tc(const float* A, int lda, int a_cb, long long a_cbs, const fl
   // Deep K over a column-blocked A (the data gradient dX = [dq|dk|dv|ds] . W4 at H = 128: K = 512): the whole [BN, K]
   // weight block (hi + lo) does not fit in shared memory unless BN is narrowed, which re-reads A once per N block.
   // Instead every column block of A is a plane (gridDim.z) with its own resident K-slice of the weights; C is zeroed
-  // first and every plane accumulates into it (vector red.global), so A is read once.
+  // first and every plane accumulates into it (vector red.global), so A is read once.  The per-plane layout is checked
+  // before C is cleared: a layout the planes cannot take (Nc = 100, say) goes to the SIMT kernel like any other.
   if (a_cb > 0 && a_cb < K && K % a_cb == 0 && !relu && Nc <= 128 && (size_t)Nc * K * 8 > SMEM_MAX &&
-      (size_t)Nc * a_cb * 8 <= SMEM_MAX && K / a_cb <= 8 && (c_cb <= 0 || c_cb >= Nc)) {
+      (size_t)Nc * a_cb * 8 <= SMEM_MAX && K / a_cb <= 8 && (c_cb <= 0 || c_cb >= Nc) &&
+      nt_tc_layout_ok(A, lda, a_cb, 0, a_cbs, C, ldc, c_cb, c_cbs, M, Nc, a_cb)) {
     cudaError_t me = (ldc == Nc) ? cudaMemsetAsync(C, 0, (size_t)M * Nc * sizeof(float), st)
                                  : cudaMemset2DAsync(C, (size_t)ldc * 4, 0, (size_t)Nc * 4, (size_t)M, st);
     if (me != cudaSuccess) return (int)me;
     int rc = gemm_nt_tc_impl(A, lda, a_cb, 0, a_cbs, B, ldb, bias, C, ldc, c_cb, c_cbs, M, Nc, a_cb, 0, K / a_cb, st);
-    return rc == PERT_ERR_UNSUPPORTED ? PERT_ERR_BADARG : rc;   // C is already cleared: no fall-back from here
+    return rc == PERT_ERR_UNSUPPORTED ? PERT_ERR_BADARG : rc;   // cannot happen after nt_tc_layout_ok; C is cleared
   }
   return gemm_nt_tc_impl(A, lda, a_cb, a_cbs, 0, B, ldb, bias, C, ldc, c_cb, c_cbs, M, Nc, K, relu, 1, st);
 }
@@ -349,10 +363,7 @@ static int gemm_nt_tc_impl(const float* A, int lda, int a_cb, long long a_cbs, l
                            int relu, int kplanes, cudaStream_t st) {
   if (a_cb <= 0 || a_cb >= K) { a_cb = K; a_cbs = 0; }
   if (c_cb <= 0) { c_cb = Nc; c_cbs = 0; }
-  if (K % 8 || K > 1024 || Nc % 16 || lda % 4 || ldc % 2 || c_cb % 16 || a_cbs % 4 || a_pz % 4 || c_cbs % 2 ||
-      !al16(A) || !al8(C) || M > 0x7fffffff)
-    return PERT_ERR_UNSUPPORTED;
-  if (a_cb < K && a_cb % 16) return PERT_ERR_UNSUPPORTED;   // a 16-column chunk must not straddle two column blocks
+  if (!nt_tc_layout_ok(A, lda, a_cb, a_cbs, a_pz, C, ldc, c_cb, c_cbs, M, Nc, K)) return PERT_ERR_UNSUPPORTED;
   // N block: <= 128 accumulator columns per warpgroup, Nc split into equal multiples of 16 (the whole [BN, K] weight
   // block is resident in shared memory, hi and lo: for a deep K it is narrowed until it fits, at the price of
   // re-reading A once per N block)

@@ -47,7 +47,8 @@ extern "C" {
 
 /* ABI version (major*1000 + minor).  2000: pert_tconv_bwd takes rpc_ws; node_depth / eval-metric entry points.
  * 2001: pert_pert_graph_count / pert_pert_graph_build.  2002: pert_allreduce_adam timing[5], reduce-scatter form.
- * 2003: pert_span_graph_count / pert_span_graph_build.  2004: pert_linear_bwd_planes(_supported). */
+ * 2003: pert_span_graph_count / pert_span_graph_build.  2004: pert_linear_bwd_planes(_supported).
+ * 2005: pert_model_forward takes dropout + dropout_state, pert_model_backward takes dropout. */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -281,17 +282,32 @@ int pert_model_forward(const PertModelDesc* desc, const float* params, float* bn
                        const float* x, const int64_t* cat_X, const int64_t* entry_id, const float* probs,
                        const float* pnn, const int64_t* batch, long long N, long long E, long long B,
                        const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc, void* workspace,
-                       long long workspace_bytes, int training, float* global_pred, float* local_pred, int* status,
-                       const PertProbe* probe, void* index_ready, void* stream);
+                       long long workspace_bytes, int training, float dropout, long long* dropout_state,
+                       float* global_pred, float* local_pred, int* status, const PertProbe* probe, void* index_ready,
+                       void* stream);
 /* index_ready: optional cudaEvent_t recorded (on another stream) after the graph index was built: the forward waits
  * for it only right before the first attention kernel, so the index build overlaps the parameter pack, the input
  * prologue and the first GEMM.  NULL = the index is already complete in `stream` order.
- * Must follow pert_model_forward on the same workspace.  d_global [B], d_local [N] or NULL. */
+ *
+ * dropout: F.dropout(x, p=dropout, training) after every BatchNorm + ReLU (model.py:103), fused into the BatchNorm
+ * apply.  Used only when training; p = 0 runs exactly the kernels of a model without dropout.  dropout_state: caller
+ * device memory, two int64 {seed, step}; a training forward with p > 0 reads it in stream order and adds 1 to step, so
+ * a captured graph draws a new mask on every replay.  The mask is a pure function of (seed, step, layer, position):
+ *   Philox4x32-10 (Random123), key = (seed & 0xffffffff, seed >> 32),
+ *   counter = (g, l, step & 0xffffffff, step >> 32), g = row*(H/4) + col/4 (the float4 group), l = the conv whose
+ *   BatchNorm output is dropped (0 .. n_convs-2); output word j of the group decides column col + j.
+ *   Element kept iff word >= T, T = floor(p * 2^32) in fp64 (p = 1: all dropped); kept values are multiplied by
+ *   (float)(1 / (1 - p)), 0 at p = 1.
+ * PERT_ERR_BADARG, before any CUDA call, when p is NaN or outside [0, 1], or when training with p > 0 and
+ * dropout_state is NULL or N*H/4 >= 2^32.
+ *
+ * Must follow pert_model_forward on the same workspace, with the same training flag and dropout (the backward applies
+ * the 1/(1-p) factor; the mask is read back from the saved activations).  d_global [B], d_local [N] or NULL. */
 int pert_model_backward(const PertModelDesc* desc, const float* params, float* grads, const int64_t* cat_X,
                         const int64_t* entry_id, const float* probs, const float* pnn, const int64_t* batch,
                         long long N, long long E, long long B, const int* rowptr, const int* csr_src,
                         const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
-                        const int* csc_dst, void* workspace, long long workspace_bytes, int training,
+                        const int* csc_dst, void* workspace, long long workspace_bytes, int training, float dropout,
                         const float* d_global, const float* d_local, const PertProbe* probe, void* stream);
 
 /* ---- device-side batch assembly from a resident pattern store (csrc/store.cu) ---------------------------------------

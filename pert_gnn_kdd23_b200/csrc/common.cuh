@@ -91,4 +91,8 @@ int pert_tconv_bwd_tiles(const float* g, int ld_g, const float* q, const float* 
 int pert_bn_fwd_ex(const float* x, int ld_x, const float* gamma, const float* beta, float* running_mean,
                    float* running_var, long long* num_batches_tracked, float eps, float momentum, int training,
                    int relu, float* mean, float* rstd, float* y, int ld_y, long long N, int H, void* workspace,
-                   long long workspace_bytes, int stats_ready, void* stream);
+                   long long workspace_bytes, int stats_ready, float dropout, const long long* drop_ctr,
+                   int drop_layer, void* stream);
+int pert_bn_bwd_ex(const float* dy, int ld_dy, const float* y, int ld_y, const float* x, int ld_x, const float* mean,
+                   const float* rstd, const float* gamma, int relu, float relu_scale, int training, float* dx,
+                   int ld_dx, float* dgamma, float* dbeta, float* sums, long long N, int H, void* stream);

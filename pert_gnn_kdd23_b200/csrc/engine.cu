@@ -156,7 +156,17 @@ struct SegList {
   Seg s[SEG_MAX];
   int count;
 };
-__global__ void k_pack(const float* __restrict__ params, float* __restrict__ packed, SegList L) {
+// dropout_state != null (first pack launch of a training forward with dropout): one thread copies the caller's
+// {seed, step} into the workspace word the BatchNorm applies of this forward read, and advances step -- no extra launch,
+// and a replayed graph reads the step as it stands at replay time.
+__global__ void k_pack(const float* __restrict__ params, float* __restrict__ packed, SegList L,
+                       long long* dropout_state, long long* drop_ctr) {
+  if (dropout_state && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
+    const long long seed = dropout_state[0], step = dropout_state[1];
+    drop_ctr[0] = seed;
+    drop_ctr[1] = step;
+    dropout_state[1] = step + 1;
+  }
   const Seg& s = L.s[blockIdx.y];
   int n = s.rows * s.cols;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -352,6 +362,7 @@ struct Ws {
   // backward temporaries
   float *dplanes, *dx, *dsp, *rpc_ws, *sums, *dpool, *dzent, *dh1;
   int* tiles;      // graph-aligned tile list of the batch (pert_tile_list_ints ints), built in forward, reused in backward
+  long long* drop_ctr;  // {seed, step} of the last training forward with dropout (k_pack -> BatchNorm applies)
   long long total;  // floats
   long long packed_floats;
 };
@@ -415,6 +426,7 @@ Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* b
   w.dpool = take(B * H);
   w.dzent = take(B * H);
   w.dh1 = take(B * H);
+  w.drop_ctr = (long long*)take(4);
   w.total = off;
   return w;
 }
@@ -541,6 +553,13 @@ int check_desc(const PertModelDesc* d) {
   if (!pert_tconv_supported_width(d->H)) return PERT_ERR_UNSUPPORTED;
   return PERT_OK;
 }
+// dropout p in [0, 1] (NaN rejected); a training forward with p > 0 needs the {seed, step} state, and its float4 groups
+// N*H/4 must fit the 32-bit counter word of the mask
+int check_dropout(const PertModelDesc* d, long long N, int training, float p, const long long* state) {
+  if (!(p >= 0.f && p <= 1.f)) return PERT_ERR_BADARG;
+  if (training && p > 0.f && (!state || N * (d->H / 4) >= (1LL << 32))) return PERT_ERR_BADARG;
+  return PERT_OK;
+}
 
 #define PROBE_START(kid, lay)                                                              \
   do {                                                                                     \
@@ -590,12 +609,15 @@ int pert_model_forward(const PertModelDesc* d, const float* params, float* bn_ru
                        const float* x, const int64_t* cat_X, const int64_t* entry_id, const float* probs,
                        const float* pnn, const int64_t* batch, long long N, long long E, long long B,
                        const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc, void* workspace,
-                       long long workspace_bytes, int training, float* global_pred, float* local_pred, int* status,
-                       const PertProbe* probe, void* index_ready, void* stream) {
+                       long long workspace_bytes, int training, float dropout, long long* dropout_state,
+                       float* global_pred, float* local_pred, int* status, const PertProbe* probe, void* index_ready,
+                       void* stream) {
   TRY(check_desc(d));
+  TRY(check_dropout(d, N, training, dropout, dropout_state));
   std::lock_guard<std::mutex> issue_lock(engine_mutex());
   if (!params || !x || !cat_X || !entry_id || !probs || !pnn || !batch || !rowptr || !workspace || !global_pred)
     return PERT_ERR_BADARG;
+  const bool drop = training && dropout > 0.f;
   if (E > 0 && (!csr_src || !csr_if || !csr_rpc)) return PERT_ERR_BADARG;
   float* base = (float*)workspace;
   Ws w = carve(d, N, E, B, base);
@@ -610,11 +632,14 @@ int pert_model_forward(const PertModelDesc* d, const float* params, float* bn_ru
   {
     SegList S;
     S.count = 0;
+    bool first = true;
     for (int l = 0; l < L; ++l) {
       append_layer_segs(S, d, w, base, l);
       if (S.count + SEGS_PER_LAYER_MAX > SEG_MAX || l == L - 1) {
-        k_pack<<<dim3(8, S.count), 256, 0, st>>>(params, base, S);
+        k_pack<<<dim3(8, S.count), 256, 0, st>>>(params, base, S, (drop && first) ? dropout_state : nullptr,
+                                                 w.drop_ctr);
         S.count = 0;
+        first = false;
       }
     }
   }
@@ -677,7 +702,7 @@ int pert_model_forward(const PertModelDesc* d, const float* params, float* bn_ru
       TRY(pert_bn_fwd_ex(w.out[l], H, params + d->off_bn_g[l], params + d->off_bn_b[l], rm, rv,
                          (training && bn_nbt) ? bn_nbt + l : nullptr, d->bn_eps, d->bn_momentum, training, 1,
                          w.bn_stats[l], w.bn_stats[l] + H, w.x[l + 1], H, N, H, w.bn_part,
-                         pert_bn_workspace_bytes(N, H), stats_fused, st));
+                         pert_bn_workspace_bytes(N, H), stats_fused, drop ? dropout : 0.f, w.drop_ctr, l, st));
     }
   }
   // 4. local head + weighted add-pool, global head
@@ -702,9 +727,13 @@ int pert_model_backward(const PertModelDesc* d, const float* params, float* grad
                         const int64_t* entry_id, const float* probs, const float* pnn, const int64_t* batch,
                         long long N, long long E, long long B, const int* rowptr, const int* csr_src,
                         const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
-                        const int* csc_dst, void* workspace, long long workspace_bytes, int training,
+                        const int* csc_dst, void* workspace, long long workspace_bytes, int training, float dropout,
                         const float* d_global, const float* d_local, const PertProbe* probe, void* stream) {
   TRY(check_desc(d));
+  if (!(dropout >= 0.f && dropout <= 1.f)) return PERT_ERR_BADARG;
+  // the saved activations already carry the mask (see k_bn_bwd_reduce): only the 1 / (1 - p) factor is needed
+  const float relu_scale = (training && dropout > 0.f) ? (dropout >= 1.f ? 0.f : (float)(1.0 / (1.0 - (double)dropout)))
+                                                       : 1.f;
   std::lock_guard<std::mutex> issue_lock(engine_mutex());
   if (!params || !grads || !cat_X || !entry_id || !probs || !pnn || !batch || !rowptr || !colptr || !workspace ||
       !d_global)
@@ -791,9 +820,9 @@ int pert_model_backward(const PertModelDesc* d, const float* params, float* grad
     PROBE_STOP(5, l);
     if (l > 0) {
       // BN(+ReLU) backward of layer l-1: dx (grad wrt x[l]) -> g of conv l-1, into the skip plane
-      TRY(pert_bn_bwd(w.dx, K, w.x[l], H, w.out[l - 1], H, w.bn_stats[l - 1], w.bn_stats[l - 1] + H,
-                      params + d->off_bn_g[l - 1], 1, training, dskip, H, grads + d->off_bn_g[l - 1],
-                      grads + d->off_bn_b[l - 1], w.sums, N, H, st));
+      TRY(pert_bn_bwd_ex(w.dx, K, w.x[l], H, w.out[l - 1], H, w.bn_stats[l - 1], w.bn_stats[l - 1] + H,
+                         params + d->off_bn_g[l - 1], 1, relu_scale, training, dskip, H, grads + d->off_bn_g[l - 1],
+                         grads + d->off_bn_b[l - 1], w.sums, N, H, st));
     }
   }
   if (forked) TRY(aux_join(ax, st));

@@ -147,15 +147,44 @@ __global__ void k_bn_eval_stats(const float* __restrict__ rm, const float* __res
   rstd[c] = 1.0f / sqrtf(rv[c] + eps);
 }
 
-// y = (relu)((x - mean) rstd gamma + beta).  acc != null (training): mean / rstd come from the fp64 sums of
-// k_bn_partial (every CTA derives them in its prologue; CTA 0 also stores them for the backward pass and updates the
-// running statistics); acc == null (eval): mean / rstd arrays are read.
+// ---------------------------------------------------------------- dropout mask (Philox4x32-10, Random123)
+// Counter-based: the mask of an element is a pure function of (seed, step, layer, position), so nothing is stored
+// between forward and backward and a replayed CUDA graph draws a new mask whenever the step word in memory moved.
+// Contract (include/pertgnn.h, pert_model_forward): key = (seed lo, seed hi), counter = (float4 group g = row*(H/4) +
+// col/4, layer, step lo, step hi); output word j decides column col + j: kept iff word >= T.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) {
+      k.x += 0x9E3779B9u;
+      k.y += 0xBB67AE85u;
+    }
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+  }
+  return c;
+}
+
+struct BnDropout {
+  const long long* ctr;   // device {seed, step} of this forward
+  unsigned long long T;   // keep iff word >= T; T = 2^32 (p = 1) drops everything
+  float scale;            // 1 / (1 - p), 0 at p = 1
+  int layer;
+};
+
+// y = (relu)((x - mean) rstd gamma + beta) [* keep * scale].  acc != null (training): mean / rstd come from the fp64
+// sums of k_bn_partial (every CTA derives them in its prologue; CTA 0 also stores them for the backward pass and
+// updates the running statistics); acc == null (eval): mean / rstd arrays are read.  DROP (training + ReLU only):
+// inverted dropout of the ReLU output, one Philox call per float4.
+template <bool DROP>
 __global__ void __launch_bounds__(256) k_bn_apply(const float* __restrict__ x, int ld_x, float* __restrict__ mean,
                                                    float* __restrict__ rstd, const float* __restrict__ gamma,
                                                    const float* __restrict__ beta, float* __restrict__ y, int ld_y,
                                                    long long N, int H, int relu, const double* __restrict__ acc,
                                                    float eps, float momentum, float* running_mean,
-                                                   float* running_var, long long* num_batches_tracked) {
+                                                   float* running_var, long long* num_batches_tracked,
+                                                   BnDropout drop) {
   extern __shared__ float s_par[];   // mean | rstd | gamma | beta
   for (int c = threadIdx.x; c < H; c += blockDim.x) {
     float mu, rs;
@@ -189,6 +218,14 @@ __global__ void __launch_bounds__(256) k_bn_apply(const float* __restrict__ x, i
   __syncthreads();
   const int vpr = H >> 2;
   const long long total = N * vpr;
+  uint2 key = make_uint2(0u, 0u);
+  uint32_t step_lo = 0u, step_hi = 0u;
+  if (DROP) {
+    const unsigned long long seed = (unsigned long long)drop.ctr[0], step = (unsigned long long)drop.ctr[1];
+    key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+    step_lo = (uint32_t)step;
+    step_hi = (uint32_t)(step >> 32);
+  }
   for (long long id0 = (long long)blockIdx.x * blockDim.x + threadIdx.x; id0 < total;
        id0 += 4LL * gridDim.x * blockDim.x) {
     float4 v[4];
@@ -209,18 +246,27 @@ __global__ void __launch_bounds__(256) k_bn_apply(const float* __restrict__ x, i
       o.z = fmaf((v[u].z - mu.z) * rs.z, ga.z, be.z);
       o.w = fmaf((v[u].w - mu.w) * rs.w, ga.w, be.w);
       if (relu) o = f4max(o, f4zero());
+      if (DROP) {   // id = row * (H/4) + col/4 is the float4 group g (< 2^32, checked by the host)
+        const uint4 r = philox4x32_10(make_uint4((uint32_t)id, (uint32_t)drop.layer, step_lo, step_hi), key);
+        o.x = r.x >= drop.T ? o.x * drop.scale : 0.f;
+        o.y = r.y >= drop.T ? o.y * drop.scale : 0.f;
+        o.z = r.z >= drop.T ? o.z * drop.scale : 0.f;
+        o.w = r.w >= drop.T ? o.w * drop.scale : 0.f;
+      }
       st4(y + (size_t)(id / vpr) * ld_y + c, o);
     }
   }
 }
 
-// sums[0:H] += sum_n dz,  sums[H:2H] += sum_n dz*xhat   with dz = dy * (y > 0 if relu)
+// sums[0:H] += sum_n dz,  sums[H:2H] += sum_n dz*xhat   with dz = dy * (y > 0 if relu) * scale.
+// With inverted dropout after the ReLU, y > 0 <=> (ReLU active and kept), so the saved output is the whole mask and only
+// the 1/(1-p) factor is applied here (scale = 1 without dropout; __fmul_rn keeps that product exact and uncontracted).
 __global__ void __launch_bounds__(256) k_bn_bwd_reduce(const float* __restrict__ dy, int ld_dy,
                                                         const float* __restrict__ y, int ld_y,
                                                         const float* __restrict__ x, int ld_x,
                                                         const float* __restrict__ mean,
                                                         const float* __restrict__ rstd, long long N, int H, int relu,
-                                                        float* __restrict__ sums) {
+                                                        float scale, float* __restrict__ sums) {
   extern __shared__ float sm[];  // [rl_n][2H]
   const int vpr = H >> 2;
   const int rl_n = blockDim.x / vpr;
@@ -244,8 +290,8 @@ __global__ void __launch_bounds__(256) k_bn_bwd_reduce(const float* __restrict__
       for (int u = 0; u < 4; ++u) {
         float4 g = gg[u];
         const float4 yy = yy4[u], v = vv[u];
-        g.x = yy.x > 0.f ? g.x : 0.f; g.y = yy.y > 0.f ? g.y : 0.f;
-        g.z = yy.z > 0.f ? g.z : 0.f; g.w = yy.w > 0.f ? g.w : 0.f;
+        g.x = yy.x > 0.f ? __fmul_rn(g.x, scale) : 0.f; g.y = yy.y > 0.f ? __fmul_rn(g.y, scale) : 0.f;
+        g.z = yy.z > 0.f ? __fmul_rn(g.z, scale) : 0.f; g.w = yy.w > 0.f ? __fmul_rn(g.w, scale) : 0.f;
         s1 = f4add(s1, g);
         s2.x = fmaf(g.x, (v.x - mu.x) * rs.x, s2.x); s2.y = fmaf(g.y, (v.y - mu.y) * rs.y, s2.y);
         s2.z = fmaf(g.z, (v.z - mu.z) * rs.z, s2.z); s2.w = fmaf(g.w, (v.w - mu.w) * rs.w, s2.w);
@@ -267,7 +313,7 @@ __global__ void k_bn_bwd_apply(const float* __restrict__ dy, int ld_dy, const fl
                                const float* __restrict__ x, int ld_x, const float* __restrict__ mean,
                                const float* __restrict__ rstd, const float* __restrict__ gamma,
                                const float* __restrict__ sums, float* __restrict__ dx, int ld_dx, long long N, int H,
-                               int relu, int training, float* dgamma, float* dbeta) {
+                               int relu, float scale, int training, float* dgamma, float* dbeta) {
   const int vpr = H >> 2;
   long long id = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (blockIdx.x == 0)  // parameter grads accumulate (+=) like autograd
@@ -281,8 +327,8 @@ __global__ void k_bn_bwd_apply(const float* __restrict__ dy, int ld_dy, const fl
   float4 g = ldg4(dy + (size_t)n * ld_dy + c);
   if (relu) {
     float4 yy = ldg4(y + (size_t)n * ld_y + c);
-    g.x = yy.x > 0.f ? g.x : 0.f; g.y = yy.y > 0.f ? g.y : 0.f;
-    g.z = yy.z > 0.f ? g.z : 0.f; g.w = yy.w > 0.f ? g.w : 0.f;
+    g.x = yy.x > 0.f ? __fmul_rn(g.x, scale) : 0.f; g.y = yy.y > 0.f ? __fmul_rn(g.y, scale) : 0.f;
+    g.z = yy.z > 0.f ? __fmul_rn(g.z, scale) : 0.f; g.w = yy.w > 0.f ? __fmul_rn(g.w, scale) : 0.f;
   }
   const float4 rs = ldg4(rstd + c), ga = ldg4(gamma + c);
   float4 o;
@@ -573,20 +619,25 @@ int pert_bn_fwd(const float* x, int ld_x, const float* gamma, const float* beta,
                 int relu, float* mean, float* rstd, float* y, int ld_y, long long N, int H, void* workspace,
                 long long workspace_bytes, void* stream) {
   return pert_bn_fwd_ex(x, ld_x, gamma, beta, running_mean, running_var, num_batches_tracked, eps, momentum, training,
-                        relu, mean, rstd, y, ld_y, N, H, workspace, workspace_bytes, 0, stream);
+                        relu, mean, rstd, y, ld_y, N, H, workspace, workspace_bytes, 0, 0.f, nullptr, 0, stream);
 }
 
 }  // extern "C"
 
 // stats_ready != 0 (training): the fp64 column sums / sums of squares already sit in `workspace` (written by the producer
-// of x, csrc/tconv_tile.cu) -- only the apply pass runs.
+// of x, csrc/tconv_tile.cu) -- only the apply pass runs.  dropout > 0 (training + ReLU): inverted dropout of the output
+// with the mask of layer `drop_layer` at the device {seed, step} `drop_ctr` (see philox4x32_10 for the contract).
 int pert_bn_fwd_ex(const float* x, int ld_x, const float* gamma, const float* beta, float* running_mean,
                    float* running_var, long long* num_batches_tracked, float eps, float momentum, int training,
                    int relu, float* mean, float* rstd, float* y, int ld_y, long long N, int H, void* workspace,
-                   long long workspace_bytes, int stats_ready, void* stream) {
+                   long long workspace_bytes, int stats_ready, float dropout, const long long* drop_ctr,
+                   int drop_layer, void* stream) {
   if (N < 0 || H <= 0 || H % 4 || H > 1024 || ld_x % 4 || ld_y % 4 || !x || !gamma || !beta || !mean || !rstd || !y)
     return PERT_ERR_BADARG;
   if (!al16(x) || !al16(gamma) || !al16(beta) || !al16(mean) || !al16(rstd) || !al16(y)) return PERT_ERR_BADARG;
+  if (!(dropout >= 0.f && dropout <= 1.f)) return PERT_ERR_BADARG;
+  const bool drop = dropout > 0.f && training;
+  if (drop && (!relu || !drop_ctr || N * (H / 4) >= (1LL << 32))) return PERT_ERR_BADARG;
   if (N == 0) return PERT_OK;
   cudaStream_t st = (cudaStream_t)stream;
   double* acc = nullptr;
@@ -614,10 +665,19 @@ int pert_bn_fwd_ex(const float* x, int ld_x, const float* gamma, const float* be
   long long total = N * (H / 4);
   long long blocks = pert_cdiv(total, 256 * 4);
   if (blocks > 8LL * PERT_NUM_SMS) blocks = 8LL * PERT_NUM_SMS;
-  k_bn_apply<<<(int)blocks, 256, (size_t)4 * H * sizeof(float), st>>>(x, ld_x, mean, rstd, gamma, beta, y, ld_y, N, H, relu, acc, eps,
-                                                              momentum, training ? running_mean : nullptr,
-                                                              training ? running_var : nullptr,
-                                                              training ? num_batches_tracked : nullptr);
+  BnDropout dp{nullptr, 0ull, 1.f, 0};
+  if (drop) {
+    dp.ctr = drop_ctr;
+    dp.T = (unsigned long long)floor((double)dropout * 4294967296.0);   // exact: p is a float, 2^32 a power of two
+    dp.scale = dropout >= 1.f ? 0.f : (float)(1.0 / (1.0 - (double)dropout));
+    dp.layer = drop_layer;
+  }
+  auto apply = drop ? k_bn_apply<true> : k_bn_apply<false>;
+  apply<<<(int)blocks, 256, (size_t)4 * H * sizeof(float), st>>>(x, ld_x, mean, rstd, gamma, beta, y, ld_y, N, H, relu,
+                                                                 acc, eps, momentum,
+                                                                 training ? running_mean : nullptr,
+                                                                 training ? running_var : nullptr,
+                                                                 training ? num_batches_tracked : nullptr, dp);
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }
@@ -628,9 +688,21 @@ extern "C" {
 int pert_bn_bwd(const float* dy, int ld_dy, const float* y, int ld_y, const float* x, int ld_x, const float* mean,
                 const float* rstd, const float* gamma, int relu, int training, float* dx, int ld_dx, float* dgamma,
                 float* dbeta, float* sums, long long N, int H, void* stream) {
+  return pert_bn_bwd_ex(dy, ld_dy, y, ld_y, x, ld_x, mean, rstd, gamma, relu, 1.f, training, dx, ld_dx, dgamma, dbeta,
+                        sums, N, H, stream);
+}
+
+}  // extern "C"
+
+// relu_scale: factor applied to the ReLU-masked gradient (1 / (1 - p) after inverted dropout, see k_bn_bwd_reduce);
+// anything but 1 needs relu.
+int pert_bn_bwd_ex(const float* dy, int ld_dy, const float* y, int ld_y, const float* x, int ld_x, const float* mean,
+                   const float* rstd, const float* gamma, int relu, float relu_scale, int training, float* dx,
+                   int ld_dx, float* dgamma, float* dbeta, float* sums, long long N, int H, void* stream) {
   if (N < 0 || H <= 0 || H % 4 || H > 1024 || !dy || !x || !mean || !rstd || !gamma || !dx || !sums)
     return PERT_ERR_BADARG;
   if (relu && !y) return PERT_ERR_BADARG;
+  if (!relu && relu_scale != 1.f) return PERT_ERR_BADARG;
   if (ld_dy % 4 || ld_x % 4 || ld_dx % 4 || (relu && ld_y % 4)) return PERT_ERR_BADARG;
   if (!al16(dy) || !al16(y) || !al16(x) || !al16(mean) || !al16(rstd) || !al16(gamma) || !al16(dx) || !al16(sums))
     return PERT_ERR_BADARG;
@@ -645,13 +717,15 @@ int pert_bn_bwd(const float* dy, int ld_dy, const float* y, int ld_y, const floa
   size_t smem = (size_t)rl_n * 2 * H * sizeof(float);
   if (smem > 48 * 1024) return PERT_ERR_UNSUPPORTED;
   k_bn_bwd_reduce<<<pert_cdiv(N, BN_BWD_ROWS), threads, smem, st>>>(dy, ld_dy, y, ld_y, x, ld_x, mean, rstd, N, H, relu,
-                                                              sums);
+                                                              relu_scale, sums);
   long long total = N * vpr;
   k_bn_bwd_apply<<<pert_cdiv(total, 256), 256, 0, st>>>(dy, ld_dy, y, ld_y, x, ld_x, mean, rstd, gamma, sums, dx,
-                                                       ld_dx, N, H, relu, training, dgamma, dbeta);
+                                                       ld_dx, N, H, relu, relu_scale, training, dgamma, dbeta);
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }
+
+extern "C" {
 
 // local[n] = <x_n, w_local> + b_local (optional);  pool[batch[n]] += x_n * probs[n] / pnn[n]  (pool zeroed here)
 int pert_pool_fwd(const float* x, int ld, const float* probs, const float* pnn, const int64_t* batch,

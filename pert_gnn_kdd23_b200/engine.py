@@ -165,9 +165,10 @@ class Engine:
         return self.ws
 
     def active_relus(self):
-        """{'bn{i}': [N,H] bool, 'head': [B,H] bool}: which ReLUs were active in the LAST forward (read from the saved
-        activations in the workspace).  Test aid: lets a reference be differentiated on the same linear piece."""
-        x, cat_X, entry_id, probs, pnn, batch, index, training, N, E, B = self._saved
+        """{'bn{i}': [N,H] bool, 'head': [B,H] bool}: the entries > 0 of the saved activations of the LAST forward,
+        i.e. which ReLUs were active -- with dropout, active AND kept.  Test aid: lets a reference be differentiated on
+        the same linear piece."""
+        x, cat_X, entry_id, probs, pnn, batch, index, training, N, E, B, p = self._saved
         H = self.desc.H
         out = {}
         for l in range(1, self.n_convs):
@@ -207,8 +208,12 @@ class Engine:
     @_lib.on_device_of
     def forward(self, x, cat_X, entry_id, probs, pnn, batch, index: GraphIndex, training, probe=None,
                 index_ready=None):
-        """-> (global_pred [B,1], local_pred [N,1]); keeps what backward needs in the workspace."""
+        """-> (global_pred [B,1], local_pred [N,1]); keeps what backward needs in the workspace.  In training the
+        BatchNorm outputs are dropped with ``model.dropout`` (mask drawn from ``model.dropout_state()``, whose step
+        this call advances on the device)."""
         N, E, B = x.size(0), index.E, entry_id.numel()
+        p_drop = float(self.model.dropout) if training else 0.0
+        state = self.model.dropout_state() if p_drop > 0 else None
         ws = self._workspace(N, E, B)
         dev = x.device
         x = x.contiguous().float()
@@ -223,18 +228,18 @@ class Engine:
         rc = self.lib.pert_model_forward(
             C.byref(self.desc), p(self.fp.flat), p(self.bn_running), p(self.bn_nbt), p(x), p(cat_X), p(entry_id),
             p(probs), p(pnn), p(batch), N, E, B, p(index.rowptr), p(index.csr_src), p(index.csr_if), p(index.csr_rpc),
-            p(ws), ws.numel() * 4, int(training), p(gpred), p(lpred), p(index.status),
+            p(ws), ws.numel() * 4, int(training), p_drop, p(state), p(gpred), p(lpred), p(index.status),
             C.byref(probe) if probe is not None else None,
             C.c_void_p(index_ready.cuda_event) if index_ready is not None else None, _lib.stream())
         _lib.check(rc, "pert_model_forward")
         ops.LAUNCHES["n"] += self.launches_forward()
-        self._saved = (x, cat_X, entry_id, probs, pnn, batch, index, bool(training), N, E, B)
+        self._saved = (x, cat_X, entry_id, probs, pnn, batch, index, bool(training), N, E, B, p_drop)
         return gpred, lpred
 
     @_lib.on_device_of
     def backward(self, d_global, d_local=None, grads=None, probe=None):
         """Accumulates (+=) parameter gradients into ``grads`` (default: the flat gradient buffer)."""
-        x, cat_X, entry_id, probs, pnn, batch, index, training, N, E, B = self._saved
+        x, cat_X, entry_id, probs, pnn, batch, index, training, N, E, B, p_drop = self._saved
         grads = self.fp.grad if grads is None else grads
         d_global = d_global.reshape(-1).contiguous().float()
         if d_local is not None:
@@ -244,7 +249,7 @@ class Engine:
         rc = self.lib.pert_model_backward(
             C.byref(self.desc), p(self.fp.flat), p(grads), p(cat_X), p(entry_id), p(probs), p(pnn), p(batch), N, E, B,
             p(index.rowptr), p(index.csr_src), p(index.csr_if), p(index.csr_rpc), p(index.colptr), p(index.csc_pos),
-            p(index.csc_dst), p(ws), ws.numel() * 4, int(training), p(d_global), p(d_local),
+            p(index.csc_dst), p(ws), ws.numel() * 4, int(training), p_drop, p(d_global), p(d_local),
             C.byref(probe) if probe is not None else None, _lib.stream())
         _lib.check(rc, "pert_model_backward")
         ops.LAUNCHES["n"] += self.launches_backward()

@@ -68,6 +68,35 @@ class SAGEDeterministic(torch.nn.Module):
         self._engine = Engine(self, flat)
         return self._engine
 
+    def dropout_state(self):
+        """The engine's dropout counter: int64 ``{seed, step}`` in device memory, on this model's device.  Every
+        training forward with ``dropout > 0`` on the engine reads it and adds 1 to ``step`` on the device (a replayed
+        CUDA graph therefore draws a new mask each replay).  Kept in ``__dict__`` -- not a buffer -- so ``state_dict``
+        keeps the reference's keys, and it outlives engine re-creation.  Seeded from torch's default generator on first
+        use, so ``torch.manual_seed`` reproduces the masks; ``seed_dropout`` sets it explicitly."""
+        dev = self.entry_embeds.weight.device
+        st = self.__dict__.get("_dropout_state")
+        if st is None:
+            seed = int(torch.randint(0, 2 ** 63 - 1, (1,), dtype=torch.int64))
+            st = torch.tensor([seed, 0], dtype=torch.int64, device=dev)
+        elif st.device != dev:
+            st = st.to(dev)
+        self.__dict__["_dropout_state"] = st
+        return st
+
+    def seed_dropout(self, seed):
+        """Sets the engine's dropout counter to ``(seed, step = 0)`` (a 64-bit seed; the state is updated in place, so
+        captured CUDA graphs see it).  Data-parallel replicas seeded alike draw alike masks on equally shaped shards, as
+        under DDP with a common seed; give each rank its own seed for independent masks."""
+        s = int(seed) & (2 ** 64 - 1)
+        s = s - 2 ** 64 if s >= 2 ** 63 else s
+        st = self.__dict__.get("_dropout_state")
+        new = torch.tensor([s, 0], dtype=torch.int64)
+        if st is not None and st.device == self.entry_embeds.weight.device:
+            st.copy_(new)
+        else:
+            self.__dict__["_dropout_state"] = new.to(self.entry_embeds.weight.device)
+
     def reset_parameters(self):
         for conv in self.convs:
             conv.reset_parameters()
@@ -82,7 +111,7 @@ class SAGEDeterministic(torch.nn.Module):
             index = cached_index(edge_index, N, edge_attr, self.interface_embeds.num_embeddings,
                                  self.rpctype_embeds.num_embeddings)
         index.num_graphs = entry_id.numel()
-        if self.use_engine and (self.dropout == 0 or not self.training):
+        if self.use_engine:     # dropout (training) runs inside the engine's BatchNorm apply
             from .engine import engine_forward
 
             return engine_forward(self.engine(), x, cat_X, entry_id, pattern_probs, pattern_num_nodes, batch, index,

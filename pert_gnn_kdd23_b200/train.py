@@ -378,7 +378,9 @@ class GraphedTrainStep:
         return loss
 
     def __call__(self, data):
-        key = self._key(data)
+        # the training flag and the dropout rate are by-value arguments of the captured engine calls: a change of
+        # either needs its own graph instead of a replay of the old ones
+        key = self._key(data) + (self.model.training, float(self.model.dropout))
         ent = self._seen.get(key, "unseen")
         if isinstance(ent, dict):
             pass

@@ -48,7 +48,8 @@ extern "C" {
 /* ABI version (major*1000 + minor).  2000: pert_tconv_bwd takes rpc_ws; node_depth / eval-metric entry points.
  * 2001: pert_pert_graph_count / pert_pert_graph_build.  2002: pert_allreduce_adam timing[5], reduce-scatter form.
  * 2003: pert_span_graph_count / pert_span_graph_build.  2004: pert_linear_bwd_planes(_supported).
- * 2005: pert_model_forward takes dropout + dropout_state, pert_model_backward takes dropout. */
+ * 2005: pert_model_forward takes dropout + dropout_state, pert_model_backward takes dropout; later, and additive (no
+ * existing signature changed): pert_bn_linear_fwd_planes(_supported). */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -152,6 +153,26 @@ int pert_linear_bwd_planes(const float* dY, long long plane_stride, const float*
                            float* dW4, int ldw4, float* db4, float* dX, int ldx_out, long long N, int H, int K, int Kd,
                            void* stream);
 int pert_linear_bwd_planes_supported(long long N, int H, int K, int Kd);
+/* Forward of the same node linear in one pass over A (tensor cores, 3xTF32), optionally with the BatchNorm(+ReLU,
+ * +dropout) of the previous conv applied while A is loaded:
+ *   planes: 4 planes [N, H] (row stride H, plane stride plane_stride) = A' . W4^T + b4,  W4 [4H, K] (ldw), b4 [4H];
+ *   bn = 0: A' = A [N, K] (lda);
+ *   bn != 0 (K = H): A' = y = relu(bn(A)) [* keep * scale], with exactly the semantics and arguments of pert_bn_fwd_ex
+ *     (training: batch statistics from `workspace`, computed here unless stats_ready; running statistics and
+ *     num_batches_tracked updated; eval: running statistics; dropout > 0 in training: the mask of layer drop_layer at
+ *     drop_ctr), and y is also written to x_out (ld_x_out), bit-identical to pert_bn_fwd_ex's output.
+ * PERT_ERR_BADARG for NULL pointers, negative sizes, a leading dimension shorter than its row, overlapping planes and
+ * the BatchNorm argument errors of pert_bn_fwd_ex.  PERT_ERR_UNSUPPORTED (nothing launched: use pert_bn_fwd_ex +
+ * pert_gemm_nt) unless H = 64, K in {64, 80} (bn: K = H), N >= 4096, lda == K, ld_x_out == K, 16-byte aligned A,
+ * x_out and plane rows, and the kernel fits on the device; also with PERT_GEMM_TC=0.
+ * pert_bn_linear_fwd_planes_supported: 1 if the shape, the switch and the current device qualify, else 0. */
+int pert_bn_linear_fwd_planes(const float* A, int lda, int bn, const float* gamma, const float* beta,
+                              float* running_mean, float* running_var, long long* num_batches_tracked, float eps,
+                              float momentum, int training, float* mean, float* rstd, float* x_out, int ld_x_out,
+                              void* workspace, long long workspace_bytes, int stats_ready, float dropout,
+                              const long long* drop_ctr, int drop_layer, const float* W4, int ldw, const float* b4,
+                              float* planes, long long plane_stride, long long N, int H, int K, void* stream);
+int pert_bn_linear_fwd_planes_supported(long long N, int H, int K);
 
 /* ---- embeddings / concat (model.py:87-97,108) -------------------------------------------------------
  * fwd: out[n,0:H] (=|+=) table[ids[n*id_stride]];  bwd: dtable[ids[n*id_stride]] += dy[n,0:H]. */

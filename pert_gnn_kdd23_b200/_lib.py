@@ -36,6 +36,9 @@ SIGNATURES = {
     "pert_colsum": (I, [P, I, I, LL, P, LL, I, P]),
     "pert_linear_bwd_planes": (I, [P, LL, P, I, P, I, P, I, P, P, I, LL, I, I, I, P]),
     "pert_linear_bwd_planes_supported": (I, [LL, I, I, I]),
+    "pert_bn_linear_fwd_planes": (I, [P, I, I, P, P, P, P, P, F, F, I, P, P, P, I, P, LL, I, F, P, I, P, I, P, P, LL,
+                                      LL, I, I, P]),
+    "pert_bn_linear_fwd_planes_supported": (I, [LL, I, I]),
     "pert_embedding_fwd": (I, [P, I, P, I, P, I, LL, I, I, P, P]),
     "pert_embedding_bwd": (I, [P, I, P, I, P, I, LL, I, P]),
     "pert_copy_cols": (I, [P, I, P, I, I, LL, P]),

@@ -93,6 +93,9 @@ int pert_bn_fwd_ex(const float* x, int ld_x, const float* gamma, const float* be
                    int relu, float* mean, float* rstd, float* y, int ld_y, long long N, int H, void* workspace,
                    long long workspace_bytes, int stats_ready, float dropout, const long long* drop_ctr,
                    int drop_layer, void* stream);
+int pert_bn_fwd_stats(const float* x, int ld_x, const float* running_mean, const float* running_var, float eps,
+                      int training, float* mean, float* rstd, long long N, int H, void* workspace,
+                      long long workspace_bytes, int stats_ready, cudaStream_t st, double** acc);
 int pert_bn_bwd_ex(const float* dy, int ld_dy, const float* y, int ld_y, const float* x, int ld_x, const float* mean,
                    const float* rstd, const float* gamma, int relu, float relu_scale, int training, float* dx,
                    int ld_dx, float* dgamma, float* dbeta, float* sums, long long N, int H, void* stream);

@@ -665,13 +665,37 @@ int pert_model_forward(const PertModelDesc* d, const float* params, float* bn_ru
   const bool want_tiles = tiles_enabled() && E > 0 && N > 0 && !pert_tile_fixed_ok(N, E, B, H, d->n_rpc);
   if (want_tiles) TRY(pert_tile_list_bounds(batch, N, B, w.tiles, s2));
   if (forked) TRY(aux_join(ax, st));
-  // 3. conv stack
+  // 3. conv stack.  Where the shape qualifies, the node linear of conv l >= 1 applies the BatchNorm(+ReLU, +dropout)
+  // of conv l - 1 while it loads out[l - 1] and writes x[l] on the way (csrc/linear_fwd.cu): one launch and one pass
+  // instead of the apply pass followed by the GEMM.  It reads the BatchNorm sums of conv l - 1 before the memset of
+  // conv l below clears them.
+  const bool bn_in_linear = pert_bn_linear_fwd_planes_supported(N, H, H) == 1;
   PertTiles tiles{};
   bool have_tiles = false;
+  int prev_stats_fused = 0;
   for (int l = 0; l < L; ++l) {
     const int K = k_of(d, l);
     PROBE_START(3, l);
-    TRY(pert_gemm_nt(w.x[l], K, 0, 0, w.w4[l], K, w.b4[l], w.planes[l], H, H, N * (long long)H, N, 4 * H, K, 0, 0, st));
+    if (l > 0 && bn_in_linear) {
+      float* rm = bn_running ? bn_running + (size_t)(l - 1) * 2 * H : nullptr;
+      float* rv = rm ? rm + H : nullptr;
+      TRY(pert_bn_linear_fwd_planes(w.out[l - 1], H, 1, params + d->off_bn_g[l - 1], params + d->off_bn_b[l - 1], rm,
+                                    rv, (training && bn_nbt) ? bn_nbt + l - 1 : nullptr, d->bn_eps, d->bn_momentum,
+                                    training, w.bn_stats[l - 1], w.bn_stats[l - 1] + H, w.x[l], H, w.bn_part,
+                                    pert_bn_workspace_bytes(N, H), prev_stats_fused, drop ? dropout : 0.f, w.drop_ctr,
+                                    l - 1, w.w4[l], K, w.b4[l], w.planes[l], N * (long long)H, N, H, K, st));
+    } else {
+      int frc = l == 0 && pert_bn_linear_fwd_planes_supported(N, H, K)
+                    ? pert_bn_linear_fwd_planes(w.x[0], K, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0.f, 0.f,
+                                                0, nullptr, nullptr, nullptr, 0, nullptr, 0, 0, 0.f, nullptr, 0,
+                                                w.w4[0], K, w.b4[0], w.planes[0], N * (long long)H, N, H, K, st)
+                    : PERT_ERR_UNSUPPORTED;
+      if (frc == PERT_ERR_UNSUPPORTED)
+        TRY(pert_gemm_nt(w.x[l], K, 0, 0, w.w4[l], K, w.b4[l], w.planes[l], H, H, N * (long long)H, N, 4 * H, K, 0, 0,
+                         st));
+      else if (frc != PERT_OK)
+        return frc;
+    }
     PROBE_STOP(3, l);
     float* pl = w.planes[l];
     if (l == 0 && index_ready) {      // the graph index was built on another stream: first use is here
@@ -696,7 +720,8 @@ int pert_model_forward(const PertModelDesc* d, const float* params, float* bn_ru
                              w.t_if[l], w.t_rpc[l], w.out[l], H, w.alpha[l], d->n_rpc, N, E, B, H, bn_acc, &stats_fused,
                              have_tiles ? &tiles : nullptr, st));
     PROBE_STOP(1, l);
-    if (l + 1 < L) {
+    prev_stats_fused = stats_fused;
+    if (l + 1 < L && !bn_in_linear) {
       float* rm = bn_running ? bn_running + (size_t)l * 2 * H : nullptr;
       float* rv = rm ? rm + H : nullptr;
       TRY(pert_bn_fwd_ex(w.out[l], H, params + d->off_bn_g[l], params + d->off_bn_b[l], rm, rv,

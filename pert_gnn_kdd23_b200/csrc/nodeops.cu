@@ -5,6 +5,7 @@
 //   local head + prob-weighted add-pool      model.py:105-107 (local_linear, x*probs/num_nodes, global_add_pool)
 //   pinball loss, Adam                       pert_gnn.py:191-193,245-247
 #include "common.cuh"
+#include "bn.cuh"
 #include <type_traits>
 
 namespace {
@@ -147,32 +148,6 @@ __global__ void k_bn_eval_stats(const float* __restrict__ rm, const float* __res
   rstd[c] = 1.0f / sqrtf(rv[c] + eps);
 }
 
-// ---------------------------------------------------------------- dropout mask (Philox4x32-10, Random123)
-// Counter-based: the mask of an element is a pure function of (seed, step, layer, position), so nothing is stored
-// between forward and backward and a replayed CUDA graph draws a new mask whenever the step word in memory moved.
-// Contract (include/pertgnn.h, pert_model_forward): key = (seed lo, seed hi), counter = (float4 group g = row*(H/4) +
-// col/4, layer, step lo, step hi); output word j decides column col + j: kept iff word >= T.
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    if (r) {
-      k.x += 0x9E3779B9u;
-      k.y += 0xBB67AE85u;
-    }
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-  }
-  return c;
-}
-
-struct BnDropout {
-  const long long* ctr;   // device {seed, step} of this forward
-  unsigned long long T;   // keep iff word >= T; T = 2^32 (p = 1) drops everything
-  float scale;            // 1 / (1 - p), 0 at p = 1
-  int layer;
-};
-
 // y = (relu)((x - mean) rstd gamma + beta) [* keep * scale].  acc != null (training): mean / rstd come from the fp64
 // sums of k_bn_partial (every CTA derives them in its prologue; CTA 0 also stores them for the backward pass and
 // updates the running statistics); acc == null (eval): mean / rstd arrays are read.  DROP (training + ReLU only):
@@ -189,23 +164,8 @@ __global__ void __launch_bounds__(256) k_bn_apply(const float* __restrict__ x, i
   for (int c = threadIdx.x; c < H; c += blockDim.x) {
     float mu, rs;
     if (acc) {
-      const double n = (double)N;
-      const double m = acc[c] / n;
-      double m2 = acc[H + c] - n * m * m;
-      if (m2 < 0.0) m2 = 0.0;
-      const double var = m2 / n;       // biased, used to normalise
-      mu = (float)m;
-      rs = (float)(1.0 / sqrt(var + (double)eps));
-      if (blockIdx.x == 0) {
-        mean[c] = mu;
-        rstd[c] = rs;
-        if (running_mean) {
-          const double unbiased = (N > 1) ? m2 / (n - 1.0) : var;
-          running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * mu;
-          running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)unbiased;
-        }
-        if (c == 0 && num_batches_tracked) *num_batches_tracked += 1;
-      }
+      bn_batch_stats(acc, N, H, c, eps, momentum, blockIdx.x == 0, mean, rstd, running_mean, running_var,
+                     num_batches_tracked, mu, rs);
     } else {
       mu = mean[c];
       rs = rstd[c];
@@ -218,14 +178,7 @@ __global__ void __launch_bounds__(256) k_bn_apply(const float* __restrict__ x, i
   __syncthreads();
   const int vpr = H >> 2;
   const long long total = N * vpr;
-  uint2 key = make_uint2(0u, 0u);
-  uint32_t step_lo = 0u, step_hi = 0u;
-  if (DROP) {
-    const unsigned long long seed = (unsigned long long)drop.ctr[0], step = (unsigned long long)drop.ctr[1];
-    key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
-    step_lo = (uint32_t)step;
-    step_hi = (uint32_t)(step >> 32);
-  }
+  const BnDropKey key = DROP ? bn_drop_key(drop) : BnDropKey{};
   for (long long id0 = (long long)blockIdx.x * blockDim.x + threadIdx.x; id0 < total;
        id0 += 4LL * gridDim.x * blockDim.x) {
     float4 v[4];
@@ -240,19 +193,8 @@ __global__ void __launch_bounds__(256) k_bn_apply(const float* __restrict__ x, i
       if (id >= total) break;
       const int c = (int)(id % vpr) * 4;
       const float4 mu = ld4(s_par + c), rs = ld4(s_par + H + c), ga = ld4(s_par + 2 * H + c), be = ld4(s_par + 3 * H + c);
-      float4 o;
-      o.x = fmaf((v[u].x - mu.x) * rs.x, ga.x, be.x);
-      o.y = fmaf((v[u].y - mu.y) * rs.y, ga.y, be.y);
-      o.z = fmaf((v[u].z - mu.z) * rs.z, ga.z, be.z);
-      o.w = fmaf((v[u].w - mu.w) * rs.w, ga.w, be.w);
-      if (relu) o = f4max(o, f4zero());
-      if (DROP) {   // id = row * (H/4) + col/4 is the float4 group g (< 2^32, checked by the host)
-        const uint4 r = philox4x32_10(make_uint4((uint32_t)id, (uint32_t)drop.layer, step_lo, step_hi), key);
-        o.x = r.x >= drop.T ? o.x * drop.scale : 0.f;
-        o.y = r.y >= drop.T ? o.y * drop.scale : 0.f;
-        o.z = r.z >= drop.T ? o.z * drop.scale : 0.f;
-        o.w = r.w >= drop.T ? o.w * drop.scale : 0.f;
-      }
+      float4 o = bn_affine4(v[u], mu, rs, ga, be, relu);
+      if (DROP) o = bn_dropout4(o, (uint32_t)id, drop, key);   // id = row * (H/4) + col/4 is the float4 group
       st4(y + (size_t)(id / vpr) * ld_y + c, o);
     }
   }
@@ -624,6 +566,38 @@ int pert_bn_fwd(const float* x, int ld_x, const float* gamma, const float* beta,
 
 }  // extern "C"
 
+// The statistics half of a BatchNorm forward, shared by pert_bn_fwd_ex and the node-linear forward that applies
+// BatchNorm to its input (csrc/linear_fwd.cu).  Training: *acc = the fp64 column sums / sums of squares in `workspace`
+// (computed here by k_bn_partial unless stats_ready, i.e. the producer of x already left them there); the apply derives
+// mean / rstd from them.  Eval: mean / rstd = the running statistics (k_bn_eval_stats), *acc = NULL.
+int pert_bn_fwd_stats(const float* x, int ld_x, const float* running_mean, const float* running_var, float eps,
+                      int training, float* mean, float* rstd, long long N, int H, void* workspace,
+                      long long workspace_bytes, int stats_ready, cudaStream_t st, double** acc) {
+  *acc = nullptr;
+  if (training) {
+    if (!workspace || workspace_bytes < pert_bn_workspace_bytes(N, H)) return PERT_ERR_BADARG;
+    int chunks = pert_cdiv(N, BN_ROWS);
+    int vpr = H / 4;
+    int threads = 256;
+    if (threads < H) threads = (H + 31) / 32 * 32;
+    int rl_n = threads / vpr;
+    if (rl_n < 1) return PERT_ERR_UNSUPPORTED;
+    size_t smem = ((size_t)rl_n * H + H) * sizeof(float);
+    if (smem > 48 * 1024) return PERT_ERR_UNSUPPORTED;
+    if ((uintptr_t)workspace & 7) return PERT_ERR_BADARG;
+    *acc = (double*)workspace;
+    if (!stats_ready) {
+      cudaError_t e = cudaMemsetAsync(*acc, 0, (size_t)2 * H * sizeof(double), st);
+      if (e != cudaSuccess) return (int)e;
+      k_bn_partial<<<chunks, threads, smem, st>>>(x, ld_x, N, H, *acc);
+    }
+  } else {
+    if (!running_mean || !running_var) return PERT_ERR_BADARG;
+    k_bn_eval_stats<<<pert_cdiv(H, 128), 128, 0, st>>>(running_mean, running_var, eps, H, mean, rstd);
+  }
+  return PERT_OK;
+}
+
 // stats_ready != 0 (training): the fp64 column sums / sums of squares already sit in `workspace` (written by the producer
 // of x, csrc/tconv_tile.cu) -- only the apply pass runs.  dropout > 0 (training + ReLU): inverted dropout of the output
 // with the mask of layer `drop_layer` at the device {seed, step} `drop_ctr` (see philox4x32_10 for the contract).
@@ -641,37 +615,13 @@ int pert_bn_fwd_ex(const float* x, int ld_x, const float* gamma, const float* be
   if (N == 0) return PERT_OK;
   cudaStream_t st = (cudaStream_t)stream;
   double* acc = nullptr;
-  if (training) {
-    if (!workspace || workspace_bytes < pert_bn_workspace_bytes(N, H)) return PERT_ERR_BADARG;
-    int chunks = pert_cdiv(N, BN_ROWS);
-    int vpr = H / 4;
-    int threads = 256;
-    if (threads < H) threads = (H + 31) / 32 * 32;
-    int rl_n = threads / vpr;
-    if (rl_n < 1) return PERT_ERR_UNSUPPORTED;
-    size_t smem = ((size_t)rl_n * H + H) * sizeof(float);
-    if (smem > 48 * 1024) return PERT_ERR_UNSUPPORTED;
-    if ((uintptr_t)workspace & 7) return PERT_ERR_BADARG;
-    acc = (double*)workspace;
-    if (!stats_ready) {
-      cudaError_t e = cudaMemsetAsync(acc, 0, (size_t)2 * H * sizeof(double), st);
-      if (e != cudaSuccess) return (int)e;
-      k_bn_partial<<<chunks, threads, smem, st>>>(x, ld_x, N, H, acc);
-    }
-  } else {
-    if (!running_mean || !running_var) return PERT_ERR_BADARG;
-    k_bn_eval_stats<<<pert_cdiv(H, 128), 128, 0, st>>>(running_mean, running_var, eps, H, mean, rstd);
-  }
+  int rc = pert_bn_fwd_stats(x, ld_x, running_mean, running_var, eps, training, mean, rstd, N, H, workspace,
+                             workspace_bytes, stats_ready, st, &acc);
+  if (rc != PERT_OK) return rc;
   long long total = N * (H / 4);
   long long blocks = pert_cdiv(total, 256 * 4);
   if (blocks > 8LL * PERT_NUM_SMS) blocks = 8LL * PERT_NUM_SMS;
-  BnDropout dp{nullptr, 0ull, 1.f, 0};
-  if (drop) {
-    dp.ctr = drop_ctr;
-    dp.T = (unsigned long long)floor((double)dropout * 4294967296.0);   // exact: p is a float, 2^32 a power of two
-    dp.scale = dropout >= 1.f ? 0.f : (float)(1.0 / (1.0 - (double)dropout));
-    dp.layer = drop_layer;
-  }
+  const BnDropout dp = drop ? bn_dropout_params(dropout, drop_ctr, drop_layer) : BnDropout{nullptr, 0ull, 1.f, 0};
   auto apply = drop ? k_bn_apply<true> : k_bn_apply<false>;
   apply<<<(int)blocks, 256, (size_t)4 * H * sizeof(float), st>>>(x, ld_x, mean, rstd, gamma, beta, y, ld_y, N, H, relu,
                                                                  acc, eps, momentum,

@@ -192,9 +192,11 @@ class Engine:
     def launches_forward(self):
         """Kernels pert_model_forward launches (memsets not counted): pack, edge tables (6 layers per launch),
         embeddings + copy, per conv GEMM + attention (whose epilogue also produces the BatchNorm statistics), per
-        BatchNorm one apply kernel, pool, head."""
-        L = self.n_convs
-        return self._pack_launches() + (L + 5) // 6 + self.desc.n_cat + 1 + 2 * L + (L - 1) + 1 + 1
+        BatchNorm one apply kernel unless pert_bn_linear_fwd_planes takes the shape (the next conv's GEMM then applies
+        it), pool, head."""
+        L, H, N = self.n_convs, self.desc.H, self._saved[8]
+        applies = 0 if self.lib.pert_bn_linear_fwd_planes_supported(N, H, H) else L - 1
+        return self._pack_launches() + (L + 5) // 6 + self.desc.n_cat + 1 + 2 * L + applies + 1 + 1
 
     def launches_backward(self):
         """head, pool, per conv (target pass, source pass, node-linear backward: one fused launch where
@@ -232,8 +234,8 @@ class Engine:
             C.byref(probe) if probe is not None else None,
             C.c_void_p(index_ready.cuda_event) if index_ready is not None else None, _lib.stream())
         _lib.check(rc, "pert_model_forward")
-        ops.LAUNCHES["n"] += self.launches_forward()
         self._saved = (x, cat_X, entry_id, probs, pnn, batch, index, bool(training), N, E, B, p_drop)
+        ops.LAUNCHES["n"] += self.launches_forward()
         return gpred, lpred
 
     @_lib.on_device_of

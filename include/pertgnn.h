@@ -49,7 +49,8 @@ extern "C" {
  * 2001: pert_pert_graph_count / pert_pert_graph_build.  2002: pert_allreduce_adam timing[5], reduce-scatter form.
  * 2003: pert_span_graph_count / pert_span_graph_build.  2004: pert_linear_bwd_planes(_supported).
  * 2005: pert_model_forward takes dropout + dropout_state, pert_model_backward takes dropout; later, and additive (no
- * existing signature changed): pert_bn_linear_fwd_planes(_supported). */
+ * existing signature changed): pert_bn_linear_fwd_planes(_supported); pert_batch_pad, pert_model_forward_live,
+ * pert_model_backward_live, pert_pinball_loss_live, pert_eval_metrics_live. */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -218,6 +219,13 @@ int pert_pinball_loss(const int64_t* y, const float* yhat, float tau, long long 
  * acc[2] += B * pinball_tau(y, yhat)  (= sum of the per-graph pinball terms).  acc: 3 doubles on the device, zeroed by
  * the caller at the start of an epoch and read back once at its end. */
 int pert_eval_metrics(const int64_t* y, const float* yhat, float tau, long long B, double* acc, void* stream);
+/* The same two on a batch padded by pert_batch_pad: y / yhat hold B (capacity) graphs, the device word live = {N, B_real}
+ * says how many are real.  The loss is the mean over the real graphs and dyhat = 0 for the ghost graphs; the metrics sum
+ * over the real graphs only.  live = NULL is exactly pert_pinball_loss / pert_eval_metrics. */
+int pert_pinball_loss_live(const int64_t* y, const float* yhat, float tau, long long B, float grad_scale, float* loss,
+                           float* dyhat, const long long* live, void* stream);
+int pert_eval_metrics_live(const int64_t* y, const float* yhat, float tau, long long B, double* acc,
+                           const long long* live, void* stream);
 
 /* torch.optim.Adam step (pert_gnn.py:343,247) over one flat parameter buffer; g is scaled by grad_scale. */
 int pert_adam_step(float* p, const float* g, float* m, float* v, long long n, float lr, float beta1, float beta2,
@@ -330,6 +338,49 @@ int pert_model_backward(const PertModelDesc* desc, const float* params, float* g
                         const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
                         const int* csc_dst, void* workspace, long long workspace_bytes, int training, float dropout,
                         const float* d_global, const float* d_local, const PertProbe* probe, void* stream);
+
+/* ---- capacity buckets: padded batches for CUDA-graph replay (csrc/pad.cu) ------------------------------------------
+ * pert_batch_pad copies a batch of N nodes, E edges and B graphs bit for bit into caller buffers of the capacity sizes
+ * (N_cap, E_cap, B_cap) -- x [N,F] fp32, cat_X [N,n_cat], edge_index [2,E], edge_attr [E,attr_cols], batch [N],
+ * entry_id [B], y [B] int64, rt_probs [N], pattern_num_nodes [N] fp32 -- fills the tail with ghost graphs and stores
+ * live = {N, B} (two int64 on the device).  Ghost node j = N + j' belongs to graph B + min(j', B_cap - B - 1) (the batch
+ * vector stays sorted, every ghost graph owns a node); ghost edge E + k' is a self-loop on ghost node
+ * N + k' mod (N_cap - N); x = 0, every id = 0, rt_probs = 0, pattern_num_nodes = 1, y = 1.  No edge joins a ghost to
+ * a real node and ghost graphs pool nothing, so a step on the padded batch that reads `live` where a count enters the
+ * arithmetic (pert_model_forward_live / backward_live, pert_pinball_loss_live, pert_eval_metrics_live) computes what
+ * the unpadded step computes for the real graphs.  One grid-stride launch; its source pointers change with every
+ * batch, so it runs eagerly in front of a replayed graph.
+ * PERT_ERR_BADARG, before any CUDA call, for NULL pointers, negative sizes, B < 1, F / n_cat / attr_cols < 1, a
+ * capacity below the real size, N_cap - N < max(1, B_cap - B), E_cap - E > PERT_PAD_MAX_GHOST_DEGREE * (N_cap - N)
+ * (a ghost in-degree above 4) or a capacity above 2^31 - 1. */
+#define PERT_PAD_MAX_GHOST_DEGREE 4
+int pert_batch_pad(const float* x, const int64_t* cat_X, const int64_t* edge_index, const int64_t* edge_attr,
+                   const int64_t* batch, const int64_t* entry_id, const int64_t* y, const float* rt_probs,
+                   const float* pattern_num_nodes, long long N, long long E, long long B, int F, int n_cat,
+                   int attr_cols, float* x_cap, int64_t* cat_X_cap, int64_t* edge_index_cap, int64_t* edge_attr_cap,
+                   int64_t* batch_cap, int64_t* entry_id_cap, int64_t* y_cap, float* rt_probs_cap,
+                   float* pattern_num_nodes_cap, long long N_cap, long long E_cap, long long B_cap, long long* live,
+                   void* stream);
+/* pert_model_forward / pert_model_backward on a padded batch: N, E, B and every array are those of the capacity
+ * buffers, live the word pert_batch_pad wrote.  In training the BatchNorm statistics (mean, variance, the running
+ * statistics with the unbiased factor of the real N) count the real rows only, and the BatchNorm backward divides by
+ * the real N and gives the ghost rows a zero gradient.  The backward's d_global must be 0 for the ghost graphs
+ * (pert_pinball_loss_live).  The dropout mask of a real row does not depend on the padding.  live = NULL is exactly
+ * pert_model_forward / pert_model_backward. */
+int pert_model_forward_live(const PertModelDesc* desc, const float* params, float* bn_running, long long* bn_nbt,
+                            const float* x, const int64_t* cat_X, const int64_t* entry_id, const float* probs,
+                            const float* pnn, const int64_t* batch, long long N, long long E, long long B,
+                            const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc,
+                            void* workspace, long long workspace_bytes, int training, float dropout,
+                            long long* dropout_state, float* global_pred, float* local_pred, int* status,
+                            const PertProbe* probe, void* index_ready, const long long* live, void* stream);
+int pert_model_backward_live(const PertModelDesc* desc, const float* params, float* grads, const int64_t* cat_X,
+                             const int64_t* entry_id, const float* probs, const float* pnn, const int64_t* batch,
+                             long long N, long long E, long long B, const int* rowptr, const int* csr_src,
+                             const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
+                             const int* csc_dst, void* workspace, long long workspace_bytes, int training,
+                             float dropout, const float* d_global, const float* d_local, const PertProbe* probe,
+                             const long long* live, void* stream);
 
 /* ---- device-side batch assembly from a resident pattern store (csrc/store.cu) ---------------------------------------
  * Replaces the host-side sample assembly + collation + per-step probability expansion of the reference:

@@ -50,6 +50,8 @@ SIGNATURES = {
     "pert_relu_bwd": (I, [P, P, LL, P]),
     "pert_pinball_loss": (I, [P, P, F, LL, F, P, P, P]),
     "pert_eval_metrics": (I, [P, P, F, LL, P, P]),
+    "pert_pinball_loss_live": (I, [P, P, F, LL, F, P, P, P, P]),
+    "pert_eval_metrics_live": (I, [P, P, F, LL, P, P, P]),
     "pert_adam_step": (I, [P, P, P, P, LL, F, F, F, F, F, LL, F, P]),
     # fused all-reduce + Adam over peer memory (csrc/peer.cu)
     "pert_peer_exchange_bytes": (LL, [LL]),
@@ -72,6 +74,13 @@ SIGNATURES = {
     "pert_model_forward": (I, [P, P, P, P, P, P, P, P, P, P, LL, LL, LL, P, P, P, P, P, LL, I, F, P, P, P, P, P, P,
                                P]),
     "pert_model_backward": (I, [P, P, P, P, P, P, P, P, LL, LL, LL, P, P, P, P, P, P, P, P, LL, I, F, P, P, P, P]),
+    # padded batches for per-bucket graph replay (csrc/pad.cu; the *_live entries read the {N, B} word it writes)
+    "pert_model_forward_live": (I, [P, P, P, P, P, P, P, P, P, P, LL, LL, LL, P, P, P, P, P, LL, I, F, P, P, P, P, P,
+                                    P, P, P]),
+    "pert_model_backward_live": (I, [P, P, P, P, P, P, P, P, LL, LL, LL, P, P, P, P, P, P, P, P, LL, I, F, P, P, P,
+                                     P, P]),
+    "pert_batch_pad": (I, [P, P, P, P, P, P, P, P, P, LL, LL, LL, I, I, I, P, P, P, P, P, P, P, P, P, LL, LL, LL, P,
+                           P]),
 }
 
 _lib = None

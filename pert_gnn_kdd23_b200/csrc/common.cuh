@@ -78,10 +78,12 @@ int pert_tile_list_view(long long N, long long E, long long B, int H, int n_rpc,
 int pert_tile_list_bounds(const int64_t* batch, long long N, long long B, int* tiles_mem, cudaStream_t st);
 int pert_tile_list_build(int has_batch, long long N, long long E, long long B, const int* rowptr, int H, int n_rpc,
                          int* tiles_mem, PertTiles* out, cudaStream_t st);
+// live: optional device {N, B} of a padded batch (pert_batch_pad); the BatchNorm sums then count the rows below live[0]
 int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                          const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if,
                          const float* t_rpc, float* out, int ld_out, float* alpha, int n_rpc, long long N, long long E,
-                         long long B_hint, int H, double* bn_acc, int* fused, const PertTiles* tiles, void* stream);
+                         long long B_hint, int H, double* bn_acc, const long long* live, int* fused,
+                         const PertTiles* tiles, void* stream);
 int pert_tconv_bwd_tiles(const float* g, int ld_g, const float* q, const float* k, const float* v, int ld,
                          const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc,
                          const int* colptr, const int* csc_pos, const int* csc_dst, const float* t_if,
@@ -92,10 +94,20 @@ int pert_bn_fwd_ex(const float* x, int ld_x, const float* gamma, const float* be
                    float* running_var, long long* num_batches_tracked, float eps, float momentum, int training,
                    int relu, float* mean, float* rstd, float* y, int ld_y, long long N, int H, void* workspace,
                    long long workspace_bytes, int stats_ready, float dropout, const long long* drop_ctr,
-                   int drop_layer, void* stream);
+                   int drop_layer, const long long* live, void* stream);
 int pert_bn_fwd_stats(const float* x, int ld_x, const float* running_mean, const float* running_var, float eps,
                       int training, float* mean, float* rstd, long long N, int H, void* workspace,
-                      long long workspace_bytes, int stats_ready, cudaStream_t st, double** acc);
+                      long long workspace_bytes, int stats_ready, const long long* live, cudaStream_t st,
+                      double** acc);
 int pert_bn_bwd_ex(const float* dy, int ld_dy, const float* y, int ld_y, const float* x, int ld_x, const float* mean,
                    const float* rstd, const float* gamma, int relu, float relu_scale, int training, float* dx,
-                   int ld_dx, float* dgamma, float* dbeta, float* sums, long long N, int H, void* stream);
+                   int ld_dx, float* dgamma, float* dbeta, float* sums, long long N, int H, const long long* live,
+                   void* stream);
+// pert_bn_linear_fwd_planes with the live word of a padded batch (BatchNorm statistics over the rows below live[0])
+int pert_bn_linear_fwd_planes_ex(const float* A, int lda, int bn, const float* gamma, const float* beta,
+                                 float* running_mean, float* running_var, long long* num_batches_tracked, float eps,
+                                 float momentum, int training, float* mean, float* rstd, float* x_out, int ld_x_out,
+                                 void* workspace, long long workspace_bytes, int stats_ready, float dropout,
+                                 const long long* drop_ctr, int drop_layer, const long long* live, const float* W4,
+                                 int ldw, const float* b4, float* planes, long long plane_stride, long long N, int H,
+                                 int K, void* stream);

@@ -612,6 +612,20 @@ int pert_model_forward(const PertModelDesc* d, const float* params, float* bn_ru
                        long long workspace_bytes, int training, float dropout, long long* dropout_state,
                        float* global_pred, float* local_pred, int* status, const PertProbe* probe, void* index_ready,
                        void* stream) {
+  return pert_model_forward_live(d, params, bn_running, bn_nbt, x, cat_X, entry_id, probs, pnn, batch, N, E, B, rowptr,
+                                 csr_src, csr_if, csr_rpc, workspace, workspace_bytes, training, dropout,
+                                 dropout_state, global_pred, local_pred, status, probe, index_ready, nullptr, stream);
+}
+
+// live: see include/pertgnn.h.  Every kernel runs at the capacity sizes N, E, B; only the BatchNorm statistics (the
+// fused conv epilogue, k_bn_partial and the apply prologues) read the real node count from the device word.
+int pert_model_forward_live(const PertModelDesc* d, const float* params, float* bn_running, long long* bn_nbt,
+                            const float* x, const int64_t* cat_X, const int64_t* entry_id, const float* probs,
+                            const float* pnn, const int64_t* batch, long long N, long long E, long long B,
+                            const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc,
+                            void* workspace, long long workspace_bytes, int training, float dropout,
+                            long long* dropout_state, float* global_pred, float* local_pred, int* status,
+                            const PertProbe* probe, void* index_ready, const long long* live, void* stream) {
   TRY(check_desc(d));
   TRY(check_dropout(d, N, training, dropout, dropout_state));
   std::lock_guard<std::mutex> issue_lock(engine_mutex());
@@ -679,11 +693,12 @@ int pert_model_forward(const PertModelDesc* d, const float* params, float* bn_ru
     if (l > 0 && bn_in_linear) {
       float* rm = bn_running ? bn_running + (size_t)(l - 1) * 2 * H : nullptr;
       float* rv = rm ? rm + H : nullptr;
-      TRY(pert_bn_linear_fwd_planes(w.out[l - 1], H, 1, params + d->off_bn_g[l - 1], params + d->off_bn_b[l - 1], rm,
-                                    rv, (training && bn_nbt) ? bn_nbt + l - 1 : nullptr, d->bn_eps, d->bn_momentum,
-                                    training, w.bn_stats[l - 1], w.bn_stats[l - 1] + H, w.x[l], H, w.bn_part,
-                                    pert_bn_workspace_bytes(N, H), prev_stats_fused, drop ? dropout : 0.f, w.drop_ctr,
-                                    l - 1, w.w4[l], K, w.b4[l], w.planes[l], N * (long long)H, N, H, K, st));
+      TRY(pert_bn_linear_fwd_planes_ex(w.out[l - 1], H, 1, params + d->off_bn_g[l - 1], params + d->off_bn_b[l - 1],
+                                       rm, rv, (training && bn_nbt) ? bn_nbt + l - 1 : nullptr, d->bn_eps,
+                                       d->bn_momentum, training, w.bn_stats[l - 1], w.bn_stats[l - 1] + H, w.x[l], H,
+                                       w.bn_part, pert_bn_workspace_bytes(N, H), prev_stats_fused,
+                                       drop ? dropout : 0.f, w.drop_ctr, l - 1, live, w.w4[l], K, w.b4[l],
+                                       w.planes[l], N * (long long)H, N, H, K, st));
     } else {
       int frc = l == 0 && pert_bn_linear_fwd_planes_supported(N, H, K)
                     ? pert_bn_linear_fwd_planes(w.x[0], K, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0.f, 0.f,
@@ -717,8 +732,8 @@ int pert_model_forward(const PertModelDesc* d, const float* params, float* bn_ru
     }
     PROBE_START(1, l);
     TRY(pert_tconv_fwd_stats(pl, pl + N * H, pl + 2 * N * H, pl + 3 * N * H, H, rowptr, csr_src, csr_if, csr_rpc,
-                             w.t_if[l], w.t_rpc[l], w.out[l], H, w.alpha[l], d->n_rpc, N, E, B, H, bn_acc, &stats_fused,
-                             have_tiles ? &tiles : nullptr, st));
+                             w.t_if[l], w.t_rpc[l], w.out[l], H, w.alpha[l], d->n_rpc, N, E, B, H, bn_acc, live,
+                             &stats_fused, have_tiles ? &tiles : nullptr, st));
     PROBE_STOP(1, l);
     prev_stats_fused = stats_fused;
     if (l + 1 < L && !bn_in_linear) {
@@ -727,7 +742,7 @@ int pert_model_forward(const PertModelDesc* d, const float* params, float* bn_ru
       TRY(pert_bn_fwd_ex(w.out[l], H, params + d->off_bn_g[l], params + d->off_bn_b[l], rm, rv,
                          (training && bn_nbt) ? bn_nbt + l : nullptr, d->bn_eps, d->bn_momentum, training, 1,
                          w.bn_stats[l], w.bn_stats[l] + H, w.x[l + 1], H, N, H, w.bn_part,
-                         pert_bn_workspace_bytes(N, H), stats_fused, drop ? dropout : 0.f, w.drop_ctr, l, st));
+                         pert_bn_workspace_bytes(N, H), stats_fused, drop ? dropout : 0.f, w.drop_ctr, l, live, st));
     }
   }
   // 4. local head + weighted add-pool, global head
@@ -754,6 +769,20 @@ int pert_model_backward(const PertModelDesc* d, const float* params, float* grad
                         const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
                         const int* csc_dst, void* workspace, long long workspace_bytes, int training, float dropout,
                         const float* d_global, const float* d_local, const PertProbe* probe, void* stream) {
+  return pert_model_backward_live(d, params, grads, cat_X, entry_id, probs, pnn, batch, N, E, B, rowptr, csr_src,
+                                  csr_if, csr_rpc, colptr, csc_pos, csc_dst, workspace, workspace_bytes, training,
+                                  dropout, d_global, d_local, probe, nullptr, stream);
+}
+
+// live: the same word as the forward's.  The BatchNorm backward divides by live[0] and gives the ghost rows dx = 0;
+// every other gradient of a ghost row or graph is 0 already (d_global of a ghost graph must be 0).
+int pert_model_backward_live(const PertModelDesc* d, const float* params, float* grads, const int64_t* cat_X,
+                             const int64_t* entry_id, const float* probs, const float* pnn, const int64_t* batch,
+                             long long N, long long E, long long B, const int* rowptr, const int* csr_src,
+                             const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
+                             const int* csc_dst, void* workspace, long long workspace_bytes, int training,
+                             float dropout, const float* d_global, const float* d_local, const PertProbe* probe,
+                             const long long* live, void* stream) {
   TRY(check_desc(d));
   if (!(dropout >= 0.f && dropout <= 1.f)) return PERT_ERR_BADARG;
   // the saved activations already carry the mask (see k_bn_bwd_reduce): only the 1 / (1 - p) factor is needed
@@ -847,7 +876,7 @@ int pert_model_backward(const PertModelDesc* d, const float* params, float* grad
       // BN(+ReLU) backward of layer l-1: dx (grad wrt x[l]) -> g of conv l-1, into the skip plane
       TRY(pert_bn_bwd_ex(w.dx, K, w.x[l], H, w.out[l - 1], H, w.bn_stats[l - 1], w.bn_stats[l - 1] + H,
                          params + d->off_bn_g[l - 1], 1, relu_scale, training, dskip, H, grads + d->off_bn_g[l - 1],
-                         grads + d->off_bn_b[l - 1], w.sums, N, H, st));
+                         grads + d->off_bn_b[l - 1], w.sums, N, H, live, st));
     }
   }
   if (forked) TRY(aux_join(ax, st));

@@ -69,6 +69,7 @@ struct LfArgs {
   float *running_mean, *running_var;
   long long* num_batches_tracked;
   BnDropout drop;
+  const long long* live;   // training on a padded batch: {N, B} of the real part (statistics over live[0] rows)
   int N;
 };
 
@@ -121,7 +122,8 @@ __global__ void __launch_bounds__(LF_THREADS, 1) k_bn_linear_fwd_planes(LfArgs g
     for (int c = tid; c < LF_H; c += LF_THREADS) {
       float mu, rs;
       if (g.acc) {
-        bn_batch_stats(g.acc, g.N, LF_H, c, g.eps, g.momentum, blockIdx.x == 0, g.mean, g.rstd, g.running_mean,
+        const long long n_stat = g.live ? g.live[0] : g.N;   // read here only, never in the tile loop
+        bn_batch_stats(g.acc, n_stat, LF_H, c, g.eps, g.momentum, blockIdx.x == 0, g.mean, g.rstd, g.running_mean,
                        g.running_var, g.num_batches_tracked, mu, rs);
       } else {
         mu = g.mean[c];
@@ -268,6 +270,21 @@ int pert_bn_linear_fwd_planes(const float* A, int lda, int bn, const float* gamm
                               void* workspace, long long workspace_bytes, int stats_ready, float dropout,
                               const long long* drop_ctr, int drop_layer, const float* W4, int ldw, const float* b4,
                               float* planes, long long plane_stride, long long N, int H, int K, void* stream) {
+  return pert_bn_linear_fwd_planes_ex(A, lda, bn, gamma, beta, running_mean, running_var, num_batches_tracked, eps,
+                                      momentum, training, mean, rstd, x_out, ld_x_out, workspace, workspace_bytes,
+                                      stats_ready, dropout, drop_ctr, drop_layer, nullptr, W4, ldw, b4, planes,
+                                      plane_stride, N, H, K, stream);
+}
+
+}  // extern "C"
+
+int pert_bn_linear_fwd_planes_ex(const float* A, int lda, int bn, const float* gamma, const float* beta,
+                                 float* running_mean, float* running_var, long long* num_batches_tracked, float eps,
+                                 float momentum, int training, float* mean, float* rstd, float* x_out, int ld_x_out,
+                                 void* workspace, long long workspace_bytes, int stats_ready, float dropout,
+                                 const long long* drop_ctr, int drop_layer, const long long* live, const float* W4,
+                                 int ldw, const float* b4, float* planes, long long plane_stride, long long N, int H,
+                                 int K, void* stream) {
   if (!A || !W4 || !b4 || !planes || N < 0 || H <= 0 || K <= 0 || lda < K || ldw < K || plane_stride < N * H)
     return PERT_ERR_BADARG;
   const bool drop = bn && training && dropout > 0.f;
@@ -299,7 +316,7 @@ int pert_bn_linear_fwd_planes(const float* A, int lda, int bn, const float* gamm
   if ((drop ? ctas_per_sm<64, LF_BN_DROP>() : ctas_per_sm<64, LF_BN>()) <= 0) return PERT_ERR_UNSUPPORTED;
   double* acc = nullptr;
   const int rc = pert_bn_fwd_stats(A, lda, running_mean, running_var, eps, training, mean, rstd, N, H, workspace,
-                                   workspace_bytes, stats_ready, st, &acc);
+                                   workspace_bytes, stats_ready, training ? live : nullptr, st, &acc);
   if (rc != PERT_OK) return rc;
   a.x_out = x_out;
   a.acc = acc;
@@ -313,10 +330,9 @@ int pert_bn_linear_fwd_planes(const float* A, int lda, int bn, const float* gamm
     a.running_mean = running_mean;
     a.running_var = running_var;
     a.num_batches_tracked = num_batches_tracked;
+    a.live = live;
   }
   if (!drop) return launch<64, LF_BN>(a, st);
   a.drop = bn_dropout_params(dropout, drop_ctr, drop_layer);
   return launch<64, LF_BN_DROP>(a, st);
 }
-
-}  // extern "C"

@@ -80,13 +80,17 @@ constexpr int BN_BWD_ROWS = 64;   // rows per CTA (backward reductions: atomics,
 // acc[c] += n_b mean_b,  acc[H + c] += M2_b + n_b mean_b^2  (fp64 atomics; sum and sum of squares of fp32 data are
 // exact enough in fp64 that  M2 = S2 - S1^2 / N  has no cancellation problem), so no finalize kernel is needed --
 // k_bn_apply derives mean / rstd from acc in its prologue.
+// live != null (padded batch, see pert_batch_pad): only the rows below live[0] are counted.
 __global__ void __launch_bounds__(256) k_bn_partial(const float* __restrict__ x, int ld, long long N, int H,
-                                                     double* __restrict__ acc /*[2][H], zeroed*/) {
+                                                     double* __restrict__ acc /*[2][H], zeroed*/,
+                                                     const long long* __restrict__ live) {
   extern __shared__ float sm[];  // [rl][H] scratch, then mean[H]
   const int vpr = H >> 2;              // float4 lanes per row
   const int rl_n = blockDim.x / vpr;   // row lanes
   const int cl = threadIdx.x % vpr, rl = threadIdx.x / vpr;
   const long long r0 = (long long)blockIdx.x * BN_ROWS;
+  if (live) N = min(N, live[0]);
+  if (r0 >= N) return;                 // a chunk of ghost rows only (block-uniform)
   const int rows = (int)min((long long)BN_ROWS, N - r0);
   float* s_red = sm;             // [rl_n][H]
   float* s_mean = sm + rl_n * H; // [H]
@@ -159,12 +163,13 @@ __global__ void __launch_bounds__(256) k_bn_apply(const float* __restrict__ x, i
                                                    long long N, int H, int relu, const double* __restrict__ acc,
                                                    float eps, float momentum, float* running_mean,
                                                    float* running_var, long long* num_batches_tracked,
-                                                   BnDropout drop) {
+                                                   BnDropout drop, const long long* __restrict__ live) {
   extern __shared__ float s_par[];   // mean | rstd | gamma | beta
+  const long long n_stat = live ? live[0] : N;   // rows the statistics count (every row is normalised)
   for (int c = threadIdx.x; c < H; c += blockDim.x) {
     float mu, rs;
     if (acc) {
-      bn_batch_stats(acc, N, H, c, eps, momentum, blockIdx.x == 0, mean, rstd, running_mean, running_var,
+      bn_batch_stats(acc, n_stat, H, c, eps, momentum, blockIdx.x == 0, mean, rstd, running_mean, running_var,
                      num_batches_tracked, mu, rs);
     } else {
       mu = mean[c];
@@ -208,12 +213,15 @@ __global__ void __launch_bounds__(256) k_bn_bwd_reduce(const float* __restrict__
                                                         const float* __restrict__ x, int ld_x,
                                                         const float* __restrict__ mean,
                                                         const float* __restrict__ rstd, long long N, int H, int relu,
-                                                        float scale, float* __restrict__ sums) {
+                                                        float scale, float* __restrict__ sums,
+                                                        const long long* __restrict__ live) {
   extern __shared__ float sm[];  // [rl_n][2H]
   const int vpr = H >> 2;
   const int rl_n = blockDim.x / vpr;
   const int cl = threadIdx.x % vpr, rl = threadIdx.x / vpr;
   const long long r0 = (long long)blockIdx.x * BN_BWD_ROWS;
+  if (live) N = min(N, live[0]);
+  if (r0 >= N) return;                 // ghost rows only (block-uniform)
   const int rows = (int)min((long long)BN_BWD_ROWS, N - r0);
   float4 s1 = f4zero(), s2 = f4zero();
   if (rl < rl_n) {
@@ -250,12 +258,15 @@ __global__ void __launch_bounds__(256) k_bn_bwd_reduce(const float* __restrict__
   }
 }
 
-// training: dx = gamma*rstd*(dz - sum_dz/N - xhat*sum_dzxhat/N); eval: dx = gamma*rstd*dz
+// training: dx = gamma*rstd*(dz - sum_dz/N - xhat*sum_dzxhat/N); eval: dx = gamma*rstd*dz.
+// live != null (padded batch): N in the mean terms is live[0], and the ghost rows n >= live[0] get dx = 0 -- the mean
+// terms would otherwise hand them a gradient that flows on into the weights and the embedding row of the ghosts.
 __global__ void k_bn_bwd_apply(const float* __restrict__ dy, int ld_dy, const float* __restrict__ y, int ld_y,
                                const float* __restrict__ x, int ld_x, const float* __restrict__ mean,
                                const float* __restrict__ rstd, const float* __restrict__ gamma,
                                const float* __restrict__ sums, float* __restrict__ dx, int ld_dx, long long N, int H,
-                               int relu, float scale, int training, float* dgamma, float* dbeta) {
+                               int relu, float scale, int training, float* dgamma, float* dbeta,
+                               const long long* __restrict__ live) {
   const int vpr = H >> 2;
   long long id = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (blockIdx.x == 0)  // parameter grads accumulate (+=) like autograd
@@ -266,6 +277,11 @@ __global__ void k_bn_bwd_apply(const float* __restrict__ dy, int ld_dy, const fl
   if (id >= N * vpr) return;
   long long n = id / vpr;
   int c = (int)(id % vpr) * 4;
+  const long long n_live = live ? live[0] : N;
+  if (n >= n_live) {
+    st4(dx + (size_t)n * ld_dx + c, f4zero());
+    return;
+  }
   float4 g = ldg4(dy + (size_t)n * ld_dy + c);
   if (relu) {
     float4 yy = ldg4(y + (size_t)n * ld_y + c);
@@ -275,7 +291,7 @@ __global__ void k_bn_bwd_apply(const float* __restrict__ dy, int ld_dy, const fl
   const float4 rs = ldg4(rstd + c), ga = ldg4(gamma + c);
   float4 o;
   if (training) {
-    const float invn = 1.0f / (float)N;
+    const float invn = 1.0f / (float)n_live;
     const float4 v = ldg4(x + (size_t)n * ld_x + c), mu = ldg4(mean + c);
     const float4 a = ldg4(sums + c), b = ldg4(sums + H + c);
     o.x = ga.x * rs.x * (g.x - a.x * invn - (v.x - mu.x) * rs.x * b.x * invn);
@@ -439,19 +455,26 @@ __global__ void k_relu_bwd(const float* __restrict__ y, float* __restrict__ dy, 
   if (i < n && !(y[i] > 0.f)) dy[i] = 0.f;
 }
 
-// pinball loss (pert_gnn.py:191-193): loss = mean(max(tau*e, (tau-1)*e)), e = y - yhat; dyhat = dloss/dyhat
+// pinball loss (pert_gnn.py:191-193): loss = mean(max(tau*e, (tau-1)*e)), e = y - yhat; dyhat = dloss/dyhat.
+// live != null (padded batch): the mean runs over the graphs i < live[1]; the ghost graphs above get dyhat = 0.
 __global__ void k_pinball(const int64_t* __restrict__ y, const float* __restrict__ yhat, float tau, int B,
-                          float grad_scale, float* __restrict__ loss, float* __restrict__ dyhat) {
+                          float grad_scale, float* __restrict__ loss, float* __restrict__ dyhat,
+                          const long long* __restrict__ live) {
   __shared__ float red[32];
+  const int Bl = live ? (int)min((long long)B, live[1]) : B;
   float s = 0.f;
   for (int i = threadIdx.x; i < B; i += blockDim.x) {
+    if (i >= Bl) {
+      if (dyhat) dyhat[i] = 0.f;
+      continue;
+    }
     float e = (float)y[i] - yhat[i];
     float a = tau * e, b = (tau - 1.f) * e;
     s += fmaxf(a, b);
     if (dyhat) {
       // torch.maximum backward: ties split the gradient evenly
       float d = (a > b) ? -tau : ((a < b) ? (1.f - tau) : 0.5f * (1.f - 2.f * tau));
-      dyhat[i] = grad_scale * d / (float)B;
+      dyhat[i] = grad_scale * d / (float)Bl;
     }
   }
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
@@ -460,7 +483,7 @@ __global__ void k_pinball(const int64_t* __restrict__ y, const float* __restrict
   if (threadIdx.x < 32) {
     float t = (threadIdx.x < (blockDim.x >> 5)) ? red[threadIdx.x] : 0.f;
     for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-    if (threadIdx.x == 0 && loss) *loss = t / (float)B;
+    if (threadIdx.x == 0 && loss) *loss = t / (float)Bl;
   }
 }
 
@@ -488,7 +511,9 @@ inline bool al16(const void* p) { return p == nullptr || ((uintptr_t)p & 15) == 
 
 // ---- eval metrics (reference pert_gnn.py:284-289, :249): block sums in double, one atomic per block and metric
 __global__ void __launch_bounds__(256) k_eval_metrics(const int64_t* __restrict__ y, const float* __restrict__ yhat,
-                                                      float tau, int B, double* __restrict__ acc) {
+                                                      float tau, int B, double* __restrict__ acc,
+                                                      const long long* __restrict__ live) {
+  if (live) B = (int)min((long long)B, live[1]);   // padded batch: the real graphs only
   double mae = 0.0, mape = 0.0, q = 0.0;
   for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < B; b += gridDim.x * blockDim.x) {
     const float yt = (float)y[b];                 // y.float() / int64 -> float32 promotion of the reference
@@ -561,7 +586,8 @@ int pert_bn_fwd(const float* x, int ld_x, const float* gamma, const float* beta,
                 int relu, float* mean, float* rstd, float* y, int ld_y, long long N, int H, void* workspace,
                 long long workspace_bytes, void* stream) {
   return pert_bn_fwd_ex(x, ld_x, gamma, beta, running_mean, running_var, num_batches_tracked, eps, momentum, training,
-                        relu, mean, rstd, y, ld_y, N, H, workspace, workspace_bytes, 0, 0.f, nullptr, 0, stream);
+                        relu, mean, rstd, y, ld_y, N, H, workspace, workspace_bytes, 0, 0.f, nullptr, 0, nullptr,
+                        stream);
 }
 
 }  // extern "C"
@@ -570,9 +596,11 @@ int pert_bn_fwd(const float* x, int ld_x, const float* gamma, const float* beta,
 // BatchNorm to its input (csrc/linear_fwd.cu).  Training: *acc = the fp64 column sums / sums of squares in `workspace`
 // (computed here by k_bn_partial unless stats_ready, i.e. the producer of x already left them there); the apply derives
 // mean / rstd from them.  Eval: mean / rstd = the running statistics (k_bn_eval_stats), *acc = NULL.
+// live != null (padded batch): the sums cover the rows below live[0] only.
 int pert_bn_fwd_stats(const float* x, int ld_x, const float* running_mean, const float* running_var, float eps,
                       int training, float* mean, float* rstd, long long N, int H, void* workspace,
-                      long long workspace_bytes, int stats_ready, cudaStream_t st, double** acc) {
+                      long long workspace_bytes, int stats_ready, const long long* live, cudaStream_t st,
+                      double** acc) {
   *acc = nullptr;
   if (training) {
     if (!workspace || workspace_bytes < pert_bn_workspace_bytes(N, H)) return PERT_ERR_BADARG;
@@ -589,7 +617,7 @@ int pert_bn_fwd_stats(const float* x, int ld_x, const float* running_mean, const
     if (!stats_ready) {
       cudaError_t e = cudaMemsetAsync(*acc, 0, (size_t)2 * H * sizeof(double), st);
       if (e != cudaSuccess) return (int)e;
-      k_bn_partial<<<chunks, threads, smem, st>>>(x, ld_x, N, H, *acc);
+      k_bn_partial<<<chunks, threads, smem, st>>>(x, ld_x, N, H, *acc, live);
     }
   } else {
     if (!running_mean || !running_var) return PERT_ERR_BADARG;
@@ -601,11 +629,12 @@ int pert_bn_fwd_stats(const float* x, int ld_x, const float* running_mean, const
 // stats_ready != 0 (training): the fp64 column sums / sums of squares already sit in `workspace` (written by the producer
 // of x, csrc/tconv_tile.cu) -- only the apply pass runs.  dropout > 0 (training + ReLU): inverted dropout of the output
 // with the mask of layer `drop_layer` at the device {seed, step} `drop_ctr` (see philox4x32_10 for the contract).
+// live != null (training on a padded batch): the statistics count the rows below live[0]; every row is normalised.
 int pert_bn_fwd_ex(const float* x, int ld_x, const float* gamma, const float* beta, float* running_mean,
                    float* running_var, long long* num_batches_tracked, float eps, float momentum, int training,
                    int relu, float* mean, float* rstd, float* y, int ld_y, long long N, int H, void* workspace,
                    long long workspace_bytes, int stats_ready, float dropout, const long long* drop_ctr,
-                   int drop_layer, void* stream) {
+                   int drop_layer, const long long* live, void* stream) {
   if (N < 0 || H <= 0 || H % 4 || H > 1024 || ld_x % 4 || ld_y % 4 || !x || !gamma || !beta || !mean || !rstd || !y)
     return PERT_ERR_BADARG;
   if (!al16(x) || !al16(gamma) || !al16(beta) || !al16(mean) || !al16(rstd) || !al16(y)) return PERT_ERR_BADARG;
@@ -616,7 +645,7 @@ int pert_bn_fwd_ex(const float* x, int ld_x, const float* gamma, const float* be
   cudaStream_t st = (cudaStream_t)stream;
   double* acc = nullptr;
   int rc = pert_bn_fwd_stats(x, ld_x, running_mean, running_var, eps, training, mean, rstd, N, H, workspace,
-                             workspace_bytes, stats_ready, st, &acc);
+                             workspace_bytes, stats_ready, live, st, &acc);
   if (rc != PERT_OK) return rc;
   long long total = N * (H / 4);
   long long blocks = pert_cdiv(total, 256 * 4);
@@ -627,7 +656,8 @@ int pert_bn_fwd_ex(const float* x, int ld_x, const float* gamma, const float* be
                                                                  acc, eps, momentum,
                                                                  training ? running_mean : nullptr,
                                                                  training ? running_var : nullptr,
-                                                                 training ? num_batches_tracked : nullptr, dp);
+                                                                 training ? num_batches_tracked : nullptr, dp,
+                                                                 training ? live : nullptr);
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }
@@ -639,16 +669,17 @@ int pert_bn_bwd(const float* dy, int ld_dy, const float* y, int ld_y, const floa
                 const float* rstd, const float* gamma, int relu, int training, float* dx, int ld_dx, float* dgamma,
                 float* dbeta, float* sums, long long N, int H, void* stream) {
   return pert_bn_bwd_ex(dy, ld_dy, y, ld_y, x, ld_x, mean, rstd, gamma, relu, 1.f, training, dx, ld_dx, dgamma, dbeta,
-                        sums, N, H, stream);
+                        sums, N, H, nullptr, stream);
 }
 
 }  // extern "C"
 
 // relu_scale: factor applied to the ReLU-masked gradient (1 / (1 - p) after inverted dropout, see k_bn_bwd_reduce);
-// anything but 1 needs relu.
+// anything but 1 needs relu.  live != null (training on a padded batch): see k_bn_bwd_apply.
 int pert_bn_bwd_ex(const float* dy, int ld_dy, const float* y, int ld_y, const float* x, int ld_x, const float* mean,
                    const float* rstd, const float* gamma, int relu, float relu_scale, int training, float* dx,
-                   int ld_dx, float* dgamma, float* dbeta, float* sums, long long N, int H, void* stream) {
+                   int ld_dx, float* dgamma, float* dbeta, float* sums, long long N, int H, const long long* live,
+                   void* stream) {
   if (N < 0 || H <= 0 || H % 4 || H > 1024 || !dy || !x || !mean || !rstd || !gamma || !dx || !sums)
     return PERT_ERR_BADARG;
   if (relu && !y) return PERT_ERR_BADARG;
@@ -666,11 +697,12 @@ int pert_bn_bwd_ex(const float* dy, int ld_dy, const float* y, int ld_y, const f
   int rl_n = threads / vpr;
   size_t smem = (size_t)rl_n * 2 * H * sizeof(float);
   if (smem > 48 * 1024) return PERT_ERR_UNSUPPORTED;
+  if (!training) live = nullptr;
   k_bn_bwd_reduce<<<pert_cdiv(N, BN_BWD_ROWS), threads, smem, st>>>(dy, ld_dy, y, ld_y, x, ld_x, mean, rstd, N, H, relu,
-                                                              relu_scale, sums);
+                                                              relu_scale, sums, live);
   long long total = N * vpr;
   k_bn_bwd_apply<<<pert_cdiv(total, 256), 256, 0, st>>>(dy, ld_dy, y, ld_y, x, ld_x, mean, rstd, gamma, sums, dx,
-                                                       ld_dx, N, H, relu, relu_scale, training, dgamma, dbeta);
+                                                       ld_dx, N, H, relu, relu_scale, training, dgamma, dbeta, live);
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }
@@ -734,8 +766,13 @@ int pert_relu_bwd(const float* y, float* dy, long long n, void* stream) {
 
 int pert_pinball_loss(const int64_t* y, const float* yhat, float tau, long long B, float grad_scale, float* loss,
                       float* dyhat, void* stream) {
+  return pert_pinball_loss_live(y, yhat, tau, B, grad_scale, loss, dyhat, nullptr, stream);
+}
+
+int pert_pinball_loss_live(const int64_t* y, const float* yhat, float tau, long long B, float grad_scale, float* loss,
+                           float* dyhat, const long long* live, void* stream) {
   if (B <= 0 || !y || !yhat) return PERT_ERR_BADARG;
-  k_pinball<<<1, 256, 0, (cudaStream_t)stream>>>(y, yhat, tau, (int)B, grad_scale, loss, dyhat);
+  k_pinball<<<1, 256, 0, (cudaStream_t)stream>>>(y, yhat, tau, (int)B, grad_scale, loss, dyhat, live);
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }
@@ -753,11 +790,16 @@ int pert_adam_step(float* p, const float* g, float* m, float* v, long long n, fl
 }
 
 int pert_eval_metrics(const int64_t* y, const float* yhat, float tau, long long B, double* acc, void* stream) {
+  return pert_eval_metrics_live(y, yhat, tau, B, acc, nullptr, stream);
+}
+
+int pert_eval_metrics_live(const int64_t* y, const float* yhat, float tau, long long B, double* acc,
+                           const long long* live, void* stream) {
   if (B < 0 || !y || !yhat || !acc) return PERT_ERR_BADARG;
   if (B == 0) return PERT_OK;
   int grid = pert_cdiv(B, 256);
   if (grid > 64) grid = 64;
-  k_eval_metrics<<<grid, 256, 0, (cudaStream_t)stream>>>(y, yhat, tau, (int)B, acc);
+  k_eval_metrics<<<grid, 256, 0, (cudaStream_t)stream>>>(y, yhat, tau, (int)B, acc, live);
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }

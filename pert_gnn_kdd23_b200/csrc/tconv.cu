@@ -432,7 +432,7 @@ inline bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 int pert_tile_fwd(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if, const float* t_rpc,
                   int n_rpc, float* out, int ld_out, float* alpha, long long N, long long E, long long B, int H,
-                  double* bn_acc, const PertTiles* tiles, cudaStream_t st);
+                  double* bn_acc, const long long* live, const PertTiles* tiles, cudaStream_t st);
 int pert_tile_bwd(const float* g_, int ld_g, const float* q, const float* k, const float* v, int ld, const int* rowptr,
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
                   const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha, float* dq, float* dk,
@@ -461,13 +461,14 @@ int pert_tconv_supported_width(int H) {
 int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                          const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if,
                          const float* t_rpc, float* out, int ld_out, float* alpha, int n_rpc, long long N, long long E,
-                         long long B_hint, int H, double* bn_acc, int* fused, const PertTiles* tiles, void* stream) {
+                         long long B_hint, int H, double* bn_acc, const long long* live, int* fused,
+                         const PertTiles* tiles, void* stream) {
   *fused = 0;
   if ((bn_acc || tiles) && N > 0 && tile_enabled() && ld_out == H && q && k && v && rowptr && out && !(ld % 4) && aligned16(q) &&
       aligned16(k) && aligned16(v) && aligned16(out) && (!s || aligned16(s)) &&
       (!t_if || (aligned16(t_if) && t_rpc && aligned16(t_rpc) && csr_if && csr_rpc))) {
     int rt = pert_tile_fwd(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, n_rpc, out, ld_out, alpha, N, E,
-                           B_hint, H, bn_acc, tiles, (cudaStream_t)stream);
+                           B_hint, H, bn_acc, live, tiles, (cudaStream_t)stream);
     if (rt == PERT_OK) {
       *fused = bn_acc ? 1 : 0;
       PERT_LAUNCH_CHECK();
@@ -517,7 +518,7 @@ int pert_tconv_fwd(const float* q, const float* k, const float* v, const float* 
   if (N == 0) return PERT_OK;
   if (tile_enabled() && ld_out == H) {
     int rt = pert_tile_fwd(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, n_rpc, out, ld_out, alpha, N, E,
-                           B_hint, H, nullptr, nullptr, (cudaStream_t)stream);
+                           B_hint, H, nullptr, nullptr, nullptr, (cudaStream_t)stream);
     if (rt != PERT_ERR_UNSUPPORTED) {
       if (rt) return rt;
       PERT_LAUNCH_CHECK();

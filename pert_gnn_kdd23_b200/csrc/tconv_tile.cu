@@ -72,6 +72,7 @@ struct TileArgs {
   float* dsp;       // bwd_dst: written; bwd_src: read
   float *dt_if, *dt_rpc;
   double* bn_acc;   // fwd: optional [2][H] column sums / sums of squares of `out` (BatchNorm statistics), +=
+  const long long* live;   // fwd, padded batch: bn_acc counts the nodes below live[0] only (null: all N)
   float* rpc_ws;    // [N][2][RPC_FAST] per-target sums over in-edges of (alpha, ds) by rpc type, or null (see bwd_src)
   int N, tile_nodes, edge_cap;
   int hot_if;          // interface id whose table-gradient row is accumulated per CTA instead of per edge (source pass)
@@ -419,10 +420,14 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
         }
         const float invZ = 1.0f / (Z + 1e-16f);
         if (valid) {
+          // padded batch: only the real nodes (below live[0]) enter the statistics.  Read per node, not kept in a
+          // register across the edge loop (a volatile load is not hoisted; it hits L1 after the first node)
+          const bool counted = !a.live || i < *reinterpret_cast<const volatile long long*>(a.live);
 #pragma unroll
           for (int u = 0; u < VPL; ++u) {
             const float4 o = f4add(f4scale(invZ, acc[u]), skip[u]);
             st4(a.out + (size_t)i * H + (lig + u * LPR) * 4, o);
+            if (!counted) continue;
             bsum[u] = f4add(bsum[u], o);
             bsq[u].x = fmaf(o.x, o.x, bsq[u].x); bsq[u].y = fmaf(o.y, o.y, bsq[u].y);
             bsq[u].z = fmaf(o.z, o.z, bsq[u].z); bsq[u].w = fmaf(o.w, o.w, bsq[u].w);
@@ -1045,13 +1050,14 @@ int launch_bwd(const TileArgs& a0, long long N, long long E, long long B, bool h
 int pert_tile_fwd(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if, const float* t_rpc,
                   int n_rpc, float* out, int ld_out, float* alpha, long long N, long long E, long long B, int H,
-                  double* bn_acc, const PertTiles* tiles, cudaStream_t st) {
+                  double* bn_acc, const long long* live, const PertTiles* tiles, cudaStream_t st) {
   if (ld != H || ld_out != H || (t_if && (size_t)n_rpc * H * 4 > 16 * 1024))
     return PERT_ERR_UNSUPPORTED;
   TileArgs a{};
   a.q = q; a.k = k; a.v = v; a.s = s;
   a.rowptr = rowptr; a.csr_src = csr_src; a.csr_if = csr_if; a.csr_rpc = csr_rpc;
   a.t_if = t_if; a.t_rpc = t_rpc; a.n_rpc = n_rpc; a.out = out; a.alpha = alpha; a.bn_acc = bn_acc;
+  a.live = bn_acc ? live : nullptr;
   a.N = (int)N; a.inv_sqrt_c = 1.0f / sqrtf((float)H);
   switch (H) {
     case 32: return launch_fwd<32>(a, N, E, B, t_if != nullptr, tiles, st);

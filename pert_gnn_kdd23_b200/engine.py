@@ -209,10 +209,12 @@ class Engine:
 
     @_lib.on_device_of
     def forward(self, x, cat_X, entry_id, probs, pnn, batch, index: GraphIndex, training, probe=None,
-                index_ready=None):
+                index_ready=None, live=None):
         """-> (global_pred [B,1], local_pred [N,1]); keeps what backward needs in the workspace.  In training the
         BatchNorm outputs are dropped with ``model.dropout`` (mask drawn from ``model.dropout_state()``, whose step
-        this call advances on the device)."""
+        this call advances on the device).  ``live``: device int64 [2] {N, B} of a batch padded by
+        ``pert_batch_pad`` (the inputs are the capacity buffers); the BatchNorm statistics then count the real rows
+        only (``pert_model_forward_live``)."""
         N, E, B = x.size(0), index.E, entry_id.numel()
         p_drop = float(self.model.dropout) if training else 0.0
         state = self.model.dropout_state() if p_drop > 0 else None
@@ -227,20 +229,24 @@ class Engine:
         gpred = torch.empty(B, 1, device=dev, dtype=torch.float32)
         lpred = torch.empty(N, 1, device=dev, dtype=torch.float32)
         p = _lib.ptr
-        rc = self.lib.pert_model_forward(
-            C.byref(self.desc), p(self.fp.flat), p(self.bn_running), p(self.bn_nbt), p(x), p(cat_X), p(entry_id),
-            p(probs), p(pnn), p(batch), N, E, B, p(index.rowptr), p(index.csr_src), p(index.csr_if), p(index.csr_rpc),
-            p(ws), ws.numel() * 4, int(training), p_drop, p(state), p(gpred), p(lpred), p(index.status),
-            C.byref(probe) if probe is not None else None,
-            C.c_void_p(index_ready.cuda_event) if index_ready is not None else None, _lib.stream())
+        args = (C.byref(self.desc), p(self.fp.flat), p(self.bn_running), p(self.bn_nbt), p(x), p(cat_X), p(entry_id),
+                p(probs), p(pnn), p(batch), N, E, B, p(index.rowptr), p(index.csr_src), p(index.csr_if),
+                p(index.csr_rpc), p(ws), ws.numel() * 4, int(training), p_drop, p(state), p(gpred), p(lpred),
+                p(index.status), C.byref(probe) if probe is not None else None,
+                C.c_void_p(index_ready.cuda_event) if index_ready is not None else None)
+        if live is None:
+            rc = self.lib.pert_model_forward(*args, _lib.stream())
+        else:
+            rc = self.lib.pert_model_forward_live(*args, p(live), _lib.stream())
         _lib.check(rc, "pert_model_forward")
         self._saved = (x, cat_X, entry_id, probs, pnn, batch, index, bool(training), N, E, B, p_drop)
         ops.LAUNCHES["n"] += self.launches_forward()
         return gpred, lpred
 
     @_lib.on_device_of
-    def backward(self, d_global, d_local=None, grads=None, probe=None):
-        """Accumulates (+=) parameter gradients into ``grads`` (default: the flat gradient buffer)."""
+    def backward(self, d_global, d_local=None, grads=None, probe=None, live=None):
+        """Accumulates (+=) parameter gradients into ``grads`` (default: the flat gradient buffer).  ``live``: the
+        word the forward got (padded batch); ``d_global`` must then be 0 for the ghost graphs."""
         x, cat_X, entry_id, probs, pnn, batch, index, training, N, E, B, p_drop = self._saved
         grads = self.fp.grad if grads is None else grads
         d_global = d_global.reshape(-1).contiguous().float()
@@ -248,11 +254,14 @@ class Engine:
             d_local = d_local.reshape(-1).contiguous().float()
         p = _lib.ptr
         ws = self.ws
-        rc = self.lib.pert_model_backward(
-            C.byref(self.desc), p(self.fp.flat), p(grads), p(cat_X), p(entry_id), p(probs), p(pnn), p(batch), N, E, B,
-            p(index.rowptr), p(index.csr_src), p(index.csr_if), p(index.csr_rpc), p(index.colptr), p(index.csc_pos),
-            p(index.csc_dst), p(ws), ws.numel() * 4, int(training), p_drop, p(d_global), p(d_local),
-            C.byref(probe) if probe is not None else None, _lib.stream())
+        args = (C.byref(self.desc), p(self.fp.flat), p(grads), p(cat_X), p(entry_id), p(probs), p(pnn), p(batch), N,
+                E, B, p(index.rowptr), p(index.csr_src), p(index.csr_if), p(index.csr_rpc), p(index.colptr),
+                p(index.csc_pos), p(index.csc_dst), p(ws), ws.numel() * 4, int(training), p_drop, p(d_global),
+                p(d_local), C.byref(probe) if probe is not None else None)
+        if live is None:
+            rc = self.lib.pert_model_backward(*args, _lib.stream())
+        else:
+            rc = self.lib.pert_model_backward_live(*args, p(live), _lib.stream())
         _lib.check(rc, "pert_model_backward")
         ops.LAUNCHES["n"] += self.launches_backward()
 

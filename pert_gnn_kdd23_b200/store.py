@@ -260,6 +260,16 @@ class StoreLoader:
     def __len__(self):
         return -(-len(self.dataset) // self.batch_size)
 
+    def max_sizes(self):
+        """Host-only upper bound (N, E, B) of any batch of any shuffle: the sums of the ``batch_size`` largest
+        per-trace node and edge counts, and ``batch_size`` graphs (``train.BucketedTrainStep.reserve``)."""
+        ids = np.asarray(self.dataset, dtype=np.int64)
+        b = min(self.batch_size, len(ids))
+        ent = self.store._h_trace_entry[ids]
+        n = np.sort(np.asarray(self.store._h_ent_nodes, dtype=np.int64)[ent])[::-1]
+        e = np.sort(np.asarray(self.store._h_ent_edges, dtype=np.int64)[ent])[::-1]
+        return int(n[:b].sum()), int(e[:b].sum()), int(b)
+
     def __iter__(self):
         ids = np.asarray(self.dataset, dtype=np.int64)
         if self.shuffle:

@@ -297,9 +297,10 @@ def _side_stream(device):
 
 
 @_lib.on_device_of
-def _fused_fwd_bwd(model, optimizer: FusedAdam, data, tau, index, probe, use_index_cache=True):
+def _fused_fwd_bwd(model, optimizer: FusedAdam, data, tau, index, probe, use_index_cache=True, live=None):
     """Device work of one step up to the gradients: (index build) -> zero grads -> engine forward -> pinball loss +
-    its gradient -> engine backward into the flat gradient buffer.  Returns (loss [1], index)."""
+    its gradient -> engine backward into the flat gradient buffer.  Returns (loss [1], index).  ``live``: the {N, B}
+    word of a padded batch (``PaddedBatch``), read by the engine and the loss."""
     from .index import build_index, cached_index
 
     eng = model.engine(optimizer.fp) if (model._engine is None or model._engine.fp is not optimizer.fp) \
@@ -323,14 +324,18 @@ def _fused_fwd_bwd(model, optimizer: FusedAdam, data, tau, index, probe, use_ind
     optimizer.zero_grad()
     with torch.no_grad():
         gpred, _ = eng.forward(x, cat_X, entry_id, probs, pnn, batch, index, model.training, probe=probe,
-                               index_ready=index_ready)
+                               index_ready=index_ready, live=live)
         B = gpred.size(0)
         loss = torch.empty(1, device=gpred.device, dtype=torch.float32)
         dy = torch.empty(B, device=gpred.device, dtype=torch.float32)
-        _lib.call("pert_pinball_loss", _lib.ptr(data.y), _lib.ptr(gpred), float(tau), B, 1.0, _lib.ptr(loss),
-                  _lib.ptr(dy), _lib.stream())
+        if live is None:
+            _lib.call("pert_pinball_loss", _lib.ptr(data.y), _lib.ptr(gpred), float(tau), B, 1.0, _lib.ptr(loss),
+                      _lib.ptr(dy), _lib.stream())
+        else:
+            _lib.call("pert_pinball_loss_live", _lib.ptr(data.y), _lib.ptr(gpred), float(tau), B, 1.0,
+                      _lib.ptr(loss), _lib.ptr(dy), _lib.ptr(live), _lib.stream())
         ops.LAUNCHES["n"] += 1
-        eng.backward(dy, None, probe=probe)
+        eng.backward(dy, None, probe=probe, live=live)
     return loss, index
 
 
@@ -426,6 +431,204 @@ class GraphedTrainStep:
         return ent
 
 
+# ------------------------------------------------------------------------------------------ capacity buckets
+def ladder(x):
+    """x up to 16, else x rounded up to 4 significant bits (m * 2^k, m in 8..15): less than 1/8 wasted."""
+    x = int(x)
+    if x <= 16:
+        return x
+    k = x.bit_length() - 4
+    m = -(-x >> k)                     # ceil(x / 2^k), in 8..16
+    return m << k
+
+
+def bucket_caps(N, E, B):
+    """Capacity bucket (N_cap, E_cap, B_cap) of a batch of N nodes, E edges and B graphs: at least one ghost graph
+    (B_cap > B), at least one ghost node per ghost graph and at most 4 ghost edges per ghost node (a single ghost hub
+    with thousands of self-loops would stall a warp of the attention kernels)."""
+    B_cap = ladder(B + 1)
+    E_cap = ladder(E)
+    return ladder(N + max(B_cap - B, -(-(E_cap - E) // 4))), E_cap, B_cap
+
+
+def bucket_bound(N, E, B):
+    """Componentwise upper bound of ``bucket_caps(n, e, b)`` over all n <= N, e <= E, b <= B (monotone in each
+    argument, which ``bucket_caps`` is not in N_cap): ``ladder`` adds less than 1/8, so a batch has at most
+    ceil((b + 1) / 8) + 1 ghost graphs and ceil(e / 8) ghost edges."""
+    return (ladder(N + max(-(-(B + 1) // 8) + 1, -(-(-(-E // 8)) // 4))), ladder(E), ladder(B + 1))
+
+
+class PaddedBatch:
+    """Persistent device buffers of one capacity bucket.  ``fill(data)`` copies a batch into them and writes the
+    ghost tail and the {N, B} word ``live`` (``pert_batch_pad``, one launch); the object then serves as the batch of
+    the padded step (``model_inputs`` works on it)."""
+
+    def __init__(self, caps, like):
+        N_cap, E_cap, B_cap = caps
+        dev = like.x.device
+        f32, i64 = torch.float32, torch.int64
+        self.caps = caps
+        self.x = torch.empty(N_cap, like.x.size(1), dtype=f32, device=dev)
+        self.cat_X = torch.empty(N_cap, like.cat_X.size(1), dtype=i64, device=dev)
+        self.edge_index = torch.empty(2, E_cap, dtype=i64, device=dev)
+        self.edge_attr = torch.empty(E_cap, like.edge_attr.size(1), dtype=i64, device=dev)
+        self.batch = torch.empty(N_cap, dtype=i64, device=dev)
+        self.entry_id = torch.empty(B_cap, dtype=i64, device=dev)
+        self.y = torch.empty(B_cap, dtype=i64, device=dev)
+        self.rt_probs = torch.empty(N_cap, 1, dtype=f32, device=dev)
+        self.pattern_num_nodes = torch.empty(N_cap, 1, dtype=f32, device=dev)
+        self.live = torch.zeros(2, dtype=i64, device=dev)
+        self.num_graphs = B_cap
+
+    def __contains__(self, key):
+        return key == "rt_probs"
+
+    @property
+    def device(self):
+        return self.x.device
+
+    @staticmethod
+    def accepts(data):
+        """True if ``fill`` can pad ``data``: per-node ``rt_probs`` and ``pattern_num_nodes``, edge attributes, at
+        least one graph.  A batch with per-pattern ``pattern_probs`` only is not padded (the callers run it eagerly)."""
+        if "rt_probs" not in data or data.edge_attr is None or data.num_graphs < 1:
+            return False
+        N = data.x.size(0)
+        return data.rt_probs.numel() == N and data.pattern_num_nodes.numel() == N
+
+    @_lib.on_device_of
+    def fill(self, data):
+        if not self.accepts(data):
+            raise _lib.PertGnnError("PaddedBatch needs per-node rt_probs and pattern_num_nodes and edge attributes")
+        x, cat_X, edge_index, edge_attr, pnn, probs, entry_id, batch = model_inputs(data)
+        N, E, B = x.size(0), edge_index.size(1), entry_id.numel()
+        c = lambda t: t.contiguous()
+        x, cat_X, edge_index, edge_attr = c(x.float()), c(cat_X), c(edge_index), c(edge_attr)
+        pnn, probs, entry_id, batch, y = c(pnn.float()), c(probs.float()), c(entry_id), c(batch), c(data.y)
+        p = _lib.ptr
+        _lib.call("pert_batch_pad", p(x), p(cat_X), p(edge_index), p(edge_attr), p(batch), p(entry_id), p(y),
+                  p(probs), p(pnn), N, E, B, x.size(1), cat_X.size(1), edge_attr.size(1), p(self.x), p(self.cat_X),
+                  p(self.edge_index), p(self.edge_attr), p(self.batch), p(self.entry_id), p(self.y),
+                  p(self.rt_probs), p(self.pattern_num_nodes), *self.caps, p(self.live), _lib.stream())
+        ops.LAUNCHES["n"] += 1
+        return self
+
+
+def _batch_sizes(data):
+    return int(data.x.size(0)), int(data.edge_index.size(1)), int(data.num_graphs)
+
+
+def _stale(ent, eng):
+    """A captured graph of bucket entry ``ent`` may not be replayed with engine ``eng``: it was captured over another
+    engine (re-created after the parameters moved) or over a workspace the engine has since re-allocated."""
+    return ent["engine"] is not eng or ent["ws_gen"] != eng.ws_generation
+
+
+def _drop_graph(ent):
+    ent["state"] = "ran-once"
+    for k in ("graph", "loss", "index", "out", "engine", "ws", "ws_gen", "launches"):
+        ent.pop(k, None)
+
+
+class BucketedTrainStep:
+    """``fused_train_step`` replayed from one CUDA graph per capacity bucket, for batches whose sizes and buffers
+    change every step (a shuffled ``StoreLoader``: ``GraphedTrainStep`` keys on both and never replays there).
+
+    Each batch is padded into the persistent buffers of its bucket ``bucket_caps(N, E, B)`` (``PaddedBatch``, one
+    eager launch); the kernels run at the capacity sizes and read the real {N, B} from a device word where a count
+    enters the arithmetic (BatchNorm statistics and backward, the loss), so the step computes what the unpadded step
+    computes for the real graphs.  Protocol of ``GraphedTrainStep``: the first visit of a bucket runs eagerly (on the
+    padded buffers), the second is captured, later ones replay.  A graph captured over an engine or workspace that has
+    since been replaced (a re-allocation for a bigger bucket, a re-created engine) is dropped and captured again on its
+    next visit (``invalidations``; ``reserve(*loader.max_sizes())`` sizes the workspace once up front).  Past
+    ``max_graphs`` buckets, after a failed capture (``capture_error``) and for a batch ``PaddedBatch`` cannot pad
+    (per-pattern probabilities only) the step runs eager ``fused_train_step`` on the unpadded batch.
+    ``pad_ratio`` = sum of N_cap / sum of N over the padded steps."""
+
+    def __init__(self, model, optimizer: FusedAdam, tau=0.5, dp: DataParallel | None = None, max_graphs=32):
+        self.model, self.opt, self.tau, self.dp = model, optimizer, tau, dp
+        self.max_graphs = max_graphs
+        self._buckets = {}   # key -> {"buf": PaddedBatch, "state": "ran-once" | "failed" | "graph", ...}
+        self.capture_error = None
+        self.replays = 0
+        self.captures = 0
+        self.invalidations = 0
+        self._n_real = 0
+        self._n_cap = 0
+
+    @property
+    def pad_ratio(self):
+        return self._n_cap / max(self._n_real, 1)
+
+    def _engine(self):
+        m = self.model
+        return m.engine(self.opt.fp) if (m._engine is None or m._engine.fp is not self.opt.fp) else m._engine
+
+    def reserve(self, N, E, B):
+        """Sizes the engine workspace for every bucket of a batch of at most N nodes, E edges and B graphs."""
+        self._engine().reserve(*bucket_bound(N, E, B))
+
+    def _finish(self, loss):
+        with torch.no_grad():
+            scale = self.dp.all_reduce_grads(self.opt) if self.dp is not None else 1.0
+            self.opt.step(grad_scale=scale)
+        return loss
+
+    def __call__(self, data):
+        if not PaddedBatch.accepts(data):
+            return fused_train_step(self.model, self.opt, data, self.tau, self.dp)
+        N, E, B = _batch_sizes(data)
+        caps = bucket_caps(N, E, B)
+        # training flag and dropout rate are by-value arguments of the captured calls: each needs its own graph
+        key = caps + (int(data.edge_attr.size(1)), self.model.training, float(self.model.dropout))
+        ent = self._buckets.get(key)
+        if ent is None:
+            if len(self._buckets) >= self.max_graphs:
+                return fused_train_step(self.model, self.opt, data, self.tau, self.dp)
+            ent = self._buckets[key] = {"buf": PaddedBatch(caps, data), "state": "new"}
+        if ent["state"] == "failed":
+            return fused_train_step(self.model, self.opt, data, self.tau, self.dp)
+        buf = ent["buf"].fill(data)
+        self._n_real += N
+        self._n_cap += caps[0]
+        eng = self._engine()
+        if ent["state"] == "graph" and _stale(ent, eng):
+            _drop_graph(ent)
+            self.invalidations += 1
+        if ent["state"] == "new":
+            ent["state"] = "ran-once"
+            loss, _ = _fused_fwd_bwd(self.model, self.opt, buf, self.tau, None, None, use_index_cache=False,
+                                     live=buf.live)
+            return self._finish(loss)
+        if ent["state"] == "ran-once" and not self._capture(ent):
+            return fused_train_step(self.model, self.opt, data, self.tau, self.dp)
+        ent["graph"].replay()
+        ops.LAUNCHES["n"] += ent["launches"]
+        self.replays += 1
+        return self._finish(ent["loss"])
+
+    def _capture(self, ent):
+        buf = ent["buf"]
+        g = torch.cuda.CUDAGraph()
+        l0 = ops.LAUNCHES["n"]
+        try:
+            with torch.cuda.graph(g):
+                loss, index = _fused_fwd_bwd(self.model, self.opt, buf, self.tau, None, None, use_index_cache=False,
+                                             live=buf.live)
+        except Exception as e:  # noqa: BLE001 - a failed capture leaves this bucket on the eager unpadded path
+            self.capture_error = repr(e)
+            ops.LAUNCHES["n"] = l0
+            ent["state"] = "failed"
+            torch.cuda.synchronize()
+            return False
+        eng = self.model._engine
+        ent.update(state="graph", graph=g, loss=loss, index=index, launches=ops.LAUNCHES["n"] - l0, engine=eng,
+                   ws_gen=eng.ws_generation, ws=eng.ws)      # "engine" / "ws" keep what the graph points into alive
+        ops.LAUNCHES["n"] = l0
+        self.captures += 1
+        return True
+
+
 class AsyncLossReader:
     """Per-step loss read-back that does not drain the stream: ``push(loss)`` enqueues a 4-byte D2H copy into a pinned
     slot + an event right behind the step that produced ``loss`` and returns the value of the PREVIOUS push (whose
@@ -511,5 +714,84 @@ def evaluate(model, loader, device, tau=0.5):
     m = EvalMetrics(device, tau)
     for data in loader:
         eval_step(model, data.to(device), tau, m)
+    model.train(was_training)
+    return m.result()
+
+
+class _BucketedEval:
+    """Per-model state of ``evaluate_bucketed``: the metric sums (one device buffer the graphs add into) and the
+    padded buffers + forward/metrics graph of every bucket seen so far."""
+
+    def __init__(self, device, tau):
+        self.metrics = EvalMetrics(device, tau)
+        self.buckets = {}
+        self.capture_error = None
+
+
+@torch.no_grad()
+def evaluate_bucketed(model, loader, device, tau=0.5, max_graphs=32):
+    """``evaluate`` (same return) with every batch padded into its capacity bucket and the engine forward + metric sums
+    replayed from one CUDA graph per bucket (eager on the first visit, captured on the second; graphs persist across
+    calls on the same model, and a graph captured over an engine or workspace that has since been replaced is captured
+    again).  Buckets beyond ``max_graphs`` and failed captures run the padded forward eagerly; a batch
+    ``PaddedBatch`` cannot pad (per-pattern probabilities only) runs through ``eval_step``."""
+    was_training = model.training
+    model.eval()
+    device = torch.device(device)
+    if device.type == "cuda" and device.index is None:      # "cuda" -> "cuda:<current>": the state is kept per device
+        device = torch.device("cuda", torch.cuda.current_device())
+    st = model.__dict__.get("_bucketed_eval")
+    if st is None or st.metrics.acc.device != device or st.metrics.tau != float(tau):
+        st = model.__dict__["_bucketed_eval"] = _BucketedEval(device, tau)
+    m = st.metrics
+    m.reset()
+    eng = model.engine()
+    n_if, n_rpc = model.interface_embeds.num_embeddings, model.rpctype_embeds.num_embeddings
+
+    def run(buf):
+        from .index import build_index
+
+        x, cat_X, edge_index, edge_attr, pnn, probs, entry_id, batch = model_inputs(buf)
+        index = build_index(edge_index, x.size(0), edge_attr, n_if, n_rpc, check=False)
+        gpred, _ = eng.forward(x, cat_X, entry_id, probs, pnn, batch, index, False, live=buf.live)
+        _lib.call("pert_eval_metrics_live", _lib.ptr(buf.y), _lib.ptr(gpred), m.tau, buf.y.numel(),
+                  _lib.ptr(m.acc), _lib.ptr(buf.live), _lib.stream())
+        ops.LAUNCHES["n"] += 1
+        return gpred, index
+
+    with torch.cuda.device(device):
+        for data in loader:
+            data = data.to(device)
+            if not PaddedBatch.accepts(data):
+                eval_step(model, data, tau, m)
+                continue
+            N, E, B = _batch_sizes(data)
+            caps = bucket_caps(N, E, B)
+            key = caps + (int(data.edge_attr.size(1)),)
+            ent = st.buckets.get(key)
+            if ent is None:
+                ent = st.buckets[key] = {"buf": PaddedBatch(caps, data), "state": "new",
+                                         "eager": len(st.buckets) >= max_graphs}
+            buf = ent["buf"].fill(data)
+            m.count += B
+            eng._workspace(*caps)
+            if ent["state"] == "graph" and _stale(ent, eng):
+                _drop_graph(ent)
+            if ent["state"] == "ran-once" and not ent.get("eager"):
+                g = torch.cuda.CUDAGraph()
+                try:
+                    with torch.cuda.graph(g):
+                        out = run(buf)
+                    ent.update(state="graph", graph=g, out=out, engine=eng, ws_gen=eng.ws_generation, ws=eng.ws)
+                except Exception as e:  # noqa: BLE001 - this bucket stays eager
+                    st.capture_error = repr(e)
+                    torch.cuda.synchronize()
+                    ent["eager"] = True
+            if ent["state"] == "graph":
+                ent["graph"].replay()
+            else:
+                if ent["state"] == "new":
+                    ent["state"] = "ran-once"
+                run(buf)
     model.train(was_training)
     return m.result()

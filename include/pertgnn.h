@@ -50,7 +50,8 @@ extern "C" {
  * 2003: pert_span_graph_count / pert_span_graph_build.  2004: pert_linear_bwd_planes(_supported).
  * 2005: pert_model_forward takes dropout + dropout_state, pert_model_backward takes dropout; later, and additive (no
  * existing signature changed): pert_bn_linear_fwd_planes(_supported); pert_batch_pad, pert_model_forward_live,
- * pert_model_backward_live, pert_pinball_loss_live, pert_eval_metrics_live. */
+ * pert_model_backward_live, pert_pinball_loss_live, pert_eval_metrics_live; pert_tconv_fwd_c, pert_tconv_bwd_c,
+ * pert_model_width (the step engine accepts every hidden width 1..256). */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -124,6 +125,19 @@ int pert_tconv_bwd(const float* g, int ld_g, const float* q, const float* k, con
                    const int* csc_pos, const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha,
                    float* dq, float* dk, float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc,
                    int n_rpc, long long N, long long E, long long B_hint, int H, void* stream);
+/* The same two for a conv of logical width C run at a kernel width H >= C (1 <= C <= H, else PERT_ERR_BADARG): the
+ * planes, tables and outputs are [*, H] with columns [C, H) zero, and the logits are scaled by 1/sqrt(C) instead of
+ * 1/sqrt(H), so the first C columns are those of the width-C conv and the rest stay 0.  pert_tconv_fwd / _bwd are these
+ * with C = H. */
+int pert_tconv_fwd_c(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
+                     const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if, const float* t_rpc,
+                     float* out, int ld_out, float* alpha, int n_rpc, long long N, long long E, long long B_hint, int H,
+                     int C, void* stream);
+int pert_tconv_bwd_c(const float* g, int ld_g, const float* q, const float* k, const float* v, int ld,
+                     const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr,
+                     const int* csc_pos, const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha,
+                     float* dq, float* dk, float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc,
+                     int n_rpc, long long N, long long E, long long B_hint, int H, int C, void* stream);
 
 /* ---- dense linears (exact fp32) --------------------------------------------------------------------
  * Replace torch_geometric.nn.Linear / the lin_* of TransformerConv (model.py:26-55,105,110-112).
@@ -262,7 +276,14 @@ int pert_allreduce_adam(float* p, const float* g, float* m, float* v, long long 
  * the reference's own tensor shapes; PertModelDesc gives the offset (in floats, each 16-byte aligned) of every
  * tensor, named after the reference's state_dict keys.  Gradients go to a second flat buffer with the same
  * offsets and are ACCUMULATED (+=), like autograd.  The workspace holds packed operands, saved activations and
- * temporaries; its first pert_model_packed_bytes() bytes must be zero when first used (padding columns). */
+ * temporaries; its first pert_model_packed_bytes() bytes must be zero when first used (padding columns).
+ *
+ * Any hidden width 1 <= H <= 256 runs: the engine runs a model of width H at the internal width Hp =
+ * pert_model_width(H), the smallest attention-kernel width >= H (one of 4, 8, 16, 32, 64, 96, 128, 192, 256; Hp = H
+ * at those).  Every parameter is copied into zero-padded Hp-wide packs each step, and columns [H, Hp) of every
+ * activation and gradient stay exactly 0; the parameters, gradients and outputs are those of the width-H model (the
+ * attention logits are scaled by 1/sqrt(H)), at the cost of a width-Hp step.  Workspace sizes and the layouts below are
+ * at Hp. */
 #define PERT_MAX_CONVS 8
 #define PERT_MAX_CAT 4
 typedef struct PertModelDesc {
@@ -272,7 +293,7 @@ typedef struct PertModelDesc {
   int32_t n_cat;    /* len(cat_dims)                                                model.py:57-60 */
   int32_t cat_rows[PERT_MAX_CAT];
   int32_t n_entry, n_if, n_rpc; /* rows of entry_embeds / interface_embeds / rpctype_embeds  model.py:63-67 */
-  int32_t k0;       /* padded input width of conv 0: round_up(F + H, 8)                          */
+  int32_t k0;       /* padded input width of conv 0: round_up(F + Hp, 8), Hp = pert_model_width(H) */
   float bn_eps, bn_momentum;
   long long off_cat[PERT_MAX_CAT];                 /* cat_embedding.{i}.weight [rows,H] */
   long long off_entry, off_if, off_rpc;            /* *_embeds.weight                   */
@@ -287,14 +308,18 @@ typedef struct PertModelDesc {
   long long off_g2_w, off_g2_b;                    /* global_linear2 [1,H],[1]  */
 } PertModelDesc;
 
+/* Hp for a model of hidden width H (see above), PERT_ERR_UNSUPPORTED outside 1..256. */
+int pert_model_width(int H);
 long long pert_model_workspace_bytes(const PertModelDesc* desc, long long N, long long E, long long B);
 long long pert_model_packed_bytes(const PertModelDesc* desc);
 /* Test / debug aid: offset (in floats) inside the workspace of a saved activation of the last forward:
- * which = 0: input of conv `layer` (>= 1) = post-BatchNorm-ReLU activations [N,H]; which = 1: relu(global_linear1) [B,H].
+ * which = 0: input of conv `layer` (>= 1) = post-BatchNorm-ReLU activations [N,Hp]; which = 1: relu(global_linear1)
+ * [B,Hp] (Hp = pert_model_width(H); columns [H, Hp) are 0).
  * Lets a reference be differentiated on the same linear piece of the network (which ReLUs were active). */
 long long pert_model_workspace_offset(const PertModelDesc* desc, long long N, long long E, long long B, int which,
                                       int layer);
-/* bn_running: [n_convs-1][2][H] (running_mean | running_var), bn_nbt: [n_convs-1] int64 (either may be NULL in
+/* bn_running: [n_convs-1][2][Hp] (running_mean | running_var; the first H of each Hp are the model's, the others belong
+ * to padding columns, whose outputs are 0 whatever they hold, and only need to be finite and >= 0 for the variance), bn_nbt: [n_convs-1] int64 (either may be NULL in
  * training mode); index arrays from pert_build_index (built with edge_attr); probs/pnn [N] fp32.
  * Outputs: global_pred [B], local_pred [N] (NULL to skip). */
 /* Optional measurement probe: the engine records the two caller-created cudaEvent_t around ONE kernel family of ONE
@@ -323,12 +348,12 @@ int pert_model_forward(const PertModelDesc* desc, const float* params, float* bn
  * device memory, two int64 {seed, step}; a training forward with p > 0 reads it in stream order and adds 1 to step, so
  * a captured graph draws a new mask on every replay.  The mask is a pure function of (seed, step, layer, position):
  *   Philox4x32-10 (Random123), key = (seed & 0xffffffff, seed >> 32),
- *   counter = (g, l, step & 0xffffffff, step >> 32), g = row*(H/4) + col/4 (the float4 group), l = the conv whose
+ *   counter = (g, l, step & 0xffffffff, step >> 32), g = row*(Hp/4) + col/4 (the float4 group), l = the conv whose
  *   BatchNorm output is dropped (0 .. n_convs-2); output word j of the group decides column col + j.
  *   Element kept iff word >= T, T = floor(p * 2^32) in fp64 (p = 1: all dropped); kept values are multiplied by
  *   (float)(1 / (1 - p)), 0 at p = 1.
  * PERT_ERR_BADARG, before any CUDA call, when p is NaN or outside [0, 1], or when training with p > 0 and
- * dropout_state is NULL or N*H/4 >= 2^32.
+ * dropout_state is NULL or N*Hp/4 >= 2^32.
  *
  * Must follow pert_model_forward on the same workspace, with the same training flag and dropout (the backward applies
  * the 1/(1-p) factor; the mask is read back from the saved activations).  d_global [B], d_local [N] or NULL. */

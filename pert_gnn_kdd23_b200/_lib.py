@@ -31,6 +31,9 @@ SIGNATURES = {
     "pert_tconv_fwd": (I, [P, P, P, P, I, P, P, P, P, P, P, P, I, P, I, LL, LL, LL, I, P]),
     "pert_tconv_bwd": (I, [P, I, P, P, P, I, P, P, P, P, P, P, P, P, P, P, P, P, P, I, P, P, P, P, I, LL, LL, LL, I,
                            P]),
+    "pert_tconv_fwd_c": (I, [P, P, P, P, I, P, P, P, P, P, P, P, I, P, I, LL, LL, LL, I, I, P]),
+    "pert_tconv_bwd_c": (I, [P, I, P, P, P, I, P, P, P, P, P, P, P, P, P, P, P, P, P, I, P, P, P, P, I, LL, LL, LL, I,
+                             I, P]),
     "pert_gemm_nt": (I, [P, I, I, LL, P, I, P, P, I, I, LL, LL, I, I, I, I, P]),
     "pert_gemm_tn": (I, [P, I, I, LL, P, I, I, LL, P, I, P, LL, I, I, P]),
     "pert_colsum": (I, [P, I, I, LL, P, LL, I, P]),
@@ -68,6 +71,7 @@ SIGNATURES = {
     "pert_span_graph_count": (I, [P, LL, P, P, I, P, P, P]),
     "pert_span_graph_build": (I, [P, LL, LL, P, P, P, P, P, P, I, I, P, P, P, P, P, P]),
     # whole-model engine (first argument: const PertModelDesc*, see engine.py)
+    "pert_model_width": (I, [I]),
     "pert_model_workspace_bytes": (LL, [P, LL, LL, LL]),
     "pert_model_packed_bytes": (LL, [P]),
     "pert_model_workspace_offset": (LL, [P, LL, LL, LL, I, I]),

@@ -189,8 +189,11 @@ __global__ void k_unpack(float* __restrict__ grads, const float* __restrict__ pa
 
 // ------------------------------------------------------------------ fused global head (reference model.py: global_linear1 -> ReLU -> global_linear2)
 // HEAD_G graphs per CTA, one warp per graph.  z = [pool | entry_emb[entry_id]], h1 = relu(W1 z + b1), out = W2 h1 + b2.
-// W1 is staged in shared memory once per CTA (all loads in flight together): transposed [2H][H] for the forward
-// (lane = output feature, conflict free, no shuffles), row-major [H][2H] for the backward (lane = input column).
+// W1 is staged in shared memory (all loads in flight together): transposed [2H][ns] for the forward (lane = output
+// feature, conflict free, no shuffles), row-major [H][cs] for the backward (lane = input column).  Up to H = 128 one
+// stage holds all of W1 (ns = H, cs = 2H); above that 2H^2 floats do not fit, and the CTA stages W1 in slices of ns
+// output rows (forward) or cs input columns (backward) one after the other (head_slice).  Each output of a slice is
+// complete within it, so the sums are those of the single-stage kernel.
 constexpr int HEAD_G = 8;
 constexpr int HEAD_T = HEAD_G * 32;
 __global__ void __launch_bounds__(HEAD_T) k_head_fwd(const float* __restrict__ pool, const float* __restrict__ table,
@@ -198,31 +201,12 @@ __global__ void __launch_bounds__(HEAD_T) k_head_fwd(const float* __restrict__ p
                                                      const float* __restrict__ W1, const float* __restrict__ b1,
                                                      const float* __restrict__ W2, const float* __restrict__ b2,
                                                      float* __restrict__ z, float* __restrict__ h1,
-                                                     float* __restrict__ out, int B, int H, int* status) {
-  extern __shared__ float hs[];                       // W1t [2H][H] | z [HEAD_G][2H]
+                                                     float* __restrict__ out, int B, int H, int ns, int* status) {
+  extern __shared__ float hs[];                       // W1t slice [2H][ns] | z [HEAD_G][2H]
   float* w1t = hs;
-  float* zs_all = hs + (size_t)2 * H * H;
+  float* zs_all = hs + (size_t)2 * H * ns;
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int K2 = 2 * H, kq = K2 / 4;
-  // lanes along n: the global reads are 16-byte pieces of different rows (32 KB, L2 resident), the transposing
-  // shared-memory stores are conflict free
-  for (int base = 0; base < H * kq; base += 8 * HEAD_T) {
-    float4 v[8];
-#pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      const int x = base + u * HEAD_T + threadIdx.x;
-      v[u] = x < H * kq ? ldg4(W1 + (size_t)(x % H) * K2 + (x / H) * 4) : f4zero();
-    }
-#pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      const int x = base + u * HEAD_T + threadIdx.x;
-      if (x < H * kq) {
-        const int n = x % H, k = (x / H) * 4;
-        w1t[(k + 0) * H + n] = v[u].x; w1t[(k + 1) * H + n] = v[u].y;
-        w1t[(k + 2) * H + n] = v[u].z; w1t[(k + 3) * H + n] = v[u].w;
-      }
-    }
-  }
   const int b = blockIdx.x * HEAD_G + w;
   const bool act = b < B;
   float* zs = zs_all + (size_t)w * K2;
@@ -238,20 +222,44 @@ __global__ void __launch_bounds__(HEAD_T) k_head_fwd(const float* __restrict__ p
       z[(size_t)b * K2 + c] = v;
     }
   }
-  __syncthreads();
-  if (!act) return;
   float o = 0.f;
-  for (int n = lane; n < H; n += 32) {
-    float a0 = 0.f, a1 = 0.f;
-#pragma unroll 4
-    for (int k = 0; k < K2; k += 2) {
-      a0 = fmaf(w1t[k * H + n], zs[k], a0);
-      a1 = fmaf(w1t[(k + 1) * H + n], zs[k + 1], a1);
+  for (int n0 = 0; n0 < H; n0 += ns) {
+    if (n0 > 0) __syncthreads();                      // every warp is done with the previous slice
+    // lanes along n: the global reads are 16-byte pieces of different rows (L2 resident), the transposing
+    // shared-memory stores are conflict free
+    for (int base = 0; base < ns * kq; base += 8 * HEAD_T) {
+      float4 v[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int x = base + u * HEAD_T + threadIdx.x;
+        v[u] = x < ns * kq ? ldg4(W1 + (size_t)(n0 + x % ns) * K2 + (x / ns) * 4) : f4zero();
+      }
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int x = base + u * HEAD_T + threadIdx.x;
+        if (x < ns * kq) {
+          const int n = x % ns, k = (x / ns) * 4;
+          w1t[(k + 0) * ns + n] = v[u].x; w1t[(k + 1) * ns + n] = v[u].y;
+          w1t[(k + 2) * ns + n] = v[u].z; w1t[(k + 3) * ns + n] = v[u].w;
+        }
+      }
     }
-    const float hv = fmaxf(a0 + a1 + __ldg(b1 + n), 0.f);
-    h1[(size_t)b * H + n] = hv;
-    o = fmaf(hv, __ldg(W2 + n), o);
+    __syncthreads();
+    if (act) {
+      for (int n = lane; n < ns; n += 32) {
+        float a0 = 0.f, a1 = 0.f;
+#pragma unroll 4
+        for (int k = 0; k < K2; k += 2) {
+          a0 = fmaf(w1t[k * ns + n], zs[k], a0);
+          a1 = fmaf(w1t[(k + 1) * ns + n], zs[k + 1], a1);
+        }
+        const float hv = fmaxf(a0 + a1 + __ldg(b1 + n0 + n), 0.f);
+        h1[(size_t)b * H + n0 + n] = hv;
+        o = fmaf(hv, __ldg(W2 + n0 + n), o);
+      }
+    }
   }
+  if (!act) return;
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) o += __shfl_xor_sync(0xffffffffu, o, off);
   if (lane == 0) out[b] = o + __ldg(b2);
@@ -264,26 +272,14 @@ __global__ void __launch_bounds__(HEAD_T) k_head_bwd(const float* __restrict__ d
                                                      const float* __restrict__ W2, const int64_t* __restrict__ ids,
                                                      int n_rows, float* __restrict__ dpool, float* __restrict__ g_entry,
                                                      float* __restrict__ gW1, float* __restrict__ gb1,
-                                                     float* __restrict__ gW2, float* __restrict__ gb2, int B, int H) {
-  extern __shared__ float hs[];                       // W1 [H][2H] | z [HEAD_G][2H] | dh [HEAD_G][H]
-  const int K2 = 2 * H;
+                                                     float* __restrict__ gW2, float* __restrict__ gb2, int B, int H,
+                                                     int cs) {
+  extern __shared__ float hs[];                       // W1 slice [H][cs] | z [HEAD_G][2H] | dh [HEAD_G][H]
+  const int K2 = 2 * H, cq = cs / 4;
   float* w1 = hs;
-  float* zs_all = hs + (size_t)H * K2;
+  float* zs_all = hs + (size_t)H * cs;
   float* dh_all = zs_all + (size_t)HEAD_G * K2;
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int base = 0; base < H * K2 / 4; base += 8 * HEAD_T) {
-    float4 v[8];
-#pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      const int x = base + u * HEAD_T + threadIdx.x;
-      v[u] = x < H * K2 / 4 ? ldg4(W1 + (size_t)x * 4) : f4zero();
-    }
-#pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      const int x = base + u * HEAD_T + threadIdx.x;
-      if (x < H * K2 / 4) st4(w1 + (size_t)x * 4, v[u]);
-    }
-  }
   const int b = blockIdx.x * HEAD_G + w;
   const bool act = b < B;
   float* zs = zs_all + (size_t)w * K2;
@@ -294,22 +290,39 @@ __global__ void __launch_bounds__(HEAD_T) k_head_bwd(const float* __restrict__ d
     const float hv = act ? h1[(size_t)b * H + n] : 0.f;
     dh[n] = hv > 0.f ? d * __ldg(W2 + n) : 0.f;
   }
-  __syncthreads();
-  if (act) {
-    int64_t r = ids[b];
-    if (r < 0 || r >= n_rows) r = 0;                  // (the forward pass already raised the status flag)
-    for (int c = lane; c < K2; c += 32) {
-      float a0 = 0.f, a1 = 0.f;
-#pragma unroll 4
-      for (int n = 0; n < H; n += 2) {
-        a0 = fmaf(dh[n], w1[n * K2 + c], a0);
-        a1 = fmaf(dh[n + 1], w1[(n + 1) * K2 + c], a1);
+  int64_t r = act ? ids[b] : 0;
+  if (r < 0 || r >= n_rows) r = 0;                    // (the forward pass already raised the status flag)
+  for (int c0 = 0; c0 < K2; c0 += cs) {
+    if (c0 > 0) __syncthreads();                      // every warp is done with the previous slice
+    for (int base = 0; base < H * cq; base += 8 * HEAD_T) {
+      float4 v[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int x = base + u * HEAD_T + threadIdx.x;
+        v[u] = x < H * cq ? ldg4(W1 + (size_t)(x / cq) * K2 + c0 + (x % cq) * 4) : f4zero();
       }
-      const float acc = a0 + a1;
-      if (c < H) {
-        if (dpool) dpool[(size_t)b * H + c] = acc;
-      } else {
-        atomicAdd(g_entry + (size_t)r * H + (c - H), acc);
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int x = base + u * HEAD_T + threadIdx.x;
+        if (x < H * cq) st4(w1 + (size_t)x * 4, v[u]);
+      }
+    }
+    __syncthreads();
+    if (act) {
+      for (int c = lane; c < cs; c += 32) {
+        float a0 = 0.f, a1 = 0.f;
+#pragma unroll 4
+        for (int n = 0; n < H; n += 2) {
+          a0 = fmaf(dh[n], w1[n * cs + c], a0);
+          a1 = fmaf(dh[n + 1], w1[(n + 1) * cs + c], a1);
+        }
+        const float acc = a0 + a1;
+        const int col = c0 + c;
+        if (col < H) {
+          if (dpool) dpool[(size_t)b * H + col] = acc;
+        } else {
+          atomicAdd(g_entry + (size_t)r * H + (col - H), acc);
+        }
       }
     }
   }
@@ -342,17 +355,60 @@ __global__ void __launch_bounds__(HEAD_T) k_head_bwd(const float* __restrict__ d
   }
 }
 
+// Widest slice of W1 -- all of it (`full` rows or columns), halved while it does not fit -- whose stage of per_unit
+// floats per row / column plus the `fixed` per-warp floats stays within the head's shared-memory budget.
+constexpr size_t HEAD_SMEM_MAX = 200 * 1024;          // below the 227 KB a CTA may opt in to on sm_90
+int head_slice(int full, size_t per_unit, size_t fixed) {
+  int s = full;
+  while (s % 8 == 0 && (per_unit * s + fixed) * sizeof(float) > HEAD_SMEM_MAX) s /= 2;
+  return s;
+}
+int head_smem(const void* kernel, size_t bytes) {
+  if (bytes <= 48 * 1024) return PERT_OK;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  return e == cudaSuccess ? PERT_OK : (int)e;
+}
+
 
 inline long long al64(long long n) { return (n + 63) / 64 * 64; }
 
+// The model tensors the kernels read besides the conv packs, each with rows of Hp floats (global_linear1.weight: 2 Hp,
+// its [pool | entry] column blocks at 0 and Hp).  At Hp = H they are the reference's tensors in the flat buffer itself
+// (flat_tensors); at Hp > H zero-padded copies in the workspace.
+struct Tensors {
+  float *cat[PERT_MAX_CAT], *entry, *iface, *rpc;
+  float *bn_g[PERT_MAX_CONVS], *bn_b[PERT_MAX_CONVS];
+  float *local_w, *g1_w, *g1_b, *g2_w;
+};
+Tensors flat_tensors(const PertModelDesc* d, float* flat) {
+  Tensors t;
+  memset(&t, 0, sizeof(t));
+  for (int i = 0; i < d->n_cat; ++i) t.cat[i] = flat + d->off_cat[i];
+  t.entry = flat + d->off_entry;
+  t.iface = flat + d->off_if;
+  t.rpc = flat + d->off_rpc;
+  for (int l = 0; l + 1 < d->n_convs; ++l) {
+    t.bn_g[l] = flat + d->off_bn_g[l];
+    t.bn_b[l] = flat + d->off_bn_b[l];
+  }
+  t.local_w = flat + d->off_local_w;
+  t.g1_w = flat + d->off_g1_w;
+  t.g1_b = flat + d->off_g1_b;
+  t.g2_w = flat + d->off_g2_w;
+  return t;
+}
+
 struct Ws {
+  int Hp;  // internal width (pert_model_width): every kernel runs at Hp, columns [H, Hp) are zero
   // packed parameters (zero-initialised region: pads must stay 0)
   float *w4[PERT_MAX_CONVS], *b4[PERT_MAX_CONVS], *w4t[PERT_MAX_CONVS];
   float *weA[PERT_MAX_CONVS], *weB[PERT_MAX_CONVS], *weAt[PERT_MAX_CONVS], *weBt[PERT_MAX_CONVS];
+  Tensors pp;      // Hp > H only: padded copies of the other parameters
   // packed gradients + table gradients (zeroed at the start of every backward, one memset)
   float* gzero_begin;
   float *dw4[PERT_MAX_CONVS], *db4[PERT_MAX_CONVS], *dweA[PERT_MAX_CONVS], *dweB[PERT_MAX_CONVS];
   float *dt_if[PERT_MAX_CONVS], *dt_rpc[PERT_MAX_CONVS];
+  Tensors pg;      // Hp > H only: their gradients, unpacked like the conv packs
   float* gzero_end;
   // forward state
   float *t_if[PERT_MAX_CONVS], *t_rpc[PERT_MAX_CONVS];
@@ -367,7 +423,14 @@ struct Ws {
   long long packed_floats;
 };
 
-int k_of(const PertModelDesc* d, int l) { return l == 0 ? d->k0 : d->H; }
+// smallest width of the attention kernels >= H (pert_tconv_supported_width), PERT_ERR_UNSUPPORTED outside 1..256
+int model_width(int H) {
+  for (int w = H < 1 ? 257 : H; w <= 256; ++w)
+    if (pert_tconv_supported_width(w)) return w;
+  return PERT_ERR_UNSUPPORTED;
+}
+
+int k_of(const PertModelDesc* d, const Ws& w, int l) { return l == 0 ? d->k0 : w.Hp; }
 
 Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* base) {
   Ws w;
@@ -378,9 +441,26 @@ Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* b
     off += al64(n > 0 ? n : 1);
     return p;
   };
-  const int H = d->H, L = d->n_convs;
+  auto take_tensors = [&](Tensors& t) {
+    const long long Hp = w.Hp;
+    for (int i = 0; i < d->n_cat; ++i) t.cat[i] = take(d->cat_rows[i] * Hp);
+    t.entry = take(d->n_entry * Hp);
+    t.iface = take(d->n_if * Hp);
+    t.rpc = take(d->n_rpc * Hp);
+    for (int l = 0; l + 1 < d->n_convs; ++l) {
+      t.bn_g[l] = take(Hp);
+      t.bn_b[l] = take(Hp);
+    }
+    t.local_w = take(Hp);
+    t.g1_w = take(2 * Hp * Hp);
+    t.g1_b = take(Hp);
+    t.g2_w = take(Hp);
+  };
+  w.Hp = model_width(d->H);
+  const bool padded = w.Hp != d->H;
+  const int H = w.Hp, L = d->n_convs;
   for (int l = 0; l < L; ++l) {
-    int K = k_of(d, l);
+    int K = k_of(d, w, l);
     w.w4[l] = take(4LL * H * K);
     w.b4[l] = take(4LL * H);
     w.w4t[l] = take(4LL * H * K);
@@ -389,10 +469,11 @@ Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* b
     w.weAt[l] = take((long long)H * H);
     w.weBt[l] = take((long long)H * H);
   }
+  if (padded) take_tensors(w.pp);
   w.packed_floats = off;
   w.gzero_begin = base ? base + off : nullptr;
   for (int l = 0; l < L; ++l) {
-    int K = k_of(d, l);
+    int K = k_of(d, w, l);
     w.dw4[l] = take(4LL * H * K);
     w.db4[l] = take(4LL * H);
     w.dweA[l] = take((long long)H * H);
@@ -400,9 +481,10 @@ Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* b
     w.dt_if[l] = take((long long)d->n_if * H);
     w.dt_rpc[l] = take((long long)d->n_rpc * H);
   }
+  if (padded) take_tensors(w.pg);
   w.gzero_end = base ? base + off : nullptr;
   for (int l = 0; l < L; ++l) {
-    int K = k_of(d, l);
+    int K = k_of(d, w, l);
     w.t_if[l] = take((long long)d->n_if * H);
     w.t_rpc[l] = take((long long)d->n_rpc * H);
     if (l == 0) w.x[l] = take(N * K);
@@ -432,10 +514,11 @@ Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* b
 }
 
 // segment list of conv layer l: weights -> W4 / W4^T (conv 0: columns permuted to [emb | x | pad]), biases,
-// lin_edge halves and their transposes
+// lin_edge halves and their transposes.  Every block lands at its place in the Hp-wide packs; rows and columns
+// [H, Hp) are never written.
 constexpr int SEGS_PER_LAYER_MAX = 24;
 void append_layer_segs(SegList& S, const PertModelDesc* d, const Ws& w, float* base, int l) {
-  const int H = d->H, F = d->F, K = k_of(d, l);
+  const int H = d->H, Hp = w.Hp, F = d->F, K = k_of(d, w, l);
   const int Din = (l == 0) ? F + H : H;
   auto add = [&](long long src, float* dst, int rows, int cols, int src_ld, int dst_ld, int tr) {
     Seg& s = S.s[S.count++];
@@ -445,24 +528,24 @@ void append_layer_segs(SegList& S, const PertModelDesc* d, const Ws& w, float* b
   const long long* wq[4] = {&d->off_wq[l], &d->off_wk[l], &d->off_wv[l], &d->off_ws[l]};
   const long long* bq[4] = {&d->off_bq[l], &d->off_bk[l], &d->off_bv[l], &d->off_bs[l]};
   for (int p = 0; p < 4; ++p) {
-    float* dstw = w.w4[l] + (size_t)p * H * K;  // rows p*H..
-    float* dstt = w.w4t[l] + (size_t)p * H;     // W4^T [K, 4H]: column block p
+    float* dstw = w.w4[l] + (size_t)p * Hp * K;  // rows p*Hp..
+    float* dstt = w.w4t[l] + (size_t)p * Hp;     // W4^T [K, 4Hp]: column block p
     if (l == 0) {
-      // reference input order [x(F) | emb(H)] -> internal [emb(H) | x(F) | pad]
+      // reference input order [x(F) | emb(H)] -> internal [emb(Hp) | x(F) | pad]
       add(*wq[p] + F, dstw, H, H, Din, K, 0);          // emb columns -> cols 0..H
-      add(*wq[p], dstw + H, H, F, Din, K, 0);          // x columns   -> cols H..H+F
-      add(*wq[p] + F, dstt, H, H, Din, 4 * H, 1);
-      add(*wq[p], dstt + (size_t)H * 4 * H, H, F, Din, 4 * H, 1);
+      add(*wq[p], dstw + Hp, H, F, Din, K, 0);         // x columns   -> cols Hp..Hp+F
+      add(*wq[p] + F, dstt, H, H, Din, 4 * Hp, 1);
+      add(*wq[p], dstt + (size_t)Hp * 4 * Hp, H, F, Din, 4 * Hp, 1);
     } else {
       add(*wq[p], dstw, H, H, Din, K, 0);
-      add(*wq[p], dstt, H, H, Din, 4 * H, 1);
+      add(*wq[p], dstt, H, H, Din, 4 * Hp, 1);
     }
-    add(*bq[p], w.b4[l] + (size_t)p * H, 1, H, H, H, 0);
+    add(*bq[p], w.b4[l] + (size_t)p * Hp, 1, H, H, Hp, 0);
   }
-  add(d->off_we[l], w.weA[l], H, H, 2 * H, H, 0);
-  add(d->off_we[l] + H, w.weB[l], H, H, 2 * H, H, 0);
-  add(d->off_we[l], w.weAt[l], H, H, 2 * H, H, 1);
-  add(d->off_we[l] + H, w.weBt[l], H, H, 2 * H, H, 1);
+  add(d->off_we[l], w.weA[l], H, H, 2 * H, Hp, 0);
+  add(d->off_we[l] + H, w.weB[l], H, H, 2 * H, Hp, 0);
+  add(d->off_we[l], w.weAt[l], H, H, 2 * H, Hp, 1);
+  add(d->off_we[l] + H, w.weBt[l], H, H, 2 * H, Hp, 1);
 }
 // same list but pointing at the packed-gradient buffers (for k_unpack)
 void append_layer_grad_segs(SegList& S, const PertModelDesc* d, const Ws& w, float* base, int l) {
@@ -473,12 +556,35 @@ void append_layer_grad_segs(SegList& S, const PertModelDesc* d, const Ws& w, flo
     Seg& s = S.s[i];
     if (s.transpose) continue;
     float* p = base + s.dst;
-    const int H = d->H, K = k_of(d, l);
-    if (p >= w.w4[l] && p < w.w4[l] + 4LL * H * K) s.dst = (w.dw4[l] + (p - w.w4[l])) - base;
-    else if (p >= w.b4[l] && p < w.b4[l] + 4LL * H) s.dst = (w.db4[l] + (p - w.b4[l])) - base;
+    const int Hp = w.Hp, K = k_of(d, w, l);
+    if (p >= w.w4[l] && p < w.w4[l] + 4LL * Hp * K) s.dst = (w.dw4[l] + (p - w.w4[l])) - base;
+    else if (p >= w.b4[l] && p < w.b4[l] + 4LL * Hp) s.dst = (w.db4[l] + (p - w.b4[l])) - base;
     else if (p == w.weA[l]) s.dst = w.dweA[l] - base;
     else if (p == w.weB[l]) s.dst = w.dweB[l] - base;
   }
+}
+// Hp > H: segment list of the other model tensors (Tensors) -> their zero-padded copies t (w.pp to pack the
+// parameters, w.pg to unpack the gradients); one launch, at most 4 + 3 + 2 * 7 + 5 segments
+void append_tensor_segs(SegList& S, const PertModelDesc* d, const Tensors& t, int Hp, float* base) {
+  const int H = d->H;
+  auto add = [&](long long src, float* dst, int rows, int src_ld, int dst_ld) {
+    Seg& s = S.s[S.count++];
+    s.src = src; s.dst = dst - base; s.rows = rows; s.cols = H; s.src_ld = src_ld; s.dst_ld = dst_ld;
+    s.transpose = 0;
+  };
+  for (int i = 0; i < d->n_cat; ++i) add(d->off_cat[i], t.cat[i], d->cat_rows[i], H, Hp);
+  add(d->off_entry, t.entry, d->n_entry, H, Hp);
+  add(d->off_if, t.iface, d->n_if, H, Hp);
+  add(d->off_rpc, t.rpc, d->n_rpc, H, Hp);
+  for (int l = 0; l + 1 < d->n_convs; ++l) {
+    add(d->off_bn_g[l], t.bn_g[l], 1, H, Hp);
+    add(d->off_bn_b[l], t.bn_b[l], 1, H, Hp);
+  }
+  add(d->off_local_w, t.local_w, 1, H, Hp);
+  add(d->off_g1_w, t.g1_w, H, 2 * H, 2 * Hp);          // pool columns  -> [0, H)
+  add(d->off_g1_w + H, t.g1_w + Hp, H, 2 * H, 2 * Hp); // entry columns -> [Hp, Hp + H)
+  add(d->off_g1_b, t.g1_b, 1, H, Hp);
+  add(d->off_g2_w, t.g2_w, 1, H, Hp);
 }
 
 // Auxiliary stream for the few places where independent small kernels can run beside the main chain (input prologue
@@ -549,15 +655,17 @@ int aux_join(AuxStream* a, cudaStream_t st) {
 int check_desc(const PertModelDesc* d) {
   if (!d) return PERT_ERR_BADARG;
   if (d->n_convs < 2 || d->n_convs > PERT_MAX_CONVS || d->n_cat < 1 || d->n_cat > PERT_MAX_CAT) return PERT_ERR_BADARG;
-  if (d->H <= 0 || d->F <= 0 || d->k0 < d->F + d->H || d->k0 % 4) return PERT_ERR_BADARG;
-  if (!pert_tconv_supported_width(d->H)) return PERT_ERR_UNSUPPORTED;
+  if (d->H <= 0 || d->F <= 0 || d->k0 % 4) return PERT_ERR_BADARG;
+  const int Hp = model_width(d->H);
+  if (Hp < 0) return PERT_ERR_UNSUPPORTED;
+  if (d->k0 < d->F + Hp) return PERT_ERR_BADARG;
   return PERT_OK;
 }
 // dropout p in [0, 1] (NaN rejected); a training forward with p > 0 needs the {seed, step} state, and its float4 groups
-// N*H/4 must fit the 32-bit counter word of the mask
+// N*Hp/4 must fit the 32-bit counter word of the mask
 int check_dropout(const PertModelDesc* d, long long N, int training, float p, const long long* state) {
   if (!(p >= 0.f && p <= 1.f)) return PERT_ERR_BADARG;
-  if (training && p > 0.f && (!state || N * (d->H / 4) >= (1LL << 32))) return PERT_ERR_BADARG;
+  if (training && p > 0.f && (!state || N * (model_width(d->H) / 4) >= (1LL << 32))) return PERT_ERR_BADARG;
   return PERT_OK;
 }
 
@@ -599,6 +707,7 @@ long long pert_model_workspace_offset(const PertModelDesc* d, long long N, long 
   if (which == 1) return w.h1 - base;
   return PERT_ERR_BADARG;
 }
+int pert_model_width(int H) { return model_width(H); }
 long long pert_model_packed_bytes(const PertModelDesc* d) {
   if (check_desc(d)) return PERT_ERR_BADARG;
   Ws w = carve(d, 0, 0, 0, nullptr);
@@ -637,8 +746,17 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
   Ws w = carve(d, N, E, B, base);
   if (workspace_bytes < w.total * 4) return PERT_ERR_BADARG;
   cudaStream_t st = (cudaStream_t)stream;
-  const int H = d->H, L = d->n_convs;
-  // the input prologue (2.) does not depend on the packed parameters: it runs on the auxiliary stream beside 1.
+  const int H = w.Hp, L = d->n_convs;
+  // Hp > H: the zero-padded copies of the embeddings, BatchNorm and head parameters first (the prologue reads them)
+  const bool padded = H != d->H;
+  const Tensors P = padded ? w.pp : flat_tensors(d, const_cast<float*>(params));
+  if (padded) {
+    SegList S;
+    S.count = 0;
+    append_tensor_segs(S, d, w.pp, H, base);
+    k_pack<<<dim3(32, S.count), 256, 0, st>>>(params, base, S, nullptr, nullptr);
+  }
+  // the input prologue (2.) does not depend on the packed conv parameters: it runs on the auxiliary stream beside 1.
   AuxStream* ax = aux_stream();
   const bool forked = aux_fork(ax, st);
   cudaStream_t s2 = forked ? ax->s : st;
@@ -662,8 +780,8 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
     gb.count = 0;
     for (int l = 0; l < L; ++l) {
       // T_if = if_emb . WeA^T ;  T_rpc = rpc_emb . WeB^T      (B(k,n) = WeA[n,k])
-      gb.p[gb.count++] = sg(params + d->off_if, H, 1, w.weA[l], 1, H, nullptr, w.t_if[l], H, d->n_if, H, H);
-      gb.p[gb.count++] = sg(params + d->off_rpc, H, 1, w.weB[l], 1, H, nullptr, w.t_rpc[l], H, d->n_rpc, H, H);
+      gb.p[gb.count++] = sg(P.iface, H, 1, w.weA[l], 1, H, nullptr, w.t_if[l], H, d->n_if, H, H);
+      gb.p[gb.count++] = sg(P.rpc, H, 1, w.weB[l], 1, H, nullptr, w.t_rpc[l], H, d->n_rpc, H, H);
       if (gb.count + 2 > SG_MAX || l == L - 1) {
         launch_small(gb, st);
         gb.count = 0;
@@ -672,7 +790,7 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
   }
   // 2. prologue: X0 = [sum_i cat_emb_i[cat_X[:,i]] | x | 0]
   for (int i = 0; i < d->n_cat; ++i)
-    TRY(pert_embedding_fwd(params + d->off_cat[i], d->cat_rows[i], cat_X + i, d->n_cat, w.x[0], d->k0, N, H, i > 0,
+    TRY(pert_embedding_fwd(P.cat[i], d->cat_rows[i], cat_X + i, d->n_cat, w.x[0], d->k0, N, H, i > 0,
                            status, s2));
   TRY(pert_copy_cols(x, d->F, w.x[0], d->k0, H, N, s2));
   // graph boundaries of the batch for the tile list (needs only the batch vector): beside the prologue as well
@@ -688,12 +806,12 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
   bool have_tiles = false;
   int prev_stats_fused = 0;
   for (int l = 0; l < L; ++l) {
-    const int K = k_of(d, l);
+    const int K = k_of(d, w, l);
     PROBE_START(3, l);
     if (l > 0 && bn_in_linear) {
       float* rm = bn_running ? bn_running + (size_t)(l - 1) * 2 * H : nullptr;
       float* rv = rm ? rm + H : nullptr;
-      TRY(pert_bn_linear_fwd_planes_ex(w.out[l - 1], H, 1, params + d->off_bn_g[l - 1], params + d->off_bn_b[l - 1],
+      TRY(pert_bn_linear_fwd_planes_ex(w.out[l - 1], H, 1, P.bn_g[l - 1], P.bn_b[l - 1],
                                        rm, rv, (training && bn_nbt) ? bn_nbt + l - 1 : nullptr, d->bn_eps,
                                        d->bn_momentum, training, w.bn_stats[l - 1], w.bn_stats[l - 1] + H, w.x[l], H,
                                        w.bn_part, pert_bn_workspace_bytes(N, H), prev_stats_fused,
@@ -732,31 +850,29 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
     }
     PROBE_START(1, l);
     TRY(pert_tconv_fwd_stats(pl, pl + N * H, pl + 2 * N * H, pl + 3 * N * H, H, rowptr, csr_src, csr_if, csr_rpc,
-                             w.t_if[l], w.t_rpc[l], w.out[l], H, w.alpha[l], d->n_rpc, N, E, B, H, bn_acc, live,
+                             w.t_if[l], w.t_rpc[l], w.out[l], H, w.alpha[l], d->n_rpc, N, E, B, H, d->H, bn_acc, live,
                              &stats_fused, have_tiles ? &tiles : nullptr, st));
     PROBE_STOP(1, l);
     prev_stats_fused = stats_fused;
     if (l + 1 < L && !bn_in_linear) {
       float* rm = bn_running ? bn_running + (size_t)l * 2 * H : nullptr;
       float* rv = rm ? rm + H : nullptr;
-      TRY(pert_bn_fwd_ex(w.out[l], H, params + d->off_bn_g[l], params + d->off_bn_b[l], rm, rv,
+      TRY(pert_bn_fwd_ex(w.out[l], H, P.bn_g[l], P.bn_b[l], rm, rv,
                          (training && bn_nbt) ? bn_nbt + l : nullptr, d->bn_eps, d->bn_momentum, training, 1,
                          w.bn_stats[l], w.bn_stats[l] + H, w.x[l + 1], H, N, H, w.bn_part,
                          pert_bn_workspace_bytes(N, H), stats_fused, drop ? dropout : 0.f, w.drop_ctr, l, live, st));
     }
   }
   // 4. local head + weighted add-pool, global head
-  TRY(pert_pool_fwd(w.out[L - 1], H, probs, pnn, batch, params + d->off_local_w, params + d->off_local_b, local_pred,
-                    w.pool, N, B, H, status, st));
+  TRY(pert_pool_fwd(w.out[L - 1], H, probs, pnn, batch, P.local_w, params + d->off_local_b, local_pred, w.pool, N, B,
+                    H, status, st));
   if (B > 0) {
-    const size_t hsm = ((size_t)2 * H * H + (size_t)HEAD_G * 2 * H) * sizeof(float);
-    if (hsm > 48 * 1024) {
-      cudaError_t he = cudaFuncSetAttribute(k_head_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsm);
-      if (he != cudaSuccess) return (int)he;
-    }
+    const int ns = head_slice(H, 2 * H, (size_t)HEAD_G * 2 * H);
+    const size_t hsm = ((size_t)2 * H * ns + (size_t)HEAD_G * 2 * H) * sizeof(float);
+    TRY(head_smem((const void*)k_head_fwd, hsm));
     k_head_fwd<<<pert_cdiv(B, HEAD_G), HEAD_T, hsm, st>>>(
-        w.pool, params + d->off_entry, d->n_entry, entry_id, params + d->off_g1_w, params + d->off_g1_b,
-        params + d->off_g2_w, params + d->off_g2_b, w.z, w.h1, global_pred, (int)B, H, status);
+        w.pool, P.entry, d->n_entry, entry_id, P.g1_w, P.g1_b, P.g2_w, params + d->off_g2_b, w.z, w.h1, global_pred,
+        (int)B, H, ns, status);
   }
   PERT_LAUNCH_CHECK();
   return PERT_OK;
@@ -796,28 +912,28 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
   Ws w = carve(d, N, E, B, base);
   if (workspace_bytes < w.total * 4) return PERT_ERR_BADARG;
   cudaStream_t st = (cudaStream_t)stream;
-  const int H = d->H, L = d->n_convs;
+  const int H = w.Hp, L = d->n_convs;
+  const bool padded = H != d->H;
+  const Tensors P = padded ? w.pp : flat_tensors(d, const_cast<float*>(params));
+  const Tensors G = padded ? w.pg : flat_tensors(d, grads);
   cudaError_t e = cudaMemsetAsync(w.gzero_begin, 0, (size_t)(w.gzero_end - w.gzero_begin) * sizeof(float), st);
   if (e != cudaSuccess) return (int)e;
   // ---- global head backward
   if (B > 0) {
-    const size_t hsm = ((size_t)2 * H * H + (size_t)HEAD_G * 3 * H) * sizeof(float);
-    if (hsm > 48 * 1024) {
-      cudaError_t he = cudaFuncSetAttribute(k_head_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hsm);
-      if (he != cudaSuccess) return (int)he;
-    }
+    const int cs = head_slice(2 * H, H, (size_t)HEAD_G * 3 * H);
+    const size_t hsm = ((size_t)H * cs + (size_t)HEAD_G * 3 * H) * sizeof(float);
+    TRY(head_smem((const void*)k_head_bwd, hsm));
     k_head_bwd<<<pert_cdiv(B, HEAD_G), HEAD_T, hsm, st>>>(
-        d_global, w.z, w.h1, params + d->off_g1_w, params + d->off_g2_w, entry_id, d->n_entry, w.dpool,
-        grads + d->off_entry, grads + d->off_g1_w, grads + d->off_g1_b, grads + d->off_g2_w, grads + d->off_g2_b,
-        (int)B, H);
+        d_global, w.z, w.h1, P.g1_w, P.g2_w, entry_id, d->n_entry, w.dpool, G.entry, G.g1_w, G.g1_b, G.g2_w,
+        grads + d->off_g2_b, (int)B, H, cs);
   }
   // ---- pool / local head backward: g = dL/d out[L-1], written straight into the skip plane of dplanes
   float* dq = w.dplanes;
   float* dk = dq + N * H;
   float* dv = dk + N * H;
   float* dskip = dv + N * H;
-  TRY(pert_pool_bwd(B > 0 ? w.dpool : nullptr, d_local, w.out[L - 1], H, probs, pnn, batch, params + d->off_local_w,
-                    dskip, H, grads + d->off_local_w, grads + d->off_local_b, N, B, H, st));
+  TRY(pert_pool_bwd(B > 0 ? w.dpool : nullptr, d_local, w.out[L - 1], H, probs, pnn, batch, P.local_w, dskip, H,
+                    G.local_w, grads + d->off_local_b, N, B, H, st));
   // ---- edge tables: dWeA = dT_if^T . if_emb ; d if_emb += dT_if . WeA   (and the rpc halves), all layers grouped.
   // They depend only on the conv backward passes (dT tables), so they run on the auxiliary stream beside the conv-0
   // GEMMs and the embedding scatters; the unpack at the end waits for them.
@@ -826,12 +942,12 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
     gb.count = 0;
     for (int l = 0; l < L; ++l) {
       int ks_if = d->n_if >= 512 ? 8 : 1, ks_rpc = 1;
-      gb.p[gb.count++] = sg(w.dt_if[l], 1, H, params + d->off_if, H, 1, nullptr, w.dweA[l], H, H, H, d->n_if, 0, 1, ks_if);
-      gb.p[gb.count++] = sg(w.dt_rpc[l], 1, H, params + d->off_rpc, H, 1, nullptr, w.dweB[l], H, H, H, d->n_rpc, 0, 1, ks_rpc);
+      gb.p[gb.count++] = sg(w.dt_if[l], 1, H, P.iface, H, 1, nullptr, w.dweA[l], H, H, H, d->n_if, 0, 1, ks_if);
+      gb.p[gb.count++] = sg(w.dt_rpc[l], 1, H, P.rpc, H, 1, nullptr, w.dweB[l], H, H, H, d->n_rpc, 0, 1, ks_rpc);
       // every layer adds into the same embedding-gradient rows: atomic accumulation, all layers in one launch
-      gb.p[gb.count] = sg(w.dt_if[l], H, 1, w.weA[l], H, 1, nullptr, grads + d->off_if, H, d->n_if, H, H, 0, 1);
+      gb.p[gb.count] = sg(w.dt_if[l], H, 1, w.weA[l], H, 1, nullptr, G.iface, H, d->n_if, H, H, 0, 1);
       gb.p[gb.count++].atomic = 1;
-      gb.p[gb.count] = sg(w.dt_rpc[l], H, 1, w.weB[l], H, 1, nullptr, grads + d->off_rpc, H, d->n_rpc, H, H, 0, 1);
+      gb.p[gb.count] = sg(w.dt_rpc[l], H, 1, w.weB[l], H, 1, nullptr, G.rpc, H, d->n_rpc, H, H, 0, 1);
       gb.p[gb.count++].atomic = 1;
       if (gb.count + 4 > SG_MAX || l == 0 + L - 1) {
         launch_small(gb, ts);
@@ -845,12 +961,12 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
   const bool have_tiles = tiles_enabled() && E > 0 && !pert_tile_fixed_ok(N, E, B, H, d->n_rpc) &&
                           pert_tile_list_view(N, E, B, H, d->n_rpc, w.tiles, &tiles) == PERT_OK;
   for (int l = L - 1; l >= 0; --l) {
-    const int K = k_of(d, l);
+    const int K = k_of(d, w, l);
     float* pl = w.planes[l];
     PROBE_START(2, l);
     TRY(pert_tconv_bwd_tiles(dskip, H, pl, pl + N * H, pl + 2 * N * H, H, rowptr, csr_src, csr_if, csr_rpc, colptr,
                              csc_pos, csc_dst, w.t_if[l], w.t_rpc[l], w.alpha[l], dq, dk, dv, H, w.dsp, w.rpc_ws,
-                             w.dt_if[l], w.dt_rpc[l], d->n_rpc, N, E, B, H, have_tiles ? &tiles : nullptr, st));
+                             w.dt_if[l], w.dt_rpc[l], d->n_rpc, N, E, B, H, d->H, have_tiles ? &tiles : nullptr, st));
     PROBE_STOP(2, l);
     if (l == 0) {                       // every dT table is complete now
       forked = aux_fork(ax, st);
@@ -875,8 +991,8 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
     if (l > 0) {
       // BN(+ReLU) backward of layer l-1: dx (grad wrt x[l]) -> g of conv l-1, into the skip plane
       TRY(pert_bn_bwd_ex(w.dx, K, w.x[l], H, w.out[l - 1], H, w.bn_stats[l - 1], w.bn_stats[l - 1] + H,
-                         params + d->off_bn_g[l - 1], 1, relu_scale, training, dskip, H, grads + d->off_bn_g[l - 1],
-                         grads + d->off_bn_b[l - 1], w.sums, N, H, live, st));
+                         P.bn_g[l - 1], 1, relu_scale, training, dskip, H, G.bn_g[l - 1], G.bn_b[l - 1], w.sums, N, H,
+                         live, st));
     }
   }
   if (forked) TRY(aux_join(ax, st));
@@ -884,7 +1000,7 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
   // ---- categorical embedding gradients from dX0[:, 0:H] (auxiliary stream) beside the gradient unpack (main stream)
   const bool forked2 = aux_fork(ax, st);
   for (int i = 0; i < d->n_cat; ++i)
-    TRY(pert_embedding_bwd(w.dx, d->k0, cat_X + i, d->n_cat, grads + d->off_cat[i], d->cat_rows[i], N, H,
+    TRY(pert_embedding_bwd(w.dx, d->k0, cat_X + i, d->n_cat, G.cat[i], d->cat_rows[i], N, H,
                            forked2 ? ax->s : st));
   {
     SegList S;
@@ -898,6 +1014,12 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
     }
   }
   if (forked2) TRY(aux_join(ax, st));
+  if (padded) {   // after the join: the categorical embedding gradients are among them
+    SegList S;
+    S.count = 0;
+    append_tensor_segs(S, d, w.pg, H, base);
+    k_unpack<<<dim3(32, S.count), 256, 0, st>>>(grads, base, S);
+  }
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }

@@ -431,13 +431,13 @@ inline bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 // shared-memory-staged kernels (tconv_tile.cu); PERT_ERR_UNSUPPORTED => use the per-row gather kernels below
 int pert_tile_fwd(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if, const float* t_rpc,
-                  int n_rpc, float* out, int ld_out, float* alpha, long long N, long long E, long long B, int H,
+                  int n_rpc, float* out, int ld_out, float* alpha, long long N, long long E, long long B, int H, int C,
                   double* bn_acc, const long long* live, const PertTiles* tiles, cudaStream_t st);
 int pert_tile_bwd(const float* g_, int ld_g, const float* q, const float* k, const float* v, int ld, const int* rowptr,
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
                   const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha, float* dq, float* dk,
                   float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc, int n_rpc, long long N,
-                  long long E, long long B, int H, const PertTiles* tiles, cudaStream_t st);
+                  long long E, long long B, int H, int C, const PertTiles* tiles, cudaStream_t st);
 static bool tile_enabled() {
   static int on = -1;
   if (on < 0) {
@@ -455,20 +455,20 @@ int pert_tconv_supported_width(int H) {
 
 }  // extern "C"
 
-// Engine-internal form of pert_tconv_fwd: bn_acc (optional, [2][H] doubles, zeroed by the caller) receives the column
+// Engine-internal form of pert_tconv_fwd_c: bn_acc (optional, [2][H] doubles, zeroed by the caller) receives the column
 // sums / sums of squares of `out` when the staged tile kernel runs (*fused = 1); otherwise *fused = 0 and the caller
 // computes the BatchNorm statistics with its own pass.
 int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                          const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if,
                          const float* t_rpc, float* out, int ld_out, float* alpha, int n_rpc, long long N, long long E,
-                         long long B_hint, int H, double* bn_acc, const long long* live, int* fused,
+                         long long B_hint, int H, int C, double* bn_acc, const long long* live, int* fused,
                          const PertTiles* tiles, void* stream) {
   *fused = 0;
   if ((bn_acc || tiles) && N > 0 && tile_enabled() && ld_out == H && q && k && v && rowptr && out && !(ld % 4) && aligned16(q) &&
       aligned16(k) && aligned16(v) && aligned16(out) && (!s || aligned16(s)) &&
       (!t_if || (aligned16(t_if) && t_rpc && aligned16(t_rpc) && csr_if && csr_rpc))) {
     int rt = pert_tile_fwd(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, n_rpc, out, ld_out, alpha, N, E,
-                           B_hint, H, bn_acc, live, tiles, (cudaStream_t)stream);
+                           B_hint, H, C, bn_acc, live, tiles, (cudaStream_t)stream);
     if (rt == PERT_OK) {
       *fused = bn_acc ? 1 : 0;
       PERT_LAUNCH_CHECK();
@@ -476,23 +476,23 @@ int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const f
     }
     if (rt != PERT_ERR_UNSUPPORTED) return rt;
   }
-  return pert_tconv_fwd(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, out, ld_out, alpha, n_rpc, N, E,
-                        B_hint, H, stream);
+  return pert_tconv_fwd_c(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, out, ld_out, alpha, n_rpc, N,
+                          E, B_hint, H, C, stream);
 }
 
-// Engine-internal form of pert_tconv_bwd with a graph-aligned tile list (falls back to the public entry without one).
+// Engine-internal form of pert_tconv_bwd_c with a graph-aligned tile list (falls back to the public entry without one).
 int pert_tconv_bwd_tiles(const float* g, int ld_g, const float* q, const float* k, const float* v, int ld,
                          const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc,
                          const int* colptr, const int* csc_pos, const int* csc_dst, const float* t_if,
                          const float* t_rpc, const float* alpha, float* dq, float* dk, float* dv, int ld_d, float* dsp,
                          float* rpc_ws, float* dt_if, float* dt_rpc, int n_rpc, long long N, long long E,
-                         long long B_hint, int H, const PertTiles* tiles, void* stream) {
+                         long long B_hint, int H, int C, const PertTiles* tiles, void* stream) {
   if (tiles && N > 0 && tile_enabled() && ld_d == H && g && q && k && v && rowptr && colptr && dq && dk && dv &&
       !(ld % 4) && !(ld_g % 4) && aligned16(g) && aligned16(q) && aligned16(k) && aligned16(v) && aligned16(dq) &&
       aligned16(dk) && aligned16(dv) &&
       (!t_if || (t_rpc && dt_if && dt_rpc && csr_if && csr_rpc && aligned16(dt_if) && aligned16(dt_rpc)))) {
     int rt = pert_tile_bwd(g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, colptr, csc_pos, csc_dst, t_if, t_rpc,
-                           alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, tiles,
+                           alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, C, tiles,
                            (cudaStream_t)stream);
     if (rt == PERT_OK) {
       PERT_LAUNCH_CHECK();
@@ -500,8 +500,8 @@ int pert_tconv_bwd_tiles(const float* g, int ld_g, const float* q, const float* 
     }
     if (rt != PERT_ERR_UNSUPPORTED) return rt;
   }
-  return pert_tconv_bwd(g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, colptr, csc_pos, csc_dst, t_if, t_rpc,
-                        alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, stream);
+  return pert_tconv_bwd_c(g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, colptr, csc_pos, csc_dst, t_if, t_rpc,
+                          alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, C, stream);
 }
 
 extern "C" {
@@ -510,7 +510,15 @@ int pert_tconv_fwd(const float* q, const float* k, const float* v, const float* 
                    const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if, const float* t_rpc,
                    float* out, int ld_out, float* alpha, int n_rpc, long long N, long long E, long long B_hint, int H,
                    void* stream) {
-  if (N < 0 || E < 0 || !q || !k || !v || !rowptr || !out) return PERT_ERR_BADARG;
+  return pert_tconv_fwd_c(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, out, ld_out, alpha, n_rpc, N,
+                          E, B_hint, H, H, stream);
+}
+
+int pert_tconv_fwd_c(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
+                     const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if, const float* t_rpc,
+                     float* out, int ld_out, float* alpha, int n_rpc, long long N, long long E, long long B_hint, int H,
+                     int C, void* stream) {
+  if (N < 0 || E < 0 || !q || !k || !v || !rowptr || !out || C < 1 || C > H) return PERT_ERR_BADARG;
   if (ld % 4 || ld_out % 4 || !aligned16(q) || !aligned16(k) || !aligned16(v) || !aligned16(out) ||
       (s && !aligned16(s)) || (t_if && (!aligned16(t_if) || !aligned16(t_rpc) || !t_rpc)) ||
       (t_if && E > 0 && (!csr_if || !csr_rpc)))   // an edgeless batch may pass null edge arrays
@@ -518,7 +526,7 @@ int pert_tconv_fwd(const float* q, const float* k, const float* v, const float* 
   if (N == 0) return PERT_OK;
   if (tile_enabled() && ld_out == H) {
     int rt = pert_tile_fwd(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, n_rpc, out, ld_out, alpha, N, E,
-                           B_hint, H, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+                           B_hint, H, C, nullptr, nullptr, nullptr, (cudaStream_t)stream);
     if (rt != PERT_ERR_UNSUPPORTED) {
       if (rt) return rt;
       PERT_LAUNCH_CHECK();
@@ -526,7 +534,7 @@ int pert_tconv_fwd(const float* q, const float* k, const float* v, const float* 
     }
   }
   TconvArgs a{q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, out, ld_out, alpha, (int)N,
-              1.0f / sqrtf((float)H)};
+              1.0f / sqrtf((float)C)};
   int rc = dispatch_h(H, [&](auto lpr, auto vpl) {
     constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
     const int gpw = 32 / LPR;
@@ -544,7 +552,17 @@ int pert_tconv_bwd(const float* g, int ld_g, const float* q, const float* k, con
                    const int* csc_pos, const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha,
                    float* dq, float* dk, float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc,
                    int n_rpc, long long N, long long E, long long B_hint, int H, void* stream) {
-  if (N < 0 || E < 0 || !g || !q || !k || !v || !rowptr || !colptr || !dq || !dk || !dv) return PERT_ERR_BADARG;
+  return pert_tconv_bwd_c(g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, colptr, csc_pos, csc_dst, t_if, t_rpc,
+                          alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, H, stream);
+}
+
+int pert_tconv_bwd_c(const float* g, int ld_g, const float* q, const float* k, const float* v, int ld,
+                     const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr,
+                     const int* csc_pos, const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha,
+                     float* dq, float* dk, float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc,
+                     int n_rpc, long long N, long long E, long long B_hint, int H, int C, void* stream) {
+  if (N < 0 || E < 0 || !g || !q || !k || !v || !rowptr || !colptr || !dq || !dk || !dv || C < 1 || C > H)
+    return PERT_ERR_BADARG;
   if (ld % 4 || ld_g % 4 || ld_d % 4 || !aligned16(g) || !aligned16(q) || !aligned16(k) || !aligned16(v) ||
       !aligned16(dq) || !aligned16(dk) || !aligned16(dv))
     return PERT_ERR_BADARG;
@@ -553,14 +571,15 @@ int pert_tconv_bwd(const float* g, int ld_g, const float* q, const float* k, con
   if (N == 0) return PERT_OK;
   if (tile_enabled() && ld_d == H) {
     int rt = pert_tile_bwd(g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, colptr, csc_pos, csc_dst, t_if, t_rpc,
-                           alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, nullptr, (cudaStream_t)stream);
+                           alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, C, nullptr,
+                           (cudaStream_t)stream);
     if (rt != PERT_ERR_UNSUPPORTED) {
       if (rt) return rt;
       PERT_LAUNCH_CHECK();
       return PERT_OK;
     }
   }
-  const float isc = 1.0f / sqrtf((float)H);
+  const float isc = 1.0f / sqrtf((float)C);
   TconvBwdDstArgs ad{g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, alpha, dq, ld_d, dsp,
                      (int)N, isc};
   TconvBwdSrcArgs as{g, ld_g, q, ld, colptr, csc_pos, csc_dst, csr_if, csr_rpc, alpha, dsp, dk, dv, ld_d,

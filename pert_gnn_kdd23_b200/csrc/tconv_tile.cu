@@ -1050,7 +1050,7 @@ int launch_bwd(const TileArgs& a0, long long N, long long E, long long B, bool h
 int pert_tile_fwd(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if, const float* t_rpc,
                   int n_rpc, float* out, int ld_out, float* alpha, long long N, long long E, long long B, int H,
-                  double* bn_acc, const long long* live, const PertTiles* tiles, cudaStream_t st) {
+                  int C, double* bn_acc, const long long* live, const PertTiles* tiles, cudaStream_t st) {
   if (ld != H || ld_out != H || (t_if && (size_t)n_rpc * H * 4 > 16 * 1024))
     return PERT_ERR_UNSUPPORTED;
   TileArgs a{};
@@ -1058,7 +1058,7 @@ int pert_tile_fwd(const float* q, const float* k, const float* v, const float* s
   a.rowptr = rowptr; a.csr_src = csr_src; a.csr_if = csr_if; a.csr_rpc = csr_rpc;
   a.t_if = t_if; a.t_rpc = t_rpc; a.n_rpc = n_rpc; a.out = out; a.alpha = alpha; a.bn_acc = bn_acc;
   a.live = bn_acc ? live : nullptr;
-  a.N = (int)N; a.inv_sqrt_c = 1.0f / sqrtf((float)H);
+  a.N = (int)N; a.inv_sqrt_c = 1.0f / sqrtf((float)C);
   switch (H) {
     case 32: return launch_fwd<32>(a, N, E, B, t_if != nullptr, tiles, st);
     case 64: return launch_fwd<64>(a, N, E, B, t_if != nullptr, tiles, st);
@@ -1071,7 +1071,7 @@ int pert_tile_bwd(const float* g_, int ld_g, const float* q, const float* k, con
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
                   const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha, float* dq, float* dk,
                   float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc, int n_rpc, long long N,
-                  long long E, long long B, int H, const PertTiles* tiles, cudaStream_t st) {
+                  long long E, long long B, int H, int C, const PertTiles* tiles, cudaStream_t st) {
   if (ld != H || ld_g != H || ld_d != H || (t_if && (size_t)n_rpc * H * 4 > 16 * 1024))
     return PERT_ERR_UNSUPPORTED;
   TileArgs a{};
@@ -1081,7 +1081,7 @@ int pert_tile_bwd(const float* g_, int ld_g, const float* q, const float* k, con
   a.t_if = t_if; a.t_rpc = t_rpc; a.n_rpc = n_rpc;
   a.out = dq; a.dk = dk; a.dv = dv; a.alpha = const_cast<float*>(alpha); a.dsp = dsp;
   a.dt_if = dt_if; a.dt_rpc = dt_rpc; a.rpc_ws = rpc_ws; a.hot_if = 0;
-  a.N = (int)N; a.inv_sqrt_c = 1.0f / sqrtf((float)H);
+  a.N = (int)N; a.inv_sqrt_c = 1.0f / sqrtf((float)C);
   switch (H) {
     case 32: return launch_bwd<32>(a, N, E, B, t_if != nullptr, tiles, st);
     case 64: return launch_bwd<64>(a, N, E, B, t_if != nullptr, tiles, st);

@@ -91,25 +91,31 @@ class Engine:
         self.lib = _bind()
         dev = self.fp.flat.device
         H = model.hidden_channels
+        # the engine runs the width-H model at the kernel width Hp >= H, columns [H, Hp) zero (include/pertgnn.h)
+        Hp = self.lib.pert_model_width(H)
+        _lib.check(min(Hp, 0), f"pert_model_width({H})")
+        self.Hp = Hp
         n_convs = len(model.convs)
         assert n_convs <= MAX_CONVS and len(model.cat_embedding) <= MAX_CAT
-        # BN running statistics as one flat buffer; the module buffers become views of it
+        # BN running statistics as one flat buffer [n_bn, 2, Hp]; the module buffers become views of its first H columns
+        # (the padding columns start at mean 0, variance 1 and never reach an output)
         n_bn = n_convs - 1
-        self.bn_running = torch.empty(n_bn, 2, H, device=dev, dtype=torch.float32)
+        self.bn_running = torch.zeros(n_bn, 2, Hp, device=dev, dtype=torch.float32)
+        self.bn_running[:, 1] = 1.0
         self.bn_nbt = torch.zeros(n_bn, device=dev, dtype=torch.int64)
         for l, bn in enumerate(model.bns):
-            self.bn_running[l, 0].copy_(bn.running_mean)
-            self.bn_running[l, 1].copy_(bn.running_var)
+            self.bn_running[l, 0, :H].copy_(bn.running_mean)
+            self.bn_running[l, 1, :H].copy_(bn.running_var)
             self.bn_nbt[l] = bn.num_batches_tracked
-            bn._buffers["running_mean"] = self.bn_running[l, 0]
-            bn._buffers["running_var"] = self.bn_running[l, 1]
+            bn._buffers["running_mean"] = self.bn_running[l, 0, :H]
+            bn._buffers["running_var"] = self.bn_running[l, 1, :H]
             bn._buffers["num_batches_tracked"] = self.bn_nbt[l]
         d = PertModelDesc()
         d.F, d.H, d.n_convs, d.n_cat = model.in_channels, H, n_convs, len(model.cat_embedding)
         d.n_entry = model.entry_embeds.num_embeddings
         d.n_if = model.interface_embeds.num_embeddings
         d.n_rpc = model.rpctype_embeds.num_embeddings
-        d.k0 = (model.in_channels + H + 7) // 8 * 8
+        d.k0 = (model.in_channels + Hp + 7) // 8 * 8
         d.bn_eps = model.bns[0].eps
         d.bn_momentum = model.bns[0].momentum if model.bns[0].momentum is not None else 0.0
         base = self.fp.flat.data_ptr()
@@ -169,20 +175,21 @@ class Engine:
         i.e. which ReLUs were active -- with dropout, active AND kept.  Test aid: lets a reference be differentiated on
         the same linear piece."""
         x, cat_X, entry_id, probs, pnn, batch, index, training, N, E, B, p = self._saved
-        H = self.desc.H
+        H, Hp = self.desc.H, self.Hp
         out = {}
         for l in range(1, self.n_convs):
             off = self.lib.pert_model_workspace_offset(C.byref(self.desc), N, E, B, 0, l)
             _lib.check(int(min(off, 0)), "pert_model_workspace_offset")
-            out[f"bn{l - 1}"] = self.ws[off:off + N * H].view(N, H) > 0
+            out[f"bn{l - 1}"] = self.ws[off:off + N * Hp].view(N, Hp)[:, :H] > 0
         off = self.lib.pert_model_workspace_offset(C.byref(self.desc), N, E, B, 1, 0)
         _lib.check(int(min(off, 0)), "pert_model_workspace_offset")
-        out["head"] = self.ws[off:off + B * H].view(B, H) > 0
+        out["head"] = self.ws[off:off + B * Hp].view(B, Hp)[:, :H] > 0
         return out
 
     def _pack_launches(self):
-        # mirrors engine.cu: conv 0 contributes 24 segments, the others 16; a launch holds at most 96
-        n, count = 0, 0
+        # mirrors engine.cu: conv 0 contributes 24 segments, the others 16; a launch holds at most 96.  A padded width
+        # (Hp > H) adds one launch for the zero-padded copies of the other tensors.
+        n, count = int(self.Hp != self.desc.H), 0
         for l in range(self.n_convs):
             count += 24 if l == 0 else 16
             if count + 24 > 96 or l == self.n_convs - 1:
@@ -194,7 +201,7 @@ class Engine:
         embeddings + copy, per conv GEMM + attention (whose epilogue also produces the BatchNorm statistics), per
         BatchNorm one apply kernel unless pert_bn_linear_fwd_planes takes the shape (the next conv's GEMM then applies
         it), pool, head."""
-        L, H, N = self.n_convs, self.desc.H, self._saved[8]
+        L, H, N = self.n_convs, self.Hp, self._saved[8]
         applies = 0 if self.lib.pert_bn_linear_fwd_planes_supported(N, H, H) else L - 1
         return self._pack_launches() + (L + 5) // 6 + self.desc.n_cat + 1 + 2 * L + applies + 1 + 1
 
@@ -202,7 +209,7 @@ class Engine:
         """head, pool, per conv (target pass, source pass, node-linear backward: one fused launch where
         pert_linear_bwd_planes takes the shape, else weight GEMM + data GEMM), per BatchNorm reduce + apply,
         embedding scatters, edge-table gradients (3 layers per launch), unpack."""
-        L, H, N = self.n_convs, self.desc.H, self._saved[8]
+        L, H, N = self.n_convs, self.Hp, self._saved[8]
         linear = sum(1 if self.lib.pert_linear_bwd_planes_supported(N, H, self.desc.k0 if l == 0 else H,
                                                                      H) else 2 for l in range(L))
         return 1 + 1 + 2 * L + linear + 2 * (L - 1) + self.desc.n_cat + (L + 2) // 3 + self._pack_launches()

@@ -16,17 +16,13 @@
  *   - return value: 0 = ok; > 0 = cudaError_t of a failed launch/memset; < 0 = library code
  *     (PERT_ERR_*).  Never throws, never exits.  Out-of-range indices found ON THE DEVICE are
  *     reported by writing PERT_ERR_RANGE into the optional device word `status`;
- *   - library-owned state (all of it; none of it is data): (1) a per-device ring of 8192 self-resetting tile-ticket
- *     counters for the dynamically scheduled graph-tile kernels -- every launch takes the next slot (host atomic), so
- *     concurrent launches on different streams / threads / captured graphs do not share a counter unless 8192 such
- *     launches separate them while the first is still running; (2) per device, one auxiliary non-blocking stream and
+ *   - library-owned state (all of it; none of it is data): (1) per device, one auxiliary non-blocking stream and
  *     two events the step engine (pert_model_forward/backward) uses to run independent small kernels beside the main
- *     chain (fork/join by events, capture-safe; PERT_ENGINE_FORK=0 disables); the host-side issue of engine calls on
+ *     chain (fork/join by events, capture-safe); the host-side issue of engine calls on
  *     one device is serialised by a mutex, so engines driven from several host threads / streams stay correct (their
- *     side work shares that one auxiliary stream); (3) the SM count of
- *     each device, read once; (4) environment switches read once (debug / measurement A/B only):
- *     PERT_GEMM_TC, PERT_TCONV_TILE, PERT_TCONV_VPL, PERT_TCONV_VPL_BWD,
- *     PERT_TILE_LIST, PERT_BN_FUSE, PERT_ENGINE_FORK, PERT_PEER_MODE, PERT_LINEAR_BWD_FUSED.
+ *     side work shares that one auxiliary stream); (2) the SM count of
+ *     each device, read once; (3) environment switches read once (debug / measurement A/B only):
+ *     PERT_GEMM_TC, PERT_LINEAR_BWD_FUSED, PERT_PEER_MODE.
  *     With that, operator-level calls are re-entrant and thread-safe across streams;
  *   - rows of float matrices must be 16-byte aligned (ld % 4 == 0, base pointer 16-byte aligned)
  *     unless stated otherwise.

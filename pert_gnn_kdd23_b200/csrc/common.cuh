@@ -66,31 +66,15 @@ __device__ __forceinline__ float group_sum(float v, unsigned gmask) {
 }
 
 // engine-internal entry points (not part of the C-ABI)
-struct PertTiles {            // graph-aligned tile list of one batch for one row width (csrc/tconv_tile.cu)
-  const int* tile_ptr;        // [*ntiles + 1] node boundaries (device)
-  const int* ntiles;          // device scalar
-  int max_tiles, T, ecap;     // capacity of tile_ptr; nodes / staged edges a tile may hold
-};
-unsigned int* pert_ticket_slot();   // next slot of the self-resetting ticket ring (csrc/gemm_tc.cu)
-long long pert_tile_list_ints(long long N, long long B);
-bool pert_tile_fixed_ok(long long N, long long E, long long B, int H, int n_rpc);
-int pert_tile_list_view(long long N, long long E, long long B, int H, int n_rpc, int* tiles_mem, PertTiles* out);
-int pert_tile_list_bounds(const int64_t* batch, long long N, long long B, int* tiles_mem, cudaStream_t st);
-int pert_tile_list_build(int has_batch, long long N, long long E, long long B, const int* rowptr, int H, int n_rpc,
-                         int* tiles_mem, PertTiles* out, cudaStream_t st);
+// PERT_GEMM_TC=0: the exact-fp32 SIMT GEMMs of gemm.cu instead of the tensor-core kernels (csrc/gemm_tc.cu), read once
+bool pert_gemm_tc_enabled();
 // live: optional device {N, B} of a padded batch (pert_batch_pad); the BatchNorm sums then count the rows below live[0].
 // C: the logical width whose 1/sqrt(C) scales the logits (pert_tconv_fwd_c; C = H for an unpadded model)
 int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                          const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if,
                          const float* t_rpc, float* out, int ld_out, float* alpha, int n_rpc, long long N, long long E,
                          long long B_hint, int H, int C, double* bn_acc, const long long* live, int* fused,
-                         const PertTiles* tiles, void* stream);
-int pert_tconv_bwd_tiles(const float* g, int ld_g, const float* q, const float* k, const float* v, int ld,
-                         const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc,
-                         const int* colptr, const int* csc_pos, const int* csc_dst, const float* t_if,
-                         const float* t_rpc, const float* alpha, float* dq, float* dk, float* dv, int ld_d, float* dsp,
-                         float* rpc_ws, float* dt_if, float* dt_rpc, int n_rpc, long long N, long long E,
-                         long long B_hint, int H, int C, const PertTiles* tiles, void* stream);
+                         void* stream);
 int pert_bn_fwd_ex(const float* x, int ld_x, const float* gamma, const float* beta, float* running_mean,
                    float* running_var, long long* num_batches_tracked, float eps, float momentum, int training,
                    int relu, float* mean, float* rstd, float* y, int ld_y, long long N, int H, void* workspace,

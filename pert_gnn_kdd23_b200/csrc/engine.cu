@@ -417,7 +417,6 @@ struct Ws {
   float *bn_part, *pool, *z, *h1;
   // backward temporaries
   float *dplanes, *dx, *dsp, *rpc_ws, *sums, *dpool, *dzent, *dh1;
-  int* tiles;      // graph-aligned tile list of the batch (pert_tile_list_ints ints), built in forward, reused in backward
   long long* drop_ctr;  // {seed, step} of the last training forward with dropout (k_pack -> BatchNorm applies)
   long long total;  // floats
   long long packed_floats;
@@ -495,7 +494,6 @@ Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* b
     w.bn_stats[l] = take(2LL * H);
   }
   w.bn_part = take(pert_bn_workspace_bytes(N, H) / 4 + 16);
-  w.tiles = (int*)take(pert_tile_list_ints(N, B));
   w.pool = take(B * H);
   w.z = take(B * 2 * H);
   w.h1 = take(B * H);
@@ -589,8 +587,8 @@ void append_tensor_segs(SegList& S, const PertModelDesc* d, const Tensors& t, in
 
 // Auxiliary stream for the few places where independent small kernels can run beside the main chain (input prologue
 // next to the parameter pack + edge tables; edge-table gradients next to the conv-0 GEMMs).  Fork / join with events,
-// so the dependencies also hold inside a CUDA-graph capture.  Created on first (eager) use per device;
-// PERT_ENGINE_FORK=0 keeps everything on the caller's stream.
+// so the dependencies also hold inside a CUDA-graph capture.  Created on first (eager) use per device; where it cannot
+// be created, everything runs on the caller's stream.
 struct AuxStream {
   cudaStream_t s = nullptr;
   cudaEvent_t fork = nullptr, join = nullptr;
@@ -601,34 +599,8 @@ std::mutex& engine_mutex() {
   static std::mutex m;
   return m;
 }
-// Graph-aligned tile lists (csrc/tconv_tile.cu:k_build_tiles) are OFF by default: fixed T-node tiles have the minimal
-// number of tiles (one wave of CTAs at cfg2) and the global-gather variant that cut graphs need is only ~10 % slower
-// than the all-in-tile variant, while whole-graph tiles cost a packing kernel per batch and more, unevenly filled
-// tiles.  PERT_TILE_LIST=1 turns them on.
-bool tiles_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("PERT_TILE_LIST");
-    on = (e && e[0] == '1') ? 1 : 0;
-  }
-  return on == 1;
-}
-bool bn_fuse_enabled() {   // PERT_BN_FUSE=0: statistics by the separate k_bn_partial pass (debug A/B)
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("PERT_BN_FUSE");
-    on = (e && e[0] == '0') ? 0 : 1;
-  }
-  return on == 1;
-}
 AuxStream* aux_stream() {
   static AuxStream aux[64];
-  static int enabled = -1;
-  if (enabled < 0) {
-    const char* e = getenv("PERT_ENGINE_FORK");
-    enabled = (e && e[0] == '0') ? 0 : 1;
-  }
-  if (!enabled) return nullptr;
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
   AuxStream& a = aux[dev];
@@ -793,17 +765,12 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
     TRY(pert_embedding_fwd(P.cat[i], d->cat_rows[i], cat_X + i, d->n_cat, w.x[0], d->k0, N, H, i > 0,
                            status, s2));
   TRY(pert_copy_cols(x, d->F, w.x[0], d->k0, H, N, s2));
-  // graph boundaries of the batch for the tile list (needs only the batch vector): beside the prologue as well
-  const bool want_tiles = tiles_enabled() && E > 0 && N > 0 && !pert_tile_fixed_ok(N, E, B, H, d->n_rpc);
-  if (want_tiles) TRY(pert_tile_list_bounds(batch, N, B, w.tiles, s2));
   if (forked) TRY(aux_join(ax, st));
   // 3. conv stack.  Where the shape qualifies, the node linear of conv l >= 1 applies the BatchNorm(+ReLU, +dropout)
   // of conv l - 1 while it loads out[l - 1] and writes x[l] on the way (csrc/linear_fwd.cu): one launch and one pass
   // instead of the apply pass followed by the GEMM.  It reads the BatchNorm sums of conv l - 1 before the memset of
   // conv l below clears them.
   const bool bn_in_linear = pert_bn_linear_fwd_planes_supported(N, H, H) == 1;
-  PertTiles tiles{};
-  bool have_tiles = false;
   int prev_stats_fused = 0;
   for (int l = 0; l < L; ++l) {
     const int K = k_of(d, w, l);
@@ -835,15 +802,10 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
       cudaError_t we = cudaStreamWaitEvent(st, (cudaEvent_t)index_ready, 0);
       if (we != cudaSuccess) return (int)we;
     }
-    if (l == 0 && want_tiles) {   // graph-aligned tile list (whole graphs per tile), once per batch
-      int trc = pert_tile_list_build(batch != nullptr && B > 0, N, E, B, rowptr, H, d->n_rpc, w.tiles, &tiles, st);
-      have_tiles = trc == PERT_OK;
-      if (!have_tiles && trc != PERT_ERR_UNSUPPORTED) return trc;
-    }
     // BatchNorm statistics of out[l] are produced by the conv kernel's epilogue (training, staged tile path)
     int stats_fused = 0;
     double* bn_acc = nullptr;
-    if (l + 1 < L && training && bn_fuse_enabled()) {
+    if (l + 1 < L && training) {
       bn_acc = (double*)w.bn_part;
       cudaError_t me = cudaMemsetAsync(bn_acc, 0, (size_t)2 * H * sizeof(double), st);
       if (me != cudaSuccess) return (int)me;
@@ -851,7 +813,7 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
     PROBE_START(1, l);
     TRY(pert_tconv_fwd_stats(pl, pl + N * H, pl + 2 * N * H, pl + 3 * N * H, H, rowptr, csr_src, csr_if, csr_rpc,
                              w.t_if[l], w.t_rpc[l], w.out[l], H, w.alpha[l], d->n_rpc, N, E, B, H, d->H, bn_acc, live,
-                             &stats_fused, have_tiles ? &tiles : nullptr, st));
+                             &stats_fused, st));
     PROBE_STOP(1, l);
     prev_stats_fused = stats_fused;
     if (l + 1 < L && !bn_in_linear) {
@@ -957,16 +919,13 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
   };
   AuxStream* ax = aux_stream();
   bool forked = false;
-  PertTiles tiles{};            // the list forward built for this batch (same geometry: a pure function of the sizes)
-  const bool have_tiles = tiles_enabled() && E > 0 && !pert_tile_fixed_ok(N, E, B, H, d->n_rpc) &&
-                          pert_tile_list_view(N, E, B, H, d->n_rpc, w.tiles, &tiles) == PERT_OK;
   for (int l = L - 1; l >= 0; --l) {
     const int K = k_of(d, w, l);
     float* pl = w.planes[l];
     PROBE_START(2, l);
-    TRY(pert_tconv_bwd_tiles(dskip, H, pl, pl + N * H, pl + 2 * N * H, H, rowptr, csr_src, csr_if, csr_rpc, colptr,
-                             csc_pos, csc_dst, w.t_if[l], w.t_rpc[l], w.alpha[l], dq, dk, dv, H, w.dsp, w.rpc_ws,
-                             w.dt_if[l], w.dt_rpc[l], d->n_rpc, N, E, B, H, d->H, have_tiles ? &tiles : nullptr, st));
+    TRY(pert_tconv_bwd_c(dskip, H, pl, pl + N * H, pl + 2 * N * H, H, rowptr, csr_src, csr_if, csr_rpc, colptr,
+                         csc_pos, csc_dst, w.t_if[l], w.t_rpc[l], w.alpha[l], dq, dk, dv, H, w.dsp, w.rpc_ws,
+                         w.dt_if[l], w.dt_rpc[l], d->n_rpc, N, E, B, H, d->H, st));
     PROBE_STOP(2, l);
     if (l == 0) {                       // every dT table is complete now
       forked = aux_fork(ax, st);

@@ -28,7 +28,6 @@
 // These GEMMs are memory-bound by shape (K <= 256): A read once, C written once.
 #include "common.cuh"
 #include "sm90.cuh"
-#include <atomic>
 #include <stdlib.h>
 
 namespace {
@@ -256,38 +255,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_gemm_tn_wg(TnArgs g) {
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Tile tickets (used by the graph-aligned conv kernels, csrc/tconv_tile.cu): every launch of a dynamically scheduled
-// kernel draws its tickets from its OWN slot of a ring of self-resetting device counters (8 counters per slot).  The
-// host hands out slots round-robin (atomic), so two launches that run concurrently on different streams -- or two
-// replicas captured into different CUDA graphs -- never share a counter unless TICKET_SLOTS launches were issued in
-// between while the first was still running.  The CTA that draws the last ticket of a launch resets the counter, so
-// a slot (also one baked into a captured graph) is reusable as soon as its launch has finished.
-constexpr int TICKET_SLOTS = 8192;
-__device__ unsigned int g_ticket_ring[TICKET_SLOTS * 8];
-
 inline bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 inline bool al8(const void* p) { return ((uintptr_t)p & 7) == 0; }
-// next ticket slot of the current device's ring (host side: one atomic increment per launch, thread-safe)
-static unsigned int* ticket_slot() {
-  static std::atomic<unsigned int> next{0};
-  static std::atomic<unsigned int*> base_of[64];          // per device; resolved on the first (eager) launch
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
-  unsigned int* base = base_of[dev].load(std::memory_order_acquire);
-  if (!base) {
-    if (cudaGetSymbolAddress((void**)&base, g_ticket_ring) != cudaSuccess) return nullptr;
-    base_of[dev].store(base, std::memory_order_release);
-  }
-  return base + (size_t)(next.fetch_add(1u, std::memory_order_relaxed) % TICKET_SLOTS) * 8;
-}
-static bool tc_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("PERT_GEMM_TC");
-    on = (e && e[0] == '0') ? 0 : 1;
-  }
-  return on == 1;
-}
 
 // grid size of a persistent launch: as many CTAs as fit on the device, shared by `parts` independent grid columns
 template <typename Kern>
@@ -317,7 +286,14 @@ static int launch_nt(const NtArgs& g, int nblk, int kplanes, cudaStream_t st) {
 
 }  // namespace
 
-unsigned int* pert_ticket_slot() { return ticket_slot(); }
+bool pert_gemm_tc_enabled() {
+  static int on = -1;
+  if (on < 0) {
+    const char* e = getenv("PERT_GEMM_TC");
+    on = (e && e[0] == '0') ? 0 : 1;
+  }
+  return on == 1;
+}
 
 // Returns PERT_ERR_UNSUPPORTED when the shape / layout is outside what the tensor-core kernels handle (the caller
 // then uses the exact-fp32 SIMT kernels of gemm.cu).
@@ -340,7 +316,7 @@ static bool nt_tc_layout_ok(const float* A, int lda, int a_cb, long long a_cbs, 
 int pert_gemm_nt_tc(const float* A, int lda, int a_cb, long long a_cbs, const float* B, int ldb, const float* bias,
                     float* C, int ldc, int c_cb, long long c_cbs, long long M, int Nc, int K, int relu,
                     cudaStream_t st) {
-  if (!tc_enabled() || M < 1024) return PERT_ERR_UNSUPPORTED;
+  if (!pert_gemm_tc_enabled() || M < 1024) return PERT_ERR_UNSUPPORTED;
   // Deep K over a column-blocked A (the data gradient dX = [dq|dk|dv|ds] . W4 at H = 128: K = 512): the whole [BN, K]
   // weight block (hi + lo) does not fit in shared memory unless BN is narrowed, which re-reads A once per N block.
   // Instead every column block of A is a plane (gridDim.z) with its own resident K-slice of the weights; C is zeroed
@@ -409,7 +385,7 @@ static int launch_tn(TnArgs g, int mblk, cudaStream_t st) {
 int pert_gemm_tn_tc(const float* A, int lda, int a_cb, long long a_cbs, const float* B, int ldb, int b_cb,
                     long long b_cbs, float* C, int ldc, float* a_colsum, long long R, int Mc, int Nc,
                     cudaStream_t st) {
-  if (!tc_enabled() || R < 4096) return PERT_ERR_UNSUPPORTED;
+  if (!pert_gemm_tc_enabled() || R < 4096) return PERT_ERR_UNSUPPORTED;
   if (a_cb <= 0) { a_cb = Mc; a_cbs = 0; }
   if (b_cb > 0 && b_cb < Nc) return PERT_ERR_UNSUPPORTED;   // B must be a plain matrix
   // two adjacent output rows per thread (8-byte loads of A), two adjacent columns per vector reduction into C

@@ -252,10 +252,9 @@ bool fused_enabled() {   // PERT_LINEAR_BWD_FUSED=0: the two-kernel path (A/B); 
   static int on = -1;
   if (on < 0) {
     const char* e = getenv("PERT_LINEAR_BWD_FUSED");
-    const char* tc = getenv("PERT_GEMM_TC");
-    on = ((e && e[0] == '0') || (tc && tc[0] == '0')) ? 0 : 1;
+    on = (e && e[0] == '0') ? 0 : 1;
   }
-  return on == 1;
+  return on == 1 && pert_gemm_tc_enabled();
 }
 
 bool shape_ok(long long N, int H, int K, int Kd) {

@@ -27,7 +27,6 @@
 #include "common.cuh"
 #include "bn.cuh"
 #include "sm90.cuh"
-#include <stdlib.h>
 
 namespace {
 
@@ -204,17 +203,8 @@ __global__ void __launch_bounds__(LF_THREADS, 1) k_bn_linear_fwd_planes(LfArgs g
   }
 }
 
-bool tc_enabled() {   // PERT_GEMM_TC=0 keeps every node linear on the exact-fp32 SIMT kernels
-  static int on = -1;
-  if (on < 0) {
-    const char* tc = getenv("PERT_GEMM_TC");
-    on = (tc && tc[0] == '0') ? 0 : 1;
-  }
-  return on == 1;
-}
-
 bool shape_ok(long long N, int H, int K) {
-  return tc_enabled() && H == LF_H && (K == 64 || K == 80) && N >= 4096 && N <= 0x7fffffffLL - LF_TM;
+  return pert_gemm_tc_enabled() && H == LF_H && (K == 64 || K == 80) && N >= 4096 && N <= 0x7fffffffLL - LF_TM;
 }
 
 // CTAs of k_bn_linear_fwd_planes<K, MODE> one SM holds (the shared-memory attribute is set on the way), queried once

@@ -25,7 +25,6 @@
 // so a node costs 3 dependent memory latencies instead of ~3 per edge per pass (r1 ncu: 50 % warps
 // active, 36 % issue-active, DRAM at 10 % with bytes == algorithmic bytes).
 #include "common.cuh"
-#include <stdlib.h>
 #include <type_traits>
 
 namespace {
@@ -432,20 +431,12 @@ inline bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 int pert_tile_fwd(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if, const float* t_rpc,
                   int n_rpc, float* out, int ld_out, float* alpha, long long N, long long E, long long B, int H, int C,
-                  double* bn_acc, const long long* live, const PertTiles* tiles, cudaStream_t st);
+                  double* bn_acc, const long long* live, cudaStream_t st);
 int pert_tile_bwd(const float* g_, int ld_g, const float* q, const float* k, const float* v, int ld, const int* rowptr,
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
                   const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha, float* dq, float* dk,
                   float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc, int n_rpc, long long N,
-                  long long E, long long B, int H, int C, const PertTiles* tiles, cudaStream_t st);
-static bool tile_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("PERT_TCONV_TILE");
-    on = (e && e[0] == '0') ? 0 : 1;
-  }
-  return on == 1;
-}
+                  long long E, long long B, int H, int C, cudaStream_t st);
 
 extern "C" {
 
@@ -462,15 +453,15 @@ int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const f
                          const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if,
                          const float* t_rpc, float* out, int ld_out, float* alpha, int n_rpc, long long N, long long E,
                          long long B_hint, int H, int C, double* bn_acc, const long long* live, int* fused,
-                         const PertTiles* tiles, void* stream) {
+                         void* stream) {
   *fused = 0;
-  if ((bn_acc || tiles) && N > 0 && tile_enabled() && ld_out == H && q && k && v && rowptr && out && !(ld % 4) && aligned16(q) &&
+  if (bn_acc && N > 0 && ld_out == H && q && k && v && rowptr && out && !(ld % 4) && aligned16(q) &&
       aligned16(k) && aligned16(v) && aligned16(out) && (!s || aligned16(s)) &&
       (!t_if || (aligned16(t_if) && t_rpc && aligned16(t_rpc) && csr_if && csr_rpc))) {
     int rt = pert_tile_fwd(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, n_rpc, out, ld_out, alpha, N, E,
-                           B_hint, H, C, bn_acc, live, tiles, (cudaStream_t)stream);
+                           B_hint, H, C, bn_acc, live, (cudaStream_t)stream);
     if (rt == PERT_OK) {
-      *fused = bn_acc ? 1 : 0;
+      *fused = 1;
       PERT_LAUNCH_CHECK();
       return PERT_OK;
     }
@@ -478,30 +469,6 @@ int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const f
   }
   return pert_tconv_fwd_c(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, out, ld_out, alpha, n_rpc, N,
                           E, B_hint, H, C, stream);
-}
-
-// Engine-internal form of pert_tconv_bwd_c with a graph-aligned tile list (falls back to the public entry without one).
-int pert_tconv_bwd_tiles(const float* g, int ld_g, const float* q, const float* k, const float* v, int ld,
-                         const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc,
-                         const int* colptr, const int* csc_pos, const int* csc_dst, const float* t_if,
-                         const float* t_rpc, const float* alpha, float* dq, float* dk, float* dv, int ld_d, float* dsp,
-                         float* rpc_ws, float* dt_if, float* dt_rpc, int n_rpc, long long N, long long E,
-                         long long B_hint, int H, int C, const PertTiles* tiles, void* stream) {
-  if (tiles && N > 0 && tile_enabled() && ld_d == H && g && q && k && v && rowptr && colptr && dq && dk && dv &&
-      !(ld % 4) && !(ld_g % 4) && aligned16(g) && aligned16(q) && aligned16(k) && aligned16(v) && aligned16(dq) &&
-      aligned16(dk) && aligned16(dv) &&
-      (!t_if || (t_rpc && dt_if && dt_rpc && csr_if && csr_rpc && aligned16(dt_if) && aligned16(dt_rpc)))) {
-    int rt = pert_tile_bwd(g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, colptr, csc_pos, csc_dst, t_if, t_rpc,
-                           alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, C, tiles,
-                           (cudaStream_t)stream);
-    if (rt == PERT_OK) {
-      PERT_LAUNCH_CHECK();
-      return PERT_OK;
-    }
-    if (rt != PERT_ERR_UNSUPPORTED) return rt;
-  }
-  return pert_tconv_bwd_c(g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, colptr, csc_pos, csc_dst, t_if, t_rpc,
-                          alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, C, stream);
 }
 
 extern "C" {
@@ -524,9 +491,9 @@ int pert_tconv_fwd_c(const float* q, const float* k, const float* v, const float
       (t_if && E > 0 && (!csr_if || !csr_rpc)))   // an edgeless batch may pass null edge arrays
     return PERT_ERR_BADARG;
   if (N == 0) return PERT_OK;
-  if (tile_enabled() && ld_out == H) {
+  if (ld_out == H) {
     int rt = pert_tile_fwd(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, n_rpc, out, ld_out, alpha, N, E,
-                           B_hint, H, C, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+                           B_hint, H, C, nullptr, nullptr, (cudaStream_t)stream);
     if (rt != PERT_ERR_UNSUPPORTED) {
       if (rt) return rt;
       PERT_LAUNCH_CHECK();
@@ -569,9 +536,9 @@ int pert_tconv_bwd_c(const float* g, int ld_g, const float* q, const float* k, c
   if (t_if && (!t_rpc || !dt_if || !dt_rpc || !aligned16(dt_if) || !aligned16(dt_rpc))) return PERT_ERR_BADARG;
   if (t_if && E > 0 && (!csr_if || !csr_rpc)) return PERT_ERR_BADARG;   // an edgeless batch may pass null edge arrays
   if (N == 0) return PERT_OK;
-  if (tile_enabled() && ld_d == H) {
+  if (ld_d == H) {
     int rt = pert_tile_bwd(g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, colptr, csc_pos, csc_dst, t_if, t_rpc,
-                           alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, C, nullptr,
+                           alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, C,
                            (cudaStream_t)stream);
     if (rt != PERT_ERR_UNSUPPORTED) {
       if (rt) return rt;

@@ -16,7 +16,6 @@
 // Tile size (nodes) is chosen by the host so that two CTAs of 512 threads fit one SM; when the batch holds equally
 // sized graphs the tile is a whole number of graphs (no cut edges).
 #include "common.cuh"
-#include <stdlib.h>
 #include <type_traits>
 
 namespace {
@@ -77,11 +76,6 @@ struct TileArgs {
   int N, tile_nodes, edge_cap;
   int hot_if;          // interface id whose table-gradient row is accumulated per CTA instead of per edge (source pass)
   float inv_sqrt_c;
-  // graph-aligned tile list (csrc: k_build_tiles): tile t = nodes [tile_ptr[t], tile_ptr[t+1]); null = fixed tiles of
-  // tile_nodes nodes, one per CTA.  CTAs draw tiles from `ticket` (self-resetting counter) until it exceeds *ntiles.
-  const int* tile_ptr;
-  const int* ntiles;
-  unsigned int* ticket;
 };
 
 // Gradient of the (tiny, hot) rpc-type table without per-edge atomics: for an edge t -> i of rpc type b the table row
@@ -128,51 +122,18 @@ static size_t smem_bytes(int T, int H, int n_rpc, int ecap, int n_edge_arrays) {
                                (size_t)n_edge_arrays * ecap);
 }
 
-// Tile scheduling shared by the three kernels: with a tile list the CTA draws tile ids from a self-resetting ticket
-// (the draw that returns ntiles + gridDim.x - 1 is the last of the launch and zeroes the counter), else it owns the one
-// fixed tile blockIdx.x.  Returns false when there is no more work.  Contains CTA barriers: call from all threads.
-__device__ __forceinline__ bool next_tile(const TileArgs& a, bool first, int& n0, int& nt) {
-  __shared__ int s_tile;
-  if (!a.tile_ptr) {
-    if (!first) return false;
-    n0 = blockIdx.x * a.tile_nodes;
-    nt = min(a.tile_nodes, a.N - n0);
-    return nt > 0;
-  }
-  const int total = *a.ntiles;
-  int t;
-  if (first) {
-    t = blockIdx.x;                      // the first tile of a CTA needs no ticket: tickets hand out tiles >= gridDim.x
-  } else {
-    __syncthreads();                     // every reader of the previous tile's shared memory (and of s_tile) is done
-    if (threadIdx.x == 0) {
-      // draw c -> tile gridDim.x + c.  Every CTA ends with exactly one failing draw, so the launch makes
-      // max(0, total - gridDim.x) + gridDim.x draws; the last one resets the counter for the next launch.
-      const unsigned int c = atomicAdd(a.ticket, 1u);
-      const unsigned int extra = total > (int)gridDim.x ? (unsigned int)(total - (int)gridDim.x) : 0u;
-      if (c == extra + gridDim.x - 1) *a.ticket = 0;
-      s_tile = (int)gridDim.x + (int)c;
-    }
-    __syncthreads();
-    t = s_tile;
-  }
-  if (t >= total) {
-    if (first) {                         // no first tile: still owes its one failing draw
-      if (threadIdx.x == 0) {
-        const unsigned int c = atomicAdd(a.ticket, 1u);
-        const unsigned int extra = total > (int)gridDim.x ? (unsigned int)(total - (int)gridDim.x) : 0u;
-        if (c == extra + gridDim.x - 1) *a.ticket = 0;
-      }
-    }
-    return false;
-  }
-  n0 = a.tile_ptr[t];
-  nt = a.tile_ptr[t + 1] - n0;
-  return true;
+// This CTA's tile: nodes [n0, n0 + nt), tiles of tile_nodes consecutive nodes, one per CTA.  The empty asm hides where
+// the two values come from.  Without it the compiler works with blockIdx.x * tile_nodes itself, and ptxas gives the
+// 1024-thread forward kernels with edge attributes 228-256 bytes of spill stores instead of 156-168 (nvcc 12.9,
+// -Xptxas -v).  Whether it still helps depends on the compiler: re-check those spill counts after an nvcc upgrade.
+__device__ __forceinline__ void cta_tile(const TileArgs& a, int& n0, int& nt) {
+  n0 = blockIdx.x * a.tile_nodes;
+  nt = min(a.tile_nodes, a.N - n0);
+  asm volatile("" : "+r"(n0), "+r"(nt));
 }
 
 // stage the two operand tiles + the node-pointer slice + the degree-sorted node order; returns after the pointers and
-// the order are visible (tiles: mbar_wait on the caller's phase).  The mbarrier is initialised once by the caller.
+// the order are visible (tiles: the caller's mbar_wait).  The mbarrier is initialised by the caller.
 // Lane groups of a warp walk their nodes' edges in lockstep (trip count = the largest degree in the warp): handing the
 // nodes out in DESCENDING DEGREE order puts equal degrees side by side (no idle lockstep iterations: E[max of 2 degrees]
 // is 3.8 against a mean of 3.0 at cfg2) and starts the long rows first.  Counting sort over degrees clamped to 32.
@@ -280,172 +241,171 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
 #pragma unroll
     for (int u = 0; u < VPL; ++u) v[u] = ldg4(base + row * H + (lig + u * LPR) * 4);
   };
-  tile_barrier_init(S, tid);
-  uint32_t phase = 0;
   int n0, nt;
-  for (bool first = true; next_tile(a, first, n0, nt); first = false, phase ^= 1) {
-    stage_tiles<H, NT>(S, a.k, a.v, a.rowptr, n0, nt, tid);
-    const int e_lo = S.ptr[0];
-    const int ne_c = min(S.ptr[nt] - e_lo, a.edge_cap);
-    int bad = 0, wide = 0;   // a staged neighbour outside this tile / staged ids that do not pack
-    for (int x = tid; x < ne_c; x += NT) {
-      const int nb_id = __ldg(a.csr_src + e_lo + x);
-      S.e0[x] = nb_id;
-      bad |= (unsigned)(nb_id - n0) >= (unsigned)nt;
-      if (HAS_E) {
-        const int ia = __ldg(a.csr_if + e_lo + x), ib = __ldg(a.csr_rpc + e_lo + x);
-        wide |= !packable(ia, ib);
-        S.e1[x] = PACK_ID(ia, ib);
-      }
+  cta_tile(a, n0, nt);
+  if (nt <= 0) return;                         // uniform across the CTA
+  tile_barrier_init(S, tid);
+  stage_tiles<H, NT>(S, a.k, a.v, a.rowptr, n0, nt, tid);
+  const int e_lo = S.ptr[0];
+  const int ne_c = min(S.ptr[nt] - e_lo, a.edge_cap);
+  int bad = 0, wide = 0;   // a staged neighbour outside this tile / staged ids that do not pack
+  for (int x = tid; x < ne_c; x += NT) {
+    const int nb_id = __ldg(a.csr_src + e_lo + x);
+    S.e0[x] = nb_id;
+    bad |= (unsigned)(nb_id - n0) >= (unsigned)nt;
+    if (HAS_E) {
+      const int ia = __ldg(a.csr_if + e_lo + x), ib = __ldg(a.csr_rpc + e_lo + x);
+      wide |= !packable(ia, ib);
+      S.e1[x] = PACK_ID(ia, ib);
     }
-    // fast variant of the edge loops when every edge of the tile is staged and every neighbour row is in the tile
-    // (whole-graph tiles): no global-memory fallbacks are compiled into it
-    // (one barrier in the common case; a second one tells unpackable ids from neighbours outside the tile)
-    const bool any = __syncthreads_or(bad | wide) != 0;
-    const bool narrow = !(HAS_E && any && __syncthreads_or(wide));   // else every edge takes the global path
-    const int ne_s = narrow ? ne_c : 0;
-    const bool all_in = !any && (S.ptr[nt] - e_lo <= a.edge_cap);
-    mbar_wait(S.bar, phase);
+  }
+  // fast variant of the edge loops when every edge of the tile is staged and every neighbour row is in the tile
+  // (whole-graph tiles): no global-memory fallbacks are compiled into it
+  // (one barrier in the common case; a second one tells unpackable ids from neighbours outside the tile)
+  const bool any = __syncthreads_or(bad | wide) != 0;
+  const bool narrow = !(HAS_E && any && __syncthreads_or(wide));   // else every edge takes the global path
+  const int ne_s = narrow ? ne_c : 0;
+  const bool all_in = !any && (S.ptr[nt] - e_lo <= a.edge_cap);
+  mbar_wait(S.bar, 0);
 
-    // node slots are handed out in descending-degree order (S.ord); the q row is requested one node ahead, the skip row
-    // at the start of its own node (it is consumed after the edge loop, which hides its latency)
-    int slot = g0 + grp;
-    int loc = slot < nt ? ldsu16(sa.ord + slot * 2) : 0;
-    float4 q_n[VPL];
+  // node slots are handed out in descending-degree order (S.ord); the q row is requested one node ahead, the skip row
+  // at the start of its own node (it is consumed after the edge loop, which hides its latency)
+  int slot = g0 + grp;
+  int loc = slot < nt ? ldsu16(sa.ord + slot * 2) : 0;
+  float4 q_n[VPL];
 #pragma unroll
-    for (int u = 0; u < VPL; ++u) q_n[u] = f4zero();
-    if (slot < nt) ldrow(a.q, (size_t)(n0 + loc), q_n);
-    auto run = [&](auto fast_c) {
-      constexpr bool FAST = decltype(fast_c)::value;
-      for (; slot - grp < nt; slot += GPC) {   // warp-uniform: the warp's first group still has a node
-        const bool valid = slot < nt;
-        const int i = n0 + loc;
-        float4 q[VPL], skip[VPL];
+  for (int u = 0; u < VPL; ++u) q_n[u] = f4zero();
+  if (slot < nt) ldrow(a.q, (size_t)(n0 + loc), q_n);
+  auto run = [&](auto fast_c) {
+    constexpr bool FAST = decltype(fast_c)::value;
+    for (; slot - grp < nt; slot += GPC) {   // warp-uniform: the warp's first group still has a node
+      const bool valid = slot < nt;
+      const int i = n0 + loc;
+      float4 q[VPL], skip[VPL];
 #pragma unroll
-        for (int u = 0; u < VPL; ++u) {
-          q[u] = f4scale(qscale, q_n[u]);
-          skip[u] = f4zero();
-        }
-        if (valid && a.s) ldrow(a.s, (size_t)i, skip);
-        const int p0 = valid ? ldsi(sa.ptr + loc * 4) : 0;
-        const int p1 = valid ? ldsi(sa.ptr + loc * 4 + 4) : 0;
-        if (slot + GPC < nt) {
-          loc = ldsu16(sa.ord + (slot + GPC) * 2);
-          ldrow(a.q, (size_t)(n0 + loc), q_n);
-        }
-        const int deg = p1 - p0;
-        const int degmax = __reduce_max_sync(0xffffffffu, deg);
-        float4 acc[VPL];
+      for (int u = 0; u < VPL; ++u) {
+        q[u] = f4scale(qscale, q_n[u]);
+        skip[u] = f4zero();
+      }
+      if (valid && a.s) ldrow(a.s, (size_t)i, skip);
+      const int p0 = valid ? ldsi(sa.ptr + loc * 4) : 0;
+      const int p1 = valid ? ldsi(sa.ptr + loc * 4 + 4) : 0;
+      if (slot + GPC < nt) {
+        loc = ldsu16(sa.ord + (slot + GPC) * 2);
+        ldrow(a.q, (size_t)(n0 + loc), q_n);
+      }
+      const int deg = p1 - p0;
+      const int degmax = __reduce_max_sync(0xffffffffu, deg);
+      float4 acc[VPL];
 #pragma unroll
-        for (int u = 0; u < VPL; ++u) acc[u] = f4zero();
-        float m = -INFINITY, Z = 0.f;
-        // software pipeline over edges: ids + table rows of edge t+1 are requested before edge t is consumed
-        int j = n0;
-        float4 eif[VPL], erp[VPL];
+      for (int u = 0; u < VPL; ++u) acc[u] = f4zero();
+      float m = -INFINITY, Z = 0.f;
+      // software pipeline over edges: ids + table rows of edge t+1 are requested before edge t is consumed
+      int j = n0;
+      float4 eif[VPL], erp[VPL];
 #pragma unroll
-        for (int u = 0; u < VPL; ++u) eif[u] = erp[u] = f4zero();
-        auto fetch = [&](int p, bool on) {
-          j = n0;
-          int ia = 0, ib = 0;
-          if (on) {
-            const int le = p - e_lo;
-            if (FAST || le < ne_s) {
-              j = ldsi(sa.e0 + le * 4);
-              if (HAS_E) {
-                const int id = ldsi(sa.e1 + le * 4);
-                ia = ID_IF(id);
-                ib = ID_RPC(id);
-              }
-            } else {
-              j = __ldg(a.csr_src + p);
-              if (HAS_E) {
-                ia = __ldg(a.csr_if + p);
-                ib = __ldg(a.csr_rpc + p);
-              }
-            }
-          }
-          if (HAS_E) {
-            ldrow(a.t_if, (size_t)ia, eif);
-            ldrow(a.t_rpc, (size_t)ib, erp);
-          }
-        };
-        fetch(p0, 0 < deg);
-        for (int t = 0; t < degmax; ++t) {
-          const bool on = t < deg;
-          const int p = p0 + t;
-          const int cj = j;
-          float4 e[VPL];
-#pragma unroll
-          for (int u = 0; u < VPL; ++u) e[u] = f4add(eif[u], erp[u]);
-          fetch(p + 1, t + 1 < deg);
-          float4 kk[VPL], vv[VPL];
-          const unsigned sl = (unsigned)(cj - n0);
-          if (FAST || sl < (unsigned)nt) {
-#pragma unroll
-            for (int u = 0; u < VPL; ++u) {
-              kk[u] = lds4s(sa.ta + sl * (H * 4) + (lig + u * LPR) * 16);
-              vv[u] = lds4s(sa.tb + sl * (H * 4) + (lig + u * LPR) * 16);
+      for (int u = 0; u < VPL; ++u) eif[u] = erp[u] = f4zero();
+      auto fetch = [&](int p, bool on) {
+        j = n0;
+        int ia = 0, ib = 0;
+        if (on) {
+          const int le = p - e_lo;
+          if (FAST || le < ne_s) {
+            j = ldsi(sa.e0 + le * 4);
+            if (HAS_E) {
+              const int id = ldsi(sa.e1 + le * 4);
+              ia = ID_IF(id);
+              ib = ID_RPC(id);
             }
           } else {
-            ldrow(a.k, (size_t)cj, kk);
-            ldrow(a.v, (size_t)cj, vv);
-          }
-          float part = 0.f;
-#pragma unroll
-          for (int u = 0; u < VPL; ++u) {
+            j = __ldg(a.csr_src + p);
             if (HAS_E) {
-              kk[u] = f4add(kk[u], e[u]);
-              vv[u] = f4add(vv[u], e[u]);
+              ia = __ldg(a.csr_if + p);
+              ib = __ldg(a.csr_rpc + p);
             }
-            part += f4dot(q[u], kk[u]);
-          }
-          const float s = gsum_full<LPR>(part);
-          if (on && lig == 0) {
-            const int le = p - e_lo;
-            if (FAST || le < ne_s) stsf(sa.f0 + le * 4, s);
-            else a.alpha[p] = s;
-          }
-          const float mn = on ? fmaxf(m, s) : m;
-          const float sc = on ? ex2(m - mn) : 1.f;
-          const float pz = on ? ex2(s - mn) : 0.f;
-          Z = fmaf(Z, sc, pz);
-#pragma unroll
-          for (int u = 0; u < VPL; ++u) {
-            acc[u].x = fmaf(pz, vv[u].x, acc[u].x * sc);
-            acc[u].y = fmaf(pz, vv[u].y, acc[u].y * sc);
-            acc[u].z = fmaf(pz, vv[u].z, acc[u].z * sc);
-            acc[u].w = fmaf(pz, vv[u].w, acc[u].w * sc);
-          }
-          m = mn;
-        }
-        const float invZ = 1.0f / (Z + 1e-16f);
-        if (valid) {
-          // padded batch: only the real nodes (below live[0]) enter the statistics.  Read per node, not kept in a
-          // register across the edge loop (a volatile load is not hoisted; it hits L1 after the first node)
-          const bool counted = !a.live || i < *reinterpret_cast<const volatile long long*>(a.live);
-#pragma unroll
-          for (int u = 0; u < VPL; ++u) {
-            const float4 o = f4add(f4scale(invZ, acc[u]), skip[u]);
-            st4(a.out + (size_t)i * H + (lig + u * LPR) * 4, o);
-            if (!counted) continue;
-            bsum[u] = f4add(bsum[u], o);
-            bsq[u].x = fmaf(o.x, o.x, bsq[u].x); bsq[u].y = fmaf(o.y, o.y, bsq[u].y);
-            bsq[u].z = fmaf(o.z, o.z, bsq[u].z); bsq[u].w = fmaf(o.w, o.w, bsq[u].w);
           }
         }
-        __syncwarp();
-        for (int p = p0 + lig; p < p1; p += LPR) {
+        if (HAS_E) {
+          ldrow(a.t_if, (size_t)ia, eif);
+          ldrow(a.t_rpc, (size_t)ib, erp);
+        }
+      };
+      fetch(p0, 0 < deg);
+      for (int t = 0; t < degmax; ++t) {
+        const bool on = t < deg;
+        const int p = p0 + t;
+        const int cj = j;
+        float4 e[VPL];
+#pragma unroll
+        for (int u = 0; u < VPL; ++u) e[u] = f4add(eif[u], erp[u]);
+        fetch(p + 1, t + 1 < deg);
+        float4 kk[VPL], vv[VPL];
+        const unsigned sl = (unsigned)(cj - n0);
+        if (FAST || sl < (unsigned)nt) {
+#pragma unroll
+          for (int u = 0; u < VPL; ++u) {
+            kk[u] = lds4s(sa.ta + sl * (H * 4) + (lig + u * LPR) * 16);
+            vv[u] = lds4s(sa.tb + sl * (H * 4) + (lig + u * LPR) * 16);
+          }
+        } else {
+          ldrow(a.k, (size_t)cj, kk);
+          ldrow(a.v, (size_t)cj, vv);
+        }
+        float part = 0.f;
+#pragma unroll
+        for (int u = 0; u < VPL; ++u) {
+          if (HAS_E) {
+            kk[u] = f4add(kk[u], e[u]);
+            vv[u] = f4add(vv[u], e[u]);
+          }
+          part += f4dot(q[u], kk[u]);
+        }
+        const float s = gsum_full<LPR>(part);
+        if (on && lig == 0) {
           const int le = p - e_lo;
-          const float s = (FAST || le < ne_s) ? ldsf(sa.f0 + le * 4) : a.alpha[p];
-          a.alpha[p] = ex2(s - m) * invZ;
+          if (FAST || le < ne_s) stsf(sa.f0 + le * 4, s);
+          else a.alpha[p] = s;
+        }
+        const float mn = on ? fmaxf(m, s) : m;
+        const float sc = on ? ex2(m - mn) : 1.f;
+        const float pz = on ? ex2(s - mn) : 0.f;
+        Z = fmaf(Z, sc, pz);
+#pragma unroll
+        for (int u = 0; u < VPL; ++u) {
+          acc[u].x = fmaf(pz, vv[u].x, acc[u].x * sc);
+          acc[u].y = fmaf(pz, vv[u].y, acc[u].y * sc);
+          acc[u].z = fmaf(pz, vv[u].z, acc[u].z * sc);
+          acc[u].w = fmaf(pz, vv[u].w, acc[u].w * sc);
+        }
+        m = mn;
+      }
+      const float invZ = 1.0f / (Z + 1e-16f);
+      if (valid) {
+        // padded batch: only the real nodes (below live[0]) enter the statistics.  Read per node, not kept in a
+        // register across the edge loop (a volatile load is not hoisted; it hits L1 after the first node)
+        const bool counted = !a.live || i < *reinterpret_cast<const volatile long long*>(a.live);
+#pragma unroll
+        for (int u = 0; u < VPL; ++u) {
+          const float4 o = f4add(f4scale(invZ, acc[u]), skip[u]);
+          st4(a.out + (size_t)i * H + (lig + u * LPR) * 4, o);
+          if (!counted) continue;
+          bsum[u] = f4add(bsum[u], o);
+          bsq[u].x = fmaf(o.x, o.x, bsq[u].x); bsq[u].y = fmaf(o.y, o.y, bsq[u].y);
+          bsq[u].z = fmaf(o.z, o.z, bsq[u].z); bsq[u].w = fmaf(o.w, o.w, bsq[u].w);
         }
       }
-    };
-    if (all_in) run(std::true_type{});
-    else run(std::false_type{});
-  }
+      __syncwarp();
+      for (int p = p0 + lig; p < p1; p += LPR) {
+        const int le = p - e_lo;
+        const float s = (FAST || le < ne_s) ? ldsf(sa.f0 + le * 4) : a.alpha[p];
+        a.alpha[p] = ex2(s - m) * invZ;
+      }
+    }
+  };
+  if (all_in) run(std::true_type{});
+  else run(std::false_type{});
   if (a.bn_acc) {
-    // BatchNorm statistics of this layer's output, fused: column sums and sums of squares over the CTA's tiles (per-lane
+    // BatchNorm statistics of this layer's output, fused: column sums and sums of squares over the CTA's tile (per-lane
     // fp32 partials, combined in fp64) -> one fp64 atomic per column and CTA into bn_acc, the accumulator k_bn_apply
     // derives mean / rstd from (nodeops.cu).  Saves the separate statistics pass over `out`.
     __syncthreads();                                   // every warp is done with the staged tiles
@@ -485,166 +445,165 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
 #pragma unroll
     for (int u = 0; u < VPL; ++u) v[u] = ldg4(base + row * H + (lig + u * LPR) * 4);
   };
-  tile_barrier_init(S, tid);
-  uint32_t phase = 0;
   int n0, nt;
-  for (bool first = true; next_tile(a, first, n0, nt); first = false, phase ^= 1) {
-    stage_tiles<H, NT>(S, a.k, a.v, a.rowptr, n0, nt, tid);
-    const int e_lo = S.ptr[0];
-    const int ne_c = min(S.ptr[nt] - e_lo, a.edge_cap);
-    int bad = 0, wide = 0;   // a staged neighbour outside this tile / staged ids that do not pack
-    for (int x = tid; x < ne_c; x += NT) {
-      const int nb_id = __ldg(a.csr_src + e_lo + x);
-      S.e0[x] = nb_id;
-      bad |= (unsigned)(nb_id - n0) >= (unsigned)nt;
-      S.f0[x] = __ldg(a.alpha + e_lo + x);
-      if (HAS_E) {
-        const int ia = __ldg(a.csr_if + e_lo + x), ib = __ldg(a.csr_rpc + e_lo + x);
-        wide |= !packable(ia, ib);
-        S.e1[x] = PACK_ID(ia, ib);
-      }
+  cta_tile(a, n0, nt);
+  if (nt <= 0) return;                         // uniform across the CTA
+  tile_barrier_init(S, tid);
+  stage_tiles<H, NT>(S, a.k, a.v, a.rowptr, n0, nt, tid);
+  const int e_lo = S.ptr[0];
+  const int ne_c = min(S.ptr[nt] - e_lo, a.edge_cap);
+  int bad = 0, wide = 0;   // a staged neighbour outside this tile / staged ids that do not pack
+  for (int x = tid; x < ne_c; x += NT) {
+    const int nb_id = __ldg(a.csr_src + e_lo + x);
+    S.e0[x] = nb_id;
+    bad |= (unsigned)(nb_id - n0) >= (unsigned)nt;
+    S.f0[x] = __ldg(a.alpha + e_lo + x);
+    if (HAS_E) {
+      const int ia = __ldg(a.csr_if + e_lo + x), ib = __ldg(a.csr_rpc + e_lo + x);
+      wide |= !packable(ia, ib);
+      S.e1[x] = PACK_ID(ia, ib);
     }
-    // fast variant of the edge loops when every edge of the tile is staged and every neighbour row is in the tile
-    // (whole-graph tiles): no global-memory fallbacks are compiled into it
-    // (one barrier in the common case; a second one tells unpackable ids from neighbours outside the tile)
-    const bool any = __syncthreads_or(bad | wide) != 0;
-    const bool narrow = !(HAS_E && any && __syncthreads_or(wide));   // else every edge takes the global path
-    const int ne_s = narrow ? ne_c : 0;
-    const bool all_in = !any && (S.ptr[nt] - e_lo <= a.edge_cap);
-    mbar_wait(S.bar, phase);
+  }
+  // fast variant of the edge loops when every edge of the tile is staged and every neighbour row is in the tile
+  // (whole-graph tiles): no global-memory fallbacks are compiled into it
+  // (one barrier in the common case; a second one tells unpackable ids from neighbours outside the tile)
+  const bool any = __syncthreads_or(bad | wide) != 0;
+  const bool narrow = !(HAS_E && any && __syncthreads_or(wide));   // else every edge takes the global path
+  const int ne_s = narrow ? ne_c : 0;
+  const bool all_in = !any && (S.ptr[nt] - e_lo <= a.edge_cap);
+  mbar_wait(S.bar, 0);
 
-    int slot = g0 + grp;
-    int loc = slot < nt ? ldsu16(sa.ord + slot * 2) : 0;
-    float4 g_n[VPL];
+  int slot = g0 + grp;
+  int loc = slot < nt ? ldsu16(sa.ord + slot * 2) : 0;
+  float4 g_n[VPL];
 #pragma unroll
-    for (int u = 0; u < VPL; ++u) g_n[u] = f4zero();
-    if (slot < nt) ldrow(a.g, (size_t)(n0 + loc), g_n);
-    auto run = [&](auto fast_c) {
-      constexpr bool FAST = decltype(fast_c)::value;
-      for (; slot - grp < nt; slot += GPC) {
-        const bool valid = slot < nt;
-        const int i = n0 + loc;
-        float4 g[VPL];
+  for (int u = 0; u < VPL; ++u) g_n[u] = f4zero();
+  if (slot < nt) ldrow(a.g, (size_t)(n0 + loc), g_n);
+  auto run = [&](auto fast_c) {
+    constexpr bool FAST = decltype(fast_c)::value;
+    for (; slot - grp < nt; slot += GPC) {
+      const bool valid = slot < nt;
+      const int i = n0 + loc;
+      float4 g[VPL];
 #pragma unroll
-        for (int u = 0; u < VPL; ++u) g[u] = g_n[u];
-        const int p0 = valid ? ldsi(sa.ptr + loc * 4) : 0;
-        const int p1 = valid ? ldsi(sa.ptr + loc * 4 + 4) : 0;
-        if (slot + GPC < nt) {
-          loc = ldsu16(sa.ord + (slot + GPC) * 2);
-          ldrow(a.g, (size_t)(n0 + loc), g_n);
-        }
-        const int deg = p1 - p0;
-        const int degmax = __reduce_max_sync(0xffffffffu, deg);
-        // one edge record: source row offsets + e = T_if[a] + T_rpc[b]
-        auto edge = [&](int p, bool on, int& j, float& al, float4 (&e)[VPL], int& rid) {
-          j = n0;
-          al = 0.f;
-          int ia = 0, ib = 0;
-          if (on) {
-            const int le = p - e_lo;
-            if (FAST || le < ne_s) {
-              j = ldsi(sa.e0 + le * 4);
-              al = ldsf(sa.f0 + le * 4);
-              if (HAS_E) {
-                const int id = ldsi(sa.e1 + le * 4);
-                ia = ID_IF(id);
-                ib = ID_RPC(id);
-              }
-            } else {
-              j = __ldg(a.csr_src + p);
-              al = __ldg(a.alpha + p);
-              if (HAS_E) {
-                ia = __ldg(a.csr_if + p);
-                ib = __ldg(a.csr_rpc + p);
-              }
-            }
-          }
-#pragma unroll
-          for (int u = 0; u < VPL; ++u) {
-            e[u] = f4zero();
-            if (HAS_E)
-              e[u] = f4add(ldg4(a.t_if + (size_t)ia * H + (lig + u * LPR) * 4),
-                           ldg4(a.t_rpc + ib * H + (lig + u * LPR) * 4));
-          }
-          rid = ib;
-        };
-        // ONE pass over the in-edges.  With d_t = <g_i, v_j + e_t> (shifted by the first edge's value c, which cancels
-        // exactly: sum_t ds_t = 0), w_t = alpha_t (d_t - c) and dot = sum_t w_t:
-        //   ds_t = alpha_t (d_t - c - dot) / sqrt(C)
-        //   dq_i = sum_t ds_t (k_j + e_t) = (P - dot Q) / sqrt(C),   P = sum_t w_t (k_j + e_t),  Q = sum_t alpha_t (k_j + e_t)
-        // so k_j, v_j and the table rows of an edge are fetched once (the two-pass form fetched the edge record and
-        // its table rows twice); ds_t is written by a scalar post-pass with the lanes spread over the node's edges.
-        float dot = 0.f, c_shift = 0.f;
-        float4 P[VPL], Q[VPL];
-#pragma unroll
-        for (int u = 0; u < VPL; ++u) P[u] = Q[u] = f4zero();
-        float sumA = 0.f, sumW = 0.f;          // lane b: sums of alpha / w over this node's in-edges of rpc type b
-        for (int t = 0; t < degmax; ++t) {
-          const bool on = t < deg;
-          const int p = p0 + t;
-          int j, rid;
-          float al;
-          float4 e[VPL];
-          edge(p, on, j, al, e, rid);
-          float4 kk[VPL], vv[VPL];
-          const unsigned sl = (unsigned)(j - n0);
-          if (FAST || sl < (unsigned)nt) {
-#pragma unroll
-            for (int u = 0; u < VPL; ++u) {
-              kk[u] = lds4s(sa.ta + sl * (H * 4) + (lig + u * LPR) * 16);
-              vv[u] = lds4s(sa.tb + sl * (H * 4) + (lig + u * LPR) * 16);
+      for (int u = 0; u < VPL; ++u) g[u] = g_n[u];
+      const int p0 = valid ? ldsi(sa.ptr + loc * 4) : 0;
+      const int p1 = valid ? ldsi(sa.ptr + loc * 4 + 4) : 0;
+      if (slot + GPC < nt) {
+        loc = ldsu16(sa.ord + (slot + GPC) * 2);
+        ldrow(a.g, (size_t)(n0 + loc), g_n);
+      }
+      const int deg = p1 - p0;
+      const int degmax = __reduce_max_sync(0xffffffffu, deg);
+      // one edge record: source row offsets + e = T_if[a] + T_rpc[b]
+      auto edge = [&](int p, bool on, int& j, float& al, float4 (&e)[VPL], int& rid) {
+        j = n0;
+        al = 0.f;
+        int ia = 0, ib = 0;
+        if (on) {
+          const int le = p - e_lo;
+          if (FAST || le < ne_s) {
+            j = ldsi(sa.e0 + le * 4);
+            al = ldsf(sa.f0 + le * 4);
+            if (HAS_E) {
+              const int id = ldsi(sa.e1 + le * 4);
+              ia = ID_IF(id);
+              ib = ID_RPC(id);
             }
           } else {
-            ldrow(a.k, (size_t)j, kk);
-            ldrow(a.v, (size_t)j, vv);
-          }
-          float part = 0.f;
-#pragma unroll
-          for (int u = 0; u < VPL; ++u) part += f4dot(g[u], f4add(vv[u], e[u]));
-          const float da = gsum_full<LPR>(part);
-          if (t == 0) c_shift = da;
-          const float dc = da - c_shift;
-          const float w = al * dc;             // alpha is 0 on finished groups
-          dot += w;
-#pragma unroll
-          for (int u = 0; u < VPL; ++u) {
-            const float4 ke = f4add(kk[u], e[u]);
-            P[u] = f4fma(w, ke, P[u]);
-            Q[u] = f4fma(al, ke, Q[u]);
-          }
-          if (HAS_E && on && lig == rid) { sumA += al; sumW += w; }
-          if (on && lig == 0) {
-            const int le = p - e_lo;
-            if (FAST || le < ne_s) stsf(sa.f1 + le * 4, dc);
-            else a.dsp[p] = dc;
+            j = __ldg(a.csr_src + p);
+            al = __ldg(a.alpha + p);
+            if (HAS_E) {
+              ia = __ldg(a.csr_if + p);
+              ib = __ldg(a.csr_rpc + p);
+            }
           }
         }
-        const float sumS = (sumW - dot * sumA) * a.inv_sqrt_c;
-        __syncwarp();
-        for (int p = p0 + lig; p < p1; p += LPR) {
+#pragma unroll
+        for (int u = 0; u < VPL; ++u) {
+          e[u] = f4zero();
+          if (HAS_E)
+            e[u] = f4add(ldg4(a.t_if + (size_t)ia * H + (lig + u * LPR) * 4),
+                         ldg4(a.t_rpc + ib * H + (lig + u * LPR) * 4));
+        }
+        rid = ib;
+      };
+      // ONE pass over the in-edges.  With d_t = <g_i, v_j + e_t> (shifted by the first edge's value c, which cancels
+      // exactly: sum_t ds_t = 0), w_t = alpha_t (d_t - c) and dot = sum_t w_t:
+      //   ds_t = alpha_t (d_t - c - dot) / sqrt(C)
+      //   dq_i = sum_t ds_t (k_j + e_t) = (P - dot Q) / sqrt(C),   P = sum_t w_t (k_j + e_t),  Q = sum_t alpha_t (k_j + e_t)
+      // so k_j, v_j and the table rows of an edge are fetched once (the two-pass form fetched the edge record and
+      // its table rows twice); ds_t is written by a scalar post-pass with the lanes spread over the node's edges.
+      float dot = 0.f, c_shift = 0.f;
+      float4 P[VPL], Q[VPL];
+#pragma unroll
+      for (int u = 0; u < VPL; ++u) P[u] = Q[u] = f4zero();
+      float sumA = 0.f, sumW = 0.f;          // lane b: sums of alpha / w over this node's in-edges of rpc type b
+      for (int t = 0; t < degmax; ++t) {
+        const bool on = t < deg;
+        const int p = p0 + t;
+        int j, rid;
+        float al;
+        float4 e[VPL];
+        edge(p, on, j, al, e, rid);
+        float4 kk[VPL], vv[VPL];
+        const unsigned sl = (unsigned)(j - n0);
+        if (FAST || sl < (unsigned)nt) {
+#pragma unroll
+          for (int u = 0; u < VPL; ++u) {
+            kk[u] = lds4s(sa.ta + sl * (H * 4) + (lig + u * LPR) * 16);
+            vv[u] = lds4s(sa.tb + sl * (H * 4) + (lig + u * LPR) * 16);
+          }
+        } else {
+          ldrow(a.k, (size_t)j, kk);
+          ldrow(a.v, (size_t)j, vv);
+        }
+        float part = 0.f;
+#pragma unroll
+        for (int u = 0; u < VPL; ++u) part += f4dot(g[u], f4add(vv[u], e[u]));
+        const float da = gsum_full<LPR>(part);
+        if (t == 0) c_shift = da;
+        const float dc = da - c_shift;
+        const float w = al * dc;             // alpha is 0 on finished groups
+        dot += w;
+#pragma unroll
+        for (int u = 0; u < VPL; ++u) {
+          const float4 ke = f4add(kk[u], e[u]);
+          P[u] = f4fma(w, ke, P[u]);
+          Q[u] = f4fma(al, ke, Q[u]);
+        }
+        if (HAS_E && on && lig == rid) { sumA += al; sumW += w; }
+        if (on && lig == 0) {
           const int le = p - e_lo;
-          const float dc = (FAST || le < ne_s) ? ldsf(sa.f1 + le * 4) : a.dsp[p];
-          const float al = (FAST || le < ne_s) ? ldsf(sa.f0 + le * 4) : __ldg(a.alpha + p);
-          a.dsp[p] = al * (dc - dot) * a.inv_sqrt_c;
-        }
-        if (valid) {
-#pragma unroll
-          for (int u = 0; u < VPL; ++u) {
-            float4 dq;
-            dq.x = (P[u].x - dot * Q[u].x) * a.inv_sqrt_c; dq.y = (P[u].y - dot * Q[u].y) * a.inv_sqrt_c;
-            dq.z = (P[u].z - dot * Q[u].z) * a.inv_sqrt_c; dq.w = (P[u].w - dot * Q[u].w) * a.inv_sqrt_c;
-            st4(a.out + (size_t)i * H + (lig + u * LPR) * 4, dq);
-          }
-        }
-        if (HAS_E && a.rpc_ws && valid && lig < RPC_FAST) {
-          a.rpc_ws[(size_t)i * 2 * RPC_FAST + lig] = sumA;
-          a.rpc_ws[(size_t)i * 2 * RPC_FAST + RPC_FAST + lig] = sumS;
+          if (FAST || le < ne_s) stsf(sa.f1 + le * 4, dc);
+          else a.dsp[p] = dc;
         }
       }
-    };
-    if (all_in) run(std::true_type{});
-    else run(std::false_type{});
-  }
+      const float sumS = (sumW - dot * sumA) * a.inv_sqrt_c;
+      __syncwarp();
+      for (int p = p0 + lig; p < p1; p += LPR) {
+        const int le = p - e_lo;
+        const float dc = (FAST || le < ne_s) ? ldsf(sa.f1 + le * 4) : a.dsp[p];
+        const float al = (FAST || le < ne_s) ? ldsf(sa.f0 + le * 4) : __ldg(a.alpha + p);
+        a.dsp[p] = al * (dc - dot) * a.inv_sqrt_c;
+      }
+      if (valid) {
+#pragma unroll
+        for (int u = 0; u < VPL; ++u) {
+          float4 dq;
+          dq.x = (P[u].x - dot * Q[u].x) * a.inv_sqrt_c; dq.y = (P[u].y - dot * Q[u].y) * a.inv_sqrt_c;
+          dq.z = (P[u].z - dot * Q[u].z) * a.inv_sqrt_c; dq.w = (P[u].w - dot * Q[u].w) * a.inv_sqrt_c;
+          st4(a.out + (size_t)i * H + (lig + u * LPR) * 4, dq);
+        }
+      }
+      if (HAS_E && a.rpc_ws && valid && lig < RPC_FAST) {
+        a.rpc_ws[(size_t)i * 2 * RPC_FAST + lig] = sumA;
+        a.rpc_ws[(size_t)i * 2 * RPC_FAST + RPC_FAST + lig] = sumS;
+      }
+    }
+  };
+  if (all_in) run(std::true_type{});
+  else run(std::false_type{});
 }
 
 // ============================================================== backward, source pass (dk, dv, table grads)
@@ -665,15 +624,15 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
   // Interface id `hot_if` (0: what the reference writes on every chain and return edge of a PERT graph, misc.py:247,289,
   // i.e. 3 of 4 edges of real data) would serialise tens of thousands of REDG.128 on ONE 4H-byte row per layer.  Its
   // contributions stay in registers
-  // and leave once per CTA (through the first row of tile A, which is dead after the tile loop: the geometry of cfg2
+  // and leave once per CTA (through the first row of tile A, which is dead after the edge loops: the geometry of cfg2
   // fits its 200-node graphs into a two-CTA tile with less than 256 bytes to spare).
   float4 hot[VPL];
 #pragma unroll
   for (int u = 0; u < VPL; ++u) hot[u] = f4zero();
-  tile_barrier_init(S, tid);
-  uint32_t phase = 0;
   int n0, nt;
-  for (bool first = true; next_tile(a, first, n0, nt); first = false, phase ^= 1) {
+  cta_tile(a, n0, nt);
+  if (nt <= 0) return;                         // uniform across the CTA
+  tile_barrier_init(S, tid);
   stage_tiles<H, NT>(S, a.g, a.q, a.colptr, n0, nt, tid);   // targets of a node's out-edges live in the same graph
   const int c_lo = S.ptr[0];
   const int ne_c = min(S.ptr[nt] - c_lo, a.edge_cap);
@@ -699,7 +658,7 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
   const bool narrow = !(HAS_E && any && __syncthreads_or(wide));   // else every edge takes the global path
   const int ne_s = narrow ? ne_c : 0;
   const bool all_in = !any && (S.ptr[nt] - c_lo <= a.edge_cap);
-  mbar_wait(S.bar, phase);
+  mbar_wait(S.bar, 0);
 
   auto run = [&](auto fast_c) {
     constexpr bool FAST = decltype(fast_c)::value;
@@ -797,7 +756,6 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
     for (int b = 0; b < RPC_FAST; ++b)
       if (b < a.n_rpc && acc[b] != 0.f) atomicAdd(s_drpc + b * H + col, acc[b]);
   }
-  }   // tile loop
   if (HAS_E) {
     __syncthreads();                       // every warp is done with the staged tiles
     float* s_hot = S.ta;
@@ -825,12 +783,15 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
 
 // Tile geometry: nodes per tile (T) and staged-edge capacity (ecap) within the per-CTA shared-memory budget -- two CTAs
 // per SM ((233472 / 2) - 1024 reserved each) unless the average graph does not fit, then one.  ONE geometry serves the
-// three kernels of a layer (sized for the most demanding one: 4 per-edge arrays + the privatised rpc table), so one
-// tile list does too.
+// three kernels of a layer (sized for the most demanding one: 4 per-edge arrays + the privatised rpc table).  Tiles are
+// T consecutive nodes, one per CTA.  N % B == 0 is a hint, not a proof: should the graphs differ after all, the tiles
+// cut some of them and those CTAs run the global-gather variant of the edge loops (same results, slower).
 struct TileGeom {
   int T, ecap;
 };
-constexpr int STATIC_SMEM = 160;   // s_tile + s_hist[34] of the kernels' static shared memory, rounded up
+// Room kept for the kernels' static shared memory (s_hist[34]: 136 B).  T, ecap and the CTAs per SM depend on this
+// value, and with them the order of every tile sum, so it is not tightened to the bytes in use.
+constexpr int STATIC_SMEM = 160;
 TileGeom tile_geom(int H, int n_rpc, long long N, long long E, long long B) {
   const double budget2 = 115712.0 - STATIC_SMEM, budget1 = 231424.0 - STATIC_SMEM;
   const double deg = N > 0 ? (double)E / (double)N : 1.0;
@@ -839,7 +800,7 @@ TileGeom tile_geom(int H, int n_rpc, long long N, long long E, long long B) {
   auto fit = [&](double b) { return (long long)((b - fixed) / per_node); };
   long long T = fit(budget2);
   const double avg = B > 0 ? (double)N / (double)B : 0.0;
-  const bool uniform = B > 0 && N % B == 0;                 // equally sized graphs (hint; the tile list does not rely on it)
+  const bool uniform = B > 0 && N % B == 0;                 // equally sized graphs (a hint, see above)
   // two CTAs per SM when the graphs fit such a tile (exactly, if they are uniform; comfortably -- average <= 60 % of the
   // tile -- if their sizes vary: larger ones would be cut); else whole-SM tiles that pack one or two graphs
   const bool two = T >= 64 && (avg == 0.0 || (uniform ? avg <= (double)T : avg <= 0.6 * (double)T));
@@ -853,109 +814,19 @@ TileGeom tile_geom(int H, int n_rpc, long long N, long long E, long long B) {
   return TileGeom{(int)T, ecap};
 }
 
-// ---- graph-aligned tile list: greedy packing of WHOLE graphs (never cut while a graph fits a tile) up to T nodes /
-// ecap edges; a graph that alone exceeds a tile is cut into T-node pieces (those tiles run the global-gather variant).
-// Two kernels: (1) graph boundaries from the sorted `batch` vector, fully parallel (a node that starts a graph writes
-// its index; depends only on the batch vector, so the engine issues it beside the input prologue); (2) one CTA: the
-// boundaries and the edge offsets of the graph starts go to shared memory in parallel, then a serial packing pass over
-// the B graphs (~10 cycles per graph).  batch == nullptr: fixed T-node tiles.
-__global__ void k_tile_bounds(const int64_t* __restrict__ batch, int N, int B, int* __restrict__ gptr) {
-  const int n = blockIdx.x * blockDim.x + threadIdx.x;
-  if (n == 0) gptr[B] = N;
-  if (n >= N) return;
-  const int64_t g = batch[n];
-  if (g < 0 || g >= B) return;
-  if (n == 0 || batch[n - 1] != g) gptr[g] = n;     // gptr was filled with -1: graphs without nodes stay -1
-}
-__global__ void __launch_bounds__(1024) k_build_tiles(int has_batch, int N, int B, const int* __restrict__ rowptr, int T,
-                                                      int ecap, const int* __restrict__ gptr,
-                                                      int* __restrict__ tile_ptr, int* __restrict__ ntiles,
-                                                      int max_tiles) {
-  extern __shared__ int sg[];   // gptr copy [B+1] | edge offset of every graph start [B+1] | nxt [B+1]
-  const int tid = threadIdx.x;
-  if (!has_batch || B <= 0) {
-    const int nt = (N + T - 1) / T;
-    for (int t = tid; t <= nt && t <= max_tiles; t += blockDim.x) tile_ptr[t] = min(t * T, N);
-    if (tid == 0) *ntiles = min(nt, max_tiles);
-    return;
-  }
-  for (int g = tid; g <= B; g += blockDim.x) sg[g] = gptr[g];
-  __syncthreads();
-  if (tid == 0)                                     // graphs without nodes start where the next graph starts
-    for (int g = B - 1; g >= 0; --g)
-      if (sg[g] < 0) sg[g] = sg[g + 1];
-  __syncthreads();
-  for (int g = tid; g <= B; g += blockDim.x) sg[B + 1 + g] = rowptr[sg[g]];
-  __syncthreads();
-  // nxt[g] = first graph that no longer fits a tile opened at graph g (node AND edge capacity; binary search over the two
-  // prefix arrays, all graphs in parallel).  A graph that exceeds a tile on its own gets nxt = g + 1 and is cut below.
-  int* nxt = sg + 2 * (B + 1);
-  const int* cn = sg;
-  const int* ce = sg + B + 1;
-  for (int g = tid; g < B; g += blockDim.x) {
-    int lo = g + 1, hi = B;             // largest h in [g+1, B] with cn[h]-cn[g] <= T and ce[h]-ce[g] <= ecap
-    if (cn[lo] - cn[g] > T || ce[lo] - ce[g] > ecap) {
-      nxt[g] = g + 1;
-      continue;
-    }
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (cn[mid] - cn[g] <= T && ce[mid] - ce[g] <= ecap) lo = mid;
-      else hi = mid - 1;
-    }
-    nxt[g] = lo;
-  }
-  __syncthreads();
-  if (tid != 0) return;
-  // the tile sequence is the chain 0 -> nxt[0] -> nxt[nxt[0]] ...: one dependent shared-memory load per TILE
-  int nt = 0, last = cn[0];
-  tile_ptr[0] = last;
-  auto close_at = [&](int node) {
-    if (node > last && nt < max_tiles) {
-      tile_ptr[++nt] = node;
-      last = node;
-    }
-  };
-  for (int g = 0; g < B;) {
-    const int h = nxt[g];
-    if (h == g + 1 && (cn[h] - cn[g] > T || ce[h] - ce[g] > ecap)) {   // oversize graph: T-node pieces
-      for (int x = cn[g]; x < cn[h]; x += T) close_at(min(x + T, cn[h]));
-    } else {
-      close_at(cn[h]);
-    }
-    g = h;
-  }
-  if (last < N) close_at(N);                   // nodes after the last graph boundary (defensive)
-  *ntiles = nt;
-}
-
 template <typename K>
 int set_smem(K kernel, size_t bytes) {
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
   return e == cudaSuccess ? 0 : (int)e;
 }
 
-// grid + tile fields of a launch: with a tile list, persistent CTAs (as many as fit the SMs) draw tiles by ticket.
-// Returns the CTAs per SM the shared-memory footprint allows (2 -> 512-thread CTAs, 1 -> 1024-thread CTAs).
-int plan_launch(TileArgs& a, const PertTiles* tl, const TileGeom& g, size_t bytes, long long N, int& grid) {
+// grid + tile fields of a launch: one T-node tile per CTA.  Returns the CTAs per SM the shared-memory footprint allows
+// (2 -> 512-thread CTAs, 256 for the VPL = 2 forward; 1 -> 1024-thread CTAs).
+int plan_launch(TileArgs& a, const TileGeom& g, size_t bytes, long long N, int& grid) {
   a.tile_nodes = g.T;
   a.edge_cap = g.ecap;
-  a.tile_ptr = nullptr;
-  a.ntiles = nullptr;
-  a.ticket = nullptr;
-  const int per_sm = bytes + STATIC_SMEM + 1024 <= 233472 / 2 ? 2 : 1;
-  if (!tl) {
-    grid = pert_cdiv(N, g.T);
-    return per_sm;
-  }
-  a.tile_ptr = tl->tile_ptr;
-  a.ntiles = tl->ntiles;
-  a.ticket = pert_ticket_slot();
-  if (!a.ticket) return -1;
-  grid = PERT_NUM_SMS * per_sm;
-  if (grid > tl->max_tiles) grid = tl->max_tiles;
-  if (grid < 1) grid = 1;
-  return per_sm;
+  grid = pert_cdiv(N, g.T);
+  return bytes + STATIC_SMEM + 1024 <= 233472 / 2 ? 2 : 1;
 }
 
 template <typename K>
@@ -967,68 +838,36 @@ int launch_k(K kernel, int grid, int threads, size_t bytes, const TileArgs& a, c
 }
 
 // forward launch for row width H: the VPL = 2 variant (LPR = H / 8 lanes per node, 256-thread CTAs with up to 128
-// registers, still two CTAs per SM) when two CTAs fit an SM, else VPL = 1 with 1024-thread CTAs.  PERT_TCONV_VPL=1 forces
-// the one-vector-per-lane kernels (A/B).
-static int fwd_vpl() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("PERT_TCONV_VPL");
-    v = (e && e[0] == '1') ? 1 : 2;
-  }
-  return v;
-}
+// registers, still two CTAs per SM) when two CTAs fit an SM, else VPL = 1 with 1024-thread CTAs.
 template <int H>
-int launch_fwd(const TileArgs& a0, long long N, long long E, long long B, bool has_e, const PertTiles* tl,
-               cudaStream_t st) {
-  const TileGeom g = tl ? TileGeom{tl->T, tl->ecap} : tile_geom(H, a0.n_rpc, N, E, B);
+int launch_fwd(const TileArgs& a0, long long N, long long E, long long B, bool has_e, cudaStream_t st) {
+  const TileGeom g = tile_geom(H, a0.n_rpc, N, E, B);
   const size_t bytes = smem_bytes(g.T, H, 0, g.ecap, 3);   // src, packed ids, logit staging
   TileArgs a = a0;
   int grid = 0;
-  const int per_sm = plan_launch(a, tl, g, bytes, N, grid);
-  if (per_sm < 0) return (int)cudaGetLastError();
-  if (per_sm == 2) {
-    if (fwd_vpl() == 2 && H >= 32)
-      return has_e ? launch_k(k_tile_fwd<H / 8, 2, true, 256>, grid, 256, bytes, a, st)
-                   : launch_k(k_tile_fwd<H / 8, 2, false, 256>, grid, 256, bytes, a, st);
-    return has_e ? launch_k(k_tile_fwd<H / 4, 1, true, 512>, grid, 512, bytes, a, st)
-                 : launch_k(k_tile_fwd<H / 4, 1, false, 512>, grid, 512, bytes, a, st);
-  }
+  if (plan_launch(a, g, bytes, N, grid) == 2)
+    return has_e ? launch_k(k_tile_fwd<H / 8, 2, true, 256>, grid, 256, bytes, a, st)
+                 : launch_k(k_tile_fwd<H / 8, 2, false, 256>, grid, 256, bytes, a, st);
   return has_e ? launch_k(k_tile_fwd<H / 4, 1, true, 1024>, grid, 1024, bytes, a, st)
                : launch_k(k_tile_fwd<H / 4, 1, false, 1024>, grid, 1024, bytes, a, st);
 }
+// backward launches for row width H: one vector per lane (LPR = H / 4), 512-thread CTAs when two CTAs fit an SM, else
+// 1024.  (The backward pair's REDG and shared-memory atomics want the resident warps more than the fewer instructions
+// of two vectors per lane.)
 template <int H>
-int launch_bwd(const TileArgs& a0, long long N, long long E, long long B, bool has_e, const PertTiles* tl,
-               cudaStream_t st) {
-  const TileGeom g = tl ? TileGeom{tl->T, tl->ecap} : tile_geom(H, a0.n_rpc, N, E, B);
+int launch_bwd(const TileArgs& a0, long long N, long long E, long long B, bool has_e, cudaStream_t st) {
+  const TileGeom g = tile_geom(H, a0.n_rpc, N, E, B);
   const size_t bd = smem_bytes(g.T, H, 0, g.ecap, 4);                      // src, ids, alpha, dalpha staging
   const size_t bs = smem_bytes(g.T, H, has_e ? a0.n_rpc : 0, g.ecap, 4);   // dst, ids, alpha, ds
   TileArgs ad = a0, as = a0;
   int gd = 0, gs = 0;
-  const int pd = plan_launch(ad, tl, g, bd, N, gd), ps = plan_launch(as, tl, g, bs, N, gs);
-  if (pd < 0 || ps < 0) return (int)cudaGetLastError();
-  // VPL = 2 (H / 8 lanes per node, 256-thread CTAs) whenever two CTAs share an SM and the rpc sums still have a lane per
-  // type (LPR >= RPC_FAST), i.e. H >= 64; else one vector per lane
-  // (the backward pair's REDG and shared-memory atomics want the resident warps more than fewer instructions, so the
-  // backward default stays one vector per lane; PERT_TCONV_VPL_BWD=2 selects the other for A/B.)
-  static int bwd_v = -1;
-  if (bwd_v < 0) {
-    const char* e = getenv("PERT_TCONV_VPL_BWD");
-    bwd_v = (e && e[0] == '2') ? 2 : 1;
-  }
-  const bool vpl2 = bwd_v == 2 && pd == 2 && ps == 2 && H / 8 >= RPC_FAST;
-  constexpr int L1 = H / 4, L2 = H / 8 > 0 ? H / 8 : 1;
+  const int pd = plan_launch(ad, g, bd, N, gd), ps = plan_launch(as, g, bs, N, gs);
+  constexpr int L1 = H / 4;
   // per-target rpc sums (see RPC_FAST) live in caller scratch; without it the general atomics path runs
-  const int lpr = vpl2 ? L2 : L1, nthr = vpl2 ? 256 : (ps == 2 ? 512 : 1024);
-  float* ws = (has_e && a0.n_rpc <= RPC_FAST && lpr >= RPC_FAST && nthr % H == 0) ? a0.rpc_ws : nullptr;
+  const int nthr = ps == 2 ? 512 : 1024;
+  float* ws = (has_e && a0.n_rpc <= RPC_FAST && L1 >= RPC_FAST && nthr % H == 0) ? a0.rpc_ws : nullptr;
   ad.rpc_ws = as.rpc_ws = ws;
   int rc;
-  if (vpl2) {
-    rc = has_e ? launch_k(k_tile_bwd_dst<L2, 2, true, 256>, gd, 256, bd, ad, st)
-               : launch_k(k_tile_bwd_dst<L2, 2, false, 256>, gd, 256, bd, ad, st);
-    if (rc) return rc;
-    return has_e ? launch_k(k_tile_bwd_src<L2, 2, true, 256>, gs, 256, bs, as, st)
-                 : launch_k(k_tile_bwd_src<L2, 2, false, 256>, gs, 256, bs, as, st);
-  }
   if (pd == 2)
     rc = has_e ? launch_k(k_tile_bwd_dst<L1, 1, true, 512>, gd, 512, bd, ad, st)
                : launch_k(k_tile_bwd_dst<L1, 1, false, 512>, gd, 512, bd, ad, st);
@@ -1050,7 +889,7 @@ int launch_bwd(const TileArgs& a0, long long N, long long E, long long B, bool h
 int pert_tile_fwd(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if, const float* t_rpc,
                   int n_rpc, float* out, int ld_out, float* alpha, long long N, long long E, long long B, int H,
-                  int C, double* bn_acc, const long long* live, const PertTiles* tiles, cudaStream_t st) {
+                  int C, double* bn_acc, const long long* live, cudaStream_t st) {
   if (ld != H || ld_out != H || (t_if && (size_t)n_rpc * H * 4 > 16 * 1024))
     return PERT_ERR_UNSUPPORTED;
   TileArgs a{};
@@ -1060,9 +899,9 @@ int pert_tile_fwd(const float* q, const float* k, const float* v, const float* s
   a.live = bn_acc ? live : nullptr;
   a.N = (int)N; a.inv_sqrt_c = 1.0f / sqrtf((float)C);
   switch (H) {
-    case 32: return launch_fwd<32>(a, N, E, B, t_if != nullptr, tiles, st);
-    case 64: return launch_fwd<64>(a, N, E, B, t_if != nullptr, tiles, st);
-    case 128: return launch_fwd<128>(a, N, E, B, t_if != nullptr, tiles, st);
+    case 32: return launch_fwd<32>(a, N, E, B, t_if != nullptr, st);
+    case 64: return launch_fwd<64>(a, N, E, B, t_if != nullptr, st);
+    case 128: return launch_fwd<128>(a, N, E, B, t_if != nullptr, st);
     default: return PERT_ERR_UNSUPPORTED;
   }
 }
@@ -1071,7 +910,7 @@ int pert_tile_bwd(const float* g_, int ld_g, const float* q, const float* k, con
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
                   const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha, float* dq, float* dk,
                   float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc, int n_rpc, long long N,
-                  long long E, long long B, int H, int C, const PertTiles* tiles, cudaStream_t st) {
+                  long long E, long long B, int H, int C, cudaStream_t st) {
   if (ld != H || ld_g != H || ld_d != H || (t_if && (size_t)n_rpc * H * 4 > 16 * 1024))
     return PERT_ERR_UNSUPPORTED;
   TileArgs a{};
@@ -1083,64 +922,9 @@ int pert_tile_bwd(const float* g_, int ld_g, const float* q, const float* k, con
   a.dt_if = dt_if; a.dt_rpc = dt_rpc; a.rpc_ws = rpc_ws; a.hot_if = 0;
   a.N = (int)N; a.inv_sqrt_c = 1.0f / sqrtf((float)C);
   switch (H) {
-    case 32: return launch_bwd<32>(a, N, E, B, t_if != nullptr, tiles, st);
-    case 64: return launch_bwd<64>(a, N, E, B, t_if != nullptr, tiles, st);
-    case 128: return launch_bwd<128>(a, N, E, B, t_if != nullptr, tiles, st);
+    case 32: return launch_bwd<32>(a, N, E, B, t_if != nullptr, st);
+    case 64: return launch_bwd<64>(a, N, E, B, t_if != nullptr, st);
+    case 128: return launch_bwd<128>(a, N, E, B, t_if != nullptr, st);
     default: return PERT_ERR_UNSUPPORTED;
   }
-}
-
-// Plans (host) and builds (device, stream-ordered) the graph-aligned tile list of a batch for row width H.
-// tiles_mem: int32 scratch of pert_tile_list_ints(N, B) (layout: ntiles | gptr [B+1] | tile_ptr [max_tiles+1]).
-long long pert_tile_list_ints(long long N, long long B) { return 1 + (B + 1) + (B + N / 32 + 8) + 1; }
-// Equally sized graphs (B divides N) whose size fits a two-CTA tile are served by FIXED tiles of whole graphs computed
-// arithmetically (no list, no ticket: ~8 % faster at the cfg2 headline shape than drawing the same tiles from a list).
-// N % B == 0 is a hint, not a proof: should the graphs differ after all, the fixed tiles cut some of them and those CTAs
-// run the global-gather variant of the edge loops (same results, slower) -- every other batch gets a tile list.
-bool pert_tile_fixed_ok(long long N, long long E, long long B, int H, int n_rpc) {
-  if (B <= 0 || N % B) return false;
-  const TileGeom g = tile_geom(H, n_rpc, N, E, B);
-  return N / B <= g.T;
-}
-// fills `out` (geometry + pointers into tiles_mem) without launching anything: what backward uses after forward built it
-int pert_tile_list_view(long long N, long long E, long long B, int H, int n_rpc, int* tiles_mem, PertTiles* out) {
-  if (!tiles_mem || !out || N <= 0) return PERT_ERR_BADARG;
-  if (H != 32 && H != 64 && H != 128) return PERT_ERR_UNSUPPORTED;
-  const TileGeom g = tile_geom(H, n_rpc, N, E, B);
-  out->T = g.T;
-  out->ecap = g.ecap;
-  out->max_tiles = (int)(B + N / 32 + 8);
-  if ((long long)B + pert_cdiv(N, g.T) + 2 > out->max_tiles) return PERT_ERR_UNSUPPORTED;
-  if ((size_t)3 * (B + 1) * sizeof(int) > 200 * 1024) return PERT_ERR_UNSUPPORTED;   // builder's shared-memory copy
-  out->ntiles = tiles_mem;
-  out->tile_ptr = tiles_mem + 1 + (B + 1);
-  return PERT_OK;
-}
-// step 1 (depends on the batch vector only): graph boundaries into the scratch
-int pert_tile_list_bounds(const int64_t* batch, long long N, long long B, int* tiles_mem, cudaStream_t st) {
-  if (!tiles_mem || N <= 0) return PERT_ERR_BADARG;
-  if (!batch || B <= 0) return PERT_OK;
-  int* gptr = tiles_mem + 1;
-  cudaError_t e = cudaMemsetAsync(gptr, 0xff, (size_t)(B + 1) * sizeof(int), st);
-  if (e != cudaSuccess) return (int)e;
-  k_tile_bounds<<<pert_cdiv(N, 256), 256, 0, st>>>(batch, (int)N, (int)B, gptr);
-  return PERT_OK;
-}
-// step 2 (needs rowptr): packing.  `has_batch` = step 1 ran for this batch.
-int pert_tile_list_build(int has_batch, long long N, long long E, long long B, const int* rowptr, int H, int n_rpc,
-                         int* tiles_mem, PertTiles* out, cudaStream_t st) {
-  if (!rowptr) return PERT_ERR_BADARG;
-  int rc = pert_tile_list_view(N, E, B, H, n_rpc, tiles_mem, out);
-  if (rc) return rc;
-  int* ntiles = tiles_mem;
-  int* gptr = tiles_mem + 1;
-  int* tile_ptr = gptr + (B + 1);
-  const size_t sm = has_batch && B > 0 ? (size_t)3 * (B + 1) * sizeof(int) : 0;
-  if (sm > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(k_build_tiles, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
-    if (e != cudaSuccess) return (int)e;
-  }
-  k_build_tiles<<<1, 1024, sm, st>>>(has_batch, (int)N, (int)B, rowptr, out->T, out->ecap, gptr, tile_ptr, ntiles,
-                                     out->max_tiles);
-  return PERT_OK;
 }

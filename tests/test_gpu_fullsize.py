@@ -210,7 +210,7 @@ def test_model_cfg5_full():
 
 
 def test_model_cfg2_jittered_sizes():
-    """cfg2 with graph sizes 200 +- 20 % (no tile is a whole number of equal graphs): the graph-aligned tiles.  Compared
+    """cfg2 with graph sizes 200 +- 20 % (no tile is a whole number of equal graphs): tiles that cut graphs.  Compared
     like the other full-size batches, on the same linear piece (see _full_parity): the free-running fp32 oracle puts a
     few BatchNorm ReLU arguments of this batch on the other side of zero depending on the host's summation order, which
     moves conv 0/1 and embedding gradients by 1e-3..1e-2 for every GPU GEMM path alike."""
@@ -360,8 +360,8 @@ def test_graph_replay_survives_workspace_growth():
 
 
 def test_two_engines_on_two_streams_concurrently():
-    """Two model replicas stepping at the same time on two streams of one device (tile-ticket ring, shared auxiliary
-    stream): every replica must produce what it produces alone."""
+    """Two model replicas stepping at the same time on two streams of one device (shared auxiliary stream): every
+    replica must produce what it produces alone."""
     import copy
 
     from pert_gnn_kdd23_b200.train import FlatParams, FusedAdam, fused_train_step

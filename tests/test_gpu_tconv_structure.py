@@ -2,7 +2,7 @@
 kernels (csrc/tconv_tile.cu) and of the per-row gather kernels (csrc/tconv.cu): in- and out-hubs that overflow the
 staged edge capacity, isolated nodes and edgeless batches, duplicate edges and self loops, sharp logits, graphs larger
 than a tile, a batch whose N % B == 0 size hint is wrong, whole-graph tiles that overflow their edge capacity, PERT-like
-attributes (interface 0 on 3 of 4 edges), interface ids >= 2^22, and the step engine's graph-aligned tile list.
+attributes (interface 0 on 3 of 4 edges), interface ids >= 2^22, and step-engine batches whose tiles cut graphs.
 
 The reference (ref_tconv) is checked against the oracle conv once; the graph builders assert the structure they exist
 for against a restatement of the tile geometry, so a case that stops reaching its branch fails instead of passing
@@ -658,20 +658,20 @@ def _hub_batch(cfg, seed):
     return Batch.from_data_list(dl)
 
 
-def _assert_tile_list(b, H):
+def _assert_cut_tiles(b, H):
     N, E, B = b.x.size(0), b.edge_index.size(1), b.num_graphs
     T, _, _ = tile_geom(H, 8, N, E, B)
-    assert not (N % B == 0 and N // B <= T), "batch would run fixed tiles, not the tile list"
+    assert not (N % B == 0 and N // B <= T), "batch would run whole-graph fixed tiles, not tiles that cut graphs"
 
 
 @gpu
 @pytest.mark.parametrize("cfg", [1, 2, 3])
-def test_engine_hubs_on_tile_list(cfg):
+def test_engine_hubs_on_cut_tiles(cfg):
     from pert_gnn_kdd23_b200.synthetic import CONFIGS
     from tests.test_gpu_fullsize import _full_parity
 
     b = _hub_batch(cfg, 100 + cfg)
-    _assert_tile_list(b, CONFIGS[cfg]["hidden"])
+    _assert_cut_tiles(b, CONFIGS[cfg]["hidden"])
     _full_parity(cfg, None, f"cfg{cfg} hubs", batch=b)
 
 
@@ -700,7 +700,7 @@ def test_engine_mixed_sizes_cfg3():
     b = Batch.from_data_list([_data(rng, n, 3 * n if n > 2 else n - 1) for n in sizes])
     N, E = b.x.size(0), b.edge_index.size(1)
     assert 700 > tile_fits(128, 8, E / N)[1]
-    _assert_tile_list(b, 128)
+    _assert_cut_tiles(b, 128)
     _full_parity(3, None, "cfg3 mixed sizes", batch=b)
 
 

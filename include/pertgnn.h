@@ -47,7 +47,7 @@ extern "C" {
  * 2005: pert_model_forward takes dropout + dropout_state, pert_model_backward takes dropout; later, and additive (no
  * existing signature changed): pert_bn_linear_fwd_planes(_supported); pert_batch_pad, pert_model_forward_live,
  * pert_model_backward_live, pert_pinball_loss_live, pert_eval_metrics_live; pert_tconv_fwd_c, pert_tconv_bwd_c,
- * pert_model_width (the step engine accepts every hidden width 1..256). */
+ * pert_model_width (the step engine accepts every hidden width 1..256); pert_trace_group_* (trace grouping). */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -487,6 +487,62 @@ int pert_span_graph_build(const int64_t* row_ptr, long long T, long long R, cons
                           const int64_t* interface, const int64_t* rpctype, const int64_t* root_ms,
                           const int64_t* node_ptr, int max_rows, int global_ids, int64_t* ms_id, int64_t* edge_index,
                           int64_t* edge_attr, int64_t* root_nid, int* status, void* stream);
+
+/* ---- trace grouping: runtime patterns, entry mixes, trace labels (csrc/tracegroup.cu) ------------------------------
+ * Replaces the body of preprocess.py main() after get_df() (:269-381): get_tr2ts_map (:32-41, bucket = floor(min
+ * timestamp / 30000) * 30000), the label tr2delay (:290-292, y = max |rt|), the runtime id of every trace (:280-293:
+ * factorize of the " ".join of its um_dm_interface strings), the entry x trace iteration (:295-316) with its
+ * representative trace per runtime (:317-367) and the normalised entry mixes (:371-375).
+ * Input: the processed span table, one row per span in file order, int64 device columns of R rows.  Traces are the
+ * distinct traceids (ascending, t = 0..T-1); a trace's rows keep file order.  traceid and entryid must lie in
+ * [0, 2^31) (else PERT_ERR_RANGE in status and the row / trace is left out); every row of a trace must carry the same
+ * entryid (else PERT_ERR_RANGE).  Four calls, the caller reading a size from the device between them:
+ *   pert_trace_group_range  -> maxes[2] = {max traceid, max entryid} (-1: none)   => n_keys = maxes[0] + 1
+ *   pert_trace_group_keys   -> key_ptr[n_keys+1] (first row slot of every traceid), key_trace[n_keys+1] (trace index of
+ *                              every traceid; key_trace[n_keys] = T)             => T
+ *   pert_trace_group_build  -> every per-trace / per-runtime / per-entry array, sizes[3] = {n_runtimes, n_pairs, R'}
+ *   pert_trace_group_gather -> the rows of the representatives (R'), the only rows the host needs (GraphConstruct).
+ * Runtime ids: two traces share one iff their (um, dm, interface) sequences are equal (order and length included);
+ * ids count from 0 in order of the smallest traceid of each runtime (Series.factorize over ascending traceids).  The
+ * grouping hashes every trace (order-sensitive, 2 x hash_bits bits) into an open-addressing table and merges two traces
+ * only after a row-by-row comparison, so hash collisions cost time and never a wrong merge; hash_bits (1..64) is 64
+ * except in tests that force collisions.  Iteration order = entries ascending, traceids ascending inside an entry
+ * (tr2data's key order).  Outputs do not depend on thread scheduling. */
+typedef struct PertSpanTable {
+  long long R;
+  const int64_t *traceid, *timestamp, *rpcid, *um, *dm, *interface, *rpctype, *rt, *entryid;
+} PertSpanTable;
+/* Outputs of pert_trace_group_build.  Sizes T (traces), n_ent = max entryid + 1.  Arrays marked [T*] are sized T and
+ * hold n_runtimes or n_pairs valid entries (sizes[]); ids are int32 unless stated. */
+typedef struct PertTraceGroups {
+  int32_t *row_ptr;                  /* [T+1] trace t owns perm[row_ptr[t] .. row_ptr[t+1])                     */
+  int32_t *perm;                     /* [R]   row ids grouped by trace, file order inside a trace               */
+  int64_t *trace_id, *bucket, *y;    /* [T]   traceid, timestamp bucket (:39), label (:290-292)                 */
+  int32_t *entry, *runtime;          /* [T]   entry id, runtime id                                              */
+  int32_t *order;                    /* [T]   iteration order: trace index at position p (tr2data key order)    */
+  int32_t *ent_trace_ptr;            /* [n_ent+1] entry e owns positions ent_trace_ptr[e] .. [e+1] of `order`   */
+  int32_t *ent_pair_ptr;             /* [n_ent+1] entry e owns pairs ent_pair_ptr[e] .. [e+1]                   */
+  int32_t *pair_runtime;             /* [T*]  runtime of every (entry, runtime) pair, entry-major, first met first */
+  double *pair_prob;                 /* [T*]  count / entry total in fp64 (entry2runtimes, :371-375)            */
+  int32_t *occurrences;              /* [T*]  traces per runtime id (:336, :342)                                */
+  int32_t *ins_runtime;              /* [T*]  runtime id at insertion index k (runtime2*graph_map key order)    */
+  int32_t *rep_trace;                /* [T*]  representative trace (first in iteration order) at insertion index */
+  int32_t *runtime_ins;              /* [T*]  insertion index of every runtime id                               */
+  int32_t *rep_ptr;                  /* [T+1] row offsets of the representatives' rows, insertion order         */
+  int64_t *sizes;                    /* [3]   n_runtimes, n_pairs, R' = rep_ptr[n_runtimes]                      */
+} PertTraceGroups;
+int pert_trace_group_range(const PertSpanTable* table, int* maxes, int* status, void* stream);
+int pert_trace_group_keys(const PertSpanTable* table, long long n_keys, int* key_ptr, int* key_trace, void* workspace,
+                          long long workspace_bytes, void* stream);
+/* workspace bytes of pert_trace_group_keys (n_traces < 0) or pert_trace_group_build; -1 for bad sizes. */
+long long pert_trace_group_workspace_bytes(long long R, long long n_keys, long long n_traces, long long n_ent);
+int pert_trace_group_build(const PertSpanTable* table, long long n_keys, long long n_traces, long long n_ent,
+                           int hash_bits, const int* key_ptr, const int* key_trace, const PertTraceGroups* out,
+                           void* workspace, long long workspace_bytes, int* status, void* stream);
+/* rows[8][R'] int64: um, dm, interface, rpctype, timestamp, endTimestamp (= timestamp + |rt|, :263), rpcid, rt of the
+ * representatives' rows, representative k at rep_ptr[k], file order inside it. */
+int pert_trace_group_gather(const PertSpanTable* table, const int* perm, const int* row_ptr, const int* rep_trace,
+                            const int* rep_ptr, long long n_runtimes, long long R_rep, int64_t* rows, void* stream);
 
 #ifdef __cplusplus
 }

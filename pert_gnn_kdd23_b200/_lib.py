@@ -70,6 +70,12 @@ SIGNATURES = {
     "pert_pert_graph_build": (I, [P, LL, LL, P, P, P, P, P, P, P, P, I, I, P, P, P, P, P, P]),
     "pert_span_graph_count": (I, [P, LL, P, P, I, P, P, P]),
     "pert_span_graph_build": (I, [P, LL, LL, P, P, P, P, P, P, I, I, P, P, P, P, P, P]),
+    # trace grouping (tracegroup.py; first argument: const PertSpanTable*)
+    "pert_trace_group_range": (I, [P, P, P, P]),
+    "pert_trace_group_keys": (I, [P, LL, P, P, P, LL, P]),
+    "pert_trace_group_workspace_bytes": (LL, [LL, LL, LL, LL]),
+    "pert_trace_group_build": (I, [P, LL, LL, LL, I, P, P, P, P, LL, P, P]),
+    "pert_trace_group_gather": (I, [P, P, P, P, P, LL, LL, P, P]),
     # whole-model engine (first argument: const PertModelDesc*, see engine.py)
     "pert_model_width": (I, [I]),
     "pert_model_workspace_bytes": (LL, [P, LL, LL, LL]),

@@ -190,6 +190,87 @@ class PatternStore:
         return cls(art["runtime2graph"], art["entry2runtimes"], art["resource_index"], art["resource_values"],
                    art["tr2data"], device, n_ms=art.get("n_ms"))
 
+    @classmethod
+    def from_trace_groups(cls, groups, kind, resource_index, resource_values, device=None, n_ms=None):
+        """The store of ``PatternStore(runtime2graph, groups.entry2runtimes(), resource_index, resource_values,
+        groups.tr2data(), ...)`` with runtime2graph the ``kind`` ("pert" / "span") graph map, built from the device
+        arrays of a ``tracegroup.TraceGroups`` without a Python loop over entries, patterns or traces.  Patterns in the
+        reference's insertion order, traces in tr2data's key order; the one device->host copy besides the graph build
+        is the host sizing arrays the store keeps (per-trace entry and id, per-entry node / edge / pattern totals).
+        Microservice ids must lie in [0, 2^31)."""
+        graphs, rt_ids = groups.graphs(kind)
+        dev = torch.device(device) if device is not None else graphs.ms_id.device
+        if dev.type != "cuda":
+            raise _lib.PertGnnError("PatternStore lives on a CUDA device (no CPU fallback for the hot path)")
+        self = cls.__new__(cls)
+        self.device, self.rt_ids = dev, list(rt_ids)
+        i32, i64 = torch.int32, torch.int64
+        with torch.cuda.device(dev):
+            nptr = torch.from_numpy(np.asarray(graphs.node_ptr, dtype=np.int64)).to(dev)
+            eptr = torch.from_numpy(np.asarray(graphs.edge_ptr, dtype=np.int64)).to(dev)
+            n_pat, n_all = len(self.rt_ids), int(graphs.node_ptr[-1])
+            ms = graphs.ms_id.reshape(-1).to(dev, i64)
+            # get_x keeps the LAST node of every microservice of a pattern (pert_gnn.py:54-65): stable sort by
+            # (pattern, ms); the last of every run of equal keys is the largest node index
+            pid = torch.repeat_interleave(torch.arange(n_pat, device=dev), nptr.diff(), output_size=n_all)
+            key, idx = torch.sort(pid * (1 << 32) + ms, stable=True)
+            run_end = torch.ones(n_all, dtype=torch.bool, device=dev)
+            run_end[:-1] = key[1:] != key[:-1]
+            last = torch.zeros(n_all, dtype=torch.uint8, device=dev)
+            last[idx[run_end]] = 1
+            # entries: entry2runtimes[e] in key order = the (entry, runtime) pairs of the groups
+            ent_ptr = groups.ent_pair_ptr
+            n_ent, n_pairs = int(ent_ptr.shape[0]) - 1, int(groups.pair_runtime.shape[0])
+            ent_pat = groups.runtime_ins[groups.pair_runtime.long()]
+            pair_entry = torch.repeat_interleave(torch.arange(n_ent, device=dev), ent_ptr.diff(), output_size=n_pairs)
+            sums = []
+            for per_pat in (nptr.diff(), eptr.diff(), torch.ones(n_pat, dtype=i64, device=dev)):
+                sums.append(torch.zeros(n_ent, dtype=i64, device=dev).index_add_(0, pair_entry,
+                                                                                  per_pat[ent_pat.long()]))
+            ent_nodes, ent_edges, ent_pats = sums
+            order = groups.order.long()
+            t_ent = groups.entry[order]
+            host = torch.cat([t_ent.long(), groups.trace_id[order], ent_nodes, ent_edges, ent_pats,
+                              ms.max().reshape(1) if n_all else torch.zeros(1, dtype=i64, device=dev)]).cpu().numpy()
+        T = int(order.shape[0])
+        self._h_trace_entry, self.trace_keys = host[:T], host[T:2 * T].tolist()
+        self._h_ent_nodes, self._h_ent_edges, self._h_ent_pats = (host[2 * T + k * n_ent:2 * T + (k + 1) * n_ent]
+                                                                 for k in range(3))
+        res_ms = np.array([m for _, m in resource_index], dtype=np.int64)
+        res_ts = np.array([t for t, _ in resource_index], dtype=np.int64)
+        self.n_ms = int(n_ms if n_ms is not None else max(int(host[-1]), int(res_ms.max(initial=0))) + 1)
+        keys = res_ts * self.n_ms + res_ms
+        korder = np.argsort(keys, kind="stable")
+        has = np.zeros(self.n_ms, dtype=np.uint8)
+        has[res_ms] = 1                                          # ms_with_resources (pert_gnn.py:138)
+        self.attr_cols = int(graphs.edge_attr.shape[1])
+
+        def up(a, dtype):
+            return torch.from_numpy(np.ascontiguousarray(a, dtype=dtype)).to(dev)
+
+        ei = graphs.edge_index.to(dev)
+        self.t = {
+            "pat_nptr": nptr.to(i32), "pat_eptr": eptr.to(i32), "pat_ms": ms.contiguous(),
+            "pat_depth": graphs.node_depth.reshape(-1).to(dev, i64).contiguous(), "pat_last": last,
+            "pat_src": ei[0].to(i32).contiguous(), "pat_dst": ei[1].to(i32).contiguous(),
+            "pat_attr": graphs.edge_attr.to(dev, i64).contiguous(),
+            "ent_ptr": ent_ptr.to(dev, i32).contiguous(), "ent_pat": ent_pat.to(i32).contiguous(),
+            "ent_prob": groups.pair_prob.to(dev, torch.float32).contiguous(),      # float64 -> float32 rounding
+            "ent_nodes": ent_nodes.to(i32), "ent_edges": ent_edges.to(i32),
+            "res_keys": up(keys[korder], np.int64),
+            "res_vals": up(np.asarray(resource_values, dtype=np.float64)[korder].astype(np.float32), np.float32),
+            "ms_has_res": up(has, np.uint8), "trace_entry": t_ent.to(i32).contiguous(),
+            "trace_ts": groups.bucket[order].contiguous(), "trace_y": groups.y[order].contiguous(),
+        }
+        d = _PertStore()
+        d.n_pat, d.n_ent, d.n_res, d.n_ms, d.attr_cols = n_pat, n_ent, int(keys.shape[0]), self.n_ms, self.attr_cols
+        d.n_traces = T
+        for k, v in self.t.items():
+            setattr(d, k, v.data_ptr())
+        self.desc = d
+        self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+        return self
+
     def __len__(self):
         return len(self.trace_keys)
 

@@ -325,3 +325,124 @@ def make_pert_artifacts(seed=3, n_patterns=256, n_entries=64, n_traces=4096, cal
     info = {"patterns": len(pg), "span_rows": int(sum(len(t["um"]) for t in tables)), "nodes": int(pg.node_ptr[-1]),
             "edges": int(pg.edge_ptr[-1]), "build_s": secs}
     return art, info
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Processed span tables (what preprocess.py get_df() returns, :191-266): one row per span in file order, the traces
+# interleaved, every column an integer.  Input of tracegroup.group_traces (the body of preprocess.py main()).
+TRACE_COLUMNS = ("traceid", "timestamp", "rpcid", "um", "dm", "interface", "rpctype", "rt", "entryid")   # tracegroup.COLUMNS
+
+
+def _interleave(rng, trace_of_row):
+    """File order of rows whose per-trace order is already right: traces interleave, each trace keeps its row order."""
+    u = rng.random(trace_of_row.shape[0])
+    by_trace = np.lexsort((u, trace_of_row))                 # rows grouped by trace, u ascending inside a trace
+    key = np.empty_like(u)
+    key[np.argsort(trace_of_row, kind="stable")] = u[by_trace]
+    return np.argsort(key, kind="stable")
+
+
+def make_trace_table(seed=5, n_ms=24, n_traces=300):
+    """Small processed span table covering what the trace grouping must get right (tests/golden/ref_preprocess.npz):
+    interleaved traces with traceid gaps; one-row traces; the same rows in a different order (another runtime);
+    one runtime under two entries whose lower entry's trace has the higher traceid and other timings (so the
+    representative matters); negative rt; buckets on both sides of a 30000 boundary; the drop_wrong_edges anomalies of
+    make_span_tables; an entry-id gap (entries 0, 1, 2, 4, 6).  -> dict(columns={TRACE_COLUMNS: int64 [R]},
+    resource_index [(bucket, ms)] for every bucket and microservice, resource_values [len, 8] float64, n_ms)."""
+    from .pertgraph import drop_wrong_edges, get_root_ms
+
+    def root_kept(tab):              # misc.py:204 / :306 look the root up among the surviving rows (KeyError otherwise)
+        root = get_root_ms(tab)
+        keep = drop_wrong_edges(tab, root)
+        return root in set(tab["um"][keep]) | set(tab["dm"][keep])
+
+    rng = np.random.default_rng(seed)
+    pats = make_span_tables(seed, 30, n_ms=n_ms, calls=(2, 12)) + make_span_tables(seed + 1, 3, n_ms=n_ms, calls=(1, 1))
+    pats = [t for t in pats if root_kept(t)]
+    rev = [{k: v[::-1].copy() for k, v in t.items()} for t in pats if len(t["um"]) > 2]
+    pats.append(next(t for t in rev if root_kept(t)))            # same rows as a pattern, reversed: another runtime
+    entries = np.array([0, 1, 2, 4, 6])
+    pat_entry = entries[rng.integers(0, len(entries), len(pats))]
+    shared = 5                                                   # pattern filed under entries 6 and 1 (see below)
+    pat_entry[shared] = 6
+    weights = 1.0 / np.arange(1, len(pats) + 1)
+    weights[len(pats) - 4:] = 0.5                                # the one-row and reversed patterns occur too
+    pick = rng.choice(len(pats), size=n_traces - 1, p=weights / weights.sum())
+    tids = np.sort(rng.choice(3 * n_traces, size=n_traces, replace=False))      # gaps
+    traces = []
+    for i, p in enumerate(pick):
+        traces.append((int(tids[i]), int(p), int(pat_entry[p])))
+    traces.append((int(tids[-1]), shared, 1))   # highest traceid, lower entry: the representative of `shared`
+    cols = {k: [] for k in TRACE_COLUMNS}
+    for n, (tid, p, ent) in enumerate(traces):
+        tab = pats[p]
+        m = len(tab["um"])
+        t0 = int(rng.integers(29990, 30010)) if n % 3 else int(rng.integers(0, 90000))   # around the 30000 boundary
+        off = tab["timestamp"] - tab["timestamp"].min()
+        root = int(np.argmax(np.abs(tab["rt"])))
+        if n == len(traces) - 1:
+            off = off[::-1].copy()                               # other timings for the late representative
+            j = int(np.argmin(off))
+            off[root], off[j] = off[j], off[root]                  # the root call still starts first
+        rt = tab["rt"].copy()
+        jit = rng.integers(-3, 4, m)
+        jit[root] = 0
+        rt = np.where(np.arange(m) == root, rt, rt + jit)
+        cols["traceid"].append(np.full(m, tid))
+        cols["timestamp"].append(t0 + off)
+        cols["rpcid"].append(tab["rpcid"])
+        cols["um"].append(tab["um"])
+        cols["dm"].append(tab["dm"])
+        cols["interface"].append(tab["interface"])
+        cols["rpctype"].append(rng.integers(0, 6, m) if n % 2 else tab["rpctype"])
+        cols["rt"].append(rt)
+        cols["entryid"].append(np.full(m, ent))
+    cols = {k: np.concatenate(v).astype(np.int64) for k, v in cols.items()}
+    order = _interleave(rng, cols["traceid"])
+    cols = {k: v[order] for k, v in cols.items()}
+    buckets = np.unique(np.array([(cols["timestamp"][cols["traceid"] == t].min() // 30000) * 30000
+                                  for t in np.unique(cols["traceid"])]))
+    index = [(int(b), ms) for b in buckets for ms in range(n_ms)]
+    values = rng.random((len(index), N_FEAT - 1))
+    return {"columns": cols, "resource_index": index, "resource_values": values, "n_ms": n_ms}
+
+
+def make_random_trace_table(seed, n_traces, rows=(20, 40), n_patterns=2000, n_entries=64, n_ms=4096, n_if=1024,
+                            long_rows=0, n_long=0, span=300000):
+    """Large processed span table for scale tests and timing, generated without a Python loop over traces.
+    ``n_patterns`` call sequences (lengths uniform in ``rows``; ``n_long`` more of ``long_rows`` rows) are drawn with a
+    Zipf-like law, so runtimes repeat heavily; a pattern belongs to one entry, a few to two.  Row 0 of every trace is its
+    root call (smallest timestamp, largest |rt|), rpcids are unique inside a trace, traceids have gaps and the rows of
+    all traces interleave.  -> dict of TRACE_COLUMNS, int64 [R]."""
+    rng = np.random.default_rng(seed)
+    lens = rng.integers(rows[0], rows[1] + 1, n_patterns)
+    if n_long:
+        lens = np.concatenate([lens, np.full(n_long, long_rows)])
+    P = lens.shape[0]
+    pptr = np.concatenate([[0], np.cumsum(lens)])
+    um = rng.integers(0, n_ms, pptr[-1])
+    dm = (um + rng.integers(1, n_ms, pptr[-1])) % n_ms           # no self loop: every representative keeps rows
+    itf = rng.integers(0, n_if, pptr[-1])
+    pat_entry = rng.integers(0, n_entries, P)
+    w = 1.0 / np.arange(1, P + 1) ** 0.8
+    pick = rng.choice(P, size=n_traces, p=w / w.sum())
+    if n_long:
+        pick[rng.choice(n_traces, n_long, replace=False)] = np.arange(n_patterns, P)
+    ent = pat_entry[pick]
+    other = rng.random(n_traces) < 0.02                           # a pattern met under a second entry
+    ent[other] = (ent[other] + 1 + rng.integers(0, n_entries - 1, int(other.sum()))) % n_entries
+    tids = np.sort(rng.choice(2 * n_traces + 7, size=n_traces, replace=False)) + 3
+    tl = lens[pick]
+    tr = np.repeat(np.arange(n_traces), tl)
+    start = np.concatenate([[0], np.cumsum(tl)])[:-1]
+    pos = np.arange(tr.shape[0]) - start[tr]
+    src = pptr[pick][tr] + pos
+    t0 = rng.integers(0, span, n_traces)[tr]
+    first = pos == 0
+    ts = t0 + np.where(first, 0, rng.integers(0, 9, tr.shape[0]))
+    rt = np.where(first, 1000 + rng.integers(0, 500, tr.shape[0]),
+                  rng.integers(-400, 400, tr.shape[0]))
+    cols = {"traceid": tids[tr], "timestamp": ts, "rpcid": pos, "um": um[src], "dm": dm[src], "interface": itf[src],
+            "rpctype": rng.integers(0, 8, tr.shape[0]), "rt": rt, "entryid": ent[tr]}
+    order = _interleave(rng, tr)
+    return {k: np.ascontiguousarray(v[order], dtype=np.int64) for k, v in cols.items()}

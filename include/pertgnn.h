@@ -47,7 +47,8 @@ extern "C" {
  * 2005: pert_model_forward takes dropout + dropout_state, pert_model_backward takes dropout; later, and additive (no
  * existing signature changed): pert_bn_linear_fwd_planes(_supported); pert_batch_pad, pert_model_forward_live,
  * pert_model_backward_live, pert_pinball_loss_live, pert_eval_metrics_live; pert_tconv_fwd_c, pert_tconv_bwd_c,
- * pert_model_width (the step engine accepts every hidden width 1..256); pert_trace_group_* (trace grouping). */
+ * pert_model_width (the step engine accepts every hidden width 1..256); pert_trace_group_* (trace grouping);
+ * pert_store_assemble_requests (request assembly with the exact or as-of resource join). */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -456,6 +457,31 @@ typedef struct PertBatchOut {
  * reference raises KeyError there). */
 int pert_store_assemble(const PertStore* store, const int64_t* trace_ids, long long B, long long N, long long E,
                         int* offsets, const PertBatchOut* out, int* status, void* stream);
+
+/* ---- request assembly: batches for prediction, keyed by (entry, time) instead of a trace id ---------------------------
+ * Graph b is entry entry_ids[b] at the time bucket floor(timestamps[b] / 30000) * 30000 (floor division: -1 maps to
+ * -30000, preprocess.py:39).  The outputs are those of pert_store_assemble for a trace of that entry and bucket, except
+ * y, which is not written (out->y may be NULL): a request has no label.  Entries, patterns and resources come from
+ * `store`; its trace table is not read.  N, E and the sum of the entries' pattern counts size the outputs as above.
+ * Resource join, for the node that receives statistics (the last node of a resourced microservice in its pattern):
+ *   asof == NULL (exact): the (bucket, ms) row; a missing row sets PERT_ERR_RANGE in status (as pert_store_assemble);
+ *   asof != NULL (as-of): the row of that ms with the largest timestamp <= bucket; among rows sharing that timestamp the
+ *     one the exact join picks (the first in the store's sorted order), so an exact hit gives identical features in both
+ *     modes.  No such row: the node keeps the missing indicator [0 x 8, 1]; this is not an error.
+ * PertResourceAsOf indexes the store's resource rows by microservice: rows of ms m are k = ms_ptr[m] .. ms_ptr[m+1]-1,
+ * ts[k] (int64) ascending, and row[k] (int32) is the row's index into res_keys / res_vals (ascending among equal ts).
+ * 12 bytes per resource row (ts and row may be NULL when n_res = 0); PatternStore builds it on the device with the store.
+ * On the device, an entry < 0, >= n_ent or without patterns sets PERT_ERR_RANGE and the graph is assembled as entry 0
+ * (as a bad trace id reads trace 0).  PERT_ERR_BADARG, before any CUDA call, for NULL pointers and negative sizes;
+ * B = 0 returns PERT_OK and launches nothing. */
+typedef struct PertResourceAsOf {
+  const int32_t* ms_ptr;  /* [n_ms+1] */
+  const int64_t* ts;      /* [n_res]  */
+  const int32_t* row;     /* [n_res]  */
+} PertResourceAsOf;
+int pert_store_assemble_requests(const PertStore* store, const PertResourceAsOf* asof, const int64_t* entry_ids,
+                                 const int64_t* timestamps, long long B, long long N, long long E, int* offsets,
+                                 const PertBatchOut* out, int* status, void* stream);
 
 /* ---- PERT-graph construction (SURVEY 8f row N2) ---------------------------------------------------------------
  * Replaces misc.py:221-319 (GraphConstruct.get_pert_edge_index) for T traces at once.  Input: the cleaned span rows

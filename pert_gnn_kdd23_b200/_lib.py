@@ -65,6 +65,8 @@ SIGNATURES = {
     "pert_allreduce_adam": (I, [P, P, P, P, LL, F, F, F, F, F, LL, F, P, I, I, P, P, P]),
     # device-side batch assembly from the pattern store (first / 7th argument: struct pointers, see store.py)
     "pert_store_assemble": (I, [P, P, LL, LL, LL, P, P, P, P]),
+    # request assembly (second argument: const PertResourceAsOf* or NULL for the exact join)
+    "pert_store_assemble_requests": (I, [P, P, P, P, LL, LL, LL, P, P, P, P]),
     # PERT-graph construction (pertgraph.py)
     "pert_pert_graph_count": (I, [P, LL, P, P, I, P, P, P]),
     "pert_pert_graph_build": (I, [P, LL, LL, P, P, P, P, P, P, P, P, I, I, P, P, P, P, P, P]),
@@ -98,6 +100,12 @@ _lib = None
 
 class PertGnnError(RuntimeError):
     pass
+
+
+class PertResourceAsOf(C.Structure):
+    """The as-of index of a store's resource rows (include/pertgnn.h): device pointers ms_ptr [n_ms+1] int32,
+    ts [n_res] int64, row [n_res] int32."""
+    _fields_ = [("ms_ptr", P), ("ts", P), ("row", P)]
 
 
 def lib():

@@ -28,6 +28,15 @@ static inline int pert_num_sms() {
 
 static inline int pert_cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// Time bucket of a timestamp (ms): floor(ts / 30000) * 30000 with floor division (pandas //), so -1 -> -30000
+// (preprocess.py:39 get_tr2ts_map).  The trace grouping labels traces with it; request assembly joins resources on it.
+constexpr int64_t TG_BUCKET = 30000;
+__host__ __device__ __forceinline__ int64_t pert_time_bucket(int64_t ts) {
+  int64_t q = ts / TG_BUCKET;
+  if (ts % TG_BUCKET != 0 && ts < 0) --q;
+  return q * TG_BUCKET;
+}
+
 __device__ __forceinline__ float4 ldg4(const float* p) {
   return __ldg(reinterpret_cast<const float4*>(p));
 }

@@ -18,6 +18,10 @@
 // times in one pattern only its LAST node receives the resource statistics; earlier duplicates keep [0 x 8, 1]
 // (`last_occ` flag, computed when the store is built).  A resourced microservice whose (timestamp, ms) row is missing
 // raises KeyError in the reference; here it sets PERT_ERR_RANGE in `status` and the node keeps the missing indicator.
+//
+// Serving (pert_store_assemble_requests): the same kernels, with graph b taken from a request (entry, timestamp) instead
+// of a trace row -- the source is a template parameter -- and optionally the as-of resource join: the newest row of the
+// microservice at or before the request's time bucket, through a per-microservice index of the sorted rows.
 #include "common.cuh"
 
 namespace {
@@ -35,10 +39,47 @@ __device__ __forceinline__ int upper_seg(const int* __restrict__ off, int n, int
   return lo;
 }
 
-// exclusive prefix sums of the per-trace node / edge / pattern counts (one CTA; B is a batch size)
-__global__ void __launch_bounds__(1024) k_store_offsets(PertStore s, const int64_t* __restrict__ trace_ids, int B,
-                                                        int* __restrict__ node_off, int* __restrict__ edge_off,
-                                                        int* __restrict__ pat_off, int* status) {
+// Where graph b of a batch takes its entry, time bucket and label from: a row of the store's trace table
+// (pert_store_assemble) or a request (pert_store_assemble_requests).  entry() flags a bad id in `bad` and falls back to
+// trace 0 / entry 0; the other reads repeat the fallback, so every kernel sees the same graph.
+struct TraceRows {
+  const int64_t* __restrict__ ids;
+  static constexpr bool kLabel = true;
+  __device__ __forceinline__ int64_t row(const PertStore& s, int b, bool& bad) const {
+    const int64_t t = ids[b];
+    bad = t < 0 || t >= s.n_traces;
+    return bad ? 0 : t;
+  }
+  __device__ __forceinline__ int entry(const PertStore& s, int b, bool& bad) const {
+    return s.trace_entry[row(s, b, bad)];
+  }
+  __device__ __forceinline__ int64_t bucket(const PertStore& s, int b) const {
+    bool bad;
+    return s.trace_ts[row(s, b, bad)];
+  }
+  __device__ __forceinline__ int64_t label(const PertStore& s, int b) const {
+    bool bad;
+    return s.trace_y[row(s, b, bad)];
+  }
+};
+
+struct Requests {
+  const int64_t* __restrict__ entry_ids;
+  const int64_t* __restrict__ timestamps;
+  static constexpr bool kLabel = false;
+  __device__ __forceinline__ int entry(const PertStore& s, int b, bool& bad) const {
+    const int64_t e = entry_ids[b];
+    bad = e < 0 || e >= s.n_ent || s.ent_ptr[e + 1] == s.ent_ptr[e];
+    return bad ? 0 : (int)e;
+  }
+  __device__ __forceinline__ int64_t bucket(const PertStore&, int b) const { return pert_time_bucket(timestamps[b]); }
+};
+
+// exclusive prefix sums of the per-graph node / edge / pattern counts (one CTA; B is a batch size)
+template <class Src>
+__global__ void __launch_bounds__(1024) k_store_offsets(PertStore s, Src src, int B, int* __restrict__ node_off,
+                                                        int* __restrict__ edge_off, int* __restrict__ pat_off,
+                                                        int* status) {
   __shared__ int carry[3];
   __shared__ int wsum[3][32];
   if (threadIdx.x < 3) carry[threadIdx.x] = 0;
@@ -48,12 +89,9 @@ __global__ void __launch_bounds__(1024) k_store_offsets(PertStore s, const int64
     const int b = base + threadIdx.x;
     int v[3] = {0, 0, 0};
     if (b < B) {
-      int64_t t = trace_ids[b];
-      if (t < 0 || t >= s.n_traces) {
-        if (status) atomicExch(status, PERT_ERR_RANGE);
-        t = 0;
-      }
-      const int ent = s.trace_entry[t];
+      bool bad;
+      const int ent = src.entry(s, b, bad);
+      if (bad && status) atomicExch(status, PERT_ERR_RANGE);
       v[0] = s.ent_nodes[ent];
       v[1] = s.ent_edges[ent];
       v[2] = s.ent_ptr[ent + 1] - s.ent_ptr[ent];
@@ -99,7 +137,7 @@ __global__ void __launch_bounds__(1024) k_store_offsets(PertStore s, const int64
 }
 
 // pattern instance of local node / edge index l inside entry `ent`: returns slot k (into ent_pat / ent_prob) and the
-// offsets of that pattern inside the trace
+// offsets of that pattern inside the graph
 __device__ __forceinline__ int find_pattern(const PertStore& s, int ent, int l, bool edges, int& node_base,
                                             int& local) {
   int nb = 0, acc = 0;
@@ -121,15 +159,50 @@ __device__ __forceinline__ int find_pattern(const PertStore& s, int ent, int l, 
   return k0;
 }
 
-__global__ void __launch_bounds__(256) k_store_nodes(PertStore s, const int64_t* __restrict__ trace_ids, int B,
+// exact join: the sorted row of key (bucket, ms) (the lower bound over res_keys), -1 if there is none
+__device__ __forceinline__ int exact_row(const PertStore& s, int64_t bucket, int64_t ms) {
+  const int64_t key = bucket * (int64_t)s.n_ms + ms;
+  int lo = 0, hi = s.n_res;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (s.res_keys[mid] < key) lo = mid + 1;
+    else hi = mid;
+  }
+  return (lo < s.n_res && s.res_keys[lo] == key) ? lo : -1;
+}
+
+// as-of join: the row of ms with the largest timestamp <= bucket, the first of the rows sharing that timestamp (the one
+// exact_row returns for it); -1 if every row of ms is later than bucket
+__device__ __forceinline__ int asof_row(const PertResourceAsOf& a, int64_t bucket, int64_t ms) {
+  const int first = a.ms_ptr[ms];
+  int lo = first, hi = a.ms_ptr[ms + 1];
+  while (lo < hi) {                               // first k with ts[k] > bucket
+    const int mid = (lo + hi) >> 1;
+    if (a.ts[mid] <= bucket) lo = mid + 1;
+    else hi = mid;
+  }
+  if (lo == first) return -1;
+  const int64_t t = a.ts[lo - 1];
+  hi = lo - 1;
+  lo = first;
+  while (lo < hi) {                               // first k with ts[k] == t
+    const int mid = (lo + hi) >> 1;
+    if (a.ts[mid] < t) lo = mid + 1;
+    else hi = mid;
+  }
+  return a.row[lo];
+}
+
+// asof.ms_ptr == NULL: exact join (a missing row sets status)
+template <class Src>
+__global__ void __launch_bounds__(256) k_store_nodes(PertStore s, Src src, PertResourceAsOf asof, int B,
                                                      const int* __restrict__ node_off, PertBatchOut o, int* status) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   const int N = node_off[B];
   if (n >= N) return;
   const int b = upper_seg(node_off, B, n);
-  int64_t t = trace_ids[b];
-  if (t < 0 || t >= s.n_traces) t = 0;
-  const int ent = s.trace_entry[t];
+  bool bad;
+  const int ent = src.entry(s, b, bad);
   int node_base, local;
   const int k = find_pattern(s, ent, n - node_off[b], false, node_base, local);
   const int p = s.ent_pat[k];
@@ -146,18 +219,13 @@ __global__ void __launch_bounds__(256) k_store_nodes(PertStore s, const int64_t*
   for (int c = 0; c < NF; ++c) f[c] = 0.f;
   f[NF] = 1.f;
   if (s.pat_last[g] && ms >= 0 && ms < s.n_ms && s.ms_has_res[ms]) {
-    const int64_t key = s.trace_ts[t] * (int64_t)s.n_ms + ms;
-    int lo = 0, hi = s.n_res;        // lower bound over the sorted keys
-    while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
-      if (s.res_keys[mid] < key) lo = mid + 1;
-      else hi = mid;
-    }
-    if (lo < s.n_res && s.res_keys[lo] == key) {
+    const int64_t bucket = src.bucket(s, b);
+    const int r = asof.ms_ptr ? asof_row(asof, bucket, ms) : exact_row(s, bucket, ms);
+    if (r >= 0) {
 #pragma unroll
-      for (int c = 0; c < NF; ++c) f[c] = s.res_vals[(size_t)lo * NF + c];
+      for (int c = 0; c < NF; ++c) f[c] = s.res_vals[(size_t)r * NF + c];
       f[NF] = 0.f;
-    } else if (status) {
+    } else if (!asof.ms_ptr && status) {
       atomicExch(status, PERT_ERR_RANGE);      // the reference raises KeyError here (resource_df.loc)
     }
   }
@@ -165,16 +233,15 @@ __global__ void __launch_bounds__(256) k_store_nodes(PertStore s, const int64_t*
   for (int c = 0; c <= NF; ++c) o.x[(size_t)n * (NF + 1) + c] = f[c];
 }
 
-__global__ void __launch_bounds__(256) k_store_edges(PertStore s, const int64_t* __restrict__ trace_ids, int B,
-                                                     const int* __restrict__ node_off,
+template <class Src>
+__global__ void __launch_bounds__(256) k_store_edges(PertStore s, Src src, int B, const int* __restrict__ node_off,
                                                      const int* __restrict__ edge_off, PertBatchOut o) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   const int E = edge_off[B];
   if (e >= E) return;
   const int b = upper_seg(edge_off, B, e);
-  int64_t t = trace_ids[b];
-  if (t < 0 || t >= s.n_traces) t = 0;
-  const int ent = s.trace_entry[t];
+  bool bad;
+  const int ent = src.entry(s, b, bad);
   int node_base, local;
   const int k = find_pattern(s, ent, e - edge_off[b], true, node_base, local);
   const int p = s.ent_pat[k];
@@ -185,21 +252,37 @@ __global__ void __launch_bounds__(256) k_store_edges(PertStore s, const int64_t*
   for (int c = 0; c < s.attr_cols; ++c) o.edge_attr[(size_t)e * s.attr_cols + c] = s.pat_attr[ge * s.attr_cols + c];
 }
 
-// per-trace outputs: entry_id, y, ptr (int64), and the concatenated per-pattern probabilities
-__global__ void __launch_bounds__(256) k_store_traces(PertStore s, const int64_t* __restrict__ trace_ids, int B,
-                                                      const int* __restrict__ node_off,
+// per-graph outputs: entry_id, y (trace rows only), ptr (int64), and the concatenated per-pattern probabilities
+template <class Src>
+__global__ void __launch_bounds__(256) k_store_traces(PertStore s, Src src, int B, const int* __restrict__ node_off,
                                                       const int* __restrict__ pat_off, PertBatchOut o) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b > B) return;
   o.ptr[b] = node_off[b];
   if (b == B) return;
-  int64_t t = trace_ids[b];
-  if (t < 0 || t >= s.n_traces) t = 0;
-  const int ent = s.trace_entry[t];
+  bool bad;
+  const int ent = src.entry(s, b, bad);
   o.entry_id[b] = ent;
-  o.y[b] = s.trace_y[t];
+  if constexpr (Src::kLabel) o.y[b] = src.label(s, b);
   const int k0 = s.ent_ptr[ent], k1 = s.ent_ptr[ent + 1];
   for (int k = k0; k < k1; ++k) o.pattern_probs[pat_off[b] + (k - k0)] = s.ent_prob[k];
+}
+
+bool entries_ok(const PertStore* s) { return s->ent_ptr && s->ent_pat && s->ent_prob && s->pat_nptr && s->pat_eptr; }
+
+template <class Src>
+int assemble(const PertStore& s, const Src& src, const PertResourceAsOf& asof, long long B, long long N, long long E,
+             int* offsets, const PertBatchOut& out, int* status, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  int* node_off = offsets;
+  int* edge_off = offsets + (B + 1);
+  int* pat_off = offsets + 2 * (B + 1);
+  k_store_offsets<<<1, 1024, 0, st>>>(s, src, (int)B, node_off, edge_off, pat_off, status);
+  k_store_traces<<<pert_cdiv(B + 1, 256), 256, 0, st>>>(s, src, (int)B, node_off, pat_off, out);
+  if (N > 0) k_store_nodes<<<pert_cdiv(N, 256), 256, 0, st>>>(s, src, asof, (int)B, node_off, out, status);
+  if (E > 0) k_store_edges<<<pert_cdiv(E, 256), 256, 0, st>>>(s, src, (int)B, node_off, edge_off, out);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
 }
 
 }  // namespace
@@ -209,19 +292,21 @@ extern "C" {
 int pert_store_assemble(const PertStore* s, const int64_t* trace_ids, long long B, long long N, long long E,
                         int* offsets, const PertBatchOut* out, int* status, void* stream) {
   if (!s || !out || B < 0 || N < 0 || E < 0 || (B > 0 && (!trace_ids || !offsets))) return PERT_ERR_BADARG;
-  if (!s->ent_ptr || !s->ent_pat || !s->ent_prob || !s->pat_nptr || !s->pat_eptr || !s->trace_entry)
+  if (!entries_ok(s) || !s->trace_entry) return PERT_ERR_BADARG;
+  if (B == 0) return PERT_OK;
+  return assemble(*s, TraceRows{trace_ids}, PertResourceAsOf{}, B, N, E, offsets, *out, status, stream);
+}
+
+int pert_store_assemble_requests(const PertStore* s, const PertResourceAsOf* asof, const int64_t* entry_ids,
+                                 const int64_t* timestamps, long long B, long long N, long long E, int* offsets,
+                                 const PertBatchOut* out, int* status, void* stream) {
+  if (!s || !out || B < 0 || N < 0 || E < 0 || (B > 0 && (!entry_ids || !timestamps || !offsets)))
+    return PERT_ERR_BADARG;
+  if (!entries_ok(s) || (asof && (!asof->ms_ptr || (s->n_res > 0 && (!asof->ts || !asof->row)))))
     return PERT_ERR_BADARG;
   if (B == 0) return PERT_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  int* node_off = offsets;
-  int* edge_off = offsets + (B + 1);
-  int* pat_off = offsets + 2 * (B + 1);
-  k_store_offsets<<<1, 1024, 0, st>>>(*s, trace_ids, (int)B, node_off, edge_off, pat_off, status);
-  k_store_traces<<<pert_cdiv(B + 1, 256), 256, 0, st>>>(*s, trace_ids, (int)B, node_off, pat_off, *out);
-  if (N > 0) k_store_nodes<<<pert_cdiv(N, 256), 256, 0, st>>>(*s, trace_ids, (int)B, node_off, *out, status);
-  if (E > 0) k_store_edges<<<pert_cdiv(E, 256), 256, 0, st>>>(*s, trace_ids, (int)B, node_off, edge_off, *out);
-  PERT_LAUNCH_CHECK();
-  return PERT_OK;
+  return assemble(*s, Requests{entry_ids, timestamps}, asof ? *asof : PertResourceAsOf{}, B, N, E, offsets, *out,
+                  status, stream);
 }
 
 }  // extern "C"

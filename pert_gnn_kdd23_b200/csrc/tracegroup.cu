@@ -29,7 +29,6 @@ namespace {
 constexpr int TG_WARPS = 8;             // warps per CTA of the warp-per-trace kernels
 constexpr int TG_SHORT = 1024;          // longer traces are rank-sorted by a whole CTA
 constexpr int TG_TILE = 1024;           // traces per tile of the entry counting sort
-constexpr int TG_BUCKET = 30000;        // preprocess.py:39
 constexpr int TG_EMPTY = -1;
 constexpr unsigned long long TG_NOKEY = ~0ull;
 
@@ -187,9 +186,7 @@ __global__ void __launch_bounds__(TG_WARPS * 32) k_trace_reduce(PertSpanTable ta
   s2 = warp_sum64(s2);
   mixed = __any_sync(0xffffffffu, mixed);
   if (lane == 0) {
-    int64_t q = tmin / TG_BUCKET;
-    if (tmin % TG_BUCKET != 0 && tmin < 0) --q;          // floor division (pandas //)
-    bucket[t] = q * TG_BUCKET;
+    bucket[t] = pert_time_bucket(tmin);                  // floor division (pandas //)
     y[t] = amax;
     const bool ok = !mixed && e0 >= 0 && e0 < n_ent;
     if (!ok) atomicExch(status, PERT_ERR_RANGE);        // a trace filed under two entries (or an entry out of range)

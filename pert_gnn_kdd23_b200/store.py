@@ -52,6 +52,19 @@ def _last_occurrence_flags(all_ms, nptr):
     return flags
 
 
+def asof_index(res_keys, n_ms):
+    """As-of index of a store's sorted resource keys (``timestamp * n_ms + ms``, ascending), on their device:
+    (ms_ptr [n_ms+1] int32, ts [n_res] int64, row [n_res] int32) -- the rows of microservice m are
+    ms_ptr[m] .. ms_ptr[m+1]-1, with ascending timestamps ``ts`` and ``row`` their index into the sorted keys (ascending
+    among equal timestamps: a stable regrouping by ms of an order that is already timestamp-major)."""
+    ms = torch.remainder(res_keys, n_ms)
+    ts = torch.div(res_keys - ms, n_ms, rounding_mode="floor")
+    _, row = torch.sort(ms, stable=True)
+    ms_ptr = torch.zeros(n_ms + 1, dtype=torch.int64, device=res_keys.device)
+    ms_ptr[1:] = torch.cumsum(torch.bincount(ms, minlength=n_ms), 0)
+    return ms_ptr.to(torch.int32), ts[row].contiguous(), row.to(torch.int32)
+
+
 class _BulkPatterns:
     """Concatenated host arrays of many patterns (PatternStore.from_graphs)."""
 
@@ -166,6 +179,7 @@ class PatternStore:
             setattr(d, k, v.data_ptr())
         self.desc = d
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._build_asof()
 
     @classmethod
     def from_graphs(cls, graphs, runtime_ids, entry2runtimes, resource_index, resource_values, tr2data, device=None,
@@ -269,7 +283,19 @@ class PatternStore:
             setattr(d, k, v.data_ptr())
         self.desc = d
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._build_asof()
         return self
+
+    def _build_asof(self):
+        """The as-of index of the resource rows (``asof_index``), 12 bytes per row, kept beside the descriptor: the
+        resource table is fixed once the store is built."""
+        with torch.cuda.device(self.device):
+            ms_ptr, ts, row = asof_index(self.t["res_keys"], self.n_ms)
+        self.asof_t = {"ms_ptr": ms_ptr, "ts": ts, "row": row}
+        a = _lib.PertResourceAsOf()
+        for k, v in self.asof_t.items():
+            setattr(a, k, v.data_ptr())
+        self.asof_desc = a
 
     def __len__(self):
         return len(self.trace_keys)
@@ -283,17 +309,10 @@ class PatternStore:
         ent = self._h_trace_entry[np.asarray(trace_ids, dtype=np.int64)]
         return int(self._h_ent_nodes[ent].sum()), int(self._h_ent_edges[ent].sum()), int(self._h_ent_pats[ent].sum())
 
-    @_lib.on_device_of
-    def assemble(self, trace_ids, ids_device=None):
-        """-> device ``Batch`` of the traces ``trace_ids`` (sequence of ints into the store's trace table).
-        ``ids_device``: the same ids already on the device (int64) -- e.g. a slice of a resident epoch permutation --
-        to skip even the 8-byte-per-graph H2D copy."""
-        ids = np.asarray(trace_ids, dtype=np.int64)
-        B = int(ids.shape[0])
-        N, E, Pn = self.sizes(ids)
+    def _outputs(self, B, N, E, Pn, launch, keepalive, label=True):
+        """Allocates the Batch tensors, runs ``launch(offsets_ptr, out_ptr)`` (one of the assembly entry points) and
+        wraps the outputs into a device ``Batch``; without ``label`` there is no ``y`` (its pointer stays NULL)."""
         dev = self.device
-        if ids_device is None:
-            ids_device = torch.from_numpy(ids).to(dev, non_blocking=True)
         f32, i64 = torch.float32, torch.int64
         out = {
             "x": torch.empty(N, 9, dtype=f32, device=dev), "edge_index": torch.empty(2, E, dtype=i64, device=dev),
@@ -303,27 +322,90 @@ class PatternStore:
             "pattern_probs": torch.empty(Pn, 1, dtype=f32, device=dev),
             "entry_id": torch.empty(B, dtype=i64, device=dev), "y": torch.empty(B, dtype=i64, device=dev),
             "rt_probs": torch.empty(N, 1, dtype=f32, device=dev), "batch": torch.empty(N, dtype=i64, device=dev),
-            "ptr": torch.empty(B + 1, dtype=i64, device=dev),
+            "ptr": torch.empty(B + 1, dtype=i64, device=dev) if B else torch.zeros(1, dtype=i64, device=dev),
         }
+        if not label:
+            del out["y"]
         offsets = torch.empty(3 * (B + 1), dtype=torch.int32, device=dev)
         o = _PertBatchOut()
-        for k in ("x", "cat_X", "node_depth", "pattern_num_nodes", "rt_probs", "batch", "edge_index", "edge_attr",
-                  "entry_id", "y", "ptr", "pattern_probs"):
-            setattr(o, k, out[k].data_ptr())
-        rc = _lib.lib().pert_store_assemble(C.byref(self.desc), ids_device.data_ptr(), B, N, E, offsets.data_ptr(),
-                                            C.byref(o), self.status.data_ptr(), _lib.stream())
-        _lib.check(rc, "pert_store_assemble")
+        for k, v in out.items():
+            setattr(o, k, v.data_ptr())
+        launch(offsets.data_ptr(), C.byref(o))
         from . import ops
 
-        ops.LAUNCHES["n"] += 4
+        if B:
+            ops.LAUNCHES["n"] += 4
         b = Batch()
         b._store.update(out)
         object.__setattr__(b, "_num_graphs", B)
-        object.__setattr__(b, "_keepalive", (ids_device, offsets))
+        object.__setattr__(b, "_keepalive", keepalive + (offsets,))
         return b
 
+    @_lib.on_device_of
+    def assemble(self, trace_ids, ids_device=None):
+        """-> device ``Batch`` of the traces ``trace_ids`` (sequence of ints into the store's trace table).
+        ``ids_device``: the same ids already on the device (int64) -- e.g. a slice of a resident epoch permutation --
+        to skip even the 8-byte-per-graph H2D copy."""
+        ids = np.asarray(trace_ids, dtype=np.int64)
+        B = int(ids.shape[0])
+        N, E, Pn = self.sizes(ids)
+        if ids_device is None:
+            ids_device = torch.from_numpy(ids).to(self.device, non_blocking=True)
+
+        def launch(offsets, out):
+            rc = _lib.lib().pert_store_assemble(C.byref(self.desc), ids_device.data_ptr(), B, N, E, offsets, out,
+                                                self.status.data_ptr(), _lib.stream())
+            _lib.check(rc, "pert_store_assemble")
+
+        return self._outputs(B, N, E, Pn, launch, (ids_device,))
+
+    def check_entries(self, entry_ids):
+        """Raises ``PertGnnError`` naming the first request whose entry id is out of range or has no patterns."""
+        ent = np.asarray(entry_ids, dtype=np.int64).reshape(-1)
+        n_ent = int(self._h_ent_nodes.shape[0])
+        inside = (ent >= 0) & (ent < n_ent)
+        bad = ~inside
+        bad[inside] = self._h_ent_pats[ent[inside]] == 0
+        if bad.any():
+            i = int(np.argmax(bad))
+            why = "has no patterns" if inside[i] else f"is outside [0, {n_ent})"
+            raise _lib.PertGnnError(f"request {i}: entry {int(ent[i])} {why}")
+        return ent
+
+    @_lib.on_device_of
+    def assemble_requests(self, entry_ids, timestamps, asof=False, device_arrays=None):
+        """-> device ``Batch`` of the requests (entry ``entry_ids[b]`` at time ``timestamps[b]``, in ms): every field of
+        ``assemble`` but ``y``.  The resources are those of the time bucket floor(t / 30000) * 30000, joined exactly
+        (a missing row of a resourced microservice sets the status word, see ``check``) or, with ``asof``, from the
+        newest row at or before the bucket (none: the missing indicator, no error).  The entry ids are checked and the
+        outputs sized on the host (``PertGnnError`` before any launch); ``device_arrays``: the same two columns already
+        on the device (int64), e.g. slices of a request list uploaded once -- ``timestamps`` may then be None."""
+        ent = self.check_entries(entry_ids)
+        B = int(ent.shape[0])
+        N, E, Pn = (int(self._h_ent_nodes[ent].sum()), int(self._h_ent_edges[ent].sum()),
+                    int(self._h_ent_pats[ent].sum()))
+        if device_arrays is None:
+            ts = np.asarray(timestamps, dtype=np.int64).reshape(-1)
+            if ts.shape[0] != B:
+                raise _lib.PertGnnError(f"{B} entry ids but {ts.shape[0]} timestamps")
+            device_arrays = (torch.from_numpy(ent).to(self.device, non_blocking=True),
+                             torch.from_numpy(ts).to(self.device, non_blocking=True))
+        ent_d, ts_d = device_arrays
+        if ent_d.numel() != B or ts_d.numel() != B or ent_d.dtype != torch.int64 or ts_d.dtype != torch.int64:
+            raise _lib.PertGnnError("device_arrays: two int64 device tensors of one element per request")
+        ent_d, ts_d = ent_d.contiguous(), ts_d.contiguous()
+
+        def launch(offsets, out):
+            rc = _lib.lib().pert_store_assemble_requests(
+                C.byref(self.desc), C.byref(self.asof_desc) if asof else None, ent_d.data_ptr(), ts_d.data_ptr(), B,
+                N, E, offsets, out, self.status.data_ptr(), _lib.stream())
+            _lib.check(rc, "pert_store_assemble_requests")
+
+        return self._outputs(B, N, E, Pn, launch, (ent_d, ts_d), label=False)
+
     def check(self):
-        """Synchronising check of the status word (trace id out of range / missing (timestamp, ms) row)."""
+        """Synchronising check of the status word (trace id or entry id out of range / missing (timestamp, ms) row of
+        the exact join)."""
         code = int(self.status.item())
         if code != 0:
             _lib.check(code, "pert_store_assemble")

@@ -4,6 +4,7 @@ flat-buffer gradient all-reduce per step).
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -718,14 +719,60 @@ def evaluate(model, loader, device, tau=0.5):
     return m.result()
 
 
-class _BucketedEval:
+class _BucketState:
+    """Padded buffers and captured graph of every capacity bucket one bucketed forward has seen (``_bucket_run``)."""
+
+    def __init__(self):
+        self.buckets = {}    # key -> {"buf": PaddedBatch, "state": "new" | "ran-once" | "graph", "eager": bool, ...}
+        self.capture_error = None
+        self.captures = 0
+        self.replays = 0
+
+
+class _BucketedEval(_BucketState):
     """Per-model state of ``evaluate_bucketed``: the metric sums (one device buffer the graphs add into) and the
     padded buffers + forward/metrics graph of every bucket seen so far."""
 
     def __init__(self, device, tau):
+        super().__init__()
         self.metrics = EvalMetrics(device, tau)
-        self.buckets = {}
-        self.capture_error = None
+
+
+def _bucket_run(st: _BucketState, data, eng, run, max_graphs):
+    """Pads ``data`` into the buffers of its capacity bucket in ``st`` and runs ``run(buf)`` on them: eagerly on the
+    bucket's first visit, captured into a CUDA graph on the second and replayed from then on.  A graph captured over an
+    engine or workspace that has since been replaced is captured again; buckets beyond ``max_graphs`` and failed
+    captures (``st.capture_error``) stay eager.  -> what ``run`` returned (on a replay: the tensors of the capture,
+    which the replay has just rewritten)."""
+    N, E, B = _batch_sizes(data)
+    caps = bucket_caps(N, E, B)
+    key = caps + (int(data.edge_attr.size(1)),)
+    ent = st.buckets.get(key)
+    if ent is None:
+        ent = st.buckets[key] = {"buf": PaddedBatch(caps, data), "state": "new",
+                                 "eager": len(st.buckets) >= max_graphs}
+    buf = ent["buf"].fill(data)
+    eng._workspace(*caps)
+    if ent["state"] == "graph" and _stale(ent, eng):
+        _drop_graph(ent)
+    if ent["state"] == "ran-once" and not ent.get("eager"):
+        g = torch.cuda.CUDAGraph()
+        try:
+            with torch.cuda.graph(g):
+                out = run(buf)
+            ent.update(state="graph", graph=g, out=out, engine=eng, ws_gen=eng.ws_generation, ws=eng.ws)
+            st.captures += 1
+        except Exception as e:  # noqa: BLE001 - this bucket stays eager
+            st.capture_error = repr(e)
+            torch.cuda.synchronize()
+            ent["eager"] = True
+    if ent["state"] == "graph":
+        ent["graph"].replay()
+        st.replays += 1
+        return ent["out"]
+    if ent["state"] == "new":
+        ent["state"] = "ran-once"
+    return run(buf)
 
 
 @torch.no_grad()
@@ -765,33 +812,92 @@ def evaluate_bucketed(model, loader, device, tau=0.5, max_graphs=32):
             if not PaddedBatch.accepts(data):
                 eval_step(model, data, tau, m)
                 continue
-            N, E, B = _batch_sizes(data)
-            caps = bucket_caps(N, E, B)
-            key = caps + (int(data.edge_attr.size(1)),)
-            ent = st.buckets.get(key)
-            if ent is None:
-                ent = st.buckets[key] = {"buf": PaddedBatch(caps, data), "state": "new",
-                                         "eager": len(st.buckets) >= max_graphs}
-            buf = ent["buf"].fill(data)
-            m.count += B
-            eng._workspace(*caps)
-            if ent["state"] == "graph" and _stale(ent, eng):
-                _drop_graph(ent)
-            if ent["state"] == "ran-once" and not ent.get("eager"):
-                g = torch.cuda.CUDAGraph()
-                try:
-                    with torch.cuda.graph(g):
-                        out = run(buf)
-                    ent.update(state="graph", graph=g, out=out, engine=eng, ws_gen=eng.ws_generation, ws=eng.ws)
-                except Exception as e:  # noqa: BLE001 - this bucket stays eager
-                    st.capture_error = repr(e)
-                    torch.cuda.synchronize()
-                    ent["eager"] = True
-            if ent["state"] == "graph":
-                ent["graph"].replay()
-            else:
-                if ent["state"] == "new":
-                    ent["state"] = "ran-once"
-                run(buf)
+            m.count += int(data.num_graphs)
+            _bucket_run(st, data, eng, run, max_graphs)
     model.train(was_training)
     return m.result()
+
+
+class _BucketedPredict(_BucketState):
+    """Per-model state of ``predict``: the padded buffers + forward graph of every bucket seen so far, and a zero label
+    column for ``PaddedBatch.fill`` (requests have no label; the pad kernel, which runs eagerly in front of every
+    replay, is the only reader, so one buffer serves every bucket)."""
+
+    def __init__(self, device):
+        super().__init__()
+        self.device = device
+        self.zero_y = torch.zeros(0, dtype=torch.int64, device=device)
+
+    def labels(self, B):
+        if self.zero_y.numel() < B:
+            self.zero_y = torch.zeros(B, dtype=torch.int64, device=self.device)
+        return self.zero_y[:B]
+
+
+@torch.no_grad()
+def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, local=False, max_graphs=32):
+    """Predicted latency of every request (entry ``entry_ids[q]`` at time ``timestamps[q]``, ms) of a pattern store's
+    entries: float32 device tensor [Q], in request order (duplicates and any order allowed).  With ``local``, also the
+    local (per-node) predictions [sum of the requests' node counts] and ``node_ptr`` [Q+1] (int64), request q owning
+    rows node_ptr[q] .. node_ptr[q+1]-1.
+
+    The requests are assembled on the device in slices of ``batch_size`` (``PatternStore.assemble_requests``: the
+    exact resource join, or with ``asof`` the newest row at or before the request's time bucket -- with the exact join a
+    missing row sets the store's status word, see ``PatternStore.check``), and every slice runs the eval-mode forward
+    padded into its capacity bucket, replayed from one CUDA graph per bucket as in ``evaluate_bucketed``.  The workspace
+    is sized once, on the host, for the largest slice.  Runs in eval mode under ``no_grad`` and restores the training
+    flag; BatchNorm statistics, the dropout counter, parameters and optimizer state are left as they were.  A bad entry id
+    raises ``PertGnnError`` before any launch."""
+    ent = store.check_entries(entry_ids)
+    ts = np.asarray(timestamps, dtype=np.int64).reshape(-1)
+    if ts.shape != ent.shape:
+        raise _lib.PertGnnError(f"{ent.shape[0]} entry ids but {ts.shape[0]} timestamps")
+    bs = int(batch_size)
+    if bs < 1:
+        raise _lib.PertGnnError("batch_size must be >= 1")
+    Q = int(ent.shape[0])
+    dev = store.device
+    if dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    nodes, edges = store._h_ent_nodes[ent], store._h_ent_edges[ent]
+    node_ptr = np.zeros(Q + 1, dtype=np.int64)
+    np.cumsum(nodes, out=node_ptr[1:])
+    was_training = model.training
+    model.eval()
+    try:
+        with torch.cuda.device(dev):
+            st = model.__dict__.get("_bucketed_predict")
+            if st is None or st.device != dev:
+                st = model.__dict__["_bucketed_predict"] = _BucketedPredict(dev)
+            eng = model.engine()
+            gpred = torch.empty(Q, dtype=torch.float32, device=dev)
+            lpred = torch.empty(int(node_ptr[-1]), dtype=torch.float32, device=dev) if local else None
+            if Q:
+                starts = np.arange(0, Q, bs)          # the slices' sizes, exactly: host-only, no device sync
+                eng.reserve(*bucket_bound(int(np.add.reduceat(nodes, starts).max()),
+                                          int(np.add.reduceat(edges, starts).max()), min(bs, Q)))
+                ent_d = torch.from_numpy(ent).to(dev, non_blocking=True)
+                ts_d = torch.from_numpy(ts).to(dev, non_blocking=True)
+            n_if, n_rpc = model.interface_embeds.num_embeddings, model.rpctype_embeds.num_embeddings
+
+            def run(buf):
+                from .index import build_index
+
+                x, cat_X, edge_index, edge_attr, pnn, probs, entry_id, batch = model_inputs(buf)
+                index = build_index(edge_index, x.size(0), edge_attr, n_if, n_rpc, check=False)
+                g, loc = eng.forward(x, cat_X, entry_id, probs, pnn, batch, index, False, live=buf.live)
+                return g, loc, index
+
+            for i in range(0, Q, bs):
+                j = min(i + bs, Q)
+                data = store.assemble_requests(ent[i:j], None, asof=asof, device_arrays=(ent_d[i:j], ts_d[i:j]))
+                data.y = st.labels(j - i)
+                g, loc, _ = _bucket_run(st, data, eng, run, max_graphs)
+                gpred[i:j].copy_(g[:j - i, 0])
+                if local:
+                    lpred[node_ptr[i]:node_ptr[j]].copy_(loc[:node_ptr[j] - node_ptr[i], 0])
+    finally:
+        model.train(was_training)
+    if not local:
+        return gpred
+    return gpred, lpred, torch.from_numpy(node_ptr).to(dev)

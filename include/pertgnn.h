@@ -49,7 +49,7 @@ extern "C" {
  * pert_model_backward_live, pert_pinball_loss_live, pert_eval_metrics_live; pert_tconv_fwd_c, pert_tconv_bwd_c,
  * pert_model_width (the step engine accepts every hidden width 1..256); pert_trace_group_* (trace grouping);
  * pert_store_assemble_requests (request assembly with the exact or as-of resource join); pert_store_resources_count /
- * _merge (appending and evicting resource rows of a live store). */
+ * _merge (appending and evicting resource rows of a live store); pert_ingest_* (appending traces to a live store). */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -519,6 +519,69 @@ int pert_store_resources_merge(const PertStore* store, const PertResourceAsOf* a
                                const int32_t* ms_ptr_out, const int32_t* seg, long long p, long long q,
                                long long n_out, int64_t* keys_out, float* vals_out, uint8_t* has_out, int64_t* ts_out,
                                int32_t* row_out, void* stream);
+
+/* ---- trace ingest: appending traces to a live store (csrc/ingest.cu) ------------------------------------------------
+ * A chunk of span rows, grouped on its own by pert_trace_group_*, is taken into a store whose patterns are runtimes
+ * with known key rows (PatternStore.from_trace_groups).  Pattern j of the store is runtime j's representative; the
+ * runtime ids of a store built that way are 0 .. n_pat-1, so a new runtime's id is n_pat + its rank.
+ * Runtime keys: the (um, dm, interface) rows of every representative, file order: rows [3][ld] int64 (um at rows[0..],
+ * dm at rows[ld..], interface at rows[2*ld..]), runtime k owning ptr[k] .. ptr[k+1]-1 of each ([n+1] int32).  The
+ * runtime table is an open-addressing table over them with the hashes of the trace grouping (2 x hash_bits bits, the
+ * same function): slot [S] int32 (runtime index or -1; S a power of two, 64 <= S <= 2^30, n <= S / 2), h1 / h2 [>= n]
+ * uint64 the hashes of every runtime. */
+typedef struct PertRuntimeKeys {
+  long long n;             /* runtimes */
+  long long ld;            /* row stride of rows */
+  const int32_t* ptr;      /* [n+1] */
+  const int64_t* rows;     /* [3][ld] */
+} PertRuntimeKeys;
+typedef struct PertRuntimeTable {
+  long long S;
+  int32_t hash_bits;       /* 1..64 (64 except in tests that force collisions) */
+  int32_t* slot;           /* [S] */
+  uint64_t *h1, *h2;       /* [capacity >= n] */
+} PertRuntimeTable;
+/* Inserts runtimes first .. keys->n - 1 (their key rows must differ from every other runtime's) and writes their
+ * hashes; first = 0 empties the table first (a build or a rebuild into a larger table). */
+int pert_ingest_table_insert(const PertRuntimeKeys* keys, long long first, const PertRuntimeTable* table,
+                             void* stream);
+/* Match of a chunk's runtimes against the store's.  chunk: the chunk's representatives' key rows in the chunk's
+ * insertion order (the first three rows of pert_trace_group_gather's output, with its rep_ptr); chunk_runtime_ins
+ * [chunk->n]: the insertion index of every chunk runtime id (PertTraceGroups.runtime_ins).  The chunk's runtimes must be
+ * distinct (as the grouping makes them).  A chunk runtime matches a store runtime only when the hashes, the length
+ * and every row agree.  Outputs: pat_of [chunk->n] = the store pattern of every chunk runtime, insertion order; a new
+ * runtime gets n_pat + its rank in insertion order; new_rep [chunk->n] lists the insertion indices of the new runtimes
+ * and new_rt [chunk->n] their runtime ids n_pat + rank by chunk runtime id (smallest traceid); n_new [1] int64 their
+ * count.  The table is not changed.  workspace: pert_ingest_match_workspace_bytes(chunk->n). */
+long long pert_ingest_match_workspace_bytes(long long n_chunk);
+int pert_ingest_match(const PertRuntimeKeys* keys, const PertRuntimeTable* table, const PertRuntimeKeys* chunk,
+                      const int32_t* chunk_runtime_ins, int32_t* pat_of, int32_t* new_rep, int32_t* new_rt,
+                      long long* n_new, void* workspace, long long workspace_bytes, void* stream);
+/* Entry-mix merge.  Old mixes: store->n_ent, ent_ptr, ent_pat, ent_nodes, ent_edges (only these fields are read),
+ * cnt [n_pairs] the count of every pair, tot [n_ent] the trace total of every entry.  The chunk's mixes (PertChunkMix,
+ * from its grouping): ent_pair_ptr / ent_trace_ptr [n_ent+1], pair_runtime / pair_prob [n_pairs], runtime_ins, and
+ * pat_of from pert_ingest_match.  pat_nptr / pat_eptr: node / edge offsets of every pattern after the append.
+ * Outputs (PertMixOut), n_ent_out = max(store->n_ent, chunk->n_ent) entries: ent_ptr [n_ent_out+1]; ent_pat, ent_prob
+ * (fp32), cnt [>= n_pairs + chunk->n_pairs, the first ent_ptr[n_ent_out] written]; ent_nodes, ent_edges, tot
+ * [n_ent_out].  Entry e keeps its old pairs in order, then the pairs new to it in chunk order; probability =
+ * (old + chunk count) / (old + chunk total) in fp64, rounded to fp32.  Outputs may not overlap the inputs.
+ * workspace: pert_ingest_merge_workspace_bytes(n_pairs, chunk->n_pairs, n_ent_out).  PERT_ERR_BADARG, before any CUDA
+ * call, for NULL pointers, negative sizes, n_ent_out below either entry count and more than 2^31 - 1 pairs. */
+typedef struct PertChunkMix {
+  long long n_ent, n_pairs;
+  const int32_t *ent_pair_ptr, *ent_trace_ptr, *pair_runtime;
+  const double* pair_prob;
+  const int32_t *runtime_ins, *pat_of;
+} PertChunkMix;
+typedef struct PertMixOut {
+  int32_t *ent_ptr, *ent_pat;
+  float* ent_prob;
+  int32_t *cnt, *ent_nodes, *ent_edges, *tot;
+} PertMixOut;
+long long pert_ingest_merge_workspace_bytes(long long n_pairs, long long n_chunk_pairs, long long n_ent_out);
+int pert_ingest_merge(const PertStore* store, const int32_t* cnt, const int32_t* tot, long long n_pairs,
+                      const PertChunkMix* chunk, const int32_t* pat_nptr, const int32_t* pat_eptr, long long n_ent_out,
+                      const PertMixOut* out, void* workspace, long long workspace_bytes, void* stream);
 
 /* ---- PERT-graph construction (SURVEY 8f row N2) ---------------------------------------------------------------
  * Replaces misc.py:221-319 (GraphConstruct.get_pert_edge_index) for T traces at once.  Input: the cleaned span rows

@@ -70,6 +70,12 @@ SIGNATURES = {
     # resource updates of a live store (csrc/resources.cu; first two arguments: PertStore*, PertResourceAsOf*)
     "pert_store_resources_count": (I, [P, P, P, P, LL, LL, P, P, P, P]),
     "pert_store_resources_merge": (I, [P, P, P, P, P, P, LL, P, P, LL, LL, LL, P, P, P, P, P, P]),
+    # trace ingest of a live store (csrc/ingest.cu; struct pointers, see store.py)
+    "pert_ingest_table_insert": (I, [P, LL, P, P]),
+    "pert_ingest_match_workspace_bytes": (LL, [LL]),
+    "pert_ingest_match": (I, [P, P, P, P, P, P, P, P, P, LL, P]),
+    "pert_ingest_merge_workspace_bytes": (LL, [LL, LL, LL]),
+    "pert_ingest_merge": (I, [P, P, P, LL, P, P, P, LL, P, P, LL, P]),
     # PERT-graph construction (pertgraph.py)
     "pert_pert_graph_count": (I, [P, LL, P, P, I, P, P, P]),
     "pert_pert_graph_build": (I, [P, LL, LL, P, P, P, P, P, P, P, P, I, I, P, P, P, P, P, P]),

@@ -20,6 +20,7 @@
 // Every atomic is a min, an add or a slot claim whose winner does not change any output, so the results do not depend
 // on scheduling.
 #include "common.cuh"
+#include "rowhash.cuh"
 #include "scan.cuh"
 
 #include <algorithm>
@@ -31,21 +32,6 @@ constexpr int TG_SHORT = 1024;          // longer traces are rank-sorted by a wh
 constexpr int TG_TILE = 1024;           // traces per tile of the entry counting sort
 constexpr int TG_EMPTY = -1;
 constexpr unsigned long long TG_NOKEY = ~0ull;
-
-__device__ __forceinline__ unsigned long long mix64(unsigned long long z) {   // splitmix64 finaliser
-  z += 0x9e3779b97f4a7c15ull;
-  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
-  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
-  return z ^ (z >> 31);
-}
-
-__device__ __forceinline__ unsigned long long row_mix(unsigned long long seed, int pos, int64_t um, int64_t dm,
-                                                      int64_t itf) {
-  unsigned long long h = mix64(seed ^ (unsigned long long)pos);
-  h = mix64(h ^ (unsigned long long)um);
-  h = mix64(h ^ (unsigned long long)dm);
-  return mix64(h ^ (unsigned long long)itf);
-}
 
 __device__ __forceinline__ bool valid_id(int64_t v) { return v >= 0 && v <= 0x7fffffffLL; }
 
@@ -177,8 +163,8 @@ __global__ void __launch_bounds__(TG_WARPS * 32) k_trace_reduce(PertSpanTable ta
     amax = max(amax, rt < 0 ? -rt : rt);
     mixed |= tab.entryid[r] != e0;
     const int64_t um = tab.um[r], dm = tab.dm[r], itf = tab.interface[r];
-    s1 += row_mix(0x243f6a8885a308d3ull, i, um, dm, itf);
-    s2 += row_mix(0x13198a2e03707344ull, i, um, dm, itf);
+    s1 += row_mix(RT_SEED1, i, um, dm, itf);
+    s2 += row_mix(RT_SEED2, i, um, dm, itf);
   }
   tmin = warp_min64(tmin);
   amax = warp_max64(amax);
@@ -191,19 +177,24 @@ __global__ void __launch_bounds__(TG_WARPS * 32) k_trace_reduce(PertSpanTable ta
     const bool ok = !mixed && e0 >= 0 && e0 < n_ent;
     if (!ok) atomicExch(status, PERT_ERR_RANGE);        // a trace filed under two entries (or an entry out of range)
     entry[t] = ok ? (int)e0 : 0;
-    const unsigned long long mask = hash_bits >= 64 ? ~0ull : ((1ull << hash_bits) - 1);
+    const unsigned long long mask = hash_mask(hash_bits);
     h1[t] = s1 & mask;
     h2[t] = s2 & mask;
   }
 }
 
-__device__ __forceinline__ bool same_rows(PertSpanTable tab, const int* perm, int a, int b, int len, int lane) {
-  bool eq = true;
-  for (int i = lane; i < len && eq; i += 32) {
-    const int ra = perm[a + i], rb = perm[b + i];
-    eq = tab.um[ra] == tab.um[rb] && tab.dm[ra] == tab.dm[rb] && tab.interface[ra] == tab.interface[rb];
-  }
-  return __all_sync(0xffffffffu, eq);
+// the rows of one trace of the table: perm[b + i] is its row i
+struct PermRows {
+  const PertSpanTable& tab;
+  const int* perm;
+  int b;
+  __device__ int64_t um(int i) const { return tab.um[perm[b + i]]; }
+  __device__ int64_t dm(int i) const { return tab.dm[perm[b + i]]; }
+  __device__ int64_t itf(int i) const { return tab.interface[perm[b + i]]; }
+};
+
+__device__ __forceinline__ bool same_rows(const PertSpanTable& tab, const int* perm, int a, int b, int len, int lane) {
+  return warp_same_rows(PermRows{tab, perm, a}, PermRows{tab, perm, b}, len, lane);
 }
 
 // warp per trace: find (or claim) the slot of its runtime; slots only ever go from empty to an owner
@@ -217,7 +208,7 @@ __global__ void __launch_bounds__(TG_WARPS * 32) k_runtime_insert(PertSpanTable 
   if (t >= T) return;
   const int b = row_ptr[t], len = row_ptr[t + 1] - b;
   const unsigned long long a1 = h1[t], a2 = h2[t];
-  long long s = (long long)(mix64(a1 ^ mix64(a2 ^ (unsigned long long)len)) & (unsigned long long)(S - 1));
+  long long s = runtime_slot(a1, a2, len, S);
   for (;;) {
     int o = 0;
     if (lane == 0) o = atomicCAS(&owner[s], TG_EMPTY, (int)t);

@@ -39,6 +39,37 @@ class _PertBatchOut(C.Structure):
                                  "edge_attr", "entry_id", "y", "ptr", "pattern_probs")]
 
 
+class _RuntimeKeys(C.Structure):
+    _fields_ = [("n", I64), ("ld", I64), ("ptr", P), ("rows", P)]
+
+
+class _RuntimeTable(C.Structure):
+    _fields_ = [("S", I64), ("hash_bits", I32), ("slot", P), ("h1", P), ("h2", P)]
+
+
+class _ChunkMix(C.Structure):
+    _fields_ = [("n_ent", I64), ("n_pairs", I64)] + [(k, P) for k in ("ent_pair_ptr", "ent_trace_ptr", "pair_runtime",
+                                                                     "pair_prob", "runtime_ins", "pat_of")]
+
+
+class _MixOut(C.Structure):
+    _fields_ = [(k, P) for k in ("ent_ptr", "ent_pat", "ent_prob", "cnt", "ent_nodes", "ent_edges", "tot")]
+
+
+def _last_flags_device(nptr, ms):
+    """pat_last on the device: get_x keeps the LAST node of every microservice of a pattern (pert_gnn.py:54-65); a
+    stable sort by (pattern, ms), where the last of every run of equal keys is the largest node index.  ``nptr``: int64
+    [n_pat+1] node offsets, ``ms``: int64 [n_all]."""
+    dev, n_all = ms.device, int(ms.shape[0])
+    pid = torch.repeat_interleave(torch.arange(int(nptr.shape[0]) - 1, device=dev), nptr.diff(), output_size=n_all)
+    key, idx = torch.sort(pid * (1 << 32) + ms, stable=True)
+    run_end = torch.ones(n_all, dtype=torch.bool, device=dev)
+    run_end[:-1] = key[1:] != key[:-1]
+    last = torch.zeros(n_all, dtype=torch.uint8, device=dev)
+    last[idx[run_end]] = 1
+    return last
+
+
 def _last_occurrence_flags(all_ms, nptr):
     """flags[i] = 1 iff node i is the LAST node of its microservice inside its pattern (patterns = nptr slices)."""
     n_all = int(all_ms.shape[0])
@@ -120,6 +151,72 @@ class _BulkPatterns:
     def __init__(self, rt_ids, node_ptr, edge_ptr, ms_id, node_depth, edge_index, edge_attr):
         self.rt_ids, self.node_ptr, self.edge_ptr = rt_ids, node_ptr, edge_ptr
         self.ms_id, self.node_depth, self.edge_index, self.edge_attr = ms_id, node_depth, edge_index, edge_attr
+
+
+class _TraceIngest:
+    """What ``append_traces`` keeps beside a store built by ``from_trace_groups`` (outside ``t``): the graph kind, the
+    runtime keys -- rows [3, R'] int64 (um, dm, interface of every pattern's representative, pattern order) and ptr
+    [n_pat+1] int32 --, cnt [n_pairs] int32 (traces of every (entry, pattern) pair, in ent_pat order), tot [n_ent] int32
+    (traces per entry), tids [n_traces] int64 (every traceid, ascending), the node / edge totals of the patterns, and
+    the runtime table (csrc/ingest.cu), built at the first append."""
+
+    def __init__(self, kind, rows, ptr, cnt, tot, tids, n_nodes, n_edges):
+        self.kind, self.rows, self.ptr, self.cnt, self.tot, self.tids = kind, rows, ptr, cnt, tot, tids
+        self.n_nodes, self.n_edges = n_nodes, n_edges
+        self.table = None                                # dict(slot, h1, h2, S, bits)
+
+    def keys(self):
+        return _RuntimeKeys(int(self.ptr.shape[0]) - 1, int(self.rows.shape[1]), self.ptr.data_ptr(),
+                            self.rows.data_ptr())
+
+    def table_desc(self):
+        t = self.table
+        return _RuntimeTable(t["S"], t["bits"], t["slot"].data_ptr(), t["h1"].data_ptr(), t["h2"].data_ptr())
+
+    def insert(self, first, hash_bits):
+        """Inserts runtimes first.. into the table; rebuilds it (larger) first when the load would pass 1/2 or the hash
+        width changes."""
+        n = int(self.ptr.shape[0]) - 1
+        t = self.table
+        if t is None or t["bits"] != hash_bits or 2 * n > t["S"]:
+            S = 64
+            while S < 4 * n:                             # room to grow to twice the runtimes before the next rebuild
+                S <<= 1
+            dev = self.rows.device
+            self.table = t = {"S": S, "bits": int(hash_bits), "slot": torch.empty(S, dtype=torch.int32, device=dev),
+                              "h1": torch.empty(S // 2, dtype=torch.int64, device=dev),
+                              "h2": torch.empty(S // 2, dtype=torch.int64, device=dev)}
+            first = 0
+        keys, tab = self.keys(), self.table_desc()
+        _lib.check(_lib.lib().pert_ingest_table_insert(C.byref(keys), first, C.byref(tab), _lib.stream()),
+                   "pert_ingest_table_insert")
+
+
+def _check_span_ms(columns, n_ms):
+    """Raises ``PertGnnError`` naming the first span row whose um or dm lies outside [0, n_ms).  Host columns are
+    checked on the host; CUDA columns cost one device -> host read of their minima and maxima (and the rows
+    themselves only when one is out of range)."""
+    host = {}
+    dev = [k for k in ("um", "dm") if torch.is_tensor(columns[k]) and columns[k].is_cuda]
+    if dev:
+        mm = torch.stack([f(columns[k].reshape(-1).long()) for k in dev for f in (torch.min, torch.max)]).tolist()
+        if min(mm[0::2]) >= 0 and max(mm[1::2]) < n_ms:
+            dev = []
+    for k in ("um", "dm"):
+        v = columns[k]
+        if k in dev:
+            host[k] = v.reshape(-1).cpu().numpy()
+        elif not (torch.is_tensor(v) and v.is_cuda):
+            host[k] = np.asarray(v.numpy() if torch.is_tensor(v) else v).reshape(-1)
+    bad = None
+    for k, v in host.items():
+        b = np.flatnonzero((v < 0) | (v >= n_ms))
+        if b.size and (bad is None or b[0] < bad[0]):
+            bad = (int(b[0]), k, int(v[b[0]]))
+    if bad is not None:
+        i, k, v = bad
+        raise _lib.PertGnnError(f"span row {i}: {k} = {v} is outside [0, {n_ms}); the store's microservice ids are "
+                                f"fixed by its n_ms")
 
 
 class PatternStore:
@@ -273,14 +370,7 @@ class PatternStore:
             eptr = torch.from_numpy(np.asarray(graphs.edge_ptr, dtype=np.int64)).to(dev)
             n_pat, n_all = len(self.rt_ids), int(graphs.node_ptr[-1])
             ms = graphs.ms_id.reshape(-1).to(dev, i64)
-            # get_x keeps the LAST node of every microservice of a pattern (pert_gnn.py:54-65): stable sort by
-            # (pattern, ms); the last of every run of equal keys is the largest node index
-            pid = torch.repeat_interleave(torch.arange(n_pat, device=dev), nptr.diff(), output_size=n_all)
-            key, idx = torch.sort(pid * (1 << 32) + ms, stable=True)
-            run_end = torch.ones(n_all, dtype=torch.bool, device=dev)
-            run_end[:-1] = key[1:] != key[:-1]
-            last = torch.zeros(n_all, dtype=torch.uint8, device=dev)
-            last[idx[run_end]] = 1
+            last = _last_flags_device(nptr, ms)
             # entries: entry2runtimes[e] in key order = the (entry, runtime) pairs of the groups
             ent_ptr = groups.ent_pair_ptr
             n_ent, n_pairs = int(ent_ptr.shape[0]) - 1, int(groups.pair_runtime.shape[0])
@@ -291,6 +381,12 @@ class PatternStore:
                 sums.append(torch.zeros(n_ent, dtype=i64, device=dev).index_add_(0, pair_entry,
                                                                                   per_pat[ent_pat.long()]))
             ent_nodes, ent_edges, ent_pats = sums
+            # what append_traces needs besides self.t: the runtime keys and the pair counts.  pair_prob = count / total
+            # correctly rounded with count <= total < 2^31, so prob * total rounds back to the count exactly
+            tot = groups.ent_trace_ptr.diff().to(i32)
+            cnt = torch.round(groups.pair_prob * tot[pair_entry].double()).to(i32)
+            self._ingest = _TraceIngest(kind, groups._rows[:3].contiguous(), groups.rep_ptr.clone(), cnt, tot,
+                                        groups.trace_id, int(graphs.node_ptr[-1]), int(graphs.edge_ptr[-1]))
             order = groups.order.long()
             t_ent = groups.entry[order]
             host = torch.cat([t_ent.long(), groups.trace_id[order], ent_nodes, ent_edges, ent_pats,
@@ -466,6 +562,159 @@ class PatternStore:
     def evict_resources(self, before):
         """Drops every resource row whose timestamp is < ``before``: ``append_resources`` with no rows."""
         return self.append_resources(np.zeros((0, 2), dtype=np.int64), np.zeros((0, 8)), evict_before=before)
+
+    @_lib.on_device_of
+    def append_traces(self, columns, hash_bits=64):
+        """Takes a chunk of processed span rows (``columns``: the nine ``tracegroup.COLUMNS``, int64 host arrays or CUDA
+        tensors, whole traces) into the live store and returns the store indices of its traces, a ``range`` at the
+        end of the trace table: existing trace indices, pattern indices and entry key orders stay valid.  Only stores
+        built by ``from_trace_groups`` keep the runtime keys this needs.
+
+        Afterwards the store equals, bit for bit (``t``, the descriptor's counts, ``rt_ids``, ``trace_keys`` and the
+        host sizing arrays), the constructor fed the grouping of all chunks so far in which the chunk is the leading
+        key of every order: runtime ids by (chunk, smallest traceid), so a new runtime gets id n_rt + j; iteration
+        order (chunk, entry, traceid); a runtime the store has keeps its representative and graph, a new one's
+        representative is its first trace in the chunk's iteration order and its pattern goes after the existing ones;
+        entry e keeps its old keys in order, then the runtimes new to it in order of first appearance in the chunk;
+        probabilities (old count + chunk count) / (old total + chunk total) in fp64, rounded to fp32.  The graphs of
+        the new runtimes are built as ``TraceGroups.graphs`` builds them, with the store's graph kind.  The resource
+        rows and the as-of index are untouched.  ``hash_bits`` narrows the runtime hashes (tests force collisions
+        with it); a collision costs a row comparison and never merges two runtimes.
+
+        Checked before anything changes (``PertGnnError``, the store is left as it was): the chunk's grouping errors
+        (``TraceGroups.check``), a traceid the store already has, um / dm outside [0, n_ms) (naming the first row),
+        a new representative emptied by the row filters (naming the runtime), an ``edge_attr`` width other than the
+        store's, and node, edge, pair or trace counts above 2^31 - 1.
+
+        Host synchronisations: those of ``group_traces`` and its ``check()``; for CUDA um / dm columns one read of their
+        minima and maxima; one read of the chunk's traceids and entries; one of the match result (new runtimes and the
+        representatives' row offsets), followed, when there are new runtimes, by the copy of their rows for the host
+        row filters and the graph build's own read; one of the merged entry sizes.  Ordered on the current stream,
+        like ``append_resources``: the old arrays return to torch's allocator on that stream."""
+        from . import pertgraph, tracegroup
+
+        ing = getattr(self, "_ingest", None)
+        if ing is None:
+            raise _lib.PertGnnError("append_traces: this store keeps no runtime keys (it was built from dicts or by "
+                                    "from_graphs); build it with PatternStore.from_trace_groups to append traces")
+        missing = [k for k in tracegroup.COLUMNS if k not in columns]
+        if missing:
+            raise _lib.PertGnnError(f"append_traces: columns {missing} are missing")
+        dev, L = self.device, _lib.lib()
+        i32, i64 = torch.int32, torch.int64
+        _check_span_ms(columns, self.n_ms)
+        g = tracegroup.group_traces(columns, dev, hash_bits).check()
+        T_old, Tc = len(self.trace_keys), len(g)
+        order = g.order.long()
+        c_tid, c_ent = g.trace_id[order], g.entry[order]
+        tids = ing.tids
+        pos = torch.searchsorted(tids, g.trace_id).clamp_(max=max(int(tids.shape[0]) - 1, 0))
+        dup = tids[pos] == g.trace_id
+        host = torch.cat([c_tid, c_ent.long(), g.trace_id, dup.long()]).cpu().numpy()
+        h_tid, h_ent = host[:Tc], host[Tc:2 * Tc]
+        if host[3 * Tc:].any():
+            raise _lib.PertGnnError(f"append_traces: traceid {int(host[2 * Tc + np.argmax(host[3 * Tc:])])} is "
+                                    "already in the store (a chunk holds whole traces, each traceid once)")
+        if T_old + Tc > _I32_MAX:
+            raise _lib.PertGnnError(f"append_traces: {T_old + Tc} traces exceed the store's 2^31 - 1")
+        # ---- match the chunk's runtimes against the store's (runtime table, csrc/ingest.cu)
+        n_pat, n_c = len(self.rt_ids), g.n_runtimes
+        if ing.table is None or ing.table["bits"] != hash_bits:
+            ing.insert(0, hash_bits)
+        keys, tab = ing.keys(), ing.table_desc()
+        ck = _RuntimeKeys(n_c, int(g._rows.shape[1]), g.rep_ptr.data_ptr(), g._rows.data_ptr())
+        pat_of, new_rep, new_rt = (torch.empty(n_c, dtype=i32, device=dev) for _ in range(3))
+        n_new_d = torch.empty(1, dtype=i64, device=dev)
+        ws = torch.empty(int(L.pert_ingest_match_workspace_bytes(n_c)), dtype=torch.uint8, device=dev)
+        _lib.check(L.pert_ingest_match(C.byref(keys), C.byref(tab), C.byref(ck), g.runtime_ins.data_ptr(),
+                                       pat_of.data_ptr(), new_rep.data_ptr(), new_rt.data_ptr(), n_new_d.data_ptr(),
+                                       ws.data_ptr(), ws.numel(), _lib.stream()), "pert_ingest_match")
+        h = torch.cat([n_new_d, new_rep.long(), new_rt.long(), g.rep_ptr.long()]).cpu().numpy()
+        k = int(h[0])
+        reps, new_ids, rep_ptr = h[1:1 + k], h[1 + n_c:1 + n_c + k], h[1 + 2 * n_c:]
+        # ---- graphs of the new runtimes: host row filters, then the CUDA builder (TraceGroups.graphs' path)
+        lens = rep_ptr[reps + 1] - rep_ptr[reps]
+        new_ptr = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+        sel = torch.from_numpy(np.repeat(rep_ptr[reps] - new_ptr[:-1], lens) + np.arange(int(new_ptr[-1]))).to(dev)
+        new_rows = g._rows[:, sel]
+        if k:
+            rows = new_rows.cpu().numpy()
+            keep, nptr2, roots = pertgraph.clean_span_tables_flat(dict(zip(tracegroup.GATHERED, rows)), new_ptr)
+            empty = np.flatnonzero(np.diff(nptr2) == 0)
+            if empty.size:
+                raise _lib.PertGnnError(f"append_traces: runtime {int(new_ids[empty[0]])}: the row filters "
+                                        "(misc.py:87-105) leave its representative trace without rows")
+            graphs = pertgraph.build_pert_graphs_flat(rows[:len(pertgraph.COLUMNS)][:, keep], nptr2, roots, dev,
+                                                      ing.kind).check()
+            if int(graphs.edge_attr.shape[1]) != self.attr_cols:
+                raise _lib.PertGnnError(f"append_traces: edge_attr has {int(graphs.edge_attr.shape[1])} columns, the "
+                                        f"store {self.attr_cols}")
+            g_nptr, g_eptr = (np.asarray(p, dtype=np.int64) for p in (graphs.node_ptr, graphs.edge_ptr))
+        else:
+            g_nptr = g_eptr = np.zeros(1, dtype=np.int64)
+        n_nodes, n_edges = ing.n_nodes + int(g_nptr[-1]), ing.n_edges + int(g_eptr[-1])
+        n_pairs, n_pc = int(ing.cnt.shape[0]), int(g.pair_runtime.shape[0])
+        for what, v in (("pattern nodes", n_nodes), ("pattern edges", n_edges), ("(entry, runtime) pairs",
+                                                                                  n_pairs + n_pc)):
+            if v > _I32_MAX:
+                raise _lib.PertGnnError(f"append_traces: {v} {what} exceed the store's 2^31 - 1")
+        t = {}
+        t["pat_nptr"] = torch.cat([self.t["pat_nptr"], torch.from_numpy(g_nptr[1:] + ing.n_nodes).to(dev, i32)])
+        t["pat_eptr"] = torch.cat([self.t["pat_eptr"], torch.from_numpy(g_eptr[1:] + ing.n_edges).to(dev, i32)])
+        if k:
+            ms = graphs.ms_id.reshape(-1).to(dev, i64)
+            ei = graphs.edge_index.to(dev)
+            for name, v in (("pat_ms", ms), ("pat_depth", graphs.node_depth.reshape(-1).to(dev, i64)),
+                            ("pat_last", _last_flags_device(torch.from_numpy(g_nptr).to(dev), ms)),
+                            ("pat_src", ei[0].to(i32)), ("pat_dst", ei[1].to(i32)),
+                            ("pat_attr", graphs.edge_attr.to(dev, i64))):
+                t[name] = torch.cat([self.t[name], v])
+        # ---- entry mixes (csrc/ingest.cu)
+        n_ent_c = int(g.ent_pair_ptr.shape[0]) - 1
+        n_ent = max(int(self.desc.n_ent), n_ent_c)
+        mix = _ChunkMix(n_ent_c, n_pc, g.ent_pair_ptr.data_ptr(), g.ent_trace_ptr.data_ptr(),
+                        g.pair_runtime.data_ptr(), g.pair_prob.data_ptr(), g.runtime_ins.data_ptr(), pat_of.data_ptr())
+        o = {"ent_ptr": torch.empty(n_ent + 1, dtype=i32, device=dev),
+             "ent_pat": torch.empty(n_pairs + n_pc, dtype=i32, device=dev),
+             "ent_prob": torch.empty(n_pairs + n_pc, dtype=torch.float32, device=dev),
+             "cnt": torch.empty(n_pairs + n_pc, dtype=i32, device=dev),
+             "ent_nodes": torch.empty(n_ent, dtype=i32, device=dev),
+             "ent_edges": torch.empty(n_ent, dtype=i32, device=dev), "tot": torch.empty(n_ent, dtype=i32, device=dev)}
+        out = _MixOut(*(o[name].data_ptr() for name, _ in _MixOut._fields_))
+        ws = torch.empty(int(L.pert_ingest_merge_workspace_bytes(n_pairs, n_pc, n_ent)), dtype=torch.uint8, device=dev)
+        _lib.check(L.pert_ingest_merge(C.byref(self.desc), ing.cnt.data_ptr(), ing.tot.data_ptr(), n_pairs,
+                                       C.byref(mix), t["pat_nptr"].data_ptr(), t["pat_eptr"].data_ptr(), n_ent,
+                                       C.byref(out), ws.data_ptr(), ws.numel(), _lib.stream()), "pert_ingest_merge")
+        sizes = torch.cat([o["ent_ptr"], o["ent_nodes"], o["ent_edges"]]).long().cpu().numpy()
+        ent_ptr_h = sizes[:n_ent + 1]
+        n_pairs_out = int(ent_ptr_h[-1])
+        t.update({"ent_ptr": o["ent_ptr"], "ent_pat": o["ent_pat"][:n_pairs_out],
+                  "ent_prob": o["ent_prob"][:n_pairs_out], "ent_nodes": o["ent_nodes"], "ent_edges": o["ent_edges"],
+                  "trace_entry": torch.cat([self.t["trace_entry"], c_ent]),
+                  "trace_ts": torch.cat([self.t["trace_ts"], g.bucket[order]]),
+                  "trace_y": torch.cat([self.t["trace_y"], g.y[order]])})
+        # ---- every check passed: swap the new arrays in
+        st = torch.cuda.current_stream()
+        for old in [self.t[name] for name in t] + [ing.rows, ing.ptr, ing.cnt, ing.tot, ing.tids]:
+            old.record_stream(st)                        # the kernels above and earlier assembly on `st` read them
+        for name, v in t.items():
+            self.t[name] = v
+            setattr(self.desc, name, v.data_ptr())
+        self.desc.n_pat, self.desc.n_ent, self.desc.n_traces = n_pat + k, n_ent, T_old + Tc
+        self.rt_ids.extend(int(r) for r in new_ids)
+        self.trace_keys.extend(h_tid.tolist())
+        self._h_trace_entry = np.concatenate([self._h_trace_entry, h_ent])
+        self._h_ent_nodes, self._h_ent_edges = sizes[n_ent + 1:2 * n_ent + 1], sizes[2 * n_ent + 1:]
+        self._h_ent_pats = np.diff(ent_ptr_h)
+        key_rows_old = int(ing.rows.shape[1])
+        ing.rows = torch.cat([ing.rows, new_rows[:3]], dim=1)
+        ing.ptr = torch.cat([ing.ptr, torch.from_numpy(new_ptr[1:] + key_rows_old).to(dev, i32)])
+        ing.cnt, ing.tot = o["cnt"][:n_pairs_out], o["tot"]
+        ing.tids = torch.sort(torch.cat([ing.tids, g.trace_id])).values
+        ing.n_nodes, ing.n_edges = n_nodes, n_edges
+        if k:
+            ing.insert(n_pat, hash_bits)
+        return range(T_old, T_old + Tc)
 
     def __len__(self):
         return len(self.trace_keys)

@@ -49,7 +49,8 @@ extern "C" {
  * pert_model_backward_live, pert_pinball_loss_live, pert_eval_metrics_live; pert_tconv_fwd_c, pert_tconv_bwd_c,
  * pert_model_width (the step engine accepts every hidden width 1..256); pert_trace_group_* (trace grouping);
  * pert_store_assemble_requests (request assembly with the exact or as-of resource join); pert_store_resources_count /
- * _merge (appending and evicting resource rows of a live store); pert_ingest_* (appending traces to a live store). */
+ * _merge (appending and evicting resource rows of a live store); pert_ingest_* (appending traces to a live store);
+ * pert_ingest_evict_* (evicting traces from a live store). */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -523,7 +524,8 @@ int pert_store_resources_merge(const PertStore* store, const PertResourceAsOf* a
 /* ---- trace ingest: appending traces to a live store (csrc/ingest.cu) ------------------------------------------------
  * A chunk of span rows, grouped on its own by pert_trace_group_*, is taken into a store whose patterns are runtimes
  * with known key rows (PatternStore.from_trace_groups).  Pattern j of the store is runtime j's representative; the
- * runtime ids of a store built that way are 0 .. n_pat-1, so a new runtime's id is n_pat + its rank.
+ * runtime ids of a store built that way are 0 .. n_pat-1, so a new runtime's id is n_pat + its rank (after an
+ * eviction has dropped patterns, the caller shifts these ids to the next unissued one: ids are not reused).
  * Runtime keys: the (um, dm, interface) rows of every representative, file order: rows [3][ld] int64 (um at rows[0..],
  * dm at rows[ld..], interface at rows[2*ld..]), runtime k owning ptr[k] .. ptr[k+1]-1 of each ([n+1] int32).  The
  * runtime table is an open-addressing table over them with the hashes of the trace grouping (2 x hash_bits bits, the
@@ -582,6 +584,55 @@ long long pert_ingest_merge_workspace_bytes(long long n_pairs, long long n_chunk
 int pert_ingest_merge(const PertStore* store, const int32_t* cnt, const int32_t* tot, long long n_pairs,
                       const PertChunkMix* chunk, const int32_t* pat_nptr, const int32_t* pat_eptr, long long n_ent_out,
                       const PertMixOut* out, void* workspace, long long workspace_bytes, void* stream);
+/* Trace eviction: drops every trace whose bucket (trace_ts) is < before, with the (entry, pattern) pairs left without
+ * a trace and the patterns left without a pair.  What the store keeps beside PertStore (PertIngestState): the runtime
+ * keys (keys.n = n_pat), trace_pat [n_traces] the pattern of every trace, trace_tid [n_traces] its traceid, cnt
+ * [n_pairs] / tot [n_ent] as for pert_ingest_merge, and the totals of pattern nodes, edges and key rows.  The store
+ * fields read: n_traces, trace_entry, trace_ts, trace_y, n_ent, ent_ptr, ent_pat, n_pat, pat_nptr, pat_eptr, pat_ms,
+ * pat_depth, pat_last, pat_src, pat_dst, pat_attr, attr_cols.
+ * Two calls with one host read between them, so that every output is allocated at its exact new size:
+ *   pert_ingest_evict_count -> sizes [6] int64 (device): traces T', pairs P', patterns n_pat', nodes N', edges E',
+ *                              key rows K' that survive; fills the workspace.
+ *   pert_ingest_evict_apply  -> with those sizes (host) and the same workspace: stable compaction into PertEvictOut.
+ * Traces keep their order (remap [n_traces] int64: new index or -1, monotone on the survivors); entry e keeps its
+ * surviving pairs in order, probability = surviving count / surviving total in fp64 rounded to fp32 (an entry with no
+ * trace left gets no pairs and tot 0; n_ent is kept); patterns keep their order (pat_new [n_pat] int32: new index or
+ * -1), their nodes, edges and key rows unchanged; ent_pat and trace_pat are renumbered.  Output sizes: mix.ent_ptr
+ * [n_ent+1], mix.ent_nodes / ent_edges / tot [n_ent], mix.ent_pat / ent_prob / cnt [P'], trace_* [T'], pat_nptr /
+ * pat_eptr / key_ptr [n_pat'+1], pat_ms / pat_depth / pat_last [N'], pat_src / pat_dst [E'], pat_attr [E'][attr_cols],
+ * key_rows [3][key_ld] with key_ld >= K'.  Outputs may not overlap the inputs.  The integer atomics of the count
+ * make no output depend on scheduling.  workspace: pert_ingest_evict_workspace_bytes(n_traces, n_pairs, n_pat, n_ent).
+ * PERT_ERR_BADARG, before any CUDA call, for NULL pointers, negative sizes or sizes above 2^31 - 16, keys.n != n_pat,
+ * an undersized workspace, and (apply) sizes outside [0, old size]. */
+typedef struct PertIngestState {
+  PertRuntimeKeys keys;
+  const int32_t* trace_pat;  /* [n_traces] */
+  const int64_t* trace_tid;  /* [n_traces] (read by the apply only) */
+  const int32_t *cnt, *tot;  /* [n_pairs], [n_ent] */
+  long long n_pairs, n_nodes, n_edges, n_key_rows;
+} PertIngestState;
+typedef struct PertEvictOut {
+  PertMixOut mix;
+  int64_t* remap;            /* [n_traces] */
+  int32_t* trace_entry;      /* [T'] */
+  int64_t *trace_ts, *trace_y;
+  int32_t* trace_pat;
+  int64_t* trace_tid;
+  int32_t *pat_new;          /* [n_pat] */
+  int32_t *pat_nptr, *pat_eptr;
+  int64_t *pat_ms, *pat_depth;
+  uint8_t* pat_last;
+  int32_t *pat_src, *pat_dst;
+  int64_t* pat_attr;
+  int32_t* key_ptr;
+  int64_t* key_rows;
+  long long key_ld;
+} PertEvictOut;
+long long pert_ingest_evict_workspace_bytes(long long n_traces, long long n_pairs, long long n_pat, long long n_ent);
+int pert_ingest_evict_count(const PertStore* store, const PertIngestState* ing, long long before, void* workspace,
+                            long long workspace_bytes, long long* sizes, void* stream);
+int pert_ingest_evict_apply(const PertStore* store, const PertIngestState* ing, const long long* sizes,
+                            const void* workspace, long long workspace_bytes, const PertEvictOut* out, void* stream);
 
 /* ---- PERT-graph construction (SURVEY 8f row N2) ---------------------------------------------------------------
  * Replaces misc.py:221-319 (GraphConstruct.get_pert_edge_index) for T traces at once.  Input: the cleaned span rows

@@ -76,6 +76,9 @@ SIGNATURES = {
     "pert_ingest_match": (I, [P, P, P, P, P, P, P, P, P, LL, P]),
     "pert_ingest_merge_workspace_bytes": (LL, [LL, LL, LL]),
     "pert_ingest_merge": (I, [P, P, P, LL, P, P, P, LL, P, P, LL, P]),
+    "pert_ingest_evict_workspace_bytes": (LL, [LL, LL, LL, LL]),
+    "pert_ingest_evict_count": (I, [P, P, LL, P, LL, P, P]),
+    "pert_ingest_evict_apply": (I, [P, P, P, P, LL, P, P]),
     # PERT-graph construction (pertgraph.py)
     "pert_pert_graph_count": (I, [P, LL, P, P, I, P, P, P]),
     "pert_pert_graph_build": (I, [P, LL, LL, P, P, P, P, P, P, P, P, I, I, P, P, P, P, P, P]),

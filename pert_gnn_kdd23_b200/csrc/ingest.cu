@@ -18,6 +18,19 @@
 //      (old total + chunk total) in fp64, rounded to fp32.
 // The table only grows; the caller rebuilds it (pert_ingest_table_insert from 0) into a larger one when the load
 // would pass 1/2.
+//
+// Evicting old traces (PatternStore.evict_traces) is split like the resource update into a count and an apply, so the
+// caller allocates every output at its exact new size (an eviction exists to free memory):
+//   1. count: one thread per trace flags keep = bucket >= before; an evicted trace probes the (entry, pattern) pair
+//      table with its entry and pattern (the store keeps the pattern of every trace) and adds 1 to that pair's evicted
+//      count (integer atomics: the sums do not depend on scheduling).  One thread per pair keeps it while its count
+//      stays above 0 and marks its pattern alive; one thread per pattern takes the node / edge / key-row lengths of the
+//      alive ones; one warp per entry sums its surviving nodes, edges and traces.  scan.cuh scans of the trace, pair
+//      and pattern flags and of the surviving lengths give every new position; the sizes word holds their totals.
+//   2. apply: stable compaction, every output slot written once by one thread, no atomics.  Traces and pairs move to
+//      their scanned positions (a pair's pattern renumbered, its probability recomputed as emit() rounds it); the nodes,
+//      edges and key rows of a surviving pattern move as one segment (pat_src / pat_dst are pattern-local).
+// A pattern that keeps any trace keeps its representative's graph and key rows even when that trace was evicted.
 #include "rowhash.cuh"
 #include "scan.cuh"
 
@@ -256,6 +269,233 @@ void scan_launch(int* a0, int* a1, long long L, int* bsum, cudaStream_t st) {   
   k_scan_apply<<<dim3(nb, ny), SCAN_THREADS, 0, st>>>(a0, a1, (int)L, bsum, nb);
 }
 
+// ---- eviction -------------------------------------------------------------------------------------------------------
+
+// the eviction workspace, shared by the count (which fills it) and the apply (which reads it).  Flag arrays are
+// [n+1] with the flag of item i at [i+1]; after the inclusive scan [i] is the item's new position.
+struct EvictWs {
+  long long S;
+  unsigned long long* pkey;   // [S] pair table keys
+  int* pval;                  // [S] pair table values (old pair index)
+  int* ev;                    // [P] evicted traces per old pair
+  int* tkeep;                 // [T+1] trace kept
+  int* pkeep;                 // [P+1] pair kept
+  int* pa;                    // [n_pat+1] pattern kept
+  int* pn;                    // [n_pat+1] nodes of a kept pattern (0 otherwise)
+  int* pe;                    // [n_pat+1] edges of a kept pattern
+  int* pk;                    // [n_pat+1] key rows of a kept pattern
+  int* e_nodes;               // [n_ent] surviving nodes, edges and traces of every entry
+  int* e_edges;
+  int* e_tot;
+  int* bsum;
+};
+
+long long evict_scan_len(long long T, long long P, long long n_pat) {
+  long long L = T > P ? T : P;
+  return (L > n_pat ? L : n_pat) + 1;
+}
+
+long long evict_ws_bytes(long long T, long long P, long long n_pat, long long n_ent) {
+  const long long S = pow2_slots(P);
+  return 8 * S + 4 * (S + P + (T + 1) + (P + 1) + 4 * (n_pat + 1) + 3 * n_ent) + scan_ws(evict_scan_len(T, P, n_pat)) +
+         64;
+}
+
+EvictWs evict_ws(void* w, long long T, long long P, long long n_pat, long long n_ent) {
+  EvictWs a;
+  a.S = pow2_slots(P);
+  a.pkey = (unsigned long long*)w;
+  int* p = (int*)(a.pkey + a.S);
+  a.pval = p;     p += a.S;
+  a.ev = p;       p += P;
+  a.tkeep = p;    p += T + 1;
+  a.pkeep = p;    p += P + 1;
+  a.pa = p;       p += n_pat + 1;
+  a.pn = p;       p += n_pat + 1;
+  a.pe = p;       p += n_pat + 1;
+  a.pk = p;       p += n_pat + 1;
+  a.e_nodes = p;  p += n_ent;
+  a.e_edges = p;  p += n_ent;
+  a.e_tot = p;    p += n_ent;
+  a.bsum = p;
+  return a;
+}
+
+// thread per trace t: tkeep[t+1] = bucket >= before; an evicted trace adds 1 to its (entry, pattern) pair's count
+__global__ void k_evict_traces(PertStore s, const int* trace_pat, long long before, EvictWs w) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= s.n_traces) return;
+  const bool keep = s.trace_ts[t] >= before;
+  w.tkeep[t + 1] = keep;
+  if (keep) return;
+  const unsigned long long key = pair_key(s.trace_entry[t], trace_pat[t]);
+  long long q = (long long)(mix64(key) & (unsigned long long)(w.S - 1));
+  for (;;) {                                              // every trace's pair is in the table
+    const unsigned long long o = w.pkey[q];
+    if (o == key) {
+      atomicAdd(&w.ev[w.pval[q]], 1);
+      return;
+    }
+    if (o == IG_NOKEY) return;
+    q = (q + 1) & (w.S - 1);
+  }
+}
+
+// thread per pair i: kept while traces remain; a kept pair keeps its pattern (pa[pat+1] = 1, the same value from
+// every pair of the pattern)
+__global__ void k_evict_pairs(PertStore s, const int* cnt, long long n_pairs, EvictWs w) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_pairs) return;
+  const bool alive = cnt[i] - w.ev[i] > 0;
+  w.pkeep[i + 1] = alive;
+  if (alive) w.pa[s.ent_pat[i] + 1] = 1;
+}
+
+// thread per pattern p: the node / edge / key-row lengths of a kept pattern, 0 for a dropped one
+__global__ void k_evict_pat_lens(PertStore s, const int* key_ptr, EvictWs w) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= s.n_pat) return;
+  const bool alive = w.pa[p + 1];
+  w.pn[p + 1] = alive ? s.pat_nptr[p + 1] - s.pat_nptr[p] : 0;
+  w.pe[p + 1] = alive ? s.pat_eptr[p + 1] - s.pat_eptr[p] : 0;
+  w.pk[p + 1] = alive ? key_ptr[p + 1] - key_ptr[p] : 0;
+}
+
+// warp per entry e: the nodes, edges and traces of its surviving pairs (integer sums)
+__global__ void __launch_bounds__(IG_WARPS * 32) k_evict_entries(PertStore s, const int* cnt, EvictWs w) {
+  const long long e = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (e >= s.n_ent) return;
+  int nodes = 0, edges = 0, traces = 0;
+  for (int i = s.ent_ptr[e] + lane; i < s.ent_ptr[e + 1]; i += 32) {
+    const int c = cnt[i] - w.ev[i];
+    if (c <= 0) continue;
+    const int p = s.ent_pat[i];
+    nodes += s.pat_nptr[p + 1] - s.pat_nptr[p];
+    edges += s.pat_eptr[p + 1] - s.pat_eptr[p];
+    traces += c;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    nodes += __shfl_xor_sync(0xffffffffu, nodes, o);
+    edges += __shfl_xor_sync(0xffffffffu, edges, o);
+    traces += __shfl_xor_sync(0xffffffffu, traces, o);
+  }
+  if (lane) return;
+  w.e_nodes[e] = nodes;
+  w.e_edges[e] = edges;
+  w.e_tot[e] = traces;
+}
+
+__global__ void k_evict_sizes(long long T, long long P, long long n_pat, EvictWs w, long long* sizes) {
+  sizes[0] = w.tkeep[T];
+  sizes[1] = w.pkeep[P];
+  sizes[2] = w.pa[n_pat];
+  sizes[3] = w.pn[n_pat];
+  sizes[4] = w.pe[n_pat];
+  sizes[5] = w.pk[n_pat];
+}
+
+// thread per old trace t: moves to tkeep[t] if kept; remap[t] = its new index or -1
+__global__ void k_evict_apply_traces(PertStore s, PertIngestState g, EvictWs w, PertEvictOut o) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= s.n_traces) return;
+  const int j = w.tkeep[t];
+  const bool keep = w.tkeep[t + 1] != j;
+  o.remap[t] = keep ? j : -1;
+  if (!keep) return;
+  o.trace_entry[j] = s.trace_entry[t];
+  o.trace_ts[j] = s.trace_ts[t];
+  o.trace_y[j] = s.trace_y[t];
+  o.trace_pat[j] = w.pa[g.trace_pat[t]];
+  o.trace_tid[j] = g.trace_tid[t];
+}
+
+// thread per old pair i: a kept pair moves to pkeep[i] with its pattern renumbered and its probability recomputed
+__global__ void k_evict_apply_pairs(PertStore s, PertIngestState g, EvictWs w, PertMixOut out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= g.n_pairs || w.pkeep[i + 1] == w.pkeep[i]) return;
+  const int e = seg_of(s.ent_ptr, s.n_ent, i);
+  emit(out, w.pkeep[i], w.pa[s.ent_pat[i]], g.cnt[i] - w.ev[i], w.e_tot[e]);
+}
+
+// thread per entry e <= n_ent: its new pair offset (the kept pairs before it) and totals
+__global__ void k_evict_apply_entries(PertStore s, EvictWs w, PertMixOut out) {
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e > s.n_ent) return;
+  out.ent_ptr[e] = w.pkeep[s.ent_ptr[e]];
+  if (e == s.n_ent) return;
+  out.ent_nodes[e] = w.e_nodes[e];
+  out.ent_edges[e] = w.e_edges[e];
+  out.tot[e] = w.e_tot[e];
+}
+
+// thread per old pattern p <= n_pat: the offsets of a kept pattern (and the totals at p = n_pat); pat_new[p]
+__global__ void k_evict_apply_pats(PertStore s, EvictWs w, PertEvictOut o) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p > s.n_pat) return;
+  const int j = w.pa[p];
+  const bool alive = p < s.n_pat && w.pa[p + 1] != j;
+  if (p < s.n_pat) o.pat_new[p] = alive ? j : -1;
+  if (p < s.n_pat && !alive) return;
+  o.pat_nptr[j] = w.pn[p];
+  o.pat_eptr[j] = w.pe[p];
+  o.key_ptr[j] = w.pk[p];
+}
+
+// thread per old node v: the nodes of a kept pattern move as one segment
+__global__ void k_evict_apply_nodes(PertStore s, long long n_nodes, EvictWs w, PertEvictOut o) {
+  const long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n_nodes) return;
+  const int p = seg_of(s.pat_nptr, s.n_pat, v);
+  if (w.pa[p + 1] == w.pa[p]) return;
+  const long long j = w.pn[p] + (v - s.pat_nptr[p]);
+  o.pat_ms[j] = s.pat_ms[v];
+  o.pat_depth[j] = s.pat_depth[v];
+  o.pat_last[j] = s.pat_last[v];
+}
+
+// thread per old edge x: pattern-local endpoints, so a pure segment move
+__global__ void k_evict_apply_edges(PertStore s, long long n_edges, EvictWs w, PertEvictOut o) {
+  const long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= n_edges) return;
+  const int p = seg_of(s.pat_eptr, s.n_pat, x);
+  if (w.pa[p + 1] == w.pa[p]) return;
+  const long long j = w.pe[p] + (x - s.pat_eptr[p]);
+  o.pat_src[j] = s.pat_src[x];
+  o.pat_dst[j] = s.pat_dst[x];
+  for (int c = 0; c < s.attr_cols; ++c) o.pat_attr[j * s.attr_cols + c] = s.pat_attr[x * s.attr_cols + c];
+}
+
+// thread per old key row r: the runtime keys move like the nodes
+__global__ void k_evict_apply_keys(PertStore s, PertIngestState g, EvictWs w, PertEvictOut o) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= g.n_key_rows) return;
+  const int p = seg_of(g.keys.ptr, s.n_pat, r);
+  if (w.pa[p + 1] == w.pa[p]) return;
+  const long long j = w.pk[p] + (r - g.keys.ptr[p]);
+  const long long ld = g.keys.ld, nld = o.key_ld;
+  o.key_rows[j] = g.keys.rows[r];
+  o.key_rows[nld + j] = g.keys.rows[ld + r];
+  o.key_rows[2 * nld + j] = g.keys.rows[2 * ld + r];
+}
+
+constexpr long long IG_MAX = 0x7ffffff0LL;
+
+// the argument checks both eviction calls share
+bool evict_args_ok(const PertStore* s, const PertIngestState* g) {
+  if (!s || !g || s->n_traces < 0 || s->n_traces > IG_MAX || s->n_pat < 0 || s->n_ent < 0 || g->n_pairs < 0 ||
+      g->n_pairs > IG_MAX || g->n_nodes < 0 || g->n_nodes > IG_MAX || g->n_edges < 0 || g->n_edges > IG_MAX ||
+      g->n_key_rows < 0 || g->n_key_rows > g->keys.ld || s->attr_cols < 0 || !keys_ok(&g->keys) ||
+      g->keys.n != s->n_pat)
+    return false;
+  if (!s->ent_ptr || !s->pat_nptr || !s->pat_eptr || (s->n_ent > 0 && !g->tot) ||
+      (s->n_traces > 0 && (!s->trace_entry || !s->trace_ts || !g->trace_pat)) ||
+      (g->n_pairs > 0 && (!s->ent_pat || !g->cnt)))
+    return false;
+  return true;
+}
+
 }  // namespace
 
 extern "C" {
@@ -358,6 +598,77 @@ int pert_ingest_merge(const PertStore* store, const int32_t* cnt, const int32_t*
   scan_launch(out->ent_ptr, nullptr, n_ent_out + 1, bsum, st);
   if (n_pairs > 0) k_emit_old<<<pert_cdiv(n_pairs, B), B, 0, st>>>(*store, cnt, add, n_pairs, *out);
   if (np > 0) k_emit_new<<<pert_cdiv(np, B), B, 0, st>>>(*store, *chunk, nf, jent, jpat, jcnt, *out);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+long long pert_ingest_evict_workspace_bytes(long long n_traces, long long n_pairs, long long n_pat, long long n_ent) {
+  if (n_traces < 0 || n_pairs < 0 || n_pat < 0 || n_ent < 0 || n_traces > IG_MAX || n_pairs > IG_MAX ||
+      n_pat > IG_MAX || n_ent > IG_MAX)
+    return PERT_ERR_BADARG;
+  return evict_ws_bytes(n_traces, n_pairs, n_pat, n_ent);
+}
+
+int pert_ingest_evict_count(const PertStore* store, const PertIngestState* ing, long long before, void* workspace,
+                            long long workspace_bytes, long long* sizes, void* stream) {
+  if (!evict_args_ok(store, ing) || !workspace || !sizes) return PERT_ERR_BADARG;
+  const long long T = store->n_traces, P = ing->n_pairs, n_pat = store->n_pat, n_ent = store->n_ent;
+  if (workspace_bytes < evict_ws_bytes(T, P, n_pat, n_ent)) return PERT_ERR_BADARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const EvictWs w = evict_ws(workspace, T, P, n_pat, n_ent);
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(w.pkey, 0xff, 8 * w.S, st)) ||
+      (e = cudaMemsetAsync(w.pval, 0, (char*)w.bsum - (char*)w.pval, st)))
+    return (int)e;
+  const int B = IG_THREADS, WB = IG_WARPS * 32;
+  if (P > 0) k_pair_table<<<pert_cdiv(P, B), B, 0, st>>>(*store, P, w.S, w.pkey, w.pval);
+  if (T > 0) k_evict_traces<<<pert_cdiv(T, B), B, 0, st>>>(*store, ing->trace_pat, before, w);
+  if (P > 0) k_evict_pairs<<<pert_cdiv(P, B), B, 0, st>>>(*store, ing->cnt, P, w);
+  if (n_pat > 0) k_evict_pat_lens<<<pert_cdiv(n_pat, B), B, 0, st>>>(*store, ing->keys.ptr, w);
+  if (n_ent > 0) k_evict_entries<<<pert_cdiv(n_ent * 32, WB), WB, 0, st>>>(*store, ing->cnt, w);
+  if (T > 0) scan_launch(w.tkeep, nullptr, T + 1, w.bsum, st);
+  if (P > 0) scan_launch(w.pkeep, nullptr, P + 1, w.bsum, st);
+  if (n_pat > 0) {
+    scan_launch(w.pa, w.pn, n_pat + 1, w.bsum, st);
+    scan_launch(w.pe, w.pk, n_pat + 1, w.bsum, st);
+  }
+  k_evict_sizes<<<1, 1, 0, st>>>(T, P, n_pat, w, sizes);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+int pert_ingest_evict_apply(const PertStore* store, const PertIngestState* ing, const long long* sizes,
+                            const void* workspace, long long workspace_bytes, const PertEvictOut* out, void* stream) {
+  if (!evict_args_ok(store, ing) || !workspace || !sizes || !out) return PERT_ERR_BADARG;
+  const long long T = store->n_traces, P = ing->n_pairs, n_pat = store->n_pat, n_ent = store->n_ent;
+  if (workspace_bytes < evict_ws_bytes(T, P, n_pat, n_ent)) return PERT_ERR_BADARG;
+  const long long T2 = sizes[0], P2 = sizes[1], n_pat2 = sizes[2], N2 = sizes[3], E2 = sizes[4], K2 = sizes[5];
+  if (T2 < 0 || T2 > T || P2 < 0 || P2 > P || n_pat2 < 0 || n_pat2 > n_pat || N2 < 0 || N2 > ing->n_nodes ||
+      E2 < 0 || E2 > ing->n_edges || K2 < 0 || K2 > ing->n_key_rows || out->key_ld < K2)
+    return PERT_ERR_BADARG;
+  const PertMixOut& m = out->mix;
+  if ((T > 0 && (!ing->trace_tid || !out->remap)) ||
+      (T2 > 0 && (!out->trace_entry || !out->trace_ts || !out->trace_y || !out->trace_pat || !out->trace_tid)) ||
+      (T > 0 && !store->trace_y) || !m.ent_ptr || (n_ent > 0 && (!m.ent_nodes || !m.ent_edges || !m.tot)) ||
+      (P2 > 0 && (!m.ent_pat || !m.ent_prob || !m.cnt)) || (n_pat > 0 && !out->pat_new) || !out->pat_nptr ||
+      !out->pat_eptr || !out->key_ptr)
+    return PERT_ERR_BADARG;
+  if ((ing->n_nodes > 0 && (!store->pat_ms || !store->pat_depth || !store->pat_last)) ||
+      (N2 > 0 && (!out->pat_ms || !out->pat_depth || !out->pat_last)) ||
+      (ing->n_edges > 0 && (!store->pat_src || !store->pat_dst || (store->attr_cols > 0 && !store->pat_attr))) ||
+      (E2 > 0 && (!out->pat_src || !out->pat_dst || (store->attr_cols > 0 && !out->pat_attr))) ||
+      (K2 > 0 && !out->key_rows))
+    return PERT_ERR_BADARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const EvictWs w = evict_ws((void*)workspace, T, P, n_pat, n_ent);
+  const int B = IG_THREADS;
+  if (T > 0) k_evict_apply_traces<<<pert_cdiv(T, B), B, 0, st>>>(*store, *ing, w, *out);
+  if (P > 0) k_evict_apply_pairs<<<pert_cdiv(P, B), B, 0, st>>>(*store, *ing, w, m);
+  k_evict_apply_entries<<<pert_cdiv(n_ent + 1, B), B, 0, st>>>(*store, w, m);
+  k_evict_apply_pats<<<pert_cdiv(n_pat + 1, B), B, 0, st>>>(*store, w, *out);
+  if (ing->n_nodes > 0) k_evict_apply_nodes<<<pert_cdiv(ing->n_nodes, B), B, 0, st>>>(*store, ing->n_nodes, w, *out);
+  if (ing->n_edges > 0) k_evict_apply_edges<<<pert_cdiv(ing->n_edges, B), B, 0, st>>>(*store, ing->n_edges, w, *out);
+  if (ing->n_key_rows > 0) k_evict_apply_keys<<<pert_cdiv(ing->n_key_rows, B), B, 0, st>>>(*store, *ing, w, *out);
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }

@@ -15,6 +15,7 @@ tests/golden/ref_loop.npz).  No CPU fallback: the store lives on a CUDA device.
 from __future__ import annotations
 
 import ctypes as C
+import itertools
 
 import numpy as np
 import torch
@@ -54,6 +55,19 @@ class _ChunkMix(C.Structure):
 
 class _MixOut(C.Structure):
     _fields_ = [(k, P) for k in ("ent_ptr", "ent_pat", "ent_prob", "cnt", "ent_nodes", "ent_edges", "tot")]
+
+
+class _IngestState(C.Structure):
+    _fields_ = [("keys", _RuntimeKeys)] + [(k, P) for k in ("trace_pat", "trace_tid", "cnt", "tot")] + \
+        [(k, I64) for k in ("n_pairs", "n_nodes", "n_edges", "n_key_rows")]
+
+
+_EVICT_ARRAYS = ("remap", "trace_entry", "trace_ts", "trace_y", "trace_pat", "trace_tid", "pat_new", "pat_nptr",
+                 "pat_eptr", "pat_ms", "pat_depth", "pat_last", "pat_src", "pat_dst", "pat_attr", "key_ptr", "key_rows")
+
+
+class _EvictOut(C.Structure):
+    _fields_ = [("mix", _MixOut)] + [(k, P) for k in _EVICT_ARRAYS] + [("key_ld", I64)]
 
 
 def _last_flags_device(nptr, ms):
@@ -158,12 +172,21 @@ class _TraceIngest:
     runtime keys -- rows [3, R'] int64 (um, dm, interface of every pattern's representative, pattern order) and ptr
     [n_pat+1] int32 --, cnt [n_pairs] int32 (traces of every (entry, pattern) pair, in ent_pat order), tot [n_ent] int32
     (traces per entry), tids [n_traces] int64 (every traceid, ascending), the node / edge totals of the patterns, and
-    the runtime table (csrc/ingest.cu), built at the first append."""
+    the runtime table (csrc/ingest.cu), built at the first append.  For ``evict_traces``: trace_pat [n_traces] int32
+    and trace_tid [n_traces] int64 (the pattern and traceid of every trace, trace-table order), and next_rt, the
+    number of runtime ids ever issued (ids are never reused: a runtime seen again after its pattern was evicted is
+    new)."""
 
-    def __init__(self, kind, rows, ptr, cnt, tot, tids, n_nodes, n_edges):
+    def __init__(self, kind, rows, ptr, cnt, tot, tids, n_nodes, n_edges, trace_pat, trace_tid, next_rt):
         self.kind, self.rows, self.ptr, self.cnt, self.tot, self.tids = kind, rows, ptr, cnt, tot, tids
         self.n_nodes, self.n_edges = n_nodes, n_edges
+        self.trace_pat, self.trace_tid, self.next_rt = trace_pat, trace_tid, next_rt
         self.table = None                                # dict(slot, h1, h2, S, bits)
+
+    def state(self):
+        return _IngestState(self.keys(), self.trace_pat.data_ptr(), self.trace_tid.data_ptr(), self.cnt.data_ptr(),
+                            self.tot.data_ptr(), int(self.cnt.shape[0]), self.n_nodes, self.n_edges,
+                            int(self.rows.shape[1]))
 
     def keys(self):
         return _RuntimeKeys(int(self.ptr.shape[0]) - 1, int(self.rows.shape[1]), self.ptr.data_ptr(),
@@ -385,9 +408,11 @@ class PatternStore:
             # correctly rounded with count <= total < 2^31, so prob * total rounds back to the count exactly
             tot = groups.ent_trace_ptr.diff().to(i32)
             cnt = torch.round(groups.pair_prob * tot[pair_entry].double()).to(i32)
-            self._ingest = _TraceIngest(kind, groups._rows[:3].contiguous(), groups.rep_ptr.clone(), cnt, tot,
-                                        groups.trace_id, int(graphs.node_ptr[-1]), int(graphs.edge_ptr[-1]))
             order = groups.order.long()
+            self._ingest = _TraceIngest(kind, groups._rows[:3].contiguous(), groups.rep_ptr.clone(), cnt, tot,
+                                        groups.trace_id, int(graphs.node_ptr[-1]), int(graphs.edge_ptr[-1]),
+                                        groups.runtime_ins[groups.runtime[order].long()].to(i32),
+                                        groups.trace_id[order], n_pat)
             t_ent = groups.entry[order]
             host = torch.cat([t_ent.long(), groups.trace_id[order], ent_nodes, ent_edges, ent_pats,
                               ms.max().reshape(1) if n_all else torch.zeros(1, dtype=i64, device=dev)]).cpu().numpy()
@@ -572,7 +597,8 @@ class PatternStore:
 
         Afterwards the store equals, bit for bit (``t``, the descriptor's counts, ``rt_ids``, ``trace_keys`` and the
         host sizing arrays), the constructor fed the grouping of all chunks so far in which the chunk is the leading
-        key of every order: runtime ids by (chunk, smallest traceid), so a new runtime gets id n_rt + j; iteration
+        key of every order: runtime ids by (chunk, smallest traceid), so a new runtime gets id next_rt + j (next_rt:
+        the number of runtime ids the store has issued, n_rt unless ``evict_traces`` dropped patterns); iteration
         order (chunk, entry, traceid); a runtime the store has keeps its representative and graph, a new one's
         representative is its first trace in the chunk's iteration order and its pattern goes after the existing ones;
         entry e keeps its old keys in order, then the runtimes new to it in order of first appearance in the chunk;
@@ -608,8 +634,11 @@ class PatternStore:
         order = g.order.long()
         c_tid, c_ent = g.trace_id[order], g.entry[order]
         tids = ing.tids
-        pos = torch.searchsorted(tids, g.trace_id).clamp_(max=max(int(tids.shape[0]) - 1, 0))
-        dup = tids[pos] == g.trace_id
+        if tids.numel():
+            pos = torch.searchsorted(tids, g.trace_id).clamp_(max=int(tids.shape[0]) - 1)
+            dup = tids[pos] == g.trace_id
+        else:                                            # every trace was evicted
+            dup = torch.zeros_like(g.trace_id, dtype=torch.bool)
         host = torch.cat([c_tid, c_ent.long(), g.trace_id, dup.long()]).cpu().numpy()
         h_tid, h_ent = host[:Tc], host[Tc:2 * Tc]
         if host[3 * Tc:].any():
@@ -632,6 +661,7 @@ class PatternStore:
         h = torch.cat([n_new_d, new_rep.long(), new_rt.long(), g.rep_ptr.long()]).cpu().numpy()
         k = int(h[0])
         reps, new_ids, rep_ptr = h[1:1 + k], h[1 + n_c:1 + n_c + k], h[1 + 2 * n_c:]
+        new_ids = new_ids + (ing.next_rt - n_pat)        # ids n_pat + j -> next_rt + j: evicted ids are not reused
         # ---- graphs of the new runtimes: host row filters, then the CUDA builder (TraceGroups.graphs' path)
         lens = rep_ptr[reps + 1] - rep_ptr[reps]
         new_ptr = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
@@ -693,9 +723,12 @@ class PatternStore:
                   "trace_entry": torch.cat([self.t["trace_entry"], c_ent]),
                   "trace_ts": torch.cat([self.t["trace_ts"], g.bucket[order]]),
                   "trace_y": torch.cat([self.t["trace_y"], g.y[order]])})
+        trace_pat = torch.cat([ing.trace_pat, pat_of[g.runtime_ins[g.runtime[order].long()].long()]])
+        trace_tid = torch.cat([ing.trace_tid, c_tid])
         # ---- every check passed: swap the new arrays in
         st = torch.cuda.current_stream()
-        for old in [self.t[name] for name in t] + [ing.rows, ing.ptr, ing.cnt, ing.tot, ing.tids]:
+        for old in [self.t[name] for name in t] + [ing.rows, ing.ptr, ing.cnt, ing.tot, ing.tids, ing.trace_pat,
+                                                   ing.trace_tid]:
             old.record_stream(st)                        # the kernels above and earlier assembly on `st` read them
         for name, v in t.items():
             self.t[name] = v
@@ -712,9 +745,99 @@ class PatternStore:
         ing.cnt, ing.tot = o["cnt"][:n_pairs_out], o["tot"]
         ing.tids = torch.sort(torch.cat([ing.tids, g.trace_id])).values
         ing.n_nodes, ing.n_edges = n_nodes, n_edges
+        ing.trace_pat, ing.trace_tid, ing.next_rt = trace_pat, trace_tid, ing.next_rt + k
         if k:
             ing.insert(n_pat, hash_bits)
         return range(T_old, T_old + Tc)
+
+    @_lib.on_device_of
+    def evict_traces(self, before):
+        """Drops every trace whose bucket (``t["trace_ts"]``) is < ``before`` from the live store, with what only those
+        traces held, and returns ``remap``: a numpy int64 array over the old trace indices, the new index of every
+        surviving trace and -1 for an evicted one.  Survivors keep their order (``remap`` is monotone on them), so a
+        held ``StoreLoader`` dataset or index list stays valid after ``remap[ids]`` and dropping the -1s.  Only stores
+        built by ``from_trace_groups`` keep the per-trace patterns this needs.
+
+        Afterwards the store equals, bit for bit (``t``, the descriptor's counts, ``rt_ids``, ``trace_keys`` and the
+        host sizing arrays), ``PatternStore(runtime2graph', entry2runtimes', resources, tr2data', n_ms=store.n_ms)``:
+        tr2data' the old one without the evicted traces, in order; entry2runtimes'[e] for every e < n_ent (n_ent never
+        shrinks) e's old keys in order without those left with no trace, probabilities surviving count / surviving
+        total in fp64, rounded to fp32, and ``{}`` for an entry with no trace left (``check_entries`` refuses it);
+        runtime2graph' the old map restricted to the runtimes that keep a trace, in order, with the same graphs -- a
+        pattern whose representative was evicted keeps that representative's graph and key rows.  A pattern with no
+        trace left goes with its nodes, edges and runtime key; its runtime id is not reused: the runtime, seen again by
+        ``append_traces``, is new (a new id, representative and graph).  The resource rows and the as-of index are
+        untouched; every new array has its exact new size (the kernels of csrc/ingest.cu count, then compact).
+
+        ``before`` outside int64 raises ``PertGnnError``.  When no trace is evicted the store is left as it is and the
+        identity is returned.  Host synchronisations: one read of the surviving sizes, one read of the host copies
+        (remap, the surviving traces' entries, the surviving patterns, the entry sizing arrays).  Ordered on the
+        current stream, like ``append_resources``: the old arrays return to torch's allocator on that stream."""
+        cut = int(before)
+        if not _I64_MIN <= cut <= _I64_MAX:
+            raise _lib.PertGnnError(f"evict_traces: before = {cut} is outside int64")
+        ing = getattr(self, "_ingest", None)
+        if ing is None:
+            raise _lib.PertGnnError("evict_traces: this store keeps no runtime keys (it was built from dicts or by "
+                                    "from_graphs); build it with PatternStore.from_trace_groups to evict traces")
+        dev, L = self.device, _lib.lib()
+        i32, i64 = torch.int32, torch.int64
+        T, n_pat, n_ent = int(self.desc.n_traces), int(self.desc.n_pat), int(self.desc.n_ent)
+        if T == 0:
+            return np.zeros(0, dtype=np.int64)
+        state = ing.state()
+        ws = torch.empty(int(L.pert_ingest_evict_workspace_bytes(T, int(ing.cnt.shape[0]), n_pat, n_ent)),
+                         dtype=torch.uint8, device=dev)
+        sizes_d = torch.empty(6, dtype=i64, device=dev)
+        _lib.check(L.pert_ingest_evict_count(C.byref(self.desc), C.byref(state), cut, ws.data_ptr(), ws.numel(),
+                                             sizes_d.data_ptr(), _lib.stream()), "pert_ingest_evict_count")
+        sizes = [int(x) for x in sizes_d.tolist()]
+        T2, P2, n_pat2, N2, E2, K2 = sizes
+        if T2 == T:
+            return np.arange(T, dtype=np.int64)
+        empty = lambda n, dt: torch.empty(n, dtype=dt, device=dev)            # noqa: E731
+        mix = {"ent_ptr": empty(n_ent + 1, i32), "ent_pat": empty(P2, i32), "ent_prob": empty(P2, torch.float32),
+               "cnt": empty(P2, i32), "ent_nodes": empty(n_ent, i32), "ent_edges": empty(n_ent, i32),
+               "tot": empty(n_ent, i32)}
+        o = {"remap": empty(T, i64), "trace_entry": empty(T2, i32), "trace_ts": empty(T2, i64),
+             "trace_y": empty(T2, i64), "trace_pat": empty(T2, i32), "trace_tid": empty(T2, i64),
+             "pat_new": empty(n_pat, i32), "pat_nptr": empty(n_pat2 + 1, i32), "pat_eptr": empty(n_pat2 + 1, i32),
+             "pat_ms": empty(N2, i64), "pat_depth": empty(N2, i64), "pat_last": empty(N2, torch.uint8),
+             "pat_src": empty(E2, i32), "pat_dst": empty(E2, i32), "pat_attr": empty((E2, self.attr_cols), i64),
+             "key_ptr": empty(n_pat2 + 1, i32), "key_rows": empty((3, K2), i64)}
+        out = _EvictOut(_MixOut(*(mix[name].data_ptr() for name, _ in _MixOut._fields_)),
+                        *(o[name].data_ptr() for name in _EVICT_ARRAYS), K2)
+        _lib.check(L.pert_ingest_evict_apply(C.byref(self.desc), C.byref(state), (C.c_longlong * 6)(*sizes),
+                                             ws.data_ptr(), ws.numel(), C.byref(out), _lib.stream()),
+                   "pert_ingest_evict_apply")
+        host = torch.cat([o["remap"], o["trace_entry"].long(), o["pat_new"].long(), mix["ent_ptr"].long(),
+                          mix["ent_nodes"].long(), mix["ent_edges"].long()]).cpu().numpy()
+        remap, h_ent, pat_new, ent_ptr_h, h_nodes, h_edges = np.split(host, np.cumsum([T, T2, n_pat, n_ent + 1, n_ent]))
+        tids = torch.sort(o["trace_tid"]).values
+        # ---- swap the new arrays in
+        t = {"pat_nptr": o["pat_nptr"], "pat_eptr": o["pat_eptr"], "pat_ms": o["pat_ms"], "pat_depth": o["pat_depth"],
+             "pat_last": o["pat_last"], "pat_src": o["pat_src"], "pat_dst": o["pat_dst"], "pat_attr": o["pat_attr"],
+             "ent_ptr": mix["ent_ptr"], "ent_pat": mix["ent_pat"], "ent_prob": mix["ent_prob"],
+             "ent_nodes": mix["ent_nodes"], "ent_edges": mix["ent_edges"], "trace_entry": o["trace_entry"],
+             "trace_ts": o["trace_ts"], "trace_y": o["trace_y"]}
+        st = torch.cuda.current_stream()
+        for old in [self.t[name] for name in t] + [ing.rows, ing.ptr, ing.cnt, ing.tot, ing.tids, ing.trace_pat,
+                                                   ing.trace_tid]:
+            old.record_stream(st)                        # the kernels above and earlier assembly on `st` read them
+        for name, v in t.items():
+            self.t[name] = v
+            setattr(self.desc, name, v.data_ptr())
+        self.desc.n_pat, self.desc.n_traces = n_pat2, T2
+        self.rt_ids = [r for r, p in zip(self.rt_ids, pat_new) if p >= 0]
+        # the surviving keys in order: a C-level filter of the list, several times faster than a list of the device
+        # traceids (no new int objects)
+        self.trace_keys = list(itertools.compress(self.trace_keys, (remap >= 0).view(np.uint8).tobytes()))
+        self._h_trace_entry, self._h_ent_nodes, self._h_ent_edges = h_ent, h_nodes, h_edges
+        self._h_ent_pats = np.diff(ent_ptr_h)
+        ing.rows, ing.ptr, ing.cnt, ing.tot, ing.tids = o["key_rows"], o["key_ptr"], mix["cnt"], mix["tot"], tids
+        ing.trace_pat, ing.trace_tid, ing.n_nodes, ing.n_edges = o["trace_pat"], o["trace_tid"], N2, E2
+        ing.table = None                                 # it holds pattern indices: the next append rebuilds it
+        return remap
 
     def __len__(self):
         return len(self.trace_keys)

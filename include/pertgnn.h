@@ -50,7 +50,8 @@ extern "C" {
  * pert_model_width (the step engine accepts every hidden width 1..256); pert_trace_group_* (trace grouping);
  * pert_store_assemble_requests (request assembly with the exact or as-of resource join); pert_store_resources_count /
  * _merge (appending and evicting resource rows of a live store); pert_ingest_* (appending traces to a live store);
- * pert_ingest_evict_* (evicting traces from a live store). */
+ * pert_ingest_evict_* (evicting traces from a live store); pert_store_assemble_whatif (per-request pattern mixes and
+ * resource overrides), pert_store_lookup_resources. */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -484,6 +485,47 @@ typedef struct PertResourceAsOf {
 int pert_store_assemble_requests(const PertStore* store, const PertResourceAsOf* asof, const int64_t* entry_ids,
                                  const int64_t* timestamps, long long B, long long N, long long E, int* offsets,
                                  const PertBatchOut* out, int* status, void* stream);
+
+/* ---- what-if request assembly: per-request pattern mixes and resource overrides ------------------------------------
+ * pert_store_assemble_requests with two optional replacements, read from `w`:
+ *   mix_ptr [B+1] int64 (NULL: every request uses its entry's stored mix): graph b is the concatenation, in slot order,
+ *     of patterns mix_pat[k] (int32 pattern index) for k = mix_ptr[b] .. mix_ptr[b+1]-1, with probabilities
+ *     mix_prob[k] (float32) as pattern_probs and per-node rt_probs, instead of entry_ids[b]'s stored mix.  The offsets
+ *     are absolute, so a caller may pass a slice of a longer CSR without rebasing.  entry_ids[b] still selects the
+ *     entry embedding and is written to entry_id; its own mix is not read, so it may be empty.  Probabilities are used
+ *     as given (they need not sum to 1).
+ *   scenario [B] int64 (NULL: none), with n_ov override rows: ov_keys [n_ov] int64 = scenario * n_ms + ms, sorted
+ *     ascending (>= 0), and ov_vals [n_ov, 8] float32 (16-byte aligned).  At the node that receives statistics (the last
+ *     node of a microservice m in its pattern, as in pert_store_assemble), a request with scenario s >= 0 reads the
+ *     first row of key s * n_ms + m if there is one: the node gets its values and indicator 0, whether or not m has
+ *     resource rows, and no store join runs for it (so the exact join flags no missing row there).  Without such a
+ *     row (scenario -1, or no row of that key) the exact or as-of join runs as in pert_store_assemble_requests.
+ * N, E and the pattern total size the outputs as there: sums over the requests' mixes of the patterns' node / edge
+ * counts and the mixes' lengths.  On the device, an entry < 0 or >= n_ent (or, without mix_ptr, with no patterns), a
+ * pattern index outside [0, n_pat) or an empty mix sets PERT_ERR_RANGE in status; the graph then reads entry 0 /
+ * pattern 0 (an empty mix gives an empty graph).  PERT_ERR_BADARG, before any CUDA call, for NULL pointers with
+ * non-zero sizes (including w, and mix_pat / mix_prob when mix_ptr is set), negative sizes and ov_vals not 16-byte
+ * aligned; B = 0 returns PERT_OK and launches nothing. */
+typedef struct PertWhatIf {
+  const int64_t* mix_ptr;   /* [B+1] or NULL */
+  const int32_t* mix_pat;   /* [mix_ptr[B]]  */
+  const float* mix_prob;    /* [mix_ptr[B]]  */
+  const int64_t* scenario;  /* [B] or NULL   */
+  long long n_ov;
+  const int64_t* ov_keys;   /* [n_ov]        */
+  const float* ov_vals;     /* [n_ov, 8]     */
+} PertWhatIf;
+int pert_store_assemble_whatif(const PertStore* store, const PertResourceAsOf* asof, const PertWhatIf* w,
+                               const int64_t* entry_ids, const int64_t* timestamps, long long B, long long N,
+                               long long E, int* offsets, const PertBatchOut* out, int* status, void* stream);
+
+/* The resource row each join of request assembly reads, for k (timestamp, ms) queries: values [k, 8] float32 get the
+ * row of (floor(timestamps[i] / 30000) * 30000, ms[i]) -- the exact join (asof == NULL) or the as-of join -- and
+ * found [k] uint8 is 1; with no such row, or ms outside [0, n_ms), values are 0 and found is 0.  Only the resource
+ * fields of `store` are read.  PERT_ERR_BADARG, before any CUDA call, for NULL pointers with k > 0, k < 0 or
+ * k > 2^31 - 1; k = 0 returns PERT_OK and launches nothing. */
+int pert_store_lookup_resources(const PertStore* store, const PertResourceAsOf* asof, const int64_t* timestamps,
+                                const int64_t* ms, long long k, float* values, uint8_t* found, void* stream);
 
 /* ---- resource updates of a live store (csrc/resources.cu) -----------------------------------------------------------
  * Append k resource rows to a store's sorted resource table and its as-of index, and drop every row whose timestamp is

@@ -67,6 +67,9 @@ SIGNATURES = {
     "pert_store_assemble": (I, [P, P, LL, LL, LL, P, P, P, P]),
     # request assembly (second argument: const PertResourceAsOf* or NULL for the exact join)
     "pert_store_assemble_requests": (I, [P, P, P, P, LL, LL, LL, P, P, P, P]),
+    # what-if request assembly (third argument: const PertWhatIf*) and the joined resource rows of (timestamp, ms)
+    "pert_store_assemble_whatif": (I, [P, P, P, P, P, LL, LL, LL, P, P, P, P]),
+    "pert_store_lookup_resources": (I, [P, P, P, P, LL, P, P, P]),
     # resource updates of a live store (csrc/resources.cu; first two arguments: PertStore*, PertResourceAsOf*)
     "pert_store_resources_count": (I, [P, P, P, P, LL, LL, P, P, P, P]),
     "pert_store_resources_merge": (I, [P, P, P, P, P, P, LL, P, P, LL, LL, LL, P, P, P, P, P, P]),
@@ -118,6 +121,14 @@ class PertResourceAsOf(C.Structure):
     """The as-of index of a store's resource rows (include/pertgnn.h): device pointers ms_ptr [n_ms+1] int32,
     ts [n_res] int64, row [n_res] int32."""
     _fields_ = [("ms_ptr", P), ("ts", P), ("row", P)]
+
+
+class PertWhatIf(C.Structure):
+    """Per-request mixes and resource overrides of what-if assembly (include/pertgnn.h): device pointers mix_ptr [B+1]
+    int64 (absolute offsets) into mix_pat int32 / mix_prob float32, scenario [B] int64, and n_ov override rows,
+    ov_keys [n_ov] int64 sorted and ov_vals [n_ov, 8] float32 (16-byte aligned); NULL mix_ptr / scenario: none."""
+    _fields_ = [("mix_ptr", P), ("mix_pat", P), ("mix_prob", P), ("scenario", P), ("n_ov", LL), ("ov_keys", P),
+                ("ov_vals", P)]
 
 
 def lib():

@@ -39,10 +39,28 @@ __device__ __forceinline__ int upper_seg(const int* __restrict__ off, int n, int
   return lo;
 }
 
-// Where graph b of a batch takes its entry, time bucket and label from: a row of the store's trace table
-// (pert_store_assemble) or a request (pert_store_assemble_requests).  entry() flags a bad id in `bad` and falls back to
-// trace 0 / entry 0; the other reads repeat the fallback, so every kernel sees the same graph.
-struct TraceRows {
+// Where graph b of a batch takes its entry, time bucket, label and pattern mix from: a row of the store's trace table
+// (pert_store_assemble), a request (pert_store_assemble_requests) or a what-if request (pert_store_assemble_whatif).
+// entry() flags a bad id in `bad` and falls back to trace 0 / entry 0; the other reads repeat the fallback, so every
+// kernel sees the same graph.  The mix of graph b is the slot range slots() returns, pattern pat(k) with probability
+// prob(k) in slot k; sizes() gives the graph's node, edge and slot counts.
+struct OwnMix {                       // the entry's stored mix: ent_ptr / ent_pat / ent_prob
+  using Slot = int;
+  static constexpr bool kWhatIf = false;
+  __device__ __forceinline__ void slots(const PertStore& s, int, int ent, Slot& k0, Slot& k1) const {
+    k0 = s.ent_ptr[ent];
+    k1 = s.ent_ptr[ent + 1];
+  }
+  __device__ __forceinline__ int pat(const PertStore& s, Slot k) const { return s.ent_pat[k]; }
+  __device__ __forceinline__ float prob(const PertStore& s, Slot k) const { return s.ent_prob[k]; }
+  __device__ __forceinline__ void sizes(const PertStore& s, int, int ent, int v[3], bool&) const {
+    v[0] = s.ent_nodes[ent];
+    v[1] = s.ent_edges[ent];
+    v[2] = s.ent_ptr[ent + 1] - s.ent_ptr[ent];
+  }
+};
+
+struct TraceRows : OwnMix {
   const int64_t* __restrict__ ids;
   static constexpr bool kLabel = true;
   __device__ __forceinline__ int64_t row(const PertStore& s, int b, bool& bad) const {
@@ -63,7 +81,7 @@ struct TraceRows {
   }
 };
 
-struct Requests {
+struct Requests : OwnMix {
   const int64_t* __restrict__ entry_ids;
   const int64_t* __restrict__ timestamps;
   static constexpr bool kLabel = false;
@@ -73,6 +91,80 @@ struct Requests {
     return bad ? 0 : (int)e;
   }
   __device__ __forceinline__ int64_t bucket(const PertStore&, int b) const { return pert_time_bucket(timestamps[b]); }
+};
+
+// A request with its own pattern mix (w.mix_ptr != NULL: slots mix_ptr[b] .. mix_ptr[b+1]-1 of mix_pat / mix_prob,
+// absolute offsets) and / or a resource scenario (w.scenario[b] >= 0: the override rows (scenario, ms)).  A pattern
+// index outside [0, n_pat) reads pattern 0 and an empty or inverted mix gives an empty graph; sizes() flags both.
+struct WhatIfRequests {
+  const int64_t* __restrict__ entry_ids;
+  const int64_t* __restrict__ timestamps;
+  PertWhatIf w;
+  using Slot = int64_t;
+  static constexpr bool kLabel = false;
+  static constexpr bool kWhatIf = true;
+  __device__ __forceinline__ int entry(const PertStore& s, int b, bool& bad) const {
+    const int64_t e = entry_ids[b];
+    bad = e < 0 || e >= s.n_ent || (!w.mix_ptr && s.ent_ptr[e + 1] == s.ent_ptr[e]);   // own mix: not read if given
+    return bad ? 0 : (int)e;
+  }
+  __device__ __forceinline__ int64_t bucket(const PertStore&, int b) const { return pert_time_bucket(timestamps[b]); }
+  __device__ __forceinline__ void slots(const PertStore& s, int b, int ent, Slot& k0, Slot& k1) const {
+    if (w.mix_ptr) {
+      k0 = w.mix_ptr[b];
+      k1 = max(k0, w.mix_ptr[b + 1]);
+    } else {
+      k0 = s.ent_ptr[ent];
+      k1 = s.ent_ptr[ent + 1];
+    }
+  }
+  __device__ __forceinline__ int pat(const PertStore& s, Slot k) const {
+    if (!w.mix_ptr) return s.ent_pat[k];
+    const int p = w.mix_pat[k];
+    return (p < 0 || p >= s.n_pat) ? 0 : p;
+  }
+  __device__ __forceinline__ float prob(const PertStore& s, Slot k) const {
+    return w.mix_ptr ? w.mix_prob[k] : s.ent_prob[k];
+  }
+  __device__ __forceinline__ void sizes(const PertStore& s, int b, int ent, int v[3], bool& bad) const {
+    if (!w.mix_ptr) {
+      v[0] = s.ent_nodes[ent];
+      v[1] = s.ent_edges[ent];
+      v[2] = s.ent_ptr[ent + 1] - s.ent_ptr[ent];
+      return;
+    }
+    const int64_t k0 = w.mix_ptr[b], k1 = w.mix_ptr[b + 1];
+    if (k1 <= k0) bad = true;
+    v[0] = v[1] = v[2] = 0;
+    for (int64_t k = k0; k < k1; ++k) {
+      const int q = w.mix_pat[k];
+      if (q < 0 || q >= s.n_pat) bad = true;
+      const int p = (q < 0 || q >= s.n_pat) ? 0 : q;
+      v[0] += s.pat_nptr[p + 1] - s.pat_nptr[p];
+      v[1] += s.pat_eptr[p + 1] - s.pat_eptr[p];
+      v[2] += 1;
+    }
+  }
+  // the first override row of key (scenario[b], ms) -- ov_keys sorted ascending, nonnegative -- into f; false if none.
+  // A scenario above the largest one in the table has no rows (and its key could overflow int64: compared unsigned).
+  __device__ __forceinline__ bool override_row(const PertStore& s, int b, int64_t ms, float* f) const {
+    if (!w.scenario || w.n_ov == 0) return false;
+    const int64_t sc = w.scenario[b];
+    if (sc < 0 || sc > w.ov_keys[w.n_ov - 1] / s.n_ms) return false;
+    const uint64_t key = (uint64_t)sc * (uint64_t)s.n_ms + (uint64_t)ms;
+    long long lo = 0, hi = w.n_ov;
+    while (lo < hi) {
+      const long long mid = (lo + hi) >> 1;
+      if ((uint64_t)w.ov_keys[mid] < key) lo = mid + 1;
+      else hi = mid;
+    }
+    if (lo == w.n_ov || (uint64_t)w.ov_keys[lo] != key) return false;
+    const float4* v = reinterpret_cast<const float4*>(w.ov_vals + (size_t)lo * NF);
+    const float4 a = v[0], c = v[1];
+    f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w;
+    f[4] = c.x; f[5] = c.y; f[6] = c.z; f[7] = c.w;
+    return true;
+  }
 };
 
 // exclusive prefix sums of the per-graph node / edge / pattern counts (one CTA; B is a batch size)
@@ -91,10 +183,8 @@ __global__ void __launch_bounds__(1024) k_store_offsets(PertStore s, Src src, in
     if (b < B) {
       bool bad;
       const int ent = src.entry(s, b, bad);
+      src.sizes(s, b, ent, v, bad);
       if (bad && status) atomicExch(status, PERT_ERR_RANGE);
-      v[0] = s.ent_nodes[ent];
-      v[1] = s.ent_edges[ent];
-      v[2] = s.ent_ptr[ent + 1] - s.ent_ptr[ent];
     }
     int incl[3];
 #pragma unroll
@@ -136,14 +226,17 @@ __global__ void __launch_bounds__(1024) k_store_offsets(PertStore s, Src src, in
   if (B == 0 && threadIdx.x == 0) node_off[0] = edge_off[0] = pat_off[0] = 0;
 }
 
-// pattern instance of local node / edge index l inside entry `ent`: returns slot k (into ent_pat / ent_prob) and the
-// offsets of that pattern inside the graph
-__device__ __forceinline__ int find_pattern(const PertStore& s, int ent, int l, bool edges, int& node_base,
-                                            int& local) {
+// pattern instance of local node / edge index l inside graph b (entry `ent`): returns the mix slot k and the offsets
+// of that pattern inside the graph
+template <class Src>
+__device__ __forceinline__ typename Src::Slot find_pattern(const PertStore& s, const Src& src, int b, int ent, int l,
+                                                           bool edges, int& node_base, int& local) {
+  using Slot = typename Src::Slot;
   int nb = 0, acc = 0;
-  const int k0 = s.ent_ptr[ent], k1 = s.ent_ptr[ent + 1];
-  for (int k = k0; k < k1; ++k) {
-    const int p = s.ent_pat[k];
+  Slot k0, k1;
+  src.slots(s, b, ent, k0, k1);
+  for (Slot k = k0; k < k1; ++k) {
+    const int p = src.pat(s, k);
     const int nn = s.pat_nptr[p + 1] - s.pat_nptr[p];
     const int sz = edges ? s.pat_eptr[p + 1] - s.pat_eptr[p] : nn;
     if (l < acc + sz || k == k1 - 1) {
@@ -204,21 +297,28 @@ __global__ void __launch_bounds__(256) k_store_nodes(PertStore s, Src src, PertR
   bool bad;
   const int ent = src.entry(s, b, bad);
   int node_base, local;
-  const int k = find_pattern(s, ent, n - node_off[b], false, node_base, local);
-  const int p = s.ent_pat[k];
+  const auto k = find_pattern(s, src, b, ent, n - node_off[b], false, node_base, local);
+  const int p = src.pat(s, k);
   const int g = s.pat_nptr[p] + local;
   const int64_t ms = s.pat_ms[g];
   o.cat_X[n] = ms;
   o.node_depth[n] = s.pat_depth[g];
   o.pattern_num_nodes[n] = (float)(s.pat_nptr[p + 1] - s.pat_nptr[p]);
-  o.rt_probs[n] = s.ent_prob[k];
+  o.rt_probs[n] = src.prob(s, k);
   o.batch[n] = b;
   // ---- feature join (get_x): statistics of (timestamp, ms) for the LAST node of a resourced ms, else missing indicator
   float f[NF + 1];
 #pragma unroll
   for (int c = 0; c < NF; ++c) f[c] = 0.f;
   f[NF] = 1.f;
-  if (s.pat_last[g] && ms >= 0 && ms < s.n_ms && s.ms_has_res[ms]) {
+  bool overridden = false;                       // what-if: an override row of (scenario, ms) replaces the store's join
+  if constexpr (Src::kWhatIf) {
+    if (s.pat_last[g] && ms >= 0 && ms < s.n_ms && src.override_row(s, b, ms, f)) {
+      f[NF] = 0.f;
+      overridden = true;
+    }
+  }
+  if (!overridden && s.pat_last[g] && ms >= 0 && ms < s.n_ms && s.ms_has_res[ms]) {
     const int64_t bucket = src.bucket(s, b);
     const int r = asof.ms_ptr ? asof_row(asof, bucket, ms) : exact_row(s, bucket, ms);
     if (r >= 0) {
@@ -243,8 +343,8 @@ __global__ void __launch_bounds__(256) k_store_edges(PertStore s, Src src, int B
   bool bad;
   const int ent = src.entry(s, b, bad);
   int node_base, local;
-  const int k = find_pattern(s, ent, e - edge_off[b], true, node_base, local);
-  const int p = s.ent_pat[k];
+  const auto k = find_pattern(s, src, b, ent, e - edge_off[b], true, node_base, local);
+  const int p = src.pat(s, k);
   const size_t ge = (size_t)s.pat_eptr[p] + local;
   const int64_t off = (int64_t)node_off[b] + node_base;
   o.edge_index[e] = s.pat_src[ge] + off;
@@ -264,8 +364,26 @@ __global__ void __launch_bounds__(256) k_store_traces(PertStore s, Src src, int 
   const int ent = src.entry(s, b, bad);
   o.entry_id[b] = ent;
   if constexpr (Src::kLabel) o.y[b] = src.label(s, b);
-  const int k0 = s.ent_ptr[ent], k1 = s.ent_ptr[ent + 1];
-  for (int k = k0; k < k1; ++k) o.pattern_probs[pat_off[b] + (k - k0)] = s.ent_prob[k];
+  typename Src::Slot k0, k1;
+  src.slots(s, b, ent, k0, k1);
+  for (auto k = k0; k < k1; ++k) o.pattern_probs[pat_off[b] + (k - k0)] = src.prob(s, k);
+}
+
+// one thread per (timestamp, ms) query: the row the exact or the as-of join of assembly reads (pert_store_lookup_resources)
+__global__ void __launch_bounds__(256) k_store_lookup(PertStore s, PertResourceAsOf asof, const int64_t* __restrict__ ts,
+                                                      const int64_t* __restrict__ ms, int k, float* __restrict__ values,
+                                                      uint8_t* __restrict__ found) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= k) return;
+  const int64_t m = ms[i];
+  int r = -1;
+  if (m >= 0 && m < s.n_ms) {
+    const int64_t bucket = pert_time_bucket(ts[i]);
+    r = asof.ms_ptr ? asof_row(asof, bucket, m) : exact_row(s, bucket, m);
+  }
+#pragma unroll
+  for (int c = 0; c < NF; ++c) values[(size_t)i * NF + c] = r >= 0 ? s.res_vals[(size_t)r * NF + c] : 0.f;
+  found[i] = r >= 0;
 }
 
 bool entries_ok(const PertStore* s) { return s->ent_ptr && s->ent_pat && s->ent_prob && s->pat_nptr && s->pat_eptr; }
@@ -294,7 +412,7 @@ int pert_store_assemble(const PertStore* s, const int64_t* trace_ids, long long 
   if (!s || !out || B < 0 || N < 0 || E < 0 || (B > 0 && (!trace_ids || !offsets))) return PERT_ERR_BADARG;
   if (!entries_ok(s) || !s->trace_entry) return PERT_ERR_BADARG;
   if (B == 0) return PERT_OK;
-  return assemble(*s, TraceRows{trace_ids}, PertResourceAsOf{}, B, N, E, offsets, *out, status, stream);
+  return assemble(*s, TraceRows{{}, trace_ids}, PertResourceAsOf{}, B, N, E, offsets, *out, status, stream);
 }
 
 int pert_store_assemble_requests(const PertStore* s, const PertResourceAsOf* asof, const int64_t* entry_ids,
@@ -305,8 +423,37 @@ int pert_store_assemble_requests(const PertStore* s, const PertResourceAsOf* aso
   if (!entries_ok(s) || (asof && (!asof->ms_ptr || (s->n_res > 0 && (!asof->ts || !asof->row)))))
     return PERT_ERR_BADARG;
   if (B == 0) return PERT_OK;
-  return assemble(*s, Requests{entry_ids, timestamps}, asof ? *asof : PertResourceAsOf{}, B, N, E, offsets, *out,
+  return assemble(*s, Requests{{}, entry_ids, timestamps}, asof ? *asof : PertResourceAsOf{}, B, N, E, offsets, *out,
                   status, stream);
+}
+
+int pert_store_assemble_whatif(const PertStore* s, const PertResourceAsOf* asof, const PertWhatIf* w,
+                               const int64_t* entry_ids, const int64_t* timestamps, long long B, long long N,
+                               long long E, int* offsets, const PertBatchOut* out, int* status, void* stream) {
+  if (!s || !out || !w || B < 0 || N < 0 || E < 0 || (B > 0 && (!entry_ids || !timestamps || !offsets)))
+    return PERT_ERR_BADARG;
+  if (!entries_ok(s) || (asof && (!asof->ms_ptr || (s->n_res > 0 && (!asof->ts || !asof->row)))))
+    return PERT_ERR_BADARG;
+  if (w->mix_ptr && (!w->mix_pat || !w->mix_prob)) return PERT_ERR_BADARG;
+  if (w->n_ov < 0 || (w->n_ov > 0 && (!w->ov_keys || !w->ov_vals || s->n_ms < 1 ||
+                                      reinterpret_cast<uintptr_t>(w->ov_vals) % 16)))
+    return PERT_ERR_BADARG;
+  if (B == 0) return PERT_OK;
+  WhatIfRequests src{entry_ids, timestamps, *w};
+  return assemble(*s, src, asof ? *asof : PertResourceAsOf{}, B, N, E, offsets, *out, status, stream);
+}
+
+int pert_store_lookup_resources(const PertStore* s, const PertResourceAsOf* asof, const int64_t* timestamps,
+                                const int64_t* ms, long long k, float* values, uint8_t* found, void* stream) {
+  if (!s || k < 0 || k > INT32_MAX || (k > 0 && (!timestamps || !ms || !values || !found))) return PERT_ERR_BADARG;
+  if (s->n_ms < 1 || (s->n_res > 0 && (!s->res_keys || !s->res_vals)) ||
+      (asof && (!asof->ms_ptr || (s->n_res > 0 && (!asof->ts || !asof->row)))))
+    return PERT_ERR_BADARG;
+  if (k == 0) return PERT_OK;
+  k_store_lookup<<<pert_cdiv(k, 256), 256, 0, (cudaStream_t)stream>>>(*s, asof ? *asof : PertResourceAsOf{}, timestamps,
+                                                                     ms, (int)k, values, found);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
 }
 
 }  // extern "C"

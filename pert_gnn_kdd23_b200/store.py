@@ -159,6 +159,156 @@ def _check_resource_rows(ts, ms, n_ms):
                                 f"ms (n_ms = {n_ms})")
 
 
+def _int_column(a, what):
+    """1-d int64 host copy of an integer array, list or tensor; ``PertGnnError`` for anything else (floats and bools
+    are refused, not truncated)."""
+    a = a.cpu().numpy() if torch.is_tensor(a) else a
+    try:
+        a = np.asarray(a)
+    except (TypeError, ValueError) as e:
+        raise _lib.PertGnnError(f"{what}: integers expected ({e})") from None
+    if a.size == 0:
+        return np.zeros(0, dtype=np.int64)
+    if a.ndim != 1 or a.dtype.kind not in "iu" or (a.dtype.kind == "u" and (a > _I64_MAX).any()):
+        raise _lib.PertGnnError(f"{what}: a 1-d array of int64 integers expected, got {a.dtype} of shape {a.shape}")
+    return a.astype(np.int64)
+
+
+def _resolve_mixes(mixes, Q, rt_ids, pat_nodes, pat_edges):
+    """Checks the what-if mixes of Q requests and resolves their runtime ids to pattern indices (a dense table for
+    compact ids, else a sorted copy of ``rt_ids`` and ``np.searchsorted``): -> (ptr int64 [Q+1], pat int32, prob
+    float32 -- float64 rounded as the
+    constructor rounds it --, and the requests' node, edge and pattern counts, int64 [Q]).  ``PertGnnError`` naming the
+    first bad request."""
+    try:
+        mix_ptr, mix_rt, mix_prob = mixes
+    except (TypeError, ValueError):
+        raise _lib.PertGnnError("mixes: a (mix_ptr, mix_rt, mix_prob) triple expected") from None
+    ptr, rt = _int_column(mix_ptr, "mix_ptr"), _int_column(mix_rt, "mix_rt")
+    try:
+        prob = np.asarray(mix_prob.cpu().numpy() if torch.is_tensor(mix_prob) else mix_prob, dtype=np.float64)
+    except (TypeError, ValueError) as e:
+        raise _lib.PertGnnError(f"mix_prob: numbers expected ({e})") from None
+    prob = prob.reshape(-1) if prob.size == 0 else prob
+    if prob.ndim != 1 or prob.shape[0] != rt.shape[0]:
+        raise _lib.PertGnnError(f"mix_prob: shape {prob.shape}, expected ({rt.shape[0]},): one per runtime of mix_rt")
+    if ptr.shape[0] != Q + 1:
+        raise _lib.PertGnnError(f"mix_ptr: {ptr.shape[0]} offsets, expected {Q + 1} for {Q} requests")
+    if ptr[0] != 0:
+        raise _lib.PertGnnError(f"mix_ptr[0] = {int(ptr[0])}, expected 0")
+    n = np.diff(ptr)
+    if (n < 0).any():
+        i = int(np.argmax(n < 0))
+        raise _lib.PertGnnError(f"request {i}: mix_ptr is not monotone ({int(ptr[i])} > {int(ptr[i + 1])})")
+    if ptr[-1] != rt.shape[0]:
+        raise _lib.PertGnnError(f"mix_ptr[{Q}] = {int(ptr[-1])}, but mix_rt holds {rt.shape[0]} runtimes")
+    if (n == 0).any():
+        raise _lib.PertGnnError(f"request {int(np.argmax(n == 0))}: empty mix")
+    # per slot, in request order: unknown runtime, a runtime repeated within its mix, a bad probability
+    ids = np.asarray(rt_ids, dtype=np.int64)
+    if ids.shape[0] and int(ids.max()) - int(ids.min()) < 4 * ids.shape[0] + (1 << 16):
+        # compact ids (the stores' runtime numbering): a dense table, one gather per slot instead of a binary search
+        lo, hi = int(ids.min()), int(ids.max())
+        lut = np.full(hi - lo + 1, -1, dtype=np.int64)
+        lut[ids - lo] = np.arange(ids.shape[0])
+        inside = (rt >= lo) & (rt <= hi)
+        pidx = np.where(inside, lut[np.where(inside, rt - lo, 0)], -1)
+        known = pidx >= 0
+        pidx = np.maximum(pidx, 0)
+    else:
+        order = np.argsort(ids, kind="stable")
+        pos = np.minimum(np.searchsorted(ids[order], rt), max(ids.shape[0] - 1, 0))
+        known = ids[order][pos] == rt if ids.shape[0] else np.zeros(rt.shape[0], dtype=bool)
+        pidx = order[pos] if ids.shape[0] else np.zeros(rt.shape[0], dtype=np.int64)
+    owner = np.repeat(np.arange(Q, dtype=np.int64), n)
+    again = np.zeros(rt.shape[0], dtype=bool)
+    n_ids = max(ids.shape[0], 1)
+    if Q * n_ids < (1 << 62):                                   # one int64 sort finds whether any mix repeats a runtime
+        key = np.where(known, owner * n_ids + pidx, -1 - np.arange(rt.shape[0]))
+        srt = np.sort(key)
+        maybe = bool((srt[1:] == srt[:-1]).any())
+    else:
+        maybe = True
+    if maybe:                                                   # which slot: (request, runtime, slot) order
+        by = np.lexsort((np.arange(rt.shape[0]), rt, owner))
+        again[by[1:]] = (owner[by[1:]] == owner[by[:-1]]) & (rt[by[1:]] == rt[by[:-1]])
+    bad_p = ~np.isfinite(prob) | (prob < 0)
+    bad = ~known | again | bad_p
+    if bad.any():
+        k = int(np.argmax(bad))
+        q = int(owner[k])
+        if not known[k]:
+            raise _lib.PertGnnError(f"request {q}: runtime {int(rt[k])} is not in the store (never seen, or evicted)")
+        if again[k]:
+            raise _lib.PertGnnError(f"request {q}: runtime {int(rt[k])} occurs twice in its mix")
+        raise _lib.PertGnnError(f"request {q}: probability {float(prob[k])} of runtime {int(rt[k])} is negative, NaN "
+                                "or infinite")
+    pat = pidx.astype(np.int64)
+    sizes = []
+    for per_pat in (pat_nodes, pat_edges):
+        cs = np.zeros(rt.shape[0] + 1, dtype=np.int64)
+        np.cumsum(per_pat[pat], out=cs[1:])
+        sizes.append(cs[ptr[1:]] - cs[ptr[:-1]])
+    return ptr, pat.astype(np.int32), prob.astype(np.float32), sizes[0], sizes[1], n
+
+
+def _override_rows(overrides, n_ms):
+    """Checks an override table ``(scenario [k], ms [k], values [k, 8])``: -> (keys scenario * n_ms + ms int64 [k],
+    values float32 [k, 8], in input order).  ``PertGnnError`` naming the first bad row."""
+    try:
+        sc, ms, vals = overrides
+    except (TypeError, ValueError):
+        raise _lib.PertGnnError("overrides: a (scenario, ms, values) triple expected") from None
+    sc, ms = _int_column(sc, "overrides scenario"), _int_column(ms, "overrides ms")
+    k = sc.shape[0]
+    if ms.shape[0] != k:
+        raise _lib.PertGnnError(f"overrides: {k} scenario ids but {ms.shape[0]} microservices")
+    try:
+        vals = np.asarray(vals.cpu().numpy() if torch.is_tensor(vals) else vals, dtype=np.float64)
+    except (TypeError, ValueError) as e:
+        raise _lib.PertGnnError(f"overrides values: [k, 8] numbers expected ({e})") from None
+    if vals.size == 0 and k == 0:
+        vals = vals.reshape(0, 8)
+    if vals.shape != (k, 8):
+        raise _lib.PertGnnError(f"overrides values: shape {vals.shape}, expected ({k}, 8) for {k} rows")
+    bad_m = (ms < 0) | (ms >= n_ms)
+    bad_s = sc < 0
+    over = ~bad_m & ~bad_s & (sc > (_I64_MAX - np.where(bad_m, 0, ms)) // n_ms)
+    bad = bad_m | bad_s | over
+    if bad.any():
+        i = int(np.argmax(bad))
+        if bad_m[i]:
+            raise _lib.PertGnnError(f"override row {i}: microservice {int(ms[i])} is outside [0, {n_ms})")
+        if bad_s[i]:
+            raise _lib.PertGnnError(f"override row {i}: scenario {int(sc[i])} is negative")
+        raise _lib.PertGnnError(f"override row {i}: scenario {int(sc[i])} overflows the int64 key scenario * n_ms + "
+                                f"ms (n_ms = {n_ms})")
+    return sc * n_ms + ms, vals.astype(np.float32)
+
+
+class _WhatIfArrays:
+    """The checked inputs of one what-if call on the device (``PatternStore._what_if_arrays``), or a slice of them:
+    host entry ids and the requests' node / edge / pattern counts (sizing), device entry ids, timestamps, the mixes'
+    CSR (mix_ptr absolute into mix_pat / mix_prob; None: the entries' own mixes), the scenario ids (None: none) and
+    the sorted override table.  Pattern indices are resolved for the store as it is: valid until it changes."""
+
+    def __init__(self, ent, nodes, edges, pats, ent_d, ts_d, ptr_d, pat_d, prob_d, scen_d, ov_keys, ov_vals):
+        self.ent, self.nodes, self.edges, self.pats = ent, nodes, edges, pats
+        self.ent_d, self.ts_d, self.ptr_d, self.pat_d, self.prob_d = ent_d, ts_d, ptr_d, pat_d, prob_d
+        self.scen_d, self.ov_keys, self.ov_vals = scen_d, ov_keys, ov_vals
+
+    def slice(self, i, j):
+        return _WhatIfArrays(self.ent[i:j], self.nodes[i:j], self.edges[i:j], self.pats[i:j], self.ent_d[i:j],
+                             self.ts_d[i:j], None if self.ptr_d is None else self.ptr_d[i:j + 1], self.pat_d,
+                             self.prob_d, None if self.scen_d is None else self.scen_d[i:j], self.ov_keys,
+                             self.ov_vals)
+
+    def desc(self):
+        p = lambda t: None if t is None else t.data_ptr()            # noqa: E731
+        return _lib.PertWhatIf(p(self.ptr_d), p(self.pat_d), p(self.prob_d), p(self.scen_d),
+                               int(self.ov_keys.shape[0]), p(self.ov_keys), p(self.ov_vals))
+
+
 class _BulkPatterns:
     """Concatenated host arrays of many patterns (PatternStore.from_graphs)."""
 
@@ -321,6 +471,7 @@ class PatternStore:
         self._h_ent_nodes, self._h_ent_edges = ent_nodes.astype(np.int64), ent_edges.astype(np.int64)
         self._h_ent_pats = np.diff(np.array(ent_ptr)).astype(np.int64)
         self._h_trace_entry = t_ent.astype(np.int64)
+        self._h_pat_nodes, self._h_pat_edges = pat_nodes.astype(np.int64), pat_edges.astype(np.int64)
 
         def up(a, dtype):
             return torch.from_numpy(np.ascontiguousarray(a, dtype=dtype)).to(dev)
@@ -420,6 +571,8 @@ class PatternStore:
         self._h_trace_entry, self.trace_keys = host[:T], host[T:2 * T].tolist()
         self._h_ent_nodes, self._h_ent_edges, self._h_ent_pats = (host[2 * T + k * n_ent:2 * T + (k + 1) * n_ent]
                                                                  for k in range(3))
+        self._h_pat_nodes, self._h_pat_edges = (np.diff(np.asarray(p, dtype=np.int64))
+                                                for p in (graphs.node_ptr, graphs.edge_ptr))
         res_ms = np.array([m for _, m in resource_index], dtype=np.int64)
         res_ts = np.array([t for t, _ in resource_index], dtype=np.int64)
         self.n_ms = int(n_ms if n_ms is not None else max(int(host[-1]), int(res_ms.max(initial=0))) + 1)
@@ -739,6 +892,8 @@ class PatternStore:
         self._h_trace_entry = np.concatenate([self._h_trace_entry, h_ent])
         self._h_ent_nodes, self._h_ent_edges = sizes[n_ent + 1:2 * n_ent + 1], sizes[2 * n_ent + 1:]
         self._h_ent_pats = np.diff(ent_ptr_h)
+        self._h_pat_nodes = np.concatenate([self._h_pat_nodes, np.diff(g_nptr)])
+        self._h_pat_edges = np.concatenate([self._h_pat_edges, np.diff(g_eptr)])
         key_rows_old = int(ing.rows.shape[1])
         ing.rows = torch.cat([ing.rows, new_rows[:3]], dim=1)
         ing.ptr = torch.cat([ing.ptr, torch.from_numpy(new_ptr[1:] + key_rows_old).to(dev, i32)])
@@ -834,6 +989,7 @@ class PatternStore:
         self.trace_keys = list(itertools.compress(self.trace_keys, (remap >= 0).view(np.uint8).tobytes()))
         self._h_trace_entry, self._h_ent_nodes, self._h_ent_edges = h_ent, h_nodes, h_edges
         self._h_ent_pats = np.diff(ent_ptr_h)
+        self._h_pat_nodes, self._h_pat_edges = self._h_pat_nodes[pat_new >= 0], self._h_pat_edges[pat_new >= 0]
         ing.rows, ing.ptr, ing.cnt, ing.tot, ing.tids = o["key_rows"], o["key_ptr"], mix["cnt"], mix["tot"], tids
         ing.trace_pat, ing.trace_tid, ing.n_nodes, ing.n_edges = o["trace_pat"], o["trace_tid"], N2, E2
         ing.table = None                                 # it holds pattern indices: the next append rebuilds it
@@ -915,13 +1071,45 @@ class PatternStore:
         return ent
 
     @_lib.on_device_of
-    def assemble_requests(self, entry_ids, timestamps, asof=False, device_arrays=None):
+    def assemble_requests(self, entry_ids, timestamps, asof=False, device_arrays=None, mixes=None, overrides=None,
+                          scenario_ids=None):
         """-> device ``Batch`` of the requests (entry ``entry_ids[b]`` at time ``timestamps[b]``, in ms): every field of
         ``assemble`` but ``y``.  The resources are those of the time bucket floor(t / 30000) * 30000, joined exactly
         (a missing row of a resourced microservice sets the status word, see ``check``) or, with ``asof``, from the
         newest row at or before the bucket (none: the missing indicator, no error).  The entry ids are checked and the
         outputs sized on the host (``PertGnnError`` before any launch); ``device_arrays``: the same two columns already
-        on the device (int64), e.g. slices of a request list uploaded once -- ``timestamps`` may then be None."""
+        on the device (int64), e.g. slices of a request list uploaded once -- ``timestamps`` may then be None.
+
+        What-if requests (``mixes``, ``overrides``, ``scenario_ids``; with all three None the call above):
+
+        - ``mixes = (mix_ptr [Q+1], mix_rt, mix_prob)``: request q's own pattern mix, runtime ids ``mix_rt[k]`` (the
+          store's numbering, ``rt_ids``) with probabilities ``mix_prob[k]`` (float64 or float32, rounded to float32 as
+          the constructor rounds them) for k = mix_ptr[q] .. mix_ptr[q+1]-1.  The graph is the concatenation of those
+          patterns in mix order, with these probabilities as ``pattern_probs`` / ``rt_probs``, in place of the entry's
+          stored mix; the entry id still selects the entry embedding and is written to ``entry_id``.  Probabilities
+          need not sum to 1 (the model is defined for any weights, so a mix may be scaled).  Runtime ids are resolved on
+          every call, so a mix stays valid across ``append_traces`` and ``evict_traces`` unless one of its runtimes was
+          evicted.
+        - ``overrides = (scenario [k], ms [k], values [k, 8])`` and ``scenario_ids [Q]`` (-1: none): at the node that
+          receives statistics for microservice m (its last node in the pattern), a request with scenario s reads the
+          override row (s, m) if there is one -- its values, indicator 0, no store join, even for an m without resource
+          rows -- and the store's exact or as-of join otherwise.  Among several rows of one (s, m) the first given
+          wins.  A scenario without rows means no override.
+
+        Checked on the host before any launch (``PertGnnError`` naming the first bad request, row or runtime): a
+        malformed ``mix_ptr`` (length, ``mix_ptr[0] != 0``, not monotone, last offset != ``len(mix_rt)``), an empty
+        mix, a runtime the store does not hold or repeated within a mix, a negative, NaN or infinite probability, an
+        entry outside [0, n_ent) (with ``mixes`` an entry whose own mix is empty is fine: it is not read; without, as
+        above), override rows with ms outside [0, n_ms), a negative scenario or an int64-overflowing key, override
+        values that are not [k, 8] numbers, scenario ids below -1, and node, edge or pattern totals above 2^31 - 1.
+        The override table is sorted stably on the device once per call."""
+        if isinstance(device_arrays, _WhatIfArrays):
+            return self._assemble_what_if(device_arrays, asof)
+        if mixes is not None or overrides is not None or scenario_ids is not None:
+            if device_arrays is not None:
+                raise _lib.PertGnnError("device_arrays: a what-if call takes its inputs on the host")
+            return self._assemble_what_if(self._what_if_arrays(entry_ids, timestamps, mixes, overrides, scenario_ids),
+                                          asof)
         ent = self.check_entries(entry_ids)
         B = int(ent.shape[0])
         N, E, Pn = (int(self._h_ent_nodes[ent].sum()), int(self._h_ent_edges[ent].sum()),
@@ -944,6 +1132,92 @@ class PatternStore:
             _lib.check(rc, "pert_store_assemble_requests")
 
         return self._outputs(B, N, E, Pn, launch, (ent_d, ts_d), label=False)
+
+    @_lib.on_device_of
+    def _what_if_arrays(self, entry_ids, timestamps, mixes=None, overrides=None, scenario_ids=None):
+        """Checks a what-if call's inputs (``assemble_requests``) and uploads them once: -> ``_WhatIfArrays``."""
+        ent = _int_column(entry_ids, "entry_ids")
+        Q = int(ent.shape[0])
+        ts = _int_column(timestamps, "timestamps")
+        if ts.shape[0] != Q:
+            raise _lib.PertGnnError(f"{Q} entry ids but {ts.shape[0]} timestamps")
+        mix = None
+        if mixes is None:
+            self.check_entries(ent)
+            nodes, edges, pats = self._h_ent_nodes[ent], self._h_ent_edges[ent], self._h_ent_pats[ent]
+        else:
+            n_ent = int(self._h_ent_nodes.shape[0])
+            out = (ent < 0) | (ent >= n_ent)
+            if out.any():
+                i = int(np.argmax(out))
+                raise _lib.PertGnnError(f"request {i}: entry {int(ent[i])} is outside [0, {n_ent})")
+            *mix, nodes, edges, pats = _resolve_mixes(mixes, Q, self.rt_ids, self._h_pat_nodes, self._h_pat_edges)
+        sc = None
+        if scenario_ids is not None:
+            sc = _int_column(scenario_ids, "scenario_ids")
+            if sc.shape[0] != Q:
+                raise _lib.PertGnnError(f"{Q} requests but {sc.shape[0]} scenario ids")
+            if (sc < -1).any():
+                i = int(np.argmax(sc < -1))
+                raise _lib.PertGnnError(f"request {i}: scenario id {int(sc[i])} is below -1 (-1: no scenario)")
+        keys, vals = _override_rows(overrides if overrides is not None else ((), (), ()), self.n_ms)
+        # ---- every check passed: one upload of each array
+        dev = self.device
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev, non_blocking=True)    # noqa: E731
+        ptr_d, pat_d, prob_d = (None,) * 3 if mix is None else (up(a) for a in mix)
+        scen_d = None if sc is None else up(sc)
+        if keys.shape[0]:
+            ov_keys, perm = torch.sort(up(keys), stable=True)    # the first of equal keys stays first
+            ov_vals = up(vals)[perm].contiguous()                # a fresh allocation: 16-byte aligned
+        else:
+            ov_keys = torch.zeros(0, dtype=torch.int64, device=dev)
+            ov_vals = torch.zeros(0, 8, dtype=torch.float32, device=dev)
+        return _WhatIfArrays(ent, nodes, edges, pats, up(ent), up(ts), ptr_d, pat_d, prob_d, scen_d, ov_keys, ov_vals)
+
+    def _assemble_what_if(self, w, asof):
+        B = int(w.ent.shape[0])
+        N, E, Pn = int(w.nodes.sum()), int(w.edges.sum()), int(w.pats.sum())
+        for what, v in (("nodes", N), ("edges", E), ("patterns", Pn)):
+            if v > _I32_MAX:
+                raise _lib.PertGnnError(f"the requests hold {v} {what}; a batch holds at most 2^31 - 1")
+        d = w.desc()
+
+        def launch(offsets, out):
+            rc = _lib.lib().pert_store_assemble_whatif(
+                C.byref(self.desc), C.byref(self.asof_desc) if asof else None, C.byref(d), w.ent_d.data_ptr(),
+                w.ts_d.data_ptr(), B, N, E, offsets, out, self.status.data_ptr(), _lib.stream())
+            _lib.check(rc, "pert_store_assemble_whatif")
+
+        keep = tuple(t for t in (w.ent_d, w.ts_d, w.ptr_d, w.pat_d, w.prob_d, w.scen_d, w.ov_keys, w.ov_vals)
+                     if t is not None)
+        return self._outputs(B, N, E, Pn, launch, keep, label=False)
+
+    @_lib.on_device_of
+    def lookup_resources(self, timestamps, ms, asof=False):
+        """The resource row request assembly joins for each (timestamp, ms) query: -> (values [k, 8] float32, found [k]
+        bool), device tensors.  The row of (floor(t / 30000) * 30000, ms) under the exact join, or with ``asof`` the
+        newest row of ms at or before that bucket (the first of equal keys, as assembly reads it); no row, or ms
+        outside [0, n_ms): zeros and False.  E.g. the scenario "the current row x 1.2" is ``values * 1.2`` as override
+        values.  ``timestamps`` / ``ms``: int64 host arrays or CUDA tensors of one length."""
+        dev = self.device
+        cols = []
+        for a, what in ((timestamps, "timestamps"), (ms, "ms")):
+            if torch.is_tensor(a) and a.is_cuda:
+                if a.dtype.is_floating_point or a.dtype.is_complex or a.dtype == torch.bool:
+                    raise _lib.PertGnnError(f"{what}: integers expected, got {a.dtype}")
+                cols.append(a.reshape(-1).to(dev, torch.int64).contiguous())
+            else:
+                cols.append(torch.from_numpy(_int_column(a, what)).to(dev, non_blocking=True))
+        ts_d, ms_d = cols
+        k = int(ts_d.shape[0])
+        if ms_d.shape[0] != k:
+            raise _lib.PertGnnError(f"{k} timestamps but {ms_d.shape[0]} microservices")
+        values = torch.empty(k, 8, dtype=torch.float32, device=dev)
+        found = torch.empty(k, dtype=torch.bool, device=dev)
+        _lib.check(_lib.lib().pert_store_lookup_resources(
+            C.byref(self.desc), C.byref(self.asof_desc) if asof else None, ts_d.data_ptr(), ms_d.data_ptr(), k,
+            values.data_ptr(), found.data_ptr(), _lib.stream()), "pert_store_lookup_resources")
+        return values, found
 
     def check(self):
         """Synchronising check of the status word (trace id or entry id out of range / missing (timestamp, ms) row of

@@ -835,7 +835,8 @@ class _BucketedPredict(_BucketState):
 
 
 @torch.no_grad()
-def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, local=False, max_graphs=32):
+def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, local=False, max_graphs=32, mixes=None,
+            overrides=None, scenario_ids=None):
     """Predicted latency of every request (entry ``entry_ids[q]`` at time ``timestamps[q]``, ms) of a pattern store's
     entries: float32 device tensor [Q], in request order (duplicates and any order allowed).  With ``local``, also the
     local (per-node) predictions [sum of the requests' node counts] and ``node_ptr`` [Q+1] (int64), request q owning
@@ -847,19 +848,30 @@ def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, lo
     padded into its capacity bucket, replayed from one CUDA graph per bucket as in ``evaluate_bucketed``.  The workspace
     is sized once, on the host, for the largest slice.  Runs in eval mode under ``no_grad`` and restores the training
     flag; BatchNorm statistics, the dropout counter, parameters and optimizer state are left as they were.  A bad entry id
-    raises ``PertGnnError`` before any launch."""
-    ent = store.check_entries(entry_ids)
-    ts = np.asarray(timestamps, dtype=np.int64).reshape(-1)
-    if ts.shape != ent.shape:
-        raise _lib.PertGnnError(f"{ent.shape[0]} entry ids but {ts.shape[0]} timestamps")
+    raises ``PertGnnError`` before any launch.
+
+    What-if prediction: ``mixes``, ``overrides`` and ``scenario_ids`` as in ``PatternStore.assemble_requests`` (per-
+    request pattern mixes, resource override rows and each request's scenario, -1 for none), checked on the host and
+    uploaded once per call (the override table sorted once); every slice assembles from slices of them.  The slices
+    are sized, and ``node_ptr`` set, from the mixes' node counts.  A what-if slice pads into the same capacity buckets
+    as a plain one, so it replays the graphs plain calls captured."""
+    what_if = mixes is not None or overrides is not None or scenario_ids is not None
     bs = int(batch_size)
+    if what_if:
+        w = store._what_if_arrays(entry_ids, timestamps, mixes, overrides, scenario_ids)
+        ent, nodes, edges = w.ent, w.nodes, w.edges
+    else:
+        ent = store.check_entries(entry_ids)
+        ts = np.asarray(timestamps, dtype=np.int64).reshape(-1)
+        if ts.shape != ent.shape:
+            raise _lib.PertGnnError(f"{ent.shape[0]} entry ids but {ts.shape[0]} timestamps")
+        nodes, edges = store._h_ent_nodes[ent], store._h_ent_edges[ent]
     if bs < 1:
         raise _lib.PertGnnError("batch_size must be >= 1")
     Q = int(ent.shape[0])
     dev = store.device
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
-    nodes, edges = store._h_ent_nodes[ent], store._h_ent_edges[ent]
     node_ptr = np.zeros(Q + 1, dtype=np.int64)
     np.cumsum(nodes, out=node_ptr[1:])
     was_training = model.training
@@ -876,8 +888,9 @@ def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, lo
                 starts = np.arange(0, Q, bs)          # the slices' sizes, exactly: host-only, no device sync
                 eng.reserve(*bucket_bound(int(np.add.reduceat(nodes, starts).max()),
                                           int(np.add.reduceat(edges, starts).max()), min(bs, Q)))
-                ent_d = torch.from_numpy(ent).to(dev, non_blocking=True)
-                ts_d = torch.from_numpy(ts).to(dev, non_blocking=True)
+                if not what_if:
+                    ent_d = torch.from_numpy(ent).to(dev, non_blocking=True)
+                    ts_d = torch.from_numpy(ts).to(dev, non_blocking=True)
             n_if, n_rpc = model.interface_embeds.num_embeddings, model.rpctype_embeds.num_embeddings
 
             def run(buf):
@@ -890,7 +903,8 @@ def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, lo
 
             for i in range(0, Q, bs):
                 j = min(i + bs, Q)
-                data = store.assemble_requests(ent[i:j], None, asof=asof, device_arrays=(ent_d[i:j], ts_d[i:j]))
+                arrays = w.slice(i, j) if what_if else (ent_d[i:j], ts_d[i:j])
+                data = store.assemble_requests(ent[i:j], None, asof=asof, device_arrays=arrays)
                 data.y = st.labels(j - i)
                 g, loc, _ = _bucket_run(st, data, eng, run, max_graphs)
                 gpred[i:j].copy_(g[:j - i, 0])

@@ -15,6 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpertgnn.so")
 
 P, I, LL, F = C.c_void_p, C.c_int, C.c_longlong, C.c_float
+I32 = C.c_int32
 
 # name -> (restype, argtypes); must mirror include/pertgnn.h
 SIGNATURES = {
@@ -117,18 +118,93 @@ class PertGnnError(RuntimeError):
     pass
 
 
+# ---- the structs of include/pertgnn.h, field for field, checked against the header by tests/test_abi_structs.py; the
+# header documents every field
+MAX_CONVS, MAX_CAT = 8, 4                               # PERT_MAX_CONVS, PERT_MAX_CAT
+
+
+class PertModelDesc(C.Structure):
+    _fields_ = [
+        ("F", I32), ("H", I32), ("n_convs", I32), ("n_cat", I32), ("cat_rows", I32 * MAX_CAT), ("n_entry", I32),
+        ("n_if", I32), ("n_rpc", I32), ("k0", I32), ("bn_eps", F), ("bn_momentum", F),
+        ("off_cat", LL * MAX_CAT), ("off_entry", LL), ("off_if", LL), ("off_rpc", LL),
+        ("off_wq", LL * MAX_CONVS), ("off_bq", LL * MAX_CONVS), ("off_wk", LL * MAX_CONVS), ("off_bk", LL * MAX_CONVS),
+        ("off_wv", LL * MAX_CONVS), ("off_bv", LL * MAX_CONVS), ("off_ws", LL * MAX_CONVS), ("off_bs", LL * MAX_CONVS),
+        ("off_we", LL * MAX_CONVS), ("off_bn_g", LL * MAX_CONVS), ("off_bn_b", LL * MAX_CONVS),
+        ("off_local_w", LL), ("off_local_b", LL), ("off_g1_w", LL), ("off_g1_b", LL), ("off_g2_w", LL),
+        ("off_g2_b", LL),
+    ]
+
+
+class PertProbe(C.Structure):
+    _fields_ = [("kernel", I32), ("layer", I32), ("ev_start", P), ("ev_stop", P)]
+
+
+class PertStore(C.Structure):
+    _fields_ = [("n_pat", I32), ("n_ent", I32), ("n_res", I32), ("n_ms", I32), ("attr_cols", I32), ("n_traces", LL)] + \
+        [(k, P) for k in ("pat_nptr", "pat_eptr", "pat_ms", "pat_depth", "pat_last", "pat_src", "pat_dst", "pat_attr",
+                          "ent_ptr", "ent_pat", "ent_prob", "ent_nodes", "ent_edges", "res_keys", "res_vals",
+                          "ms_has_res", "trace_entry", "trace_ts", "trace_y")]
+
+
+class PertBatchOut(C.Structure):
+    _fields_ = [(k, P) for k in ("x", "cat_X", "node_depth", "pattern_num_nodes", "rt_probs", "batch", "edge_index",
+                                 "edge_attr", "entry_id", "y", "ptr", "pattern_probs")]
+
+
 class PertResourceAsOf(C.Structure):
-    """The as-of index of a store's resource rows (include/pertgnn.h): device pointers ms_ptr [n_ms+1] int32,
-    ts [n_res] int64, row [n_res] int32."""
+    """The as-of index of a store's resource rows: device pointers ms_ptr [n_ms+1] int32, ts [n_res] int64, row [n_res]
+    int32."""
     _fields_ = [("ms_ptr", P), ("ts", P), ("row", P)]
 
 
 class PertWhatIf(C.Structure):
-    """Per-request mixes and resource overrides of what-if assembly (include/pertgnn.h): device pointers mix_ptr [B+1]
-    int64 (absolute offsets) into mix_pat int32 / mix_prob float32, scenario [B] int64, and n_ov override rows,
-    ov_keys [n_ov] int64 sorted and ov_vals [n_ov, 8] float32 (16-byte aligned); NULL mix_ptr / scenario: none."""
+    """Per-request mixes and resource overrides of what-if assembly: device pointers mix_ptr [B+1] int64 (absolute
+    offsets) into mix_pat int32 / mix_prob float32, scenario [B] int64, and n_ov override rows, ov_keys [n_ov] int64
+    sorted and ov_vals [n_ov, 8] float32 (16-byte aligned); NULL mix_ptr / scenario: none."""
     _fields_ = [("mix_ptr", P), ("mix_pat", P), ("mix_prob", P), ("scenario", P), ("n_ov", LL), ("ov_keys", P),
                 ("ov_vals", P)]
+
+
+class PertRuntimeKeys(C.Structure):
+    _fields_ = [("n", LL), ("ld", LL), ("ptr", P), ("rows", P)]
+
+
+class PertRuntimeTable(C.Structure):
+    _fields_ = [("S", LL), ("hash_bits", I32), ("slot", P), ("h1", P), ("h2", P)]
+
+
+class PertChunkMix(C.Structure):
+    _fields_ = [("n_ent", LL), ("n_pairs", LL)] + [(k, P) for k in ("ent_pair_ptr", "ent_trace_ptr", "pair_runtime",
+                                                                   "pair_prob", "runtime_ins", "pat_of")]
+
+
+class PertMixOut(C.Structure):
+    _fields_ = [(k, P) for k in ("ent_ptr", "ent_pat", "ent_prob", "cnt", "ent_nodes", "ent_edges", "tot")]
+
+
+class PertIngestState(C.Structure):
+    _fields_ = [("keys", PertRuntimeKeys)] + [(k, P) for k in ("trace_pat", "trace_tid", "cnt", "tot")] + \
+        [(k, LL) for k in ("n_pairs", "n_nodes", "n_edges", "n_key_rows")]
+
+
+EVICT_ARRAYS = ("remap", "trace_entry", "trace_ts", "trace_y", "trace_pat", "trace_tid", "pat_new", "pat_nptr",
+                "pat_eptr", "pat_ms", "pat_depth", "pat_last", "pat_src", "pat_dst", "pat_attr", "key_ptr", "key_rows")
+
+
+class PertEvictOut(C.Structure):
+    _fields_ = [("mix", PertMixOut)] + [(k, P) for k in EVICT_ARRAYS] + [("key_ld", LL)]
+
+
+class PertSpanTable(C.Structure):
+    _fields_ = [("R", LL)] + [(k, P) for k in ("traceid", "timestamp", "rpcid", "um", "dm", "interface", "rpctype",
+                                               "rt", "entryid")]
+
+
+class PertTraceGroups(C.Structure):
+    _fields_ = [(k, P) for k in ("row_ptr", "perm", "trace_id", "bucket", "y", "entry", "runtime", "order",
+                                 "ent_trace_ptr", "ent_pair_ptr", "pair_runtime", "pair_prob", "occurrences",
+                                 "ins_runtime", "rep_trace", "runtime_ins", "rep_ptr", "sizes")]
 
 
 def lib():

@@ -37,6 +37,19 @@ __host__ __device__ __forceinline__ int64_t pert_time_bucket(int64_t ts) {
   return q * TG_BUCKET;
 }
 
+// Largest b in [0, n) with off[b] <= v, for an exclusive prefix sum off (non-decreasing, off[0] = 0 <= v): the segment
+// that holds item v.  The compares run in the type of v, so an int item costs 32-bit compares.
+template <typename V>
+__device__ __forceinline__ int upper_seg(const int* __restrict__ off, int n, V v) {
+  int lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (off[mid] <= v) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
 __device__ __forceinline__ float4 ldg4(const float* p) {
   return __ldg(reinterpret_cast<const float4*>(p));
 }

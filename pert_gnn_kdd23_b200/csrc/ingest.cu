@@ -137,17 +137,6 @@ __global__ void k_new_assign(long long n, long long n_pat, const int* runtime_in
   }
 }
 
-// largest e in [0, n) with ptr[e] <= v (ptr non-decreasing, ptr[0] = 0 <= v)
-__device__ __forceinline__ int seg_of(const int* __restrict__ ptr, long long n, long long v) {
-  int lo = 0, hi = (int)n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (ptr[mid] <= v) lo = mid;
-    else hi = mid;
-  }
-  return lo;
-}
-
 __device__ __forceinline__ unsigned long long pair_key(int e, int pat) {
   return ((unsigned long long)(unsigned)e << 32) | (unsigned)pat;
 }
@@ -156,7 +145,7 @@ __device__ __forceinline__ unsigned long long pair_key(int e, int pat) {
 __global__ void k_pair_table(PertStore s, long long n_pairs, long long S, unsigned long long* pkey, int* pval) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_pairs) return;
-  const int e = seg_of(s.ent_ptr, s.n_ent, i);
+  const int e = upper_seg(s.ent_ptr, s.n_ent, i);
   const unsigned long long key = pair_key(e, s.ent_pat[i]);
   long long j = (long long)(mix64(key) & (unsigned long long)(S - 1));
   while (atomicCAS(&pkey[j], IG_NOKEY, key) != IG_NOKEY) j = (j + 1) & (S - 1);
@@ -169,7 +158,7 @@ __global__ void k_chunk_pairs(PertStore s, PertChunkMix c, long long S, const un
                               const int* pval, int* add, int* nf, int* jent, int* jpat, int* jcnt) {
   const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= c.n_pairs) return;
-  const int e = seg_of(c.ent_pair_ptr, c.n_ent, j);
+  const int e = upper_seg(c.ent_pair_ptr, c.n_ent, j);
   const int pat = c.pat_of[c.runtime_ins[c.pair_runtime[j]]];
   // pair_prob = count / total, correctly rounded, with count <= total < 2^31: prob * total is within 2^-22 of count
   const int cnt = (int)llrint(c.pair_prob[j] * (double)(c.ent_trace_ptr[e + 1] - c.ent_trace_ptr[e]));
@@ -231,7 +220,7 @@ __device__ __forceinline__ void emit(const PertMixOut& out, long long slot, int 
 __global__ void k_emit_old(PertStore s, const int* cnt, const int* add, long long n_pairs, PertMixOut out) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_pairs) return;
-  const int e = seg_of(s.ent_ptr, s.n_ent, i);
+  const int e = upper_seg(s.ent_ptr, s.n_ent, i);
   emit(out, out.ent_ptr[e] + (i - s.ent_ptr[e]), s.ent_pat[i], cnt[i] + add[i], out.tot[e]);
 }
 
@@ -415,7 +404,7 @@ __global__ void k_evict_apply_traces(PertStore s, PertIngestState g, EvictWs w, 
 __global__ void k_evict_apply_pairs(PertStore s, PertIngestState g, EvictWs w, PertMixOut out) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= g.n_pairs || w.pkeep[i + 1] == w.pkeep[i]) return;
-  const int e = seg_of(s.ent_ptr, s.n_ent, i);
+  const int e = upper_seg(s.ent_ptr, s.n_ent, i);
   emit(out, w.pkeep[i], w.pa[s.ent_pat[i]], g.cnt[i] - w.ev[i], w.e_tot[e]);
 }
 
@@ -447,7 +436,7 @@ __global__ void k_evict_apply_pats(PertStore s, EvictWs w, PertEvictOut o) {
 __global__ void k_evict_apply_nodes(PertStore s, long long n_nodes, EvictWs w, PertEvictOut o) {
   const long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= n_nodes) return;
-  const int p = seg_of(s.pat_nptr, s.n_pat, v);
+  const int p = upper_seg(s.pat_nptr, s.n_pat, v);
   if (w.pa[p + 1] == w.pa[p]) return;
   const long long j = w.pn[p] + (v - s.pat_nptr[p]);
   o.pat_ms[j] = s.pat_ms[v];
@@ -459,7 +448,7 @@ __global__ void k_evict_apply_nodes(PertStore s, long long n_nodes, EvictWs w, P
 __global__ void k_evict_apply_edges(PertStore s, long long n_edges, EvictWs w, PertEvictOut o) {
   const long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (x >= n_edges) return;
-  const int p = seg_of(s.pat_eptr, s.n_pat, x);
+  const int p = upper_seg(s.pat_eptr, s.n_pat, x);
   if (w.pa[p + 1] == w.pa[p]) return;
   const long long j = w.pe[p] + (x - s.pat_eptr[p]);
   o.pat_src[j] = s.pat_src[x];
@@ -471,7 +460,7 @@ __global__ void k_evict_apply_edges(PertStore s, long long n_edges, EvictWs w, P
 __global__ void k_evict_apply_keys(PertStore s, PertIngestState g, EvictWs w, PertEvictOut o) {
   const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= g.n_key_rows) return;
-  const int p = seg_of(g.keys.ptr, s.n_pat, r);
+  const int p = upper_seg(g.keys.ptr, s.n_pat, r);
   if (w.pa[p + 1] == w.pa[p]) return;
   const long long j = w.pk[p] + (r - g.keys.ptr[p]);
   const long long ld = g.keys.ld, nld = o.key_ld;

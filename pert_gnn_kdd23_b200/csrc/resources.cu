@@ -63,17 +63,6 @@ __device__ __forceinline__ int group_start(const int64_t* __restrict__ nk, const
   return lo;
 }
 
-__device__ __forceinline__ int upper_seg(const int* __restrict__ off, int n, long long v) {
-  // largest m in [0, n) with off[m] <= v (off an exclusive prefix sum)
-  int lo = 0, hi = n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (off[mid] <= v) lo = mid;
-    else hi = mid;
-  }
-  return lo;
-}
-
 // One thread per microservice m (thread n_ms: the table-wide sizes).  seg[m] = first surviving entry of m's old as-of
 // segment (asof.ms_ptr[m] + its evicted rows), seg[n_ms + m] = first surviving grouped index of m's batch rows; the
 // surviving row count of m goes to ms_ptr_out[m] (scanned into offsets afterwards).  sizes = {p, q, n_out}: evicted

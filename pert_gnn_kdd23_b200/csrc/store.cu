@@ -28,17 +28,6 @@ namespace {
 
 constexpr int NF = 8;   // resource statistics per (timestamp, ms) row; x has NF + 1 columns (pert_gnn.py:44-52)
 
-__device__ __forceinline__ int upper_seg(const int* __restrict__ off, int n, int v) {
-  // largest b in [0, n) with off[b] <= v   (off is an exclusive prefix sum, off[n] = total)
-  int lo = 0, hi = n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (off[mid] <= v) lo = mid;
-    else hi = mid;
-  }
-  return lo;
-}
-
 // Where graph b of a batch takes its entry, time bucket, label and pattern mix from: a row of the store's trace table
 // (pert_store_assemble), a request (pert_store_assemble_requests) or a what-if request (pert_store_assemble_whatif).
 // entry() flags a bad id in `bad` and falls back to trace 0 / entry 0; the other reads repeat the fallback, so every

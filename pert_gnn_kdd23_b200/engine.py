@@ -12,33 +12,16 @@ import os
 import torch
 
 from . import _lib, ops
+from ._lib import MAX_CAT, MAX_CONVS, PertModelDesc
 from .index import GraphIndex
-
-MAX_CONVS, MAX_CAT = 8, 4
-LL = C.c_longlong
-
-
-class PertModelDesc(C.Structure):
-    _fields_ = [
-        ("F", C.c_int32), ("H", C.c_int32), ("n_convs", C.c_int32), ("n_cat", C.c_int32),
-        ("cat_rows", C.c_int32 * MAX_CAT), ("n_entry", C.c_int32), ("n_if", C.c_int32), ("n_rpc", C.c_int32),
-        ("k0", C.c_int32), ("bn_eps", C.c_float), ("bn_momentum", C.c_float),
-        ("off_cat", LL * MAX_CAT), ("off_entry", LL), ("off_if", LL), ("off_rpc", LL),
-        ("off_wq", LL * MAX_CONVS), ("off_bq", LL * MAX_CONVS), ("off_wk", LL * MAX_CONVS), ("off_bk", LL * MAX_CONVS),
-        ("off_wv", LL * MAX_CONVS), ("off_bv", LL * MAX_CONVS), ("off_ws", LL * MAX_CONVS), ("off_bs", LL * MAX_CONVS),
-        ("off_we", LL * MAX_CONVS), ("off_bn_g", LL * MAX_CONVS), ("off_bn_b", LL * MAX_CONVS),
-        ("off_local_w", LL), ("off_local_b", LL), ("off_g1_w", LL), ("off_g1_b", LL), ("off_g2_w", LL),
-        ("off_g2_b", LL),
-    ]
 
 
 def _bind():
     return _lib.lib()
 
 
-class PertProbe(C.Structure):
+class PertProbe(_lib.PertProbe):
     """Measurement probe (include/pertgnn.h): two CUDA events recorded around one kernel family of one layer."""
-    _fields_ = [("kernel", C.c_int32), ("layer", C.c_int32), ("ev_start", C.c_void_p), ("ev_stop", C.c_void_p)]
 
     KERNELS = {"tconv_fwd": 1, "tconv_bwd": 2, "gemm_fwd": 3, "gemm_wgrad": 4, "gemm_dgrad": 5}
     _rt = None

@@ -20,81 +20,63 @@ import itertools
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, pertgraph
 from .data import Batch
 
-I32, I64, P = C.c_int32, C.c_longlong, C.c_void_p
+# the C structs under the names this module has always exported (the mirrors themselves live in _lib)
+_PertStore, _PertBatchOut, _RuntimeKeys, _RuntimeTable = (_lib.PertStore, _lib.PertBatchOut, _lib.PertRuntimeKeys,
+                                                          _lib.PertRuntimeTable)
+_ChunkMix, _MixOut, _IngestState, _EvictOut = (_lib.PertChunkMix, _lib.PertMixOut, _lib.PertIngestState,
+                                                _lib.PertEvictOut)
+_EVICT_ARRAYS = _lib.EVICT_ARRAYS
 
 
-class _PertStore(C.Structure):
-    _fields_ = [("n_pat", I32), ("n_ent", I32), ("n_res", I32), ("n_ms", I32), ("attr_cols", I32),
-                ("n_traces", I64),
-                ("pat_nptr", P), ("pat_eptr", P), ("pat_ms", P), ("pat_depth", P), ("pat_last", P), ("pat_src", P),
-                ("pat_dst", P), ("pat_attr", P), ("ent_ptr", P), ("ent_pat", P), ("ent_prob", P), ("ent_nodes", P),
-                ("ent_edges", P), ("res_keys", P), ("res_vals", P), ("ms_has_res", P), ("trace_entry", P),
-                ("trace_ts", P), ("trace_y", P)]
-
-
-class _PertBatchOut(C.Structure):
-    _fields_ = [(k, P) for k in ("x", "cat_X", "node_depth", "pattern_num_nodes", "rt_probs", "batch", "edge_index",
-                                 "edge_attr", "entry_id", "y", "ptr", "pattern_probs")]
-
-
-class _RuntimeKeys(C.Structure):
-    _fields_ = [("n", I64), ("ld", I64), ("ptr", P), ("rows", P)]
-
-
-class _RuntimeTable(C.Structure):
-    _fields_ = [("S", I64), ("hash_bits", I32), ("slot", P), ("h1", P), ("h2", P)]
-
-
-class _ChunkMix(C.Structure):
-    _fields_ = [("n_ent", I64), ("n_pairs", I64)] + [(k, P) for k in ("ent_pair_ptr", "ent_trace_ptr", "pair_runtime",
-                                                                     "pair_prob", "runtime_ins", "pat_of")]
-
-
-class _MixOut(C.Structure):
-    _fields_ = [(k, P) for k in ("ent_ptr", "ent_pat", "ent_prob", "cnt", "ent_nodes", "ent_edges", "tot")]
-
-
-class _IngestState(C.Structure):
-    _fields_ = [("keys", _RuntimeKeys)] + [(k, P) for k in ("trace_pat", "trace_tid", "cnt", "tot")] + \
-        [(k, I64) for k in ("n_pairs", "n_nodes", "n_edges", "n_key_rows")]
-
-
-_EVICT_ARRAYS = ("remap", "trace_entry", "trace_ts", "trace_y", "trace_pat", "trace_tid", "pat_new", "pat_nptr",
-                 "pat_eptr", "pat_ms", "pat_depth", "pat_last", "pat_src", "pat_dst", "pat_attr", "key_ptr", "key_rows")
-
-
-class _EvictOut(C.Structure):
-    _fields_ = [("mix", _MixOut)] + [(k, P) for k in _EVICT_ARRAYS] + [("key_ld", I64)]
-
-
-def _last_flags_device(nptr, ms):
-    """pat_last on the device: get_x keeps the LAST node of every microservice of a pattern (pert_gnn.py:54-65); a
-    stable sort by (pattern, ms), where the last of every run of equal keys is the largest node index.  ``nptr``: int64
-    [n_pat+1] node offsets, ``ms``: int64 [n_all]."""
+def _last_flags(nptr, ms):
+    """pat_last: 1 for the LAST node of every microservice of a pattern, else 0 (get_x's dict ms2nid keeps the last
+    one, pert_gnn.py:54-65).  ``nptr``: int64 [n_pat+1] node offsets, ``ms``: int64 [n_all], on one device.  A stable
+    sort by ms, then a stable sort by pattern, orders the nodes by (pattern, ms, node index): the last node of every
+    run of equal (pattern, ms) is flagged.  Exact for every int64 ms, and no host synchronisation."""
     dev, n_all = ms.device, int(ms.shape[0])
     pid = torch.repeat_interleave(torch.arange(int(nptr.shape[0]) - 1, device=dev), nptr.diff(), output_size=n_all)
-    key, idx = torch.sort(pid * (1 << 32) + ms, stable=True)
+    by_ms = torch.sort(ms, stable=True)[1]
+    idx = by_ms[torch.sort(pid[by_ms], stable=True)[1]]
+    p, m = pid[idx], ms[idx]
     run_end = torch.ones(n_all, dtype=torch.bool, device=dev)
-    run_end[:-1] = key[1:] != key[:-1]
+    run_end[:-1] = (p[1:] != p[:-1]) | (m[1:] != m[:-1])
     last = torch.zeros(n_all, dtype=torch.uint8, device=dev)
     last[idx[run_end]] = 1
     return last
 
 
-def _last_occurrence_flags(all_ms, nptr):
-    """flags[i] = 1 iff node i is the LAST node of its microservice inside its pattern (patterns = nptr slices)."""
-    n_all = int(all_ms.shape[0])
-    flags = np.zeros(n_all, dtype=np.uint8)
-    if n_all:
-        pid = np.repeat(np.arange(len(nptr) - 1, dtype=np.int64), np.diff(nptr))
-        lo = int(all_ms.min())
-        key = pid * (int(all_ms.max()) - lo + 1) + (all_ms - lo)
-        _, first_rev = np.unique(key[::-1], return_index=True)
-        flags[n_all - 1 - first_rev] = 1
-    return flags
+def _pattern_arrays(graphs, dev):
+    """The pat_* entries of a store's ``t`` on ``dev`` from concatenated patterns (``pertgraph.PertGraphs``: host node /
+    edge offsets, ms_id, node_depth, pattern-local edge_index and edge_attr, host or device tensors)."""
+    i32, i64 = torch.int32, torch.int64
+    nptr, eptr = (torch.from_numpy(np.asarray(p, dtype=np.int64)).to(dev) for p in (graphs.node_ptr, graphs.edge_ptr))
+    ms = graphs.ms_id.reshape(-1).to(dev, i64).contiguous()
+    ei = graphs.edge_index.to(dev)
+    return {"pat_nptr": nptr.to(i32), "pat_eptr": eptr.to(i32), "pat_ms": ms,
+            "pat_depth": graphs.node_depth.reshape(-1).to(dev, i64).contiguous(), "pat_last": _last_flags(nptr, ms),
+            "pat_src": ei[0].to(i32).contiguous(), "pat_dst": ei[1].to(i32).contiguous(),
+            "pat_attr": graphs.edge_attr.to(dev, i64).contiguous()}
+
+
+def _mix_out(n_ent, n_pairs, dev):
+    """The arrays of a rewritten entry mix of n_ent entries with room for n_pairs pairs, and their ``PertMixOut``."""
+    i32 = torch.int32
+    o = {"ent_ptr": torch.empty(n_ent + 1, dtype=i32, device=dev),
+         "ent_pat": torch.empty(n_pairs, dtype=i32, device=dev),
+         "ent_prob": torch.empty(n_pairs, dtype=torch.float32, device=dev),
+         "cnt": torch.empty(n_pairs, dtype=i32, device=dev), "ent_nodes": torch.empty(n_ent, dtype=i32, device=dev),
+         "ent_edges": torch.empty(n_ent, dtype=i32, device=dev), "tot": torch.empty(n_ent, dtype=i32, device=dev)}
+    return o, _lib.PertMixOut(*(o[name].data_ptr() for name, _ in _lib.PertMixOut._fields_))
+
+
+def _cuda_device(device):
+    dev = torch.device(device)
+    if dev.type != "cuda":
+        raise _lib.PertGnnError("PatternStore lives on a CUDA device (no CPU fallback for the hot path)")
+    return dev
 
 
 def asof_index(res_keys, n_ms):
@@ -122,6 +104,13 @@ def _index_rows(idx):
     """int64 [k, 2] host array of (timestamp, ms) pairs (shape checked by the caller); ``PertGnnError`` naming the first
     row that is not a pair of integers within int64 (floats are refused, not truncated)."""
     rows = idx if isinstance(idx, np.ndarray) else list(idx)
+    if rows is not idx:
+        try:                                             # pairs of integers: one pass per column, no per-row arrays
+            ts, ms = np.array([t for t, _ in rows]), np.array([m for _, m in rows])
+            if ts.ndim == ms.ndim == 1 and ts.dtype.kind == ms.dtype.kind == "i":
+                return np.stack([ts, ms], 1).astype(np.int64)
+        except (TypeError, ValueError, OverflowError):
+            pass                                         # the general path below names the bad row
     try:
         a = np.asarray(rows)
         if a.dtype.kind != "i" and not isinstance(idx, np.ndarray):
@@ -309,14 +298,6 @@ class _WhatIfArrays:
                                int(self.ov_keys.shape[0]), p(self.ov_keys), p(self.ov_vals))
 
 
-class _BulkPatterns:
-    """Concatenated host arrays of many patterns (PatternStore.from_graphs)."""
-
-    def __init__(self, rt_ids, node_ptr, edge_ptr, ms_id, node_depth, edge_index, edge_attr):
-        self.rt_ids, self.node_ptr, self.edge_ptr = rt_ids, node_ptr, edge_ptr
-        self.ms_id, self.node_depth, self.edge_index, self.edge_attr = ms_id, node_depth, edge_index, edge_attr
-
-
 class _TraceIngest:
     """What ``append_traces`` keeps beside a store built by ``from_trace_groups`` (outside ``t``): the graph kind, the
     runtime keys -- rows [3, R'] int64 (um, dm, interface of every pattern's representative, pattern order) and ptr
@@ -334,17 +315,17 @@ class _TraceIngest:
         self.table = None                                # dict(slot, h1, h2, S, bits)
 
     def state(self):
-        return _IngestState(self.keys(), self.trace_pat.data_ptr(), self.trace_tid.data_ptr(), self.cnt.data_ptr(),
-                            self.tot.data_ptr(), int(self.cnt.shape[0]), self.n_nodes, self.n_edges,
-                            int(self.rows.shape[1]))
+        return _lib.PertIngestState(self.keys(), self.trace_pat.data_ptr(), self.trace_tid.data_ptr(),
+                                    self.cnt.data_ptr(), self.tot.data_ptr(), int(self.cnt.shape[0]), self.n_nodes,
+                                    self.n_edges, int(self.rows.shape[1]))
 
     def keys(self):
-        return _RuntimeKeys(int(self.ptr.shape[0]) - 1, int(self.rows.shape[1]), self.ptr.data_ptr(),
-                            self.rows.data_ptr())
+        return _lib.PertRuntimeKeys(int(self.ptr.shape[0]) - 1, int(self.rows.shape[1]), self.ptr.data_ptr(),
+                                    self.rows.data_ptr())
 
     def table_desc(self):
         t = self.table
-        return _RuntimeTable(t["S"], t["bits"], t["slot"].data_ptr(), t["h1"].data_ptr(), t["h2"].data_ptr())
+        return _lib.PertRuntimeTable(t["S"], t["bits"], t["slot"].data_ptr(), t["h1"].data_ptr(), t["h2"].data_ptr())
 
     def insert(self, first, hash_bits):
         """Inserts runtimes first.. into the table; rebuilds it (larger) first when the load would pass 1/2 or the hash
@@ -396,54 +377,41 @@ class PatternStore:
     """Patterns, entries, resource table and traces on one CUDA device."""
 
     def __init__(self, runtime2graph, entry2runtimes, resource_index, resource_values, tr2data, device, n_ms=None):
-        dev = torch.device(device)
-        if dev.type != "cuda":
-            raise _lib.PertGnnError("PatternStore lives on a CUDA device (no CPU fallback for the hot path)")
-        self.device = dev
-        # ---- patterns, in the dict order of runtime2graph (or the bulk arrays of pertgraph.PertGraphs, see from_graphs)
-        if isinstance(runtime2graph, _BulkPatterns):
-            bp = runtime2graph
-            self.rt_ids = list(bp.rt_ids)
-            nptr, eptr = bp.node_ptr.astype(np.int64), bp.edge_ptr.astype(np.int64)
-            ms = [bp.ms_id.astype(np.int64)]
-            depth = [bp.node_depth.astype(np.int64)]
-            src, dst = [bp.edge_index[0].astype(np.int32)], [bp.edge_index[1].astype(np.int32)]
-            attr = [bp.edge_attr.astype(np.int64)]
-            cols = bp.edge_attr.shape[1]
-        else:
-            self.rt_ids = list(runtime2graph.keys())
-            nptr, eptr = [0], [0]
-            ms, depth, src, dst, attr = [], [], [], [], []
-            cols = None
-            for rt in self.rt_ids:
-                g = runtime2graph[rt]
-                n = int(g["num_nodes"])
-                # patterns may be CUDA tensors (pertgraph.PertGraphs.pattern): the host copy sizes batches and finds the
-                # last occurrence of every microservice; for many patterns use PatternStore.from_graphs (one bulk copy)
-                m = g["ms_id"].reshape(-1).to(torch.int64).cpu().numpy()
-                assert m.shape[0] == n
-                ei = g["edge_index"].cpu().numpy()
-                ea = g["edge_attr"].cpu().numpy()
-                cols = ea.shape[1] if cols is None else cols
-                assert ea.shape[1] == cols
-                nptr.append(nptr[-1] + n)
-                eptr.append(eptr[-1] + ei.shape[1])
-                ms.append(m)
-                depth.append(g["node_depth"].reshape(-1).to(torch.int64).cpu().numpy())
-                src.append(ei[0].astype(np.int32))
-                dst.append(ei[1].astype(np.int32))
-                attr.append(ea.astype(np.int64))
-        rt_index = {rt: i for i, rt in enumerate(self.rt_ids)}
-        nptr, eptr = np.asarray(nptr, dtype=np.int64), np.asarray(eptr, dtype=np.int64)
-        # get_x's dict ms2nid keeps the LAST node of every microservice of a pattern (pert_gnn.py:54-65): vectorised as
-        # the first occurrence of (pattern, ms) in the reversed node list
-        all_ms = np.concatenate(ms) if ms else np.zeros(0, dtype=np.int64)
-        last_flags = _last_occurrence_flags(all_ms, nptr)
-        last = [last_flags]
-        self.attr_cols = int(cols)
-        pat_nodes = np.diff(nptr)
-        pat_edges = np.diff(eptr)
+        # ---- patterns, in the dict order of runtime2graph, concatenated on the host.  Patterns may be CUDA tensors
+        # (pertgraph.PertGraphs.pattern), copied one by one; for many patterns use PatternStore.from_graphs
+        rt_ids = list(runtime2graph.keys())
+        gs = [runtime2graph[rt] for rt in rt_ids]
+        ms = [g["ms_id"].reshape(-1).to(torch.int64).cpu() for g in gs]
+        ei, ea = [g["edge_index"].cpu() for g in gs], [g["edge_attr"].cpu() for g in gs]
+        for g, m, a in zip(gs, ms, ea):
+            assert m.shape[0] == int(g["num_nodes"]) and a.shape[1] == ea[0].shape[1]
+        ptr = lambda sizes: np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)      # noqa: E731
+        graphs = pertgraph.PertGraphs(ptr([m.shape[0] for m in ms]), ptr([e.shape[1] for e in ei]), torch.cat(ms),
+                                      torch.cat(ei, 1), torch.cat(ea),
+                                      torch.cat([g["node_depth"].reshape(-1).to(torch.int64).cpu() for g in gs]),
+                                      None, None)
+        self._init_dicts(graphs, rt_ids, entry2runtimes, resource_index, resource_values, tr2data, device, n_ms)
+
+    @classmethod
+    def from_graphs(cls, graphs, runtime_ids, entry2runtimes, resource_index, resource_values, tr2data, device=None,
+                    n_ms=None):
+        """Patterns straight from ``pertgraph.build_pert_graphs`` / ``build_span_graphs`` (``graphs``: PertGraphs;
+        ``runtime_ids[i]`` names pattern i): no per-pattern copy or Python work."""
+        self = cls.__new__(cls)
+        self._init_dicts(graphs, runtime_ids, entry2runtimes, resource_index, resource_values, tr2data,
+                         device if device is not None else graphs.ms_id.device, n_ms)
+        return self
+
+    def _init_dicts(self, graphs, rt_ids, entry2runtimes, resource_index, resource_values, tr2data, device, n_ms):
+        """The constructor's store from concatenated patterns (``graphs``: PertGraphs, host or device tensors; pattern i
+        is runtime ``rt_ids[i]``) and the reference's dicts entry2runtimes and tr2data."""
+        dev = _cuda_device(device)
+        self.rt_ids = list(rt_ids)
+        assert len(self.rt_ids) == len(graphs.node_ptr) - 1
+        t = _pattern_arrays(graphs, dev)
+        pat_nodes, pat_edges = (np.diff(np.asarray(p, dtype=np.int64)) for p in (graphs.node_ptr, graphs.edge_ptr))
         # ---- entries, in the dict order of entry2runtimes[entry] (get_all_runtimes_id_probs, pert_gnn.py:70-74)
+        rt_index = {rt: i for i, rt in enumerate(self.rt_ids)}
         n_ent = max(entry2runtimes.keys()) + 1
         ent_ptr, ent_pat, ent_prob = [0], [], []
         ent_nodes, ent_edges = np.zeros(n_ent, dtype=np.int32), np.zeros(n_ent, dtype=np.int32)
@@ -455,13 +423,6 @@ class PatternStore:
                 ent_nodes[e] += pat_nodes[k]
                 ent_edges[e] += pat_edges[k]
             ent_ptr.append(len(ent_pat))
-        res_ms = np.array([m for _, m in resource_index], dtype=np.int64)
-        res_ts = np.array([t for t, _ in resource_index], dtype=np.int64)
-        self.n_ms = int(n_ms if n_ms is not None else max(int(all_ms.max(initial=0)), int(res_ms.max(initial=0))) + 1)
-        keys = res_ts * self.n_ms + res_ms
-        order = np.argsort(keys, kind="stable")
-        has = np.zeros(self.n_ms, dtype=np.uint8)
-        has[res_ms] = 1                                          # ms_with_resources (pert_gnn.py:138)
         # ---- traces, in the dict order of tr2data (get_data_list, pert_gnn.py:176-188)
         self.trace_keys = list(tr2data.keys())
         t_ent = np.array([int(tr2data[k]["entry_id"]) for k in self.trace_keys], dtype=np.int32)
@@ -471,48 +432,20 @@ class PatternStore:
         self._h_ent_nodes, self._h_ent_edges = ent_nodes.astype(np.int64), ent_edges.astype(np.int64)
         self._h_ent_pats = np.diff(np.array(ent_ptr)).astype(np.int64)
         self._h_trace_entry = t_ent.astype(np.int64)
-        self._h_pat_nodes, self._h_pat_edges = pat_nodes.astype(np.int64), pat_edges.astype(np.int64)
+        self._h_pat_nodes, self._h_pat_edges = pat_nodes, pat_edges
 
         def up(a, dtype):
             return torch.from_numpy(np.ascontiguousarray(a, dtype=dtype)).to(dev)
 
-        cat = lambda xs, dt: np.concatenate(xs).astype(dt) if xs else np.zeros(0, dtype=dt)   # noqa: E731
-        self.t = {
-            "pat_nptr": up(nptr, np.int32), "pat_eptr": up(eptr, np.int32), "pat_ms": up(cat(ms, np.int64), np.int64),
-            "pat_depth": up(cat(depth, np.int64), np.int64), "pat_last": up(cat(last, np.uint8), np.uint8),
-            "pat_src": up(cat(src, np.int32), np.int32), "pat_dst": up(cat(dst, np.int32), np.int32),
-            "pat_attr": up(np.concatenate(attr, axis=0) if attr else np.zeros((0, 2)), np.int64),
+        t.update({
             "ent_ptr": up(ent_ptr, np.int32), "ent_pat": up(ent_pat, np.int32),
             # torch.tensor(python floats, dtype=torch.float) of the reference == float64 -> float32 rounding
             "ent_prob": up(np.array(ent_prob, dtype=np.float64).astype(np.float32), np.float32),
             "ent_nodes": up(ent_nodes, np.int32), "ent_edges": up(ent_edges, np.int32),
-            "res_keys": up(keys[order], np.int64),
-            "res_vals": up(np.asarray(resource_values, dtype=np.float64)[order].astype(np.float32), np.float32),
-            "ms_has_res": up(has, np.uint8), "trace_entry": up(t_ent, np.int32), "trace_ts": up(t_ts, np.int64),
-            "trace_y": up(t_y, np.int64),
-        }
-        d = _PertStore()
-        d.n_pat, d.n_ent, d.n_res, d.n_ms, d.attr_cols = len(self.rt_ids), n_ent, int(keys.shape[0]), self.n_ms, \
-            self.attr_cols
-        d.n_traces = len(self.trace_keys)
-        for k, v in self.t.items():
-            setattr(d, k, v.data_ptr())
-        self.desc = d
-        self.status = torch.zeros(1, dtype=torch.int32, device=dev)
-        self._build_asof()
-
-    @classmethod
-    def from_graphs(cls, graphs, runtime_ids, entry2runtimes, resource_index, resource_values, tr2data, device=None,
-                    n_ms=None):
-        """Patterns straight from ``pertgraph.build_pert_graphs`` / ``build_span_graphs`` (``graphs``: PertGraphs;
-        ``runtime_ids[i]`` names pattern i): ONE device->host copy of the concatenated tensors instead of one per
-        pattern, no per-pattern Python work."""
-        dev = torch.device(device) if device is not None else graphs.ms_id.device
-        bp = _BulkPatterns(list(runtime_ids), np.asarray(graphs.node_ptr), np.asarray(graphs.edge_ptr),
-                           graphs.ms_id.cpu().numpy().reshape(-1), graphs.node_depth.cpu().numpy().reshape(-1),
-                           graphs.edge_index.cpu().numpy(), graphs.edge_attr.cpu().numpy())
-        assert len(bp.rt_ids) == len(bp.node_ptr) - 1
-        return cls(bp, entry2runtimes, resource_index, resource_values, tr2data, dev, n_ms=n_ms)
+            "trace_entry": up(t_ent, np.int32), "trace_ts": up(t_ts, np.int64), "trace_y": up(t_y, np.int64),
+        })
+        ms_max = int(graphs.ms_id.max()) if n_ms is None and graphs.ms_id.numel() else 0
+        self._finish(dev, t, ms_max, resource_index, resource_values, n_ms)
 
     @classmethod
     def from_artifacts(cls, art, device):
@@ -530,28 +463,23 @@ class PatternStore:
         groups.tr2data(), ...)`` with runtime2graph the ``kind`` ("pert" / "span") graph map, built from the device
         arrays of a ``tracegroup.TraceGroups`` without a Python loop over entries, patterns or traces.  Patterns in the
         reference's insertion order, traces in tr2data's key order; the one device->host copy besides the graph build
-        is the host sizing arrays the store keeps (per-trace entry and id, per-entry node / edge / pattern totals).
-        Microservice ids must lie in [0, 2^31)."""
+        is the host sizing arrays the store keeps (per-trace entry and id, per-entry node / edge / pattern totals)."""
         graphs, rt_ids = groups.graphs(kind)
-        dev = torch.device(device) if device is not None else graphs.ms_id.device
-        if dev.type != "cuda":
-            raise _lib.PertGnnError("PatternStore lives on a CUDA device (no CPU fallback for the hot path)")
+        dev = _cuda_device(device if device is not None else graphs.ms_id.device)
         self = cls.__new__(cls)
-        self.device, self.rt_ids = dev, list(rt_ids)
+        self.rt_ids = list(rt_ids)
         i32, i64 = torch.int32, torch.int64
         with torch.cuda.device(dev):
-            nptr = torch.from_numpy(np.asarray(graphs.node_ptr, dtype=np.int64)).to(dev)
-            eptr = torch.from_numpy(np.asarray(graphs.edge_ptr, dtype=np.int64)).to(dev)
+            t = _pattern_arrays(graphs, dev)
             n_pat, n_all = len(self.rt_ids), int(graphs.node_ptr[-1])
-            ms = graphs.ms_id.reshape(-1).to(dev, i64)
-            last = _last_flags_device(nptr, ms)
             # entries: entry2runtimes[e] in key order = the (entry, runtime) pairs of the groups
             ent_ptr = groups.ent_pair_ptr
             n_ent, n_pairs = int(ent_ptr.shape[0]) - 1, int(groups.pair_runtime.shape[0])
             ent_pat = groups.runtime_ins[groups.pair_runtime.long()]
             pair_entry = torch.repeat_interleave(torch.arange(n_ent, device=dev), ent_ptr.diff(), output_size=n_pairs)
             sums = []
-            for per_pat in (nptr.diff(), eptr.diff(), torch.ones(n_pat, dtype=i64, device=dev)):
+            for per_pat in (t["pat_nptr"].diff().long(), t["pat_eptr"].diff().long(),
+                            torch.ones(n_pat, dtype=i64, device=dev)):
                 sums.append(torch.zeros(n_ent, dtype=i64, device=dev).index_add_(0, pair_entry,
                                                                                   per_pat[ent_pat.long()]))
             ent_nodes, ent_edges, ent_pats = sums
@@ -566,55 +494,72 @@ class PatternStore:
                                         groups.trace_id[order], n_pat)
             t_ent = groups.entry[order]
             host = torch.cat([t_ent.long(), groups.trace_id[order], ent_nodes, ent_edges, ent_pats,
-                              ms.max().reshape(1) if n_all else torch.zeros(1, dtype=i64, device=dev)]).cpu().numpy()
+                              t["pat_ms"].max().reshape(1) if n_all else torch.zeros(1, dtype=i64, device=dev)]
+                             ).cpu().numpy()
+            t.update({
+                "ent_ptr": ent_ptr.to(dev, i32).contiguous(), "ent_pat": ent_pat.to(i32).contiguous(),
+                "ent_prob": groups.pair_prob.to(dev, torch.float32).contiguous(),      # float64 -> float32 rounding
+                "ent_nodes": ent_nodes.to(i32), "ent_edges": ent_edges.to(i32),
+                "trace_entry": t_ent.to(i32).contiguous(), "trace_ts": groups.bucket[order].contiguous(),
+                "trace_y": groups.y[order].contiguous(),
+            })
         T = int(order.shape[0])
         self._h_trace_entry, self.trace_keys = host[:T], host[T:2 * T].tolist()
         self._h_ent_nodes, self._h_ent_edges, self._h_ent_pats = (host[2 * T + k * n_ent:2 * T + (k + 1) * n_ent]
                                                                  for k in range(3))
         self._h_pat_nodes, self._h_pat_edges = (np.diff(np.asarray(p, dtype=np.int64))
                                                 for p in (graphs.node_ptr, graphs.edge_ptr))
-        res_ms = np.array([m for _, m in resource_index], dtype=np.int64)
-        res_ts = np.array([t for t, _ in resource_index], dtype=np.int64)
-        self.n_ms = int(n_ms if n_ms is not None else max(int(host[-1]), int(res_ms.max(initial=0))) + 1)
-        keys = res_ts * self.n_ms + res_ms
-        korder = np.argsort(keys, kind="stable")
-        has = np.zeros(self.n_ms, dtype=np.uint8)
-        has[res_ms] = 1                                          # ms_with_resources (pert_gnn.py:138)
-        self.attr_cols = int(graphs.edge_attr.shape[1])
-
-        def up(a, dtype):
-            return torch.from_numpy(np.ascontiguousarray(a, dtype=dtype)).to(dev)
-
-        ei = graphs.edge_index.to(dev)
-        self.t = {
-            "pat_nptr": nptr.to(i32), "pat_eptr": eptr.to(i32), "pat_ms": ms.contiguous(),
-            "pat_depth": graphs.node_depth.reshape(-1).to(dev, i64).contiguous(), "pat_last": last,
-            "pat_src": ei[0].to(i32).contiguous(), "pat_dst": ei[1].to(i32).contiguous(),
-            "pat_attr": graphs.edge_attr.to(dev, i64).contiguous(),
-            "ent_ptr": ent_ptr.to(dev, i32).contiguous(), "ent_pat": ent_pat.to(i32).contiguous(),
-            "ent_prob": groups.pair_prob.to(dev, torch.float32).contiguous(),      # float64 -> float32 rounding
-            "ent_nodes": ent_nodes.to(i32), "ent_edges": ent_edges.to(i32),
-            "res_keys": up(keys[korder], np.int64),
-            "res_vals": up(np.asarray(resource_values, dtype=np.float64)[korder].astype(np.float32), np.float32),
-            "ms_has_res": up(has, np.uint8), "trace_entry": t_ent.to(i32).contiguous(),
-            "trace_ts": groups.bucket[order].contiguous(), "trace_y": groups.y[order].contiguous(),
-        }
-        d = _PertStore()
-        d.n_pat, d.n_ent, d.n_res, d.n_ms, d.attr_cols = n_pat, n_ent, int(keys.shape[0]), self.n_ms, self.attr_cols
-        d.n_traces = T
-        for k, v in self.t.items():
-            setattr(d, k, v.data_ptr())
-        self.desc = d
-        self.status = torch.zeros(1, dtype=torch.int32, device=dev)
-        self._build_asof()
+        self._finish(dev, t, int(host[-1]), resource_index, resource_values, n_ms)
         return self
 
-    def _build_asof(self):
-        """The as-of index of the resource rows (``asof_index``), 12 bytes per row, kept beside the descriptor
-        (``append_resources`` keeps it current)."""
-        with torch.cuda.device(self.device):
-            ms_ptr, ts, row = asof_index(self.t["res_keys"], self.n_ms)
-        self._set_asof(ms_ptr, ts, row)
+    def _finish(self, dev, t, ms_max, resource_index, resource_values, n_ms):
+        """Completes a constructor.  ``t``: the pattern, entry and trace arrays on ``dev``; ``ms_max``: the largest
+        microservice id of the patterns (0 without nodes; not read when ``n_ms`` is given).  Adds the resource table:
+        the rows go through ``append_resources``' conversion and checks (``PertGnnError`` naming the first bad row),
+        are sorted stably by key timestamp * n_ms + ms (equal keys keep their input order), and n_ms defaults to the
+        largest microservice id of the patterns and the rows, plus one.  Then the descriptor, the status word and the
+        as-of index of the rows (12 bytes per row, kept beside the descriptor; ``append_resources`` keeps it
+        current)."""
+        idx = _index_rows(resource_index.cpu().numpy() if torch.is_tensor(resource_index) else resource_index)
+        if n_ms is None:
+            res_max = int(idx[:, 1].max(initial=0)) if idx.ndim == 2 and idx.shape[1] == 2 else 0   # else refused below
+            n_ms = max(ms_max, res_max, 0) + 1
+        self.device, self.n_ms, self.attr_cols = dev, int(n_ms), int(t["pat_attr"].shape[1])
+        with torch.cuda.device(dev):
+            ts, ms, vals = self._resource_batch(idx, resource_values)
+            keys, order = torch.sort(ts * self.n_ms + ms, stable=True)
+            has = torch.zeros(self.n_ms, dtype=torch.uint8, device=dev)
+            has[ms] = 1                                          # ms_with_resources (pert_gnn.py:138)
+            t.update({"res_keys": keys, "res_vals": vals[order], "ms_has_res": has})
+            self.t, self.desc = {}, _lib.PertStore()
+            self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+            self._commit({name: t[name] for name, _ in _lib.PertStore._fields_[6:]}, asof=asof_index(keys, self.n_ms))
+
+    def _commit(self, t, asof=None, ingest=None):
+        """The one place where the store's arrays change: installs ``t`` (entries of ``self.t``), ``asof`` (the as-of
+        index, (ms_ptr, ts, row)) and ``ingest`` (fields of ``self._ingest``), then rewrites the descriptor, its counts
+        taken from the arrays.  Every tensor replaced is first recorded on the current stream: the kernels that made the
+        new arrays and the assembly issued earlier on that stream still read it, so torch's allocator reuses its memory
+        only after them."""
+        old = [self.t[name] for name in t if name in self.t]
+        if asof is not None and hasattr(self, "asof_t"):
+            old += list(self.asof_t.values())
+        if ingest is not None:
+            old += [v for v in (getattr(self._ingest, name) for name in ingest) if torch.is_tensor(v)]
+        st = torch.cuda.current_stream() if old else None
+        for v in old:
+            v.record_stream(st)
+        self.t.update(t)
+        if asof is not None:
+            self._set_asof(*asof)
+        for name, v in (ingest or {}).items():
+            setattr(self._ingest, name, v)
+        d = self.desc
+        d.n_pat, d.n_ent = int(self.t["pat_nptr"].shape[0]) - 1, int(self.t["ent_ptr"].shape[0]) - 1
+        d.n_res, d.n_ms, d.attr_cols = int(self.t["res_keys"].shape[0]), self.n_ms, self.attr_cols
+        d.n_traces = int(self.t["trace_entry"].shape[0])
+        for name, v in self.t.items():
+            setattr(d, name, v.data_ptr())
 
     def _set_asof(self, ms_ptr, ts, row):
         self.asof_t = {"ms_ptr": ms_ptr, "ts": ts, "row": row}
@@ -727,14 +672,7 @@ class PatternStore:
             grp.data_ptr(), k, ms_ptr.data_ptr(), seg.data_ptr(), p, q, n_out, out["res_keys"].data_ptr(),
             out["res_vals"].data_ptr(), out["ms_has_res"].data_ptr(), a_ts.data_ptr(), a_row.data_ptr(),
             _lib.stream()), "pert_store_resources_merge")
-        st = torch.cuda.current_stream()
-        for old in [self.t[name] for name in out] + list(self.asof_t.values()):
-            old.record_stream(st)                        # the merge and earlier assembly on `st` still read it
-        for name, v in out.items():
-            self.t[name] = v
-            setattr(self.desc, name, v.data_ptr())
-        self.desc.n_res = n_out
-        self._set_asof(ms_ptr, a_ts, a_row)
+        self._commit(out, asof=(ms_ptr, a_ts, a_row))
         return self
 
     def evict_resources(self, before):
@@ -770,12 +708,9 @@ class PatternStore:
         representatives' row offsets), followed, when there are new runtimes, by the copy of their rows for the host
         row filters and the graph build's own read; one of the merged entry sizes.  Ordered on the current stream,
         like ``append_resources``: the old arrays return to torch's allocator on that stream."""
-        from . import pertgraph, tracegroup
+        from . import tracegroup
 
-        ing = getattr(self, "_ingest", None)
-        if ing is None:
-            raise _lib.PertGnnError("append_traces: this store keeps no runtime keys (it was built from dicts or by "
-                                    "from_graphs); build it with PatternStore.from_trace_groups to append traces")
+        ing = self._ingest_of("append_traces")
         missing = [k for k in tracegroup.COLUMNS if k not in columns]
         if missing:
             raise _lib.PertGnnError(f"append_traces: columns {missing} are missing")
@@ -804,7 +739,7 @@ class PatternStore:
         if ing.table is None or ing.table["bits"] != hash_bits:
             ing.insert(0, hash_bits)
         keys, tab = ing.keys(), ing.table_desc()
-        ck = _RuntimeKeys(n_c, int(g._rows.shape[1]), g.rep_ptr.data_ptr(), g._rows.data_ptr())
+        ck = _lib.PertRuntimeKeys(n_c, int(g._rows.shape[1]), g.rep_ptr.data_ptr(), g._rows.data_ptr())
         pat_of, new_rep, new_rt = (torch.empty(n_c, dtype=i32, device=dev) for _ in range(3))
         n_new_d = torch.empty(1, dtype=i64, device=dev)
         ws = torch.empty(int(L.pert_ingest_match_workspace_bytes(n_c)), dtype=torch.uint8, device=dev)
@@ -815,26 +750,19 @@ class PatternStore:
         k = int(h[0])
         reps, new_ids, rep_ptr = h[1:1 + k], h[1 + n_c:1 + n_c + k], h[1 + 2 * n_c:]
         new_ids = new_ids + (ing.next_rt - n_pat)        # ids n_pat + j -> next_rt + j: evicted ids are not reused
-        # ---- graphs of the new runtimes: host row filters, then the CUDA builder (TraceGroups.graphs' path)
+        # ---- graphs of the new runtimes, built as TraceGroups.graphs builds them
         lens = rep_ptr[reps + 1] - rep_ptr[reps]
         new_ptr = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
         sel = torch.from_numpy(np.repeat(rep_ptr[reps] - new_ptr[:-1], lens) + np.arange(int(new_ptr[-1]))).to(dev)
         new_rows = g._rows[:, sel]
+        g_nptr = g_eptr = np.zeros(1, dtype=np.int64)
         if k:
-            rows = new_rows.cpu().numpy()
-            keep, nptr2, roots = pertgraph.clean_span_tables_flat(dict(zip(tracegroup.GATHERED, rows)), new_ptr)
-            empty = np.flatnonzero(np.diff(nptr2) == 0)
-            if empty.size:
-                raise _lib.PertGnnError(f"append_traces: runtime {int(new_ids[empty[0]])}: the row filters "
-                                        "(misc.py:87-105) leave its representative trace without rows")
-            graphs = pertgraph.build_pert_graphs_flat(rows[:len(pertgraph.COLUMNS)][:, keep], nptr2, roots, dev,
-                                                      ing.kind).check()
+            graphs = tracegroup.representative_graphs(new_rows.cpu().numpy(), new_ptr, new_ids, dev, ing.kind,
+                                                      "append_traces: ")
             if int(graphs.edge_attr.shape[1]) != self.attr_cols:
                 raise _lib.PertGnnError(f"append_traces: edge_attr has {int(graphs.edge_attr.shape[1])} columns, the "
                                         f"store {self.attr_cols}")
             g_nptr, g_eptr = (np.asarray(p, dtype=np.int64) for p in (graphs.node_ptr, graphs.edge_ptr))
-        else:
-            g_nptr = g_eptr = np.zeros(1, dtype=np.int64)
         n_nodes, n_edges = ing.n_nodes + int(g_nptr[-1]), ing.n_edges + int(g_eptr[-1])
         n_pairs, n_pc = int(ing.cnt.shape[0]), int(g.pair_runtime.shape[0])
         for what, v in (("pattern nodes", n_nodes), ("pattern edges", n_edges), ("(entry, runtime) pairs",
@@ -842,32 +770,22 @@ class PatternStore:
             if v > _I32_MAX:
                 raise _lib.PertGnnError(f"append_traces: {v} {what} exceed the store's 2^31 - 1")
         t = {}
-        t["pat_nptr"] = torch.cat([self.t["pat_nptr"], torch.from_numpy(g_nptr[1:] + ing.n_nodes).to(dev, i32)])
-        t["pat_eptr"] = torch.cat([self.t["pat_eptr"], torch.from_numpy(g_eptr[1:] + ing.n_edges).to(dev, i32)])
-        if k:
-            ms = graphs.ms_id.reshape(-1).to(dev, i64)
-            ei = graphs.edge_index.to(dev)
-            for name, v in (("pat_ms", ms), ("pat_depth", graphs.node_depth.reshape(-1).to(dev, i64)),
-                            ("pat_last", _last_flags_device(torch.from_numpy(g_nptr).to(dev), ms)),
-                            ("pat_src", ei[0].to(i32)), ("pat_dst", ei[1].to(i32)),
-                            ("pat_attr", graphs.edge_attr.to(dev, i64))):
-                t[name] = torch.cat([self.t[name], v])
+        if k:                                            # the new patterns go after the old ones
+            new = _pattern_arrays(graphs, dev)
+            new["pat_nptr"], new["pat_eptr"] = new["pat_nptr"][1:] + ing.n_nodes, new["pat_eptr"][1:] + ing.n_edges
+            t = {name: torch.cat([self.t[name], v]) for name, v in new.items()}
         # ---- entry mixes (csrc/ingest.cu)
         n_ent_c = int(g.ent_pair_ptr.shape[0]) - 1
         n_ent = max(int(self.desc.n_ent), n_ent_c)
-        mix = _ChunkMix(n_ent_c, n_pc, g.ent_pair_ptr.data_ptr(), g.ent_trace_ptr.data_ptr(),
-                        g.pair_runtime.data_ptr(), g.pair_prob.data_ptr(), g.runtime_ins.data_ptr(), pat_of.data_ptr())
-        o = {"ent_ptr": torch.empty(n_ent + 1, dtype=i32, device=dev),
-             "ent_pat": torch.empty(n_pairs + n_pc, dtype=i32, device=dev),
-             "ent_prob": torch.empty(n_pairs + n_pc, dtype=torch.float32, device=dev),
-             "cnt": torch.empty(n_pairs + n_pc, dtype=i32, device=dev),
-             "ent_nodes": torch.empty(n_ent, dtype=i32, device=dev),
-             "ent_edges": torch.empty(n_ent, dtype=i32, device=dev), "tot": torch.empty(n_ent, dtype=i32, device=dev)}
-        out = _MixOut(*(o[name].data_ptr() for name, _ in _MixOut._fields_))
+        mix = _lib.PertChunkMix(n_ent_c, n_pc, g.ent_pair_ptr.data_ptr(), g.ent_trace_ptr.data_ptr(),
+                                g.pair_runtime.data_ptr(), g.pair_prob.data_ptr(), g.runtime_ins.data_ptr(),
+                                pat_of.data_ptr())
+        o, out = _mix_out(n_ent, n_pairs + n_pc, dev)
         ws = torch.empty(int(L.pert_ingest_merge_workspace_bytes(n_pairs, n_pc, n_ent)), dtype=torch.uint8, device=dev)
+        nptr, eptr = (t.get(name, self.t[name]) for name in ("pat_nptr", "pat_eptr"))
         _lib.check(L.pert_ingest_merge(C.byref(self.desc), ing.cnt.data_ptr(), ing.tot.data_ptr(), n_pairs,
-                                       C.byref(mix), t["pat_nptr"].data_ptr(), t["pat_eptr"].data_ptr(), n_ent,
-                                       C.byref(out), ws.data_ptr(), ws.numel(), _lib.stream()), "pert_ingest_merge")
+                                       C.byref(mix), nptr.data_ptr(), eptr.data_ptr(), n_ent, C.byref(out),
+                                       ws.data_ptr(), ws.numel(), _lib.stream()), "pert_ingest_merge")
         sizes = torch.cat([o["ent_ptr"], o["ent_nodes"], o["ent_edges"]]).long().cpu().numpy()
         ent_ptr_h = sizes[:n_ent + 1]
         n_pairs_out = int(ent_ptr_h[-1])
@@ -876,17 +794,15 @@ class PatternStore:
                   "trace_entry": torch.cat([self.t["trace_entry"], c_ent]),
                   "trace_ts": torch.cat([self.t["trace_ts"], g.bucket[order]]),
                   "trace_y": torch.cat([self.t["trace_y"], g.y[order]])})
-        trace_pat = torch.cat([ing.trace_pat, pat_of[g.runtime_ins[g.runtime[order].long()].long()]])
-        trace_tid = torch.cat([ing.trace_tid, c_tid])
-        # ---- every check passed: swap the new arrays in
-        st = torch.cuda.current_stream()
-        for old in [self.t[name] for name in t] + [ing.rows, ing.ptr, ing.cnt, ing.tot, ing.tids, ing.trace_pat,
-                                                   ing.trace_tid]:
-            old.record_stream(st)                        # the kernels above and earlier assembly on `st` read them
-        for name, v in t.items():
-            self.t[name] = v
-            setattr(self.desc, name, v.data_ptr())
-        self.desc.n_pat, self.desc.n_ent, self.desc.n_traces = n_pat + k, n_ent, T_old + Tc
+        key_rows_old = int(ing.rows.shape[1])
+        self._commit(t, ingest={
+            "rows": torch.cat([ing.rows, new_rows[:3]], dim=1),
+            "ptr": torch.cat([ing.ptr, torch.from_numpy(new_ptr[1:] + key_rows_old).to(dev, i32)]),
+            "cnt": o["cnt"][:n_pairs_out], "tot": o["tot"],
+            "tids": torch.sort(torch.cat([ing.tids, g.trace_id])).values,
+            "trace_pat": torch.cat([ing.trace_pat, pat_of[g.runtime_ins[g.runtime[order].long()].long()]]),
+            "trace_tid": torch.cat([ing.trace_tid, c_tid]), "n_nodes": n_nodes, "n_edges": n_edges,
+            "next_rt": ing.next_rt + k})
         self.rt_ids.extend(int(r) for r in new_ids)
         self.trace_keys.extend(h_tid.tolist())
         self._h_trace_entry = np.concatenate([self._h_trace_entry, h_ent])
@@ -894,13 +810,6 @@ class PatternStore:
         self._h_ent_pats = np.diff(ent_ptr_h)
         self._h_pat_nodes = np.concatenate([self._h_pat_nodes, np.diff(g_nptr)])
         self._h_pat_edges = np.concatenate([self._h_pat_edges, np.diff(g_eptr)])
-        key_rows_old = int(ing.rows.shape[1])
-        ing.rows = torch.cat([ing.rows, new_rows[:3]], dim=1)
-        ing.ptr = torch.cat([ing.ptr, torch.from_numpy(new_ptr[1:] + key_rows_old).to(dev, i32)])
-        ing.cnt, ing.tot = o["cnt"][:n_pairs_out], o["tot"]
-        ing.tids = torch.sort(torch.cat([ing.tids, g.trace_id])).values
-        ing.n_nodes, ing.n_edges = n_nodes, n_edges
-        ing.trace_pat, ing.trace_tid, ing.next_rt = trace_pat, trace_tid, ing.next_rt + k
         if k:
             ing.insert(n_pat, hash_bits)
         return range(T_old, T_old + Tc)
@@ -931,10 +840,7 @@ class PatternStore:
         cut = int(before)
         if not _I64_MIN <= cut <= _I64_MAX:
             raise _lib.PertGnnError(f"evict_traces: before = {cut} is outside int64")
-        ing = getattr(self, "_ingest", None)
-        if ing is None:
-            raise _lib.PertGnnError("evict_traces: this store keeps no runtime keys (it was built from dicts or by "
-                                    "from_graphs); build it with PatternStore.from_trace_groups to evict traces")
+        ing = self._ingest_of("evict_traces")
         dev, L = self.device, _lib.lib()
         i32, i64 = torch.int32, torch.int64
         T, n_pat, n_ent = int(self.desc.n_traces), int(self.desc.n_pat), int(self.desc.n_ent)
@@ -951,17 +857,14 @@ class PatternStore:
         if T2 == T:
             return np.arange(T, dtype=np.int64)
         empty = lambda n, dt: torch.empty(n, dtype=dt, device=dev)            # noqa: E731
-        mix = {"ent_ptr": empty(n_ent + 1, i32), "ent_pat": empty(P2, i32), "ent_prob": empty(P2, torch.float32),
-               "cnt": empty(P2, i32), "ent_nodes": empty(n_ent, i32), "ent_edges": empty(n_ent, i32),
-               "tot": empty(n_ent, i32)}
+        mix, mix_out = _mix_out(n_ent, P2, dev)
         o = {"remap": empty(T, i64), "trace_entry": empty(T2, i32), "trace_ts": empty(T2, i64),
              "trace_y": empty(T2, i64), "trace_pat": empty(T2, i32), "trace_tid": empty(T2, i64),
              "pat_new": empty(n_pat, i32), "pat_nptr": empty(n_pat2 + 1, i32), "pat_eptr": empty(n_pat2 + 1, i32),
              "pat_ms": empty(N2, i64), "pat_depth": empty(N2, i64), "pat_last": empty(N2, torch.uint8),
              "pat_src": empty(E2, i32), "pat_dst": empty(E2, i32), "pat_attr": empty((E2, self.attr_cols), i64),
              "key_ptr": empty(n_pat2 + 1, i32), "key_rows": empty((3, K2), i64)}
-        out = _EvictOut(_MixOut(*(mix[name].data_ptr() for name, _ in _MixOut._fields_)),
-                        *(o[name].data_ptr() for name in _EVICT_ARRAYS), K2)
+        out = _lib.PertEvictOut(mix_out, *(o[name].data_ptr() for name in _lib.EVICT_ARRAYS), K2)
         _lib.check(L.pert_ingest_evict_apply(C.byref(self.desc), C.byref(state), (C.c_longlong * 6)(*sizes),
                                              ws.data_ptr(), ws.numel(), C.byref(out), _lib.stream()),
                    "pert_ingest_evict_apply")
@@ -969,20 +872,15 @@ class PatternStore:
                           mix["ent_nodes"].long(), mix["ent_edges"].long()]).cpu().numpy()
         remap, h_ent, pat_new, ent_ptr_h, h_nodes, h_edges = np.split(host, np.cumsum([T, T2, n_pat, n_ent + 1, n_ent]))
         tids = torch.sort(o["trace_tid"]).values
-        # ---- swap the new arrays in
         t = {"pat_nptr": o["pat_nptr"], "pat_eptr": o["pat_eptr"], "pat_ms": o["pat_ms"], "pat_depth": o["pat_depth"],
              "pat_last": o["pat_last"], "pat_src": o["pat_src"], "pat_dst": o["pat_dst"], "pat_attr": o["pat_attr"],
              "ent_ptr": mix["ent_ptr"], "ent_pat": mix["ent_pat"], "ent_prob": mix["ent_prob"],
              "ent_nodes": mix["ent_nodes"], "ent_edges": mix["ent_edges"], "trace_entry": o["trace_entry"],
              "trace_ts": o["trace_ts"], "trace_y": o["trace_y"]}
-        st = torch.cuda.current_stream()
-        for old in [self.t[name] for name in t] + [ing.rows, ing.ptr, ing.cnt, ing.tot, ing.tids, ing.trace_pat,
-                                                   ing.trace_tid]:
-            old.record_stream(st)                        # the kernels above and earlier assembly on `st` read them
-        for name, v in t.items():
-            self.t[name] = v
-            setattr(self.desc, name, v.data_ptr())
-        self.desc.n_pat, self.desc.n_traces = n_pat2, T2
+        self._commit(t, ingest={"rows": o["key_rows"], "ptr": o["key_ptr"], "cnt": mix["cnt"], "tot": mix["tot"],
+                                "tids": tids, "trace_pat": o["trace_pat"], "trace_tid": o["trace_tid"], "n_nodes": N2,
+                                "n_edges": E2})
+        ing.table = None                                 # it holds pattern indices: the next append rebuilds it
         self.rt_ids = [r for r, p in zip(self.rt_ids, pat_new) if p >= 0]
         # the surviving keys in order: a C-level filter of the list, several times faster than a list of the device
         # traceids (no new int objects)
@@ -990,10 +888,16 @@ class PatternStore:
         self._h_trace_entry, self._h_ent_nodes, self._h_ent_edges = h_ent, h_nodes, h_edges
         self._h_ent_pats = np.diff(ent_ptr_h)
         self._h_pat_nodes, self._h_pat_edges = self._h_pat_nodes[pat_new >= 0], self._h_pat_edges[pat_new >= 0]
-        ing.rows, ing.ptr, ing.cnt, ing.tot, ing.tids = o["key_rows"], o["key_ptr"], mix["cnt"], mix["tot"], tids
-        ing.trace_pat, ing.trace_tid, ing.n_nodes, ing.n_edges = o["trace_pat"], o["trace_tid"], N2, E2
-        ing.table = None                                 # it holds pattern indices: the next append rebuilds it
         return remap
+
+    def _ingest_of(self, fn):
+        """``_ingest``, or ``PertGnnError`` for ``fn`` when the store keeps no runtime keys."""
+        ing = getattr(self, "_ingest", None)
+        if ing is None:
+            raise _lib.PertGnnError(f"{fn}: this store keeps no runtime keys (it was built from dicts or by "
+                                    "from_graphs); build it with PatternStore.from_trace_groups to "
+                                    f"{fn.replace('_', ' ')}")
+        return ing
 
     def __len__(self):
         return len(self.trace_keys)
@@ -1025,7 +929,7 @@ class PatternStore:
         if not label:
             del out["y"]
         offsets = torch.empty(3 * (B + 1), dtype=torch.int32, device=dev)
-        o = _PertBatchOut()
+        o = _lib.PertBatchOut()
         for k, v in out.items():
             setattr(o, k, v.data_ptr())
         launch(offsets.data_ptr(), C.byref(o))

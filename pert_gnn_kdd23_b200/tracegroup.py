@@ -20,17 +20,8 @@ from . import pertgraph
 COLUMNS = ("traceid", "timestamp", "rpcid", "um", "dm", "interface", "rpctype", "rt", "entryid")
 GATHERED = pertgraph.COLUMNS + ("rpcid", "rt")          # row order of pert_trace_group_gather's output
 
-P = C.c_void_p
-
-
-class _SpanTable(C.Structure):
-    _fields_ = [("R", C.c_longlong)] + [(k, P) for k in COLUMNS]
-
-
-class _Groups(C.Structure):
-    _fields_ = [(k, P) for k in ("row_ptr", "perm", "trace_id", "bucket", "y", "entry", "runtime", "order",
-                                 "ent_trace_ptr", "ent_pair_ptr", "pair_runtime", "pair_prob", "occurrences",
-                                 "ins_runtime", "rep_trace", "runtime_ins", "rep_ptr", "sizes")]
+# the C structs under the names this module has always exported (the mirrors themselves live in _lib)
+_SpanTable, _Groups = _lib.PertSpanTable, _lib.PertTraceGroups
 
 
 class TraceGroups:
@@ -92,19 +83,25 @@ class TraceGroups:
     def graphs(self, kind="pert"):
         """-> (PertGraphs, runtime_ids): the graphs of runtime2{kind}graph_map in insertion order, built from the
         representatives' rows by the host row filters (pertgraph.clean_span_tables_flat, misc.py:87-105, :138-142) and
-        the CUDA graph builder.  A representative whose rows are all removed by the filters raises PertGnnError (the
-        reference fails on edge_index.max() of an empty tensor)."""
+        the CUDA graph builder (``representative_graphs``)."""
         rows, rep_ptr = self.representative_rows()
-        cols = dict(zip(GATHERED, rows))
-        keep, new_ptr, roots = pertgraph.clean_span_tables_flat(cols, rep_ptr)
         ids = self.ins_runtime.cpu().numpy().astype(np.int64)
-        empty = np.flatnonzero(np.diff(new_ptr) == 0)
-        if empty.size:
-            raise _lib.PertGnnError(f"runtime {int(ids[empty[0]])}: the row filters (misc.py:87-105) leave its "
-                                    "representative trace without rows")
-        flat = rows[:len(pertgraph.COLUMNS)][:, keep]
-        g = pertgraph.build_pert_graphs_flat(flat, new_ptr, roots, self.trace_id.device, kind).check()
-        return g, [int(r) for r in ids]
+        return representative_graphs(rows, rep_ptr, ids, self.trace_id.device, kind), [int(r) for r in ids]
+
+
+def representative_graphs(rows, rep_ptr, runtime_ids, device, kind, prefix=""):
+    """-> the checked PertGraphs of representative traces: ``rows`` host int64 [8, R'] (GATHERED), representative k
+    owning rows rep_ptr[k] .. rep_ptr[k+1]-1, through the host row filters (pertgraph.clean_span_tables_flat,
+    misc.py:87-105, :138-142) and the CUDA graph builder.  A representative whose rows are all removed by the filters
+    raises PertGnnError naming its runtime id ``runtime_ids[k]``, after ``prefix`` (the reference fails on
+    edge_index.max() of an empty tensor)."""
+    keep, new_ptr, roots = pertgraph.clean_span_tables_flat(dict(zip(GATHERED, rows)), rep_ptr)
+    empty = np.flatnonzero(np.diff(new_ptr) == 0)
+    if empty.size:
+        raise _lib.PertGnnError(f"{prefix}runtime {int(runtime_ids[empty[0]])}: the row filters (misc.py:87-105) leave "
+                                "its representative trace without rows")
+    return pertgraph.build_pert_graphs_flat(rows[:len(pertgraph.COLUMNS)][:, keep], new_ptr, roots, device,
+                                            kind).check()
 
 
 def _column(v, dev):
@@ -130,7 +127,7 @@ def group_traces(columns, device="cuda", hash_bits=64):
             raise _lib.PertGnnError("group_traces: the span table is empty")
         if any(int(c.shape[0]) != R for c in cols.values()):
             raise ValueError("group_traces: columns of different lengths")
-        tab = _SpanTable(R, *(cols[k].data_ptr() for k in COLUMNS))
+        tab = _lib.PertSpanTable(R, **{k: cols[k].data_ptr() for k in COLUMNS})
         st = _lib.stream()
         L = _lib.lib()
         i32 = dict(dtype=torch.int32, device=dev)
@@ -161,7 +158,7 @@ def group_traces(columns, device="cuda", hash_bits=64):
              "occurrences": torch.empty(T, **i32), "ins_runtime": torch.empty(T, **i32),
              "rep_trace": torch.empty(T, **i32), "runtime_ins": torch.empty(T, **i32),
              "rep_ptr": torch.empty(T + 1, **i32), "sizes": torch.empty(3, **i64)}
-        out = _Groups(*(t[k].data_ptr() for k, _ in _Groups._fields_))
+        out = _lib.PertTraceGroups(*(t[k].data_ptr() for k, _ in _lib.PertTraceGroups._fields_))
         _lib.check(L.pert_trace_group_build(C.byref(tab), n_keys, T, n_ent, int(hash_bits), key_ptr.data_ptr(),
                                             key_trace.data_ptr(), C.byref(out), ws.data_ptr(), ws.numel(),
                                             status.data_ptr(), st), "pert_trace_group_build")

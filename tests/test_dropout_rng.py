@@ -63,7 +63,7 @@ def test_mask_layout():
 
 
 def _desc(H=64):
-    from pert_gnn_kdd23_b200.engine import PertModelDesc
+    from pert_gnn_kdd23_b200._lib import PertModelDesc
 
     d = PertModelDesc()
     d.F, d.H, d.n_convs, d.n_cat = 9, H, 3, 1

@@ -138,7 +138,7 @@ def test_bad_requests():
     import ctypes as C
 
     from pert_gnn_kdd23_b200 import _lib, ops
-    from pert_gnn_kdd23_b200.store import _PertBatchOut
+    from pert_gnn_kdd23_b200._lib import PertBatchOut
 
     store, empty = _store_with_an_empty_entry()
     n_ent = empty + 2
@@ -154,7 +154,7 @@ def test_bad_requests():
     ts = np.array([60000, 60000, 90000, 120000], dtype=np.int64)
     like = store.assemble_requests([1, 0, 0, 0], ts, asof=True)
     out = {k: torch.full_like(like[k], 7) for k in OUT_KEYS}
-    o = _PertBatchOut()
+    o = PertBatchOut()
     for k, v in out.items():
         setattr(o, k, v.data_ptr())
     offsets = torch.empty(3 * 5, dtype=torch.int32, device="cuda")

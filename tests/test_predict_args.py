@@ -113,21 +113,21 @@ def test_bad_entry_ids_are_rejected_on_the_host():
 
 
 def _store_desc():
-    from pert_gnn_kdd23_b200.store import _PertStore
+    from pert_gnn_kdd23_b200._lib import PertStore
 
-    d = _PertStore()
+    d = PertStore()
     d.n_pat, d.n_ent, d.n_res, d.n_ms, d.attr_cols, d.n_traces = 2, 2, 3, 4, 2, 0
-    for name, _ in _PertStore._fields_[6:]:
+    for name, _ in PertStore._fields_[6:]:
         setattr(d, name, 1)                                   # non-NULL, never dereferenced on the host
     return d
 
 
 def _req_args(**over):
     from pert_gnn_kdd23_b200._lib import PertResourceAsOf
-    from pert_gnn_kdd23_b200.store import _PertBatchOut
+    from pert_gnn_kdd23_b200._lib import PertBatchOut
 
     a = dict(store=C.byref(_store_desc()), asof=None, entry_ids=1, timestamps=1, B=2, N=10, E=20, offsets=1,
-             out=C.byref(_PertBatchOut()), status=None, stream=None)
+             out=C.byref(PertBatchOut()), status=None, stream=None)
     if over.pop("with_asof", False):
         a["asof"] = C.byref(PertResourceAsOf(1, 1, 1))
     a.update(over)

@@ -81,13 +81,14 @@ class _FakeLib:
 def _host_store(n_ms=48, n_res=6):
     """A store whose arrays live in host memory: enough for every check that runs before a launch."""
     from pert_gnn_kdd23_b200 import _lib
-    from pert_gnn_kdd23_b200.store import PatternStore, _PertStore
+    from pert_gnn_kdd23_b200._lib import PertStore
+    from pert_gnn_kdd23_b200.store import PatternStore
 
     s = PatternStore.__new__(PatternStore)
     s.device, s.n_ms = torch.device("cpu"), n_ms
     keys = torch.arange(n_res, dtype=torch.int64) * n_ms
     s.t = {"res_keys": keys, "res_vals": torch.rand(n_res, 8), "ms_has_res": torch.zeros(n_ms, dtype=torch.uint8)}
-    s.desc = _PertStore()
+    s.desc = PertStore()
     s.desc.n_res, s.desc.n_ms = n_res, n_ms
     for k, v in s.t.items():
         setattr(s.desc, k, v.data_ptr())
@@ -178,11 +179,11 @@ def test_too_many_rows_are_rejected_after_the_count(monkeypatch):
 # --------------------------------------------------------------------------------------------- C-ABI argument checks
 def _descs(n_res=3, n_ms=4):
     from pert_gnn_kdd23_b200._lib import PertResourceAsOf
-    from pert_gnn_kdd23_b200.store import _PertStore
+    from pert_gnn_kdd23_b200._lib import PertStore
 
-    d = _PertStore()
+    d = PertStore()
     d.n_res, d.n_ms = n_res, n_ms
-    for name, _ in _PertStore._fields_[6:]:
+    for name, _ in PertStore._fields_[6:]:
         setattr(d, name, 16)                           # non-NULL and aligned, never dereferenced on the host
     return d, PertResourceAsOf(16, 16, 16)
 

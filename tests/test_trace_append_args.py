@@ -124,15 +124,15 @@ def test_stores_without_runtime_keys_refuse():
 
 
 def _keys(n=2, ld=4, ptr=1, rows=1):
-    from pert_gnn_kdd23_b200.store import _RuntimeKeys
+    from pert_gnn_kdd23_b200._lib import PertRuntimeKeys
 
-    return _RuntimeKeys(n, ld, ptr, rows)
+    return PertRuntimeKeys(n, ld, ptr, rows)
 
 
 def _table(S=64, bits=64, slot=1, h=1):
-    from pert_gnn_kdd23_b200.store import _RuntimeTable
+    from pert_gnn_kdd23_b200._lib import PertRuntimeTable
 
-    return _RuntimeTable(S, bits, slot, h, h)
+    return PertRuntimeTable(S, bits, slot, h, h)
 
 
 @pytest.mark.parametrize("over", [dict(keys=None), dict(first=-1), dict(first=3), dict(table=_table(S=48)),
@@ -164,9 +164,9 @@ def test_match_rejects_bad_arguments(over):
 
 
 def _mix(n_ent=3, n_pairs=4, ptr=1):
-    from pert_gnn_kdd23_b200.store import _ChunkMix
+    from pert_gnn_kdd23_b200._lib import PertChunkMix
 
-    return _ChunkMix(n_ent, n_pairs, ptr, 1, 1, 1, 1, 1)
+    return PertChunkMix(n_ent, n_pairs, ptr, 1, 1, 1, 1, 1)
 
 
 @pytest.mark.parametrize("over", [dict(store=None), dict(chunk=None), dict(out=None), dict(ws=None),
@@ -175,13 +175,13 @@ def _mix(n_ent=3, n_pairs=4, ptr=1):
                                   dict(tot=None), dict(nptr=None), dict(n_pairs=1 << 31)])
 def test_merge_rejects_bad_arguments(over):
     from pert_gnn_kdd23_b200 import _lib
-    from pert_gnn_kdd23_b200.store import _MixOut, _PertStore
+    from pert_gnn_kdd23_b200._lib import PertMixOut, PertStore
 
-    s = _PertStore()
+    s = PertStore()
     s.n_ent = 2
     for f in ("ent_ptr", "ent_pat", "ent_nodes", "ent_edges"):
         setattr(s, f, 1)
-    a = dict(store=s, cnt=1, tot=1, n_pairs=5, chunk=_mix(), nptr=1, n_ent_out=3, out=_MixOut(*([1] * 7)), ws=1,
+    a = dict(store=s, cnt=1, tot=1, n_pairs=5, chunk=_mix(), nptr=1, n_ent_out=3, out=PertMixOut(*([1] * 7)), ws=1,
              ws_bytes=1 << 20)
     a.update(over)
     ref = lambda x: C.byref(x) if x is not None else None                # noqa: E731

@@ -143,20 +143,20 @@ def test_stores_without_runtime_keys_refuse():
 
 # ---- C-ABI argument checks --------------------------------------------------------------------------------------------
 def _store(T=4, n_pat=2, n_ent=3):
-    from pert_gnn_kdd23_b200.store import _PertStore
+    from pert_gnn_kdd23_b200._lib import PertStore
 
-    s = _PertStore()
+    s = PertStore()
     s.n_traces, s.n_pat, s.n_ent, s.attr_cols = T, n_pat, n_ent, 2
-    for f, _ in _PertStore._fields_:
+    for f, _ in PertStore._fields_:
         if f not in ("n_pat", "n_ent", "n_res", "n_ms", "attr_cols", "n_traces"):
             setattr(s, f, 1)
     return s
 
 
 def _state(n_pat=2, pairs=5, ptr=1, trace_pat=1, cnt=1, tot=1, tid=1, key_rows=6):
-    from pert_gnn_kdd23_b200.store import _IngestState, _RuntimeKeys
+    from pert_gnn_kdd23_b200._lib import PertIngestState, PertRuntimeKeys
 
-    return _IngestState(_RuntimeKeys(n_pat, 8, ptr, 1), trace_pat, tid, cnt, tot, pairs, 10, 12, key_rows)
+    return PertIngestState(PertRuntimeKeys(n_pat, 8, ptr, 1), trace_pat, tid, cnt, tot, pairs, 10, 12, key_rows)
 
 
 WS = 1 << 20
@@ -188,10 +188,10 @@ def test_evict_workspace_bytes_rejects_bad_sizes():
 
 
 def _out(**null):
-    from pert_gnn_kdd23_b200.store import _EVICT_ARRAYS, _EvictOut, _MixOut
+    from pert_gnn_kdd23_b200._lib import EVICT_ARRAYS, PertEvictOut, PertMixOut
 
-    mix = _MixOut(*[0 if null.get(k) else 1 for k, _ in _MixOut._fields_])
-    return _EvictOut(mix, *[0 if null.get(k) else 1 for k in _EVICT_ARRAYS], null.get("key_ld", 8))
+    mix = PertMixOut(*[0 if null.get(k) else 1 for k, _ in PertMixOut._fields_])
+    return PertEvictOut(mix, *[0 if null.get(k) else 1 for k in EVICT_ARRAYS], null.get("key_ld", 8))
 
 
 @pytest.mark.parametrize("over", [dict(store=None), dict(ing=None), dict(ws=None), dict(out=None), dict(sizes=None),

@@ -69,31 +69,31 @@ def test_oracle_rejects_a_trace_under_two_entries():
 
 def test_trace_group_abi_rejects_bad_arguments_before_cuda():
     from pert_gnn_kdd23_b200 import _lib
-    from pert_gnn_kdd23_b200.tracegroup import _Groups, _SpanTable
+    from pert_gnn_kdd23_b200._lib import PertSpanTable, PertTraceGroups
 
     L = _lib.lib()
     word = ctypes.c_int(0)
     status = ctypes.addressof(word)                       # never written: the calls must return before any CUDA call
-    tab = _SpanTable(-1, *([None] * 9))
+    tab = PertSpanTable(-1, *([None] * 9))
     assert L.pert_trace_group_range(None, status, status, None) == -1
     assert L.pert_trace_group_range(ctypes.byref(tab), status, status, None) == -1                 # R < 0
-    tab = _SpanTable(10, *([None] * 9))
+    tab = PertSpanTable(10, *([None] * 9))
     assert L.pert_trace_group_range(ctypes.byref(tab), status, status, None) == -1                 # NULL columns
-    ok = _SpanTable(0, *([None] * 9))
+    ok = PertSpanTable(0, *([None] * 9))
     assert L.pert_trace_group_range(ctypes.byref(ok), None, status, None) == -1
     assert L.pert_trace_group_keys(ctypes.byref(ok), -1, status, status, status, 1 << 20, None) == -1
     assert L.pert_trace_group_keys(ctypes.byref(ok), 4, None, status, status, 1 << 20, None) == -1
     assert L.pert_trace_group_workspace_bytes(-1, 0, 0, 0) == -1
     assert L.pert_trace_group_workspace_bytes(10, 5, 11, 1) == -1                                    # T > R
     assert L.pert_trace_group_workspace_bytes(10, 5, 4, 2) > 0
-    out = _Groups(*([None] * len(_Groups._fields_)))
-    rows = _SpanTable(10, *([status] * 9))                 # plausible pointers: only the tested argument is wrong
+    out = PertTraceGroups(*([None] * len(PertTraceGroups._fields_)))
+    rows = PertSpanTable(10, *([status] * 9))             # plausible pointers: only the tested argument is wrong
 
     def build(o=out, n_keys=5, T=4, n_ent=2, bits=64, ws=1 << 30):
         return L.pert_trace_group_build(ctypes.byref(rows), n_keys, T, n_ent, bits, status, status, ctypes.byref(o),
                                         status, ws, status, None)
     assert build() == -1                                                                             # NULL outputs
-    full = _Groups(*([status] * len(_Groups._fields_)))
+    full = PertTraceGroups(*([status] * len(PertTraceGroups._fields_)))
     assert build(full, T=-1) == -1 and build(full, n_ent=-1) == -1 and build(full, n_keys=-1) == -1
     assert build(full, bits=0) == -1 and build(full, bits=65) == -1 and build(full, ws=16) == -1
     assert L.pert_trace_group_gather(ctypes.byref(rows), status, status, status, status, -1, 0, status, None) == -1

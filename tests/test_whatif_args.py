@@ -196,11 +196,11 @@ def test_device_arrays_of_a_plain_call_are_refused_with_what_if_inputs():
 
 # ------------------------------------------------------------------------------------------------ C-ABI checks
 def _store_desc():
-    from pert_gnn_kdd23_b200.store import _PertStore
+    from pert_gnn_kdd23_b200._lib import PertStore
 
-    d = _PertStore()
+    d = PertStore()
     d.n_pat, d.n_ent, d.n_res, d.n_ms, d.attr_cols, d.n_traces = 2, 2, 3, 4, 2, 0
-    for name, _ in _PertStore._fields_[6:]:
+    for name, _ in PertStore._fields_[6:]:
         setattr(d, name, 16)                                  # non-NULL, never dereferenced on the host
     return d
 
@@ -215,10 +215,10 @@ def _whatif(**over):
 
 def _args(**over):
     from pert_gnn_kdd23_b200._lib import PertResourceAsOf
-    from pert_gnn_kdd23_b200.store import _PertBatchOut
+    from pert_gnn_kdd23_b200._lib import PertBatchOut
 
     a = dict(store=C.byref(_store_desc()), asof=None, w=C.byref(_whatif()), entry_ids=16, timestamps=16, B=2, N=10,
-             E=20, offsets=16, out=C.byref(_PertBatchOut()), status=None, stream=None)
+             E=20, offsets=16, out=C.byref(PertBatchOut()), status=None, stream=None)
     if over.pop("with_asof", False):
         a["asof"] = C.byref(PertResourceAsOf(16, 16, 16))
     a.update(over)

@@ -16,7 +16,7 @@ def width_rule(H):
 
 
 def _desc(H, k0_width=None):
-    from pert_gnn_kdd23_b200.engine import PertModelDesc
+    from pert_gnn_kdd23_b200._lib import PertModelDesc
 
     d = PertModelDesc()
     d.F, d.H, d.n_convs, d.n_cat = F, H, L, len(CAT_ROWS)

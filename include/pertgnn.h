@@ -51,7 +51,7 @@ extern "C" {
  * pert_store_assemble_requests (request assembly with the exact or as-of resource join); pert_store_resources_count /
  * _merge (appending and evicting resource rows of a live store); pert_ingest_* (appending traces to a live store);
  * pert_ingest_evict_* (evicting traces from a live store); pert_store_assemble_whatif (per-request pattern mixes and
- * resource overrides), pert_store_lookup_resources. */
+ * resource overrides), pert_store_lookup_resources; pert_raw_* (processed tables from raw rows). */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -762,6 +762,68 @@ int pert_trace_group_build(const PertSpanTable* table, long long n_keys, long lo
  * representatives' rows, representative k at rep_ptr[k], file order inside it. */
 int pert_trace_group_gather(const PertSpanTable* table, const int* perm, const int* row_ptr, const int* rep_trace,
                             const int* rep_ptr, long long n_runtimes, long long R_rep, int64_t* rows, void* stream);
+
+/* ---- raw tables: the processed span and resource tables from raw rows (csrc/rawtable.cu) ---------------------------
+ * Replaces the else-branch of preprocess.py get_df() (:201-261) after the CSV read: drop_duplicates (:212), the sort by
+ * timestamp (:213), map_consecutive_ids of traceid / interface / entryid / rpcid / rpctype (:216-221), the entry
+ * detection of filter_traces_with_missing_entry_and_get_delay (:99-149), the resource-coverage filter (:155-177), the
+ * per-entry occurrence filter (:180-188), the microservice ids (:248-254) and the resource groupby(["timestamp",
+ * "msname"]).agg([max, min, mean, median]) (:227-242).
+ * Input: dictionary-encoded device columns.  Every call-graph column but timestamp and rt holds codes into a host
+ * dictionary of n_* entries; um, dm and the resource msname share ONE dictionary whose codes are in lexicographic name
+ * order.  A row with a code outside its dictionary sets PERT_ERR_RANGE in status and is left out.  At most 2^30
+ * call-graph rows and traceid codes (every hash-table slot is an int32), else PERT_ERR_BADARG.  The calls, in order
+ * (the caller reads a size between them):
+ *   pert_raw_resource_groups -> groups of the resource rows sorted (stable) by (timestamp, ms), has_res[n_ms] => G
+ *   pert_raw_resource_stats  -> vals[G, 8]: cpu max, min, mean, median, memory max, min, mean, median (pandas' NaN
+ *                               skipping group_max / group_min / Kahan group_mean / median, bit for bit)
+ *   pert_raw_dedup           -> rows[n_kept] (the first of every set of equal rows, concatenation order) and their
+ *                               timestamps keys[n_kept]                         => n_kept; the caller sorts keys stably
+ *   pert_raw_process         -> sizes[7] = {M rows, n_ms ids, traceid, interface, entryid, rpcid, rpctype codes}
+ *   pert_raw_emit            -> the nine processed columns [M], res_index[G, 2] = (timestamp, ms id) and the code
+ *                               dictionaries of PertRawOut.
+ * Codes count from 0 by first appearance in sorted order (Series.factorize); entryid / rpcid / rpctype over the rows of
+ * traces with an entry, so later filters leave gaps as in the reference.  Microservice ids number the union of the
+ * surviving um / dm and every resource msname in dictionary (lexicographic) order; the reference numbers that set in
+ * Python set order, which is hash-randomised.  The duplicate table compares rows column by column before merging, so
+ * a hash collision costs time and never a wrong merge; hash_bits (1..64) is 64 except in tests.  Outputs do not depend
+ * on thread scheduling. */
+typedef struct PertRawCalls {
+  long long R;                                         /* rows, concatenation order                         */
+  long long n_trace, n_iface, n_rpcid, n_rpctype, n_ms; /* dictionary sizes                                 */
+  long long http, unknown;                             /* codes of rpctype "http" and microservice "(?)", -1: none */
+  const int64_t *traceid, *timestamp, *rpcid, *um, *rpctype, *dm, *interface, *rt;
+} PertRawCalls;
+/* Outputs of pert_raw_emit, all int64, sized by pert_raw_process's sizes[] (and G). */
+typedef struct PertRawOut {
+  int64_t *traceid, *timestamp, *rpcid, *um, *dm, *interface, *rpctype, *rt, *entryid;   /* [M] processed rows   */
+  int64_t *row;                                        /* [M] concatenation index of every processed row */
+  int64_t *res_index;                                  /* [G, 2] (timestamp, ms id)                          */
+  int64_t *ms_code;                                    /* [n_ms ids] dictionary code of every ms id          */
+  int64_t *tr_code, *if_code, *rpc_code, *rty_code;    /* dictionary code of every traceid / interface / rpcid / rpctype id */
+  int64_t *ent_dm, *ent_if;                            /* [entryid ids] the entry's dm code and interface id  */
+} PertRawOut;
+long long pert_raw_resource_workspace_bytes(long long K);
+/* K resource rows ts / ms, perm[K] = row at sorted position, rows with an ms outside [0, n_ms) after all others (they
+ * set PERT_ERR_RANGE and join no group); gflag[K+1], gptr[K+1], g_ts[K], g_ms[K] (group g: positions gptr[g] ..
+ * gptr[g+1], key (g_ts, g_ms)), n_groups[1] = G; has_res[n_ms] = ms has a row. */
+int pert_raw_resource_groups(long long K, const int64_t* ts, const int64_t* ms, const int64_t* perm, long long n_ms,
+                             int* gflag, int* has_res, int* gptr, int64_t* g_ts, int64_t* g_ms, int64_t* n_groups,
+                             void* workspace, long long workspace_bytes, int* status, void* stream);
+/* cpu / mem [K] by row; cpu_sorted / mem_sorted [K]: every group's values ascending (NaN last) at its positions. */
+int pert_raw_resource_stats(long long G, const int64_t* perm, const int* gptr, const double* cpu, const double* mem,
+                            const double* cpu_sorted, const double* mem_sorted, double* vals, void* stream);
+long long pert_raw_dedup_workspace_bytes(long long R);
+int pert_raw_dedup(const PertRawCalls* calls, int hash_bits, int* rows, int64_t* keys, int64_t* n_kept,
+                   void* workspace, long long workspace_bytes, int* status, void* stream);
+/* workspace of pert_raw_process and pert_raw_emit (one buffer, passed to both); order[N] = row at sorted position */
+long long pert_raw_process_workspace_bytes(const PertRawCalls* calls, long long N);
+int pert_raw_process(const PertRawCalls* calls, long long N, const int64_t* order, const int* has_res,
+                     long long min_occurence, int64_t* sizes, void* workspace, long long workspace_bytes,
+                     void* stream);
+int pert_raw_emit(const PertRawCalls* calls, long long N, const int64_t* order, long long G, const int64_t* g_ts,
+                  const int64_t* g_ms, const PertRawOut* out, void* workspace, long long workspace_bytes,
+                  void* stream);
 
 #ifdef __cplusplus
 }

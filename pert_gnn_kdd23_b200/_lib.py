@@ -94,6 +94,15 @@ SIGNATURES = {
     "pert_trace_group_workspace_bytes": (LL, [LL, LL, LL, LL]),
     "pert_trace_group_build": (I, [P, LL, LL, LL, I, P, P, P, P, LL, P, P]),
     "pert_trace_group_gather": (I, [P, P, P, P, P, LL, LL, P, P]),
+    # processed tables from raw rows (rawtable.py; PertRawCalls* / PertRawOut* arguments)
+    "pert_raw_resource_workspace_bytes": (LL, [LL]),
+    "pert_raw_resource_groups": (I, [LL, P, P, P, LL, P, P, P, P, P, P, P, LL, P, P]),
+    "pert_raw_resource_stats": (I, [LL, P, P, P, P, P, P, P, P]),
+    "pert_raw_dedup_workspace_bytes": (LL, [LL]),
+    "pert_raw_dedup": (I, [P, I, P, P, P, P, LL, P, P]),
+    "pert_raw_process_workspace_bytes": (LL, [P, LL]),
+    "pert_raw_process": (I, [P, LL, P, P, LL, P, P, LL, P]),
+    "pert_raw_emit": (I, [P, LL, P, LL, P, P, P, P, LL, P]),
     # whole-model engine (first argument: const PertModelDesc*, see engine.py)
     "pert_model_width": (I, [I]),
     "pert_model_workspace_bytes": (LL, [P, LL, LL, LL]),
@@ -205,6 +214,19 @@ class PertTraceGroups(C.Structure):
     _fields_ = [(k, P) for k in ("row_ptr", "perm", "trace_id", "bucket", "y", "entry", "runtime", "order",
                                  "ent_trace_ptr", "ent_pair_ptr", "pair_runtime", "pair_prob", "occurrences",
                                  "ins_runtime", "rep_trace", "runtime_ins", "rep_ptr", "sizes")]
+
+
+class PertRawCalls(C.Structure):
+    _fields_ = [(k, LL) for k in ("R", "n_trace", "n_iface", "n_rpcid", "n_rpctype", "n_ms", "http", "unknown")] + \
+        [(k, P) for k in ("traceid", "timestamp", "rpcid", "um", "rpctype", "dm", "interface", "rt")]
+
+
+RAW_OUT = ("traceid", "timestamp", "rpcid", "um", "dm", "interface", "rpctype", "rt", "entryid", "row", "res_index",
+           "ms_code", "tr_code", "if_code", "rpc_code", "rty_code", "ent_dm", "ent_if")
+
+
+class PertRawOut(C.Structure):
+    _fields_ = [(k, P) for k in RAW_OUT]
 
 
 def lib():

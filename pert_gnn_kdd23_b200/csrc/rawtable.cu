@@ -1,0 +1,603 @@
+// Raw call-graph and resource rows -> the processed span and resource tables: the else-branch of the reference's
+// preprocess.py get_df() (:191-266) on dictionary-encoded columns.
+//
+// The host reads the CSV files and gives every string (and every rpcid value) a dictionary code; everything after that
+// is integer and float work over the whole table, restated here step by step:
+//   1. drop_duplicates (:212): an open-addressing table over a 64-bit row hash; a slot matches only after a column-by-
+//      column comparison with its owner, so a collision costs a comparison and never merges two rows.  atomicMin of the
+//      row index per slot keeps the first row in concatenation order;
+//   2. sort_values("timestamp") (:213): done by the caller as a stable sort of the kept rows' timestamps (ties keep
+//      concatenation order); ``order`` maps sorted position -> row;
+//   3. map_consecutive_ids (:216-221): for every dictionary code, atomicMin of its first position, then a scan of the
+//      "first position" flags numbers the codes by first appearance (Series.factorize).  traceid and interface over the
+//      whole sorted table, entryid / rpcid / rpctype over the rows of traces that keep an entry, so the later filters
+//      leave gaps in the codes exactly as in the reference;
+//   4. filter_traces_with_missing_entry_and_get_delay (:99-149): per trace (atomics on its dictionary code) the minimum
+//      timestamp is the timestamp at its first sorted position, max |rt| an atomicMax; candidates are the http rows at
+//      that timestamp with that |rt|; one candidate is the entry, several are narrowed to um == "(?)" and kept only if
+//      exactly one is left.  The entry key (dm, interface code) is factorised through a second hash table;
+//   5. filter_traces_with_missing_features (:155-177): the distinct {um, dm} of a trace are the first claims of
+//      (trace, ms) pairs in a third table; kept iff (double) resourced / (double) distinct >= 0.6;
+//   6. filter_traces_by_occurence_per_entry (:180-188): traces surviving 5 counted per entry, kept iff > min_occurence;
+//   7. microservice ids (:248-254): the union of the surviving um / dm and every resource msname, numbered by a scan of
+//      presence flags over the dictionary, whose codes are in lexicographic name order;
+//   8. compaction of the surviving rows into the nine processed columns;
+//   9. the resource groupby(["timestamp", "msname"]).agg([max, min, mean, median]) (:227-242): a thread per group walks
+//      its rows in concatenation order (the caller's stable key sort) with pandas' group_max / group_min / group_mean
+//      (Kahan-compensated sum over the non-NaN count) and reads the median from the caller's per-group value sort.
+// Every atomic is a min, a max, an add or a slot claim whose winner changes no output, so results do not depend on
+// scheduling.
+#include "common.cuh"
+#include "rowhash.cuh"
+#include "scan.cuh"
+
+#include <algorithm>
+
+namespace {
+
+constexpr int RW_NONE = 0x7f7f7f7f;                     // "no position yet": the 0x7f byte fill of every atomicMin
+constexpr long long RW_MAX_ROWS = 1LL << 30;            // rows and traceids: every table slot fits an int
+constexpr unsigned long long RW_NOKEY = ~0ull;
+constexpr unsigned long long RW_SEED = 0x452821e638d01377ull;
+
+__device__ __forceinline__ bool in_dict(int64_t v, long long n) { return v >= 0 && v < n; }
+
+__device__ __forceinline__ bool codes_ok(const PertRawCalls& c, long long r) {
+  return in_dict(c.traceid[r], c.n_trace) && in_dict(c.interface[r], c.n_iface) && in_dict(c.rpcid[r], c.n_rpcid) &&
+         in_dict(c.rpctype[r], c.n_rpctype) && in_dict(c.um[r], c.n_ms) && in_dict(c.dm[r], c.n_ms);
+}
+
+__device__ __forceinline__ unsigned long long row_hash(const PertRawCalls& c, long long r) {
+  unsigned long long h = mix64(RW_SEED ^ (unsigned long long)c.traceid[r]);
+  h = mix64(h ^ (unsigned long long)c.timestamp[r]);
+  h = mix64(h ^ (unsigned long long)c.rpcid[r]);
+  h = mix64(h ^ (unsigned long long)c.um[r]);
+  h = mix64(h ^ (unsigned long long)c.rpctype[r]);
+  h = mix64(h ^ (unsigned long long)c.dm[r]);
+  h = mix64(h ^ (unsigned long long)c.interface[r]);
+  return mix64(h ^ (unsigned long long)c.rt[r]);
+}
+
+__device__ __forceinline__ bool same_row(const PertRawCalls& c, long long a, long long b) {
+  return c.traceid[a] == c.traceid[b] && c.timestamp[a] == c.timestamp[b] && c.rpcid[a] == c.rpcid[b] &&
+         c.um[a] == c.um[b] && c.rpctype[a] == c.rpctype[b] && c.dm[a] == c.dm[b] &&
+         c.interface[a] == c.interface[b] && c.rt[a] == c.rt[b];
+}
+
+__device__ __forceinline__ int64_t abs64(int64_t v) { return v < 0 ? -v : v; }
+
+// ---- 1. drop_duplicates ----------------------------------------------------------------------------------------------
+__global__ void k_dedup_insert(PertRawCalls c, long long S, int hash_bits, int* owner, int* first, int* slot_of,
+                               int* status) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= c.R) return;
+  if (!codes_ok(c, r)) {                                 // reported, and the row is left out
+    atomicExch(status, PERT_ERR_RANGE);
+    slot_of[r] = -1;
+    return;
+  }
+  long long s = (long long)(mix64(row_hash(c, r) & hash_mask(hash_bits)) & (unsigned long long)(S - 1));
+  for (;;) {
+    const int o = atomicCAS(&owner[s], -1, (int)r);
+    if (o == -1 || same_row(c, o, r)) break;
+    s = (s + 1) & (S - 1);
+  }
+  atomicMin(&first[s], (int)r);
+  slot_of[r] = (int)s;
+}
+
+__global__ void k_dedup_flags(long long R, const int* slot_of, const int* first, int* flags) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= R) return;
+  const int s = slot_of[r];
+  flags[r + 1] = s >= 0 && first[s] == r;
+}
+
+__global__ void k_dedup_compact(PertRawCalls c, const int* flags, int* rows, int64_t* keys, int64_t* n_kept) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= c.R) return;
+  const int q = flags[r];
+  if (flags[r + 1] != q) {
+    rows[q] = (int)r;
+    keys[q] = c.timestamp[r];
+  }
+  if (r == c.R - 1) *n_kept = flags[c.R];
+}
+
+// ---- 3.-8. over the sorted kept rows: position p holds row order[p] ----------------------------------------------------
+struct Work {                 // carved from the caller's workspace by layout()
+  int *fl_tr, *fl_if, *fl_ent, *fl_rpc, *fl_rty, *fl_row;           // [N+1] first-position / survivor flags, scanned
+  int *first_tr, *first_if, *first_rpc, *first_rty;                 // [dictionary] first position of every code
+  int *fl_ms;                                                       // [n_ms+1] microservice presence, scanned
+  int *ncand, *nq, *cand_pos, *q_pos, *epos, *eslot, *ndist, *nres, *covered;   // [n_trace] per trace
+  int64_t* amax;                                                    // [n_trace] max |rt|
+  unsigned long long *ekey, *pkey;                                  // [SE], [SP] entry / (trace, ms) tables
+  int *efirst, *ecnt;                                               // [SE]
+  int* bsum;
+  long long SE, SP;
+};
+
+long long pow2_at_least(long long n) {
+  long long S = 64;
+  while (S < n) S <<= 1;
+  return S;
+}
+
+long long scan_bytes(long long L) { return 2LL * pert_cdiv(L, SCAN_TILE) * 4 + 16; }
+
+// bytes of the workspace of pert_raw_process / pert_raw_emit; w != NULL also carves it
+long long layout(const PertRawCalls& c, long long N, void* base, Work* w) {
+  const long long SE = pow2_at_least(2 * c.n_trace), SP = pow2_at_least(4 * N);
+  long long off = 0;
+  auto take = [&](long long bytes) {
+    char* p = base ? (char*)base + off : nullptr;
+    off += (bytes + 15) / 16 * 16;
+    return (void*)p;
+  };
+  Work x;
+  x.SE = SE;
+  x.SP = SP;
+  x.ekey = (unsigned long long*)take(8 * SE);
+  x.pkey = (unsigned long long*)take(8 * SP);
+  x.amax = (int64_t*)take(8 * c.n_trace);
+  int** flags[] = {&x.fl_tr, &x.fl_if, &x.fl_ent, &x.fl_rpc, &x.fl_rty, &x.fl_row};
+  for (int** f : flags) *f = (int*)take(4 * (N + 1));
+  x.first_tr = (int*)take(4 * c.n_trace);
+  x.first_if = (int*)take(4 * c.n_iface);
+  x.first_rpc = (int*)take(4 * c.n_rpcid);
+  x.first_rty = (int*)take(4 * c.n_rpctype);
+  x.fl_ms = (int*)take(4 * (c.n_ms + 1));
+  int** per_trace[] = {&x.ncand, &x.nq, &x.cand_pos, &x.q_pos, &x.epos, &x.eslot, &x.ndist, &x.nres, &x.covered};
+  for (int** f : per_trace) *f = (int*)take(4 * c.n_trace);
+  x.efirst = (int*)take(4 * SE);
+  x.ecnt = (int*)take(4 * SE);
+  x.bsum = (int*)take(scan_bytes(std::max(N, c.n_ms) + 1));
+  if (w) *w = x;
+  return off;
+}
+
+__global__ void k_first_codes(PertRawCalls c, long long N, const int64_t* order, Work w) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= N) return;
+  const long long r = order[p];
+  const int64_t tr = c.traceid[r];
+  atomicMin(&w.first_tr[tr], (int)p);
+  atomicMin(&w.first_if[c.interface[r]], (int)p);
+  atomicMax((long long*)&w.amax[tr], (long long)abs64(c.rt[r]));
+}
+
+// first-position flags of traceid / interface; entry candidates: http, the trace's first timestamp, its max |rt|
+__global__ void k_candidates(PertRawCalls c, long long N, const int64_t* order, Work w) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= N) return;
+  const long long r = order[p];
+  const int64_t tr = c.traceid[r];
+  const int f = w.first_tr[tr];
+  w.fl_tr[p + 1] = f == p;
+  w.fl_if[p + 1] = w.first_if[c.interface[r]] == p;
+  const int64_t ts = c.timestamp[r];
+  if (c.rpctype[r] == c.http && ts == c.timestamp[order[f]] && abs64(c.rt[r]) == w.amax[tr]) {
+    atomicAdd(&w.ncand[tr], 1);
+    atomicMin(&w.cand_pos[tr], (int)p);
+    if (c.um[r] == c.unknown) {
+      atomicAdd(&w.nq[tr], 1);
+      atomicMin(&w.q_pos[tr], (int)p);
+    }
+  }
+}
+
+// per trace (dictionary code): its entry row, and the slot of its (dm, interface) key in the entry table
+__global__ void k_entries(PertRawCalls c, const int64_t* order, Work w) {
+  const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= c.n_trace) return;
+  int e = -1;
+  if (w.first_tr[k] != RW_NONE) {
+    const int n = w.ncand[k];
+    e = n == 1 ? w.cand_pos[k] : (n > 1 && w.nq[k] == 1 ? w.q_pos[k] : -1);
+  }
+  w.epos[k] = e;
+  w.eslot[k] = -1;
+  if (e < 0) return;
+  const long long r = order[e];
+  const unsigned long long key = ((unsigned long long)c.dm[r] << 32) | (unsigned long long)c.interface[r];
+  long long s = (long long)(mix64(key) & (unsigned long long)(w.SE - 1));
+  for (;;) {
+    const unsigned long long o = atomicCAS(&w.ekey[s], RW_NOKEY, key);
+    if (o == RW_NOKEY || o == key) break;
+    s = (s + 1) & (w.SE - 1);
+  }
+  w.eslot[k] = (int)s;
+}
+
+__device__ __forceinline__ void claim_pair(const Work& w, int64_t tr, int64_t ms, const int* has_res) {
+  const unsigned long long key = ((unsigned long long)tr << 32) | (unsigned long long)ms;
+  long long s = (long long)(mix64(key) & (unsigned long long)(w.SP - 1));
+  for (;;) {
+    const unsigned long long o = atomicCAS(&w.pkey[s], RW_NOKEY, key);
+    if (o == key) return;                                // the trace already counted this microservice
+    if (o == RW_NOKEY) break;
+    s = (s + 1) & (w.SP - 1);
+  }
+  atomicAdd(&w.ndist[tr], 1);
+  if (has_res[ms]) atomicAdd(&w.nres[tr], 1);
+}
+
+// rows of traces with an entry: first positions of entryid / rpcid / rpctype, and the distinct (trace, ms) pairs
+__global__ void k_entry_rows(PertRawCalls c, long long N, const int64_t* order, const int* has_res, Work w) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= N) return;
+  const long long r = order[p];
+  const int64_t tr = c.traceid[r];
+  const int s = w.eslot[tr];
+  if (s < 0) return;
+  atomicMin(&w.efirst[s], (int)p);
+  atomicMin(&w.first_rpc[c.rpcid[r]], (int)p);
+  atomicMin(&w.first_rty[c.rpctype[r]], (int)p);
+  claim_pair(w, tr, c.um[r], has_res);
+  claim_pair(w, tr, c.dm[r], has_res);
+}
+
+__global__ void k_entry_flags(PertRawCalls c, long long N, const int64_t* order, Work w) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= N) return;
+  const long long r = order[p];
+  const int s = w.eslot[c.traceid[r]];
+  const bool ok = s >= 0;
+  w.fl_ent[p + 1] = ok && w.efirst[s] == p;
+  w.fl_rpc[p + 1] = ok && w.first_rpc[c.rpcid[r]] == p;
+  w.fl_rty[p + 1] = ok && w.first_rty[c.rpctype[r]] == p;
+}
+
+// resource coverage (IEEE double quotient, as Python's int / int) and the per-entry trace count of the survivors
+__global__ void k_coverage(long long n_trace, Work w) {
+  const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n_trace) return;
+  const int s = w.eslot[k];
+  const bool cov = s >= 0 && (double)w.nres[k] / (double)w.ndist[k] >= 0.6;
+  w.covered[k] = cov;
+  if (cov) atomicAdd(&w.ecnt[s], 1);
+}
+
+__global__ void k_ms_init(long long n_ms, const int* has_res, Work w) {
+  const long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (m < n_ms) w.fl_ms[m + 1] = has_res[m] != 0;
+}
+
+__global__ void k_survivors(PertRawCalls c, long long N, const int64_t* order, long long min_occurence, Work w) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= N) return;
+  const long long r = order[p];
+  const int64_t tr = c.traceid[r];
+  const int s = w.eslot[tr];
+  const bool keep = s >= 0 && w.covered[tr] && (long long)w.ecnt[s] > min_occurence;
+  w.fl_row[p + 1] = keep;
+  if (keep) {
+    w.fl_ms[c.um[r] + 1] = 1;
+    w.fl_ms[c.dm[r] + 1] = 1;
+  }
+}
+
+__global__ void k_sizes(long long N, long long n_ms, Work w, int64_t* sizes) {
+  sizes[0] = w.fl_row[N];
+  sizes[1] = w.fl_ms[n_ms];
+  sizes[2] = w.fl_tr[N];
+  sizes[3] = w.fl_if[N];
+  sizes[4] = w.fl_ent[N];
+  sizes[5] = w.fl_rpc[N];
+  sizes[6] = w.fl_rty[N];
+}
+
+__global__ void k_emit_rows(PertRawCalls c, long long N, const int64_t* order, Work w, PertRawOut o) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= N) return;
+  const long long r = order[p];
+  const int64_t tr = c.traceid[r], itf = c.interface[r];
+  // dictionaries: the code each new id was given at its first position
+  if (w.fl_tr[p + 1] != w.fl_tr[p]) o.tr_code[w.fl_tr[p]] = tr;
+  if (w.fl_if[p + 1] != w.fl_if[p]) o.if_code[w.fl_if[p]] = itf;
+  if (w.fl_rpc[p + 1] != w.fl_rpc[p]) o.rpc_code[w.fl_rpc[p]] = c.rpcid[r];
+  if (w.fl_rty[p + 1] != w.fl_rty[p]) o.rty_code[w.fl_rty[p]] = c.rpctype[r];
+  if (w.fl_ent[p + 1] != w.fl_ent[p]) {
+    const long long er = order[w.epos[tr]];
+    o.ent_dm[w.fl_ent[p]] = c.dm[er];
+    o.ent_if[w.fl_ent[p]] = w.fl_if[w.first_if[c.interface[er]]];
+  }
+  const int q = w.fl_row[p];
+  if (w.fl_row[p + 1] == q) return;
+  o.traceid[q] = w.fl_tr[w.first_tr[tr]];
+  o.timestamp[q] = c.timestamp[r];
+  o.rpcid[q] = w.fl_rpc[w.first_rpc[c.rpcid[r]]];
+  o.um[q] = w.fl_ms[c.um[r]];
+  o.dm[q] = w.fl_ms[c.dm[r]];
+  o.interface[q] = w.fl_if[w.first_if[itf]];
+  o.rpctype[q] = w.fl_rty[w.first_rty[c.rpctype[r]]];
+  o.rt[q] = c.rt[r];
+  o.entryid[q] = w.fl_ent[w.efirst[w.eslot[tr]]];
+  o.row[q] = r;
+}
+
+__global__ void k_emit_ms(long long n_ms, Work w, int64_t* ms_code) {
+  const long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (m < n_ms && w.fl_ms[m + 1] != w.fl_ms[m]) ms_code[w.fl_ms[m]] = m;
+}
+
+__global__ void k_emit_res(long long G, long long n_ms, const int64_t* g_ts, const int64_t* g_ms, Work w,
+                           int64_t* res_index) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= G) return;
+  const int64_t m = g_ms[g];
+  res_index[2 * g] = g_ts[g];
+  res_index[2 * g + 1] = in_dict(m, n_ms) ? w.fl_ms[m] : -1;   // groups hold valid codes only; guarded all the same
+}
+
+// ---- 9. resource groups ----------------------------------------------------------------------------------------------
+__global__ void k_res_flags(long long K, const int64_t* ts, const int64_t* ms, const int64_t* perm, long long n_ms,
+                            int* gflag, int* has_res, int* status) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= K) return;
+  const long long r = perm[p];
+  const int64_t m = ms[r];
+  if (!in_dict(m, n_ms)) {                               // reported, and the row is left out of every group
+    atomicExch(status, PERT_ERR_RANGE);
+    gflag[p + 1] = 0;
+    return;
+  }
+  has_res[m] = 1;
+  bool start = p == 0;
+  if (!start) {
+    const long long q = perm[p - 1];
+    start = ts[q] != ts[r] || ms[q] != m;
+  }
+  gflag[p + 1] = start;
+}
+
+// valid rows come first in perm (rows with an ms outside [0, n_ms) last), so the groups are the valid prefix
+__global__ void k_res_groups(long long K, long long n_ms, const int64_t* ts, const int64_t* ms, const int64_t* perm,
+                             const int* gflag, int* gptr, int64_t* g_ts, int64_t* g_ms, int64_t* n_groups) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= K) return;
+  if (p == K - 1) *n_groups = gflag[K];
+  const long long r = perm[p];
+  if (!in_dict(ms[r], n_ms)) return;
+  const int g = gflag[p];
+  if (gflag[p + 1] != g) {
+    gptr[g] = (int)p;
+    g_ts[g] = ts[r];
+    g_ms[g] = ms[r];
+  }
+  if (p == K - 1 || !in_dict(ms[perm[p + 1]], n_ms)) gptr[gflag[p + 1]] = (int)(p + 1);   // end of the last group
+}
+
+struct GroupStats {
+  double mx = -INFINITY, mn = INFINITY, sum = 0.0, comp = 0.0;
+  long long nobs = 0;
+  // pandas group_max / group_min (strict compare, first value kept on ties) and group_mean (Kahan, :GH#50367 reset of
+  // a NaN compensation after an infinite value)
+  __device__ __forceinline__ void add(double v) {
+    if (v != v) return;
+    ++nobs;
+    if (v > mx) mx = v;
+    if (v < mn) mn = v;
+    const double y = __dsub_rn(v, comp);
+    const double t = __dadd_rn(sum, y);
+    comp = __dsub_rn(__dsub_rn(t, sum), y);
+    if (comp != comp) comp = 0.0;
+    sum = t;
+  }
+};
+
+// median of the nobs non-NaN values at the front of a group's ascending sort (NaN sorts last)
+__device__ __forceinline__ double median_of(const double* sorted, long long nobs) {
+  if (nobs == 0) return NAN;
+  const long long h = nobs / 2;
+  if (nobs % 2) return sorted[h];
+  return __ddiv_rn(__dadd_rn(sorted[h], sorted[h - 1]), 2.0);
+}
+
+__global__ void k_res_stats(long long G, const int64_t* perm, const int* gptr, const double* cpu, const double* mem,
+                            const double* cpu_sorted, const double* mem_sorted, double* vals) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= G) return;
+  const int b = gptr[g], e = gptr[g + 1];
+  GroupStats a, m;
+  for (int p = b; p < e; ++p) {
+    const long long r = perm[p];
+    a.add(cpu[r]);
+    m.add(mem[r]);
+  }
+  double* out = vals + 8 * g;
+  const GroupStats* st[2] = {&a, &m};
+  const double* sorted[2] = {cpu_sorted, mem_sorted};
+  for (int j = 0; j < 2; ++j) {
+    const GroupStats& s = *st[j];
+    const bool none = s.nobs == 0;
+    out[4 * j + 0] = none ? NAN : s.mx;
+    out[4 * j + 1] = none ? NAN : s.mn;
+    out[4 * j + 2] = none ? NAN : __ddiv_rn(s.sum, (double)s.nobs);
+    out[4 * j + 3] = median_of(sorted[j] + b, s.nobs);
+  }
+}
+
+bool calls_ok(const PertRawCalls* c) {
+  return c && c->R >= 0 && c->R <= RW_MAX_ROWS && c->n_trace >= 0 && c->n_trace <= RW_MAX_ROWS &&
+         c->n_iface >= 0 && c->n_iface <= 0x7fffffffLL && c->n_rpcid >= 0 && c->n_rpcid <= 0x7fffffffLL &&
+         c->n_rpctype >= 0 && c->n_rpctype <= 0x7fffffffLL && c->n_ms >= 0 && c->n_ms <= 0x7ffffff0LL &&
+         (c->R == 0 || (c->traceid && c->timestamp && c->rpcid && c->um && c->rpctype && c->dm && c->interface &&
+                        c->rt));
+}
+
+int scan(int* a0, int* a1, long long L, int* bsum, cudaStream_t st) {   // inclusive, in place; a1 may be NULL
+  const int nb = pert_cdiv(L, SCAN_TILE), ny = a1 ? 2 : 1;
+  k_scan_tile_sums<<<dim3(nb, ny), SCAN_THREADS, 0, st>>>(a0, a1, (int)L, bsum, nb);
+  k_scan_block_sums<<<dim3(1, ny), SCAN_THREADS, 0, st>>>(bsum, nb);
+  k_scan_apply<<<dim3(nb, ny), SCAN_THREADS, 0, st>>>(a0, a1, (int)L, bsum, nb);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+long long dedup_table(long long R) { return pow2_at_least(2 * R); }
+
+}  // namespace
+
+extern "C" {
+
+long long pert_raw_dedup_workspace_bytes(long long R) {
+  if (R < 0 || R > RW_MAX_ROWS) return PERT_ERR_BADARG;
+  const long long S = dedup_table(R);
+  return 4 * (2 * S + R + (R + 1)) + scan_bytes(R + 1) + 64;
+}
+
+int pert_raw_dedup(const PertRawCalls* calls, int hash_bits, int* rows, int64_t* keys, int64_t* n_kept,
+                   void* workspace, long long workspace_bytes, int* status, void* stream_) {
+  if (!calls_ok(calls) || hash_bits < 1 || hash_bits > 64 || !rows || !keys || !n_kept || !workspace || !status)
+    return PERT_ERR_BADARG;
+  const long long R = calls->R;
+  if (workspace_bytes < pert_raw_dedup_workspace_bytes(R)) return PERT_ERR_BADARG;
+  cudaStream_t st = (cudaStream_t)stream_;
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(n_kept, 0, sizeof(int64_t), st)) != cudaSuccess) return (int)e;
+  if (R == 0) return PERT_OK;
+  const long long S = dedup_table(R);
+  int* owner = (int*)workspace;
+  int* first = owner + S;
+  int* slot_of = first + S;
+  int* flags = slot_of + R;
+  int* bsum = flags + R + 1;
+  if ((e = cudaMemsetAsync(owner, 0xff, 4 * S, st)) || (e = cudaMemsetAsync(first, 0x7f, 4 * S, st)) ||
+      (e = cudaMemsetAsync(flags, 0, 4, st)))
+    return (int)e;
+  const int B = 256, gR = pert_cdiv(R, B);
+  k_dedup_insert<<<gR, B, 0, st>>>(*calls, S, hash_bits, owner, first, slot_of, status);
+  k_dedup_flags<<<gR, B, 0, st>>>(R, slot_of, first, flags);
+  PERT_LAUNCH_CHECK();
+  int rc;
+  if ((rc = scan(flags, nullptr, R + 1, bsum, st)) != PERT_OK) return rc;
+  k_dedup_compact<<<gR, B, 0, st>>>(*calls, flags, rows, keys, n_kept);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+long long pert_raw_process_workspace_bytes(const PertRawCalls* calls, long long N) {
+  if (!calls_ok(calls) || N < 0 || N > calls->R) return PERT_ERR_BADARG;
+  return layout(*calls, N, nullptr, nullptr) + 64;
+}
+
+int pert_raw_process(const PertRawCalls* calls, long long N, const int64_t* order, const int* has_res,
+                     long long min_occurence, int64_t* sizes, void* workspace, long long workspace_bytes,
+                     void* stream_) {
+  if (!calls_ok(calls) || N < 0 || N > calls->R || (N > 0 && !order) || !has_res || !sizes || !workspace)
+    return PERT_ERR_BADARG;
+  const long long need = pert_raw_process_workspace_bytes(calls, N);
+  if (need < 0 || workspace_bytes < need) return PERT_ERR_BADARG;
+  const PertRawCalls& c = *calls;
+  cudaStream_t st = (cudaStream_t)stream_;
+  Work w;
+  layout(c, N, workspace, &w);
+  cudaError_t e;
+  auto fill = [&](void* p, long long bytes, int v) { return cudaMemsetAsync(p, v, (size_t)bytes, st); };
+  if ((e = fill(w.ekey, 8 * w.SE, 0xff)) || (e = fill(w.pkey, 8 * w.SP, 0xff)) ||
+      (e = fill(w.amax, 8 * c.n_trace, 0)) || (e = fill(w.first_tr, 4 * c.n_trace, 0x7f)) ||
+      (e = fill(w.first_if, 4 * c.n_iface, 0x7f)) || (e = fill(w.first_rpc, 4 * c.n_rpcid, 0x7f)) ||
+      (e = fill(w.first_rty, 4 * c.n_rpctype, 0x7f)) || (e = fill(w.fl_ms, 4 * (c.n_ms + 1), 0)) ||
+      (e = fill(w.ncand, 4 * c.n_trace, 0)) || (e = fill(w.nq, 4 * c.n_trace, 0)) ||
+      (e = fill(w.cand_pos, 4 * c.n_trace, 0x7f)) || (e = fill(w.q_pos, 4 * c.n_trace, 0x7f)) ||
+      (e = fill(w.ndist, 4 * c.n_trace, 0)) || (e = fill(w.nres, 4 * c.n_trace, 0)) ||
+      (e = fill(w.efirst, 4 * w.SE, 0x7f)) || (e = fill(w.ecnt, 4 * w.SE, 0)) ||
+      (e = fill(sizes, 7 * sizeof(int64_t), 0)))
+    return (int)e;
+  int* flags[] = {w.fl_tr, w.fl_if, w.fl_ent, w.fl_rpc, w.fl_rty, w.fl_row};
+  for (int* f : flags)
+    if ((e = fill(f, 4, 0))) return (int)e;
+  const int B = 256, gN = pert_cdiv(std::max(N, 1LL), B), gT = pert_cdiv(std::max(c.n_trace, 1LL), B);
+  const int gM = pert_cdiv(std::max(c.n_ms, 1LL), B);
+  int rc;
+  if (N > 0) {
+    // 3. + 4. traceid / interface codes, entry candidates, entry keys
+    k_first_codes<<<gN, B, 0, st>>>(c, N, order, w);
+    k_candidates<<<gN, B, 0, st>>>(c, N, order, w);
+    PERT_LAUNCH_CHECK();
+    if ((rc = scan(w.fl_tr, w.fl_if, N + 1, w.bsum, st)) != PERT_OK) return rc;
+    k_entries<<<gT, B, 0, st>>>(c, order, w);
+    // entryid / rpcid / rpctype codes over the rows of traces with an entry; 5. coverage; 6. occurrences
+    k_entry_rows<<<gN, B, 0, st>>>(c, N, order, has_res, w);
+    k_entry_flags<<<gN, B, 0, st>>>(c, N, order, w);
+    PERT_LAUNCH_CHECK();
+    if ((rc = scan(w.fl_ent, w.fl_rpc, N + 1, w.bsum, st)) != PERT_OK) return rc;
+    if ((rc = scan(w.fl_rty, nullptr, N + 1, w.bsum, st)) != PERT_OK) return rc;
+    k_coverage<<<gT, B, 0, st>>>(c.n_trace, w);
+  }
+  // 7. microservice presence (every resource msname, the surviving rows' um / dm); 8. survivor positions
+  k_ms_init<<<gM, B, 0, st>>>(c.n_ms, has_res, w);
+  if (N > 0) k_survivors<<<gN, B, 0, st>>>(c, N, order, min_occurence, w);
+  PERT_LAUNCH_CHECK();
+  if ((rc = scan(w.fl_ms, nullptr, c.n_ms + 1, w.bsum, st)) != PERT_OK) return rc;
+  if ((rc = scan(w.fl_row, nullptr, N + 1, w.bsum, st)) != PERT_OK) return rc;
+  k_sizes<<<1, 1, 0, st>>>(N, c.n_ms, w, sizes);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+int pert_raw_emit(const PertRawCalls* calls, long long N, const int64_t* order, long long G, const int64_t* g_ts,
+                  const int64_t* g_ms, const PertRawOut* out, void* workspace, long long workspace_bytes,
+                  void* stream_) {
+  if (!calls_ok(calls) || N < 0 || N > calls->R || (N > 0 && !order) || G < 0 || (G > 0 && (!g_ts || !g_ms)) ||
+      !out || !workspace)
+    return PERT_ERR_BADARG;
+  const PertRawOut& o = *out;
+  if (!o.traceid || !o.timestamp || !o.rpcid || !o.um || !o.dm || !o.interface || !o.rpctype || !o.rt ||
+      !o.entryid || !o.row || !o.res_index || !o.ms_code || !o.tr_code || !o.if_code || !o.rpc_code || !o.rty_code ||
+      !o.ent_dm || !o.ent_if)
+    return PERT_ERR_BADARG;
+  const long long need = pert_raw_process_workspace_bytes(calls, N);
+  if (need < 0 || workspace_bytes < need) return PERT_ERR_BADARG;
+  cudaStream_t st = (cudaStream_t)stream_;
+  Work w;
+  layout(*calls, N, workspace, &w);
+  const int B = 256;
+  if (N > 0) k_emit_rows<<<pert_cdiv(N, B), B, 0, st>>>(*calls, N, order, w, o);
+  if (calls->n_ms > 0) k_emit_ms<<<pert_cdiv(calls->n_ms, B), B, 0, st>>>(calls->n_ms, w, o.ms_code);
+  if (G > 0) k_emit_res<<<pert_cdiv(G, B), B, 0, st>>>(G, calls->n_ms, g_ts, g_ms, w, o.res_index);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+long long pert_raw_resource_workspace_bytes(long long K) {
+  if (K < 0 || K > 0x7ffffff0LL) return PERT_ERR_BADARG;
+  return scan_bytes(K + 1) + 64;
+}
+
+int pert_raw_resource_groups(long long K, const int64_t* ts, const int64_t* ms, const int64_t* perm, long long n_ms,
+                             int* gflag, int* has_res, int* gptr, int64_t* g_ts, int64_t* g_ms, int64_t* n_groups,
+                             void* workspace, long long workspace_bytes, int* status, void* stream_) {
+  if (K < 0 || K > 0x7ffffff0LL || n_ms < 0 || (K > 0 && (!ts || !ms || !perm)) || !gflag || !has_res || !gptr ||
+      !g_ts || !g_ms || !n_groups || !workspace || !status)
+    return PERT_ERR_BADARG;
+  if (workspace_bytes < pert_raw_resource_workspace_bytes(K)) return PERT_ERR_BADARG;
+  cudaStream_t st = (cudaStream_t)stream_;
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(n_groups, 0, sizeof(int64_t), st)) || (e = cudaMemsetAsync(gflag, 0, 4, st)) ||
+      (e = cudaMemsetAsync(gptr, 0, 4, st)) || (n_ms > 0 && (e = cudaMemsetAsync(has_res, 0, 4 * n_ms, st))))
+    return (int)e;
+  if (K == 0) return PERT_OK;
+  const int B = 256, gK = pert_cdiv(K, B);
+  k_res_flags<<<gK, B, 0, st>>>(K, ts, ms, perm, n_ms, gflag, has_res, status);
+  PERT_LAUNCH_CHECK();
+  int rc;
+  if ((rc = scan(gflag, nullptr, K + 1, (int*)workspace, st)) != PERT_OK) return rc;
+  k_res_groups<<<gK, B, 0, st>>>(K, n_ms, ts, ms, perm, gflag, gptr, g_ts, g_ms, n_groups);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+int pert_raw_resource_stats(long long G, const int64_t* perm, const int* gptr, const double* cpu, const double* mem,
+                            const double* cpu_sorted, const double* mem_sorted, double* vals, void* stream_) {
+  if (G < 0 || (G > 0 && (!perm || !gptr || !cpu || !mem || !cpu_sorted || !mem_sorted || !vals)))
+    return PERT_ERR_BADARG;
+  if (G == 0) return PERT_OK;
+  k_res_stats<<<pert_cdiv(G, 128), 128, 0, (cudaStream_t)stream_>>>(G, perm, gptr, cpu, mem, cpu_sorted, mem_sorted,
+                                                                   vals);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+}  // extern "C"

@@ -446,3 +446,204 @@ def make_random_trace_table(seed, n_traces, rows=(20, 40), n_patterns=2000, n_en
             "rpctype": rng.integers(0, 8, tr.shape[0]), "rt": rt, "entryid": ent[tr]}
     order = _interleave(rng, tr)
     return {k: np.ascontiguousarray(v[order], dtype=np.int64) for k, v in cols.items()}
+
+
+def make_raw_tables(seed=0, dotted_rpcid=False):
+    """Deterministic raw CSV text of the Alibaba MSCallGraph / MSResource schema (the input of the reference's
+    get_df(), preprocess.py:191-266) -> {"callgraph": {file name: text}, "resource": {file name: text}}.
+    Call-graph files carry the leading unnamed index column; rows of a trace are interleaved with other traces.  Every
+    trace's first timestamp is unique and the only timestamp ties are rows of one trace that differ in um (and, for
+    the two-"(?)" case, in the sign of rt), so the reference's unstable sort cannot decide the result.  Covers:
+      exact duplicate rows within one file and across files; negative rt; null string cells (um, interface, rpctype,
+      and rpcid when ``dotted_rpcid``); a numeric rpcid column (some files written as "1.0", which pyarrow reads as
+      floats) or dotted-string rpcids;
+      entry detection: one candidate, several resolved by um == "(?)", several with zero or two "(?)", none;
+      resource coverage exactly 0.6 (kept) and 4/7 (dropped); entries with 100 traces (dropped) and 101 (kept);
+      resource microservices in no trace; resource groups of 1..5 rows, NaN usages, an all-NaN group and the Kahan
+      group [1e16, 1, 1, -1e16] (mean 0.5), groups split across two files, rows with a null timestamp or msname."""
+    rng = np.random.default_rng(seed)
+    res_ms = [f"MS_{k:03d}" for k in range(24)]              # microservices with resource rows (and "USER")
+    bare_ms = [f"NR_{k:02d}" for k in range(6)]               # microservices without
+    types = ["rpc", "mc", "db", "mq"]
+    traces = []                                               # (rows, kind); a row: dict of the call columns
+
+    def rpcid(k):
+        return f"0.1.{k}" if dotted_rpcid else str(k)
+
+    def body(n, ms):
+        """n child rows over microservices ``ms`` (all of them used), |rt| < 1000."""
+        rows, prev = [], ms[0]
+        for k in range(max(n, len(ms) - 1)):
+            nxt = ms[(k + 1) % len(ms)]
+            rows.append(dict(um=prev, dm=nxt, rpctype=types[rng.integers(len(types))],
+                             interface=f"IF_{rng.integers(40):02d}", rpcid=rpcid(k + 1),
+                             rt=int(rng.integers(1, 1000)) * (-1 if rng.random() < 0.3 else 1)))
+            prev = nxt
+        return rows
+
+    def entry(um, dm, itf, rt):
+        return dict(um=um, dm=dm, rpctype="http", interface=itf, rpcid=rpcid(0), rt=rt)
+
+    def plain(dm, itf, um="USER", cover=None):
+        rt = int(rng.integers(1000, 5000)) * (-1 if rng.random() < 0.2 else 1)
+        ms = cover if cover is not None else [dm] + list(rng.choice(res_ms, size=int(rng.integers(2, 5)),
+                                                                      replace=False))
+        rows = [[entry(um, dm, itf, rt)]] + [[r] for r in body(int(rng.integers(2, 6)), ms)]
+        if cover is None and rng.random() < 0.1:              # null string cells in a child row
+            rows[-1][0][("um", "interface", "rpctype")[rng.integers(3)]] = None
+        return rows
+
+    for _ in range(95):
+        traces.append(plain("MS_001", "IF_A"))
+    for _ in range(6):                                        # two candidates, one of them "(?)": resolved
+        t = plain("MS_001", "IF_A")
+        t[0].append(dict(t[0][0], um="(?)"))
+        traces.append(t)
+    for _ in range(100):
+        traces.append(plain("MS_002", "IF_B"))
+    for _ in range(98):
+        traces.append(plain("MS_003", "IF_C"))
+    for k in range(3):                                        # coverage 3/5 = 0.6: kept
+        traces.append(plain("MS_003", "IF_C", um="MS_004", cover=["MS_003", "MS_005", bare_ms[k], bare_ms[k + 1]]))
+    for k in range(3):                                        # coverage 4/7: dropped
+        traces.append(plain("MS_003", "IF_C", um="MS_004",
+                            cover=["MS_003", "MS_005", "MS_006", bare_ms[k], bare_ms[k + 1], bare_ms[k + 2]]))
+    for _ in range(3):                                        # two candidates, none "(?)": dropped
+        t = plain("MS_007", "IF_D", um="MS_008")
+        t[0].append(dict(t[0][0], um="MS_009"))
+        traces.append(t)
+    for _ in range(3):                                        # two "(?)" candidates (rt and -rt): dropped
+        t = plain("MS_007", "IF_D", um="(?)")
+        t[0].append(dict(t[0][0], um="(?)", rt=-t[0][0]["rt"]))
+        traces.append(t)
+    for _ in range(3):                                        # no http row at the first timestamp: dropped
+        t = plain("MS_007", "IF_D")
+        t[0][0]["rpctype"] = "rpc"
+        traces.append(t)
+
+    if dotted_rpcid:
+        traces[0][-1][0]["rpcid"] = None                     # a null string rpcid (a child row)
+    # interleave: every group of rows (tie partners share one group) gets a unique timestamp, in trace order
+    order = rng.permutation(len(traces))
+    events = []
+    for rank, ti in enumerate(order):
+        t0 = rank * 40.0
+        for j in range(len(traces[ti])):
+            events.append((t0 + j * rng.uniform(5, 60) if j else t0, ti, j))
+    events.sort()
+    base = 1_700_000_000_000 + seed * 10_000_000
+    out_rows = []
+    for k, (_, ti, j) in enumerate(events):
+        for r in traces[ti][j]:
+            out_rows.append(dict(r, traceid=f"tr{ti:04d}x{seed}", timestamp=base + 7 * k))
+    # duplicates: within the same file and across files
+    files = [[], [], []]
+    for r in out_rows:
+        files[int(rng.integers(3))].append(r)
+    for _ in range(12):
+        f = int(rng.integers(3))
+        src = files[f][int(rng.integers(len(files[f])))]
+        files[f].insert(int(rng.integers(len(files[f]) + 1)), dict(src))
+    for _ in range(12):
+        f, g = (int(v) for v in rng.choice(3, size=2, replace=False))
+        files[g].insert(int(rng.integers(len(files[g]) + 1)), dict(files[f][int(rng.integers(len(files[f])))]))
+
+    def cell(v):
+        return "" if v is None else str(v)
+
+    def rpc_cell(v, float_file):
+        if v is None:
+            return ""
+        return f"{v}.0" if float_file and not dotted_rpcid else v
+
+    callgraph = {}
+    for f, rows in enumerate(files):
+        lines = [",traceid,timestamp,rpcid,um,rpctype,dm,interface,rt"]
+        for i, r in enumerate(rows):
+            lines.append(",".join([str(1000 * f + i), r["traceid"], str(r["timestamp"]), rpc_cell(r["rpcid"], f == 2),
+                                   cell(r["um"]), cell(r["rpctype"]), r["dm"], cell(r["interface"]), str(r["rt"])]))
+        callgraph[f"MSCallGraph_{f}.csv"] = "\n".join(lines) + "\n"
+
+    # resources: groups per (timestamp, msname) of 1..5 instance rows, split over two files
+    extra = [f"MS_R{k}" for k in range(3)]                    # resourced, in no trace
+    res_files = [[], []]
+    b0 = base // 30000 * 30000                                # the traces' buckets are b0 and b0 + 30000
+    ts_list = [b0 - 30000, b0, b0 + 30000]
+    for ts in ts_list:
+        for m in res_ms + extra + ["USER"]:
+            n = int(rng.integers(1, 6))
+            for i in range(n):
+                cpu = None if rng.random() < 0.1 else float(rng.random())
+                mem = None if rng.random() < 0.1 else float(rng.random() * 2)
+                res_files[int(rng.integers(2))].append((ts, m, f"{m}_i{i}", cpu, mem))
+    t3 = b0 + 60000
+    res_files[0] += [(t3, "MS_000", "k0", 1e16, 0.25), (t3, "MS_000", "k1", 1.0, 0.5), (t3, "MS_000", "k2", 1.0, None),
+                     (t3, "MS_000", "k3", -1e16, 0.125), (t3, "MS_001", "n0", None, None),
+                     (t3, "MS_001", "n1", None, None), (None, "MS_002", "z0", 0.5, 0.5), (t3, None, "z1", 0.5, 0.5)]
+    resource = {}
+    for f, rows in enumerate(res_files):
+        lines = ["timestamp,msname,msinstanceid,nodeid,instance_cpu_usage,instance_memory_usage"]
+        for ts, m, inst, cpu, mem in rows:
+            lines.append(",".join([cell(ts), cell(m), inst, f"node{len(lines) % 7}",
+                                   "" if cpu is None else repr(cpu), "" if mem is None else repr(mem)]))
+        resource[f"MSResource_{f}.csv"] = "\n".join(lines) + "\n"
+    return {"callgraph": callgraph, "resource": resource}
+
+
+def make_random_raw_tables(seed, n_traces, rows=(4, 56), n_entries=64, n_ms=3000, n_if=512, dup=0.05):
+    """Large dictionary-encoded raw tables (rawtable.RawTables) for scale tests: heavy timestamp ties across traces
+    (timestamps drawn from a narrow range), ``dup`` of the rows repeated exactly, entry rows with "(?)" tie partners,
+    traces without an entry, partial resource coverage and resource groups of 1..8 rows with NaN usages."""
+    from .rawtable import RawTables
+
+    rng = np.random.default_rng(seed)
+    lens = rng.integers(rows[0], rows[1] + 1, size=n_traces)
+    R = int(lens.sum())
+    tr = np.repeat(np.arange(n_traces), lens)
+    first = np.concatenate([[0], np.cumsum(lens)[:-1]])
+    is_first = np.zeros(R, bool)
+    is_first[first] = True
+    ent = rng.integers(n_entries, size=n_traces)
+    start = rng.integers(0, n_traces * 4, size=n_traces)
+    ts = start[tr] + rng.integers(0, 200, size=R) * (~is_first)
+    rt = rng.integers(-900, 900, size=R)
+    rt[first] = rng.integers(1000, 3000, size=n_traces) * np.where(rng.random(n_traces) < 0.2, -1, 1)
+    ms_names = sorted({f"m{k:05d}" for k in range(n_ms - 1)} | {"(?)"})
+    q = ms_names.index("(?)")
+    um = rng.integers(n_ms, size=R)
+    dm = rng.integers(n_ms, size=R)
+    dm[first] = (ent * 7) % n_ms
+    um[first] = np.where(rng.random(n_traces) < 0.5, q, um[first])
+    itf = rng.integers(n_if, size=R)
+    itf[first] = ent % n_if
+    rty = rng.integers(1, 4, size=R)                          # 0 = "http"
+    rty[first] = np.where(rng.random(n_traces) < 0.95, 0, 1)
+    rpc = rng.integers(0, 64, size=R)
+    cols = dict(traceid=tr, timestamp=ts, rpcid=rpc, um=um, rpctype=rty, dm=dm, interface=itf, rt=rt)
+    # "(?)" tie partners of some entry rows, and exact duplicates
+    tie = first[rng.random(n_traces) < 0.2]
+    dup_rows = rng.integers(R, size=int(dup * R))
+    extra = np.concatenate([tie, dup_rows])
+    for k, v in cols.items():
+        add = v[extra].copy()
+        if k == "um":
+            add[:len(tie)] = np.where(add[:len(tie)] == q, 0, q)
+        cols[k] = np.concatenate([v, add])
+    perm = rng.permutation(len(cols["traceid"]))
+    cols = {k: v[perm] for k, v in cols.items()}
+    # resources: about 80 % of the microservices, 1..8 rows per (timestamp, ms) group
+    have = np.flatnonzero(rng.random(n_ms) < 0.8)
+    n_ts = 4
+    gm = np.repeat(have, n_ts)
+    gt = np.tile(np.arange(n_ts) * 30000, len(have))
+    cnt = rng.integers(1, 9, size=len(gm))
+    r_ms, r_ts = np.repeat(gm, cnt), np.repeat(gt, cnt)
+    K = len(r_ms)
+    cpu, mem = rng.random(K), rng.random(K) * 1e3
+    cpu[rng.random(K) < 0.05] = np.nan
+    mem[rng.random(K) < 0.05] = np.nan
+    rp = rng.permutation(K)
+    resources = dict(timestamp=r_ts[rp], msname=r_ms[rp], instance_cpu_usage=cpu[rp], instance_memory_usage=mem[rp])
+    dicts = dict(traceid=[f"t{k}" for k in range(n_traces)], interface=[f"i{k}" for k in range(n_if)],
+                 rpcid=list(range(64)), rpctype=["http", "rpc", "mc", "db"], ms=ms_names)
+    return RawTables(cols, resources, dicts)

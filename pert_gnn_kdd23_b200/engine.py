@@ -138,7 +138,8 @@ class Engine:
 
     def reserve(self, N, E, B):
         """Pre-size the workspace (growth only).  ``ws_generation`` changes whenever the buffer is re-allocated: a CUDA
-        graph captured over the old buffer must not be replayed any more (train.GraphedTrainStep checks it)."""
+        graph captured over the old buffer must not be replayed any more (train._GraphCache checks it, and calls this
+        before every capture so that no capture allocates the workspace)."""
         return self._workspace(int(N), int(E), int(B))
 
     def _workspace(self, N, E, B):

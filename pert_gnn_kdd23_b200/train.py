@@ -304,8 +304,7 @@ def _fused_fwd_bwd(model, optimizer: FusedAdam, data, tau, index, probe, use_ind
     word of a padded batch (``PaddedBatch``), read by the engine and the loss."""
     from .index import build_index, cached_index
 
-    eng = model.engine(optimizer.fp) if (model._engine is None or model._engine.fp is not optimizer.fp) \
-        else model._engine
+    eng = _engine_of(model, optimizer)
     x, cat_X, edge_index, edge_attr, pnn, probs, entry_id, batch = model_inputs(data)
     index_ready = None
     if index is None:
@@ -340,36 +339,120 @@ def _fused_fwd_bwd(model, optimizer: FusedAdam, data, tau, index, probe, use_ind
     return loss, index
 
 
-def fused_train_step(model, optimizer: FusedAdam, data, tau=0.5, dp: DataParallel | None = None, index=None,
-                     probe=None):
-    """Same step as ``train_step`` but without autograd: engine forward -> pinball loss + its gradient (one
-    kernel) -> engine backward into the flat gradient buffer -> (all-reduce) -> fused Adam.  5 C calls per step.
-    Returns the device loss tensor [1]."""
-    loss, _ = _fused_fwd_bwd(model, optimizer, data, tau, index, probe)
+def _engine_of(model, optimizer: FusedAdam):
+    """The step engine of ``model`` over ``optimizer``'s FlatParams (``model.engine`` is only asked when the current
+    engine is over another one: the per-step path makes no ownership check)."""
+    eng = model._engine
+    return model.engine(optimizer.fp) if eng is None or eng.fp is not optimizer.fp else eng
+
+
+def _reduce_and_step(optimizer: FusedAdam, dp: DataParallel | None, loss):
+    """The end of a fused step once the gradients are in the flat buffer: (gradient all-reduce) -> fused Adam, issued
+    eagerly (the Adam step count is a by-value kernel argument).  Returns ``loss``."""
     with torch.no_grad():
         scale = dp.all_reduce_grads(optimizer) if dp is not None else 1.0
         optimizer.step(grad_scale=scale)
     return loss
 
 
-class GraphedTrainStep:
+def fused_train_step(model, optimizer: FusedAdam, data, tau=0.5, dp: DataParallel | None = None, index=None,
+                     probe=None):
+    """Same step as ``train_step`` but without autograd: engine forward -> pinball loss + its gradient (one
+    kernel) -> engine backward into the flat gradient buffer -> (all-reduce) -> fused Adam.  5 C calls per step.
+    Returns the device loss tensor [1]."""
+    loss, _ = _fused_fwd_bwd(model, optimizer, data, tau, index, probe)
+    return _reduce_and_step(optimizer, dp, loss)
+
+
+def _batch_sizes(data):
+    return int(data.x.size(0)), int(data.edge_index.size(1)), int(data.num_graphs)
+
+
+class _GraphCache:
+    """One CUDA graph per key, for the steps below that replay their device work.
+
+    ``cache(key, eng, sizes, fn, pin)`` returns what ``fn()`` returns.  A key's first visit runs ``fn`` eagerly (it also
+    does the library's one-time initialisation), the second captures it and every visit from then on replays it; a
+    replay returns the tensors of the capture, which it has just rewritten.  ``eng.reserve(*sizes)`` comes first, so
+    the workspace is never allocated inside a capture.  A graph captured over another engine (re-created after the
+    parameters moved) or over a workspace the engine has since re-allocated points into freed memory: that key's graph
+    is dropped and captured again on the visit that finds it (``invalidations``).  At most ``max_graphs`` keys hold a
+    graph; a key past that, or one whose capture raised (``capture_error``), runs ``fn`` eagerly on every visit.
+    ``ops.LAUNCHES`` counts the launches a replay runs, not the ones a capture records.  An entry keeps alive what its
+    graph points into: the outputs, the engine and its workspace, and ``pin`` (the caller's input buffers).  The
+    callers that pad a batch into its capacity bucket (``pad``) key on the bucket and keep its ``PaddedBatch`` here."""
+
+    def __init__(self, max_graphs=32):
+        self.max_graphs = max_graphs
+        self.buckets = {}    # key -> {"state": "ran-once" | "eager" | "graph", and with a graph what it keeps alive}
+        self.bufs = {}       # capacity bucket -> its PaddedBatch (``pad``)
+        self.capture_error = None
+        self.replays = 0
+        self.captures = 0
+        self.invalidations = 0
+
+    def pad(self, data):
+        """Copies ``data`` into the ``PaddedBatch`` of its capacity bucket (made on the bucket's first visit).
+        -> (bucket: the capacities and the edge-attribute width, the filled PaddedBatch)."""
+        caps = bucket_caps(*_batch_sizes(data))
+        bucket = caps + (int(data.edge_attr.size(1)),)
+        buf = self.bufs.get(bucket)
+        if buf is None:
+            buf = self.bufs[bucket] = PaddedBatch(caps, data)
+        return bucket, buf.fill(data)
+
+    def cache(self, key, eng, sizes, fn, pin=None):
+        eng.reserve(*sizes)
+        ent = self.buckets.get(key)
+        if ent is None:
+            self.buckets[key] = {"state": "ran-once"}
+            return fn()
+        if ent["state"] == "graph" and (ent["engine"] is not eng or ent["ws_gen"] != eng.ws_generation):
+            ent = self.buckets[key] = {"state": "ran-once"}
+            self.invalidations += 1
+        if ent["state"] == "ran-once":
+            held = sum(e["state"] == "graph" for e in self.buckets.values())
+            if held >= self.max_graphs or not self._capture(ent, eng, fn, pin):
+                ent["state"] = "eager"
+        if ent["state"] == "eager":
+            return fn()
+        ent["graph"].replay()
+        ops.LAUNCHES["n"] += ent["launches"]
+        self.replays += 1
+        return ent["out"]
+
+    def _capture(self, ent, eng, fn, pin):
+        g = torch.cuda.CUDAGraph()
+        l0 = ops.LAUNCHES["n"]
+        try:
+            with torch.cuda.graph(g):
+                out = fn()
+        except Exception as e:  # noqa: BLE001 - any capture failure leaves this key on the eager path
+            self.capture_error = repr(e)
+            torch.cuda.synchronize()
+            return False
+        finally:
+            launches, ops.LAUNCHES["n"] = ops.LAUNCHES["n"] - l0, l0      # a capture runs nothing
+        ent.update(state="graph", graph=g, out=out, launches=launches, engine=eng, ws_gen=eng.ws_generation,
+                   ws=eng.ws, pin=pin)
+        self.captures += 1
+        return True
+
+
+class GraphedTrainStep(_GraphCache):
     """``fused_train_step`` with the device work up to the gradients replayed from a CUDA graph.
 
     One graph per (input buffers, shapes) key -- e.g. one per slab of ``data.DevicePrefetcher``'s ring, or one per
     resident batch.  The graph holds: index build, gradient zeroing, engine forward, pinball loss, engine backward
     (~45 kernel launches become one ``cudaGraphLaunch``: no per-kernel launch gaps on the GPU, ~0.5 ms less host
     work per step).  The gradient all-reduce and Adam (its step count is a by-value kernel argument) are issued
-    eagerly after the replay.  The first step on a new key runs eagerly (it also does the library's one-time
-    initialisation), the second is captured; a key whose capture fails stays eager.  The reference has no
-    counterpart (its loop body, pert_gnn.py:231-247, launches every operator from Python each step)."""
+    eagerly after the replay.  Eager first visit, capture, replays, invalidation and ``max_graphs`` as in
+    ``_GraphCache``.  The reference has no counterpart (its loop body, pert_gnn.py:231-247, launches every operator
+    from Python each step)."""
 
     def __init__(self, model, optimizer: FusedAdam, tau=0.5, dp: DataParallel | None = None, max_graphs=32):
+        super().__init__(max_graphs)
         self.model, self.opt, self.tau, self.dp = model, optimizer, tau, dp
-        self.max_graphs = max_graphs
-        self._seen = {}      # key -> "ran-once" | "failed" | entry dict
-        self.capture_error = None
-        self.replays = 0
-        self.invalidations = 0
 
     @staticmethod
     def _key(data):
@@ -377,59 +460,15 @@ class GraphedTrainStep:
         ptrs = tuple(t.data_ptr() for t in model_inputs(data) if torch.is_tensor(t)) + (data.y.data_ptr(),)
         return ptrs + (tuple(data.x.shape), int(data.edge_index.size(1)), int(data.num_graphs))
 
-    def _finish(self, loss):
-        with torch.no_grad():
-            scale = self.dp.all_reduce_grads(self.opt) if self.dp is not None else 1.0
-            self.opt.step(grad_scale=scale)
-        return loss
-
     def __call__(self, data):
         # the training flag and the dropout rate are by-value arguments of the captured engine calls: a change of
         # either needs its own graph instead of a replay of the old ones
         key = self._key(data) + (self.model.training, float(self.model.dropout))
-        ent = self._seen.get(key, "unseen")
-        if isinstance(ent, dict):
-            pass
-        elif ent == "ran-once" and len(self._seen) <= self.max_graphs:
-            ent = self._capture(data, key)
-        else:
-            if ent == "unseen":
-                self._seen[key] = "ran-once"
-            ent = None
-        if isinstance(ent, dict) and ent["ws_gen"] != ent["engine"].ws_generation:
-            # the engine re-allocated its workspace since the capture (a bigger batch came by): the captured kernels
-            # point into freed memory -> drop EVERY graph of that generation and start over on the eager path
-            self._seen = {k: "ran-once" for k in self._seen}
-            self.invalidations += 1
-            ent = None
-        if not isinstance(ent, dict):          # eager: first visit, capture failed, or too many keys
-            loss, _ = _fused_fwd_bwd(self.model, self.opt, data, self.tau, None, None)
-            return self._finish(loss)
-        ent["graph"].replay()
-        ops.LAUNCHES["n"] += ent["launches"]
-        self.replays += 1
-        return self._finish(ent["loss"])
-
-    def _capture(self, data, key):
-        g = torch.cuda.CUDAGraph()
-        l0 = ops.LAUNCHES["n"]
-        try:
-            with torch.cuda.graph(g):
-                # the index is rebuilt inside the graph: the same buffers may hold another batch at replay time
-                loss, index = _fused_fwd_bwd(self.model, self.opt, data, self.tau, None, None, use_index_cache=False)
-        except Exception as e:  # noqa: BLE001 - any capture failure leaves this key on the eager path
-            self.capture_error = repr(e)
-            ops.LAUNCHES["n"] = l0
-            self._seen[key] = "failed"
-            torch.cuda.synchronize()
-            return None
-        n = ops.LAUNCHES["n"] - l0
-        ops.LAUNCHES["n"] = l0
-        eng = self.model._engine
-        ent = {"graph": g, "loss": loss, "index": index, "data": data, "launches": n, "engine": eng,
-               "ws_gen": eng.ws_generation, "ws": eng.ws}       # "ws" keeps the captured workspace alive
-        self._seen[key] = ent
-        return ent
+        # the index is built inside the step: the same buffers may hold another batch at replay time
+        loss, _ = self.cache(key, _engine_of(self.model, self.opt), _batch_sizes(data),
+                             lambda: _fused_fwd_bwd(self.model, self.opt, data, self.tau, None, None,
+                                                    use_index_cache=False), pin=data)
+        return _reduce_and_step(self.opt, self.dp, loss)
 
 
 # ------------------------------------------------------------------------------------------ capacity buckets
@@ -515,45 +554,23 @@ class PaddedBatch:
         return self
 
 
-def _batch_sizes(data):
-    return int(data.x.size(0)), int(data.edge_index.size(1)), int(data.num_graphs)
-
-
-def _stale(ent, eng):
-    """A captured graph of bucket entry ``ent`` may not be replayed with engine ``eng``: it was captured over another
-    engine (re-created after the parameters moved) or over a workspace the engine has since re-allocated."""
-    return ent["engine"] is not eng or ent["ws_gen"] != eng.ws_generation
-
-
-def _drop_graph(ent):
-    ent["state"] = "ran-once"
-    for k in ("graph", "loss", "index", "out", "engine", "ws", "ws_gen", "launches"):
-        ent.pop(k, None)
-
-
-class BucketedTrainStep:
+class BucketedTrainStep(_GraphCache):
     """``fused_train_step`` replayed from one CUDA graph per capacity bucket, for batches whose sizes and buffers
     change every step (a shuffled ``StoreLoader``: ``GraphedTrainStep`` keys on both and never replays there).
 
     Each batch is padded into the persistent buffers of its bucket ``bucket_caps(N, E, B)`` (``PaddedBatch``, one
     eager launch); the kernels run at the capacity sizes and read the real {N, B} from a device word where a count
     enters the arithmetic (BatchNorm statistics and backward, the loss), so the step computes what the unpadded step
-    computes for the real graphs.  Protocol of ``GraphedTrainStep``: the first visit of a bucket runs eagerly (on the
-    padded buffers), the second is captured, later ones replay.  A graph captured over an engine or workspace that has
-    since been replaced (a re-allocation for a bigger bucket, a re-created engine) is dropped and captured again on its
-    next visit (``invalidations``; ``reserve(*loader.max_sizes())`` sizes the workspace once up front).  Past
-    ``max_graphs`` buckets, after a failed capture (``capture_error``) and for a batch ``PaddedBatch`` cannot pad
-    (per-pattern probabilities only) the step runs eager ``fused_train_step`` on the unpadded batch.
-    ``pad_ratio`` = sum of N_cap / sum of N over the padded steps."""
+    computes for the real graphs.  Eager first visit, capture, replays and ``max_graphs`` as in ``_GraphCache``: past
+    ``max_graphs`` buckets and after a failed capture the padded step runs eagerly.  A graph captured over an engine or
+    workspace that has since been replaced (a re-allocation for a bigger bucket, a re-created engine) is captured again
+    (``invalidations``; ``reserve(*loader.max_sizes())`` sizes the workspace once up front).  A batch ``PaddedBatch``
+    cannot pad (per-pattern probabilities only) runs eager ``fused_train_step``.  ``pad_ratio`` = sum of N_cap / sum
+    of N over the padded steps."""
 
     def __init__(self, model, optimizer: FusedAdam, tau=0.5, dp: DataParallel | None = None, max_graphs=32):
+        super().__init__(max_graphs)
         self.model, self.opt, self.tau, self.dp = model, optimizer, tau, dp
-        self.max_graphs = max_graphs
-        self._buckets = {}   # key -> {"buf": PaddedBatch, "state": "ran-once" | "failed" | "graph", ...}
-        self.capture_error = None
-        self.replays = 0
-        self.captures = 0
-        self.invalidations = 0
         self._n_real = 0
         self._n_cap = 0
 
@@ -561,73 +578,22 @@ class BucketedTrainStep:
     def pad_ratio(self):
         return self._n_cap / max(self._n_real, 1)
 
-    def _engine(self):
-        m = self.model
-        return m.engine(self.opt.fp) if (m._engine is None or m._engine.fp is not self.opt.fp) else m._engine
-
     def reserve(self, N, E, B):
         """Sizes the engine workspace for every bucket of a batch of at most N nodes, E edges and B graphs."""
-        self._engine().reserve(*bucket_bound(N, E, B))
-
-    def _finish(self, loss):
-        with torch.no_grad():
-            scale = self.dp.all_reduce_grads(self.opt) if self.dp is not None else 1.0
-            self.opt.step(grad_scale=scale)
-        return loss
+        _engine_of(self.model, self.opt).reserve(*bucket_bound(N, E, B))
 
     def __call__(self, data):
         if not PaddedBatch.accepts(data):
             return fused_train_step(self.model, self.opt, data, self.tau, self.dp)
-        N, E, B = _batch_sizes(data)
-        caps = bucket_caps(N, E, B)
+        bucket, buf = self.pad(data)
+        self._n_real += int(data.x.size(0))
+        self._n_cap += buf.caps[0]
         # training flag and dropout rate are by-value arguments of the captured calls: each needs its own graph
-        key = caps + (int(data.edge_attr.size(1)), self.model.training, float(self.model.dropout))
-        ent = self._buckets.get(key)
-        if ent is None:
-            if len(self._buckets) >= self.max_graphs:
-                return fused_train_step(self.model, self.opt, data, self.tau, self.dp)
-            ent = self._buckets[key] = {"buf": PaddedBatch(caps, data), "state": "new"}
-        if ent["state"] == "failed":
-            return fused_train_step(self.model, self.opt, data, self.tau, self.dp)
-        buf = ent["buf"].fill(data)
-        self._n_real += N
-        self._n_cap += caps[0]
-        eng = self._engine()
-        if ent["state"] == "graph" and _stale(ent, eng):
-            _drop_graph(ent)
-            self.invalidations += 1
-        if ent["state"] == "new":
-            ent["state"] = "ran-once"
-            loss, _ = _fused_fwd_bwd(self.model, self.opt, buf, self.tau, None, None, use_index_cache=False,
-                                     live=buf.live)
-            return self._finish(loss)
-        if ent["state"] == "ran-once" and not self._capture(ent):
-            return fused_train_step(self.model, self.opt, data, self.tau, self.dp)
-        ent["graph"].replay()
-        ops.LAUNCHES["n"] += ent["launches"]
-        self.replays += 1
-        return self._finish(ent["loss"])
-
-    def _capture(self, ent):
-        buf = ent["buf"]
-        g = torch.cuda.CUDAGraph()
-        l0 = ops.LAUNCHES["n"]
-        try:
-            with torch.cuda.graph(g):
-                loss, index = _fused_fwd_bwd(self.model, self.opt, buf, self.tau, None, None, use_index_cache=False,
-                                             live=buf.live)
-        except Exception as e:  # noqa: BLE001 - a failed capture leaves this bucket on the eager unpadded path
-            self.capture_error = repr(e)
-            ops.LAUNCHES["n"] = l0
-            ent["state"] = "failed"
-            torch.cuda.synchronize()
-            return False
-        eng = self.model._engine
-        ent.update(state="graph", graph=g, loss=loss, index=index, launches=ops.LAUNCHES["n"] - l0, engine=eng,
-                   ws_gen=eng.ws_generation, ws=eng.ws)      # "engine" / "ws" keep what the graph points into alive
-        ops.LAUNCHES["n"] = l0
-        self.captures += 1
-        return True
+        key = bucket + (self.model.training, float(self.model.dropout))
+        loss, _ = self.cache(key, _engine_of(self.model, self.opt), buf.caps,
+                             lambda: _fused_fwd_bwd(self.model, self.opt, buf, self.tau, None, None,
+                                                    use_index_cache=False, live=buf.live), pin=buf)
+        return _reduce_and_step(self.opt, self.dp, loss)
 
 
 class AsyncLossReader:
@@ -719,60 +685,15 @@ def evaluate(model, loader, device, tau=0.5):
     return m.result()
 
 
-class _BucketState:
-    """Padded buffers and captured graph of every capacity bucket one bucketed forward has seen (``_bucket_run``)."""
+def _padded_forward(model, eng, buf):
+    """Index build + eval-mode engine forward of a ``PaddedBatch`` -> (global_pred, local_pred, index)."""
+    from .index import build_index
 
-    def __init__(self):
-        self.buckets = {}    # key -> {"buf": PaddedBatch, "state": "new" | "ran-once" | "graph", "eager": bool, ...}
-        self.capture_error = None
-        self.captures = 0
-        self.replays = 0
-
-
-class _BucketedEval(_BucketState):
-    """Per-model state of ``evaluate_bucketed``: the metric sums (one device buffer the graphs add into) and the
-    padded buffers + forward/metrics graph of every bucket seen so far."""
-
-    def __init__(self, device, tau):
-        super().__init__()
-        self.metrics = EvalMetrics(device, tau)
-
-
-def _bucket_run(st: _BucketState, data, eng, run, max_graphs):
-    """Pads ``data`` into the buffers of its capacity bucket in ``st`` and runs ``run(buf)`` on them: eagerly on the
-    bucket's first visit, captured into a CUDA graph on the second and replayed from then on.  A graph captured over an
-    engine or workspace that has since been replaced is captured again; buckets beyond ``max_graphs`` and failed
-    captures (``st.capture_error``) stay eager.  -> what ``run`` returned (on a replay: the tensors of the capture,
-    which the replay has just rewritten)."""
-    N, E, B = _batch_sizes(data)
-    caps = bucket_caps(N, E, B)
-    key = caps + (int(data.edge_attr.size(1)),)
-    ent = st.buckets.get(key)
-    if ent is None:
-        ent = st.buckets[key] = {"buf": PaddedBatch(caps, data), "state": "new",
-                                 "eager": len(st.buckets) >= max_graphs}
-    buf = ent["buf"].fill(data)
-    eng._workspace(*caps)
-    if ent["state"] == "graph" and _stale(ent, eng):
-        _drop_graph(ent)
-    if ent["state"] == "ran-once" and not ent.get("eager"):
-        g = torch.cuda.CUDAGraph()
-        try:
-            with torch.cuda.graph(g):
-                out = run(buf)
-            ent.update(state="graph", graph=g, out=out, engine=eng, ws_gen=eng.ws_generation, ws=eng.ws)
-            st.captures += 1
-        except Exception as e:  # noqa: BLE001 - this bucket stays eager
-            st.capture_error = repr(e)
-            torch.cuda.synchronize()
-            ent["eager"] = True
-    if ent["state"] == "graph":
-        ent["graph"].replay()
-        st.replays += 1
-        return ent["out"]
-    if ent["state"] == "new":
-        ent["state"] = "ran-once"
-    return run(buf)
+    x, cat_X, edge_index, edge_attr, pnn, probs, entry_id, batch = model_inputs(buf)
+    index = build_index(edge_index, x.size(0), edge_attr, model.interface_embeds.num_embeddings,
+                        model.rpctype_embeds.num_embeddings, check=False)
+    gpred, lpred = eng.forward(x, cat_X, entry_id, probs, pnn, batch, index, False, live=buf.live)
+    return gpred, lpred, index
 
 
 @torch.no_grad()
@@ -789,22 +710,20 @@ def evaluate_bucketed(model, loader, device, tau=0.5, max_graphs=32):
         device = torch.device("cuda", torch.cuda.current_device())
     st = model.__dict__.get("_bucketed_eval")
     if st is None or st.metrics.acc.device != device or st.metrics.tau != float(tau):
-        st = model.__dict__["_bucketed_eval"] = _BucketedEval(device, tau)
+        # the graphs add into these metric sums: new sums, new graphs
+        st = model.__dict__["_bucketed_eval"] = _GraphCache()
+        st.metrics = EvalMetrics(device, tau)
+    st.max_graphs = max_graphs
     m = st.metrics
     m.reset()
     eng = model.engine()
-    n_if, n_rpc = model.interface_embeds.num_embeddings, model.rpctype_embeds.num_embeddings
 
     def run(buf):
-        from .index import build_index
-
-        x, cat_X, edge_index, edge_attr, pnn, probs, entry_id, batch = model_inputs(buf)
-        index = build_index(edge_index, x.size(0), edge_attr, n_if, n_rpc, check=False)
-        gpred, _ = eng.forward(x, cat_X, entry_id, probs, pnn, batch, index, False, live=buf.live)
-        _lib.call("pert_eval_metrics_live", _lib.ptr(buf.y), _lib.ptr(gpred), m.tau, buf.y.numel(),
+        out = _padded_forward(model, eng, buf)
+        _lib.call("pert_eval_metrics_live", _lib.ptr(buf.y), _lib.ptr(out[0]), m.tau, buf.y.numel(),
                   _lib.ptr(m.acc), _lib.ptr(buf.live), _lib.stream())
         ops.LAUNCHES["n"] += 1
-        return gpred, index
+        return out
 
     with torch.cuda.device(device):
         for data in loader:
@@ -813,25 +732,10 @@ def evaluate_bucketed(model, loader, device, tau=0.5, max_graphs=32):
                 eval_step(model, data, tau, m)
                 continue
             m.count += int(data.num_graphs)
-            _bucket_run(st, data, eng, run, max_graphs)
+            bucket, buf = st.pad(data)
+            st.cache(bucket, eng, buf.caps, lambda: run(buf), pin=buf)
     model.train(was_training)
     return m.result()
-
-
-class _BucketedPredict(_BucketState):
-    """Per-model state of ``predict``: the padded buffers + forward graph of every bucket seen so far, and a zero label
-    column for ``PaddedBatch.fill`` (requests have no label; the pad kernel, which runs eagerly in front of every
-    replay, is the only reader, so one buffer serves every bucket)."""
-
-    def __init__(self, device):
-        super().__init__()
-        self.device = device
-        self.zero_y = torch.zeros(0, dtype=torch.int64, device=device)
-
-    def labels(self, B):
-        if self.zero_y.numel() < B:
-            self.zero_y = torch.zeros(B, dtype=torch.int64, device=self.device)
-        return self.zero_y[:B]
 
 
 @torch.no_grad()
@@ -879,8 +783,14 @@ def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, lo
     try:
         with torch.cuda.device(dev):
             st = model.__dict__.get("_bucketed_predict")
-            if st is None or st.device != dev:
-                st = model.__dict__["_bucketed_predict"] = _BucketedPredict(dev)
+            if st is None or st.zero_y.device != dev:
+                st = model.__dict__["_bucketed_predict"] = _GraphCache()
+                st.zero_y = torch.zeros(0, dtype=torch.int64, device=dev)
+            st.max_graphs = max_graphs
+            if st.zero_y.numel() < min(bs, Q):
+                # requests have no label: the pad kernel, which runs eagerly in front of every replay, is the only
+                # reader of this zero column, so one buffer serves every bucket
+                st.zero_y = torch.zeros(min(bs, Q), dtype=torch.int64, device=dev)
             eng = model.engine()
             gpred = torch.empty(Q, dtype=torch.float32, device=dev)
             lpred = torch.empty(int(node_ptr[-1]), dtype=torch.float32, device=dev) if local else None
@@ -891,22 +801,13 @@ def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, lo
                 if not what_if:
                     ent_d = torch.from_numpy(ent).to(dev, non_blocking=True)
                     ts_d = torch.from_numpy(ts).to(dev, non_blocking=True)
-            n_if, n_rpc = model.interface_embeds.num_embeddings, model.rpctype_embeds.num_embeddings
-
-            def run(buf):
-                from .index import build_index
-
-                x, cat_X, edge_index, edge_attr, pnn, probs, entry_id, batch = model_inputs(buf)
-                index = build_index(edge_index, x.size(0), edge_attr, n_if, n_rpc, check=False)
-                g, loc = eng.forward(x, cat_X, entry_id, probs, pnn, batch, index, False, live=buf.live)
-                return g, loc, index
-
             for i in range(0, Q, bs):
                 j = min(i + bs, Q)
                 arrays = w.slice(i, j) if what_if else (ent_d[i:j], ts_d[i:j])
                 data = store.assemble_requests(ent[i:j], None, asof=asof, device_arrays=arrays)
-                data.y = st.labels(j - i)
-                g, loc, _ = _bucket_run(st, data, eng, run, max_graphs)
+                data.y = st.zero_y[:j - i]
+                bucket, buf = st.pad(data)
+                g, loc, _ = st.cache(bucket, eng, buf.caps, lambda: _padded_forward(model, eng, buf), pin=buf)
                 gpred[i:j].copy_(g[:j - i, 0])
                 if local:
                     lpred[node_ptr[i]:node_ptr[j]].copy_(loc[:node_ptr[j] - node_ptr[i], 0])

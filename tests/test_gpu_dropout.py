@@ -197,10 +197,10 @@ def test_eval_ignores_dropout():
     assert _state(model) == [SEED, 0]
 
 
-def test_counter_under_graph_replay():
+def test_counter_under_graph_replay_and_a_new_rate():
     """GraphedTrainStep (eager, capture + replay, replays on two keys) against fused_train_step on a copy seeded alike:
     same losses, both counters at 8, and a replay draws the mask of ITS step, not the captured one.  Changing the rate
-    re-captures."""
+    is a new key: eager once, then exactly one capture."""
     from pert_gnn_kdd23_b200.train import FlatParams, FusedAdam, GraphedTrainStep, fused_train_step
 
     _, model_a = make_models(2)
@@ -231,14 +231,13 @@ def test_counter_under_graph_replay():
     assert int(((x1 != 0) & ~now).sum()) == 0
     assert int(((x1 != 0) & ~captured).sum()) > 0
     # a new rate is a new key: eager once, then captured and replayed with the new rate
-    graphs = lambda: sum(isinstance(v, dict) for v in step_b._seen.values())  # noqa: E731
-    n_graphs = graphs()
+    c0 = step_b.captures
     model_a.dropout = model_b.dropout = 0.3
     for it in range(2):
         la = fused_train_step(model_a, opt_a, batches[0], 0.5)
         lb = step_b(batches[0])
         assert_close(lb, la, rtol=1e-4, what=f"loss step {it} at p=0.3")
-    assert graphs() == n_graphs + 1 and step_b.replays == 7
+    assert step_b.captures == c0 + 1 and step_b.replays == 7
     torch.cuda.synchronize()
     assert _state(model_b) == [SEED, 10]
     x1 = _saved_acts(model_b, N, E, B)[1].cpu()

@@ -108,10 +108,10 @@ __global__ void __launch_bounds__(256) k_bn_partial(const float* __restrict__ x,
     }
   if (rl < rl_n) st4(s_red + rl * H + cl * 4, s);
   __syncthreads();
-  if (threadIdx.x < H) {
+  for (int c = threadIdx.x; c < H; c += blockDim.x) {   // H > 256: a thread owns several columns
     float t = 0.f;
-    for (int i = 0; i < rl_n; ++i) t += s_red[i * H + threadIdx.x];
-    s_mean[threadIdx.x] = t / (float)rows;
+    for (int i = 0; i < rl_n; ++i) t += s_red[i * H + c];
+    s_mean[c] = t / (float)rows;
   }
   __syncthreads();
   float4 mu = (rl < rl_n) ? ld4(s_mean + cl * 4) : f4zero();
@@ -134,12 +134,12 @@ __global__ void __launch_bounds__(256) k_bn_partial(const float* __restrict__ x,
   __syncthreads();
   if (rl < rl_n) st4(s_red + rl * H + cl * 4, q);
   __syncthreads();
-  if (threadIdx.x < H) {
+  for (int c = threadIdx.x; c < H; c += blockDim.x) {
     float t = 0.f;
-    for (int i = 0; i < rl_n; ++i) t += s_red[i * H + threadIdx.x];
-    const double m = (double)s_mean[threadIdx.x], n = (double)rows;
-    atomicAdd(acc + threadIdx.x, n * m);
-    atomicAdd(acc + H + threadIdx.x, (double)t + n * m * m);
+    for (int i = 0; i < rl_n; ++i) t += s_red[i * H + c];
+    const double m = (double)s_mean[c], n = (double)rows;
+    atomicAdd(acc + c, n * m);
+    atomicAdd(acc + H + c, (double)t + n * m * m);
   }
 }
 
@@ -605,10 +605,10 @@ int pert_bn_fwd_stats(const float* x, int ld_x, const float* running_mean, const
   if (training) {
     if (!workspace || workspace_bytes < pert_bn_workspace_bytes(N, H)) return PERT_ERR_BADARG;
     int chunks = pert_cdiv(N, BN_ROWS);
-    int vpr = H / 4;
-    int threads = 256;
-    if (threads < H) threads = (H + 31) / 32 * 32;
-    int rl_n = threads / vpr;
+    // 256 threads at every width (the kernel's launch bound): H <= 1024 gives H/4 <= 256 float4 lanes, so rl_n >= 1
+    const int vpr = H / 4;
+    const int threads = 256;
+    const int rl_n = threads / vpr;
     if (rl_n < 1) return PERT_ERR_UNSUPPORTED;
     size_t smem = ((size_t)rl_n * H + H) * sizeof(float);
     if (smem > 48 * 1024) return PERT_ERR_UNSUPPORTED;
@@ -713,9 +713,11 @@ extern "C" {
 int pert_pool_fwd(const float* x, int ld, const float* probs, const float* pnn, const int64_t* batch,
                   const float* w_local, const float* b_local, float* local, float* pool, long long N, long long B,
                   int H, int* status, void* stream) {
-  if (N < 0 || B < 0 || !x || !probs || !pnn || !batch || !pool || ld % 4 || !al16(x) || !al16(w_local) ||
-      !al16(pool))
+  // an empty batch (N = 0) or pool (B = 0) may come with NULL pointers (empty tensors)
+  if (N < 0 || B < 0 || (N > 0 && (!x || !probs || !pnn || !batch)) || (B > 0 && !pool) || ld % 4 || !al16(x) ||
+      !al16(w_local) || !al16(pool))
     return PERT_ERR_BADARG;
+  if (dispatch_h(H, [](auto, auto) { return PERT_OK; }) != PERT_OK) return PERT_ERR_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
   if (B > 0) {
     cudaError_t e = cudaMemsetAsync(pool, 0, sizeof(float) * B * H, st);
@@ -738,8 +740,8 @@ int pert_pool_fwd(const float* x, int ld, const float* probs, const float* pnn, 
 int pert_pool_bwd(const float* dpool, const float* dlocal, const float* x, int ld, const float* probs,
                   const float* pnn, const int64_t* batch, const float* w_local, float* dx, int ld_dx,
                   float* dw_local, float* db_local, long long N, long long B, int H, void* stream) {
-  if (N < 0 || !probs || !pnn || !batch || !dx || ld % 4 || ld_dx % 4 || !al16(dpool) || !al16(x) ||
-      !al16(w_local) || !al16(dx))
+  if (N < 0 || B < 0 || (N > 0 && (!probs || !pnn || !batch || !dx)) || ld % 4 || ld_dx % 4 || !al16(dpool) ||
+      !al16(x) || !al16(w_local) || !al16(dx))
     return PERT_ERR_BADARG;
   if (dlocal && (!x || !w_local)) return PERT_ERR_BADARG;
   if (N == 0) return PERT_OK;

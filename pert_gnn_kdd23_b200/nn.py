@@ -48,14 +48,30 @@ class Linear(torch.nn.Module):
 
 
 class BatchNorm1d(torch.nn.BatchNorm1d):
-    """torch.nn.BatchNorm1d (reference model.py:33,43) with an optional fused ReLU epilogue."""
+    """torch.nn.BatchNorm1d (reference model.py:33,43) over [N, C] input, with an optional fused ReLU epilogue.
+
+    ``affine=False`` normalises with unit scale and zero shift.  Not implemented, and refused before anything runs:
+    the [N, C, L] input form and ``momentum=None`` (the cumulative moving average) when the running statistics are
+    updated.  A training batch of one row raises torch's ValueError."""
 
     def forward(self, x, relu=False):
+        if x.dim() != 2:
+            if x.dim() == 3:
+                raise NotImplementedError("BatchNorm1d: only [N, C] input is implemented, not [N, C, L]")
+            raise ValueError(f"expected 2D or 3D input (got {x.dim()}D input)")
         training = self.training or (self.running_mean is None)
+        updates = self.training and self.running_mean is not None
+        if updates and self.momentum is None:
+            raise NotImplementedError("BatchNorm1d(momentum=None): the cumulative moving average is not implemented")
+        if training and x.size(0) == 1:
+            raise ValueError(f"Expected more than 1 value per channel when training, got input size {x.size()}")
+        weight, bias = self.weight, self.bias
+        if not self.affine:
+            weight = torch.ones(self.num_features, device=x.device, dtype=torch.float32)
+            bias = torch.zeros(self.num_features, device=x.device, dtype=torch.float32)
         mom = 0.0 if self.momentum is None else self.momentum
-        return ops.batch_norm(x, self.weight, self.bias, self.running_mean, self.running_var,
-                              self.num_batches_tracked if (self.training and self.track_running_stats) else None,
-                              training, self.eps, mom, relu)
+        return ops.batch_norm(x, weight, bias, self.running_mean, self.running_var,
+                              self.num_batches_tracked if updates else None, training, self.eps, mom, relu)
 
 
 class TransformerConv(torch.nn.Module):
@@ -134,8 +150,11 @@ def _edge_row_index(edge_index, N):
 
 
 def global_add_pool(x, batch, size=None):
-    """torch_geometric.nn.global_add_pool (reference model.py:107).  ``size`` avoids PyG's batch.max() sync."""
-    if size is None:
+    """torch_geometric.nn.global_add_pool (reference model.py:107).  ``size`` avoids PyG's batch.max() sync;
+    ``batch=None`` sums all rows into one [1, H] graph, as PyG does."""
+    if batch is None:
+        batch, size = torch.zeros(x.size(0), device=x.device, dtype=torch.int64), 1
+    elif size is None:
         size = int(batch.max()) + 1 if batch.numel() else 0
     ones = torch.ones(x.size(0), device=x.device)
     pool, _ = ops.pool_local(x, ones, ones, batch, None, None, size)

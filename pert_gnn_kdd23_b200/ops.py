@@ -381,14 +381,17 @@ class _BatchNormFn(torch.autograd.Function):
         N, H = x.shape
         dy = _c(_pad_cols(dy, H))
         dx = torch.empty_like(x)
-        dgamma = torch.zeros(H, device=x.device, dtype=torch.float32)
-        dbeta = torch.zeros(H, device=x.device, dtype=torch.float32)
+        # a scale / shift that is no parameter (BatchNorm1d(affine=False)) gets no gradient
+        dgamma = torch.zeros(H, device=x.device, dtype=torch.float32) if ctx.needs_input_grad[1] else None
+        dbeta = torch.zeros(H, device=x.device, dtype=torch.float32) if ctx.needs_input_grad[2] else None
         sums = torch.empty(2 * H, device=x.device, dtype=torch.float32)
         call("pert_bn_bwd", ptr(dy), dy.stride(0), ptr(y), H, ptr(x), H, ptr(stats[0]), ptr(stats[1]), ptr(gamma),
              int(relu), int(training), ptr(dx), H, ptr(dgamma), ptr(dbeta), ptr(sums), N, H, stream())
         LAUNCHES["n"] += 2
         if H != H0:
-            dx, dgamma, dbeta = dx[:, :H0], dgamma[:H0], dbeta[:H0]
+            dx = dx[:, :H0]
+            dgamma = dgamma[:H0] if dgamma is not None else None
+            dbeta = dbeta[:H0] if dbeta is not None else None
         return dx, dgamma, dbeta, None, None, None, None, None, None, None
 
 

@@ -49,7 +49,8 @@ extern "C" {
  * pert_model_backward_live, pert_pinball_loss_live, pert_eval_metrics_live; pert_tconv_fwd_c, pert_tconv_bwd_c,
  * pert_model_width (the step engine accepts every hidden width 1..256); pert_trace_group_* (trace grouping);
  * pert_store_assemble_requests (request assembly with the exact or as-of resource join); pert_store_resources_count /
- * _merge (appending and evicting resource rows of a live store); pert_ingest_* (appending traces to a live store);
+ * _merge (appending and evicting resource rows of a live store), pert_store_resources_update_count / _update_merge
+ * (replacing and deleting them by key); pert_ingest_* (appending traces to a live store);
  * pert_ingest_evict_* (evicting traces from a live store); pert_store_assemble_whatif (per-request pattern mixes and
  * resource overrides), pert_store_lookup_resources; pert_raw_* (processed tables from raw rows). */
 int pert_version(void);
@@ -533,7 +534,7 @@ int pert_store_lookup_resources(const PertStore* store, const PertResourceAsOf* 
  * equal, bit for bit, what the store's constructor builds from the surviving rows in arrival order (the old rows first,
  * in their table order, then the batch in input order): res_keys sorted with equal keys in arrival order, res_vals,
  * ms_has_res [n_ms] = 1 iff ms keeps a row, and the as-of index of those keys.  No old row is re-sorted; equal keys are
- * all kept (the joins read the first), so a later row never replaces an earlier one.
+ * all kept (the joins read the first), so a later row never replaces an earlier one: that is the update pair below.
  * Inputs, all device arrays:
  *   store, asof: the current table (store->res_keys, res_vals, n_res, n_ms >= 1) and its index (ts / row may be NULL
  *     when n_res = 0); only these fields of the store are read;
@@ -562,6 +563,35 @@ int pert_store_resources_merge(const PertStore* store, const PertResourceAsOf* a
                                const int32_t* ms_ptr_out, const int32_t* seg, long long p, long long q,
                                long long n_out, int64_t* keys_out, float* vals_out, uint8_t* has_out, int64_t* ts_out,
                                int32_t* row_out, void* stream);
+
+/* Replacing and deleting resource rows by key (PatternStore.append_resources(replace=True), delete_resources): the same
+ * two calls with a drop set, whose keys' old rows all leave the table before the batch goes in.  With L the rows in
+ * arrival order and D the drop set, the result is what the constructor builds from [r in L : key(r) not in D and
+ * timestamp(r) >= evict_before] followed by the surviving batch rows in input order.  A replace passes its batch's
+ * keys as D and the last row of each key as the batch, a delete passes D and no batch, and D empty is the plain append.
+ *   drop_keys [n_drop] int64: sorted ascending, unique (0 <= ms < n_ms); drop_group [n_drop] int32: positions into
+ *     drop_keys ordered by (ms, position), as new_group;
+ *   drop_cnt [2 * (n_drop + 1)] int32: written by the count, read by the merge: the old rows at or above the cut each
+ *     drop key removes, as exclusive scans in key order and in drop_group order, each followed by its total;
+ *   seg [3 * n_ms + 1] int32: pert_store_resources_count's two parts, then the first drop_group position of every
+ *     microservice and n_drop;
+ *   sizes [4] int64 = {p, q, n_out, n_dropped}: n_dropped = the old rows the drop set removes (rows it names below
+ *     the cut are counted in p), n_out = (n_res - p - n_dropped) + (k - q).
+ * The merge takes drop_cnt, seg, p, q, n_dropped and n_out as the count left them.  Arguments, outputs and refusals
+ * as pert_store_resources_count / _merge; also PERT_ERR_BADARG for n_drop < 0 or >= 2^31 - 1, NULL drop arrays with
+ * n_drop > 0, a NULL drop_cnt, and n_dropped outside [0, n_res - p] or above 0 with n_drop = 0. */
+int pert_store_resources_update_count(const PertStore* store, const PertResourceAsOf* asof, const int64_t* drop_keys,
+                                      const int32_t* drop_group, long long n_drop, const int64_t* new_keys,
+                                      const int32_t* new_group, long long k, long long evict_before,
+                                      int32_t* drop_cnt, int32_t* ms_ptr_out, int32_t* seg, long long* sizes,
+                                      void* stream);
+int pert_store_resources_update_merge(const PertStore* store, const PertResourceAsOf* asof, const int64_t* drop_keys,
+                                      const int32_t* drop_group, const int32_t* drop_cnt, long long n_drop,
+                                      const int64_t* new_keys, const int64_t* new_perm, const float* new_vals,
+                                      const int32_t* new_group, long long k, const int32_t* ms_ptr_out,
+                                      const int32_t* seg, long long p, long long q, long long n_dropped,
+                                      long long n_out, int64_t* keys_out, float* vals_out, uint8_t* has_out,
+                                      int64_t* ts_out, int32_t* row_out, void* stream);
 
 /* ---- trace ingest: appending traces to a live store (csrc/ingest.cu) ------------------------------------------------
  * A chunk of span rows, grouped on its own by pert_trace_group_*, is taken into a store whose patterns are runtimes

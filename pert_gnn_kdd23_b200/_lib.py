@@ -74,6 +74,9 @@ SIGNATURES = {
     # resource updates of a live store (csrc/resources.cu; first two arguments: PertStore*, PertResourceAsOf*)
     "pert_store_resources_count": (I, [P, P, P, P, LL, LL, P, P, P, P]),
     "pert_store_resources_merge": (I, [P, P, P, P, P, P, LL, P, P, LL, LL, LL, P, P, P, P, P, P]),
+    "pert_store_resources_update_count": (I, [P, P, P, P, LL, P, P, LL, LL, P, P, P, P, P]),
+    "pert_store_resources_update_merge": (I, [P, P, P, P, P, LL, P, P, P, P, LL, P, P, LL, LL, LL, LL, P, P, P, P, P,
+                                              P]),
     # trace ingest of a live store (csrc/ingest.cu; struct pointers, see store.py)
     "pert_ingest_table_insert": (I, [P, LL, P, P]),
     "pert_ingest_match_workspace_bytes": (LL, [LL]),

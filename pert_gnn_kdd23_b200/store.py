@@ -570,18 +570,7 @@ class PatternStore:
 
     def _resource_batch(self, resource_index, resource_values):
         """Checked (ts, ms, values) of an update on the store's device: int64 [k], int64 [k], float32 [k, 8]."""
-        dev, n_ms = self.device, self.n_ms
-        if torch.is_tensor(resource_index) and resource_index.is_cuda:
-            if resource_index.dtype.is_floating_point or resource_index.dtype.is_complex or \
-                    resource_index.dtype == torch.bool:
-                raise _lib.PertGnnError(f"resource_index: integer (timestamp, ms) pairs expected, got "
-                                        f"{resource_index.dtype}")
-            idx = resource_index.to(dev, torch.int64)
-        else:
-            idx = _index_rows(resource_index.numpy() if torch.is_tensor(resource_index) else resource_index)
-        if idx.ndim != 2 or idx.shape[1] != 2:
-            raise _lib.PertGnnError(f"resource_index: [k, 2] (timestamp, ms) pairs expected, got shape "
-                                    f"{tuple(idx.shape)}")
+        idx = self._index_array(resource_index)
         k = int(idx.shape[0])
         vals = resource_values
         if not (torch.is_tensor(vals) and vals.is_cuda):
@@ -593,31 +582,60 @@ class PatternStore:
                 vals = vals.reshape(0, 8)
         if tuple(vals.shape) != (k, 8):
             raise _lib.PertGnnError(f"resource_values: shape {tuple(vals.shape)}, expected ({k}, 8) for {k} rows")
-        if torch.is_tensor(idx):
-            ts, ms = idx[:, 0].contiguous(), idx[:, 1].contiguous()
-            if k:
-                lo, hi = _key_bounds(n_ms)
-                mm = torch.stack([ms.min(), ms.max(), ts.min(), ts.max()]).tolist()   # one device -> host read
-                if mm[0] < 0 or mm[1] >= n_ms or mm[2] < lo or mm[3] > hi:
-                    _check_resource_rows(ts.cpu().numpy(), ms.cpu().numpy(), n_ms)
-        else:
-            ts, ms = idx[:, 0], idx[:, 1]
-            _check_resource_rows(ts, ms, n_ms)
-            ts, ms = (torch.from_numpy(np.ascontiguousarray(c)).to(dev) for c in (ts, ms))
+        ts, ms = self._index_columns(idx)
         if torch.is_tensor(vals):
-            vals = vals.to(dev)
+            vals = vals.to(self.device)
             vals = (vals if vals.dtype == torch.float32 else vals.double().float()).contiguous()
             if vals.data_ptr() % 16:                     # the merge reads rows with 16-byte vector loads
                 vals = vals.clone()
         else:
-            vals = torch.from_numpy(vals.astype(np.float32)).to(dev)    # the constructor's float64 -> float32 rounding
+            vals = torch.from_numpy(vals.astype(np.float32)).to(self.device)  # the constructor's float64 -> float32
         return ts, ms, vals
 
+    def _index_array(self, resource_index):
+        """[k, 2] integer (timestamp, ms) pairs of an update: an int64 tensor on the store's device for CUDA input, else
+        an int64 host array (``PertGnnError`` naming the first row that is not a pair of int64 integers)."""
+        if torch.is_tensor(resource_index) and resource_index.is_cuda:
+            if resource_index.dtype.is_floating_point or resource_index.dtype.is_complex or \
+                    resource_index.dtype == torch.bool:
+                raise _lib.PertGnnError(f"resource_index: integer (timestamp, ms) pairs expected, got "
+                                        f"{resource_index.dtype}")
+            idx = resource_index.to(self.device, torch.int64)
+        else:
+            idx = _index_rows(resource_index.numpy() if torch.is_tensor(resource_index) else resource_index)
+        if idx.ndim != 2 or idx.shape[1] != 2:
+            raise _lib.PertGnnError(f"resource_index: [k, 2] (timestamp, ms) pairs expected, got shape "
+                                    f"{tuple(idx.shape)}")
+        return idx
+
+    def _index_columns(self, idx):
+        """Checked (ts, ms) int64 [k] on the store's device of ``_index_array``'s pairs: ``PertGnnError`` naming the first
+        row whose microservice is outside [0, n_ms) or whose key overflows int64."""
+        n_ms = self.n_ms
+        if torch.is_tensor(idx):
+            ts, ms = idx[:, 0].contiguous(), idx[:, 1].contiguous()
+            if int(idx.shape[0]):
+                lo, hi = _key_bounds(n_ms)
+                mm = torch.stack([ms.min(), ms.max(), ts.min(), ts.max()]).tolist()   # one device -> host read
+                if mm[0] < 0 or mm[1] >= n_ms or mm[2] < lo or mm[3] > hi:
+                    _check_resource_rows(ts.cpu().numpy(), ms.cpu().numpy(), n_ms)
+            return ts, ms
+        ts, ms = idx[:, 0], idx[:, 1]
+        _check_resource_rows(ts, ms, n_ms)
+        return tuple(torch.from_numpy(np.ascontiguousarray(c)).to(self.device) for c in (ts, ms))
+
     @_lib.on_device_of
-    def append_resources(self, resource_index, resource_values, evict_before=None):
+    def append_resources(self, resource_index, resource_values, evict_before=None, replace=False):
         """Appends resource rows to the live store and, with ``evict_before``, drops every row whose timestamp is
         < ``evict_before`` (old rows and the appended ones alike), on the device: the sorted table and the as-of index
         are merged, not rebuilt (csrc/resources.cu, O(n + k log k) for n rows and k new ones).
+
+        ``replace=True`` gives the table dict-update semantics: every (timestamp, ms) key of the batch first removes all
+        the store's rows with that key (duplicates left by plain appends included), then the batch's last row of that
+        key, in input order, goes in.  A key the store does not hold is simply inserted.  The result is the constructor's
+        store of the old rows without the batch's keys, followed by those last rows in input order; the cut applies as
+        for a plain append.  It costs one more device -> host read (the number of distinct keys) and one binary search
+        per old row into the batch's keys.  ``replace=False`` (the default) keeps every row, as described below.
 
         ``resource_index``: the constructor's (timestamp, ms) pairs, or an integer array / CUDA tensor [k, 2] (floats
         are refused, not truncated); ``resource_values``: [k, 8], a host array (float64, rounded to float32 as the
@@ -625,7 +643,7 @@ class PatternStore:
         ``t["res_vals"]``, ``t["ms_has_res"]``, ``asof_t``) is bit for bit that of a store built by the constructor,
         with the same ``n_ms``, from the surviving rows in arrival order: the constructor's rows, then every append's in
         order.  Rows with equal (timestamp, ms) are all kept and the joins read the first to arrive: a later row does
-        not replace an earlier one (replacing values is not supported).  A microservice gains ``ms_has_res`` with its
+        not replace an earlier one unless the call has ``replace=True``.  A microservice gains ``ms_has_res`` with its
         first row and loses it with its last.
 
         Checked on the host before anything changes (``PertGnnError`` naming the first bad row; the store is left as it
@@ -638,15 +656,13 @@ class PatternStore:
         torch's caching allocator on that stream.  Other streams that read the store need the caller's
         synchronisation, as for any tensor, and a CUDA graph the caller captured around ``pert_store_assemble*`` holds
         the old pointers and has to be captured again (``train.predict`` assembles eagerly and needs nothing)."""
-        if evict_before is None:
-            cut = _I64_MIN
-        else:
-            cut = int(evict_before)
-            if not _I64_MIN <= cut <= _I64_MAX:
-                raise _lib.PertGnnError(f"evict_before = {cut} is outside int64")
+        cut = self._cut(evict_before)
         ts, ms, vals = self._resource_batch(resource_index, resource_values)
         k = int(ts.shape[0])
         if k == 0 and evict_before is None:
+            return self
+        if replace:
+            self._update_resources(ts * self.n_ms + ms, vals, cut, insert=True)
             return self
         dev, n_ms, i32 = self.device, self.n_ms, torch.int32
         L = _lib.lib()
@@ -674,6 +690,73 @@ class PatternStore:
             _lib.stream()), "pert_store_resources_merge")
         self._commit(out, asof=(ms_ptr, a_ts, a_row))
         return self
+
+    @_lib.on_device_of
+    def delete_resources(self, resource_index, evict_before=None):
+        """Removes every resource row whose (timestamp, ms) key is in ``resource_index`` and, with ``evict_before``,
+        every row whose timestamp is < ``evict_before``; returns the number of rows removed, by key and by the cut
+        together.  Keys the store does not hold and repeated keys are allowed and remove nothing more.  The result is
+        the constructor's store of the surviving rows in arrival order: the exact join then reports a deleted
+        ``(bucket, ms)`` row as missing (``PERT_ERR_RANGE``) while ``ms`` keeps other rows, the as-of join reads the
+        newest earlier row, and ``ms`` loses ``ms_has_res`` with its last row.
+
+        ``resource_index`` takes the formats of ``append_resources`` and the same host checks (microservice ids in
+        [0, n_ms), keys within int64; ``PertGnnError`` naming the first bad row, the store left as it was).  The count
+        comes from the sizes the update reads back anyway.  Ordered on the current stream, fresh arrays swapped in, as
+        ``append_resources``."""
+        cut = self._cut(evict_before)
+        ts, ms = self._index_columns(self._index_array(resource_index))
+        if int(ts.shape[0]) == 0 and evict_before is None:
+            return 0
+        return self._update_resources(ts * self.n_ms + ms, None, cut, insert=False)
+
+    def _cut(self, evict_before):
+        if evict_before is None:
+            return _I64_MIN
+        cut = int(evict_before)
+        if not _I64_MIN <= cut <= _I64_MAX:
+            raise _lib.PertGnnError(f"evict_before = {cut} is outside int64")
+        return cut
+
+    def _update_resources(self, keys, vals, cut, insert):
+        """The drop-set update of ``append_resources(replace=True)`` (``insert``: the last row of each key goes back in)
+        and ``delete_resources``: ``keys`` int64 [k] checked batch keys on the device, ``vals`` float32 [k, 8] or None.
+        Returns the number of rows removed."""
+        dev, n_ms, i32 = self.device, self.n_ms, torch.int32
+        L = _lib.lib()
+        nk, perm = torch.sort(keys, stable=True)
+        last = torch.ones_like(nk, dtype=torch.bool)
+        last[:-1] = nk[1:] != nk[:-1]                    # the last of each run of a stable sort: the last in input order
+        dk = nk[last]                                    # the drop set: sorted unique keys (one device -> host read)
+        dgrp = torch.sort(torch.remainder(dk, n_ms), stable=True)[1].to(i32)
+        n_drop = int(dk.shape[0])
+        # a replace inserts the drop set's keys (grouped alike), with the values of each key's last row
+        ik, iperm, igrp, k = (dk, perm[last], dgrp, n_drop) if insert else (dk[:0], perm[:0], dgrp[:0], 0)
+        cnt = torch.empty(2 * (n_drop + 1), dtype=i32, device=dev)
+        ms_ptr = torch.empty(n_ms + 1, dtype=i32, device=dev)
+        seg = torch.empty(3 * n_ms + 1, dtype=i32, device=dev)
+        sizes = torch.empty(4, dtype=torch.int64, device=dev)
+        _lib.check(L.pert_store_resources_update_count(
+            C.byref(self.desc), C.byref(self.asof_desc), dk.data_ptr(), dgrp.data_ptr(), n_drop, ik.data_ptr(),
+            igrp.data_ptr(), k, cut, cnt.data_ptr(), ms_ptr.data_ptr(), seg.data_ptr(), sizes.data_ptr(),
+            _lib.stream()), "pert_store_resources_update_count")
+        p, q, n_out, n_dropped = sizes.tolist()
+        if n_out > _I32_MAX:
+            raise _lib.PertGnnError(f"the update would leave {n_out} resource rows; a store holds at most 2^31 - 1")
+        if p == 0 and q == k and n_dropped == 0:
+            return 0                                     # nothing evicted, inserted or dropped
+        out = {"res_keys": torch.empty(n_out, dtype=torch.int64, device=dev),
+               "res_vals": torch.empty(n_out, 8, dtype=torch.float32, device=dev),
+               "ms_has_res": torch.empty(n_ms, dtype=torch.uint8, device=dev)}
+        a_ts, a_row = torch.empty(n_out, dtype=torch.int64, device=dev), torch.empty(n_out, dtype=i32, device=dev)
+        _lib.check(L.pert_store_resources_update_merge(
+            C.byref(self.desc), C.byref(self.asof_desc), dk.data_ptr(), dgrp.data_ptr(), cnt.data_ptr(), n_drop,
+            ik.data_ptr(), iperm.data_ptr(), vals.data_ptr() if insert else 0, igrp.data_ptr(), k, ms_ptr.data_ptr(),
+            seg.data_ptr(), p, q, n_dropped, n_out, out["res_keys"].data_ptr(), out["res_vals"].data_ptr(),
+            out["ms_has_res"].data_ptr(), a_ts.data_ptr(), a_row.data_ptr(), _lib.stream()),
+            "pert_store_resources_update_merge")
+        self._commit(out, asof=(ms_ptr, a_ts, a_row))
+        return p + n_dropped
 
     def evict_resources(self, before):
         """Drops every resource row whose timestamp is < ``before``: ``append_resources`` with no rows."""

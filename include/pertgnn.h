@@ -52,7 +52,8 @@ extern "C" {
  * _merge (appending and evicting resource rows of a live store), pert_store_resources_update_count / _update_merge
  * (replacing and deleting them by key); pert_ingest_* (appending traces to a live store);
  * pert_ingest_evict_* (evicting traces from a live store); pert_store_assemble_whatif (per-request pattern mixes and
- * resource overrides), pert_store_lookup_resources; pert_raw_* (processed tables from raw rows). */
+ * resource overrides), pert_store_lookup_resources; pert_raw_* (processed tables from raw rows); pert_raw_window_*
+ * (raw resource samples aggregated into the open buckets' statistics). */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -854,6 +855,39 @@ int pert_raw_process(const PertRawCalls* calls, long long N, const int64_t* orde
 int pert_raw_emit(const PertRawCalls* calls, long long N, const int64_t* order, long long G, const int64_t* g_ts,
                   const int64_t* g_ms, const PertRawOut* out, void* workspace, long long workspace_bytes,
                   void* stream);
+
+/* ---- the open-bucket sample window: raw resource samples -> running statistics (csrc/rawtable.cu) -------------------
+ * Continues preprocess.py:237-242 (groupby(["timestamp", "msname"]).agg([max, min, mean, median])) sample batch by
+ * sample batch: after any sequence of batches every open key's 8 statistics are bit for bit those
+ * pert_raw_resource_stats gives for the concatenation of the key's samples in arrival order.  The window is caller
+ * memory: keys[U] int64 (sorted unique ts * n_ms + ms), off[U+1] int32 run offsets (off[0] = 0, off[U] = S),
+ * state[U] of 80 bytes (the cpu and the memory fold: max, min, Kahan sum, compensation as doubles and the non-NaN count
+ * as int64) and cpu_run / mem_run [S] float64: each key's values ascending, NaN last (NaN equal to NaN, -0.0 == 0.0),
+ * ties in arrival order.  A batch of k samples comes as bkeys[k] sorted stably (arrival order within a key), perm[k]
+ * (sorted position -> input row of cpu / mem [k]) and cpu_sorted / mem_sorted [k]: every key's batch values ascending
+ * in that order at the key's positions of bkeys.  Samples with floor(key / n_ms) < seal are late: a prefix of bkeys,
+ * counted and skipped.  At most 2^31 - 16 keys, samples and batch samples.  The calls of one batch, in order:
+ *   pert_raw_window_count -> flags[2(k+1)] (scanned first-of-key flags), sizes[3] = {late samples, keys the batch
+ *                            touches u, keys after the merge U2}; the caller reads sizes and allocates the new window
+ *   pert_raw_window_merge -> the new window (U2 keys, S + k - late samples), ustart[u+1] (first batch position of each
+ *                            touched key, ustart[u] = k) and upos[u] (its slot in the new window), ascending by key
+ *   pert_raw_window_emit  -> index[n, 2] (timestamp, ms) and vals[n, 8] (STATS order) of slot[0..n) (or slots 0..n-1
+ *                            when slot is NULL).
+ * One workspace of pert_raw_window_workspace_bytes(U, k, U2) serves both count and merge (U2 <= U + k bounds it).
+ * Integer merge positions only: no atomics, every output written once, results independent of scheduling. */
+long long pert_raw_window_workspace_bytes(long long U, long long k, long long U2);
+int pert_raw_window_count(long long k, const int64_t* bkeys, long long n_ms, long long seal, long long U,
+                          const int64_t* keys, int* flags, int64_t* sizes, void* workspace, long long workspace_bytes,
+                          void* stream);
+int pert_raw_window_merge(long long U, long long S, const int64_t* keys, const int* off, const void* state,
+                          const double* cpu_run, const double* mem_run, long long k, const int64_t* bkeys,
+                          const int64_t* perm, const double* cpu, const double* mem, const double* cpu_sorted,
+                          const double* mem_sorted, const int* flags, long long n_late, long long u, long long U2,
+                          int64_t* keys2, int* off2, void* state2, double* cpu_run2, double* mem_run2, int* ustart,
+                          int* upos, void* workspace, long long workspace_bytes, void* stream);
+int pert_raw_window_emit(long long n, const int* slot, long long U, const int64_t* keys, const int* off,
+                         const void* state, const double* cpu_run, const double* mem_run, long long n_ms,
+                         int64_t* index, double* vals, void* stream);
 
 #ifdef __cplusplus
 }

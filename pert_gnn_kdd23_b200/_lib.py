@@ -106,6 +106,12 @@ SIGNATURES = {
     "pert_raw_process_workspace_bytes": (LL, [P, LL]),
     "pert_raw_process": (I, [P, LL, P, P, LL, P, P, LL, P]),
     "pert_raw_emit": (I, [P, LL, P, LL, P, P, P, P, LL, P]),
+    # the open-bucket sample window (rawtable.ResourceSampleWindow)
+    "pert_raw_window_workspace_bytes": (LL, [LL, LL, LL]),
+    "pert_raw_window_count": (I, [LL, P, LL, LL, LL, P, P, P, P, LL, P]),
+    "pert_raw_window_merge": (I, [LL, LL, P, P, P, P, P, LL, P, P, P, P, P, P, P, LL, LL, LL, P, P, P, P, P, P, P, P,
+                                  LL, P]),
+    "pert_raw_window_emit": (I, [LL, P, LL, P, P, P, P, P, LL, P, P, P]),
     # whole-model engine (first argument: const PertModelDesc*, see engine.py)
     "pert_model_width": (I, [I]),
     "pert_model_workspace_bytes": (LL, [P, LL, LL, LL]),

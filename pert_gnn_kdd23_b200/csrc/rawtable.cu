@@ -38,6 +38,7 @@ namespace {
 constexpr int RW_NONE = 0x7f7f7f7f;                     // "no position yet": the 0x7f byte fill of every atomicMin
 constexpr long long RW_MAX_ROWS = 1LL << 30;            // rows and traceids: every table slot fits an int
 constexpr unsigned long long RW_NOKEY = ~0ull;
+constexpr long long RW_WIN_MAX = 0x7ffffff0LL;          // window keys, samples and batch sizes: int32 offsets and scans
 constexpr unsigned long long RW_SEED = 0x452821e638d01377ull;
 
 __device__ __forceinline__ bool in_dict(int64_t v, long long n) { return v >= 0 && v < n; }
@@ -394,6 +395,21 @@ __device__ __forceinline__ double median_of(const double* sorted, long long nobs
   return __ddiv_rn(__dadd_rn(sorted[h], sorted[h - 1]), 2.0);
 }
 
+// the 8 statistics of one group from its folds and its ascending value runs (NaN last)
+__device__ __forceinline__ void put_stats(const GroupStats& a, const GroupStats& m, const double* cpu_sorted,
+                                          const double* mem_sorted, double* out) {
+  const GroupStats* st[2] = {&a, &m};
+  const double* sorted[2] = {cpu_sorted, mem_sorted};
+  for (int j = 0; j < 2; ++j) {
+    const GroupStats& s = *st[j];
+    const bool none = s.nobs == 0;
+    out[4 * j + 0] = none ? NAN : s.mx;
+    out[4 * j + 1] = none ? NAN : s.mn;
+    out[4 * j + 2] = none ? NAN : __ddiv_rn(s.sum, (double)s.nobs);
+    out[4 * j + 3] = median_of(sorted[j], s.nobs);
+  }
+}
+
 __global__ void k_res_stats(long long G, const int64_t* perm, const int* gptr, const double* cpu, const double* mem,
                             const double* cpu_sorted, const double* mem_sorted, double* vals) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -405,17 +421,188 @@ __global__ void k_res_stats(long long G, const int64_t* perm, const int* gptr, c
     a.add(cpu[r]);
     m.add(mem[r]);
   }
-  double* out = vals + 8 * g;
-  const GroupStats* st[2] = {&a, &m};
-  const double* sorted[2] = {cpu_sorted, mem_sorted};
-  for (int j = 0; j < 2; ++j) {
-    const GroupStats& s = *st[j];
-    const bool none = s.nobs == 0;
-    out[4 * j + 0] = none ? NAN : s.mx;
-    out[4 * j + 1] = none ? NAN : s.mn;
-    out[4 * j + 2] = none ? NAN : __ddiv_rn(s.sum, (double)s.nobs);
-    out[4 * j + 3] = median_of(sorted[j] + b, s.nobs);
+  put_stats(a, m, cpu_sorted + b, mem_sorted + b, vals + 8 * g);
+}
+
+// ---- the open-bucket sample window (ResourceSampleWindow) ---------------------------------------------------------
+// Window state: keys[U] (sorted unique ts * n_ms + ms), off[U+1] (run offsets), st[U][2] (the GroupStats fold of cpu
+// and memory) and the runs cpu_run / mem_run [S]: every key's values ascending in the order of vo_lt, ties in arrival
+// order.  A batch is given sorted by key (stable, so arrival order within a key), and each column also as bsorted[k]:
+// the batch's values of each key ascending (ties in arrival order) at the key's positions.
+static_assert(sizeof(GroupStats) == 40, "the window stores GroupStats as 5 doubles per column");
+
+// value order of the runs: NaN above every number and equal to NaN; -0.0 == 0.0 (IEEE compare)
+__device__ __forceinline__ bool vo_lt(double a, double b) { return a < b || (b != b && a == a); }
+
+__device__ __forceinline__ int64_t floor_div(int64_t a, long long n) {
+  int64_t q = a / n;
+  return (a % n != 0 && a < 0) ? q - 1 : q;
+}
+
+__device__ __forceinline__ long long lower_bound(const int64_t* a, long long n, int64_t v) {
+  long long lo = 0, hi = n;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (a[mid] < v) lo = mid + 1; else hi = mid;
   }
+  return lo;
+}
+
+// #values of the ascending run a[0, n) that are below v (le = false) or not above v (le = true)
+__device__ __forceinline__ int count_below(const double* a, int n, double v, bool le) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (le ? !vo_lt(v, a[mid]) : vo_lt(a[mid], v)) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// flags[0..k] / flags[k+1..2k+1]: 1 at p + 1 if batch position p starts a key that is not late (fu), and one that is
+// also absent from the window (fn); slot 0 of each is 0.  Scanned, fu[p] / fn[p] count such starts before p.
+__global__ void k_win_flags(long long k, const int64_t* bkeys, long long n_ms, long long seal, long long U,
+                            const int64_t* keys, int* fu, int* fn) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= k) return;
+  if (p == 0) fu[0] = fn[0] = 0;
+  const int64_t key = bkeys[p];
+  const bool first = floor_div(key, n_ms) >= seal && (p == 0 || bkeys[p - 1] != key);
+  bool fresh = false;
+  if (first) {
+    const long long j = lower_bound(keys, U, key);
+    fresh = j == U || keys[j] != key;
+  }
+  fu[p + 1] = first;
+  fn[p + 1] = fresh;
+}
+
+// sizes = {late samples (a prefix of the sorted batch), keys the batch touches, keys after the merge}
+__global__ void k_win_sizes(long long k, const int64_t* bkeys, long long n_ms, long long seal, long long U,
+                            const int* fu, const int* fn, int64_t* sizes) {
+  long long lo = 0, hi = k;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (floor_div(bkeys[mid], n_ms) < seal) lo = mid + 1; else hi = mid;
+  }
+  sizes[0] = lo;
+  sizes[1] = k ? fu[k] : 0;
+  sizes[2] = U + (k ? fn[k] : 0);
+}
+
+// the key merge: every old key and every touched key finds its slot of the merged table; each slot field is written
+// once.  src[s]: old index or -1; bsrc[s]: touched key index or -1; opos[j]: slot of old key j; ustart[b]: first batch
+// position of touched key b (ustart[u] = k); upos[b]: its slot.
+__global__ void k_win_keys(long long U, const int64_t* keys, long long k, const int64_t* bkeys, const int* fu,
+                           const int* fn, int64_t* keys2, int* src, int* bsrc, int* opos, int* ustart, int* upos) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < U) {
+    const int64_t key = keys[t];
+    const long long lb = lower_bound(bkeys, k, key);
+    const int pos = (int)(t + fn[lb]);
+    keys2[pos] = key;
+    src[pos] = (int)t;
+    opos[t] = pos;
+    if (lb == k || bkeys[lb] != key) bsrc[pos] = -1;
+  }
+  if (t < k) {
+    if (t == k - 1) ustart[fu[k]] = (int)k;
+    if (fu[t + 1] == fu[t]) return;                      // late, or not the first sample of its key
+    const int64_t key = bkeys[t];
+    const int b = fu[t];
+    const long long j = lower_bound(keys, U, key);
+    const int pos = (int)(j + fn[t]);
+    ustart[b] = (int)t;
+    upos[b] = pos;
+    bsrc[pos] = b;
+    if (j == U || keys[j] != key) {
+      keys2[pos] = key;
+      src[pos] = -1;
+    }
+  }
+}
+
+// the fold: each slot continues its key's GroupStats over the key's batch samples in arrival order (untouched keys
+// copy theirs) and writes its run length at cnt[s + 1]
+__global__ void k_win_fold(long long U2, const int* src, const int* bsrc, const int* ustart, const int* off,
+                           const GroupStats* st, const int64_t* perm, const double* cpu, const double* mem,
+                           GroupStats* st2, int* cnt) {
+  const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= U2) return;
+  if (s == 0) cnt[0] = 0;
+  const int j = src[s], b = bsrc[s];
+  GroupStats a, m;
+  int n = 0;
+  if (j >= 0) {
+    a = st[2 * j];
+    m = st[2 * j + 1];
+    n = off[j + 1] - off[j];
+  }
+  if (b >= 0) {
+    const int e = ustart[b + 1];
+    for (int p = ustart[b]; p < e; ++p) {
+      const long long r = perm[p];
+      a.add(cpu[r]);
+      m.add(mem[r]);
+    }
+    n += e - ustart[b];
+  }
+  st2[2 * s] = a;
+  st2[2 * s + 1] = m;
+  cnt[s + 1] = n;
+}
+
+// the run merge, one thread per value: old value i of key K goes to off2(K) + i + #(batch values of K below it), batch
+// value i to off2(K) + i + #(old values of K not above it), so ties keep arrival order
+__global__ void k_win_runs(long long U, long long S, const int* off, const double* cpu_run, const double* mem_run,
+                           long long n_late, long long n_new, const int* fu, const int* ustart, const int* upos,
+                           const double* cpu_sorted, const double* mem_sorted, const int* src, const int* bsrc,
+                           const int* opos, const int* off2, double* cpu_run2, double* mem_run2) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < S) {
+    int lo = 0, hi = (int)U - 1;                         // the key j with off[j] <= t < off[j + 1]
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (off[mid] <= t) lo = mid; else hi = mid - 1;
+    }
+    const int pos = opos[lo], b = bsrc[pos];
+    const long long dst = off2[pos] + (t - off[lo]);
+    const double c = cpu_run[t], m = mem_run[t];
+    if (b < 0) {
+      cpu_run2[dst] = c;
+      mem_run2[dst] = m;
+    } else {
+      const int bb = ustart[b], bn = ustart[b + 1] - bb;
+      cpu_run2[dst + count_below(cpu_sorted + bb, bn, c, false)] = c;
+      mem_run2[dst + count_below(mem_sorted + bb, bn, m, false)] = m;
+    }
+  } else if (t < S + n_new) {
+    const long long p = n_late + (t - S);
+    const int b = fu[p + 1] - 1, pos = upos[b], j = src[pos];
+    const long long dst = off2[pos] + (p - ustart[b]);
+    const double c = cpu_sorted[p], m = mem_sorted[p];
+    if (j < 0) {
+      cpu_run2[dst] = c;
+      mem_run2[dst] = m;
+    } else {
+      const int ob = off[j], on = off[j + 1] - ob;
+      cpu_run2[dst + count_below(cpu_run + ob, on, c, true)] = c;
+      mem_run2[dst + count_below(mem_run + ob, on, m, true)] = m;
+    }
+  }
+}
+
+// (timestamp, ms) and the 8 statistics of n slots: slot[i], or slot i itself when slot is NULL
+__global__ void k_win_emit(long long n, const int* slot, const int64_t* keys, const int* off, const GroupStats* st,
+                           const double* cpu_run, const double* mem_run, long long n_ms, int64_t* index,
+                           double* vals) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const long long s = slot ? slot[i] : i;
+  const int64_t key = keys[s], ts = floor_div(key, n_ms);
+  index[2 * i] = ts;
+  index[2 * i + 1] = key - ts * n_ms;
+  const int b = off[s];
+  put_stats(st[2 * s], st[2 * s + 1], cpu_run + b, mem_run + b, vals + 8 * i);
 }
 
 bool calls_ok(const PertRawCalls* c) {
@@ -596,6 +783,90 @@ int pert_raw_resource_stats(long long G, const int64_t* perm, const int* gptr, c
   if (G == 0) return PERT_OK;
   k_res_stats<<<pert_cdiv(G, 128), 128, 0, (cudaStream_t)stream_>>>(G, perm, gptr, cpu, mem, cpu_sorted, mem_sorted,
                                                                    vals);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+// ---- the open-bucket sample window ----------------------------------------------------------------------------------
+static bool win_count_ok(long long n) { return n >= 0 && n <= RW_WIN_MAX; }
+
+long long pert_raw_window_workspace_bytes(long long U, long long k, long long U2) {
+  if (!win_count_ok(U) || !win_count_ok(k) || !win_count_ok(U2)) return PERT_ERR_BADARG;
+  return 4 * (2 * (U2 + 16) + (U + 16)) + scan_bytes(std::max(k, U2) + 1) + 64;
+}
+
+int pert_raw_window_count(long long k, const int64_t* bkeys, long long n_ms, long long seal, long long U,
+                          const int64_t* keys, int* flags, int64_t* sizes, void* workspace, long long workspace_bytes,
+                          void* stream_) {
+  if (!win_count_ok(k) || !win_count_ok(U) || n_ms < 1 || (k > 0 && (!bkeys || !flags)) || (U > 0 && !keys) ||
+      !sizes || !workspace || workspace_bytes < pert_raw_window_workspace_bytes(U, k, 0))
+    return PERT_ERR_BADARG;
+  cudaStream_t st = (cudaStream_t)stream_;
+  int* fu = flags;
+  int* fn = flags ? flags + k + 1 : nullptr;
+  if (k > 0) {
+    k_win_flags<<<pert_cdiv(k, 256), 256, 0, st>>>(k, bkeys, n_ms, seal, U, keys, fu, fn);
+    PERT_LAUNCH_CHECK();
+    int rc;
+    if ((rc = scan(fu, fn, k + 1, (int*)workspace, st)) != PERT_OK) return rc;
+  }
+  k_win_sizes<<<1, 1, 0, st>>>(k, bkeys, n_ms, seal, U, fu, fn, sizes);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+int pert_raw_window_merge(long long U, long long S, const int64_t* keys, const int* off, const void* state,
+                          const double* cpu_run, const double* mem_run, long long k, const int64_t* bkeys, const int64_t* perm,
+                          const double* cpu, const double* mem, const double* cpu_sorted, const double* mem_sorted,
+                          const int* flags, long long n_late, long long u, long long U2, int64_t* keys2, int* off2,
+                          void* state2, double* cpu_run2, double* mem_run2, int* ustart, int* upos, void* workspace,
+                          long long workspace_bytes, void* stream_) {
+  if (!win_count_ok(U) || !win_count_ok(S) || S < U || (U == 0 && S > 0) || !win_count_ok(k) || !win_count_ok(U2) ||
+      S + k > RW_WIN_MAX || n_late < 0 || n_late > k || u < 0 ||
+      u > k - n_late || U2 < U || U2 > U + u || !off || !off2 || !ustart ||
+      (U > 0 && (!keys || !state || !cpu_run || !mem_run)) ||
+      (k > 0 && (!bkeys || !perm || !cpu || !mem || !cpu_sorted || !mem_sorted || !flags)) ||
+      (U2 > 0 && (!keys2 || !state2 || !cpu_run2 || !mem_run2)) || (u > 0 && !upos) || !workspace ||
+      workspace_bytes < pert_raw_window_workspace_bytes(U, k, U2))
+    return PERT_ERR_BADARG;
+  cudaStream_t st = (cudaStream_t)stream_;
+  int* src = (int*)workspace;
+  int* bsrc = src + U2 + 16;
+  int* opos = bsrc + U2 + 16;
+  int* bsum = opos + U + 16;
+  const int* fu = flags;
+  const int* fn = flags ? flags + k + 1 : nullptr;
+  const int B = 256;
+  if (U > 0 || k > 0) {
+    k_win_keys<<<pert_cdiv(std::max(U, k), B), B, 0, st>>>(U, keys, k, bkeys, fu, fn, keys2, src, bsrc, opos, ustart,
+                                                           upos);
+    PERT_LAUNCH_CHECK();
+  }
+  if (U2 == 0) return (int)cudaMemsetAsync(off2, 0, 4, st);
+  k_win_fold<<<pert_cdiv(U2, 128), 128, 0, st>>>(U2, src, bsrc, ustart, off, (const GroupStats*)state, perm, cpu, mem,
+                                                 (GroupStats*)state2, off2);
+  PERT_LAUNCH_CHECK();
+  int rc;
+  if ((rc = scan(off2, nullptr, U2 + 1, bsum, st)) != PERT_OK) return rc;
+  const long long n_new = k - n_late;
+  if (S + n_new > 0) {
+    k_win_runs<<<pert_cdiv(S + n_new, B), B, 0, st>>>(U, S, off, cpu_run, mem_run, n_late, n_new, fu, ustart, upos,
+                                                      cpu_sorted, mem_sorted, src, bsrc, opos, off2, cpu_run2,
+                                                      mem_run2);
+    PERT_LAUNCH_CHECK();
+  }
+  return PERT_OK;
+}
+
+int pert_raw_window_emit(long long n, const int* slot, long long U, const int64_t* keys, const int* off,
+                         const void* state, const double* cpu_run, const double* mem_run, long long n_ms,
+                         int64_t* index, double* vals, void* stream_) {
+  if (!win_count_ok(n) || !win_count_ok(U) || (!slot && n > U) || n_ms < 1 ||
+      (n > 0 && (!keys || !off || !state || !cpu_run || !mem_run || !index || !vals)))
+    return PERT_ERR_BADARG;
+  if (n == 0) return PERT_OK;
+  k_win_emit<<<pert_cdiv(n, 128), 128, 0, (cudaStream_t)stream_>>>(n, slot, keys, off, (const GroupStats*)state,
+                                                                   cpu_run, mem_run, n_ms, index, vals);
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }

@@ -6,7 +6,8 @@ factorise five columns, find every trace's entry in a Python loop over traces, f
 per-entry occurrence, renumber the microservices and aggregate the resource rows per (timestamp, msname).
 
 Here the host only parses the files and dictionary-encodes their values (``read_raw``); everything after that runs
-over the whole table in csrc/rawtable.cu (``process_raw``).  The result's ``columns`` are the nine
+over the whole table in csrc/rawtable.cu (``process_raw``).  ``ResourceSampleWindow`` keeps the same resource
+statistics of the still-open (timestamp, msname) keys up to date as raw samples arrive.  The result's ``columns`` are the nine
 ``tracegroup.COLUMNS`` that ``group_traces`` takes, and ``resource_index`` / ``resource_values`` are the rows the
 ``PatternStore`` constructors take.  There is no CPU fallback: without the CUDA library the calls raise.
 
@@ -18,11 +19,13 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from typing import NamedTuple
 
 import numpy as np
 import torch
 
 from . import _lib
+from .store import _I64_MAX, _I64_MIN, _check_resource_rows, _index_rows, _key_bounds
 from .tracegroup import COLUMNS
 
 CALL_COLUMNS = ("traceid", "timestamp", "rpcid", "um", "rpctype", "dm", "interface", "rt")   # MSCallGraph order
@@ -316,3 +319,224 @@ def process_raw(raw, device="cuda", min_occurence=100, hash_bits=64):
 def list_csvs(directory):
     """The .csv files of a directory in os.listdir order, the order get_df() concatenates them in."""
     return [os.path.join(directory, f) for f in os.listdir(directory) if f.endswith(".csv")]
+
+
+_WIN_MAX = 0x7ffffff0                                    # keys, samples and batch samples of a window (int32 offsets)
+
+
+class WindowRows(NamedTuple):
+    """Statistics rows of a ``ResourceSampleWindow``: ``index`` int64 CUDA [u, 2] (timestamp, ms) ascending by key,
+    ``values`` float64 CUDA [u, 8] in STATS order, ``late`` the samples an ``add`` skipped because their key is sealed
+    (0 for ``rows()``).  ``index`` / ``values`` are what ``PatternStore.append_resources`` takes."""
+    index: torch.Tensor
+    values: torch.Tensor
+    late: int
+
+
+def _usage_column(a, what, k, dev):
+    """float64 [k] on ``dev`` of a usage column: any real numbers (NaN and +-inf allowed, as pandas); ``PertGnnError``
+    naming the first sample that is not one."""
+    if torch.is_tensor(a) and a.is_cuda:
+        if a.dtype == torch.bool or a.dtype.is_complex:
+            raise _lib.PertGnnError(f"{what}: numbers expected, got {a.dtype}")
+        if a.dim() != 1 or int(a.shape[0]) != k:
+            raise _lib.PertGnnError(f"{what}: shape {tuple(a.shape)}, expected ({k},): one value per sample")
+        return a.to(dev, torch.float64).contiguous()
+    a = a.numpy() if torch.is_tensor(a) else a
+    try:
+        v = np.asarray(a)
+    except (TypeError, ValueError) as e:
+        raise _lib.PertGnnError(f"{what}: numbers expected ({e})") from None
+    if v.ndim != 1 or v.shape[0] != k:
+        raise _lib.PertGnnError(f"{what}: shape {v.shape}, expected ({k},): one value per sample")
+    if v.dtype.kind not in "iuf":
+        v = np.asarray(a, dtype=object)
+        for i, x in enumerate(v):
+            if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, float, np.integer, np.floating)):
+                raise _lib.PertGnnError(f"sample {i}: {what} {x!r} is not a number")
+    return torch.from_numpy(v.astype(np.float64)).to(dev)
+
+
+class ResourceSampleWindow:
+    """The open buckets of a live resource table, fed raw samples: the statistics preprocess.py:237-242 computes with
+    ``groupby(["timestamp", "msname"]).agg(["max", "min", "mean", "median"])``, kept on the GPU and continued sample by
+    sample, so a server can publish its open buckets without a host pass or a rebuild over every open sample.
+
+    ``n_ms``: the store's microservice count; samples carry the store's ids (``process_raw``'s name-order ids:
+    ``{name: i for i, name in enumerate(proc.ms_names)}``).  A sample's key is its exact (timestamp, ms), as in
+    get_df()'s groupby; a caller who wants 30 s buckets floors the timestamps first.
+
+    ``add(timestamps, ms, cpu, mem)`` -> ``WindowRows`` of the keys the call touched, each with the statistics of ALL
+    its samples so far: after any sequence of ``add`` and ``seal`` calls they are bit for bit ``process_raw``'s for the
+    concatenation of the key's samples in arrival order (calls in order, input order within a call): max / min with a
+    strict compare (the first of tied values, so -0.0 vs 0.0, is kept), the Kahan mean, NaN skipped (an all-NaN key
+    has NaN statistics), and the median of the key's values in a stable ascending sort, NaN last and +-0 tied.
+    ``seal(before)`` makes every key with timestamp < before final and frees its samples; later samples of such keys
+    are counted in ``late`` and change nothing.  ``rows()``: the same pair for every open key.
+
+    Device state (csrc/rawtable.cu, pert_raw_window_*): the sorted unique open keys, their run offsets, the resumable
+    fold of both columns per key (80 bytes) and each key's values of both columns kept sorted (NaN last, so the runs
+    of both columns share the offsets): 16 bytes per open sample and 92 per open key.  An ``add`` sorts the batch
+    (torch), merges the keys, continues the folds of the touched keys and merges each touched key's sorted run with
+    the batch's, O(S + k log k) for S open and k new samples."""
+
+    STATE_BYTES = 80                                      # per key: GroupStats of cpu and memory (5 doubles each)
+
+    def __init__(self, n_ms, device="cuda"):
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise _lib.PertGnnError("ResourceSampleWindow needs a CUDA device (no CPU fallback)")
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        n_ms = int(n_ms)
+        if not 1 <= n_ms <= _I64_MAX:
+            raise _lib.PertGnnError(f"ResourceSampleWindow: n_ms = {n_ms} must be at least 1")
+        self.device, self.n_ms = dev, n_ms
+        self.sealed = _I64_MIN                           # samples with timestamp < sealed are late
+        self.n_samples = 0                               # S, known on the host: no read needed to size an add
+        self._set(torch.zeros(0, dtype=torch.int64, device=dev), torch.zeros(1, dtype=torch.int32, device=dev),
+                  torch.zeros(0, self.STATE_BYTES // 8, dtype=torch.float64, device=dev),
+                  torch.zeros(0, dtype=torch.float64, device=dev), torch.zeros(0, dtype=torch.float64, device=dev))
+
+    def _set(self, keys, off, state, cpu_run, mem_run):
+        self.t = {"keys": keys, "off": off, "state": state, "cpu_run": cpu_run, "mem_run": mem_run}
+
+    @property
+    def n_keys(self):
+        return int(self.t["keys"].shape[0])
+
+    def _batch(self, timestamps, ms, cpu, mem):
+        """Checked (ts, ms, cpu, mem) on the window's device: int64, int64, float64, float64 [k].  ``PertGnnError``
+        naming the first bad sample, before anything changes."""
+        dev, n_ms = self.device, self.n_ms
+        cols = [timestamps, ms, cpu, mem]
+        lens = []
+        for c in cols:
+            try:
+                lens.append(int(c.shape[0]) if hasattr(c, "shape") and len(c.shape) else len(c))
+            except TypeError:
+                raise _lib.PertGnnError("add: the four columns must be 1-d sequences") from None
+        if len(set(lens)) != 1:
+            raise _lib.PertGnnError(f"add: columns of different lengths {lens} (timestamps, ms, cpu, mem)")
+        k = lens[0]
+        if k > _WIN_MAX:
+            raise _lib.PertGnnError(f"add: {k} samples exceed 2^31 - 16 per call")
+        if all(torch.is_tensor(c) and c.is_cuda for c in cols[:2]):
+            for c, what in ((timestamps, "timestamps"), (ms, "ms")):
+                if c.dtype.is_floating_point or c.dtype.is_complex or c.dtype == torch.bool:
+                    raise _lib.PertGnnError(f"{what}: integers expected, got {c.dtype}")
+                if c.dim() != 1:
+                    raise _lib.PertGnnError(f"{what}: a 1-d column expected, got shape {tuple(c.shape)}")
+            ts, m = (c.to(dev, torch.int64).contiguous() for c in cols[:2])
+            if k:
+                lo, hi = _key_bounds(n_ms)
+                mm = torch.stack([m.min(), m.max(), ts.min(), ts.max()]).tolist()   # one device -> host read
+                if mm[0] < 0 or mm[1] >= n_ms or mm[2] < lo or mm[3] > hi:
+                    _check_resource_rows(ts.cpu().numpy(), m.cpu().numpy(), n_ms)
+        else:
+            h = [c.cpu().numpy() if torch.is_tensor(c) else c for c in cols[:2]]
+            pairs = np.stack([np.asarray(h[0]), np.asarray(h[1])], 1) if all(
+                isinstance(x, np.ndarray) for x in h) else list(zip(h[0], h[1]))
+            idx = _index_rows(pairs)                      # floats refused, not truncated; names the first bad sample
+            if idx.ndim != 2 or idx.shape[1] != 2:
+                raise _lib.PertGnnError("add: timestamps and ms must be 1-d integer columns")
+            _check_resource_rows(idx[:, 0], idx[:, 1], n_ms)
+            ts, m = (torch.from_numpy(np.ascontiguousarray(idx[:, j])).to(dev) for j in (0, 1))
+        return ts, m, _usage_column(cpu, "instance_cpu_usage", k, dev), _usage_column(mem, "instance_memory_usage",
+                                                                                       k, dev)
+
+    @_lib.on_device_of
+    def add(self, timestamps, ms, cpu, mem):
+        """Adds raw samples, one per element of the four columns (host arrays / lists or CUDA tensors): integer
+        timestamps (floats are refused), ms in [0, n_ms), cpu and memory usage (numbers; NaN and +-inf allowed).
+        Returns ``WindowRows`` of the distinct keys this call touched, ascending by key, with the statistics of all
+        their samples so far.  k = 0 is allowed.  Checked on the host before anything changes (``PertGnnError`` naming
+        the first bad sample, the window left as it was): equal column lengths, integer timestamps, ms in [0, n_ms),
+        keys timestamp * n_ms + ms within int64, numeric usages; CUDA index columns cost one read of their minima and
+        maxima.  Beyond that the call makes one device -> host read: the sizes of the merged key table.  Ordered on the
+        current stream."""
+        ts, m, cpu, mem = self._batch(timestamps, ms, cpu, mem)
+        k = int(ts.shape[0])
+        dev, n_ms = self.device, self.n_ms
+        i32, i64, f64 = (dict(dtype=d, device=dev) for d in (torch.int32, torch.int64, torch.float64))
+        if k == 0:
+            return WindowRows(torch.zeros(0, 2, **i64), torch.zeros(0, 8, **f64), 0)
+        L, st = _lib.lib(), _lib.stream()
+        t, U, S = self.t, self.n_keys, self.n_samples
+        key = ts * n_ms + m
+        bkeys, perm = torch.sort(key, stable=True)        # arrival order within a key
+        flags, sizes = torch.empty(2 * (k + 1), **i32), torch.empty(3, **i64)
+        ws = torch.empty(int(L.pert_raw_window_workspace_bytes(U, k, min(U + k, _WIN_MAX))), dtype=torch.uint8,
+                         device=dev)
+        _lib.check(L.pert_raw_window_count(k, bkeys.data_ptr(), n_ms, self.sealed, U, t["keys"].data_ptr(),
+                                           flags.data_ptr(), sizes.data_ptr(), ws.data_ptr(), ws.numel(), st),
+                   "pert_raw_window_count")
+        # every key's batch values ascending (NaN last, ties in arrival order) at the key's positions of bkeys
+        srt = []
+        for c in (cpu, mem):
+            s = torch.sort(c, stable=True)
+            srt.append(s.values[torch.sort(key[s.indices], stable=True).indices].contiguous())
+        n_late, u, U2 = sizes.tolist()                    # the one device -> host read
+        if u == 0:
+            return WindowRows(torch.zeros(0, 2, **i64), torch.zeros(0, 8, **f64), n_late)
+        S2 = S + k - n_late
+        if U2 > _WIN_MAX or S2 > _WIN_MAX:
+            raise _lib.PertGnnError(f"add: the window would hold {U2} keys and {S2} samples; at most 2^31 - 16 each")
+        new = (torch.empty(U2, **i64), torch.empty(U2 + 1, **i32), torch.empty(U2, self.STATE_BYTES // 8, **f64),
+               torch.empty(S2, **f64), torch.empty(S2, **f64))
+        ustart, upos = torch.empty(u + 1, **i32), torch.empty(u, **i32)
+        p = lambda x: x.data_ptr() if x.numel() else None      # noqa: E731
+        _lib.check(L.pert_raw_window_merge(
+            U, S, p(t["keys"]), t["off"].data_ptr(), p(t["state"]), p(t["cpu_run"]), p(t["mem_run"]), k,
+            bkeys.data_ptr(), perm.data_ptr(), cpu.data_ptr(), mem.data_ptr(), srt[0].data_ptr(), srt[1].data_ptr(),
+            flags.data_ptr(), n_late, u, U2, *(p(x) for x in new), ustart.data_ptr(), upos.data_ptr(), ws.data_ptr(),
+            ws.numel(), st), "pert_raw_window_merge")
+        self._set(*new)
+        self.n_samples = S2
+        index, values = self._emit(u, upos)
+        return WindowRows(index, values, n_late)
+
+    def _emit(self, n, slot):
+        t, dev = self.t, self.device
+        index = torch.empty(n, 2, dtype=torch.int64, device=dev)
+        values = torch.empty(n, 8, dtype=torch.float64, device=dev)
+        p = lambda x: x.data_ptr() if x.numel() else None      # noqa: E731
+        _lib.check(_lib.lib().pert_raw_window_emit(
+            n, None if slot is None else slot.data_ptr(), self.n_keys, p(t["keys"]), t["off"].data_ptr(),
+            p(t["state"]), p(t["cpu_run"]), p(t["mem_run"]), self.n_ms, p(index), p(values), _lib.stream()),
+            "pert_raw_window_emit")
+        return index, values
+
+    @_lib.on_device_of
+    def rows(self):
+        """``WindowRows`` of every open key (late = 0): what a restarted server republishes."""
+        index, values = self._emit(self.n_keys, None)
+        return WindowRows(index, values, 0)
+
+    @_lib.on_device_of
+    def seal(self, before):
+        """Makes every key with timestamp < ``before`` final: its samples are freed now, and later samples of such keys
+        are late.  Monotone: a cut at or below the current one does nothing.  One device -> host read (the sealed
+        prefix's key and sample counts) when the window holds keys."""
+        cut = int(before)
+        if not _I64_MIN <= cut <= _I64_MAX:
+            raise _lib.PertGnnError(f"seal: before = {cut} is outside int64")
+        if cut <= self.sealed:
+            return self
+        self.sealed = cut
+        t, U = self.t, self.n_keys
+        if U == 0:
+            return self
+        ck = cut * self.n_ms                               # ts < cut  <=>  key < cut * n_ms (every ms < n_ms)
+        if ck > _I64_MAX:
+            j = torch.full((), U, dtype=torch.int64, device=self.device)
+        else:
+            j = torch.searchsorted(t["keys"], torch.tensor([max(ck, _I64_MIN)], device=self.device))[0]
+        j, s0 = torch.stack([j, t["off"][j].long()]).tolist()
+        if j == 0:
+            return self
+        off = t["off"][j:] - s0
+        self._set(t["keys"][j:].clone(), off, t["state"][j:].clone(), t["cpu_run"][s0:].clone(),
+                  t["mem_run"][s0:].clone())
+        self.n_samples -= s0
+        return self

@@ -53,7 +53,8 @@ extern "C" {
  * (replacing and deleting them by key); pert_ingest_* (appending traces to a live store);
  * pert_ingest_evict_* (evicting traces from a live store); pert_store_assemble_whatif (per-request pattern mixes and
  * resource overrides), pert_store_lookup_resources; pert_raw_* (processed tables from raw rows); pert_raw_window_*
- * (raw resource samples aggregated into the open buckets' statistics). */
+ * (raw resource samples aggregated into the open buckets' statistics); pert_linear_bwd_planes_ex, pert_tconv_bwd_bn
+ * (_supported) (the BatchNorm backward folded into the node-linear and conv backward passes). */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -140,6 +141,37 @@ int pert_tconv_bwd_c(const float* g, int ld_g, const float* q, const float* k, c
                      const int* csc_pos, const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha,
                      float* dq, float* dk, float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc,
                      int n_rpc, long long N, long long E, long long B_hint, int H, int C, void* stream);
+/* The backward of the BatchNorm(+ReLU, +dropout) that feeds a conv, folded into that conv's backward (training): the
+ * conv's output gradient g is not read but computed row by row where the target pass loads it, and written to g (the
+ * node-linear backward of the conv reads it as its skip plane; pert_bn_bwd semantics):
+ *   dz = dx * (y > 0) * relu_scale,  g = gamma rstd (dz - sums[0:H] / n - xhat sums[H:2H] / n),  xhat = (x - mean) rstd,
+ *   n = live[0] (NULL: N), rows >= n get g = 0;  dbeta += sums[0:H], dgamma += sums[H:2H]  (as float).
+ * sums: the fp64 column sums of dz and dz * xhat over the rows below n, as pert_linear_bwd_planes_ex leaves them.
+ * dx, y, x are dense [N, H] rows. */
+typedef struct PertBnBwd {
+  const float* dx;        /* gradient w.r.t. y */
+  const float* y;         /* relu(bn(x)) [* keep * scale]: the forward's output of the BatchNorm */
+  const float* x;         /* BatchNorm input */
+  const float* mean;      /* [H] batch statistics of the forward */
+  const float* rstd;
+  const float* gamma;
+  const double* sums;     /* [2H] */
+  float* dgamma;          /* [H], += */
+  float* dbeta;
+  const long long* live;  /* optional {N, B} of a padded batch */
+  float relu_scale;       /* 1 / (1 - p) after inverted dropout, else 1 */
+} PertBnBwd;
+/* pert_tconv_bwd_c with g = BN backward of bn (written, not read).  PERT_ERR_BADARG as pert_tconv_bwd_c, and for NULL or
+ * misaligned BatchNorm operands.  PERT_ERR_UNSUPPORTED (nothing launched: use pert_bn_bwd + pert_tconv_bwd_c) unless
+ * H = 64 and the shared-memory-staged conv kernels take the shape: ld = ld_g = ld_d = H and an rpc table of at most
+ * 16 KiB.  pert_tconv_bwd_bn_supported: 1 if H and n_rpc qualify, else 0. */
+int pert_tconv_bwd_bn(float* g, int ld_g, const float* q, const float* k, const float* v, int ld, const int* rowptr,
+                      const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
+                      const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha, float* dq,
+                      float* dk, float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc,
+                      int n_rpc, long long N, long long E, long long B_hint, int H, int C, const PertBnBwd* bn,
+                      void* stream);
+int pert_tconv_bwd_bn_supported(int H, int n_rpc);
 
 /* ---- dense linears (exact fp32) --------------------------------------------------------------------
  * Replace torch_geometric.nn.Linear / the lin_* of TransformerConv (model.py:26-55,105,110-112).
@@ -170,6 +202,15 @@ int pert_linear_bwd_planes(const float* dY, long long plane_stride, const float*
                            float* dW4, int ldw4, float* db4, float* dX, int ldx_out, long long N, int H, int K, int Kd,
                            void* stream);
 int pert_linear_bwd_planes_supported(long long N, int H, int K, int Kd);
+/* The same with the column sums of the BatchNorm backward of the previous conv (bn_sums != NULL; K = Kd = H), for
+ * pert_tconv_bwd_bn: X is that BatchNorm's output y, dX its gradient dx, and
+ *   bn_sums[0:H] += sum dz,  bn_sums[H:2H] += sum dz * (bn_x - bn_mean) bn_rstd,  dz = dX * (X > 0) * relu_scale
+ * over the rows below live[0] (NULL: all N); bn_x dense [N, H].  dX and the weight gradients are those of
+ * pert_linear_bwd_planes (dX bit-identical).  bn_sums = NULL: pert_linear_bwd_planes. */
+int pert_linear_bwd_planes_ex(const float* dY, long long plane_stride, const float* X, int ldx, const float* W4t,
+                              int ldw, float* dW4, int ldw4, float* db4, float* dX, int ldx_out, long long N, int H,
+                              int K, int Kd, const float* bn_x, const float* bn_mean, const float* bn_rstd,
+                              float relu_scale, const long long* live, double* bn_sums, void* stream);
 /* Forward of the same node linear in one pass over A (tensor cores, 3xTF32), optionally with the BatchNorm(+ReLU,
  * +dropout) of the previous conv applied while A is loaded:
  *   planes: 4 planes [N, H] (row stride H, plane stride plane_stride) = A' . W4^T + b4,  W4 [4H, K] (ldw), b4 [4H];

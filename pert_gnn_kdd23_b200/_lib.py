@@ -35,11 +35,15 @@ SIGNATURES = {
     "pert_tconv_fwd_c": (I, [P, P, P, P, I, P, P, P, P, P, P, P, I, P, I, LL, LL, LL, I, I, P]),
     "pert_tconv_bwd_c": (I, [P, I, P, P, P, I, P, P, P, P, P, P, P, P, P, P, P, P, P, I, P, P, P, P, I, LL, LL, LL, I,
                              I, P]),
+    "pert_tconv_bwd_bn": (I, [P, I, P, P, P, I, P, P, P, P, P, P, P, P, P, P, P, P, P, I, P, P, P, P, I, LL, LL, LL, I,
+                              I, P, P]),
+    "pert_tconv_bwd_bn_supported": (I, [I, I]),
     "pert_gemm_nt": (I, [P, I, I, LL, P, I, P, P, I, I, LL, LL, I, I, I, I, P]),
     "pert_gemm_tn": (I, [P, I, I, LL, P, I, I, LL, P, I, P, LL, I, I, P]),
     "pert_colsum": (I, [P, I, I, LL, P, LL, I, P]),
     "pert_linear_bwd_planes": (I, [P, LL, P, I, P, I, P, I, P, P, I, LL, I, I, I, P]),
     "pert_linear_bwd_planes_supported": (I, [LL, I, I, I]),
+    "pert_linear_bwd_planes_ex": (I, [P, LL, P, I, P, I, P, I, P, P, I, LL, I, I, I, P, P, P, F, P, P, P]),
     "pert_bn_linear_fwd_planes": (I, [P, I, I, P, P, P, P, P, F, F, I, P, P, P, I, P, LL, I, F, P, I, P, I, P, P, LL,
                                       LL, I, I, P]),
     "pert_bn_linear_fwd_planes_supported": (I, [LL, I, I]),
@@ -156,6 +160,11 @@ class PertModelDesc(C.Structure):
 
 class PertProbe(C.Structure):
     _fields_ = [("kernel", I32), ("layer", I32), ("ev_start", P), ("ev_stop", P)]
+
+
+class PertBnBwd(C.Structure):
+    _fields_ = [(k, P) for k in ("dx", "y", "x", "mean", "rstd", "gamma", "sums", "dgamma", "dbeta", "live")] + \
+        [("relu_scale", F)]
 
 
 class PertStore(C.Structure):

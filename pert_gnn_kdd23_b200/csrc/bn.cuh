@@ -1,6 +1,8 @@
 // BatchNorm forward pieces shared by the stand-alone apply (k_bn_apply, nodeops.cu) and the node-linear forward that
 // applies BatchNorm while it loads its A operand (k_bn_linear_fwd_planes, linear_fwd.cu).  Both kernels call these
-// helpers, so the activations they write are bit-identical by construction.
+// helpers, so the activations they write are bit-identical by construction.  Likewise the backward pieces: the
+// stand-alone passes (k_bn_bwd_reduce / k_bn_bwd_apply) and their fold into the node-linear backward (linear_bwd.cu)
+// and the conv backward target pass (tconv_tile.cu).
 #pragma once
 #include <math.h>
 
@@ -87,6 +89,33 @@ __device__ __forceinline__ float4 bn_dropout4(float4 o, uint32_t g, const BnDrop
   o.y = r.y >= drop.T ? o.y * drop.scale : 0.f;
   o.z = r.z >= drop.T ? o.z * drop.scale : 0.f;
   o.w = r.w >= drop.T ? o.w * drop.scale : 0.f;
+  return o;
+}
+
+// dz = dy * (y > 0) * scale of one float4.  With inverted dropout after the ReLU, y > 0 <=> (ReLU active and kept), so
+// the saved output is the whole mask and only the 1/(1-p) factor is applied (scale = 1 without dropout; __fmul_rn keeps
+// that product exact and uncontracted).
+__device__ __forceinline__ float4 bn_bwd_dz4(float4 g, float4 y, float scale) {
+  g.x = y.x > 0.f ? __fmul_rn(g.x, scale) : 0.f; g.y = y.y > 0.f ? __fmul_rn(g.y, scale) : 0.f;
+  g.z = y.z > 0.f ? __fmul_rn(g.z, scale) : 0.f; g.w = y.w > 0.f ? __fmul_rn(g.w, scale) : 0.f;
+  return g;
+}
+
+// s1 += dz,  s2 += dz * xhat  (xhat = (x - mean) rstd): the two column sums of the training backward
+__device__ __forceinline__ void bn_bwd_acc4(float4& s1, float4& s2, float4 dz, float4 x, float4 mu, float4 rs) {
+  s1 = f4add(s1, dz);
+  s2.x = fmaf(dz.x, (x.x - mu.x) * rs.x, s2.x); s2.y = fmaf(dz.y, (x.y - mu.y) * rs.y, s2.y);
+  s2.z = fmaf(dz.z, (x.z - mu.z) * rs.z, s2.z); s2.w = fmaf(dz.w, (x.w - mu.w) * rs.w, s2.w);
+}
+
+// training: dx = gamma rstd (dz - sum_dz / n - xhat sum_dzxhat / n), a = sum_dz, b = sum_dzxhat, invn = 1 / n
+__device__ __forceinline__ float4 bn_bwd_dx4(float4 g, float4 v, float4 mu, float4 rs, float4 ga, float4 a, float4 b,
+                                             float invn) {
+  float4 o;
+  o.x = ga.x * rs.x * (g.x - a.x * invn - (v.x - mu.x) * rs.x * b.x * invn);
+  o.y = ga.y * rs.y * (g.y - a.y * invn - (v.y - mu.y) * rs.y * b.y * invn);
+  o.z = ga.z * rs.z * (g.z - a.z * invn - (v.z - mu.z) * rs.z * b.z * invn);
+  o.w = ga.w * rs.w * (g.w - a.w * invn - (v.w - mu.w) * rs.w * b.w * invn);
   return o;
 }
 

@@ -408,6 +408,7 @@ struct Ws {
   float* gzero_begin;
   float *dw4[PERT_MAX_CONVS], *db4[PERT_MAX_CONVS], *dweA[PERT_MAX_CONVS], *dweB[PERT_MAX_CONVS];
   float *dt_if[PERT_MAX_CONVS], *dt_rpc[PERT_MAX_CONVS];
+  double* bn_dsums[PERT_MAX_CONVS];   // [2H] fp64 column sums of the folded BatchNorm backward (pert_tconv_bwd_bn)
   Tensors pg;      // Hp > H only: their gradients, unpacked like the conv packs
   float* gzero_end;
   // forward state
@@ -480,6 +481,7 @@ Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* b
     w.dt_if[l] = take((long long)d->n_if * H);
     w.dt_rpc[l] = take((long long)d->n_rpc * H);
   }
+  for (int l = 0; l + 1 < L; ++l) w.bn_dsums[l] = (double*)take(4LL * H);
   if (padded) take_tensors(w.pg);
   w.gzero_end = base ? base + off : nullptr;
   for (int l = 0; l < L; ++l) {
@@ -863,7 +865,7 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
                              const long long* live, void* stream) {
   TRY(check_desc(d));
   if (!(dropout >= 0.f && dropout <= 1.f)) return PERT_ERR_BADARG;
-  // the saved activations already carry the mask (see k_bn_bwd_reduce): only the 1 / (1 - p) factor is needed
+  // the saved activations already carry the mask (see bn_bwd_dz4, bn.cuh): only the 1 / (1 - p) factor is needed
   const float relu_scale = (training && dropout > 0.f) ? (dropout >= 1.f ? 0.f : (float)(1.0 / (1.0 - (double)dropout)))
                                                        : 1.f;
   std::lock_guard<std::mutex> issue_lock(engine_mutex());
@@ -919,13 +921,36 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
   };
   AuxStream* ax = aux_stream();
   bool forked = false;
+  // BatchNorm l's backward between convs l + 1 and l, folded where both kernels take the shape (training): the
+  // node-linear backward of conv l + 1 adds its column sums into bn_dsums[l] while it writes dx, and the target pass
+  // of conv l turns dx into g on the way (pert_tconv_bwd_bn): the two pert_bn_bwd_ex passes over [N, H] planes go.
+  // The eval-mode backward keeps pert_bn_bwd_ex.
+  const bool bn_fold = training && pert_linear_bwd_planes_supported(N, H, H, H) == 1 &&
+                       pert_tconv_bwd_bn_supported(H, d->n_rpc) == 1;
+  auto bn_bwd = [&](int l) {   // the unfolded BatchNorm(+ReLU) backward of layer l: dx (grad wrt x[l + 1]) -> g
+    return pert_bn_bwd_ex(w.dx, H, w.x[l + 1], H, w.out[l], H, w.bn_stats[l], w.bn_stats[l] + H, P.bn_g[l], 1,
+                          relu_scale, training, dskip, H, G.bn_g[l], G.bn_b[l], w.sums, N, H, live, st);
+  };
+  bool folded = false;   // the sums of BatchNorm l are in bn_dsums[l] (node-linear backward of conv l + 1)
   for (int l = L - 1; l >= 0; --l) {
     const int K = k_of(d, w, l);
     float* pl = w.planes[l];
     PROBE_START(2, l);
-    TRY(pert_tconv_bwd_c(dskip, H, pl, pl + N * H, pl + 2 * N * H, H, rowptr, csr_src, csr_if, csr_rpc, colptr,
-                         csc_pos, csc_dst, w.t_if[l], w.t_rpc[l], w.alpha[l], dq, dk, dv, H, w.dsp, w.rpc_ws,
-                         w.dt_if[l], w.dt_rpc[l], d->n_rpc, N, E, B, H, d->H, st));
+    int trc = PERT_ERR_UNSUPPORTED;
+    if (folded) {
+      const PertBnBwd bn{w.dx, w.x[l + 1], w.out[l], w.bn_stats[l], w.bn_stats[l] + H, P.bn_g[l], w.bn_dsums[l],
+                         G.bn_g[l], G.bn_b[l], live, relu_scale};
+      trc = pert_tconv_bwd_bn(dskip, H, pl, pl + N * H, pl + 2 * N * H, H, rowptr, csr_src, csr_if, csr_rpc, colptr,
+                              csc_pos, csc_dst, w.t_if[l], w.t_rpc[l], w.alpha[l], dq, dk, dv, H, w.dsp, w.rpc_ws,
+                              w.dt_if[l], w.dt_rpc[l], d->n_rpc, N, E, B, H, d->H, &bn, st);
+      if (trc == PERT_ERR_UNSUPPORTED) TRY(bn_bwd(l));
+    }
+    if (trc == PERT_ERR_UNSUPPORTED)
+      TRY(pert_tconv_bwd_c(dskip, H, pl, pl + N * H, pl + 2 * N * H, H, rowptr, csr_src, csr_if, csr_rpc, colptr,
+                           csc_pos, csc_dst, w.t_if[l], w.t_rpc[l], w.alpha[l], dq, dk, dv, H, w.dsp, w.rpc_ws,
+                           w.dt_if[l], w.dt_rpc[l], d->n_rpc, N, E, B, H, d->H, st));
+    else if (trc != PERT_OK)
+      return trc;
     PROBE_STOP(2, l);
     if (l == 0) {                       // every dT table is complete now
       forked = aux_fork(ax, st);
@@ -935,8 +960,11 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
     // (conv 0: only the embedding columns [0, H) of dX0 are needed -- x and the pad columns carry no parameters)
     const int Kd = l == 0 ? H : K;
     PROBE_START(4, l);
-    int frc = pert_linear_bwd_planes(w.dplanes, N * (long long)H, w.x[l], K, w.w4t[l], 4 * H, w.dw4[l], K, w.db4[l],
-                                     w.dx, K, N, H, K, Kd, st);
+    const bool fold = bn_fold && l > 0;
+    int frc = pert_linear_bwd_planes_ex(w.dplanes, N * (long long)H, w.x[l], K, w.w4t[l], 4 * H, w.dw4[l], K,
+                                        w.db4[l], w.dx, K, N, H, K, Kd, fold ? w.out[l - 1] : nullptr,
+                                        fold ? w.bn_stats[l - 1] : nullptr, fold ? w.bn_stats[l - 1] + H : nullptr,
+                                        relu_scale, live, fold ? w.bn_dsums[l - 1] : nullptr, st);
     if (frc == PERT_ERR_UNSUPPORTED)
       TRY(pert_gemm_tn(w.dplanes, H, H, N * (long long)H, w.x[l], K, 0, 0, w.dw4[l], K, w.db4[l], N, 4 * H, K, st));
     else if (frc != PERT_OK)
@@ -947,12 +975,8 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
       TRY(pert_gemm_nt(w.dplanes, H, H, N * (long long)H, w.w4t[l], 4 * H, nullptr, w.dx, K, 0, 0, N, Kd, 4 * H, 0, 0,
                        st));
     PROBE_STOP(5, l);
-    if (l > 0) {
-      // BN(+ReLU) backward of layer l-1: dx (grad wrt x[l]) -> g of conv l-1, into the skip plane
-      TRY(pert_bn_bwd_ex(w.dx, K, w.x[l], H, w.out[l - 1], H, w.bn_stats[l - 1], w.bn_stats[l - 1] + H,
-                         P.bn_g[l - 1], 1, relu_scale, training, dskip, H, G.bn_g[l - 1], G.bn_b[l - 1], w.sums, N, H,
-                         live, st));
-    }
+    folded = fold && frc == PERT_OK;
+    if (l > 0 && !folded) TRY(bn_bwd(l - 1));   // BN(+ReLU) backward of layer l-1 -> g of conv l-1, skip plane
   }
   if (forked) TRY(aux_join(ax, st));
   else table_grads(st);

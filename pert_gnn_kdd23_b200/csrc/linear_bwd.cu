@@ -19,9 +19,17 @@
 //     k, v, skip through distributed shared memory and writes them to dX with 16-byte stores: no memset, no global
 //     atomics, and dX is bit-identical from run to run.  It does so for tile i - 1 right after its data gradient of
 //     tile i, while warpgroup 1 is still busy with the longer weight gradient.
+// Optional BatchNorm-backward reduction (bn_sums != null, K = Kd = H): X is y = relu(bn(x)) [dropout-masked] of the
+// previous conv, and the dX rows just summed are dy of that BatchNorm.  Warpgroup 0 also reads those rows of y (X) and
+// x from global memory (the stage of the tile has been refilled by then), requested before the data gradient of the
+// next tile so that they arrive while it runs, and accumulates sum dz and sum dz*xhat per column in registers (bn.cuh,
+// the expressions of k_bn_bwd_reduce) over the rows below live[0]; at the end one fp64 atomic per column and CTA adds
+// them to bn_sums.  This replaces the k_bn_bwd_reduce pass over dx, y and x; the apply runs in the conv backward target
+// pass (tconv_tile.cu).
 // Accuracy: 3xTF32 (hi*hi + lo*hi + hi*lo, round-to-nearest split); the data gradient is four K = H tensor-core sums
 // added in fp32.
 #include "common.cuh"
+#include "bn.cuh"
 #include "sm90.cuh"
 #include <stdlib.h>
 
@@ -62,6 +70,12 @@ struct LbArgs {
   float* dX;
   int ldxo;
   int N, tiles_per_cluster;
+  // BatchNorm-backward reduction (see the top): bn_sums != null turns it on
+  const float* bn_x;                  // [N, H]: the BatchNorm input
+  const float *bn_mean, *bn_rstd;
+  float relu_scale;
+  const long long* live;              // rows >= live[0] are left out (null: all N)
+  double* bn_sums;                    // [2H] += sum dz | sum dz*xhat
 };
 
 template <int K, int KD>
@@ -110,6 +124,27 @@ __global__ void __launch_bounds__(LB_THREADS, 1) k_linear_bwd_planes(LbArgs g) {
 #pragma unroll
   for (int j = 0; j < K / 2; ++j) part[j] = 0.f;
   float cs0 = 0.f, cs1 = 0.f;
+  // BatchNorm-backward reduction (K = KD = H only): this thread always handles column group tid % 16 of its rows
+  const bool bn = K == LB_H && KD == LB_H && g.bn_sums != nullptr;
+  float4 bs1 = f4zero(), bs2 = f4zero(), bmu = f4zero(), brs = f4zero();
+  int n_live = 0;
+  if (bn && wg == 0) {
+    bmu = ldg4(g.bn_mean + (tid & 15) * 4);
+    brs = ldg4(g.bn_rstd + (tid & 15) * 4);
+    n_live = g.live ? (int)min((long long)g.N, *g.live) : g.N;
+  }
+  // BatchNorm: the y (X) and x rows this thread reduces for tile i, requested one data gradient ahead of reduce(i)
+  // (the rows of thread tid: 16 rank + tid / 16 + 8 j, column group tid % 16)
+  float4 by[2], bx[2];
+  auto bn_fetch = [&](int i) {
+    const int row0 = (t0 + i) * LB_TM;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int n = row0 + 16 * (int)rank + (tid >> 4) + 8 * j;
+      by[j] = n < n_live ? ldg4(g.X + (size_t)n * K + (tid & 15) * 4) : f4zero();
+      bx[j] = n < n_live ? ldg4(g.bn_x + (size_t)n * LB_H + (tid & 15) * 4) : f4zero();
+    }
+  };
   // dX rows 16 rank .. 16 rank + 15 of tile i = q + k + v + skip partials (warpgroup 0).  The slot of tile i is written
   // before the cluster barrier of tile i, read after it and before the barrier of tile i + 1, and rewritten for tile
   // i + 2 only after that barrier.
@@ -117,15 +152,22 @@ __global__ void __launch_bounds__(LB_THREADS, 1) k_linear_bwd_planes(LbArgs g) {
     constexpr int V = KD / 4;
     const int row0 = (t0 + i) * LB_TM, rows = min(LB_TM, g.N - row0);
     const float* P = reinterpret_cast<const float*>(smem + Lay::OFF_P + (i & 1) * Lay::P_BYTES);
-    for (int e = tid; e < 16 * V; e += 128) {
+    auto one = [&](int e, float4 y, float4 x) {
       const int r = 16 * (int)rank + e / V, c4 = e - (e / V) * V;
-      if (r >= rows) continue;
+      if (r >= rows) return;
       const uint32_t a = smem_u32(P + r * Lay::PLD + c4 * 4);
       float4 acc = ld_cluster4(map_rank(a, 0));
       acc = f4add(acc, ld_cluster4(map_rank(a, 1)));
       acc = f4add(acc, ld_cluster4(map_rank(a, 2)));
       acc = f4add(acc, ld_cluster4(map_rank(a, 3)));
       st4(g.dX + (size_t)(row0 + r) * g.ldxo + c4 * 4, acc);
+      if (bn && row0 + r < n_live) bn_bwd_acc4(bs1, bs2, bn_bwd_dz4(acc, y, g.relu_scale), x, bmu, brs);
+    };
+    if constexpr (K == LB_H && KD == LB_H) {   // 16 V = 256: the two rows of bn_fetch
+#pragma unroll
+      for (int j = 0; j < 2; ++j) one(tid + 128 * j, by[j], bx[j]);
+    } else {
+      for (int e = tid; e < 16 * V; e += 128) one(e, f4zero(), f4zero());
     }
   };
 
@@ -139,6 +181,7 @@ __global__ void __launch_bounds__(LB_THREADS, 1) k_linear_bwd_planes(LbArgs g) {
     if (wg == 0) {
       // ---- data gradient of this plane: [64, H] . [H, KD]; rows past the end are computed and not stored
       const int r0 = w * 16 + gq, r1 = r0 + 8;
+      if (bn && i > 0) bn_fetch(i - 1);   // in flight during this tile's data gradient
       uint32_t ah[LB_H / 8][4], al[LB_H / 8][4];
 #pragma unroll
       for (int q = 0; q < LB_H / 16; ++q) {
@@ -227,8 +270,28 @@ __global__ void __launch_bounds__(LB_THREADS, 1) k_linear_bwd_planes(LbArgs g) {
     }
   }
   if (wg == 1 && nt > 0) cluster_wait();
-  if (wg == 0 && nt > 0) reduce(nt - 1);
+  if (wg == 0 && nt > 0) {
+    if (bn) bn_fetch(nt - 1);
+    reduce(nt - 1);
+  }
   cluster_sync();   // no CTA exits while another may still read its partials
+  if (bn && wg == 0 && nt > 0) {
+    // the 8 threads of a column group (lanes l, l + 16 of the four warps) -> one fp64 atomic per column.  The partial
+    // slots are free: no CTA of the cluster reads them after the barrier above.
+    float* red = reinterpret_cast<float*>(smem + Lay::OFF_P);   // [4 warps][2H]
+    float v[8] = {bs1.x, bs1.y, bs1.z, bs1.w, bs2.x, bs2.y, bs2.z, bs2.w};
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v[k] += __shfl_xor_sync(0xffffffffu, v[k], 16);
+    if (lane < 16) {
+      st4(red + w * 2 * LB_H + lane * 4, make_float4(v[0], v[1], v[2], v[3]));
+      st4(red + w * 2 * LB_H + LB_H + lane * 4, make_float4(v[4], v[5], v[6], v[7]));
+    }
+    bar_sync(2, 128);
+    double t = 0.0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) t += (double)red[k * 2 * LB_H + tid];
+    atomicAdd(g.bn_sums + tid, t);
+  }
   if (wg == 1 && nt > 0) {
     cs0 += __shfl_xor_sync(0xffffffffu, cs0, 1);
     cs0 += __shfl_xor_sync(0xffffffffu, cs0, 2);
@@ -335,8 +398,19 @@ int pert_linear_bwd_planes_supported(long long N, int H, int K, int Kd) {
 int pert_linear_bwd_planes(const float* dY, long long plane_stride, const float* X, int ldx, const float* W4t, int ldw,
                            float* dW4, int ldw4, float* db4, float* dX, int ldx_out, long long N, int H, int K, int Kd,
                            void* stream) {
+  return pert_linear_bwd_planes_ex(dY, plane_stride, X, ldx, W4t, ldw, dW4, ldw4, db4, dX, ldx_out, N, H, K, Kd,
+                                   nullptr, nullptr, nullptr, 1.f, nullptr, nullptr, stream);
+}
+
+int pert_linear_bwd_planes_ex(const float* dY, long long plane_stride, const float* X, int ldx, const float* W4t,
+                              int ldw, float* dW4, int ldw4, float* db4, float* dX, int ldx_out, long long N, int H,
+                              int K, int Kd, const float* bn_x, const float* bn_mean, const float* bn_rstd,
+                              float relu_scale, const long long* live, double* bn_sums, void* stream) {
   if (!dY || !X || !W4t || !dW4 || !db4 || !dX || N < 0 || H <= 0 || K <= 0 || Kd <= 0 || Kd > K || ldx < K ||
       ldw < 4 * H || ldw4 < K || ldx_out < Kd || plane_stride < N * H)
+    return PERT_ERR_BADARG;
+  if (bn_sums && (!bn_x || !bn_mean || !bn_rstd || K != H || Kd != K || !al16(bn_x) || !al16(bn_mean) ||
+                  !al16(bn_rstd) || ((uintptr_t)bn_sums & 7)))
     return PERT_ERR_BADARG;
   if (!shape_ok(N, H, K, Kd)) return PERT_ERR_UNSUPPORTED;
   // bulk copies of whole tiles (contiguous X rows, 16-byte aligned blocks), 16-byte dX stores, 8-byte dW4 reductions
@@ -345,7 +419,8 @@ int pert_linear_bwd_planes(const float* dY, long long plane_stride, const float*
     return PERT_ERR_UNSUPPORTED;
   const int clusters = clusters_for(K, Kd);
   if (clusters <= 0) return PERT_ERR_UNSUPPORTED;   // a cluster of 4 such CTAs cannot be placed
-  LbArgs a{dY, plane_stride, X, W4t, ldw, dW4, ldw4, db4, dX, ldx_out, (int)N, 0};
+  LbArgs a{dY, plane_stride, X, W4t, ldw, dW4, ldw4, db4, dX, ldx_out, (int)N, 0,
+           bn_x, bn_mean, bn_rstd, relu_scale, live, bn_sums};
   cudaStream_t st = (cudaStream_t)stream;
   if (K == 64) return launch<64, 64>(a, clusters, st);
   if (Kd == 64) return launch<80, 64>(a, clusters, st);

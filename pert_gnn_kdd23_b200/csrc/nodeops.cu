@@ -205,9 +205,7 @@ __global__ void __launch_bounds__(256) k_bn_apply(const float* __restrict__ x, i
   }
 }
 
-// sums[0:H] += sum_n dz,  sums[H:2H] += sum_n dz*xhat   with dz = dy * (y > 0 if relu) * scale.
-// With inverted dropout after the ReLU, y > 0 <=> (ReLU active and kept), so the saved output is the whole mask and only
-// the 1/(1-p) factor is applied here (scale = 1 without dropout; __fmul_rn keeps that product exact and uncontracted).
+// sums[0:H] += sum_n dz,  sums[H:2H] += sum_n dz*xhat   with dz = dy * (y > 0 if relu) * scale (bn_bwd_dz4).
 __global__ void __launch_bounds__(256) k_bn_bwd_reduce(const float* __restrict__ dy, int ld_dy,
                                                         const float* __restrict__ y, int ld_y,
                                                         const float* __restrict__ x, int ld_x,
@@ -237,15 +235,7 @@ __global__ void __launch_bounds__(256) k_bn_bwd_reduce(const float* __restrict__
         vv[u] = ok ? ldg4(x + (size_t)(r0 + r) * ld_x + cl * 4) : mu;
       }
 #pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        float4 g = gg[u];
-        const float4 yy = yy4[u], v = vv[u];
-        g.x = yy.x > 0.f ? __fmul_rn(g.x, scale) : 0.f; g.y = yy.y > 0.f ? __fmul_rn(g.y, scale) : 0.f;
-        g.z = yy.z > 0.f ? __fmul_rn(g.z, scale) : 0.f; g.w = yy.w > 0.f ? __fmul_rn(g.w, scale) : 0.f;
-        s1 = f4add(s1, g);
-        s2.x = fmaf(g.x, (v.x - mu.x) * rs.x, s2.x); s2.y = fmaf(g.y, (v.y - mu.y) * rs.y, s2.y);
-        s2.z = fmaf(g.z, (v.z - mu.z) * rs.z, s2.z); s2.w = fmaf(g.w, (v.w - mu.w) * rs.w, s2.w);
-      }
+      for (int u = 0; u < 4; ++u) bn_bwd_acc4(s1, s2, bn_bwd_dz4(gg[u], yy4[u], scale), vv[u], mu, rs);
     }
     st4(sm + rl * 2 * H + cl * 4, s1);
     st4(sm + rl * 2 * H + H + cl * 4, s2);
@@ -283,21 +273,13 @@ __global__ void k_bn_bwd_apply(const float* __restrict__ dy, int ld_dy, const fl
     return;
   }
   float4 g = ldg4(dy + (size_t)n * ld_dy + c);
-  if (relu) {
-    float4 yy = ldg4(y + (size_t)n * ld_y + c);
-    g.x = yy.x > 0.f ? __fmul_rn(g.x, scale) : 0.f; g.y = yy.y > 0.f ? __fmul_rn(g.y, scale) : 0.f;
-    g.z = yy.z > 0.f ? __fmul_rn(g.z, scale) : 0.f; g.w = yy.w > 0.f ? __fmul_rn(g.w, scale) : 0.f;
-  }
+  if (relu) g = bn_bwd_dz4(g, ldg4(y + (size_t)n * ld_y + c), scale);
   const float4 rs = ldg4(rstd + c), ga = ldg4(gamma + c);
   float4 o;
   if (training) {
     const float invn = 1.0f / (float)n_live;
     const float4 v = ldg4(x + (size_t)n * ld_x + c), mu = ldg4(mean + c);
-    const float4 a = ldg4(sums + c), b = ldg4(sums + H + c);
-    o.x = ga.x * rs.x * (g.x - a.x * invn - (v.x - mu.x) * rs.x * b.x * invn);
-    o.y = ga.y * rs.y * (g.y - a.y * invn - (v.y - mu.y) * rs.y * b.y * invn);
-    o.z = ga.z * rs.z * (g.z - a.z * invn - (v.z - mu.z) * rs.z * b.z * invn);
-    o.w = ga.w * rs.w * (g.w - a.w * invn - (v.w - mu.w) * rs.w * b.w * invn);
+    o = bn_bwd_dx4(g, v, mu, rs, ga, ldg4(sums + c), ldg4(sums + H + c), invn);
   } else {
     o = make_float4(ga.x * rs.x * g.x, ga.y * rs.y * g.y, ga.z * rs.z * g.z, ga.w * rs.w * g.w);
   }
@@ -674,7 +656,7 @@ int pert_bn_bwd(const float* dy, int ld_dy, const float* y, int ld_y, const floa
 
 }  // extern "C"
 
-// relu_scale: factor applied to the ReLU-masked gradient (1 / (1 - p) after inverted dropout, see k_bn_bwd_reduce);
+// relu_scale: factor applied to the ReLU-masked gradient (1 / (1 - p) after inverted dropout, see bn_bwd_dz4);
 // anything but 1 needs relu.  live != null (training on a padded batch): see k_bn_bwd_apply.
 int pert_bn_bwd_ex(const float* dy, int ld_dy, const float* y, int ld_y, const float* x, int ld_x, const float* mean,
                    const float* rstd, const float* gamma, int relu, float relu_scale, int training, float* dx,

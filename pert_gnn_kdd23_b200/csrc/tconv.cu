@@ -436,7 +436,25 @@ int pert_tile_bwd(const float* g_, int ld_g, const float* q, const float* k, con
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
                   const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha, float* dq, float* dk,
                   float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc, int n_rpc, long long N,
-                  long long E, long long B, int H, int C, cudaStream_t st);
+                  long long E, long long B, int H, int C, const PertBnBwd* bn, cudaStream_t st);
+
+namespace {
+
+// argument checks shared by pert_tconv_bwd_c and pert_tconv_bwd_bn
+int bwd_args_ok(const float* g, int ld_g, const float* q, const float* k, const float* v, int ld, const int* rowptr,
+                const int* csr_if, const int* csr_rpc, const int* colptr, const float* t_if, const float* t_rpc,
+                const float* dq, const float* dk, const float* dv, int ld_d, const float* dt_if, const float* dt_rpc,
+                long long N, long long E, int H, int C) {
+  if (N < 0 || E < 0 || !g || !q || !k || !v || !rowptr || !colptr || !dq || !dk || !dv || C < 1 || C > H) return 0;
+  if (ld % 4 || ld_g % 4 || ld_d % 4 || !aligned16(g) || !aligned16(q) || !aligned16(k) || !aligned16(v) ||
+      !aligned16(dq) || !aligned16(dk) || !aligned16(dv))
+    return 0;
+  if (t_if && (!t_rpc || !dt_if || !dt_rpc || !aligned16(dt_if) || !aligned16(dt_rpc))) return 0;
+  if (t_if && E > 0 && (!csr_if || !csr_rpc)) return 0;   // an edgeless batch may pass null edge arrays
+  return 1;
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -528,17 +546,13 @@ int pert_tconv_bwd_c(const float* g, int ld_g, const float* q, const float* k, c
                      const int* csc_pos, const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha,
                      float* dq, float* dk, float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc,
                      int n_rpc, long long N, long long E, long long B_hint, int H, int C, void* stream) {
-  if (N < 0 || E < 0 || !g || !q || !k || !v || !rowptr || !colptr || !dq || !dk || !dv || C < 1 || C > H)
+  if (!bwd_args_ok(g, ld_g, q, k, v, ld, rowptr, csr_if, csr_rpc, colptr, t_if, t_rpc, dq, dk, dv, ld_d, dt_if, dt_rpc,
+                   N, E, H, C))
     return PERT_ERR_BADARG;
-  if (ld % 4 || ld_g % 4 || ld_d % 4 || !aligned16(g) || !aligned16(q) || !aligned16(k) || !aligned16(v) ||
-      !aligned16(dq) || !aligned16(dk) || !aligned16(dv))
-    return PERT_ERR_BADARG;
-  if (t_if && (!t_rpc || !dt_if || !dt_rpc || !aligned16(dt_if) || !aligned16(dt_rpc))) return PERT_ERR_BADARG;
-  if (t_if && E > 0 && (!csr_if || !csr_rpc)) return PERT_ERR_BADARG;   // an edgeless batch may pass null edge arrays
   if (N == 0) return PERT_OK;
   if (ld_d == H) {
     int rt = pert_tile_bwd(g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, colptr, csc_pos, csc_dst, t_if, t_rpc,
-                           alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, C,
+                           alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, C, nullptr,
                            (cudaStream_t)stream);
     if (rt != PERT_ERR_UNSUPPORTED) {
       if (rt) return rt;
@@ -569,6 +583,33 @@ int pert_tconv_bwd_c(const float* g, int ld_g, const float* q, const float* k, c
     return PERT_OK;
   });
   if (rc) return rc;
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+int pert_tconv_bwd_bn_supported(int H, int n_rpc) {
+  return H == 64 && n_rpc >= 0 && (size_t)n_rpc * H * 4 <= 16 * 1024 ? 1 : 0;
+}
+
+int pert_tconv_bwd_bn(float* g, int ld_g, const float* q, const float* k, const float* v, int ld, const int* rowptr,
+                      const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
+                      const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha, float* dq,
+                      float* dk, float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc,
+                      int n_rpc, long long N, long long E, long long B_hint, int H, int C, const PertBnBwd* bn,
+                      void* stream) {
+  if (!bwd_args_ok(g, ld_g, q, k, v, ld, rowptr, csr_if, csr_rpc, colptr, t_if, t_rpc, dq, dk, dv, ld_d, dt_if, dt_rpc,
+                   N, E, H, C))
+    return PERT_ERR_BADARG;
+  if (!bn || !bn->dx || !bn->y || !bn->x || !bn->mean || !bn->rstd || !bn->gamma || !bn->sums || !bn->dgamma ||
+      !bn->dbeta || !aligned16(bn->dx) || !aligned16(bn->y) || !aligned16(bn->x) || !aligned16(bn->mean) ||
+      !aligned16(bn->rstd) || !aligned16(bn->gamma) || !aligned16(bn->sums))
+    return PERT_ERR_BADARG;
+  if (!pert_tconv_bwd_bn_supported(H, n_rpc) || ld != H || ld_g != H || ld_d != H) return PERT_ERR_UNSUPPORTED;
+  if (N == 0) return PERT_OK;
+  int rt = pert_tile_bwd(g, ld_g, q, k, v, ld, rowptr, csr_src, csr_if, csr_rpc, colptr, csc_pos, csc_dst, t_if, t_rpc,
+                         alpha, dq, dk, dv, ld_d, dsp, rpc_ws, dt_if, dt_rpc, n_rpc, N, E, B_hint, H, C, bn,
+                         (cudaStream_t)stream);
+  if (rt) return rt;
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }

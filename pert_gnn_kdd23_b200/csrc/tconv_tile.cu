@@ -15,6 +15,7 @@
 //
 // Tile size (nodes) is chosen by the host so that two CTAs of 512 threads fit one SM; when the batch holds equally
 // sized graphs the tile is a whole number of graphs (no cut edges).
+#include "bn.cuh"
 #include "common.cuh"
 #include <type_traits>
 
@@ -52,6 +53,7 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ float ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -76,6 +78,8 @@ struct TileArgs {
   int N, tile_nodes, edge_cap;
   int hot_if;          // interface id whose table-gradient row is accumulated per CTA instead of per edge (source pass)
   float inv_sqrt_c;
+  PertBnBwd bn;        // bwd_dst with BN: the BatchNorm backward that yields g (include/pertgnn.h, pert_tconv_bwd_bn)
+  float* g_out;        // bwd_dst with BN: g rows, written (the plane `g` of the source pass)
 };
 
 // Gradient of the (tiny, hot) rpc-type table without per-edge atomics: for an edge t -> i of rpc type b the table row
@@ -120,6 +124,14 @@ __device__ __forceinline__ Smem carve_smem(unsigned char* base, int T, int H, in
 static size_t smem_bytes(int T, int H, int n_rpc, int ecap, int n_edge_arrays) {
   return 16 + sizeof(float) * ((size_t)2 * T * H + (size_t)n_rpc * H + ((T + 1 + 3) / 4) * 4 + ((T + 7) / 8) * 4 +
                                (size_t)n_edge_arrays * ecap);
+}
+
+// A kernel parameter read where it is used: the empty asm keeps the compiler from holding the pointer (two registers)
+// through the loops that use it.
+template <typename T>
+__device__ __forceinline__ const T* fresh(const T* p) {
+  asm volatile("" : "+l"(p));
+  return p;
 }
 
 // This CTA's tile: nodes [n0, n0 + nt), tiles of tile_nodes consecutive nodes, one per CTA.  The empty asm hides where
@@ -430,7 +442,13 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
 }
 
 // ============================================================== backward, target pass (dq, ds)
-template <int LPR, int VPL, bool HAS_E, int NT>
+// BN: g is not read but computed from the rows of dx, y and x of the node (the expressions of k_bn_bwd_apply, bn.cuh)
+// and written to g_out for the source pass and the node-linear backward.  The dx row is fetched one node ahead in
+// registers as g is otherwise, the y and x rows one node ahead into L2 only: three register rows held through the edge
+// loop spill 76 bytes per thread at 64 registers, this form 20 (nvcc 12.9, -Xptxas -v), and it measured 3 us faster
+// per launch at cfg2.  This replaces the k_bn_bwd_apply pass; CTA 0 adds the column sums into dgamma / dbeta as that
+// pass's block 0 did.
+template <int LPR, int VPL, bool HAS_E, int NT, bool BN>
 __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArgs a) {
   constexpr int H = 4 * LPR * VPL;
   constexpr int GPW = 32 / LPR;
@@ -448,6 +466,11 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
   int n0, nt;
   cta_tile(a, n0, nt);
   if (nt <= 0) return;                         // uniform across the CTA
+  if (BN && blockIdx.x == 0)                   // parameter gradients accumulate (+=) like autograd
+    for (int c = tid; c < H; c += NT) {
+      a.bn.dbeta[c] += (float)a.bn.sums[c];
+      a.bn.dgamma[c] += (float)a.bn.sums[H + c];
+    }
   tile_barrier_init(S, tid);
   stage_tiles<H, NT>(S, a.k, a.v, a.rowptr, n0, nt, tid);
   const int e_lo = S.ptr[0];
@@ -475,10 +498,24 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
 
   int slot = g0 + grp;
   int loc = slot < nt ? ldsu16(sa.ord + slot * 2) : 0;
-  float4 g_n[VPL];
+  float4 g_n[VPL];   // BN: the dx row
 #pragma unroll
   for (int u = 0; u < VPL; ++u) g_n[u] = f4zero();
-  if (slot < nt) ldrow(a.g, (size_t)(n0 + loc), g_n);
+  // BN: the dx row of the next node into g_n, its y and x rows only into L2; they are read where g is formed
+  auto fetch_bn = [&](int row) {
+    ldrow(fresh(a.bn.dx), (size_t)row, g_n);
+#pragma unroll
+    for (int u = 0; u < VPL; ++u) {
+      prefetch_l2(fresh(a.bn.y) + (size_t)row * H + (lig + u * LPR) * 4);
+      prefetch_l2(fresh(a.bn.x) + (size_t)row * H + (lig + u * LPR) * 4);
+    }
+  };
+  // BN: rows >= n_live (ghosts of a padded batch) get g = 0; the mean terms divide by n_live
+  const int n_live = BN ? (a.bn.live ? (int)min((long long)a.N, *a.bn.live) : a.N) : 0;
+  if (slot < nt) {
+    if (BN) fetch_bn(n0 + loc);
+    else ldrow(a.g, (size_t)(n0 + loc), g_n);
+  }
   auto run = [&](auto fast_c) {
     constexpr bool FAST = decltype(fast_c)::value;
     for (; slot - grp < nt; slot += GPC) {
@@ -487,11 +524,31 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
       float4 g[VPL];
 #pragma unroll
       for (int u = 0; u < VPL; ++u) g[u] = g_n[u];
+      if (BN) {
+        const float invn = 1.0f / (float)n_live;
+#pragma unroll
+        for (int u = 0; u < VPL; ++u) {
+          const int c = (lig + u * LPR) * 4;
+          if (i < n_live) {
+            const float4 y = ldg4(fresh(a.bn.y) + (size_t)i * H + c), x = ldg4(fresh(a.bn.x) + (size_t)i * H + c);
+            const double2* sp = reinterpret_cast<const double2*>(fresh(a.bn.sums) + c);
+            const double2 a0 = __ldg(sp), a1 = __ldg(sp + 1), b0 = __ldg(sp + H / 2), b1 = __ldg(sp + H / 2 + 1);
+            g[u] = bn_bwd_dx4(bn_bwd_dz4(g[u], y, a.bn.relu_scale), x, ldg4(fresh(a.bn.mean) + c),
+                              ldg4(fresh(a.bn.rstd) + c), ldg4(fresh(a.bn.gamma) + c),
+                              make_float4((float)a0.x, (float)a0.y, (float)a1.x, (float)a1.y),
+                              make_float4((float)b0.x, (float)b0.y, (float)b1.x, (float)b1.y), invn);
+          } else {
+            g[u] = f4zero();
+          }
+          if (valid) st4(const_cast<float*>(fresh(a.g_out)) + (size_t)i * H + c, g[u]);
+        }
+      }
       const int p0 = valid ? ldsi(sa.ptr + loc * 4) : 0;
       const int p1 = valid ? ldsi(sa.ptr + loc * 4 + 4) : 0;
       if (slot + GPC < nt) {
         loc = ldsu16(sa.ord + (slot + GPC) * 2);
-        ldrow(a.g, (size_t)(n0 + loc), g_n);
+        if (BN) fetch_bn(n0 + loc);
+        else ldrow(a.g, (size_t)(n0 + loc), g_n);
       }
       const int deg = p1 - p0;
       const int degmax = __reduce_max_sync(0xffffffffu, deg);
@@ -854,7 +911,7 @@ int launch_fwd(const TileArgs& a0, long long N, long long E, long long B, bool h
 // backward launches for row width H: one vector per lane (LPR = H / 4), 512-thread CTAs when two CTAs fit an SM, else
 // 1024.  (The backward pair's REDG and shared-memory atomics want the resident warps more than the fewer instructions
 // of two vectors per lane.)
-template <int H>
+template <int H, bool BN>
 int launch_bwd(const TileArgs& a0, long long N, long long E, long long B, bool has_e, cudaStream_t st) {
   const TileGeom g = tile_geom(H, a0.n_rpc, N, E, B);
   const size_t bd = smem_bytes(g.T, H, 0, g.ecap, 4);                      // src, ids, alpha, dalpha staging
@@ -869,11 +926,11 @@ int launch_bwd(const TileArgs& a0, long long N, long long E, long long B, bool h
   ad.rpc_ws = as.rpc_ws = ws;
   int rc;
   if (pd == 2)
-    rc = has_e ? launch_k(k_tile_bwd_dst<L1, 1, true, 512>, gd, 512, bd, ad, st)
-               : launch_k(k_tile_bwd_dst<L1, 1, false, 512>, gd, 512, bd, ad, st);
+    rc = has_e ? launch_k(k_tile_bwd_dst<L1, 1, true, 512, BN>, gd, 512, bd, ad, st)
+               : launch_k(k_tile_bwd_dst<L1, 1, false, 512, BN>, gd, 512, bd, ad, st);
   else
-    rc = has_e ? launch_k(k_tile_bwd_dst<L1, 1, true, 1024>, gd, 1024, bd, ad, st)
-               : launch_k(k_tile_bwd_dst<L1, 1, false, 1024>, gd, 1024, bd, ad, st);
+    rc = has_e ? launch_k(k_tile_bwd_dst<L1, 1, true, 1024, BN>, gd, 1024, bd, ad, st)
+               : launch_k(k_tile_bwd_dst<L1, 1, false, 1024, BN>, gd, 1024, bd, ad, st);
   if (rc) return rc;
   if (ps == 2)
     return has_e ? launch_k(k_tile_bwd_src<L1, 1, true, 512>, gs, 512, bs, as, st)
@@ -906,11 +963,12 @@ int pert_tile_fwd(const float* q, const float* k, const float* v, const float* s
   }
 }
 
+// bn != null: the target pass computes g (BatchNorm backward, H = 64 only) and writes it to g_ (pert_tconv_bwd_bn)
 int pert_tile_bwd(const float* g_, int ld_g, const float* q, const float* k, const float* v, int ld, const int* rowptr,
                   const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr, const int* csc_pos,
                   const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha, float* dq, float* dk,
                   float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc, int n_rpc, long long N,
-                  long long E, long long B, int H, int C, cudaStream_t st) {
+                  long long E, long long B, int H, int C, const PertBnBwd* bn, cudaStream_t st) {
   if (ld != H || ld_g != H || ld_d != H || (t_if && (size_t)n_rpc * H * 4 > 16 * 1024))
     return PERT_ERR_UNSUPPORTED;
   TileArgs a{};
@@ -921,10 +979,16 @@ int pert_tile_bwd(const float* g_, int ld_g, const float* q, const float* k, con
   a.out = dq; a.dk = dk; a.dv = dv; a.alpha = const_cast<float*>(alpha); a.dsp = dsp;
   a.dt_if = dt_if; a.dt_rpc = dt_rpc; a.rpc_ws = rpc_ws; a.hot_if = 0;
   a.N = (int)N; a.inv_sqrt_c = 1.0f / sqrtf((float)C);
+  if (bn) {
+    if (H != 64) return PERT_ERR_UNSUPPORTED;
+    a.bn = *bn;
+    a.g_out = const_cast<float*>(g_);
+    return launch_bwd<64, true>(a, N, E, B, t_if != nullptr, st);
+  }
   switch (H) {
-    case 32: return launch_bwd<32>(a, N, E, B, t_if != nullptr, st);
-    case 64: return launch_bwd<64>(a, N, E, B, t_if != nullptr, st);
-    case 128: return launch_bwd<128>(a, N, E, B, t_if != nullptr, st);
+    case 32: return launch_bwd<32, false>(a, N, E, B, t_if != nullptr, st);
+    case 64: return launch_bwd<64, false>(a, N, E, B, t_if != nullptr, st);
+    case 128: return launch_bwd<128, false>(a, N, E, B, t_if != nullptr, st);
     default: return PERT_ERR_UNSUPPORTED;
   }
 }

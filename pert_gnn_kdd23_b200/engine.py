@@ -191,12 +191,16 @@ class Engine:
 
     def launches_backward(self):
         """head, pool, per conv (target pass, source pass, node-linear backward: one fused launch where
-        pert_linear_bwd_planes takes the shape, else weight GEMM + data GEMM), per BatchNorm reduce + apply,
-        embedding scatters, edge-table gradients (3 layers per launch), unpack."""
-        L, H, N = self.n_convs, self.Hp, self._saved[8]
+        pert_linear_bwd_planes takes the shape, else weight GEMM + data GEMM), per BatchNorm reduce + apply unless the
+        training backward folds them into the node-linear backward and the target pass (pert_tconv_bwd_bn), embedding
+        scatters, edge-table gradients (3 layers per launch), unpack."""
+        L, H, N, training = self.n_convs, self.Hp, self._saved[8], self._saved[7]
         linear = sum(1 if self.lib.pert_linear_bwd_planes_supported(N, H, self.desc.k0 if l == 0 else H,
                                                                      H) else 2 for l in range(L))
-        return 1 + 1 + 2 * L + linear + 2 * (L - 1) + self.desc.n_cat + (L + 2) // 3 + self._pack_launches()
+        fold = training and self.lib.pert_linear_bwd_planes_supported(N, H, H, H) and \
+            self.lib.pert_tconv_bwd_bn_supported(H, self.desc.n_rpc)
+        bn = 0 if fold else 2 * (L - 1)
+        return 1 + 1 + 2 * L + linear + bn + self.desc.n_cat + (L + 2) // 3 + self._pack_launches()
 
     @_lib.on_device_of
     def forward(self, x, cat_X, entry_id, probs, pnn, batch, index: GraphIndex, training, probe=None,

@@ -54,7 +54,8 @@ extern "C" {
  * pert_ingest_evict_* (evicting traces from a live store); pert_store_assemble_whatif (per-request pattern mixes and
  * resource overrides), pert_store_lookup_resources; pert_raw_* (processed tables from raw rows); pert_raw_window_*
  * (raw resource samples aggregated into the open buckets' statistics); pert_linear_bwd_planes_ex, pert_tconv_bwd_bn
- * (_supported) (the BatchNorm backward folded into the node-linear and conv backward passes). */
+ * (_supported) (the BatchNorm backward folded into the node-linear and conv backward passes); pert_tconv_fwd_stats
+ * (the conv forward with the BatchNorm statistics of its output). */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -141,6 +142,18 @@ int pert_tconv_bwd_c(const float* g, int ld_g, const float* q, const float* k, c
                      const int* csc_pos, const int* csc_dst, const float* t_if, const float* t_rpc, const float* alpha,
                      float* dq, float* dk, float* dv, int ld_d, float* dsp, float* rpc_ws, float* dt_if, float* dt_rpc,
                      int n_rpc, long long N, long long E, long long B_hint, int H, int C, void* stream);
+/* pert_tconv_fwd_c that also leaves the BatchNorm statistics of `out` (the training forward of the step engine):
+ * bn_acc [2][H] doubles (+=; the caller zeroes it) receives, per node tile, n_b mean_b and M2_b + n_b mean_b^2 of each
+ * column, M2_b the tile's sum of squares centred on its mean_b (so mean = bn_acc[c] / n and the biased variance
+ * (bn_acc[H + c] - n mean^2) / n, n = live[0], or N without live), counting the rows below live[0] (live: optional
+ * device {N, B} of a padded batch; NULL: all N).  *fused = 1 when the staged tile kernel ran and bn_acc holds the
+ * statistics; *fused = 0 (bn_acc untouched) when the shape takes the per-row kernels, or bn_acc is NULL: the caller
+ * then computes the statistics with its own pass.  `out` is bit-identical to pert_tconv_fwd_c's. */
+int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
+                         const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if,
+                         const float* t_rpc, float* out, int ld_out, float* alpha, int n_rpc, long long N, long long E,
+                         long long B_hint, int H, int C, double* bn_acc, const long long* live, int* fused,
+                         void* stream);
 /* The backward of the BatchNorm(+ReLU, +dropout) that feeds a conv, folded into that conv's backward (training): the
  * conv's output gradient g is not read but computed row by row where the target pass loads it, and written to g (the
  * node-linear backward of the conv reads it as its skip plane; pert_bn_bwd semantics):

@@ -35,6 +35,7 @@ SIGNATURES = {
     "pert_tconv_fwd_c": (I, [P, P, P, P, I, P, P, P, P, P, P, P, I, P, I, LL, LL, LL, I, I, P]),
     "pert_tconv_bwd_c": (I, [P, I, P, P, P, I, P, P, P, P, P, P, P, P, P, P, P, P, P, I, P, P, P, P, I, LL, LL, LL, I,
                              I, P]),
+    "pert_tconv_fwd_stats": (I, [P, P, P, P, I, P, P, P, P, P, P, P, I, P, I, LL, LL, LL, I, I, P, P, P, P]),
     "pert_tconv_bwd_bn": (I, [P, I, P, P, P, I, P, P, P, P, P, P, P, P, P, P, P, P, P, I, P, P, P, P, I, LL, LL, LL, I,
                               I, P, P]),
     "pert_tconv_bwd_bn_supported": (I, [I, I]),

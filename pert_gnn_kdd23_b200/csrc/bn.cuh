@@ -46,9 +46,19 @@ __device__ __forceinline__ BnDropKey bn_drop_key(const BnDropout& drop) {
   return BnDropKey{make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)), (uint32_t)step, (uint32_t)(step >> 32)};
 }
 
-// Training: mean / rstd of column c from the fp64 sums acc = [sum | sum of squares] (k_bn_partial or the conv
-// epilogue).  The CTA that passes `owner` also stores them for the backward pass and updates the running statistics
-// (unbiased variance) and num_batches_tracked.
+// One chunk of n rows of column c into the fp64 statistics accumulator acc = [2][H] (k_bn_partial's 128-row chunks,
+// the conv epilogue's node tiles): acc[c] += n mu,  acc[H + c] += M2 + n mu^2, where M2 is the chunk's sum of squares
+// CENTRED on mu.  Raw fp32 sums of squares would lose the variance to cancellation once |mean| >> std (a column of
+// mean 1e3 / std 1 keeps about 3 correct digits, a constant column gets a variance of rounding noise); with centred
+// chunks, acc[H + c] - acc[c]^2 / N in fp64 cancels only the n mu^2 terms, which fp64 carries exactly enough.
+__device__ __forceinline__ void bn_acc_chunk(double* acc, int H, int c, double n, double mu, double m2) {
+  atomicAdd(acc + c, n * mu);
+  atomicAdd(acc + H + c, m2 + n * mu * mu);
+}
+
+// Training: mean / rstd of column c from the fp64 sums acc = [sum | sum of squares] (bn_acc_chunk: k_bn_partial or
+// the conv epilogue).  The CTA that passes `owner` also stores them for the backward pass and updates the running
+// statistics (unbiased variance) and num_batches_tracked.
 __device__ __forceinline__ void bn_batch_stats(const double* acc, long long N, int H, int c, float eps, float momentum,
                                                bool owner, float* mean, float* rstd, float* running_mean,
                                                float* running_var, long long* num_batches_tracked, float& mu,

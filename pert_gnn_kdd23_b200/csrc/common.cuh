@@ -90,13 +90,6 @@ __device__ __forceinline__ float group_sum(float v, unsigned gmask) {
 // engine-internal entry points (not part of the C-ABI)
 // PERT_GEMM_TC=0: the exact-fp32 SIMT GEMMs of gemm.cu instead of the tensor-core kernels (csrc/gemm_tc.cu), read once
 bool pert_gemm_tc_enabled();
-// live: optional device {N, B} of a padded batch (pert_batch_pad); the BatchNorm sums then count the rows below live[0].
-// C: the logical width whose 1/sqrt(C) scales the logits (pert_tconv_fwd_c; C = H for an unpadded model)
-int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
-                         const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if,
-                         const float* t_rpc, float* out, int ld_out, float* alpha, int n_rpc, long long N, long long E,
-                         long long B_hint, int H, int C, double* bn_acc, const long long* live, int* fused,
-                         void* stream);
 int pert_bn_fwd_ex(const float* x, int ld_x, const float* gamma, const float* beta, float* running_mean,
                    float* running_var, long long* num_batches_tracked, float eps, float momentum, int training,
                    int relu, float* mean, float* rstd, float* y, int ld_y, long long N, int H, void* workspace,

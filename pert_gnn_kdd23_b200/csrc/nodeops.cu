@@ -76,10 +76,9 @@ __global__ void k_copy_cols(const float* __restrict__ x, int F, float* __restric
 constexpr int BN_ROWS = 128;      // rows per CTA chunk (forward statistics)
 constexpr int BN_BWD_ROWS = 64;   // rows per CTA (backward reductions: atomics, so the chunk count is free)
 
-// per-chunk (mean, M2) with a two-pass centred sum in fp32; the chunks are combined in double precision:
-// acc[c] += n_b mean_b,  acc[H + c] += M2_b + n_b mean_b^2  (fp64 atomics; sum and sum of squares of fp32 data are
-// exact enough in fp64 that  M2 = S2 - S1^2 / N  has no cancellation problem), so no finalize kernel is needed --
-// k_bn_apply derives mean / rstd from acc in its prologue.
+// per-chunk (mean, M2) with a two-pass centred sum in fp32; the chunks are combined in double precision by
+// bn_acc_chunk (bn.cuh: acc[c] += n_b mean_b,  acc[H + c] += M2_b + n_b mean_b^2, fp64 atomics), so no finalize kernel
+// is needed -- k_bn_apply derives mean / rstd from acc in its prologue.
 // live != null (padded batch, see pert_batch_pad): only the rows below live[0] are counted.
 __global__ void __launch_bounds__(256) k_bn_partial(const float* __restrict__ x, int ld, long long N, int H,
                                                      double* __restrict__ acc /*[2][H], zeroed*/,
@@ -137,9 +136,7 @@ __global__ void __launch_bounds__(256) k_bn_partial(const float* __restrict__ x,
   for (int c = threadIdx.x; c < H; c += blockDim.x) {
     float t = 0.f;
     for (int i = 0; i < rl_n; ++i) t += s_red[i * H + c];
-    const double m = (double)s_mean[c], n = (double)rows;
-    atomicAdd(acc + c, n * m);
-    atomicAdd(acc + H + c, (double)t + n * m * m);
+    bn_acc_chunk(acc, H, c, (double)rows, (double)s_mean[c], (double)t);
   }
 }
 

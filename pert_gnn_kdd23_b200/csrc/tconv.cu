@@ -462,11 +462,7 @@ int pert_tconv_supported_width(int H) {
   return dispatch_h(H, [](auto, auto) { return 1; }) == 1 ? 1 : 0;
 }
 
-}  // extern "C"
-
-// Engine-internal form of pert_tconv_fwd_c: bn_acc (optional, [2][H] doubles, zeroed by the caller) receives the column
-// sums / sums of squares of `out` when the staged tile kernel runs (*fused = 1); otherwise *fused = 0 and the caller
-// computes the BatchNorm statistics with its own pass.
+// pert_tconv_fwd_c with the BatchNorm statistics of `out` fused into the staged tile kernel (include/pertgnn.h)
 int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                          const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if,
                          const float* t_rpc, float* out, int ld_out, float* alpha, int n_rpc, long long N, long long E,
@@ -475,7 +471,7 @@ int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const f
   *fused = 0;
   if (bn_acc && N > 0 && ld_out == H && q && k && v && rowptr && out && !(ld % 4) && aligned16(q) &&
       aligned16(k) && aligned16(v) && aligned16(out) && (!s || aligned16(s)) &&
-      (!t_if || (aligned16(t_if) && t_rpc && aligned16(t_rpc) && csr_if && csr_rpc))) {
+      (!t_if || (aligned16(t_if) && t_rpc && aligned16(t_rpc) && (E == 0 || (csr_if && csr_rpc))))) {   // as _c
     int rt = pert_tile_fwd(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, n_rpc, out, ld_out, alpha, N, E,
                            B_hint, H, C, bn_acc, live, (cudaStream_t)stream);
     if (rt == PERT_OK) {
@@ -488,8 +484,6 @@ int pert_tconv_fwd_stats(const float* q, const float* k, const float* v, const f
   return pert_tconv_fwd_c(q, k, v, s, ld, rowptr, csr_src, csr_if, csr_rpc, t_if, t_rpc, out, ld_out, alpha, n_rpc, N,
                           E, B_hint, H, C, stream);
 }
-
-extern "C" {
 
 int pert_tconv_fwd(const float* q, const float* k, const float* v, const float* s, int ld, const int* rowptr,
                    const int* csr_src, const int* csr_if, const int* csr_rpc, const float* t_if, const float* t_rpc,

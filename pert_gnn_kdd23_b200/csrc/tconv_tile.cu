@@ -72,7 +72,7 @@ struct TileArgs {
   float* alpha;     // fwd: written; bwd: read
   float* dsp;       // bwd_dst: written; bwd_src: read
   float *dt_if, *dt_rpc;
-  double* bn_acc;   // fwd: optional [2][H] column sums / sums of squares of `out` (BatchNorm statistics), +=
+  double* bn_acc;   // fwd: optional [2][H] BatchNorm statistics of `out` (bn_acc_chunk per tile), +=
   const long long* live;   // fwd, padded batch: bn_acc counts the nodes below live[0] only (null: all N)
   float* rpc_ws;    // [N][2][RPC_FAST] per-target sums over in-edges of (alpha, ds) by rpc type, or null (see bwd_src)
   int N, tile_nodes, edge_cap;
@@ -246,9 +246,9 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
   const int lane = tid & 31, lig = lane % LPR, grp = lane / LPR;
   const float qscale = a.inv_sqrt_c * 1.4426950408889634f;   // logits kept in log2 units: exp(x) = 2^(x*log2 e)
   const int g0 = (tid >> 5) * GPW;          // first group slot of this warp
-  float4 bsum[VPL], bsq[VPL];               // this lane's columns over its nodes (fused BatchNorm statistics)
+  float4 bsum[VPL];                         // this lane's columns over its nodes (fused BatchNorm statistics)
 #pragma unroll
-  for (int u = 0; u < VPL; ++u) bsum[u] = bsq[u] = f4zero();
+  for (int u = 0; u < VPL; ++u) bsum[u] = f4zero();
   auto ldrow = [&](const float* base, size_t row, float4 (&v)[VPL]) {
 #pragma unroll
     for (int u = 0; u < VPL; ++u) v[u] = ldg4(base + row * H + (lig + u * LPR) * 4);
@@ -400,10 +400,7 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
         for (int u = 0; u < VPL; ++u) {
           const float4 o = f4add(f4scale(invZ, acc[u]), skip[u]);
           st4(a.out + (size_t)i * H + (lig + u * LPR) * 4, o);
-          if (!counted) continue;
-          bsum[u] = f4add(bsum[u], o);
-          bsq[u].x = fmaf(o.x, o.x, bsq[u].x); bsq[u].y = fmaf(o.y, o.y, bsq[u].y);
-          bsq[u].z = fmaf(o.z, o.z, bsq[u].z); bsq[u].w = fmaf(o.w, o.w, bsq[u].w);
+          if (counted) bsum[u] = f4add(bsum[u], o);
         }
       }
       __syncwarp();
@@ -417,27 +414,56 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
   if (all_in) run(std::true_type{});
   else run(std::false_type{});
   if (a.bn_acc) {
-    // BatchNorm statistics of this layer's output, fused: column sums and sums of squares over the CTA's tile (per-lane
-    // fp32 partials, combined in fp64) -> one fp64 atomic per column and CTA into bn_acc, the accumulator k_bn_apply
-    // derives mean / rstd from (nodeops.cu).  Saves the separate statistics pass over `out`.
+    // BatchNorm statistics of this layer's output, fused: the tile's column means and sums of squares centred on them
+    // (the k_bn_partial contract, bn_acc_chunk), one pair of fp64 atomics per column and CTA into bn_acc, the
+    // accumulator k_bn_apply derives mean / rstd from (nodeops.cu).  Saves the separate statistics pass over `out`.
+    // The centred pass re-reads the tile's out rows after the barrier below, which makes this CTA's stores visible to
+    // all its threads; the rows were written moments ago and are still in L2.  The counted nodes are the tile's first
+    // nb rows (live[0] cuts a prefix).
+    const long long lv = a.live ? *reinterpret_cast<const volatile long long*>(a.live) : (long long)a.N;   // as above
+    const int nb = (int)max(0LL, min((long long)nt, lv - n0));   // counted nodes of the tile (uniform across the CTA)
+    if (nb == 0) return;
     __syncthreads();                                   // every warp is done with the staged tiles
-    double* sc = reinterpret_cast<double*>(S.ta);
+    double* sc = reinterpret_cast<double*>(S.ta);      // [H] column sums, [H] centred sums of squares
+    float* smu = reinterpret_cast<float*>(sc + 2 * H);  // [H] tile means (launch_fwd sizes the allocation for these)
     for (int x = tid; x < 2 * H; x += NT) sc[x] = 0.0;
     __syncthreads();
+    auto colsum = [&](const float4 (&p)[VPL], double* dst) {   // lane partials -> one fp64 shared atomic per group 0
+#pragma unroll
+      for (int u = 0; u < VPL; ++u) {
+        float vals[4] = {p[u].x, p[u].y, p[u].z, p[u].w};
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          float v = vals[kk];
+#pragma unroll
+          for (int off = LPR; off < 32; off <<= 1) v += __shfl_xor_sync(0xffffffffu, v, off);   // the warp's groups
+          if (grp == 0) atomicAdd(&dst[(lig + u * LPR) * 4 + kk], (double)v);
+        }
+      }
+    };
+    colsum(bsum, sc);
+    __syncthreads();
+    for (int x = tid; x < H; x += NT) smu[x] = (float)(sc[x] / (double)nb);
+    __syncthreads();
+    float4 mu[VPL], q[VPL];
 #pragma unroll
     for (int u = 0; u < VPL; ++u) {
-      float vals[8] = {bsum[u].x, bsum[u].y, bsum[u].z, bsum[u].w, bsq[u].x, bsq[u].y, bsq[u].z, bsq[u].w};
+      mu[u] = ld4(smu + (lig + u * LPR) * 4);
+      q[u] = f4zero();
+    }
+    for (int r = tid / LPR; r < nb; r += GPC) {        // rows in order, a lane group per row
+      const int i = n0 + r;
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
-        float v = vals[kk];
-#pragma unroll
-        for (int off = LPR; off < 32; off <<= 1) v += __shfl_xor_sync(0xffffffffu, v, off);   // the warp's groups
-        if (grp == 0) atomicAdd(&sc[(kk < 4 ? 0 : H) + (lig + u * LPR) * 4 + (kk & 3)], (double)v);
+      for (int u = 0; u < VPL; ++u) {
+        const float4 o = ld4(a.out + (size_t)i * H + (lig + u * LPR) * 4);
+        const float dx = o.x - mu[u].x, dy = o.y - mu[u].y, dz = o.z - mu[u].z, dw = o.w - mu[u].w;
+        q[u].x = fmaf(dx, dx, q[u].x); q[u].y = fmaf(dy, dy, q[u].y);
+        q[u].z = fmaf(dz, dz, q[u].z); q[u].w = fmaf(dw, dw, q[u].w);
       }
     }
+    colsum(q, sc + H);
     __syncthreads();
-    for (int x = tid; x < 2 * H; x += NT)
-      if (sc[x] != 0.0) atomicAdd(a.bn_acc + x, sc[x]);
+    for (int x = tid; x < H; x += NT) bn_acc_chunk(a.bn_acc, H, x, (double)nb, (double)smu[x], sc[H + x]);
   }
 }
 
@@ -899,7 +925,10 @@ int launch_k(K kernel, int grid, int threads, size_t bytes, const TileArgs& a, c
 template <int H>
 int launch_fwd(const TileArgs& a0, long long N, long long E, long long B, bool has_e, cudaStream_t st) {
   const TileGeom g = tile_geom(H, a0.n_rpc, N, E, B);
-  const size_t bytes = smem_bytes(g.T, H, 0, g.ecap, 3);   // src, packed ids, logit staging
+  // src, packed ids, logit staging; and at least the BatchNorm epilogue's scratch (2H doubles + H floats after the
+  // barrier word), which outgrows the staged arrays when N < 3 makes the tiles one or two rows
+  size_t bytes = smem_bytes(g.T, H, 0, g.ecap, 3);
+  if (a0.bn_acc) bytes = max(bytes, (size_t)16 + (size_t)H * (2 * sizeof(double) + sizeof(float)));
   TileArgs a = a0;
   int grid = 0;
   if (plan_launch(a, g, bytes, N, grid) == 2)

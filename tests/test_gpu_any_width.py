@@ -21,13 +21,16 @@ REPRESENTATIVE = (10, 48, 100, 192, 200, 256)
 SEED = 0x0A11_F1D7_4B1D_7E5
 
 
-def _models(cfg, H, seed=0):
+def _models(cfg, H, seed=0, prep=None):
+    """-> (oracle, model on the GPU) with the same parameters; prep(oracle) edits them before they are copied."""
     from pert_gnn_kdd23_b200.model import SAGEDeterministic
 
     args = list(model_args(cfg))
     args[5] = H
     torch.manual_seed(seed)
     oracle = OracleSAGEDeterministic(*args)
+    if prep is not None:
+        prep(oracle)
     model = SAGEDeterministic(*args)
     model.load_state_dict(oracle.state_dict())
     return oracle, model.cuda()
@@ -37,14 +40,14 @@ def _loss(g, l, y):
     return model_oracle.torch_quantile_loss(y, g.flatten(), 0.5) + 1e-3 * l.square().mean()
 
 
-def _parity(cfg, ng, H, p=0.0, tag=""):
+def _parity(cfg, ng, H, p=0.0, tag="", prep=None):
     """One training forward + backward through the engine against the fp32 oracle with the fp64 arbiter, both run on
     the engine's active ReLUs (and dropout masks, restated at Hp and cut to H); then an eval forward against the
     oracle with its own ReLUs.  -> (model, batch) after the training step."""
     b = make_batch(cfg, ng)
     a32 = forward_args(b)
     a64 = [t.double() if t.is_floating_point() else t for t in a32]
-    oracle, model = _models(cfg, H)
+    oracle, model = _models(cfg, H, prep=prep)
     assert list(model.state_dict()) == list(oracle.state_dict())
     assert all(v.shape == oracle.state_dict()[k].shape for k, v in model.state_dict().items())
     for m in (oracle, model):

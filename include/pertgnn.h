@@ -55,7 +55,8 @@ extern "C" {
  * resource overrides), pert_store_lookup_resources; pert_raw_* (processed tables from raw rows); pert_raw_window_*
  * (raw resource samples aggregated into the open buckets' statistics); pert_linear_bwd_planes_ex, pert_tconv_bwd_bn
  * (_supported) (the BatchNorm backward folded into the node-linear and conv backward passes); pert_tconv_fwd_stats
- * (the conv forward with the BatchNorm statistics of its output). */
+ * (the conv forward with the BatchNorm statistics of its output); pert_flat_grow (relayout of the flat parameter and
+ * optimizer buffers when embedding tables grow).  An additive entry point leaves the version as it is. */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -300,6 +301,25 @@ int pert_eval_metrics_live(const int64_t* y, const float* yhat, float tau, long 
 /* torch.optim.Adam step (pert_gnn.py:343,247) over one flat parameter buffer; g is scaled by grad_scale. */
 int pert_adam_step(float* p, const float* g, float* m, float* v, long long n, float lr, float beta1, float beta2,
                    float eps, float weight_decay, long long step, float grad_scale, void* stream);
+
+/* ---- relayout of the flat parameter buffers when parameters grow (csrc/flat.cu) -----------------------------------
+ * train.FlatParams keeps every trainable parameter in one flat fp32 buffer, each starting on a PERT_FLAT_ALIGN-float
+ * boundary; Adam's m and v share that layout.  Growing a parameter (new embedding rows) moves every one after it.
+ * `segs` is a HOST array [n_seg][4] of (old_off, new_off, old_len, new_len) in floats, one row per parameter.  One
+ * launch, in stream order and without a host synchronisation:
+ *   - copies old_len floats of each segment of p_old, m_old and v_old bit for bit to new_off of p_new, m_new, v_new;
+ *   - writes 0 to every other float of the new buffers (the new tail of each segment and all padding);
+ *   - writes 0 to the whole new gradient buffer g_new.
+ * m_old / m_new and v_old / v_new may be NULL (as a pair: no optimizer state to carry).  PERT_ERR_BADARG, before any
+ * CUDA call, for n_seg outside [0, PERT_FLAT_MAX_SEGS], sizes that are negative, not multiples of PERT_FLAT_ALIGN or with
+ * n_new < n_old, offsets that are not multiples of PERT_FLAT_ALIGN, segments out of order or overlapping in either
+ * layout or running past n_old / n_new, new_len < old_len, NULL p_old / p_new / g_new or one half of a pair, pointers
+ * not 16-byte aligned, and any two buffers that overlap. */
+#define PERT_FLAT_ALIGN 64
+#define PERT_FLAT_MAX_SEGS 128
+int pert_flat_grow(const long long* segs, int n_seg, long long n_old, long long n_new, const float* p_old,
+                   float* p_new, const float* m_old, float* m_new, const float* v_old, float* v_new, float* g_new,
+                   void* stream);
 
 /* ---- gradient all-reduce fused with Adam over NVLink peer memory (csrc/peer.cu) ---------------------------
  * Data-parallel form of pert_adam_step, one kernel per step and no NCCL on the step path: every rank publishes its

@@ -62,6 +62,8 @@ SIGNATURES = {
     "pert_pinball_loss_live": (I, [P, P, F, LL, F, P, P, P, P]),
     "pert_eval_metrics_live": (I, [P, P, F, LL, P, P, P]),
     "pert_adam_step": (I, [P, P, P, P, LL, F, F, F, F, F, LL, F, P]),
+    # relayout of the flat parameter / Adam buffers when parameters grow (csrc/flat.cu; first argument: host table)
+    "pert_flat_grow": (I, [P, I, LL, LL, P, P, P, P, P, P, P, P]),
     # fused all-reduce + Adam over peer memory (csrc/peer.cu)
     "pert_peer_exchange_bytes": (LL, [LL]),
     "pert_peer_alloc": (I, [LL, P, P]),
@@ -144,6 +146,7 @@ class PertGnnError(RuntimeError):
 # ---- the structs of include/pertgnn.h, field for field, checked against the header by tests/test_abi_structs.py; the
 # header documents every field
 MAX_CONVS, MAX_CAT = 8, 4                               # PERT_MAX_CONVS, PERT_MAX_CAT
+FLAT_ALIGN, FLAT_MAX_SEGS = 64, 128                      # PERT_FLAT_ALIGN, PERT_FLAT_MAX_SEGS
 
 
 class PertModelDesc(C.Structure):

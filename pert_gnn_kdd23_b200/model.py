@@ -68,6 +68,13 @@ class SAGEDeterministic(torch.nn.Module):
         self._engine = Engine(self, flat)
         return self._engine
 
+    def reset_engine(self):
+        """Drops the step engine; the next use builds one over the current parameters.  For changes ``engine()``
+        cannot see: after ``train.grow_embeddings`` the FlatParams is the same object, still owning every parameter,
+        but the engine's descriptor holds the old row counts and offsets.  The BatchNorm running statistics live in the
+        module buffers and the dropout counter in ``dropout_state()``, so both carry over into the new engine."""
+        self._engine = None
+
     def dropout_state(self):
         """The engine's dropout counter: int64 ``{seed, step}`` in device memory, on this model's device.  Every
         training forward with ``dropout > 0`` on the engine reads it and adds 1 to ``step`` on the device (a replayed

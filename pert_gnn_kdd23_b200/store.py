@@ -1206,6 +1206,18 @@ class PatternStore:
             values.data_ptr(), found.data_ptr(), _lib.stream()), "pert_store_lookup_resources")
         return values, found
 
+    def id_bounds(self):
+        """The embedding rows the store's live data needs, {"entry", "cat", "interface", "rpctype"}: n_ent entries,
+        the largest microservice id of the patterns (``pat_ms``) + 1, and the largest interface and rpctype ids of
+        the pattern edges (``pat_attr`` columns 0 and 1) + 1; 0 where there is none.  Reduced on the device, one
+        device-to-host read (``train.grow_embeddings`` grows a model to these counts)."""
+        t = self.t
+        with torch.cuda.device(self.device):
+            cols = [t["pat_ms"].reshape(-1)] + [t["pat_attr"][:, c] if self.attr_cols > c else t["pat_ms"][:0]
+                                                for c in (0, 1)]
+            top = torch.stack([torch.cat([c, c.new_full((1,), -1)]).amax() for c in cols]).cpu().tolist()
+        return {"entry": int(self.desc.n_ent), "cat": top[0] + 1, "interface": top[1] + 1, "rpctype": top[2] + 1}
+
     def check(self):
         """Synchronising check of the status word (trace id or entry id out of range / missing (timestamp, ms) row of
         the exact join)."""

@@ -4,6 +4,9 @@ flat-buffer gradient all-reduce per step).
 """
 from __future__ import annotations
 
+import operator
+import weakref
+
 import numpy as np
 import torch
 import torch.distributed as dist
@@ -25,29 +28,38 @@ def model_inputs(data):
             data.batch)
 
 
+def flat_layout(sizes):
+    """Offsets (floats) of parameters of ``sizes`` floats in one flat buffer, each on a ``_lib.FLAT_ALIGN``-float
+    (256-byte: float4 / TMA) boundary, and the buffer's length -> (offsets, n)."""
+    a = _lib.FLAT_ALIGN
+    offs, n = [], 0
+    for k in sizes:
+        offs.append(n)
+        n += (int(k) + a - 1) // a * a
+    return offs, n
+
+
 class FlatParams:
     """All parameters (and their gradients) of a module as views into two flat fp32 buffers, so that the
     gradient all-reduce and the Adam update are ONE collective and ONE kernel (payload <= 4.8 MB, latency-bound)."""
 
     def __init__(self, module, bind_grads=True):
         params = [p for p in module.parameters() if p.requires_grad]
-        al = lambda k: (k + 63) // 64 * 64          # every parameter starts on a 256-byte boundary (float4 / TMA)
-        n = sum(al(p.numel()) for p in params)
+        offs, n = flat_layout([p.numel() for p in params])
         dev = params[0].device
         self.flat = torch.zeros(n, device=dev, dtype=torch.float32)
         self.grad = torch.zeros(n, device=dev, dtype=torch.float32)
-        off = 0
         self._layout = []                              # (offset, shape, contiguous strides) of every parameter
-        for p in params:
+        for p, off in zip(params, offs):
             k = p.numel()
             self.flat[off:off + k].copy_(p.data.reshape(-1))
             p.data = self.flat[off:off + k].view_as(p)
             if bind_grads:
                 p.grad = self.grad[off:off + k].view_as(p)
             self._layout.append((off, tuple(p.shape), tuple(p.stride())))
-            off += al(k)
         self.params = params
         self.numel = n
+        self._optimizers = []      # weak references to the FusedAdams over this object, whose m and v grow() relays
         # ONE FlatParams per module: model.engine() adopts this one instead of re-pointing p.data into a second flat
         # buffer (which would silently detach an optimizer built over this one)
         if isinstance(module, torch.nn.Module):
@@ -78,6 +90,80 @@ class FlatParams:
     def zero_grad(self):
         self.grad.zero_()
 
+    def grow_plan(self, new_shapes):
+        """The layout ``grow(new_shapes)`` moves to, host only: (shapes, offsets, length, segment table [n, 4] int64 of
+        (old_off, new_off, old_len, new_len) per parameter).  ``PertGnnError`` for a shape ``grow`` refuses."""
+        shapes = [tuple(int(d) for d in s) for s in new_shapes]
+        if len(shapes) != len(self.params):
+            raise _lib.PertGnnError(f"FlatParams.grow: {len(shapes)} shapes for {len(self.params)} parameters")
+        for i, (p, s) in enumerate(zip(self.params, shapes)):
+            old = tuple(p.shape)
+            if len(s) != len(old) or s[1:] != old[1:] or (old and s[0] < old[0]):
+                raise _lib.PertGnnError(f"FlatParams.grow: parameter {i} of shape {old} cannot become {s} (only the "
+                                        "first dimension may grow)")
+        if len(self.params) > _lib.FLAT_MAX_SEGS:
+            raise _lib.PertGnnError(f"FlatParams.grow: {len(self.params)} parameters, at most {_lib.FLAT_MAX_SEGS}")
+        sizes = [int(np.prod(s, dtype=np.int64)) for s in shapes]
+        offs, n = flat_layout(sizes)
+        segs = np.array([(o, no, p.numel(), k) for (o, _, _), no, p, k in zip(self._layout, offs, self.params, sizes)],
+                        dtype=np.int64).reshape(-1, 4)
+        return shapes, offs, n, segs
+
+    def _live_optimizers(self):
+        self._optimizers = [r for r in self._optimizers if r() is not None]
+        return [r() for r in self._optimizers]
+
+    @_lib.on_device_of
+    def grow(self, new_shapes):
+        """Grows parameters in place.  ``new_shapes``: one shape per parameter, in ``params`` order, equal to its
+        current shape except for the first dimension, which may only grow (new embedding rows).
+
+        The new layout follows the constructor's rule (``flat_layout``).  Every new buffer is allocated before anything
+        changes; then one launch (``pert_flat_grow``) copies each parameter, and each parameter's slot of the m and v
+        of the ``FusedAdam`` over this object (every one registers itself here), bit for bit to its new offset, writes 0
+        to the new rows and the padding, and zeroes the new gradient buffer.  So no optimizer over this object is left
+        with buffers of the old length, whether or not the caller names it.  Every parameter is re-pointed at the new
+        buffer.  A gradient bound to ``grad`` is bound to the new one; any other ``p.grad`` is stale and set to None.
+        This object stays the one the model, the optimizer and ``DataParallel`` hold.  ``PertGnnError``, before anything
+        changes, for host buffers, for more than one live FusedAdam over this object and for a ``PeerAdam`` over more
+        than one rank (its m and v cover its own slice)."""
+        shapes, offs, n, segs = self.grow_plan(new_shapes)
+        opts = self._live_optimizers()
+        if len(opts) > 1:
+            raise _lib.PertGnnError(f"FlatParams.grow: {len(opts)} FusedAdams hold this FlatParams; one can be relaid")
+        if opts and getattr(opts[0], "world", 1) > 1:
+            raise _lib.PertGnnError("FlatParams.grow: PeerAdam over more than one rank keeps m and v for its own slice "
+                                    "only; growing it is not supported")
+        carry = [b for o in opts for b in (o.m, o.v)]
+        if any(c.shape != self.flat.shape for c in carry):
+            raise _lib.PertGnnError("FlatParams.grow: the optimizer's m / v are not laid out like this FlatParams")
+        if not self.flat.is_cuda:
+            raise _lib.PertGnnError("FlatParams.grow needs CUDA buffers (no CPU fallback for the relayout)")
+        sizes = segs[:, 3].tolist()
+        dev = self.device
+        flat, grad = (torch.empty(n, device=dev, dtype=torch.float32) for _ in range(2))
+        out = [torch.empty(n, device=dev, dtype=torch.float32) for _ in carry]
+        src, dst = carry + [None] * (2 - len(carry)), out + [None] * (2 - len(out))
+        p = _lib.ptr
+        _lib.call("pert_flat_grow", segs.ctypes.data, segs.shape[0], self.numel, n, p(self.flat), p(flat), p(src[0]),
+                  p(dst[0]), p(src[1]), p(dst[1]), p(grad), _lib.stream())
+        ops.LAUNCHES["n"] += 1
+        st = torch.cuda.current_stream()
+        for t in (self.flat, self.grad, *carry):        # the launch still reads them: no reuse before it is done
+            t.record_stream(st)
+        lo, hi = self.grad.data_ptr(), self.grad.data_ptr() + self.grad.numel() * 4
+        layout = []
+        for q, off, s, k in zip(self.params, offs, shapes, sizes):
+            bound = q.grad is not None and lo <= q.grad.data_ptr() < hi
+            q.grad = None
+            q.data = flat[off:off + k].view(s)
+            if bound:
+                q.grad = grad[off:off + k].view(s)
+            layout.append((off, s, tuple(q.stride())))
+        self.flat, self.grad, self._layout, self.numel = flat, grad, layout, n
+        if opts:
+            opts[0].m, opts[0].v = out
+
 
 class FusedAdam:
     """torch.optim.Adam(params, lr) semantics (reference pert_gnn.py:343) in one kernel over FlatParams."""
@@ -88,6 +174,7 @@ class FusedAdam:
         self.m = torch.zeros_like(flat.flat)
         self.v = torch.zeros_like(flat.flat)
         self.t = 0
+        flat._optimizers.append(weakref.ref(self))
 
     @property
     def device(self):
@@ -96,8 +183,15 @@ class FusedAdam:
     def zero_grad(self, set_to_none=False):
         self.fp.zero_grad()
 
+    def _check_layout(self):
+        # m and v must cover the flat buffer: the kernel runs over fp.numel floats of each
+        if self.m.numel() != self.fp.numel or self.v.numel() != self.fp.numel:
+            raise _lib.PertGnnError(f"{type(self).__name__}.step: m / v hold {self.m.numel()} / {self.v.numel()} floats "
+                                    f"but the FlatParams {self.fp.numel}")
+
     @_lib.on_device_of
     def step(self, grad_scale=1.0):
+        self._check_layout()
         self.t += 1
         _lib.call("pert_adam_step", _lib.ptr(self.fp.flat), _lib.ptr(self.fp.grad), _lib.ptr(self.m),
                   _lib.ptr(self.v), self.fp.numel, self.lr, self.betas[0], self.betas[1], self.eps, self.wd, self.t,
@@ -178,6 +272,7 @@ class PeerAdam(FusedAdam):
     def step(self, grad_scale=1.0):
         if self.world == 1:
             return super().step(grad_scale)
+        self._check_layout()
         self.t += 1
         _lib.call("pert_allreduce_adam", _lib.ptr(self.fp.flat), _lib.ptr(self.fp.grad), _lib.ptr(self.m),
                   _lib.ptr(self.v), self.fp.numel, self.lr, self.betas[0], self.betas[1], self.eps, self.wd, self.t,
@@ -257,6 +352,102 @@ class DataParallel:
         for g in gs:
             g.copy_(flat[o:o + g.numel()].view_as(g))
             o += g.numel()
+
+
+GROWN_TABLES = ("cat", "entry", "interface", "rpctype")
+
+
+def _tables(model):
+    return dict(zip(GROWN_TABLES, (model.cat_embedding[0], model.entry_embeds, model.interface_embeds,
+                                   model.rpctype_embeds)))
+
+
+def grow_embeddings(model, optimizer=None, store=None, *, entry=None, interface=None, rpctype=None, cat=None,
+                    seed=None):
+    """Appends rows to the embedding tables of a trained ``SAGEDeterministic`` so that it covers the ids a live
+    ``PatternStore`` has gained (``append_traces``), keeping every trained value and the optimizer state.  Returns the
+    row counts {"cat", "entry", "interface", "rpctype"} after the call; "cat" is ``cat_embedding[0]``, the microservice
+    table that ``cat_X`` column 0 indexes.
+
+    The target of each table is the largest of its current rows, the explicit argument and, with ``store``, the
+    store's ``id_bounds()``.  An explicit count below the current one is refused: tables never shrink.  When no table
+    grows, nothing is touched (no relayout; the engine and every captured graph stay).
+
+    New rows are drawn N(0, 1), as ``nn.Embedding`` initialises them, table by table in the order above, from
+    ``torch.Generator(device).manual_seed(seed)`` when ``seed`` is given, else from torch's default generator of the
+    device: data-parallel replicas given one seed grow identically, with no collective (as ``seed_dropout``).
+
+    The parameters move through ``FlatParams.grow`` (one relayout launch, ``pert_flat_grow``): the ``FlatParams`` of
+    ``optimizer`` (``FusedAdam``), else the one registered on the model (a new one if none holds it).  Optimizer state:
+    the m and v of the ``FusedAdam`` over that ``FlatParams`` are relaid by the same launch -- also when ``optimizer``
+    is omitted, as the FlatParams knows its optimizer -- with m = v = 0 in the new rows, and its step count stays.
+    That is the state of a row present from the start that never received a gradient; with weight_decay = 0 Adam
+    leaves such a row bit-unchanged (its update is 0 / (0 + eps)) until a batch uses it.  A ``torch.optim`` optimizer
+    (the drop-in loop) gets every state tensor of a grown table padded with zero rows (Adam's exp_avg, exp_avg_sq),
+    ``step`` kept.  ``PeerAdam`` over more than one rank is refused: its m and v cover the rank's own slice and its
+    exchange buffers are mapped into the other processes.
+
+    ``num_embeddings`` follows on the modules, so ``state_dict`` has the grown shapes and loads into a model built at
+    them.  The step engine is dropped and built again on next use (its descriptor carries the row counts and the
+    offsets); the BatchNorm running statistics, ``num_batches_tracked`` and the dropout counter carry over.  Every
+    captured graph (``GraphedTrainStep``, ``BucketedTrainStep``, ``evaluate_bucketed``, ``predict``) was captured over
+    the old engine and is captured again on its next visit (``_GraphCache.invalidations``).  Refused during CUDA-graph
+    capture and for a model that is not on a CUDA device."""
+    if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+        raise _lib.PertGnnError("grow_embeddings cannot run during CUDA-graph capture")
+    if isinstance(optimizer, PeerAdam) and optimizer.world > 1:
+        raise _lib.PertGnnError("grow_embeddings: PeerAdam over more than one rank keeps m and v for its own slice "
+                                "only and maps its exchange buffers across processes; growing it is not supported")
+    if optimizer is not None and not isinstance(optimizer, (FusedAdam, torch.optim.Optimizer)):
+        raise _lib.PertGnnError(f"grow_embeddings: unsupported optimizer {type(optimizer).__name__}")
+    tables = _tables(model)
+    rows = {k: int(e.num_embeddings) for k, e in tables.items()}
+    want = dict(rows)
+    for k, v in zip(GROWN_TABLES, (cat, entry, interface, rpctype)):
+        if v is None:
+            continue
+        v = operator.index(v)
+        if v < rows[k]:
+            raise _lib.PertGnnError(f"grow_embeddings: {k} = {v} is below the table's {rows[k]} rows (tables never "
+                                    "shrink)")
+        want[k] = v
+    if store is not None:
+        for k, v in store.id_bounds().items():
+            want[k] = max(want[k], v)
+    if want == rows:
+        return want
+    if isinstance(optimizer, FusedAdam) and not optimizer.fp.owns(model):
+        raise _lib.PertGnnError("grow_embeddings: the optimizer's FlatParams does not hold this model's parameters")
+    if not model.entry_embeds.weight.is_cuda:
+        raise _lib.PertGnnError("grow_embeddings needs the model on a CUDA device (the relayout runs there)")
+    if isinstance(optimizer, FusedAdam):
+        fp = optimizer.fp
+    else:
+        reg = model.__dict__.get("_flat_params")
+        fp = reg if reg is not None and reg.owns(model) else FlatParams(model, bind_grads=False)
+    dev = fp.device
+    gen = None
+    if seed is not None:
+        gen = torch.Generator(dev)
+        gen.manual_seed(int(seed))
+    fresh = {k: torch.randn(want[k] - rows[k], e.embedding_dim, generator=gen, device=dev)
+             for k, e in tables.items() if want[k] > rows[k]}
+    grown = {id(tables[k].weight): (want[k],) + tuple(tables[k].weight.shape[1:]) for k in fresh}
+    shapes = [grown.get(id(p), tuple(p.shape)) for p in fp.params]
+    old_shapes = {k: tuple(tables[k].weight.shape) for k in fresh}
+    fp.grow(shapes)
+    with torch.no_grad():
+        for k, r in fresh.items():
+            tables[k].weight[rows[k]:].copy_(r)
+            tables[k].num_embeddings = want[k]
+    if isinstance(optimizer, torch.optim.Optimizer):
+        for k in fresh:
+            st = optimizer.state.get(tables[k].weight)
+            for name, s in (st or {}).items():
+                if torch.is_tensor(s) and tuple(s.shape) == old_shapes[k]:
+                    st[name] = torch.cat([s, s.new_zeros((want[k] - rows[k],) + old_shapes[k][1:])])
+    model.reset_engine()
+    return want
 
 
 def train_step(model, optimizer, data, tau=0.5, dp: DataParallel | None = None):

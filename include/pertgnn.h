@@ -282,7 +282,9 @@ int pert_pool_bwd(const float* dpool, const float* dlocal, const float* x, int l
 int pert_relu_bwd(const float* y, float* dy, long long n, void* stream);
 
 /* Pinball loss (pert_gnn.py:191-193): loss[0] = mean(max(tau*e,(tau-1)*e)), e = y - yhat;
- * dyhat[B] = grad_scale * dloss/dyhat (either output may be NULL). */
+ * dyhat[B] = grad_scale * dloss/dyhat (either output may be NULL); a tie (e = 0) gets torch.maximum's even split,
+ * grad_scale * 0.5 * (1 - 2 tau) / B.  B is at most INT_MAX: a larger B is PERT_ERR_BADARG before any launch, as it
+ * is for the other three loss and metric entries below. */
 int pert_pinball_loss(const int64_t* y, const float* yhat, float tau, long long B, float grad_scale, float* loss,
                       float* dyhat, void* stream);
 
@@ -298,7 +300,9 @@ int pert_pinball_loss_live(const int64_t* y, const float* yhat, float tau, long 
 int pert_eval_metrics_live(const int64_t* y, const float* yhat, float tau, long long B, double* acc,
                            const long long* live, void* stream);
 
-/* torch.optim.Adam step (pert_gnn.py:343,247) over one flat parameter buffer; g is scaled by grad_scale. */
+/* torch.optim.Adam step (pert_gnn.py:343,247) over one flat parameter buffer; g is scaled by grad_scale, weight_decay
+ * is L2 added to the scaled gradient (not AdamW's decoupled decay).  The bias corrections lr / (1 - beta1^step) and
+ * sqrt(1 - beta2^step) are computed in double on the host, as torch does, and passed to the kernel as floats. */
 int pert_adam_step(float* p, const float* g, float* m, float* v, long long n, float lr, float beta1, float beta2,
                    float eps, float weight_decay, long long step, float grad_scale, void* stream);
 

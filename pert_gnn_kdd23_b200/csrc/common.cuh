@@ -1,6 +1,7 @@
 // Shared device/host helpers for libpertgnn (sm_90a: H100).
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 #include "../../include/pertgnn.h"  // prototypes + PERT_ERR_* (keeps definitions and ABI header in sync)
@@ -79,6 +80,30 @@ __device__ __forceinline__ float4 f4scale(float s, float4 a) {
 __device__ __forceinline__ void red4(float* p, float4 v) {
   atomicAdd(reinterpret_cast<float4*>(p), v);
 }
+// Host side of one torch.optim.Adam step t: step_size = lr / (1 - beta1^t) and bc2_sqrt = sqrt(1 - beta2^t), computed
+// in double as torch does and rounded once to float.  In float, 1 - beta^t cancels: at t = 2 the rounding of
+// powf(0.999f, 2) alone is up to 1.5e-5 of 1 - beta2^t.
+struct PertAdamScalars {
+  float step_size, bc2_sqrt;
+};
+static inline PertAdamScalars pert_adam_scalars(float lr, float beta1, float beta2, long long step) {
+  const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
+  return {(float)((double)lr / bc1), (float)sqrt(bc2)};
+}
+// One element of torch.optim.Adam (amsgrad = False, maximize = False): L2 weight decay added to the scaled gradient
+// (not AdamW's decoupled decay), m by lerp as torch's foreach path, then p -= step_size * m / (sqrt(v) / bc2_sqrt + eps).
+// k_adam and the vector bodies and scalar tails of both peer kernels (peer.cu) run this one function, every rounding
+// spelled out, so that they agree bit for bit whatever the compiler contracts around it.
+__device__ __forceinline__ void adam_elem(float g, float& p, float& m, float& v, float grad_scale, float wd, float b1,
+                                          float b2, float eps, float step_size, float bc2_sqrt) {
+  float gi = __fmul_rn(g, grad_scale);
+  if (wd != 0.f) gi = fmaf(wd, p, gi);
+  m = fmaf(__fsub_rn(gi, m), __fsub_rn(1.f, b1), m);
+  v = fmaf(__fmul_rn(__fsub_rn(1.f, b2), gi), gi, __fmul_rn(b2, v));
+  const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), eps);
+  p = fmaf(-step_size, __fdiv_rn(m, denom), p);
+}
+
 // butterfly sum over a sub-warp group of LPR lanes; every lane of the group gets the sum.
 template <int LPR>
 __device__ __forceinline__ float group_sum(float v, unsigned gmask) {

@@ -6,6 +6,7 @@
 //   pinball loss, Adam                       pert_gnn.py:191-193,245-247
 #include "common.cuh"
 #include "bn.cuh"
+#include <limits.h>
 #include <type_traits>
 
 namespace {
@@ -442,7 +443,7 @@ __global__ void k_pinball(const int64_t* __restrict__ y, const float* __restrict
   __shared__ float red[32];
   const int Bl = live ? (int)min((long long)B, live[1]) : B;
   float s = 0.f;
-  for (int i = threadIdx.x; i < B; i += blockDim.x) {
+  for (long long i = threadIdx.x; i < B; i += blockDim.x) {   // 64-bit: i + 256 passes INT_MAX at B near it
     if (i >= Bl) {
       if (dyhat) dyhat[i] = 0.f;
       continue;
@@ -466,21 +467,17 @@ __global__ void k_pinball(const int64_t* __restrict__ y, const float* __restrict
   }
 }
 
-// torch.optim.Adam (amsgrad=False, maximize=False) over one flat buffer
+// torch.optim.Adam over one flat buffer (adam_elem, common.cuh)
 __global__ void k_adam(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                       float* __restrict__ v, long long n, float lr, float b1, float b2, float eps, float wd,
-                       float bc1, float bc2_sqrt, float grad_scale) {
+                       float* __restrict__ v, long long n, float b1, float b2, float eps, float wd, float step_size,
+                       float bc2_sqrt, float grad_scale) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  float gi = g[i] * grad_scale;
-  float pi = p[i];
-  if (wd != 0.f) gi = fmaf(wd, pi, gi);
-  float mi = m[i] + (1.f - b1) * (gi - m[i]);             // lerp, as torch's foreach path
-  float vi = b2 * v[i] + (1.f - b2) * gi * gi;
+  float pi = p[i], mi = m[i], vi = v[i];
+  adam_elem(g[i], pi, mi, vi, grad_scale, wd, b1, b2, eps, step_size, bc2_sqrt);
   m[i] = mi;
   v[i] = vi;
-  float denom = sqrtf(vi) / bc2_sqrt + eps;
-  p[i] = pi - (lr / bc1) * (mi / denom);
+  p[i] = pi;
 }
 
 inline bool al16(const void* p) { return p == nullptr || ((uintptr_t)p & 15) == 0; }
@@ -494,7 +491,7 @@ __global__ void __launch_bounds__(256) k_eval_metrics(const int64_t* __restrict_
                                                       const long long* __restrict__ live) {
   if (live) B = (int)min((long long)B, live[1]);   // padded batch: the real graphs only
   double mae = 0.0, mape = 0.0, q = 0.0;
-  for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < B; b += gridDim.x * blockDim.x) {
+  for (long long b = blockIdx.x * blockDim.x + threadIdx.x; b < B; b += gridDim.x * blockDim.x) {
     const float yt = (float)y[b];                 // y.float() / int64 -> float32 promotion of the reference
     const float e = yt - yhat[b];
     const float ae = fabsf(yhat[b] - yt);
@@ -752,7 +749,7 @@ int pert_pinball_loss(const int64_t* y, const float* yhat, float tau, long long 
 
 int pert_pinball_loss_live(const int64_t* y, const float* yhat, float tau, long long B, float grad_scale, float* loss,
                            float* dyhat, const long long* live, void* stream) {
-  if (B <= 0 || !y || !yhat) return PERT_ERR_BADARG;
+  if (B <= 0 || B > INT_MAX || !y || !yhat) return PERT_ERR_BADARG;
   k_pinball<<<1, 256, 0, (cudaStream_t)stream>>>(y, yhat, tau, (int)B, grad_scale, loss, dyhat, live);
   PERT_LAUNCH_CHECK();
   return PERT_OK;
@@ -762,10 +759,9 @@ int pert_adam_step(float* p, const float* g, float* m, float* v, long long n, fl
                    float eps, float weight_decay, long long step, float grad_scale, void* stream) {
   if (n < 0 || step < 1 || !p || !g || !m || !v) return PERT_ERR_BADARG;
   if (n == 0) return PERT_OK;
-  float bc1 = 1.f - powf(beta1, (float)step);
-  float bc2 = 1.f - powf(beta2, (float)step);
-  k_adam<<<pert_cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(p, g, m, v, n, lr, beta1, beta2, eps, weight_decay,
-                                                             bc1, sqrtf(bc2), grad_scale);
+  const PertAdamScalars s = pert_adam_scalars(lr, beta1, beta2, step);
+  k_adam<<<pert_cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(p, g, m, v, n, beta1, beta2, eps, weight_decay,
+                                                             s.step_size, s.bc2_sqrt, grad_scale);
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }
@@ -776,7 +772,7 @@ int pert_eval_metrics(const int64_t* y, const float* yhat, float tau, long long 
 
 int pert_eval_metrics_live(const int64_t* y, const float* yhat, float tau, long long B, double* acc,
                            const long long* live, void* stream) {
-  if (B < 0 || !y || !yhat || !acc) return PERT_ERR_BADARG;
+  if (B < 0 || B > INT_MAX || !y || !yhat || !acc) return PERT_ERR_BADARG;
   if (B == 0) return PERT_OK;
   int grid = pert_cdiv(B, 256);
   if (grid > 64) grid = 64;

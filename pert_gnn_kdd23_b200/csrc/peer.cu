@@ -40,7 +40,7 @@ struct PeerArgs {
   float* m;
   float* v;
   long long n, n_al;
-  float lr, b1, b2, eps, wd, bc1, bc2_sqrt, grad_scale;
+  float step_size, b1, b2, eps, wd, bc2_sqrt, grad_scale;   // pert_adam_scalars, common.cuh
   float* xbuf[PEER_MAX];
   int rank, world;
   unsigned long long step;     // 1, 2, 3, ... (same on every rank)
@@ -122,13 +122,8 @@ __global__ void __launch_bounds__(256) k_allreduce_adam(PeerArgs a) {
     float gs[4] = {s.x, s.y, s.z, s.w}, pp[4] = {pv.x, pv.y, pv.z, pv.w}, mm[4] = {mv.x, mv.y, mv.z, mv.w},
           vs[4] = {vv.x, vv.y, vv.z, vv.w};
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      float gi = gs[k] * a.grad_scale;
-      if (a.wd != 0.f) gi = fmaf(a.wd, pp[k], gi);
-      mm[k] = mm[k] + (1.f - a.b1) * (gi - mm[k]);
-      vs[k] = a.b2 * vs[k] + (1.f - a.b2) * gi * gi;
-      pp[k] = pp[k] - (a.lr / a.bc1) * (mm[k] / (sqrtf(vs[k]) / a.bc2_sqrt + a.eps));
-    }
+    for (int k = 0; k < 4; ++k)
+      adam_elem(gs[k], pp[k], mm[k], vs[k], a.grad_scale, a.wd, a.b1, a.b2, a.eps, a.step_size, a.bc2_sqrt);
     st4(a.p + i * 4, make_float4(pp[0], pp[1], pp[2], pp[3]));
     st4(a.m + i * 4, make_float4(mm[0], mm[1], mm[2], mm[3]));
     st4(a.v + i * 4, make_float4(vs[0], vs[1], vs[2], vs[3]));
@@ -136,14 +131,11 @@ __global__ void __launch_bounds__(256) k_allreduce_adam(PeerArgs a) {
   for (long long i = (n4 << 2) + t0; i < a.n; i += stride) {
     float s = 0.f;
     for (int r = 0; r < a.world; ++r) s += __ldcv(a.xbuf[r] + off + i);
-    float gi = s * a.grad_scale;
-    const float pi = a.p[i];
-    if (a.wd != 0.f) gi = fmaf(a.wd, pi, gi);
-    const float mi = a.m[i] + (1.f - a.b1) * (gi - a.m[i]);
-    const float vi = a.b2 * a.v[i] + (1.f - a.b2) * gi * gi;
+    float pi = a.p[i], mi = a.m[i], vi = a.v[i];
+    adam_elem(s, pi, mi, vi, a.grad_scale, a.wd, a.b1, a.b2, a.eps, a.step_size, a.bc2_sqrt);
     a.m[i] = mi;
     a.v[i] = vi;
-    a.p[i] = pi - (a.lr / a.bc1) * (mi / (sqrtf(vi) / a.bc2_sqrt + a.eps));
+    a.p[i] = pi;
   }
   if (stamp) {   // phase times of CTA 0 (publish incl. the grid arrival; wait = slowest rank's skew + flag latency)
     const long long ts3 = gtime_ns();
@@ -158,13 +150,8 @@ __device__ __forceinline__ void adam4(const PeerArgs& a, float4 s, float4& pv, f
   float gs[4] = {s.x, s.y, s.z, s.w}, pp[4] = {pv.x, pv.y, pv.z, pv.w}, mm[4] = {mv.x, mv.y, mv.z, mv.w},
         vs[4] = {vv.x, vv.y, vv.z, vv.w};
 #pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    float gi = gs[k] * a.grad_scale;
-    if (a.wd != 0.f) gi = fmaf(a.wd, pp[k], gi);
-    mm[k] = mm[k] + (1.f - a.b1) * (gi - mm[k]);
-    vs[k] = a.b2 * vs[k] + (1.f - a.b2) * gi * gi;
-    pp[k] = pp[k] - (a.lr / a.bc1) * (mm[k] / (sqrtf(vs[k]) / a.bc2_sqrt + a.eps));
-  }
+  for (int k = 0; k < 4; ++k)
+    adam_elem(gs[k], pp[k], mm[k], vs[k], a.grad_scale, a.wd, a.b1, a.b2, a.eps, a.step_size, a.bc2_sqrt);
   pv = make_float4(pp[0], pp[1], pp[2], pp[3]);
   mv = make_float4(mm[0], mm[1], mm[2], mm[3]);
   vv = make_float4(vs[0], vs[1], vs[2], vs[3]);
@@ -242,17 +229,13 @@ __global__ void __launch_bounds__(256) k_reduce_scatter_adam(PeerArgs a) {
     for (long long i = (n4 << 2) + t0; i < a.n; i += stride) {
       float s = 0.f;
       for (int r = 0; r < a.world; ++r) s += __ldcv(a.xbuf[r] + i);
-      float gi = s * a.grad_scale;
-      const float pi = a.p[i];
-      if (a.wd != 0.f) gi = fmaf(a.wd, pi, gi);
-      const float mi = a.m[i] + (1.f - a.b1) * (gi - a.m[i]);
-      const float vi = a.b2 * a.v[i] + (1.f - a.b2) * gi * gi;
-      const float pn = pi - (a.lr / a.bc1) * (mi / (sqrtf(vi) / a.bc2_sqrt + a.eps));
+      float pi = a.p[i], mi = a.m[i], vi = a.v[i];
+      adam_elem(s, pi, mi, vi, a.grad_scale, a.wd, a.b1, a.b2, a.eps, a.step_size, a.bc2_sqrt);
       a.m[i] = mi;
       a.v[i] = vi;
-      a.p[i] = pn;
+      a.p[i] = pi;
       for (int r = 0; r < a.world; ++r)
-        if (r != a.rank) a.xbuf[r][a.n_al + i] = pn;
+        if (r != a.rank) a.xbuf[r][a.n_al + i] = pi;
     }
   }
   // ---- 4. this rank's slice has landed everywhere
@@ -330,9 +313,9 @@ int pert_allreduce_adam(float* p, const float* g, float* m, float* v, long long 
   if (n == 0) return PERT_OK;
   PeerArgs a;
   a.p = p; a.g = g; a.m = m; a.v = v; a.n = n; a.n_al = al64(n);
-  a.lr = lr; a.b1 = beta1; a.b2 = beta2; a.eps = eps; a.wd = weight_decay;
-  a.bc1 = 1.f - powf(beta1, (float)step);
-  a.bc2_sqrt = sqrtf(1.f - powf(beta2, (float)step));
+  const PertAdamScalars sc = pert_adam_scalars(lr, beta1, beta2, step);
+  a.step_size = sc.step_size; a.b1 = beta1; a.b2 = beta2; a.eps = eps; a.wd = weight_decay;
+  a.bc2_sqrt = sc.bc2_sqrt;
   a.grad_scale = grad_scale;
   for (int r = 0; r < PEER_MAX; ++r) a.xbuf[r] = r < world ? (float*)xbufs[r] : nullptr;
   for (int r = 0; r < world; ++r)

@@ -322,9 +322,16 @@ struct TconvBwdSrcArgs {
   int N;
 };
 
+// Interface id 0 is what the reference writes on every chain and return edge of a PERT graph (3 of 4 edges).  Its
+// table-gradient row is summed per thread, then per CTA, then added once per CTA, as the staged kernels do
+// (tconv_tile.cu, hot_if): per-edge atomics into that one row would chain ~E fp32 additions of mixed-sign terms whose
+// sum cancels ~100-fold, and serialise every edge on one address.
+constexpr int HOT_IF = 0;
+
 template <int LPR, int VPL, bool SMEM_RPC>
 __device__ __forceinline__ void edge_table_grad(const TconvBwdSrcArgs& a, float* s_rpc, float al, float ds,
-                                                const Row<VPL>& gi, const Row<VPL>& qi, int ia, int ib, int lig) {
+                                                const Row<VPL>& gi, const Row<VPL>& qi, int ia, int ib, int lig,
+                                                Row<VPL>& hot) {
   constexpr int H = 4 * LPR * VPL;
   Row<VPL> de = row_zero<VPL>();
   row_fma(al, gi, de);
@@ -332,7 +339,8 @@ __device__ __forceinline__ void edge_table_grad(const TconvBwdSrcArgs& a, float*
   float* pif = a.dt_if + (size_t)ia * H + lig * 4;
 #pragma unroll
   for (int u = 0; u < VPL; ++u) {
-    red4(pif + u * LPR * 4, de.v[u]);
+    if (ia == HOT_IF) hot.v[u] = f4add(hot.v[u], de.v[u]);
+    else red4(pif + u * LPR * 4, de.v[u]);
     if (SMEM_RPC) {
       float* ps = s_rpc + ib * H + lig * 4 + u * LPR * 4;
       atomicAdd(ps + 0, de.v[u].x);
@@ -351,11 +359,15 @@ __global__ void __launch_bounds__(256) k_tconv_bwd_src(TconvBwdSrcArgs a) {
   constexpr int H = 4 * LPR * VPL;
   constexpr int GPW = 32 / LPR;
   extern __shared__ float s_rpc[];
+  __shared__ float s_hot[H];
   const bool has_e = a.dt_if != nullptr;
-  if (SMEM_RPC && has_e) {
-    for (int x = threadIdx.x; x < a.n_rpc * H; x += blockDim.x) s_rpc[x] = 0.f;
+  if (has_e) {
+    for (int x = threadIdx.x; x < H; x += blockDim.x) s_hot[x] = 0.f;
+    if (SMEM_RPC)
+      for (int x = threadIdx.x; x < a.n_rpc * H; x += blockDim.x) s_rpc[x] = 0.f;
     __syncthreads();
   }
+  Row<VPL> hot = row_zero<VPL>();   // this thread's part of table-gradient row HOT_IF
   const int lane = threadIdx.x & 31;
   const int lig = lane % LPR;
   const int grp = lane / LPR;
@@ -392,18 +404,31 @@ __global__ void __launch_bounds__(256) k_tconv_bwd_src(TconvBwdSrcArgs a) {
         row_fma(ds[x], qi[x], dk);
         row_fma(al[x], gi[x], dv);
         if (has_e && x < deg)
-          edge_table_grad<LPR, VPL, SMEM_RPC>(a, s_rpc, al[x], ds[x], gi[x], qi[x], ia[x], ib[x], lig);
+          edge_table_grad<LPR, VPL, SMEM_RPC>(a, s_rpc, al[x], ds[x], gi[x], qi[x], ia[x], ib[x], lig, hot);
       }
     }
     store_row<LPR, VPL>(a.dk, a.ld_d, j, lig, dk);
     store_row<LPR, VPL>(a.dv, a.ld_d, j, lig, dv);
   }
-  if (SMEM_RPC && has_e) {
-    __syncthreads();
-    for (int x = threadIdx.x; x < a.n_rpc * H; x += blockDim.x) {
-      float v = s_rpc[x];
-      if (v != 0.f) atomicAdd(a.dt_rpc + x, v);
+  if (has_e) {
+#pragma unroll
+    for (int u = 0; u < VPL; ++u) {
+      float* hp = s_hot + lig * 4 + u * LPR * 4;
+      if (hot.v[u].x != 0.f) atomicAdd(hp + 0, hot.v[u].x);
+      if (hot.v[u].y != 0.f) atomicAdd(hp + 1, hot.v[u].y);
+      if (hot.v[u].z != 0.f) atomicAdd(hp + 2, hot.v[u].z);
+      if (hot.v[u].w != 0.f) atomicAdd(hp + 3, hot.v[u].w);
     }
+    __syncthreads();
+    for (int x = threadIdx.x; x < H; x += blockDim.x) {
+      const float v = s_hot[x];
+      if (v != 0.f) atomicAdd(a.dt_if + (size_t)HOT_IF * H + x, v);
+    }
+    if (SMEM_RPC)
+      for (int x = threadIdx.x; x < a.n_rpc * H; x += blockDim.x) {
+        float v = s_rpc[x];
+        if (v != 0.f) atomicAdd(a.dt_rpc + x, v);
+      }
   }
 }
 

@@ -395,7 +395,17 @@ long long pert_model_packed_bytes(const PertModelDesc* desc);
 /* Test / debug aid: offset (in floats) inside the workspace of a saved activation of the last forward:
  * which = 0: input of conv `layer` (>= 1) = post-BatchNorm-ReLU activations [N,Hp]; which = 1: relu(global_linear1)
  * [B,Hp] (Hp = pert_model_width(H); columns [H, Hp) are 0).
- * Lets a reference be differentiated on the same linear piece of the network (which ReLUs were active). */
+ * Lets a reference be differentiated on the same linear piece of the network (which ReLUs were active).
+ * The engine's own intermediates, so that each of its kernels can be checked on its own inputs:
+ *   which = 2: z = [pool | entry_embeds[entry_id]] [B,2Hp], the global head's input (valid after a forward);
+ *   which = 3: dpool [B,Hp], the head's gradient with respect to pool (valid after a backward);
+ *   which = 4 / 5: t_if / t_rpc of conv `layer` [n_if / n_rpc, Hp] = interface / rpc embeddings . lin_edge half^T
+ *                  (forward);
+ *   which = 6 / 7: their gradients dt_if / dt_rpc, same shapes (backward);
+ *   which = 8..11: the packed gradients of conv `layer` before they are added into the flat gradient buffer (backward):
+ *                  dW4 [4Hp,K] (rows q|k|v|skip, K = k0 for conv 0 with columns [emb | x | pad], else Hp), db4 [4Hp],
+ *                  and the two lin_edge halves dWeA / dWeB [Hp,Hp] (row = output feature).
+ * which 4..11 need 0 <= layer < n_convs, else PERT_ERR_BADARG; which 1..3 ignore `layer`. */
 long long pert_model_workspace_offset(const PertModelDesc* desc, long long N, long long E, long long B, int which,
                                       int layer);
 /* bn_running: [n_convs-1][2][Hp] (running_mean | running_var; the first H of each Hp are the model's, the others belong

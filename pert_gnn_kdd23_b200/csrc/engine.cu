@@ -671,7 +671,9 @@ long long pert_model_workspace_bytes(const PertModelDesc* d, long long N, long l
 }
 // Test / debug aid: where a saved activation lives inside the workspace (floats from its start): which = 0 -> the input of
 // conv `layer` >= 1, i.e. the post-BatchNorm-ReLU activations [N, H]; which = 1 -> the global head's hidden layer
-// relu(global_linear1(.)) [B, H].  Returns the offset or a negative PERT_ERR_*.
+// relu(global_linear1(.)) [B, H]; which = 2..11 -> the head's input z, its pool gradient, the edge tables of conv
+// `layer` and their gradients, and the packed gradients of conv `layer` (include/pertgnn.h).  Returns the offset or a
+// negative PERT_ERR_*.
 long long pert_model_workspace_offset(const PertModelDesc* d, long long N, long long E, long long B, int which,
                                       int layer) {
   if (check_desc(d) || N < 0 || E < 0 || B < 0) return PERT_ERR_BADARG;
@@ -679,7 +681,20 @@ long long pert_model_workspace_offset(const PertModelDesc* d, long long N, long 
   Ws w = carve(d, N, E, B, base);
   if (which == 0 && layer >= 1 && layer < d->n_convs) return w.x[layer] - base;
   if (which == 1) return w.h1 - base;
-  return PERT_ERR_BADARG;
+  if (which == 2) return w.z - base;
+  if (which == 3) return w.dpool - base;
+  if (layer < 0 || layer >= d->n_convs) return PERT_ERR_BADARG;
+  switch (which) {
+    case 4: return w.t_if[layer] - base;
+    case 5: return w.t_rpc[layer] - base;
+    case 6: return w.dt_if[layer] - base;
+    case 7: return w.dt_rpc[layer] - base;
+    case 8: return w.dw4[layer] - base;
+    case 9: return w.db4[layer] - base;
+    case 10: return w.dweA[layer] - base;
+    case 11: return w.dweB[layer] - base;
+    default: return PERT_ERR_BADARG;
+  }
 }
 int pert_model_width(int H) { return model_width(H); }
 long long pert_model_packed_bytes(const PertModelDesc* d) {

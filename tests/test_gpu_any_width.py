@@ -12,6 +12,7 @@ from oracle import model_oracle
 from oracle.model_oracle import OracleSAGEDeterministic, OracleTransformerConv
 from pert_gnn_kdd23_b200.synthetic import model_args
 from tests.dropout_ref import dropout_masks, oracle_forward
+from tests.engine_parts_ref import packed_pad_mask
 from tests.helpers import (RTOL, assert_close, assert_close_ref, assert_grads_close_ref, forward_args,
                            is_structural_zero_grad, make_batch)
 
@@ -214,39 +215,6 @@ def test_transformer_conv_shim(H):
             assert_close(prm.grad, pr[n].grad, rtol=2e-2 if norm else 1e-3, norm_only=norm, what=f"shim H={H} {n}")
 
 
-def _packed_pad_mask(eng):
-    """bool [pert_model_packed_bytes / 4]: True where the packed region holds padding (columns / rows [H, Hp), the
-    conv-0 pad columns, the 64-float alignment tails) -- a restatement of engine.cu:carve / append_*_segs."""
-    d, H, Hp, L = eng.desc, eng.desc.H, eng.Hp, eng.n_convs
-    F, k0 = d.F, d.k0
-    parts = []
-
-    def slot(shape, *real):
-        m = torch.ones(shape, dtype=torch.bool)
-        for idx in real:
-            m[idx] = False
-        n = m.numel()
-        parts.append(torch.cat([m.reshape(-1), torch.ones((max(n, 1) + 63) // 64 * 64 - n, dtype=torch.bool)]))
-
-    for l in range(L):
-        K = k0 if l == 0 else Hp
-        cols = [slice(0, H)] + ([slice(Hp, Hp + F)] if l == 0 else [])
-        slot((4, Hp, K), *[(slice(None), slice(0, H), c) for c in cols])          # W4
-        slot((4, Hp), (slice(None), slice(0, H)))                                 # b4
-        slot((K, 4, Hp), *[(c, slice(None), slice(0, H)) for c in cols])          # W4^T
-        for _ in range(4):                                                        # lin_edge halves (+ transposes)
-            slot((Hp, Hp), (slice(0, H), slice(0, H)))
-    if Hp != H:
-        for rows in list(d.cat_rows[:d.n_cat]) + [d.n_entry, d.n_if, d.n_rpc]:
-            slot((rows, Hp), (slice(None), slice(0, H)))
-        for _ in range(2 * (L - 1) + 1):                                         # BatchNorm gamma / beta, local_linear
-            slot((Hp,), slice(0, H))
-        slot((Hp, 2 * Hp), (slice(0, H), slice(0, H)), (slice(0, H), slice(Hp, Hp + H)))   # global_linear1
-        slot((Hp,), slice(0, H))
-        slot((Hp,), slice(0, H))
-    return torch.cat(parts)
-
-
 @pytest.mark.parametrize("H", [48, 200])
 def test_padding_never_leaks(H, tmp_path):
     """20 FusedAdam steps in lockstep with the oracle trained by torch.optim.Adam; the padding slots of the packed
@@ -289,7 +257,7 @@ def test_padding_never_leaks(H, tmp_path):
     # the packed region (refreshed by that forward) is zero exactly where it holds padding
     eng = model._engine
     n_packed = eng.lib.pert_model_packed_bytes(ctypes.byref(eng.desc)) // 4
-    pad = _packed_pad_mask(eng)
+    pad = packed_pad_mask(eng.desc, eng.Hp, eng.n_convs, eng.fp.flat.numel())
     assert pad.numel() == n_packed
     packed = eng.ws[:n_packed].cpu()
     assert int((packed[pad] != 0).sum()) == 0, f"H={H}: padding slots of the packed parameters are not 0"

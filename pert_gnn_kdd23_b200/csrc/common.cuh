@@ -29,6 +29,64 @@ static inline int pert_num_sms() {
 
 static inline int pert_cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// ---- programmatic dependent launch (sm_90).  A kernel launched through launch_pdl may start while its predecessor in
+// the stream (or captured graph) is still draining, and runs its set-up (weight staging, index staging, barrier init)
+// before pdl_wait(), which returns once the predecessor has completed and its memory is visible.  Ordering rule, for
+// every kernel launched this way:
+//   - it calls pdl_wait() on every path that touches data its predecessor writes, and pdl_trigger() only after
+//     pdl_wait(), so that kernel n's set-up can start only once kernel n - 2 has completed;
+//   - before pdl_wait() it reads only data written by kernel n - 2 or earlier (packed parameters, the graph index, edge
+//     tables, forward activations in the backward) and writes no global memory at all: no read-after-write and no
+//     write-after-read race with kernel n - 1;
+//   - where unsure, pdl_wait() is its first statement.
+// The step engine launches its conv chain this way (node-linear forward, conv forward, conv backward target and source
+// passes, node-linear backward), so each kernel's set-up overlaps its predecessor's drain and launch.
+// tests/test_pdl_contract.py checks the textual form of these rules over csrc/*.cu.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+// The attribute is set only while the step engine issues its chain (PdlChain, engine.cu), where every predecessor is
+// known.  Called on its own, a kernel keeps plain stream order: the caller's last kernel may have written what its
+// set-up reads.  (griddepcontrol.wait returns at once in a kernel launched without the attribute.)
+inline thread_local bool pert_pdl_chain = false;
+struct PdlChain {
+  bool prev;
+  explicit PdlChain(bool on) : prev(pert_pdl_chain) { pert_pdl_chain = on; }
+  ~PdlChain() { pert_pdl_chain = prev; }
+};
+
+// cudaLaunchKernelEx with programmatic stream serialisation (inside a PdlChain), and with a (cluster_x, 1, 1) cluster
+// when cluster_x > 0.
+template <typename... KArgs, typename... Args>
+static inline cudaError_t launch_pdl_cluster(int cluster_x, void (*kernel)(KArgs...), dim3 grid, dim3 block,
+                                             size_t smem, cudaStream_t st, Args... args) {
+  cudaLaunchAttribute attr[2];
+  int n = 0;
+  if (pert_pdl_chain) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if (cluster_x > 0) {
+    attr[n].id = cudaLaunchAttributeClusterDimension;
+    attr[n].val.clusterDim.x = cluster_x;
+    attr[n].val.clusterDim.y = 1;
+    attr[n++].val.clusterDim.z = 1;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = n;
+  return cudaLaunchKernelEx(&cfg, kernel, ((KArgs)args)...);
+}
+template <typename... KArgs, typename... Args>
+static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                                     Args... args) {
+  return launch_pdl_cluster(0, kernel, grid, block, smem, st, args...);
+}
+
 // Time bucket of a timestamp (ms): floor(ts / 30000) * 30000 with floor division (pandas //), so -1 -> -30000
 // (preprocess.py:39 get_tr2ts_map).  The trace grouping labels traces with it; request assembly joins resources on it.
 constexpr int64_t TG_BUCKET = 30000;

@@ -419,6 +419,10 @@ struct Ws {
   // backward temporaries
   float *dplanes, *dx, *dsp, *rpc_ws, *sums, *dpool, *dzent, *dh1;
   long long* drop_ctr;  // {seed, step} of the last training forward with dropout (k_pack -> BatchNorm applies)
+  // [2H] fp64 BatchNorm sums of conv l's output, filled by its epilogue and read by the node linear of conv l + 1: one
+  // per layer and contiguous, so that one memset at the start of a training forward clears all of them and no memset
+  // sits inside the conv chain (bn_part stays the scratch of statistics computed by their own pass)
+  double* bn_acc[PERT_MAX_CONVS];
   long long total;  // floats
   long long packed_floats;
 };
@@ -509,6 +513,11 @@ Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* b
   w.dzent = take(B * H);
   w.dh1 = take(B * H);
   w.drop_ctr = (long long*)take(4);
+  {
+    const long long per = pert_bn_workspace_bytes(N, H) / 8;   // doubles, each a whole BatchNorm workspace
+    double* acc = (double*)take(2 * per * (L - 1));
+    for (int l = 0; l + 1 < L; ++l) w.bn_acc[l] = acc ? acc + per * l : nullptr;
+  }
   w.total = off;
   return w;
 }
@@ -736,6 +745,14 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
   if (workspace_bytes < w.total * 4) return PERT_ERR_BADARG;
   cudaStream_t st = (cudaStream_t)stream;
   const int H = w.Hp, L = d->n_convs;
+  // The conv chain's kernels overlap their set-up with their predecessors (common.cuh) where the node linear is the
+  // fused H = 64 kernel; around the GEMMs of the other widths the tile kernels issue their plane copies first instead.
+  const bool bn_in_linear = pert_bn_linear_fwd_planes_supported(N, H, H) == 1;
+  const PdlChain pdl_chain(bn_in_linear);
+  if (training) {             // the fused BatchNorm sums of every layer, before the chain
+    cudaError_t me = cudaMemsetAsync(w.bn_acc[0], 0, (size_t)pert_bn_workspace_bytes(N, H) * (L - 1), st);
+    if (me != cudaSuccess) return (int)me;
+  }
   // Hp > H: the zero-padded copies of the embeddings, BatchNorm and head parameters first (the prologue reads them)
   const bool padded = H != d->H;
   const Tensors P = padded ? w.pp : flat_tensors(d, const_cast<float*>(params));
@@ -785,9 +802,7 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
   if (forked) TRY(aux_join(ax, st));
   // 3. conv stack.  Where the shape qualifies, the node linear of conv l >= 1 applies the BatchNorm(+ReLU, +dropout)
   // of conv l - 1 while it loads out[l - 1] and writes x[l] on the way (csrc/linear_fwd.cu): one launch and one pass
-  // instead of the apply pass followed by the GEMM.  It reads the BatchNorm sums of conv l - 1 before the memset of
-  // conv l below clears them.
-  const bool bn_in_linear = pert_bn_linear_fwd_planes_supported(N, H, H) == 1;
+  // instead of the apply pass followed by the GEMM.  It reads the BatchNorm sums of conv l - 1 from bn_acc[l - 1].
   int prev_stats_fused = 0;
   for (int l = 0; l < L; ++l) {
     const int K = k_of(d, w, l);
@@ -798,7 +813,8 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
       TRY(pert_bn_linear_fwd_planes_ex(w.out[l - 1], H, 1, P.bn_g[l - 1], P.bn_b[l - 1],
                                        rm, rv, (training && bn_nbt) ? bn_nbt + l - 1 : nullptr, d->bn_eps,
                                        d->bn_momentum, training, w.bn_stats[l - 1], w.bn_stats[l - 1] + H, w.x[l], H,
-                                       w.bn_part, pert_bn_workspace_bytes(N, H), prev_stats_fused,
+                                       prev_stats_fused ? (void*)w.bn_acc[l - 1] : (void*)w.bn_part,
+                                       pert_bn_workspace_bytes(N, H), prev_stats_fused,
                                        drop ? dropout : 0.f, w.drop_ctr, l - 1, live, w.w4[l], K, w.b4[l],
                                        w.planes[l], N * (long long)H, N, H, K, st));
     } else {
@@ -819,14 +835,10 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
       cudaError_t we = cudaStreamWaitEvent(st, (cudaEvent_t)index_ready, 0);
       if (we != cudaSuccess) return (int)we;
     }
-    // BatchNorm statistics of out[l] are produced by the conv kernel's epilogue (training, staged tile path)
+    // BatchNorm statistics of out[l] are produced by the conv kernel's epilogue (training, staged tile path) into
+    // bn_acc[l], cleared at the start of the forward
     int stats_fused = 0;
-    double* bn_acc = nullptr;
-    if (l + 1 < L && training) {
-      bn_acc = (double*)w.bn_part;
-      cudaError_t me = cudaMemsetAsync(bn_acc, 0, (size_t)2 * H * sizeof(double), st);
-      if (me != cudaSuccess) return (int)me;
-    }
+    double* bn_acc = (l + 1 < L && training) ? w.bn_acc[l] : nullptr;
     PROBE_START(1, l);
     TRY(pert_tconv_fwd_stats(pl, pl + N * H, pl + 2 * N * H, pl + 3 * N * H, H, rowptr, csr_src, csr_if, csr_rpc,
                              w.t_if[l], w.t_rpc[l], w.out[l], H, w.alpha[l], d->n_rpc, N, E, B, H, d->H, bn_acc, live,
@@ -838,7 +850,8 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
       float* rv = rm ? rm + H : nullptr;
       TRY(pert_bn_fwd_ex(w.out[l], H, P.bn_g[l], P.bn_b[l], rm, rv,
                          (training && bn_nbt) ? bn_nbt + l : nullptr, d->bn_eps, d->bn_momentum, training, 1,
-                         w.bn_stats[l], w.bn_stats[l] + H, w.x[l + 1], H, N, H, w.bn_part,
+                         w.bn_stats[l], w.bn_stats[l] + H, w.x[l + 1], H, N, H,
+                         stats_fused ? (void*)w.bn_acc[l] : (void*)w.bn_part,
                          pert_bn_workspace_bytes(N, H), stats_fused, drop ? dropout : 0.f, w.drop_ctr, l, live, st));
     }
   }
@@ -895,6 +908,7 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
   const bool padded = H != d->H;
   const Tensors P = padded ? w.pp : flat_tensors(d, const_cast<float*>(params));
   const Tensors G = padded ? w.pg : flat_tensors(d, grads);
+  const PdlChain pdl_chain(pert_linear_bwd_planes_supported(N, H, H, H) == 1);   // as in the forward
   cudaError_t e = cudaMemsetAsync(w.gzero_begin, 0, (size_t)(w.gzero_end - w.gzero_begin) * sizeof(float), st);
   if (e != cudaSuccess) return (int)e;
   // ---- global head backward

@@ -103,8 +103,9 @@ __global__ void __launch_bounds__(LB_THREADS, 1) k_linear_bwd_planes(LbArgs g) {
   if (tid == 0) {
     for (int s = 0; s < Lay::STAGES; ++s) mbar_init(&full[s], 1);
     fence_mbar_init();
-    for (int i = 0; i < Lay::STAGES && i < nt; ++i) issue(i);
   }
+  // Set-up before pdl_wait (common.cuh): W4^T comes from the parameter pack.  dY is the conv backward's output, so the
+  // ring is filled after the wait.
   // W4^T slice [KD, H] of this plane -> shared memory, split hi / lo, K permuted as in k_gemm_nt_wg (nt_logical_k)
   for (int i = tid; i < KD * LB_H; i += LB_THREADS) {
     const int n = i / LB_H, p = i - n * LB_H;
@@ -115,6 +116,10 @@ __global__ void __launch_bounds__(LB_THREADS, 1) k_linear_bwd_planes(LbArgs g) {
     *reinterpret_cast<uint32_t*>(smem + off) = h;
     *reinterpret_cast<uint32_t*>(smem + Lay::W_HALF + off) = tf32_lo(v, h);
   }
+  pdl_wait();
+  pdl_trigger();
+  if (tid == 0)
+    for (int i = 0; i < Lay::STAGES && i < nt; ++i) issue(i);
   fence_async_smem();
   __syncthreads();
 
@@ -375,13 +380,12 @@ int clusters_for(int K, int Kd) {
 
 template <int K, int KD>
 int launch(const LbArgs& a0, int clusters, cudaStream_t st) {
-  cudaLaunchAttribute attr[1];
-  cudaLaunchConfig_t cfg = cluster_config<K, KD>(attr, st);
   LbArgs a = a0;
   const int ntiles = (a.N + LB_TM - 1) / LB_TM;
   a.tiles_per_cluster = (ntiles + clusters - 1) / clusters;
-  cfg.gridDim = dim3(4 * ((ntiles + a.tiles_per_cluster - 1) / a.tiles_per_cluster));
-  cudaError_t e = cudaLaunchKernelEx(&cfg, k_linear_bwd_planes<K, KD>, a);
+  const dim3 grid(4 * ((ntiles + a.tiles_per_cluster - 1) / a.tiles_per_cluster));
+  const cudaError_t e =
+      launch_pdl_cluster(4, k_linear_bwd_planes<K, KD>, grid, LB_THREADS, LbLayout<K, KD>::SMEM, st, a);
   return e == cudaSuccess ? PERT_OK : (int)e;
 }
 

@@ -93,8 +93,9 @@ __global__ void __launch_bounds__(LF_THREADS, 1) k_bn_linear_fwd_planes(LfArgs g
   if (tid == 0) {
     for (int s = 0; s < Lay::STAGES; ++s) mbar_init(&full[s], 1);
     fence_mbar_init();
-    for (int i = 0; i < Lay::STAGES && i < nt; ++i) issue(i);
   }
+  // Set-up before pdl_wait (common.cuh): W4 / b4 come from the parameter pack and gamma / beta from the parameters, none
+  // of them written by the preceding conv.  A and the BatchNorm sums are its output and are read after the wait.
   // W4 [4H, K] -> shared memory, split hi / lo, K permuted (nt_logical_k).  K loads per thread, issued 16 at a time
   // before any is used: one at a time, the L2 latency of each would add up to most of the kernel's time.
   constexpr int WB = 16;
@@ -119,6 +120,15 @@ __global__ void __launch_bounds__(LF_THREADS, 1) k_bn_linear_fwd_planes(LfArgs g
   for (int c = tid; c < LF_NC; c += LF_THREADS) par[c] = __ldg(g.b4 + c);
   if (BN)
     for (int c = tid; c < LF_H; c += LF_THREADS) {
+      par[LF_NC + 2 * LF_H + c] = g.gamma[c];
+      par[LF_NC + 3 * LF_H + c] = g.beta[c];
+    }
+  pdl_wait();
+  pdl_trigger();
+  if (tid == 0)
+    for (int i = 0; i < Lay::STAGES && i < nt; ++i) issue(i);
+  if (BN)
+    for (int c = tid; c < LF_H; c += LF_THREADS) {
       float mu, rs;
       if (g.acc) {
         const long long n_stat = g.live ? g.live[0] : g.N;   // read here only, never in the tile loop
@@ -130,8 +140,6 @@ __global__ void __launch_bounds__(LF_THREADS, 1) k_bn_linear_fwd_planes(LfArgs g
       }
       par[LF_NC + c] = mu;
       par[LF_NC + LF_H + c] = rs;
-      par[LF_NC + 2 * LF_H + c] = g.gamma[c];
-      par[LF_NC + 3 * LF_H + c] = g.beta[c];
     }
   fence_async_smem();   // generic-proxy weight stores -> visible to the wgmmas
   __syncthreads();
@@ -238,9 +246,8 @@ int launch(const LfArgs& a, cudaStream_t st) {
   if (per_sm <= 0) return PERT_ERR_UNSUPPORTED;
   const int ntiles = (a.N + LF_TM - 1) / LF_TM;
   const int grid = min(ntiles, PERT_NUM_SMS * per_sm);
-  k_bn_linear_fwd_planes<K, MODE><<<grid, LF_THREADS, LfLayout<K>::SMEM, st>>>(a);
-  PERT_LAUNCH_CHECK();
-  return PERT_OK;
+  const cudaError_t e = launch_pdl(k_bn_linear_fwd_planes<K, MODE>, grid, LF_THREADS, LfLayout<K>::SMEM, st, a);
+  return e == cudaSuccess ? PERT_OK : (int)e;
 }
 
 inline bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }

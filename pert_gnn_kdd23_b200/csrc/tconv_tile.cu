@@ -79,6 +79,9 @@ struct TileArgs {
   int hot_if;          // interface id whose table-gradient row is accumulated per CTA instead of per edge (source pass)
   float inv_sqrt_c;
   PertBnBwd bn;        // bwd_dst with BN: the BatchNorm backward that yields g (include/pertgnn.h, pert_tconv_bwd_bn)
+  int pdl;             // launched as a dependent of a chain kernel (launch_pdl inside a PdlChain, common.cuh): the
+                       // index set-up runs before the plane copies, which wait for the predecessor.  Else the copies
+                       // are issued first and overlap the set-up.
   float* g_out;        // bwd_dst with BN: g rows, written (the plane `g` of the source pass)
 };
 
@@ -144,21 +147,14 @@ __device__ __forceinline__ void cta_tile(const TileArgs& a, int& n0, int& nt) {
   asm volatile("" : "+r"(n0), "+r"(nt));
 }
 
-// stage the two operand tiles + the node-pointer slice + the degree-sorted node order; returns after the pointers and
-// the order are visible (tiles: the caller's mbar_wait).  The mbarrier is initialised by the caller.
+// stage the node-pointer slice + the degree-sorted node order; returns after both are visible.  Reads the graph index
+// only, so it runs before pdl_wait (common.cuh).
 // Lane groups of a warp walk their nodes' edges in lockstep (trip count = the largest degree in the warp): handing the
 // nodes out in DESCENDING DEGREE order puts equal degrees side by side (no idle lockstep iterations: E[max of 2 degrees]
 // is 3.8 against a mean of 3.0 at cfg2) and starts the long rows first.  Counting sort over degrees clamped to 32.
-template <int H, int NT>
-__device__ __forceinline__ void stage_tiles(const Smem& S, const float* pa, const float* pb, const int* nodeptr,
-                                            int n0, int nt, int tid) {
+template <int NT>
+__device__ __forceinline__ void stage_index(const Smem& S, const int* nodeptr, int n0, int nt, int tid) {
   __shared__ int s_hist[34];
-  if (tid == 0) {
-    const uint32_t tile_bytes = (uint32_t)nt * H * 4;
-    mbar_expect_tx(S.bar, 2 * tile_bytes);
-    bulk_g2s(S.ta, pa + (size_t)n0 * H, tile_bytes, S.bar);
-    bulk_g2s(S.tb, pb + (size_t)n0 * H, tile_bytes, S.bar);
-  }
   if (tid < 34) s_hist[tid] = 0;
   for (int x = tid; x <= nt; x += NT) S.ptr[x] = __ldg(nodeptr + n0 + x);
   __syncthreads();
@@ -176,6 +172,17 @@ __device__ __forceinline__ void stage_tiles(const Smem& S, const float* pa, cons
   for (int x = tid; x < nt; x += NT)
     S.ord[atomicAdd(&s_hist[32 - min(S.ptr[x + 1] - S.ptr[x], 32)], 1)] = (unsigned short)x;
   __syncthreads();
+}
+// the two operand tiles (planes the preceding kernels wrote: after pdl_wait), completion on S.bar (the caller's
+// mbar_wait).  The mbarrier is initialised by the caller.
+template <int H>
+__device__ __forceinline__ void stage_tiles(const Smem& S, const float* pa, const float* pb, int n0, int nt, int tid) {
+  if (tid == 0) {
+    const uint32_t tile_bytes = (uint32_t)nt * H * 4;
+    mbar_expect_tx(S.bar, 2 * tile_bytes);
+    bulk_g2s(S.ta, pa + (size_t)n0 * H, tile_bytes, S.bar);
+    bulk_g2s(S.tb, pb + (size_t)n0 * H, tile_bytes, S.bar);
+  }
 }
 __device__ __forceinline__ void tile_barrier_init(const Smem& S, int tid) {
   if (tid == 0) {
@@ -257,7 +264,8 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
   cta_tile(a, n0, nt);
   if (nt <= 0) return;                         // uniform across the CTA
   tile_barrier_init(S, tid);
-  stage_tiles<H, NT>(S, a.k, a.v, a.rowptr, n0, nt, tid);
+  if (!a.pdl) stage_tiles<H>(S, a.k, a.v, n0, nt, tid);
+  stage_index<NT>(S, a.rowptr, n0, nt, tid);
   const int e_lo = S.ptr[0];
   const int ne_c = min(S.ptr[nt] - e_lo, a.edge_cap);
   int bad = 0, wide = 0;   // a staged neighbour outside this tile / staged ids that do not pack
@@ -278,6 +286,10 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
   const bool narrow = !(HAS_E && any && __syncthreads_or(wide));   // else every edge takes the global path
   const int ne_s = narrow ? ne_c : 0;
   const bool all_in = !any && (S.ptr[nt] - e_lo <= a.edge_cap);
+  // the set-up above read the graph index only; the planes are the node linear's output
+  pdl_wait();
+  pdl_trigger();
+  if (a.pdl) stage_tiles<H>(S, a.k, a.v, n0, nt, tid);
   mbar_wait(S.bar, 0);
 
   // node slots are handed out in descending-degree order (S.ord); the q row is requested one node ahead, the skip row
@@ -492,13 +504,9 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
   int n0, nt;
   cta_tile(a, n0, nt);
   if (nt <= 0) return;                         // uniform across the CTA
-  if (BN && blockIdx.x == 0)                   // parameter gradients accumulate (+=) like autograd
-    for (int c = tid; c < H; c += NT) {
-      a.bn.dbeta[c] += (float)a.bn.sums[c];
-      a.bn.dgamma[c] += (float)a.bn.sums[H + c];
-    }
   tile_barrier_init(S, tid);
-  stage_tiles<H, NT>(S, a.k, a.v, a.rowptr, n0, nt, tid);
+  stage_tiles<H>(S, a.k, a.v, n0, nt, tid);    // the forward's k and v planes: no need to wait for them
+  stage_index<NT>(S, a.rowptr, n0, nt, tid);
   const int e_lo = S.ptr[0];
   const int ne_c = min(S.ptr[nt] - e_lo, a.edge_cap);
   int bad = 0, wide = 0;   // a staged neighbour outside this tile / staged ids that do not pack
@@ -520,6 +528,15 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
   const bool narrow = !(HAS_E && any && __syncthreads_or(wide));   // else every edge takes the global path
   const int ne_s = narrow ? ne_c : 0;
   const bool all_in = !any && (S.ptr[nt] - e_lo <= a.edge_cap);
+  // the set-up above read the graph index and the forward's k, v and alpha; g (or dx and the BatchNorm sums) and the
+  // writes come after the wait
+  pdl_wait();
+  pdl_trigger();
+  if (BN && blockIdx.x == 0)                   // parameter gradients accumulate (+=) like autograd
+    for (int c = tid; c < H; c += NT) {
+      a.bn.dbeta[c] += (float)a.bn.sums[c];
+      a.bn.dgamma[c] += (float)a.bn.sums[H + c];
+    }
   mbar_wait(S.bar, 0);
 
   int slot = g0 + grp;
@@ -716,10 +733,12 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
   cta_tile(a, n0, nt);
   if (nt <= 0) return;                         // uniform across the CTA
   tile_barrier_init(S, tid);
-  stage_tiles<H, NT>(S, a.g, a.q, a.colptr, n0, nt, tid);   // targets of a node's out-edges live in the same graph
+  if (!a.pdl) stage_tiles<H>(S, a.g, a.q, n0, nt, tid);
+  stage_index<NT>(S, a.colptr, n0, nt, tid);   // targets of a node's out-edges live in the same graph
   const int c_lo = S.ptr[0];
   const int ne_c = min(S.ptr[nt] - c_lo, a.edge_cap);
-  // per out-edge (CSC order): target, and through the CSR slot its alpha, ds and attribute ids
+  // per out-edge (CSC order): target, and through the CSR slot its alpha, ds and attribute ids.  ds is the target
+  // pass's output: with pdl, f1 holds the CSR slot until the wait.
   int bad = 0, wide = 0;   // a staged neighbour outside this tile / staged ids that do not pack
   for (int x = tid; x < ne_c; x += NT) {
     const int p = __ldg(a.csc_pos + c_lo + x);
@@ -727,7 +746,7 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
     S.e0[x] = nb_id;
     bad |= (unsigned)(nb_id - n0) >= (unsigned)nt;
     S.f0[x] = __ldg(a.alpha + p);
-    S.f1[x] = __ldg(a.dsp + p);
+    S.f1[x] = a.pdl ? __int_as_float(p) : __ldg(a.dsp + p);
     if (HAS_E) {
       const int ia = __ldg(a.csr_if + p), ib = __ldg(a.csr_rpc + p);
       wide |= !packable(ia, ib);
@@ -741,6 +760,13 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
   const bool narrow = !(HAS_E && any && __syncthreads_or(wide));   // else every edge takes the global path
   const int ne_s = narrow ? ne_c : 0;
   const bool all_in = !any && (S.ptr[nt] - c_lo <= a.edge_cap);
+  pdl_wait();
+  pdl_trigger();
+  if (a.pdl) {
+    stage_tiles<H>(S, a.g, a.q, n0, nt, tid);
+    for (int x = tid; x < ne_c; x += NT) S.f1[x] = __ldg(a.dsp + __float_as_int(S.f1[x]));   // this thread's slots
+    __syncthreads();
+  }
   mbar_wait(S.bar, 0);
 
   auto run = [&](auto fast_c) {
@@ -916,8 +942,10 @@ template <typename K>
 int launch_k(K kernel, int grid, int threads, size_t bytes, const TileArgs& a, cudaStream_t st) {
   int rc = set_smem(kernel, bytes);
   if (rc) return rc;
-  kernel<<<grid, threads, bytes, st>>>(a);
-  return PERT_OK;
+  TileArgs b = a;
+  b.pdl = pert_pdl_chain;
+  const cudaError_t e = launch_pdl(kernel, grid, threads, bytes, st, b);
+  return e == cudaSuccess ? PERT_OK : (int)e;
 }
 
 // forward launch for row width H: the VPL = 2 variant (LPR = H / 8 lanes per node, 256-thread CTAs with up to 128

@@ -7,8 +7,6 @@ from __future__ import annotations
 
 import ctypes as C
 
-import os
-
 import torch
 
 from . import _lib, ops
@@ -261,10 +259,6 @@ class Engine:
         ops.LAUNCHES["n"] += self.launches_backward()
 
 
-# PERT_DIRECT_GRADS=0: always hand the parameter gradients to autograd (A/B of the host-side cost, see _EngineFn.backward)
-_DIRECT_GRADS = os.environ.get("PERT_DIRECT_GRADS", "1") != "0"
-
-
 class _EngineFn(torch.autograd.Function):
     """model.forward as ONE autograd node: inputs are the parameters (so autograd routes their gradients),
     outputs (global_pred, local_pred)."""
@@ -287,21 +281,20 @@ class _EngineFn(torch.autograd.Function):
         eng.last_grad_buffer = gbuf      # every parameter gradient is a view of this buffer (one all-reduce in DP)
         views = eng.fp.views_of(gbuf)
         params = eng.fp.params
-        if _DIRECT_GRADS:
-            # The reference loop calls optimizer.zero_grad() (set_to_none) before every backward (pert_gnn.py:232): every
-            # .grad is None and autograd's AccumulateGrad would just install the 42 views one by one (~0.25 ms of host
-            # time per step, a third of this loop's budget).  In exactly that state -- no gradient to accumulate into,
-            # no hooks registered on any parameter -- the views are attached directly and autograd gets no parameter
-            # gradients to route.  Any other state takes the regular autograd path below.
-            direct = True
-            for p in params:
-                if p.grad is not None or p._backward_hooks or getattr(p, "_post_accumulate_grad_hooks", None):
-                    direct = False
-                    break
-            if direct:
-                for p, v in zip(params, views):
-                    p.grad = v
-                return (None,) * (9 + len(params))
+        # The reference loop calls optimizer.zero_grad() (set_to_none) before every backward (pert_gnn.py:232): every
+        # .grad is None and autograd's AccumulateGrad would just install the 42 views one by one (~0.25 ms of host time
+        # per step, a third of this loop's budget).  In exactly that state -- no gradient to accumulate into, no hooks
+        # registered on any parameter -- the views are attached directly and autograd gets no parameter gradients to
+        # route.  Any other state takes the regular autograd path below.
+        direct = True
+        for p in params:
+            if p.grad is not None or p._backward_hooks or getattr(p, "_post_accumulate_grad_hooks", None):
+                direct = False
+                break
+        if direct:
+            for p, v in zip(params, views):
+                p.grad = v
+            return (None,) * (9 + len(params))
         return (None,) * 9 + tuple(views)
 
 

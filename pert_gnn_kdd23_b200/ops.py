@@ -14,35 +14,6 @@ from ._lib import call, ptr, stream
 # launches issued through the C-ABI (bench.py reports it as `gpu_launches`)
 LAUNCHES = {"n": 0}
 
-# optional CUDA-event timing of selected launches on the launching stream (bench.py roofline)
-TIMING = {"on": False}
-TIMERS = {}
-
-
-class _timed:
-    def __init__(self, name):
-        self.name = name
-
-    def __enter__(self):
-        if TIMING["on"]:
-            self.e0 = torch.cuda.Event(enable_timing=True)
-            self.e1 = torch.cuda.Event(enable_timing=True)
-            self.e0.record()
-        return self
-
-    def __exit__(self, *a):
-        if TIMING["on"]:
-            self.e1.record()
-            TIMERS.setdefault(self.name, []).append((self.e0, self.e1))
-
-
-def collect_timers():
-    """name -> (total ms, count); call after a device synchronize."""
-    out = {}
-    for name, evs in TIMERS.items():
-        out[name] = (sum(a.elapsed_time(b) for a, b in evs), len(evs))
-    return out
-
 
 def _need_cuda(*ts):
     for t in ts:
@@ -85,9 +56,8 @@ def gemm_nt_raw(A, B, bias, out, relu=False, accumulate=False):
     _, lda, a_cb, a_cbs, M, K = _blocked(A)
     _, ldc, c_cb, c_cbs, M2, Nc = _blocked(out)
     assert M == M2 and B.size(0) == Nc and B.size(1) == K, (A.shape, B.shape, out.shape)
-    with _timed("gemm_nt" if M >= 4096 else "gemm_nt_small"):
-        call("pert_gemm_nt", ptr(A), lda, a_cb, a_cbs, ptr(B), B.stride(0), ptr(bias), ptr(out), ldc, c_cb, c_cbs,
-             M, Nc, K, int(relu), int(accumulate), stream())
+    call("pert_gemm_nt", ptr(A), lda, a_cb, a_cbs, ptr(B), B.stride(0), ptr(bias), ptr(out), ldc, c_cb, c_cbs,
+         M, Nc, K, int(relu), int(accumulate), stream())
     LAUNCHES["n"] += 1
     return out
 
@@ -97,9 +67,8 @@ def gemm_tn_raw(A, B, out):
     _, lda, a_cb, a_cbs, R, Mc = _blocked(A)
     _, ldb, b_cb, b_cbs, R2, Nc = _blocked(B)
     assert R == R2 and out.shape == (Mc, Nc) and out.is_contiguous()
-    with _timed("gemm_tn" if R >= 4096 else "gemm_tn_small"):
-        call("pert_gemm_tn", ptr(A), lda, a_cb, a_cbs, ptr(B), ldb, b_cb, b_cbs, ptr(out), out.stride(0), None, R, Mc,
-             Nc, stream())
+    call("pert_gemm_tn", ptr(A), lda, a_cb, a_cbs, ptr(B), ldb, b_cb, b_cbs, ptr(out), out.stride(0), None, R, Mc,
+         Nc, stream())
     LAUNCHES["n"] += 1
     return out
 
@@ -152,10 +121,9 @@ class _LinearFn(torch.autograd.Function):
             dw = torch.zeros_like(weight)
             db = torch.zeros(weight.size(0), device=dy.device, dtype=torch.float32)
             wt = weight.t().contiguous()
-            with _timed("linear_bwd_planes"):
-                rc = _lib.lib().pert_linear_bwd_planes(ptr(dy), dy.stride(0), ptr(x), x.stride(0), ptr(wt), wt.stride(0),
-                                                       ptr(dw), dw.stride(0), ptr(db), ptr(dx), dx.stride(0), M,
-                                                       weight.size(0) // 4, K, K, stream())
+            rc = _lib.lib().pert_linear_bwd_planes(ptr(dy), dy.stride(0), ptr(x), x.stride(0), ptr(wt), wt.stride(0),
+                                                   ptr(dw), dw.stride(0), ptr(db), ptr(dx), dx.stride(0), M,
+                                                   weight.size(0) // 4, K, K, stream())
             if rc == 0:
                 LAUNCHES["n"] += 1
                 return dx, dw, db, None, None
@@ -298,11 +266,10 @@ class _TConvFn(torch.autograd.Function):
         alpha = torch.empty(max(index.E, 1), device=planes.device, dtype=torch.float32)
         q, k, v = planes[0], planes[1], planes[2]
         s = planes[3] if P_ == 4 else None
-        with _timed("tconv_fwd"):
-            call("pert_tconv_fwd_c", ptr(q), ptr(k), ptr(v), ptr(s), H, ptr(index.rowptr), ptr(index.csr_src),
-                 ptr(index.csr_if) if has_e else None, ptr(index.csr_rpc) if has_e else None,
-                 ptr(t_if), ptr(t_rpc), ptr(out), H, ptr(alpha), t_rpc.size(0) if has_e else 0, N, index.E,
-                 getattr(index, "num_graphs", 0), H, C, stream())
+        call("pert_tconv_fwd_c", ptr(q), ptr(k), ptr(v), ptr(s), H, ptr(index.rowptr), ptr(index.csr_src),
+             ptr(index.csr_if) if has_e else None, ptr(index.csr_rpc) if has_e else None,
+             ptr(t_if), ptr(t_rpc), ptr(out), H, ptr(alpha), t_rpc.size(0) if has_e else 0, N, index.E,
+             getattr(index, "num_graphs", 0), H, C, stream())
         LAUNCHES["n"] += 1
         ctx.index = index
         ctx.has_e = has_e
@@ -324,13 +291,12 @@ class _TConvFn(torch.autograd.Function):
         if ctx.has_e:
             dt_if = torch.zeros_like(t_if)
             dt_rpc = torch.zeros_like(t_rpc)
-        with _timed("tconv_bwd"):
-            call("pert_tconv_bwd_c", ptr(g), g.stride(0), ptr(planes[0]), ptr(planes[1]), ptr(planes[2]), H,
-                 ptr(index.rowptr), ptr(index.csr_src), ptr(index.csr_if) if ctx.has_e else None,
-                 ptr(index.csr_rpc) if ctx.has_e else None, ptr(index.colptr), ptr(index.csc_pos),
-                 ptr(index.csc_dst), ptr(t_if), ptr(t_rpc), ptr(alpha), ptr(dplanes[0]), ptr(dplanes[1]),
-                 ptr(dplanes[2]), H, ptr(dsp), ptr(rpc_ws), ptr(dt_if), ptr(dt_rpc), t_rpc.size(0) if ctx.has_e else 0, N,
-                 index.E, getattr(index, "num_graphs", 0), H, C, stream())
+        call("pert_tconv_bwd_c", ptr(g), g.stride(0), ptr(planes[0]), ptr(planes[1]), ptr(planes[2]), H,
+             ptr(index.rowptr), ptr(index.csr_src), ptr(index.csr_if) if ctx.has_e else None,
+             ptr(index.csr_rpc) if ctx.has_e else None, ptr(index.colptr), ptr(index.csc_pos),
+             ptr(index.csc_dst), ptr(t_if), ptr(t_rpc), ptr(alpha), ptr(dplanes[0]), ptr(dplanes[1]),
+             ptr(dplanes[2]), H, ptr(dsp), ptr(rpc_ws), ptr(dt_if), ptr(dt_rpc), t_rpc.size(0) if ctx.has_e else 0, N,
+             index.E, getattr(index, "num_graphs", 0), H, C, stream())
         LAUNCHES["n"] += 2
         if P_ == 4:
             dplanes[3].copy_(g)

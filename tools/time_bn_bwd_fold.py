@@ -12,23 +12,10 @@ consecutive launches do not find each other's planes in L2; the median train giv
 import argparse
 import ctypes
 import math
-import os
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
+from measure import card, timed
 
 
 def main():
@@ -113,17 +100,7 @@ def main():
     for label, fn in cases:
         for o in sets:
             _lib.check(fn(o), label)
-        torch.cuda.synchronize()
-        times = []
-        for _ in range(a.trains):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for i in range(a.per_train):
-                fn(sets[i % 2])
-            e1.record()
-            torch.cuda.synchronize()
-            times.append(e0.elapsed_time(e1) * 1e3 / a.per_train)
-        times.sort()
+        times = sorted(timed(fn, a.per_train, rotate=sets)[1] * 1e3 for _ in range(a.trains))
         res[label] = times[len(times) // 2]
         print(f"{label:42s} {res[label]:8.1f} us per launch (median of {a.trains} trains; range "
               f"{times[0]:.1f} .. {times[-1]:.1f})")

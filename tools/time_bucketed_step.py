@@ -16,23 +16,10 @@ pad_ratio, captures and replays).
 """
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
+from measure import card, timed
 
 
 def main():
@@ -96,27 +83,19 @@ def main():
                 evaluate_bucketed(m_b, eval_loader, dev)
             return epochs * len(eval_loader), epochs * len(eval_ids)
 
-        def window(fn, epochs):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            torch.cuda.synchronize()
-            e0.record()
-            steps, dags = fn(epochs)
-            e1.record()
-            torch.cuda.synchronize()
-            return e0.elapsed_time(e1) / 1e3, steps, dags
-
         for title, arms in (("train", {"eager": train_eager, "bucketed": train_bucketed}),
                             ("eval", {"eager": eval_eager, "bucketed": eval_bucketed})):
             epochs = {}
             for k, fn in arms.items():                        # warm-up: every bucket eager, captured, replayed
                 fn(a.warmup_epochs)
-                secs, _, _ = window(fn, 1)                    # epochs per window: at least --min-seconds
+                secs = timed(lambda: fn(1))[1] / 1e3          # epochs per window: at least --min-seconds
                 epochs[k] = max(1, int(a.min_seconds / max(secs, 1e-6)) + 1)
             c0, r0 = bucketed.captures, bucketed.replays
             res = {k: [] for k in arms}
             for r in range(a.runs):
                 for k, fn in arms.items():
-                    secs, steps, dags = window(fn, epochs[k])
+                    (steps, dags), t = timed(lambda: fn(epochs[k]))
+                    secs = t / 1e3
                     ms = secs * 1e3 / steps
                     res[k].append((ms, dags / secs))
                     print(json.dumps({"batch_size": bs, "what": title, "arm": k, "run": r, "seconds": round(secs, 3),

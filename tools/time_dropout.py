@@ -11,23 +11,10 @@ Prints the card name and power limit, then one JSON line per run and a summary l
 """
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
+from measure import card, timed
 
 
 def main():
@@ -65,24 +52,14 @@ def main():
         opt = torch.optim.Adam(m.parameters(), lr=3e-4)
         return lambda d: train_step(m, opt, d, 0.5)
 
-    def timed(step, n):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        for i in range(n):
-            step(batches[i % 2])
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / n
-
     for title, arms in (("GraphedTrainStep", {"p=0": graphed(0.0), "p=0.1": graphed(0.1)}),
                         ("drop-in train_step p=0.1", {"engine": dropin(True), "operators": dropin(False)})):
         for step in arms.values():
-            timed(step, max(a.warmup, 4))           # every key: eager, capture + replay, replays
+            timed(step, max(a.warmup, 4), rotate=batches)   # every key: eager, capture + replay, replays
         res = {k: [] for k in arms}
         for r in range(a.runs):
             for k, step in arms.items():
-                ms = timed(step, a.steps)
+                _, ms = timed(step, a.steps, rotate=batches)
                 res[k].append(ms)
                 print(json.dumps({"what": title, "arm": k, "run": r, "ms_per_step": round(ms, 4),
                                   "dags_per_s": round(B / ms * 1e3, 1)}), flush=True)

@@ -19,47 +19,16 @@ Prints the card name and power limit, then one JSON line: median and [min, max] 
 """
 import argparse
 import json
-import os
 import statistics
-import subprocess
 import sys
-import time
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
+from measure import card, host_ms, timed
 
 
 def stats(xs):
     return {"median": statistics.median(xs), "min": min(xs), "max": max(xs)}
-
-
-def steady(step, batches, n):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for i in range(n):
-        step(batches[i % 2])
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) / n
-
-
-def host_ms(fn):
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    out = fn()
-    torch.cuda.synchronize()
-    return (time.perf_counter() - t0) * 1e3, out
 
 
 def main():
@@ -84,27 +53,27 @@ def main():
         model = SAGEDeterministic(*model_args(2)).cuda()
         opt = FusedAdam(FlatParams(model), lr=1e-3)
         step = GraphedTrainStep(model, opt)
-        steady(step, batches, args.warmup)
-        out["steady_before"].append(steady(step, batches, args.steps))
+        timed(step, args.warmup, rotate=batches)
+        out["steady_before"].append(timed(step, args.steps, rotate=batches)[1])
         rows = {"cat": 2 * model.cat_embedding[0].num_embeddings, "entry": 2 * model.entry_embeds.num_embeddings,
                 "interface": 2 * model.interface_embeds.num_embeddings,
                 "rpctype": 2 * model.rpctype_embeds.num_embeddings}
-        ms, _ = host_ms(lambda: grow_embeddings(model, opt, seed=rep, **rows))
+        _, ms = host_ms(lambda: grow_embeddings(model, opt, seed=rep, **rows))
         out["grow"].append(ms)
         inv = step.invalidations
-        out["first_step_after"].append(host_ms(lambda: step(batches[0]))[0])
-        out["second_key_first_step"].append(host_ms(lambda: step(batches[1]))[0])
+        out["first_step_after"].append(host_ms(lambda: step(batches[0]))[1])
+        out["second_key_first_step"].append(host_ms(lambda: step(batches[1]))[1])
         assert step.invalidations == inv + 2 and step.capture_error is None
-        steady(step, batches, args.warmup)
-        out["steady_after"].append(steady(step, batches, args.steps))
+        timed(step, args.warmup, rotate=batches)
+        out["steady_after"].append(timed(step, args.steps, rotate=batches)[1])
         del step, opt, model
         a = list(model_args(2))
         a[1], a[2], a[3], a[4] = [rows["cat"]], rows["entry"] - 1, rows["interface"] - 1, rows["rpctype"] - 1
         torch.manual_seed(rep)
         built = SAGEDeterministic(*a).cuda()
         step = GraphedTrainStep(built, FusedAdam(FlatParams(built), lr=1e-3))
-        steady(step, batches, args.warmup)
-        out["steady_built_at_grown_sizes"].append(steady(step, batches, args.steps))
+        timed(step, args.warmup, rotate=batches)
+        out["steady_built_at_grown_sizes"].append(timed(step, args.steps, rotate=batches)[1])
         del step, built
 
         a = list(model_args(2))
@@ -113,9 +82,9 @@ def main():
         big = SAGEDeterministic(*a).cuda()
         bopt = FusedAdam(FlatParams(big), lr=1e-3)
         bstep = GraphedTrainStep(big, bopt)
-        steady(bstep, batches, 3)
+        timed(bstep, 3, rotate=batches)
         n = big.entry_embeds.num_embeddings + 64
-        out["grow_1M_interface"].append(host_ms(lambda: grow_embeddings(big, bopt, entry=n, seed=rep))[0])
+        out["grow_1M_interface"].append(host_ms(lambda: grow_embeddings(big, bopt, entry=n, seed=rep))[1])
         del bstep, bopt, big
         torch.cuda.empty_cache()
     res = {k: stats(v) for k, v in out.items()}

@@ -9,26 +9,10 @@ the shapes: read dY (4 N H), read X (N K), write dX (N Kd), all fp32; 2 N 4H (K 
     python tools/time_linear_bwd.py [--trains 9] [--per-train 12]
 """
 import argparse
-import os
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-HBM_PEAK = 3.35e12        # H100 SXM data sheet, B/s
-TF32_PEAK = 495e12        # dense TF32, FLOP/s
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
+from measure import HBM_BYTES_PER_S, TF32_FLOP_PER_S, card, timed
 
 
 def main():
@@ -66,29 +50,19 @@ def main():
 
         byts = (4 * N * H + N * K + N * Kd) * 4
         flops = 3 * 2 * N * 4 * H * (K + Kd)
-        floor = max(byts / HBM_PEAK, flops / TF32_PEAK)
-        bound = "HBM" if byts / HBM_PEAK >= flops / TF32_PEAK else "TF32"
+        floor = max(byts / HBM_BYTES_PER_S, flops / TF32_FLOP_PER_S)
+        bound = "HBM" if byts / HBM_BYTES_PER_S >= flops / TF32_FLOP_PER_S else "TF32"
         print(f"{name}: N={N} H={H} K={K} Kd={Kd}  bytes {byts / 1e6:.1f} MB  3xTF32 work {flops / 1e9:.2f} GFLOP  "
               f"floor {floor * 1e6:.1f} us ({bound}-bound at the data-sheet peaks)")
         for label, fn in (("fused", fused), ("pair", pair)):
             for o in sets:                      # warm-up: module load, attribute set-up
                 _lib.check(fn(o), label)
-            torch.cuda.synchronize()
-            times = []
-            for _ in range(a.trains):
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for i in range(a.per_train):
-                    fn(sets[i % nsets])
-                e1.record()
-                torch.cuda.synchronize()
-                times.append(e0.elapsed_time(e1) * 1e3 / a.per_train)
-            times.sort()
+            times = sorted(timed(fn, a.per_train, rotate=sets)[1] * 1e3 for _ in range(a.trains))
             us = times[len(times) // 2]
             print(f"  {label:5s}: {us:7.1f} us/launch (trains: min {times[0]:.1f}, max {times[-1]:.1f})  "
-                  f"{byts / us / 1e3:7.1f} GB/s  {100 * byts / us / 1e-6 / HBM_PEAK:5.1f} % of HBM peak  "
-                  f"{100 * flops / us / 1e-6 / TF32_PEAK:5.1f} % of TF32 peak  ({100 * floor / (us * 1e-6):.1f} % of "
-                  f"the {bound} floor)")
+                  f"{byts / us / 1e3:7.1f} GB/s  {100 * byts / us / 1e-6 / HBM_BYTES_PER_S:5.1f} % of HBM peak  "
+                  f"{100 * flops / us / 1e-6 / TF32_FLOP_PER_S:5.1f} % of TF32 peak  "
+                  f"({100 * floor / (us * 1e-6):.1f} % of the {bound} floor)")
 
 
 if __name__ == "__main__":

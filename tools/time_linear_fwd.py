@@ -14,25 +14,10 @@ events around each train; the median train gives us per launch.  Bytes are the a
     python tools/time_linear_fwd.py [--trains 9] [--per-train 12]
 """
 import argparse
-import os
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-HBM_PEAK = 3.35e12        # H100 SXM data sheet, B/s
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
+from measure import HBM_BYTES_PER_S, card, timed
 
 
 def main():
@@ -81,25 +66,15 @@ def main():
                                   N * H, N, 4 * H, K, 0, 0, st)
 
         print(f"{name}: N={N} H={H} K={K}  algorithmic bytes {byts / 1e6:.1f} MB  "
-              f"HBM floor {byts / HBM_PEAK * 1e6:.1f} us at the data-sheet {HBM_PEAK / 1e12:.2f} TB/s")
+              f"HBM floor {byts / HBM_BYTES_PER_S * 1e6:.1f} us at the data-sheet {HBM_BYTES_PER_S / 1e12:.2f} TB/s")
         for label, fn in (("fused", fused), ("pair", pair)):
             for o in sets:                      # warm-up: module load, attribute set-up
                 _lib.check(fn(o), label)
-            torch.cuda.synchronize()
-            times = []
-            for _ in range(a.trains):
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for i in range(a.per_train):
-                    fn(sets[i % nsets])
-                e1.record()
-                torch.cuda.synchronize()
-                times.append(e0.elapsed_time(e1) * 1e3 / a.per_train)
-            times.sort()
+            times = sorted(timed(fn, a.per_train, rotate=sets)[1] * 1e3 for _ in range(a.trains))
             us = times[len(times) // 2]
             print(f"  {label:5s}: {us:7.1f} us/launch (trains: min {times[0]:.1f}, max {times[-1]:.1f})  "
-                  f"{byts / us / 1e6:6.2f} TB/s  {100 * byts / us / 1e-6 / HBM_PEAK:5.1f} % of the data-sheet HBM "
-                  f"bandwidth")
+                  f"{byts / us / 1e6:6.2f} TB/s  {100 * byts / us / 1e-6 / HBM_BYTES_PER_S:5.1f} % of the data-sheet "
+                  f"HBM bandwidth")
 
 
 if __name__ == "__main__":

@@ -16,24 +16,11 @@ element-wise difference between the two arms' predictions.
 """
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
+from measure import card, timed
 
 
 def main():
@@ -88,17 +75,11 @@ def main():
                 out[k] = fn()
                 if k == "predict":
                     fn()
-            torch.cuda.synchronize()
             res = {k: [] for k in arms}
             for r in range(a.runs):
                 for k, fn in arms.items():
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    torch.cuda.synchronize()
-                    e0.record()
-                    out[k] = fn()
-                    e1.record()
-                    torch.cuda.synchronize()
-                    secs = e0.elapsed_time(e1) / 1e3
+                    out[k], ms = timed(fn)
+                    secs = ms / 1e3
                     res[k].append(Q / secs)
                     print(json.dumps({"batch_size": bs, "join": "asof" if asof else "exact", "arm": k, "run": r,
                                       "seconds": round(secs, 3), "requests_per_s": round(Q / secs, 1)}), flush=True)

@@ -20,11 +20,9 @@ import warnings
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-from pert_gnn_kdd23_b200.rawtable import CALL_COLUMNS, RESOURCE_COLUMNS  # noqa: E402
-from pert_gnn_kdd23_b200.synthetic import make_random_raw_tables  # noqa: E402
+from measure import timed
+from pert_gnn_kdd23_b200.rawtable import CALL_COLUMNS, RESOURCE_COLUMNS
+from pert_gnn_kdd23_b200.synthetic import make_random_raw_tables
 
 
 def time_gpu(raw, reps):
@@ -38,12 +36,8 @@ def time_gpu(raw, reps):
     base = torch.cuda.memory_allocated()
     ms = []
     for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        p = process_raw(raw, "cuda")
-        b.record()
-        b.synchronize()
-        ms.append(a.elapsed_time(b))
+        p, t = timed(lambda: process_raw(raw, "cuda"))
+        ms.append(t)
         kept = len(p.check())
         del p
     peak = torch.cuda.max_memory_allocated() - base

@@ -25,17 +25,11 @@ line per (rows, workload).
 import argparse
 import ctypes as C
 import json
-import os
 import statistics
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from time_resource_update import HBM, card, events  # noqa: E402
+from measure import HBM_BYTES_PER_S, card, timed
 
 B, N_MS, K = 30000, 30000, 30000
 
@@ -123,10 +117,10 @@ def main():
             times = {"update": [], "append": [], "rebuild": []}
             for _ in range(a.reps):
                 restore()
-                times["update"].append(events(update))
+                times["update"].append(timed(update)[1])
                 restore()
-                times["append"].append(events(append))
-                times["rebuild"].append(events(rebuild))
+                times["append"].append(timed(append)[1])
+                times["rebuild"].append(timed(rebuild)[1])
             # kernel time of the merge alone: the count once (as _update_resources prepares it), the merge repeated
             restore()
             L = _lib.lib()
@@ -157,14 +151,14 @@ def main():
                     seg.data_ptr(), p, q, n_dropped, n_out, *(t.data_ptr() for t in out), _lib.stream()), "merge")
 
             merge()
-            t_merge = events(merge, 20)
+            t_merge = timed(merge, 20)[1]
             moved = (n + k + n_out) * 52
             med = {key: statistics.median(v) for key, v in times.items()}
             res = {"rows": n, "k": K, "workload": workload,
                    **{f"{key}_ms_median": round(m, 3) for key, m in med.items()},
                    **{f"{key}_ms_range": [round(min(v), 3), round(max(v), 3)] for key, v in times.items()},
                    "merge_kernel_ms": round(t_merge, 4), "merge_bytes": moved,
-                   "merge_bw_frac_of_3.35TBps": round(moved / (t_merge * 1e-3) / HBM, 3),
+                   "merge_bw_frac_of_3.35TBps": round(moved / (t_merge * 1e-3) / HBM_BYTES_PER_S, 3),
                    "update_vs_append": round(med["update"] / med["append"], 2),
                    "rebuild_vs_update": round(med["rebuild"] / med["update"], 2)}
             print(json.dumps(res), flush=True)

@@ -25,28 +25,15 @@ the same run, then one JSON line per window size (with --json, also into that fi
 import argparse
 import copy
 import json
-import os
 import statistics
-import subprocess
-import sys
 import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from time_resource_update import HBM, events  # noqa: E402
+from measure import HBM_BYTES_PER_S, card, timed
 
 B, N_MS = 30000, 30000
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
 
 
 def bucket(rng, b):
@@ -123,7 +110,7 @@ def main():
     assert torch.cuda.is_available(), "needs a GPU"
     from pert_gnn_kdd23_b200.rawtable import ResourceSampleWindow
 
-    print(f"card: {card()}", flush=True)
+    print(f"card: {card(sm_clock=True)}", flush=True)
     results = []
     for W in a.open:
         rng = np.random.default_rng(W)
@@ -144,13 +131,11 @@ def main():
 
         times = {"add": [], "rebuild": [], "pandas": []}
         for rep in range(a.reps + 1):
-            res = {}
-            t_add = events(lambda: res.__setitem__("add", do_add()))
-            t_reb = events(lambda: res.__setitem__("reb", rebuild(*alld)))
+            rows, t_add = timed(do_add)
+            (keys, vals), t_reb = timed(lambda: rebuild(*alld))
             t0 = time.perf_counter()
             pandas_stats(*allh)
             t_pd = (time.perf_counter() - t0) * 1e3
-            rows, (keys, vals) = res["add"], res["reb"]
             got_keys = rows.index[:, 0] * N_MS + rows.index[:, 1]
             pos = torch.searchsorted(keys, got_keys)
             assert torch.equal(keys[pos], got_keys) and same_bits(rows.values, vals[pos]), "add != rebuild"
@@ -165,14 +150,14 @@ def main():
              "add_ms": round(med["add"], 3), "rebuild_ms": round(med["rebuild"], 3), "pandas_ms": round(med["pandas"], 1),
              "add_vs_rebuild": round(med["rebuild"] / med["add"], 2), "merge_ms": round(merge_ms, 4),
              "window_kernels_ms": round(window_ms, 4), "sort_kernels_ms": round(sort_ms, 4),
-             "add_device_ms": round(device_ms, 4),
-             "merge_bytes": nbytes, "merge_bw": round(nbytes / (merge_ms * 1e-3) / HBM, 3) if merge_ms else None,
+             "add_device_ms": round(device_ms, 4), "merge_bytes": nbytes,
+             "merge_bw": round(nbytes / (merge_ms * 1e-3) / HBM_BYTES_PER_S, 3) if merge_ms else None,
              "reps": a.reps, "all_ms": {n: [round(x, 3) for x in v] for n, v in times.items()}}
         results.append(r)
         print(json.dumps(r), flush=True)
     if a.json:
         with open(a.json, "w") as f:
-            json.dump({"card": card(), "results": results}, f, indent=1)
+            json.dump({"card": card(sm_clock=True), "results": results}, f, indent=1)
 
 
 if __name__ == "__main__":

@@ -23,40 +23,14 @@ device rebuild bit for bit.  Prints the card name and power limit, then one JSON
 import argparse
 import ctypes as C
 import json
-import os
 import statistics
-import subprocess
-import sys
-import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from measure import HBM_BYTES_PER_S, card, host_ms, timed
 
 B, N_MS, K = 30000, 30000, 30000
-HBM = 3.35e12
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
-
-
-def events(fn, reps=1):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
 
 
 def main():
@@ -135,15 +109,12 @@ def main():
                 host_list = list(zip(h_ts.tolist(), h_ms.tolist()))
             for r in range(a.reps):
                 restore()
-                times["append"].append(events(append))
-                times["rebuild"].append(events(rebuild))
+                times["append"].append(timed(append)[1])
+                times["rebuild"].append(timed(rebuild)[1])
                 if host_list is not None:
-                    torch.cuda.synchronize()
-                    t0 = time.perf_counter()
-                    PatternStore(art["runtime2graph"], art["entry2runtimes"], host_list, host_vals, art["tr2data"],
-                                 dev, n_ms=N_MS)
-                    torch.cuda.synchronize()
-                    times["host"].append((time.perf_counter() - t0) * 1e3)
+                    times["host"].append(host_ms(lambda: PatternStore(
+                        art["runtime2graph"], art["entry2runtimes"], host_list, host_vals, art["tr2data"], dev,
+                        n_ms=N_MS))[1])
             # kernel time of the merge alone: the count once, then the merge repeated on the same inputs
             restore()
             nk, perm = torch.sort(ts1 * N_MS + ms1, stable=True)
@@ -168,13 +139,13 @@ def main():
                     _lib.stream()), "merge")
 
             merge()
-            t_merge = events(merge, 20)
+            t_merge = timed(merge, 20)[1]
             moved = 2 * (n + K) * 52
             res = {"rows": n, "k": K, "workload": workload,
                    **{f"{k}_ms_median": round(statistics.median(v), 3) for k, v in times.items()},
                    **{f"{k}_ms_min": round(min(v), 3) for k, v in times.items()},
                    "merge_kernel_ms": round(t_merge, 4), "merge_bytes": moved,
-                   "merge_bw_frac_of_3.35TBps": round(moved / (t_merge * 1e-3) / HBM, 3),
+                   "merge_bw_frac_of_3.35TBps": round(moved / (t_merge * 1e-3) / HBM_BYTES_PER_S, 3),
                    "append_vs_rebuild": round(statistics.median(times["rebuild"]) / statistics.median(times["append"]),
                                               2)}
             print(json.dumps(res), flush=True)

@@ -13,25 +13,13 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
-import sys
 import tempfile
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from measure import card
 
 N_ROT = 8   # distinct resident batches, as bench.py
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
 
 
 def make_batches(cfg, count, dev):

@@ -16,63 +16,14 @@ Prints the card name and power limit, then one JSON line per store size: median 
 """
 import argparse
 import json
-import os
 import statistics
-import subprocess
-import sys
-import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from measure import Probe, card, host_ms
 
 CHUNK = 10_000
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
-
-
-class Probe:
-    """Wraps library calls and Python stages to time them inside append_traces: CUDA events around a C call (its
-    kernels, in stream order), a synchronised host clock around a Python stage."""
-
-    def __init__(self):
-        self.ev, self.host = {}, {}
-
-    def cuda(self, name, fn):
-        def wrapped(*a):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            rc = fn(*a)
-            e1.record()
-            self.ev.setdefault(name, []).append((e0, e1))
-            return rc
-        return wrapped
-
-    def clock(self, name, fn):
-        def wrapped(*a, **k):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            out = fn(*a, **k)
-            torch.cuda.synchronize()
-            self.host[name] = self.host.get(name, 0.0) + (time.perf_counter() - t0) * 1e3
-            return out
-        return wrapped
-
-    def take(self):
-        torch.cuda.synchronize()
-        out = {k: sum(a.elapsed_time(b) for a, b in v) for k, v in self.ev.items()}
-        out.update(self.host)
-        self.ev, self.host = {}, {}
-        return out
 
 
 def stats(xs):
@@ -128,11 +79,7 @@ def main():
                     n_pat = len(s.rt_ids)
                     probe.take()
                     tracegroup.group_traces = probe.clock("group_chunk", group)
-                    torch.cuda.synchronize()
-                    t0 = time.perf_counter()
-                    s.append_traces(chunk)
-                    torch.cuda.synchronize()
-                    dt = (time.perf_counter() - t0) * 1e3
+                    dt = host_ms(lambda: s.append_traces(chunk))[1]
                     tracegroup.group_traces = group
                     p = probe.take()
                     n_c = group(chunk).n_runtimes
@@ -141,12 +88,10 @@ def main():
                         parts.append(p)
                         new_share.append((len(s.rt_ids) - n_pat) / n_c)
                 else:
-                    torch.cuda.synchronize()
-                    t0 = time.perf_counter()
-                    PatternStore.from_trace_groups(group(whole).check(), "span", *res, "cuda", n_ms=4096)
-                    torch.cuda.synchronize()
+                    dt = host_ms(lambda: PatternStore.from_trace_groups(group(whole).check(), "span", *res, "cuda",
+                                                                        n_ms=4096))[1]
                     if r:
-                        rows["rebuild"].append((time.perf_counter() - t0) * 1e3)
+                        rows["rebuild"].append(dt)
                     probe.take()
         out = {"store_traces": n, "chunk_traces": CHUNK, "new_runtime_share": stats(new_share),
                "append_ms": stats(rows["append"]), "rebuild_ms": stats(rows["rebuild"]),

@@ -20,53 +20,16 @@ Prints the card name and power limit, then one JSON line per store size: median 
 import argparse
 import itertools
 import json
-import os
 import statistics
-import subprocess
-import sys
 import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from measure import HBM_BYTES_PER_S, Probe, card, host_ms
 
 BUCKET = 30000
 CHUNK = 10_000
-HBM_BYTES_PER_S = 3.35e12
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
-
-
-class Probe:
-    """CUDA events around a library call (its kernels, in stream order)."""
-
-    def __init__(self):
-        self.ev = {}
-
-    def cuda(self, name, fn):
-        def wrapped(*a):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            rc = fn(*a)
-            e1.record()
-            self.ev.setdefault(name, []).append((e0, e1))
-            return rc
-        return wrapped
-
-    def take(self):
-        torch.cuda.synchronize()
-        out = {k: sum(a.elapsed_time(b) for a, b in v) for k, v in self.ev.items()}
-        self.ev = {}
-        return out
 
 
 def stats(xs):
@@ -129,11 +92,7 @@ def main():
                            int(s._ingest.rows.shape[1]))
                     keys = list(s.trace_keys)
                     probe.take()
-                    torch.cuda.synchronize()
-                    t0 = time.perf_counter()
-                    remap = s.evict_traces(BUCKET)
-                    torch.cuda.synchronize()
-                    dt = (time.perf_counter() - t0) * 1e3
+                    remap, dt = host_ms(lambda: s.evict_traces(BUCKET))
                     p = probe.take()
                     new = (len(s), int(s._ingest.cnt.shape[0]), len(s.rt_ids), s._ingest.n_nodes, s._ingest.n_edges,
                            int(s._ingest.rows.shape[1]))
@@ -150,12 +109,9 @@ def main():
                         evicted.append(int((remap < 0).sum()))
                     del s
                 else:
-                    torch.cuda.synchronize()
-                    t0 = time.perf_counter()
-                    build(survivors)
-                    torch.cuda.synchronize()
+                    dt = host_ms(lambda: build(survivors))[1]
                     if r:
-                        rows["rebuild"].append((time.perf_counter() - t0) * 1e3)
+                        rows["rebuild"].append(dt)
                     probe.take()
         out = {"store_traces": n, "evicted_traces": stats(evicted), "evict_ms": stats(rows["evict"]),
                "rebuild_ms": stats(rows["rebuild"]),
@@ -173,13 +129,9 @@ def main():
             host = {c: v[sel].copy() for c, v in cols.items()}
             host["timestamp"] += 300000 + k * BUCKET - t_min[inv[sel]]       # every chunk trace in the next bucket
             chunk = {c: torch.from_numpy(v).cuda() for c, v in host.items()}
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            s.append_traces(chunk)
-            s.evict_traces((k + 1) * BUCKET)
-            torch.cuda.synchronize()
+            dt = host_ms(lambda: (s.append_traces(chunk), s.evict_traces((k + 1) * BUCKET)))[1]
             if k:                                        # step 0 builds the runtime table
-                step_ms.append((time.perf_counter() - t0) * 1e3)
+                step_ms.append(dt)
         probe.take()
         out["loop_store_traces_end"] = len(s)
         out["loop_step_ms"] = stats(step_ms)

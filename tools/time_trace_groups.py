@@ -18,42 +18,15 @@ and the share of the 3.35 TB/s HBM3 data-sheet bandwidth of the H100 SXM they im
 """
 import argparse
 import json
-import os
-import subprocess
-import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import numpy as np
+import torch
 
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
+from measure import HBM_BYTES_PER_S, card, per_call
 
-PEAK_BYTES_S = 3.35e12
 ROW_BYTES = 24 + 12 + 52 + 2 * 28
 TRACE_BYTES = 160
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i",
-                            str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30)
-        name, power = (s.strip() for s in q.stdout.strip().split(","))
-    except Exception as e:                                    # the card name still comes from the runtime
-        name, power = torch.cuda.get_device_name(), f"unknown ({type(e).__name__})"
-    return name, power
-
-
-def timed(fn, iters):
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2 * iters)]
-    out = None
-    for i in range(iters):
-        ev[2 * i].record()
-        out = fn()
-        ev[2 * i + 1].record()
-    torch.cuda.synchronize()
-    ms = [ev[2 * i].elapsed_time(ev[2 * i + 1]) for i in range(iters)]
-    return out, float(np.median(ms)), ms
 
 
 def main():
@@ -84,13 +57,14 @@ def main():
         g = group_traces(cols).check()
         PatternStore.from_trace_groups(g, a.kind, res_index, res_vals, "cuda")
     torch.cuda.synchronize()
-    g, group_ms, group_all = timed(lambda: group_traces(cols).check(), a.iters)
-    _, graphs_ms, _ = timed(lambda: g.graphs(a.kind), a.iters)
-    store, store_ms, _ = timed(lambda: PatternStore.from_trace_groups(g, a.kind, res_index, res_vals, "cuda"),
-                               a.iters)
+    g, group_all = per_call(lambda: group_traces(cols).check(), a.iters)
+    graphs_all = per_call(lambda: g.graphs(a.kind), a.iters)[1]
+    store, store_all = per_call(lambda: PatternStore.from_trace_groups(g, a.kind, res_index, res_vals, "cuda"),
+                                a.iters)
+    group_ms, graphs_ms, store_ms = (float(np.median(ms)) for ms in (group_all, graphs_all, store_all))
     T, n_rt = len(g), g.n_runtimes
     R2 = int(g.rep_ptr[-1])
-    name, power = card()
+    name, power = card(split=True)
     alg = ROW_BYTES * R + TRACE_BYTES * T
     print(json.dumps({
         "card": name, "power_limit": power, "rows": R, "traces": T, "runtimes": n_rt, "rep_rows": R2,
@@ -100,7 +74,7 @@ def main():
         "table_to_store_ms": round(group_ms + store_ms, 3),
         "group_rows_per_s": R / (group_ms * 1e-3), "table_to_store_rows_per_s": R / ((group_ms + store_ms) * 1e-3),
         "group_alg_bytes": alg, "group_alg_GBps": alg / (group_ms * 1e-3) / 1e9,
-        "group_share_of_3.35TBps": alg / (group_ms * 1e-3) / PEAK_BYTES_S,
+        "group_share_of_3.35TBps": alg / (group_ms * 1e-3) / HBM_BYTES_PER_S,
         "store_traces": len(store), "generate_s_cpu": round(gen_s, 1),
     }))
 

@@ -20,34 +20,11 @@ summary with the mean node count per request of every arm.
 """
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
-
-
-def timed(fn):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    out = fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return out, e0.elapsed_time(e1) / 1e3
+from measure import card, timed
 
 
 def main():
@@ -137,7 +114,7 @@ def main():
     rate = {n: [] for n in arms}
     for r in range(a.runs):
         for name, kw in arms.items():
-            _, secs = timed(lambda: predict(model, store, ent, ts, batch_size=bs, asof=True, **kw))
+            secs = timed(lambda: predict(model, store, ent, ts, batch_size=bs, asof=True, **kw))[1] / 1e3
             rate[name].append(Q / secs)
             print(json.dumps({"arm": name, "run": r, "seconds": round(secs, 3), "requests_per_s": round(Q / secs, 1)}),
                   flush=True)
@@ -159,15 +136,15 @@ def main():
     prepared = {}
     for r in range(a.runs):
         for n in prep:
-            prepared[n], secs = timed(lambda: store._what_if_arrays(ent, ts, **arms[n]))
-            prep[n].append(secs)
+            prepared[n], ms = timed(lambda: store._what_if_arrays(ent, ts, **arms[n]))
+            prep[n].append(ms / 1e3)
     loops = {"plain": plain_loop, **{n: what_if_loop(w) for n, w in prepared.items()}}
     asm = {n: [] for n in loops}
     for fn in loops.values():
         fn()
     for r in range(a.runs):
         for name, fn in loops.items():
-            _, secs = timed(fn)
+            secs = timed(fn)[1] / 1e3
             asm[name].append(secs)
             print(json.dumps({"assembly": name, "run": r, "seconds": round(secs, 4)}), flush=True)
     nodes = {"plain": float(store._h_ent_nodes[ent].mean()), "own": float(prepared["own"].nodes.mean()),

@@ -10,24 +10,11 @@ limit, one JSON line per run and a summary line per width (median ms per step an
 """
 import argparse
 import json
-import os
 import statistics
-import subprocess
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name() + " (power limit not readable)"
+from measure import card, timed
 
 
 def main():
@@ -62,15 +49,8 @@ def main():
 
     def window(step):
         n, ms = 0, 0.0
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         while ms < 1e3 * a.min_seconds:
-            torch.cuda.synchronize()
-            e0.record()
-            for _ in range(20):
-                step(data)
-            e1.record()
-            torch.cuda.synchronize()
-            ms += e0.elapsed_time(e1)
+            ms += 20 * timed(lambda: step(data), 20)[1]
             n += 20
         return ms / n
 

@@ -56,7 +56,9 @@ extern "C" {
  * (raw resource samples aggregated into the open buckets' statistics); pert_linear_bwd_planes_ex, pert_tconv_bwd_bn
  * (_supported) (the BatchNorm backward folded into the node-linear and conv backward passes); pert_tconv_fwd_stats
  * (the conv forward with the BatchNorm statistics of its output); pert_flat_grow (relayout of the flat parameter and
- * optimizer buffers when embedding tables grow).  An additive entry point leaves the version as it is. */
+ * optimizer buffers when embedding tables grow); pert_model_workspace_bytes_q, pert_model_packed_bytes_q,
+ * pert_model_workspace_offset_q, pert_model_forward_q, pert_model_backward_q, pert_pinball_loss_q, pert_eval_metrics_q
+ * (a global head with several quantile outputs).  An additive entry point leaves the version as it is. */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -299,6 +301,22 @@ int pert_pinball_loss_live(const int64_t* y, const float* yhat, float tau, long 
                            float* dyhat, const long long* live, void* stream);
 int pert_eval_metrics_live(const int64_t* y, const float* yhat, float tau, long long B, double* acc,
                            const long long* live, void* stream);
+/* The same two for a head with T quantile outputs: yhat [B, T] (row-major), column t the taus[t]-quantile.  taus is a
+ * HOST array of T levels, read during the call and passed to the kernel by value (a captured graph keeps them).
+ *   loss[0] = 1/(B T) sum_b sum_t max(tau_t e_bt, (tau_t - 1) e_bt), e_bt = y_b - yhat_bt; dyhat [B, T] its gradient
+ *   times grad_scale, ties split evenly as in pert_pinball_loss.
+ *   acc: 4T + 1 doubles; for level t, acc[4t + 0..3] += sum |yhat_t - y|, sum |yhat_t - y| / y, sum of the pinball
+ *   terms at tau_t and the count of graphs with y <= yhat_t (coverage); acc[4T] += the count of graphs whose levels
+ *   cross (yhat_t > yhat_{t+1} for some t).
+ * live as above (NULL: every graph is real; ghost graphs get dyhat = 0 in every column and are not counted).  At T = 1
+ * the loss runs pert_pinball_loss's kernel, and the metric sums acc[0..2] follow pert_eval_metrics's arithmetic.
+ * PERT_ERR_BADARG, before any CUDA call, for T outside 1..PERT_MAX_QUANTILES, taus NULL, NaN, outside [0, 1] or not
+ * strictly increasing, and everything the plain forms refuse. */
+#define PERT_MAX_QUANTILES 8
+int pert_pinball_loss_q(const int64_t* y, const float* yhat, const float* taus, int T, long long B, float grad_scale,
+                        float* loss, float* dyhat, const long long* live, void* stream);
+int pert_eval_metrics_q(const int64_t* y, const float* yhat, const float* taus, int T, long long B, double* acc,
+                        const long long* live, void* stream);
 
 /* torch.optim.Adam step (pert_gnn.py:343,247) over one flat parameter buffer; g is scaled by grad_scale, weight_decay
  * is L2 added to the scaled gradient (not AdamW's decoupled decay).  The bias corrections lr / (1 - beta1^step) and
@@ -496,6 +514,30 @@ int pert_model_backward_live(const PertModelDesc* desc, const float* params, flo
                              const int* csc_dst, void* workspace, long long workspace_bytes, int training,
                              float dropout, const float* d_global, const float* d_local, const PertProbe* probe,
                              const long long* live, void* stream);
+/* A global head with n_out outputs (1 <= n_out <= PERT_MAX_QUANTILES): global_linear2 is [n_out, H] / [n_out] at
+ * off_g2_w / off_g2_b, global_pred and d_global are [B, n_out] (row-major).  Everything else is as in the _live forms
+ * (live may be NULL); at n_out = 1 these are exactly those calls.  At Hp > H the padded copy of global_linear2.weight
+ * (and its gradient) is [n_out, Hp], so the workspace layout depends on n_out: size, offsets and packed bytes come from
+ * the _q forms.  PERT_ERR_BADARG, before any CUDA call, for n_out outside 1..PERT_MAX_QUANTILES and everything the
+ * plain forms refuse. */
+long long pert_model_workspace_bytes_q(const PertModelDesc* desc, int n_out, long long N, long long E, long long B);
+long long pert_model_packed_bytes_q(const PertModelDesc* desc, int n_out);
+long long pert_model_workspace_offset_q(const PertModelDesc* desc, int n_out, long long N, long long E, long long B,
+                                        int which, int layer);
+int pert_model_forward_q(const PertModelDesc* desc, int n_out, const float* params, float* bn_running,
+                         long long* bn_nbt, const float* x, const int64_t* cat_X, const int64_t* entry_id,
+                         const float* probs, const float* pnn, const int64_t* batch, long long N, long long E,
+                         long long B, const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc,
+                         void* workspace, long long workspace_bytes, int training, float dropout,
+                         long long* dropout_state, float* global_pred, float* local_pred, int* status,
+                         const PertProbe* probe, void* index_ready, const long long* live, void* stream);
+int pert_model_backward_q(const PertModelDesc* desc, int n_out, const float* params, float* grads,
+                          const int64_t* cat_X, const int64_t* entry_id, const float* probs, const float* pnn,
+                          const int64_t* batch, long long N, long long E, long long B, const int* rowptr,
+                          const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr,
+                          const int* csc_pos, const int* csc_dst, void* workspace, long long workspace_bytes,
+                          int training, float dropout, const float* d_global, const float* d_local,
+                          const PertProbe* probe, const long long* live, void* stream);
 
 /* ---- device-side batch assembly from a resident pattern store (csrc/store.cu) ---------------------------------------
  * Replaces the host-side sample assembly + collation + per-step probability expansion of the reference:

@@ -134,7 +134,18 @@ SIGNATURES = {
                                      P, P]),
     "pert_batch_pad": (I, [P, P, P, P, P, P, P, P, P, LL, LL, LL, I, I, I, P, P, P, P, P, P, P, P, P, LL, LL, LL, P,
                            P]),
+    # a global head with n_out quantile outputs (int n_out after the descriptor; the _live argument lists)
+    "pert_model_workspace_bytes_q": (LL, [P, I, LL, LL, LL]),
+    "pert_model_packed_bytes_q": (LL, [P, I]),
+    "pert_model_workspace_offset_q": (LL, [P, I, LL, LL, LL, I, I]),
+    "pert_model_forward_q": (I, [P, I, P, P, P, P, P, P, P, P, P, LL, LL, LL, P, P, P, P, P, LL, I, F, P, P, P, P, P,
+                                 P, P, P]),
+    "pert_model_backward_q": (I, [P, I, P, P, P, P, P, P, P, LL, LL, LL, P, P, P, P, P, P, P, P, LL, I, F, P, P, P,
+                                  P, P]),
+    "pert_pinball_loss_q": (I, [P, P, P, I, LL, F, P, P, P, P]),
+    "pert_eval_metrics_q": (I, [P, P, P, I, LL, P, P, P]),
 }
+MAX_QUANTILES = 8                                       # PERT_MAX_QUANTILES
 
 _lib = None
 

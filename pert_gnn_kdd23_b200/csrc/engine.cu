@@ -12,6 +12,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <mutex>
+#include <type_traits>
 
 namespace {
 
@@ -194,14 +195,19 @@ __global__ void k_unpack(float* __restrict__ grads, const float* __restrict__ pa
 // stage holds all of W1 (ns = H, cs = 2H); above that 2H^2 floats do not fit, and the CTA stages W1 in slices of ns
 // output rows (forward) or cs input columns (backward) one after the other (head_slice).  Each output of a slice is
 // complete within it, so the sums are those of the single-stage kernel.
+// A head with T outputs (quantile levels, pert_model_forward_q): W2 is [T][H], out [B][T]; each lane keeps T partial
+// sums of h1 . W2[t].  TM (1, 2, 4, 8) is the compiled bound on T; TM = 1 is the one-output kernel.
 constexpr int HEAD_G = 8;
 constexpr int HEAD_T = HEAD_G * 32;
+template <int TM>
 __global__ void __launch_bounds__(HEAD_T) k_head_fwd(const float* __restrict__ pool, const float* __restrict__ table,
                                                      int n_rows, const int64_t* __restrict__ ids,
                                                      const float* __restrict__ W1, const float* __restrict__ b1,
                                                      const float* __restrict__ W2, const float* __restrict__ b2,
                                                      float* __restrict__ z, float* __restrict__ h1,
-                                                     float* __restrict__ out, int B, int H, int ns, int* status) {
+                                                     float* __restrict__ out, int B, int H, int ns, int T_,
+                                                     int* status) {
+  const int T = TM == 1 ? 1 : T_;
   extern __shared__ float hs[];                       // W1t slice [2H][ns] | z [HEAD_G][2H]
   float* w1t = hs;
   float* zs_all = hs + (size_t)2 * H * ns;
@@ -222,7 +228,9 @@ __global__ void __launch_bounds__(HEAD_T) k_head_fwd(const float* __restrict__ p
       z[(size_t)b * K2 + c] = v;
     }
   }
-  float o = 0.f;
+  float o[TM];
+#pragma unroll
+  for (int t = 0; t < TM; ++t) o[t] = 0.f;
   for (int n0 = 0; n0 < H; n0 += ns) {
     if (n0 > 0) __syncthreads();                      // every warp is done with the previous slice
     // lanes along n: the global reads are 16-byte pieces of different rows (L2 resident), the transposing
@@ -255,25 +263,35 @@ __global__ void __launch_bounds__(HEAD_T) k_head_fwd(const float* __restrict__ p
         }
         const float hv = fmaxf(a0 + a1 + __ldg(b1 + n0 + n), 0.f);
         h1[(size_t)b * H + n0 + n] = hv;
-        o = fmaf(hv, __ldg(W2 + n0 + n), o);
+#pragma unroll
+        for (int t = 0; t < TM; ++t)
+          if (t < T) o[t] = fmaf(hv, __ldg(W2 + (size_t)t * H + n0 + n), o[t]);
       }
     }
   }
   if (!act) return;
 #pragma unroll
-  for (int off = 16; off > 0; off >>= 1) o += __shfl_xor_sync(0xffffffffu, o, off);
-  if (lane == 0) out[b] = o + __ldg(b2);
+  for (int t = 0; t < TM; ++t) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) o[t] += __shfl_xor_sync(0xffffffffu, o[t], off);
+  }
+#pragma unroll
+  for (int t = 0; t < TM; ++t)      // lane t writes level t
+    if (t < T && lane == t) out[(size_t)b * T + t] = o[t] + __ldg(b2 + t);
 }
 
 // Backward of the head for HEAD_G graphs per CTA: dh1 = dg W2 (h1 > 0); dz = dh1 W1 -> dpool | entry-embedding rows
 // (atomic scatter); dW2 += dg h1; db2 += dg; dW1 += dh1^T z; db1 += dh1 (block-level sums, then one atomic per value).
+// T outputs: dg [B][T], dh1 = sum_t dg[t] W2[t] (the levels in order), dW2 [T][H], db2 [T].
+template <int TM>
 __global__ void __launch_bounds__(HEAD_T) k_head_bwd(const float* __restrict__ dg, const float* __restrict__ z,
                                                      const float* __restrict__ h1, const float* __restrict__ W1,
                                                      const float* __restrict__ W2, const int64_t* __restrict__ ids,
                                                      int n_rows, float* __restrict__ dpool, float* __restrict__ g_entry,
                                                      float* __restrict__ gW1, float* __restrict__ gb1,
                                                      float* __restrict__ gW2, float* __restrict__ gb2, int B, int H,
-                                                     int cs) {
+                                                     int cs, int T_) {
+  const int T = TM == 1 ? 1 : T_;
   extern __shared__ float hs[];                       // W1 slice [H][cs] | z [HEAD_G][2H] | dh [HEAD_G][H]
   const int K2 = 2 * H, cq = cs / 4;
   float* w1 = hs;
@@ -284,11 +302,17 @@ __global__ void __launch_bounds__(HEAD_T) k_head_bwd(const float* __restrict__ d
   const bool act = b < B;
   float* zs = zs_all + (size_t)w * K2;
   float* dh = dh_all + (size_t)w * H;
-  const float d = act ? dg[b] : 0.f;
+  float d[TM];
+#pragma unroll
+  for (int t = 0; t < TM; ++t) d[t] = (act && t < T) ? dg[(size_t)b * T + t] : 0.f;
   for (int c = lane; c < K2; c += 32) zs[c] = act ? z[(size_t)b * K2 + c] : 0.f;
   for (int n = lane; n < H; n += 32) {
     const float hv = act ? h1[(size_t)b * H + n] : 0.f;
-    dh[n] = hv > 0.f ? d * __ldg(W2 + n) : 0.f;
+    float s = d[0] * __ldg(W2 + n);
+#pragma unroll
+    for (int t = 1; t < TM; ++t)
+      if (t < T) s = fmaf(d[t], __ldg(W2 + (size_t)t * H + n), s);
+    dh[n] = hv > 0.f ? s : 0.f;
   }
   int64_t r = act ? ids[b] : 0;
   if (r < 0 || r >= n_rows) r = 0;                    // (the forward pass already raised the status flag)
@@ -335,24 +359,42 @@ __global__ void __launch_bounds__(HEAD_T) k_head_bwd(const float* __restrict__ d
     if (t != 0.f) atomicAdd(gW1 + x, t);
   }
   for (int n = threadIdx.x; n < H; n += blockDim.x) {
-    float t1 = 0.f, t2 = 0.f;
+    float t1 = 0.f, t2[TM];
+#pragma unroll
+    for (int t = 0; t < TM; ++t) t2[t] = 0.f;
 #pragma unroll
     for (int g = 0; g < HEAD_G; ++g) {
       t1 += dh_all[g * H + n];
       const int bb = blockIdx.x * HEAD_G + g;
-      if (bb < B) t2 = fmaf(dg[bb], h1[(size_t)bb * H + n], t2);
+      if (bb < B) {
+        const float hv = h1[(size_t)bb * H + n];
+#pragma unroll
+        for (int t = 0; t < TM; ++t)
+          if (t < T) t2[t] = fmaf(dg[(size_t)bb * T + t], hv, t2[t]);
+      }
     }
     if (t1 != 0.f) atomicAdd(gb1 + n, t1);
-    if (t2 != 0.f) atomicAdd(gW2 + n, t2);
+#pragma unroll
+    for (int t = 0; t < TM; ++t)
+      if (t < T && t2[t] != 0.f) atomicAdd(gW2 + (size_t)t * H + n, t2[t]);
   }
-  if (threadIdx.x == 0) {
+  if (threadIdx.x < T) {              // thread t: db2[t]
     float t = 0.f;
     for (int g = 0; g < HEAD_G; ++g) {
       const int bb = blockIdx.x * HEAD_G + g;
-      if (bb < B) t += dg[bb];
+      if (bb < B) t += dg[(size_t)bb * T + threadIdx.x];
     }
-    atomicAdd(gb2, t);
+    atomicAdd(gb2 + threadIdx.x, t);
   }
+}
+
+// The instantiation of T outputs: the next compiled bound up (1, 2, 4, 8).
+template <typename F>
+int head_dispatch(int T, F&& f) {
+  if (T == 1) return f(std::integral_constant<int, 1>());
+  if (T == 2) return f(std::integral_constant<int, 2>());
+  if (T <= 4) return f(std::integral_constant<int, 4>());
+  return f(std::integral_constant<int, 8>());
 }
 
 // Widest slice of W1 -- all of it (`full` rows or columns), halved while it does not fit -- whose stage of per_unit
@@ -436,7 +478,8 @@ int model_width(int H) {
 
 int k_of(const PertModelDesc* d, const Ws& w, int l) { return l == 0 ? d->k0 : w.Hp; }
 
-Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* base) {
+// n_out: rows of global_linear2 (its padded copy and gradient are [n_out, Hp])
+Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* base, int n_out = 1) {
   Ws w;
   memset(&w, 0, sizeof(w));
   long long off = 0;
@@ -458,7 +501,7 @@ Ws carve(const PertModelDesc* d, long long N, long long E, long long B, float* b
     t.local_w = take(Hp);
     t.g1_w = take(2 * Hp * Hp);
     t.g1_b = take(Hp);
-    t.g2_w = take(Hp);
+    t.g2_w = take(n_out * Hp);
   };
   w.Hp = model_width(d->H);
   const bool padded = w.Hp != d->H;
@@ -574,7 +617,7 @@ void append_layer_grad_segs(SegList& S, const PertModelDesc* d, const Ws& w, flo
 }
 // Hp > H: segment list of the other model tensors (Tensors) -> their zero-padded copies t (w.pp to pack the
 // parameters, w.pg to unpack the gradients); one launch, at most 4 + 3 + 2 * 7 + 5 segments
-void append_tensor_segs(SegList& S, const PertModelDesc* d, const Tensors& t, int Hp, float* base) {
+void append_tensor_segs(SegList& S, const PertModelDesc* d, const Tensors& t, int Hp, float* base, int n_out) {
   const int H = d->H;
   auto add = [&](long long src, float* dst, int rows, int src_ld, int dst_ld) {
     Seg& s = S.s[S.count++];
@@ -593,7 +636,7 @@ void append_tensor_segs(SegList& S, const PertModelDesc* d, const Tensors& t, in
   add(d->off_g1_w, t.g1_w, H, 2 * H, 2 * Hp);          // pool columns  -> [0, H)
   add(d->off_g1_w + H, t.g1_w + Hp, H, 2 * H, 2 * Hp); // entry columns -> [Hp, Hp + H)
   add(d->off_g1_b, t.g1_b, 1, H, Hp);
-  add(d->off_g2_w, t.g2_w, 1, H, Hp);
+  add(d->off_g2_w, t.g2_w, n_out, H, Hp);
 }
 
 // Auxiliary stream for the few places where independent small kernels can run beside the main chain (input prologue
@@ -646,6 +689,7 @@ int check_desc(const PertModelDesc* d) {
 }
 // dropout p in [0, 1] (NaN rejected); a training forward with p > 0 needs the {seed, step} state, and its float4 groups
 // N*Hp/4 must fit the 32-bit counter word of the mask
+int check_nout(int n_out) { return n_out >= 1 && n_out <= PERT_MAX_QUANTILES ? PERT_OK : PERT_ERR_BADARG; }
 int check_dropout(const PertModelDesc* d, long long N, int training, float p, const long long* state) {
   if (!(p >= 0.f && p <= 1.f)) return PERT_ERR_BADARG;
   if (training && p > 0.f && (!state || N * (model_width(d->H) / 4) >= (1LL << 32))) return PERT_ERR_BADARG;
@@ -674,8 +718,11 @@ int check_dropout(const PertModelDesc* d, long long N, int training, float p, co
 extern "C" {
 
 long long pert_model_workspace_bytes(const PertModelDesc* d, long long N, long long E, long long B) {
-  if (check_desc(d) || N < 0 || E < 0 || B < 0) return PERT_ERR_BADARG;
-  Ws w = carve(d, N, E, B, nullptr);
+  return pert_model_workspace_bytes_q(d, 1, N, E, B);
+}
+long long pert_model_workspace_bytes_q(const PertModelDesc* d, int n_out, long long N, long long E, long long B) {
+  if (check_desc(d) || check_nout(n_out) || N < 0 || E < 0 || B < 0) return PERT_ERR_BADARG;
+  Ws w = carve(d, N, E, B, nullptr, n_out);
   return w.total * 4;
 }
 // Test / debug aid: where a saved activation lives inside the workspace (floats from its start): which = 0 -> the input of
@@ -685,9 +732,13 @@ long long pert_model_workspace_bytes(const PertModelDesc* d, long long N, long l
 // negative PERT_ERR_*.
 long long pert_model_workspace_offset(const PertModelDesc* d, long long N, long long E, long long B, int which,
                                       int layer) {
-  if (check_desc(d) || N < 0 || E < 0 || B < 0) return PERT_ERR_BADARG;
+  return pert_model_workspace_offset_q(d, 1, N, E, B, which, layer);
+}
+long long pert_model_workspace_offset_q(const PertModelDesc* d, int n_out, long long N, long long E, long long B,
+                                        int which, int layer) {
+  if (check_desc(d) || check_nout(n_out) || N < 0 || E < 0 || B < 0) return PERT_ERR_BADARG;
   float* base = reinterpret_cast<float*>(4096);     // carve() only does pointer arithmetic
-  Ws w = carve(d, N, E, B, base);
+  Ws w = carve(d, N, E, B, base, n_out);
   if (which == 0 && layer >= 1 && layer < d->n_convs) return w.x[layer] - base;
   if (which == 1) return w.h1 - base;
   if (which == 2) return w.z - base;
@@ -706,9 +757,10 @@ long long pert_model_workspace_offset(const PertModelDesc* d, long long N, long 
   }
 }
 int pert_model_width(int H) { return model_width(H); }
-long long pert_model_packed_bytes(const PertModelDesc* d) {
-  if (check_desc(d)) return PERT_ERR_BADARG;
-  Ws w = carve(d, 0, 0, 0, nullptr);
+long long pert_model_packed_bytes(const PertModelDesc* d) { return pert_model_packed_bytes_q(d, 1); }
+long long pert_model_packed_bytes_q(const PertModelDesc* d, int n_out) {
+  if (check_desc(d) || check_nout(n_out)) return PERT_ERR_BADARG;
+  Ws w = carve(d, 0, 0, 0, nullptr, n_out);
   return w.packed_floats * 4;
 }
 
@@ -733,7 +785,21 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
                             void* workspace, long long workspace_bytes, int training, float dropout,
                             long long* dropout_state, float* global_pred, float* local_pred, int* status,
                             const PertProbe* probe, void* index_ready, const long long* live, void* stream) {
+  return pert_model_forward_q(d, 1, params, bn_running, bn_nbt, x, cat_X, entry_id, probs, pnn, batch, N, E, B, rowptr,
+                              csr_src, csr_if, csr_rpc, workspace, workspace_bytes, training, dropout, dropout_state,
+                              global_pred, local_pred, status, probe, index_ready, live, stream);
+}
+
+// n_out outputs of the global head: global_pred [B, n_out]
+int pert_model_forward_q(const PertModelDesc* d, int n_out, const float* params, float* bn_running,
+                         long long* bn_nbt, const float* x, const int64_t* cat_X, const int64_t* entry_id,
+                         const float* probs, const float* pnn, const int64_t* batch, long long N, long long E,
+                         long long B, const int* rowptr, const int* csr_src, const int* csr_if, const int* csr_rpc,
+                         void* workspace, long long workspace_bytes, int training, float dropout,
+                         long long* dropout_state, float* global_pred, float* local_pred, int* status,
+                         const PertProbe* probe, void* index_ready, const long long* live, void* stream) {
   TRY(check_desc(d));
+  TRY(check_nout(n_out));
   TRY(check_dropout(d, N, training, dropout, dropout_state));
   std::lock_guard<std::mutex> issue_lock(engine_mutex());
   if (!params || !x || !cat_X || !entry_id || !probs || !pnn || !batch || !rowptr || !workspace || !global_pred)
@@ -741,7 +807,7 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
   const bool drop = training && dropout > 0.f;
   if (E > 0 && (!csr_src || !csr_if || !csr_rpc)) return PERT_ERR_BADARG;
   float* base = (float*)workspace;
-  Ws w = carve(d, N, E, B, base);
+  Ws w = carve(d, N, E, B, base, n_out);
   if (workspace_bytes < w.total * 4) return PERT_ERR_BADARG;
   cudaStream_t st = (cudaStream_t)stream;
   const int H = w.Hp, L = d->n_convs;
@@ -759,7 +825,7 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
   if (padded) {
     SegList S;
     S.count = 0;
-    append_tensor_segs(S, d, w.pp, H, base);
+    append_tensor_segs(S, d, w.pp, H, base, n_out);
     k_pack<<<dim3(32, S.count), 256, 0, st>>>(params, base, S, nullptr, nullptr);
   }
   // the input prologue (2.) does not depend on the packed conv parameters: it runs on the auxiliary stream beside 1.
@@ -861,10 +927,14 @@ int pert_model_forward_live(const PertModelDesc* d, const float* params, float* 
   if (B > 0) {
     const int ns = head_slice(H, 2 * H, (size_t)HEAD_G * 2 * H);
     const size_t hsm = ((size_t)2 * H * ns + (size_t)HEAD_G * 2 * H) * sizeof(float);
-    TRY(head_smem((const void*)k_head_fwd, hsm));
-    k_head_fwd<<<pert_cdiv(B, HEAD_G), HEAD_T, hsm, st>>>(
-        w.pool, P.entry, d->n_entry, entry_id, P.g1_w, P.g1_b, P.g2_w, params + d->off_g2_b, w.z, w.h1, global_pred,
-        (int)B, H, ns, status);
+    TRY(head_dispatch(n_out, [&](auto tm) {
+      constexpr int TM = decltype(tm)::value;
+      TRY(head_smem((const void*)k_head_fwd<TM>, hsm));
+      k_head_fwd<TM><<<pert_cdiv(B, HEAD_G), HEAD_T, hsm, st>>>(
+          w.pool, P.entry, d->n_entry, entry_id, P.g1_w, P.g1_b, P.g2_w, params + d->off_g2_b, w.z, w.h1, global_pred,
+          (int)B, H, ns, n_out, status);
+      return PERT_OK;
+    }));
   }
   PERT_LAUNCH_CHECK();
   return PERT_OK;
@@ -891,7 +961,21 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
                              const int* csc_dst, void* workspace, long long workspace_bytes, int training,
                              float dropout, const float* d_global, const float* d_local, const PertProbe* probe,
                              const long long* live, void* stream) {
+  return pert_model_backward_q(d, 1, params, grads, cat_X, entry_id, probs, pnn, batch, N, E, B, rowptr, csr_src,
+                               csr_if, csr_rpc, colptr, csc_pos, csc_dst, workspace, workspace_bytes, training, dropout,
+                               d_global, d_local, probe, live, stream);
+}
+
+// n_out outputs of the global head: d_global [B, n_out]
+int pert_model_backward_q(const PertModelDesc* d, int n_out, const float* params, float* grads,
+                          const int64_t* cat_X, const int64_t* entry_id, const float* probs, const float* pnn,
+                          const int64_t* batch, long long N, long long E, long long B, const int* rowptr,
+                          const int* csr_src, const int* csr_if, const int* csr_rpc, const int* colptr,
+                          const int* csc_pos, const int* csc_dst, void* workspace, long long workspace_bytes,
+                          int training, float dropout, const float* d_global, const float* d_local,
+                          const PertProbe* probe, const long long* live, void* stream) {
   TRY(check_desc(d));
+  TRY(check_nout(n_out));
   if (!(dropout >= 0.f && dropout <= 1.f)) return PERT_ERR_BADARG;
   // the saved activations already carry the mask (see bn_bwd_dz4, bn.cuh): only the 1 / (1 - p) factor is needed
   const float relu_scale = (training && dropout > 0.f) ? (dropout >= 1.f ? 0.f : (float)(1.0 / (1.0 - (double)dropout)))
@@ -901,7 +985,7 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
       !d_global)
     return PERT_ERR_BADARG;
   float* base = (float*)workspace;
-  Ws w = carve(d, N, E, B, base);
+  Ws w = carve(d, N, E, B, base, n_out);
   if (workspace_bytes < w.total * 4) return PERT_ERR_BADARG;
   cudaStream_t st = (cudaStream_t)stream;
   const int H = w.Hp, L = d->n_convs;
@@ -915,10 +999,14 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
   if (B > 0) {
     const int cs = head_slice(2 * H, H, (size_t)HEAD_G * 3 * H);
     const size_t hsm = ((size_t)H * cs + (size_t)HEAD_G * 3 * H) * sizeof(float);
-    TRY(head_smem((const void*)k_head_bwd, hsm));
-    k_head_bwd<<<pert_cdiv(B, HEAD_G), HEAD_T, hsm, st>>>(
-        d_global, w.z, w.h1, P.g1_w, P.g2_w, entry_id, d->n_entry, w.dpool, G.entry, G.g1_w, G.g1_b, G.g2_w,
-        grads + d->off_g2_b, (int)B, H, cs);
+    TRY(head_dispatch(n_out, [&](auto tm) {
+      constexpr int TM = decltype(tm)::value;
+      TRY(head_smem((const void*)k_head_bwd<TM>, hsm));
+      k_head_bwd<TM><<<pert_cdiv(B, HEAD_G), HEAD_T, hsm, st>>>(
+          d_global, w.z, w.h1, P.g1_w, P.g2_w, entry_id, d->n_entry, w.dpool, G.entry, G.g1_w, G.g1_b, G.g2_w,
+          grads + d->off_g2_b, (int)B, H, cs, n_out);
+      return PERT_OK;
+    }));
   }
   // ---- pool / local head backward: g = dL/d out[L-1], written straight into the skip plane of dplanes
   float* dq = w.dplanes;
@@ -1029,7 +1117,7 @@ int pert_model_backward_live(const PertModelDesc* d, const float* params, float*
   if (padded) {   // after the join: the categorical embedding gradients are among them
     SegList S;
     S.count = 0;
-    append_tensor_segs(S, d, w.pg, H, base);
+    append_tensor_segs(S, d, w.pg, H, base, n_out);
     k_unpack<<<dim3(32, S.count), 256, 0, st>>>(grads, base, S);
   }
   PERT_LAUNCH_CHECK();

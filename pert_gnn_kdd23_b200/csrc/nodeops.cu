@@ -7,6 +7,7 @@
 #include "common.cuh"
 #include "bn.cuh"
 #include <limits.h>
+#include <string.h>
 #include <type_traits>
 
 namespace {
@@ -467,6 +468,50 @@ __global__ void k_pinball(const int64_t* __restrict__ y, const float* __restrict
   }
 }
 
+// T quantile levels, passed by value (a captured graph keeps them)
+struct Taus {
+  float v[PERT_MAX_QUANTILES];
+};
+
+// pinball loss over [B, T] (pert_pinball_loss_q): loss = mean over the B*T terms, element i = b*T + t at level t; the
+// terms, the tie rule and the reduction are k_pinball's.  Ghost graphs (b >= live[1]) get dyhat = 0 in every column.
+__global__ void k_pinball_q(const int64_t* __restrict__ y, const float* __restrict__ yhat, Taus taus, int T, int B,
+                            float grad_scale, float* __restrict__ loss, float* __restrict__ dyhat,
+                            const long long* __restrict__ live) {
+  __shared__ float red[32];
+  const int Bl = live ? (int)min((long long)B, live[1]) : B;
+  const long long n = (long long)B * T, nl = (long long)Bl * T;
+  const float inv = (float)nl;
+  float s = 0.f;
+  for (long long i = threadIdx.x; i < n; i += blockDim.x) {
+    if (i >= nl) {
+      if (dyhat) dyhat[i] = 0.f;
+      continue;
+    }
+    const long long b = i / T;
+    const int lt = (int)(i - b * T);
+    float tau = taus.v[0];
+#pragma unroll
+    for (int t = 1; t < PERT_MAX_QUANTILES; ++t)   // select, not index: the levels stay in parameter space
+      if (t == lt) tau = taus.v[t];
+    float e = (float)y[b] - yhat[i];
+    float a = tau * e, c = (tau - 1.f) * e;
+    s += fmaxf(a, c);
+    if (dyhat) {
+      float d = (a > c) ? -tau : ((a < c) ? (1.f - tau) : 0.5f * (1.f - 2.f * tau));
+      dyhat[i] = grad_scale * d / inv;
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float t = (threadIdx.x < (blockDim.x >> 5)) ? red[threadIdx.x] : 0.f;
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if (threadIdx.x == 0 && loss) *loss = t / inv;
+  }
+}
+
 // torch.optim.Adam over one flat buffer (adam_elem, common.cuh)
 __global__ void k_adam(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                        float* __restrict__ v, long long n, float b1, float b2, float eps, float wd, float step_size,
@@ -515,6 +560,73 @@ __global__ void __launch_bounds__(256) k_eval_metrics(const int64_t* __restrict_
     atomicAdd(acc + threadIdx.x, t);
   }
 }
+
+// ---- eval metrics of T quantile levels (pert_eval_metrics_q): per level the sums of k_eval_metrics (same arithmetic)
+// and the coverage count, then the count of graphs whose levels cross.  TM (1, 2, 4, 8) bounds T.
+template <int TM>
+__global__ void __launch_bounds__(256) k_eval_metrics_q(const int64_t* __restrict__ y, const float* __restrict__ yhat,
+                                                        Taus taus, int T_, int B, double* __restrict__ acc,
+                                                        const long long* __restrict__ live) {
+  constexpr int NV = 4 * TM + 1;
+  const int T = TM == 1 ? 1 : T_;
+  if (live) B = (int)min((long long)B, live[1]);
+  double v[NV];
+#pragma unroll
+  for (int k = 0; k < NV; ++k) v[k] = 0.0;
+  for (long long b = blockIdx.x * blockDim.x + threadIdx.x; b < B; b += gridDim.x * blockDim.x) {
+    const float yt = (float)y[b];
+    float prev = 0.f;
+    bool cross = false;
+#pragma unroll
+    for (int t = 0; t < TM; ++t) {
+      if (t >= T) continue;
+      const float yh = yhat[b * T + t];
+      const float tau = taus.v[t];
+      const float e = yt - yh;
+      const float ae = fabsf(yh - yt);
+      v[4 * t + 0] += (double)ae;
+      v[4 * t + 1] += (double)(ae / yt);
+      v[4 * t + 2] += (double)fmaxf(tau * e, (tau - 1.0f) * e);
+      v[4 * t + 3] += yt <= yh ? 1.0 : 0.0;
+      if (t > 0 && prev > yh) cross = true;
+      prev = yh;
+    }
+    v[4 * TM] += cross ? 1.0 : 0.0;
+  }
+  __shared__ double red[NV][8];
+#pragma unroll
+  for (int k = 0; k < NV; ++k) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], off);
+  }
+  const int w = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int k = 0; k < NV; ++k) red[k][w] = v[k];
+  }
+  __syncthreads();
+  // value k of the 4T + 1: level sums at 4t + j (t < T), the crossing count last (slot 4 TM of red)
+  if (threadIdx.x < 4 * T + 1) {
+    const int k = threadIdx.x < 4 * T ? threadIdx.x : 4 * TM;
+    double t = 0.0;
+    for (int i = 0; i < 8; ++i) t += red[k][i];
+    atomicAdd(acc + threadIdx.x, t);
+  }
+}
+
+namespace {
+// T in 1..PERT_MAX_QUANTILES, taus a host array of T levels in [0, 1], strictly increasing (NaN fails every test)
+int load_taus(const float* taus, int T, Taus* out) {
+  if (T < 1 || T > PERT_MAX_QUANTILES || !taus) return PERT_ERR_BADARG;
+  memset(out, 0, sizeof(*out));
+  for (int t = 0; t < T; ++t) {
+    if (!(taus[t] >= 0.f && taus[t] <= 1.f)) return PERT_ERR_BADARG;
+    if (t > 0 && !(taus[t] > taus[t - 1])) return PERT_ERR_BADARG;
+    out->v[t] = taus[t];
+  }
+  return PERT_OK;
+}
+}  // namespace
 
 extern "C" {
 
@@ -755,6 +867,17 @@ int pert_pinball_loss_live(const int64_t* y, const float* yhat, float tau, long 
   return PERT_OK;
 }
 
+int pert_pinball_loss_q(const int64_t* y, const float* yhat, const float* taus, int T, long long B, float grad_scale,
+                        float* loss, float* dyhat, const long long* live, void* stream) {
+  Taus tv;
+  if (load_taus(taus, T, &tv)) return PERT_ERR_BADARG;
+  if (T == 1) return pert_pinball_loss_live(y, yhat, tv.v[0], B, grad_scale, loss, dyhat, live, stream);
+  if (B <= 0 || B > INT_MAX || !y || !yhat) return PERT_ERR_BADARG;
+  k_pinball_q<<<1, 256, 0, (cudaStream_t)stream>>>(y, yhat, tv, T, (int)B, grad_scale, loss, dyhat, live);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
 int pert_adam_step(float* p, const float* g, float* m, float* v, long long n, float lr, float beta1, float beta2,
                    float eps, float weight_decay, long long step, float grad_scale, void* stream) {
   if (n < 0 || step < 1 || !p || !g || !m || !v) return PERT_ERR_BADARG;
@@ -777,6 +900,23 @@ int pert_eval_metrics_live(const int64_t* y, const float* yhat, float tau, long 
   int grid = pert_cdiv(B, 256);
   if (grid > 64) grid = 64;
   k_eval_metrics<<<grid, 256, 0, (cudaStream_t)stream>>>(y, yhat, tau, (int)B, acc, live);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+int pert_eval_metrics_q(const int64_t* y, const float* yhat, const float* taus, int T, long long B, double* acc,
+                        const long long* live, void* stream) {
+  Taus tv;
+  if (load_taus(taus, T, &tv)) return PERT_ERR_BADARG;
+  if (B < 0 || B > INT_MAX || !y || !yhat || !acc) return PERT_ERR_BADARG;
+  if (B == 0) return PERT_OK;
+  int grid = pert_cdiv(B, 256);
+  if (grid > 64) grid = 64;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (T == 1) k_eval_metrics_q<1><<<grid, 256, 0, st>>>(y, yhat, tv, T, (int)B, acc, live);
+  else if (T == 2) k_eval_metrics_q<2><<<grid, 256, 0, st>>>(y, yhat, tv, T, (int)B, acc, live);
+  else if (T <= 4) k_eval_metrics_q<4><<<grid, 256, 0, st>>>(y, yhat, tv, T, (int)B, acc, live);
+  else k_eval_metrics_q<8><<<grid, 256, 0, st>>>(y, yhat, tv, T, (int)B, acc, live);
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }

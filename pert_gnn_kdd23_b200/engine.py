@@ -123,6 +123,8 @@ class Engine:
         d.off_g1_w, d.off_g1_b = off(model.global_linear1.weight), off(model.global_linear1.bias)
         d.off_g2_w, d.off_g2_b = off(model.global_linear2.weight), off(model.global_linear2.bias)
         self.desc = d
+        # outputs of the global head (quantile levels); a one-output head calls the plain entry points
+        self.n_out = int(model.global_linear2.weight.size(0))
         self.n_convs = n_convs
         self.ws = None
         self.ws_key = (0, 0, 0)
@@ -143,7 +145,10 @@ class Engine:
     def _workspace(self, N, E, B):
         if self.ws is None or N > self.ws_key[0] or E > self.ws_key[1] or B > self.ws_key[2]:
             key = (max(N, self.ws_key[0]), max(E, self.ws_key[1]), max(B, self.ws_key[2]))
-            nbytes = self.lib.pert_model_workspace_bytes(C.byref(self.desc), *key)
+            if self.n_out == 1:
+                nbytes = self.lib.pert_model_workspace_bytes(C.byref(self.desc), *key)
+            else:
+                nbytes = self.lib.pert_model_workspace_bytes_q(C.byref(self.desc), self.n_out, *key)
             if nbytes < 0:
                 _lib.check(int(nbytes), "pert_model_workspace_bytes")
             with torch.cuda.device(self.fp.flat.device):
@@ -151,6 +156,15 @@ class Engine:
             self.ws_key = key
             self.ws_generation += 1
         return self.ws
+
+    def workspace_offset(self, which, layer, N, E, B):
+        """pert_model_workspace_offset(_q) of this engine's head: where an intermediate lives in ``ws`` (floats)."""
+        if self.n_out == 1:
+            off = self.lib.pert_model_workspace_offset(C.byref(self.desc), N, E, B, which, layer)
+        else:
+            off = self.lib.pert_model_workspace_offset_q(C.byref(self.desc), self.n_out, N, E, B, which, layer)
+        _lib.check(int(min(off, 0)), "pert_model_workspace_offset")
+        return off
 
     def active_relus(self):
         """{'bn{i}': [N,H] bool, 'head': [B,H] bool}: the entries > 0 of the saved activations of the LAST forward,
@@ -160,11 +174,9 @@ class Engine:
         H, Hp = self.desc.H, self.Hp
         out = {}
         for l in range(1, self.n_convs):
-            off = self.lib.pert_model_workspace_offset(C.byref(self.desc), N, E, B, 0, l)
-            _lib.check(int(min(off, 0)), "pert_model_workspace_offset")
+            off = self.workspace_offset(0, l, N, E, B)
             out[f"bn{l - 1}"] = self.ws[off:off + N * Hp].view(N, Hp)[:, :H] > 0
-        off = self.lib.pert_model_workspace_offset(C.byref(self.desc), N, E, B, 1, 0)
-        _lib.check(int(min(off, 0)), "pert_model_workspace_offset")
+        off = self.workspace_offset(1, 0, N, E, B)
         out["head"] = self.ws[off:off + B * Hp].view(B, Hp)[:, :H] > 0
         return out
 
@@ -203,7 +215,7 @@ class Engine:
     @_lib.on_device_of
     def forward(self, x, cat_X, entry_id, probs, pnn, batch, index: GraphIndex, training, probe=None,
                 index_ready=None, live=None):
-        """-> (global_pred [B,1], local_pred [N,1]); keeps what backward needs in the workspace.  In training the
+        """-> (global_pred [B, n_out], local_pred [N,1]); keeps what backward needs in the workspace.  In training the
         BatchNorm outputs are dropped with ``model.dropout`` (mask drawn from ``model.dropout_state()``, whose step
         this call advances on the device).  ``live``: device int64 [2] {N, B} of a batch padded by
         ``pert_batch_pad`` (the inputs are the capacity buffers); the BatchNorm statistics then count the real rows
@@ -219,7 +231,7 @@ class Engine:
         probs = probs.reshape(-1).contiguous().float()
         pnn = pnn.reshape(-1).contiguous().float()
         batch = batch.contiguous()
-        gpred = torch.empty(B, 1, device=dev, dtype=torch.float32)
+        gpred = torch.empty(B, self.n_out, device=dev, dtype=torch.float32)
         lpred = torch.empty(N, 1, device=dev, dtype=torch.float32)
         p = _lib.ptr
         args = (C.byref(self.desc), p(self.fp.flat), p(self.bn_running), p(self.bn_nbt), p(x), p(cat_X), p(entry_id),
@@ -227,7 +239,9 @@ class Engine:
                 p(index.csr_rpc), p(ws), ws.numel() * 4, int(training), p_drop, p(state), p(gpred), p(lpred),
                 p(index.status), C.byref(probe) if probe is not None else None,
                 C.c_void_p(index_ready.cuda_event) if index_ready is not None else None)
-        if live is None:
+        if self.n_out > 1:
+            rc = self.lib.pert_model_forward_q(args[0], self.n_out, *args[1:], p(live), _lib.stream())
+        elif live is None:
             rc = self.lib.pert_model_forward(*args, _lib.stream())
         else:
             rc = self.lib.pert_model_forward_live(*args, p(live), _lib.stream())
@@ -239,7 +253,7 @@ class Engine:
     @_lib.on_device_of
     def backward(self, d_global, d_local=None, grads=None, probe=None, live=None):
         """Accumulates (+=) parameter gradients into ``grads`` (default: the flat gradient buffer).  ``live``: the
-        word the forward got (padded batch); ``d_global`` must then be 0 for the ghost graphs."""
+        word the forward got (padded batch); ``d_global`` [B, n_out] must then be 0 for the ghost graphs."""
         x, cat_X, entry_id, probs, pnn, batch, index, training, N, E, B, p_drop = self._saved
         grads = self.fp.grad if grads is None else grads
         d_global = d_global.reshape(-1).contiguous().float()
@@ -251,7 +265,9 @@ class Engine:
                 E, B, p(index.rowptr), p(index.csr_src), p(index.csr_if), p(index.csr_rpc), p(index.colptr),
                 p(index.csc_pos), p(index.csc_dst), p(ws), ws.numel() * 4, int(training), p_drop, p(d_global),
                 p(d_local), C.byref(probe) if probe is not None else None)
-        if live is None:
+        if self.n_out > 1:
+            rc = self.lib.pert_model_backward_q(args[0], self.n_out, *args[1:], p(live), _lib.stream())
+        elif live is None:
             rc = self.lib.pert_model_backward(*args, _lib.stream())
         else:
             rc = self.lib.pert_model_backward_live(*args, p(live), _lib.stream())

@@ -5,6 +5,10 @@ pattern_probs, entry_id, batch) -> (global_predict [B,1], local_predict [N,1])``
 buffer names (``state_dict`` keys) and same layer-count quirk (``max(2, num_layers)`` convs,
 SURVEY.md fact 4), so ``pert_gnn.py``'s train loop (``model(...)``, ``loss.backward()``,
 ``torch.optim.Adam(model.parameters())``) runs unchanged.  All compute is libpertgnn CUDA kernels.
+
+``quantiles=(tau_1 < ... < tau_T)`` (keyword only, at most 8 levels) gives the global head T outputs:
+``global_linear2`` is ``Linear(H, T)`` and ``global_predict`` is [B, T], column t the tau_t-quantile, trained on the
+mean pinball loss over the T levels (``train``).  Without it the model is the reference's.
 """
 from __future__ import annotations
 
@@ -16,10 +20,30 @@ from .index import cached_index
 from .nn import BatchNorm1d, Linear, TransformerConv
 
 
+MAX_QUANTILES = 8     # PERT_MAX_QUANTILES
+
+
+def check_quantiles(quantiles):
+    """-> the levels as a tuple of floats: 1 to 8 of them, each in [0, 1], strictly increasing."""
+    try:
+        q = tuple(float(t) for t in quantiles)
+    except TypeError:
+        raise ValueError(f"quantiles must be a sequence of levels, got {quantiles!r}") from None
+    if not 1 <= len(q) <= MAX_QUANTILES:
+        raise ValueError(f"quantiles: 1 to {MAX_QUANTILES} levels, got {len(q)}")
+    if not all(0.0 <= t <= 1.0 for t in q):          # NaN fails too
+        raise ValueError(f"quantiles must lie in [0, 1], got {q}")
+    if any(b <= a for a, b in zip(q, q[1:])):
+        raise ValueError(f"quantiles must be strictly increasing, got {q}")
+    return q
+
+
 class SAGEDeterministic(torch.nn.Module):
     def __init__(self, in_channels, cat_dims, entry_id_max, interface_id_max, rpctype_id_max,
-                 hidden_channels, num_layers, dropout):
+                 hidden_channels, num_layers, dropout, *, quantiles=None):
         super().__init__()
+        # the levels are a constructor argument, not state: state_dict keeps the reference's keys
+        self.quantiles = None if quantiles is None else check_quantiles(quantiles)
         H = hidden_channels
         self.in_channels, self.hidden_channels = in_channels, H
         self.convs = torch.nn.ModuleList()
@@ -32,7 +56,7 @@ class SAGEDeterministic(torch.nn.Module):
         self.convs.append(TransformerConv(H, H, heads=1, edge_dim=2 * H))
         self.local_linear = Linear(H, 1)
         self.global_linear1 = Linear(2 * H, H)
-        self.global_linear2 = Linear(H, 1)
+        self.global_linear2 = Linear(H, 1 if quantiles is None else len(self.quantiles))
         self.cat_embedding = torch.nn.ModuleList([torch.nn.Embedding(n, H) for n in cat_dims])
         self.dropout = dropout
         self.entry_embeds = torch.nn.Embedding(entry_id_max + 1, H)

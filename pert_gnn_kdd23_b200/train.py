@@ -1,9 +1,13 @@
 """Train / eval step mirroring reference pert_gnn.py:191-193 (pinball loss), :213-251 (train), :254-294 (test),
 plus the data-parallel wrapper the reference lacks (SURVEY.md 8e: shard independent graphs over GPUs, ONE
 flat-buffer gradient all-reduce per step).
+
+Every step, metric and evaluation takes ``tau=None``: the levels of a quantile model (``model.quantiles``; an explicit
+``tau`` must equal them), else 0.5.  A model with T > 1 levels trains on the mean pinball loss over its T outputs.
 """
 from __future__ import annotations
 
+import ctypes as C
 import operator
 import weakref
 
@@ -14,10 +18,44 @@ import torch.distributed as dist
 from . import _lib, ops
 
 
-def torch_quantile_loss(y_test, y_hat, tau):
-    """reference pert_gnn.py:191-193."""
+def torch_quantile_loss(y_test, y_hat, tau=None):
+    """reference pert_gnn.py:191-193 (tau None: 0.5).  With a sequence of T levels, y_hat is [B, T] and the loss is the
+    mean over the B T pinball terms, column t at level tau[t]."""
+    if tau is None:
+        tau = 0.5
+    if isinstance(tau, (tuple, list)):
+        taus = torch.tensor(tau, dtype=y_hat.dtype, device=y_hat.device)
+        e = y_test.reshape(-1, 1) - y_hat
+        return torch.mean(torch.maximum(taus * e, (taus - 1) * e))
     e = y_test - y_hat
     return torch.mean(torch.maximum(tau * e, (tau - 1) * e))
+
+
+def _as_levels(tau):
+    try:
+        return (float(tau),)
+    except TypeError:
+        return tuple(float(t) for t in tau)
+
+
+def resolve_tau(model, tau=None):
+    """-> the quantile levels a step or evaluation of ``model`` uses, as a tuple.  ``tau`` None: ``model.quantiles``,
+    else (0.5,).  On a quantile model an explicit ``tau`` (a level or a sequence) must equal its levels; a model without
+    quantiles takes one level.  ``ValueError`` otherwise."""
+    q = getattr(model, "quantiles", None)
+    if tau is None:
+        return q if q is not None else (0.5,)
+    given = _as_levels(tau)
+    if q is not None and given != q:
+        raise ValueError(f"tau {given} differs from the model's quantile levels {q}")
+    if q is None and len(given) != 1:
+        raise ValueError(f"a model without quantiles has one output, got {len(given)} levels")
+    return given
+
+
+def _c_levels(levels):
+    """The levels as the host float array the _q entry points read (by value, so a captured graph keeps them)."""
+    return (C.c_float * len(levels))(*levels)
 
 
 def model_inputs(data):
@@ -450,9 +488,10 @@ def grow_embeddings(model, optimizer=None, store=None, *, entry=None, interface=
     return want
 
 
-def train_step(model, optimizer, data, tau=0.5, dp: DataParallel | None = None):
+def train_step(model, optimizer, data, tau=None, dp: DataParallel | None = None):
     """One iteration of the loop body of reference pert_gnn.py:231-247 on a device-resident Batch.
     Returns the (device) loss tensor; no host sync."""
+    levels = resolve_tau(model, tau)
     fused = isinstance(optimizer, FusedAdam)
     if fused and hasattr(model, "engine"):
         # the model must read the SAME flat buffer the optimizer updates, and its p.grad must be the views of fp.grad
@@ -465,7 +504,10 @@ def train_step(model, optimizer, data, tau=0.5, dp: DataParallel | None = None):
                 p.grad = optimizer.fp.grad[o:o + p.numel()].view_as(p)
     optimizer.zero_grad()
     global_pred, _ = model(*model_inputs(data))
-    loss = torch_quantile_loss(data.y.float(), global_pred.flatten(), tau)
+    if len(levels) == 1:
+        loss = torch_quantile_loss(data.y.float(), global_pred.flatten(), levels[0])
+    else:
+        loss = torch_quantile_loss(data.y.float(), global_pred, levels)
     loss.backward()
     if fused:
         scale = dp.all_reduce_grads(optimizer) if dp is not None else 1.0
@@ -492,9 +534,10 @@ def _side_stream(device):
 def _fused_fwd_bwd(model, optimizer: FusedAdam, data, tau, index, probe, use_index_cache=True, live=None):
     """Device work of one step up to the gradients: (index build) -> zero grads -> engine forward -> pinball loss +
     its gradient -> engine backward into the flat gradient buffer.  Returns (loss [1], index).  ``live``: the {N, B}
-    word of a padded batch (``PaddedBatch``), read by the engine and the loss."""
+    word of a padded batch (``PaddedBatch``), read by the engine and the loss.  ``tau``: as in ``resolve_tau``."""
     from .index import build_index, cached_index
 
+    tau = resolve_tau(model, tau)
     eng = _engine_of(model, optimizer)
     x, cat_X, edge_index, edge_attr, pnn, probs, entry_id, batch = model_inputs(data)
     index_ready = None
@@ -516,14 +559,19 @@ def _fused_fwd_bwd(model, optimizer: FusedAdam, data, tau, index, probe, use_ind
     with torch.no_grad():
         gpred, _ = eng.forward(x, cat_X, entry_id, probs, pnn, batch, index, model.training, probe=probe,
                                index_ready=index_ready, live=live)
-        B = gpred.size(0)
+        B, T = gpred.size(0), len(tau)
+        if gpred.size(1) != T:
+            raise ValueError(f"{T} quantile levels for a head of {gpred.size(1)} outputs")
         loss = torch.empty(1, device=gpred.device, dtype=torch.float32)
-        dy = torch.empty(B, device=gpred.device, dtype=torch.float32)
-        if live is None:
-            _lib.call("pert_pinball_loss", _lib.ptr(data.y), _lib.ptr(gpred), float(tau), B, 1.0, _lib.ptr(loss),
+        dy = torch.empty((B, T) if T > 1 else (B,), device=gpred.device, dtype=torch.float32)
+        if T > 1:
+            _lib.call("pert_pinball_loss_q", _lib.ptr(data.y), _lib.ptr(gpred), _c_levels(tau), T, B, 1.0,
+                      _lib.ptr(loss), _lib.ptr(dy), _lib.ptr(live), _lib.stream())
+        elif live is None:
+            _lib.call("pert_pinball_loss", _lib.ptr(data.y), _lib.ptr(gpred), float(tau[0]), B, 1.0, _lib.ptr(loss),
                       _lib.ptr(dy), _lib.stream())
         else:
-            _lib.call("pert_pinball_loss_live", _lib.ptr(data.y), _lib.ptr(gpred), float(tau), B, 1.0,
+            _lib.call("pert_pinball_loss_live", _lib.ptr(data.y), _lib.ptr(gpred), float(tau[0]), B, 1.0,
                       _lib.ptr(loss), _lib.ptr(dy), _lib.ptr(live), _lib.stream())
         ops.LAUNCHES["n"] += 1
         eng.backward(dy, None, probe=probe, live=live)
@@ -546,7 +594,7 @@ def _reduce_and_step(optimizer: FusedAdam, dp: DataParallel | None, loss):
     return loss
 
 
-def fused_train_step(model, optimizer: FusedAdam, data, tau=0.5, dp: DataParallel | None = None, index=None,
+def fused_train_step(model, optimizer: FusedAdam, data, tau=None, dp: DataParallel | None = None, index=None,
                      probe=None):
     """Same step as ``train_step`` but without autograd: engine forward -> pinball loss + its gradient (one
     kernel) -> engine backward into the flat gradient buffer -> (all-reduce) -> fused Adam.  5 C calls per step.
@@ -641,9 +689,9 @@ class GraphedTrainStep(_GraphCache):
     ``_GraphCache``.  The reference has no counterpart (its loop body, pert_gnn.py:231-247, launches every operator
     from Python each step)."""
 
-    def __init__(self, model, optimizer: FusedAdam, tau=0.5, dp: DataParallel | None = None, max_graphs=32):
+    def __init__(self, model, optimizer: FusedAdam, tau=None, dp: DataParallel | None = None, max_graphs=32):
         super().__init__(max_graphs)
-        self.model, self.opt, self.tau, self.dp = model, optimizer, tau, dp
+        self.model, self.opt, self.tau, self.dp = model, optimizer, resolve_tau(model, tau), dp
 
     @staticmethod
     def _key(data):
@@ -759,9 +807,9 @@ class BucketedTrainStep(_GraphCache):
     cannot pad (per-pattern probabilities only) runs eager ``fused_train_step``.  ``pad_ratio`` = sum of N_cap / sum
     of N over the padded steps."""
 
-    def __init__(self, model, optimizer: FusedAdam, tau=0.5, dp: DataParallel | None = None, max_graphs=32):
+    def __init__(self, model, optimizer: FusedAdam, tau=None, dp: DataParallel | None = None, max_graphs=32):
         super().__init__(max_graphs)
-        self.model, self.opt, self.tau, self.dp = model, optimizer, tau, dp
+        self.model, self.opt, self.tau, self.dp = model, optimizer, resolve_tau(model, tau), dp
         self._n_real = 0
         self._n_cap = 0
 
@@ -821,12 +869,18 @@ class AsyncLossReader:
 
 class EvalMetrics:
     """Device-side accumulators of the reference's eval loop (pert_gnn.py:254-294): sum |pred - y|, sum |pred - y| / y
-    and sum of the per-graph pinball terms, kept in three doubles ON THE DEVICE (``pert_eval_metrics``) so that a
-    whole epoch needs ONE D2H read (``result()``) instead of the reference's per-batch syncs."""
+    and sum of the per-graph pinball terms, kept in doubles ON THE DEVICE (``pert_eval_metrics_q``) so that a whole
+    epoch needs ONE D2H read (``result()``) instead of the reference's per-batch syncs.
 
-    def __init__(self, device, tau=0.5):
-        self.acc = torch.zeros(3, dtype=torch.float64, device=device)
-        self.tau = float(tau)
+    ``tau``: one level (None: 0.5) or a sequence of T quantile levels for predictions [B, T].  ``acc`` holds 4T + 1
+    doubles: per level the three sums and the count of graphs with y <= pred (``coverage``), then the count of graphs
+    whose levels cross (``crossing``)."""
+
+    def __init__(self, device, tau=None):
+        self.levels = (0.5,) if tau is None else _as_levels(tau)
+        self.tau = self.levels[0] if len(self.levels) == 1 else self.levels
+        self._taus = _c_levels(self.levels)
+        self.acc = torch.zeros(4 * len(self.levels) + 1, dtype=torch.float64, device=device)
         self.count = 0
 
     @property
@@ -837,41 +891,67 @@ class EvalMetrics:
         self.acc.zero_()
         self.count = 0
 
-    @_lib.on_device_of
     def update(self, y, yhat):
-        y = y.contiguous()
-        yhat = yhat.reshape(-1).contiguous().float()
-        _lib.call("pert_eval_metrics", _lib.ptr(y), _lib.ptr(yhat), self.tau, y.numel(), _lib.ptr(self.acc),
-                  _lib.stream())
-        ops.LAUNCHES["n"] += 1
+        """Adds the graphs of labels ``y`` [B] and predictions ``yhat`` [B, T] ([B] or [B, 1] at T = 1)."""
+        self.add(y, yhat)
         self.count += int(y.numel())
 
+    @_lib.on_device_of
+    def add(self, y, yhat, live=None):
+        """The sums of ``update`` without counting the graphs; ``live``: the {N, B} word of a padded batch, whose ghost
+        graphs are left out of the sums."""
+        y = y.contiguous()
+        T = len(self.levels)
+        if yhat.numel() != y.numel() * T:
+            raise ValueError(f"predictions {tuple(yhat.shape)} for {y.numel()} labels and {T} levels")
+        yhat = yhat.reshape(-1).contiguous().float()
+        _lib.call("pert_eval_metrics_q", _lib.ptr(y), _lib.ptr(yhat), self._taus, T, y.numel(), _lib.ptr(self.acc),
+                  _lib.ptr(live), _lib.stream())
+        ops.LAUNCHES["n"] += 1
+
     def result(self):
-        """-> (mae, mape, quantile loss), each divided by the number of graphs seen, like pert_gnn.py:290-294."""
+        """-> (mae, mape, quantile loss), each divided by the number of graphs seen, like pert_gnn.py:290-294; with T > 1
+        levels each is a T-tuple in level order."""
         a = self.acc.cpu()
         n = max(self.count, 1)
-        return float(a[0]) / n, float(a[1]) / n, float(a[2]) / n
+        T = len(self.levels)
+        per = [tuple(float(a[4 * t + k]) / n for t in range(T)) for k in range(3)]
+        return tuple(per) if T > 1 else tuple(p[0] for p in per)
+
+    def coverage(self):
+        """-> T floats: the fraction of the graphs seen whose label is at or below the prediction of each level."""
+        a = self.acc.cpu()
+        n = max(self.count, 1)
+        return tuple(float(a[4 * t + 3]) / n for t in range(len(self.levels)))
+
+    def crossing(self):
+        """-> the fraction of the graphs seen whose predicted levels cross (a higher level below a lower one)."""
+        return float(self.acc[4 * len(self.levels)].item()) / max(self.count, 1)
 
 
 @torch.no_grad()
-def eval_step(model, data, tau=0.5, metrics: EvalMetrics | None = None):
+def eval_step(model, data, tau=None, metrics: EvalMetrics | None = None):
     """Loop body of reference pert_gnn.py:260-289 on a device-resident Batch: engine forward (eval mode: BatchNorm
-    running statistics), then the three sums on the device.  With ``metrics`` the sums are accumulated there and
-    nothing is returned to the host; without, returns the device tensor [3] (mae, mape, quantile loss * B)."""
+    running statistics), then the sums on the device.  With ``metrics`` the sums are accumulated there and nothing is
+    returned to the host; without, returns the device tensor ``EvalMetrics.acc`` (at T = 1: mae, mape, quantile loss
+    * B, coverage count, crossing count)."""
+    levels = resolve_tau(model, tau)
     global_pred, _ = model(*model_inputs(data))
-    m = metrics if metrics is not None else EvalMetrics(global_pred.device, tau)
+    m = metrics if metrics is not None else EvalMetrics(global_pred.device, levels)
     m.update(data.y, global_pred)
     return m.acc if metrics is None else None
 
 
 @torch.no_grad()
-def evaluate(model, loader, device, tau=0.5):
-    """reference ``test(loader)`` (pert_gnn.py:254-294): model.eval(), every batch through eval_step, one read-back."""
+def evaluate(model, loader, device, tau=None):
+    """reference ``test(loader)`` (pert_gnn.py:254-294): model.eval(), every batch through eval_step, one read-back.
+    A model with T > 1 quantile levels gets (mae, mape, qloss) as T-tuples in level order."""
+    levels = resolve_tau(model, tau)
     was_training = model.training
     model.eval()
-    m = EvalMetrics(device, tau)
+    m = EvalMetrics(device, levels)
     for data in loader:
-        eval_step(model, data.to(device), tau, m)
+        eval_step(model, data.to(device), levels, m)
     model.train(was_training)
     return m.result()
 
@@ -888,22 +968,23 @@ def _padded_forward(model, eng, buf):
 
 
 @torch.no_grad()
-def evaluate_bucketed(model, loader, device, tau=0.5, max_graphs=32):
+def evaluate_bucketed(model, loader, device, tau=None, max_graphs=32):
     """``evaluate`` (same return) with every batch padded into its capacity bucket and the engine forward + metric sums
     replayed from one CUDA graph per bucket (eager on the first visit, captured on the second; graphs persist across
     calls on the same model, and a graph captured over an engine or workspace that has since been replaced is captured
     again).  Buckets beyond ``max_graphs`` and failed captures run the padded forward eagerly; a batch
     ``PaddedBatch`` cannot pad (per-pattern probabilities only) runs through ``eval_step``."""
+    levels = resolve_tau(model, tau)
     was_training = model.training
     model.eval()
     device = torch.device(device)
     if device.type == "cuda" and device.index is None:      # "cuda" -> "cuda:<current>": the state is kept per device
         device = torch.device("cuda", torch.cuda.current_device())
     st = model.__dict__.get("_bucketed_eval")
-    if st is None or st.metrics.acc.device != device or st.metrics.tau != float(tau):
-        # the graphs add into these metric sums: new sums, new graphs
+    if st is None or st.metrics.acc.device != device or st.metrics.levels != levels:
+        # the graphs add into these metric sums (and hold the levels by value): new sums, new graphs
         st = model.__dict__["_bucketed_eval"] = _GraphCache()
-        st.metrics = EvalMetrics(device, tau)
+        st.metrics = EvalMetrics(device, levels)
     st.max_graphs = max_graphs
     m = st.metrics
     m.reset()
@@ -911,16 +992,14 @@ def evaluate_bucketed(model, loader, device, tau=0.5, max_graphs=32):
 
     def run(buf):
         out = _padded_forward(model, eng, buf)
-        _lib.call("pert_eval_metrics_live", _lib.ptr(buf.y), _lib.ptr(out[0]), m.tau, buf.y.numel(),
-                  _lib.ptr(m.acc), _lib.ptr(buf.live), _lib.stream())
-        ops.LAUNCHES["n"] += 1
+        m.add(buf.y, out[0], live=buf.live)
         return out
 
     with torch.cuda.device(device):
         for data in loader:
             data = data.to(device)
             if not PaddedBatch.accepts(data):
-                eval_step(model, data, tau, m)
+                eval_step(model, data, levels, m)
                 continue
             m.count += int(data.num_graphs)
             bucket, buf = st.pad(data)
@@ -940,7 +1019,8 @@ def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, lo
     The requests are assembled on the device in slices of ``batch_size`` (``PatternStore.assemble_requests``: the
     exact resource join, or with ``asof`` the newest row at or before the request's time bucket -- with the exact join a
     missing row sets the store's status word, see ``PatternStore.check``), and every slice runs the eval-mode forward
-    padded into its capacity bucket, replayed from one CUDA graph per bucket as in ``evaluate_bucketed``.  The workspace
+    padded into its capacity bucket, replayed from one CUDA graph per bucket as in ``evaluate_bucketed``.  A model with
+    T > 1 quantile levels predicts [Q, T], column t the level-t quantile.  The workspace
     is sized once, on the host, for the largest slice.  Runs in eval mode under ``no_grad`` and restores the training
     flag; BatchNorm statistics, the dropout counter, parameters and optimizer state are left as they were.  A bad entry id
     raises ``PertGnnError`` before any launch.
@@ -983,7 +1063,8 @@ def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, lo
                 # reader of this zero column, so one buffer serves every bucket
                 st.zero_y = torch.zeros(min(bs, Q), dtype=torch.int64, device=dev)
             eng = model.engine()
-            gpred = torch.empty(Q, dtype=torch.float32, device=dev)
+            T = eng.n_out
+            gpred = torch.empty((Q, T) if T > 1 else (Q,), dtype=torch.float32, device=dev)
             lpred = torch.empty(int(node_ptr[-1]), dtype=torch.float32, device=dev) if local else None
             if Q:
                 starts = np.arange(0, Q, bs)          # the slices' sizes, exactly: host-only, no device sync
@@ -999,7 +1080,7 @@ def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, lo
                 data.y = st.zero_y[:j - i]
                 bucket, buf = st.pad(data)
                 g, loc, _ = st.cache(bucket, eng, buf.caps, lambda: _padded_forward(model, eng, buf), pin=buf)
-                gpred[i:j].copy_(g[:j - i, 0])
+                gpred[i:j].copy_(g[:j - i] if T > 1 else g[:j - i, 0])
                 if local:
                     lpred[node_ptr[i]:node_ptr[j]].copy_(loc[:node_ptr[j] - node_ptr[i], 0])
     finally:

@@ -47,7 +47,8 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
 
 // The attribute is set only while the step engine issues its chain (PdlChain, engine.cu), where every predecessor is
 // known.  Called on its own, a kernel keeps plain stream order: the caller's last kernel may have written what its
-// set-up reads.  (griddepcontrol.wait returns at once in a kernel launched without the attribute.)
+// set-up reads.  (griddepcontrol.wait returns at once in a kernel launched without the attribute.)  The same flag turns
+// on the chain's L2 eviction hints and its discards of dead scratch (sm90.cuh, DESIGN section 1).
 inline thread_local bool pert_pdl_chain = false;
 struct PdlChain {
   bool prev;

@@ -76,6 +76,7 @@ struct LbArgs {
   float relu_scale;
   const long long* live;              // rows >= live[0] are left out (null: all N)
   double* bn_sums;                    // [2H] += sum dz | sum dz*xhat
+  int l2;   // the step engine's chain (PdlChain, common.cuh): L2 hints, and dY is discarded once staged (see the loop)
 };
 
 template <int K, int KD>
@@ -97,8 +98,13 @@ __global__ void __launch_bounds__(LB_THREADS, 1) k_linear_bwd_planes(LbArgs g) {
     unsigned char* st = smem + Lay::OFF_STAGE + (i % Lay::STAGES) * Lay::STAGE;
     uint64_t* bar = &full[i % Lay::STAGES];
     mbar_arrive_tx(bar, (uint32_t)rows * (LB_H + K) * 4);
-    bulk_g2s(st, Yp + (size_t)row0 * LB_H, (uint32_t)rows * LB_H * 4, bar);
-    bulk_g2s(st + Lay::Y_BYTES, g.X + (size_t)row0 * K, (uint32_t)rows * K * 4, bar);
+    // dY: its last read.  X (and bn_x below): streamed as well, although with the BatchNorm sums the next kernel, the
+    // target pass of the conv before, reads X and bn_x again as y and x.  Keeping those 26 MB (evict_last) or leaving
+    // them at the default policy measured no faster at cfg2 (DESIGN section 7), and L2 then holds dX and the backward
+    // planes this kernel reads instead.
+    const uint64_t pol = l2_stream(g.l2);
+    bulk_g2s_hint(st, Yp + (size_t)row0 * LB_H, (uint32_t)rows * LB_H * 4, bar, pol);
+    bulk_g2s_hint(st + Lay::Y_BYTES, g.X + (size_t)row0 * K, (uint32_t)rows * K * 4, bar, pol);
   };
   if (tid == 0) {
     for (int s = 0; s < Lay::STAGES; ++s) mbar_init(&full[s], 1);
@@ -146,8 +152,9 @@ __global__ void __launch_bounds__(LB_THREADS, 1) k_linear_bwd_planes(LbArgs g) {
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       const int n = row0 + 16 * (int)rank + (tid >> 4) + 8 * j;
-      by[j] = n < n_live ? ldg4(g.X + (size_t)n * K + (tid & 15) * 4) : f4zero();
-      bx[j] = n < n_live ? ldg4(g.bn_x + (size_t)n * LB_H + (tid & 15) * 4) : f4zero();
+      const uint64_t pol = l2_stream(g.l2);
+      by[j] = n < n_live ? ldg4_hint(g.X + (size_t)n * K + (tid & 15) * 4, pol) : f4zero();
+      bx[j] = n < n_live ? ldg4_hint(g.bn_x + (size_t)n * LB_H + (tid & 15) * 4, pol) : f4zero();
     }
   };
   // dX rows 16 rank .. 16 rank + 15 of tile i = q + k + v + skip partials (warpgroup 0).  The slot of tile i is written
@@ -165,7 +172,9 @@ __global__ void __launch_bounds__(LB_THREADS, 1) k_linear_bwd_planes(LbArgs g) {
       acc = f4add(acc, ld_cluster4(map_rank(a, 1)));
       acc = f4add(acc, ld_cluster4(map_rank(a, 2)));
       acc = f4add(acc, ld_cluster4(map_rank(a, 3)));
-      st4(g.dX + (size_t)(row0 + r) * g.ldxo + c4 * 4, acc);
+      // with the BatchNorm sums the target pass reads dX next and demotes it; else (dX0, which the embedding
+      // backward reads, or the eval backward) the default policy
+      st4_hint(g.dX + (size_t)(row0 + r) * g.ldxo + c4 * 4, acc, l2_keep(g.l2 && g.bn_sums));
       if (bn && row0 + r < n_live) bn_bwd_acc4(bs1, bs2, bn_bwd_dz4(acc, y, g.relu_scale), x, bmu, brs);
     };
     if constexpr (K == LB_H && KD == LB_H) {   // 16 V = 256: the two rows of bn_fetch
@@ -183,6 +192,9 @@ __global__ void __launch_bounds__(LB_THREADS, 1) k_linear_bwd_planes(LbArgs g) {
     const float* sX = reinterpret_cast<const float*>(smem + so + Lay::Y_BYTES);
     float* P = reinterpret_cast<float*>(smem + Lay::OFF_P + (i & 1) * Lay::P_BYTES);
     mbar_wait(&full[i % Lay::STAGES], (i / Lay::STAGES) & 1);
+    // The tile's dY block (this CTA's plane) is in shared memory and nothing reads it from global memory again in the
+    // step: drop its lines from L2 without a write-back, one 128-byte line per thread of warpgroup 0.
+    if (g.l2 && wg == 0 && tid * 128 < rows * LB_H * 4) discard_l2(Yp + (size_t)row0 * LB_H + tid * 32);
     if (wg == 0) {
       // ---- data gradient of this plane: [64, H] . [H, KD]; rows past the end are computed and not stored
       const int r0 = w * 16 + gq, r1 = r0 + 8;
@@ -381,6 +393,7 @@ int clusters_for(int K, int Kd) {
 template <int K, int KD>
 int launch(const LbArgs& a0, int clusters, cudaStream_t st) {
   LbArgs a = a0;
+  a.l2 = pert_pdl_chain;
   const int ntiles = (a.N + LB_TM - 1) / LB_TM;
   a.tiles_per_cluster = (ntiles + clusters - 1) / clusters;
   const dim3 grid(4 * ((ntiles + a.tiles_per_cluster - 1) / a.tiles_per_cluster));

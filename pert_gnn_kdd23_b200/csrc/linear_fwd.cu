@@ -70,6 +70,7 @@ struct LfArgs {
   BnDropout drop;
   const long long* live;   // training on a padded batch: {N, B} of the real part (statistics over live[0] rows)
   int N;
+  int l2;              // the step engine's chain (PdlChain, common.cuh): L2 hints, see the epilogue
 };
 
 template <int K, int MODE>
@@ -88,7 +89,8 @@ __global__ void __launch_bounds__(LF_THREADS, 1) k_bn_linear_fwd_planes(LfArgs g
     const int s = i % Lay::STAGES;
     const int row0 = ((int)blockIdx.x + i * (int)gridDim.x) * LF_TM, rows = min(LF_TM, g.N - row0);
     mbar_arrive_tx(&full[s], (uint32_t)rows * K * 4);
-    bulk_g2s(smem + Lay::OFF_STAGE + s * Lay::STAGE, g.A + (size_t)row0 * K, (uint32_t)rows * K * 4, &full[s]);
+    bulk_g2s_hint(smem + Lay::OFF_STAGE + s * Lay::STAGE, g.A + (size_t)row0 * K, (uint32_t)rows * K * 4, &full[s],
+                  l2_stream(g.l2));   // out[l - 1] (x[0]): last read in the forward
   };
   if (tid == 0) {
     for (int s = 0; s < Lay::STAGES; ++s) mbar_init(&full[s], 1);
@@ -171,8 +173,9 @@ __global__ void __launch_bounds__(LF_THREADS, 1) k_bn_linear_fwd_planes(LfArgs g
           v0 = bn_dropout4(v0, (uint32_t)(row0 + r0) * (LF_H / 4) + (uint32_t)(c >> 2), g.drop, key);
           v1 = bn_dropout4(v1, (uint32_t)(row0 + r1) * (LF_H / 4) + (uint32_t)(c >> 2), g.drop, key);
         }
-        if (r0 < rows) st4(g.x_out + (size_t)(row0 + r0) * LF_H + c, v0);
-        if (r1 < rows) st4(g.x_out + (size_t)(row0 + r1) * LF_H + c, v1);
+        const uint64_t pol = l2_stream(g.l2);   // x[l]: next read by the backward
+        if (r0 < rows) st4_hint(g.x_out + (size_t)(row0 + r0) * LF_H + c, v0, pol);
+        if (r1 < rows) st4_hint(g.x_out + (size_t)(row0 + r1) * LF_H + c, v1, pol);
       }
       split4({v0.x, v1.x, v0.y, v1.y}, ah[q & 1][0], al[q & 1][0]);   // K-step 2q:     columns 4t, 4t+1
       split4({v0.z, v1.z, v0.w, v1.w}, ah[q & 1][1], al[q & 1][1]);   // K-step 2q + 1: columns 4t+2, 4t+3
@@ -198,15 +201,19 @@ __global__ void __launch_bounds__(LF_THREADS, 1) k_bn_linear_fwd_planes(LfArgs g
       wgmma_commit();
     }
     wgmma_wait0();
-    // ---- epilogue: + bias, two adjacent columns per store (four lanes cover one 32-byte sector of a row)
+    // ---- epilogue: + bias, two adjacent columns per store (four lanes cover one 32-byte sector of a row).  In the
+    // chain the k and v planes are kept in L2: the conv forward copies their tiles before it computes anything, while
+    // it reads the q and skip rows one node at a time.  All four (52 MB at cfg2) would not fit the 50 MB L2.
+    const uint64_t keep = l2_keep(g.l2), norm = l2_evict_normal();
 #pragma unroll
     for (int j = 0; j < LF_NC / 2; j += 2) {
       const int col = (j / 16) * 32 + acc_col(j & 15, tq);
       const int r = (j & 2) ? r1 : r0;
       if (r >= rows) continue;
       const float2 b = *reinterpret_cast<const float2*>(par + col);
-      *reinterpret_cast<float2*>(g.planes + (size_t)(col >> 6) * g.pz + (size_t)(row0 + r) * LF_H + (col & 63)) =
-          make_float2(d[j] + b.x, d[j + 1] + b.y);
+      const int plane = col >> 6;
+      st2_hint(g.planes + (size_t)plane * g.pz + (size_t)(row0 + r) * LF_H + (col & 63),
+               make_float2(d[j] + b.x, d[j + 1] + b.y), plane == 1 || plane == 2 ? keep : norm);
     }
   }
 }
@@ -246,7 +253,9 @@ int launch(const LfArgs& a, cudaStream_t st) {
   if (per_sm <= 0) return PERT_ERR_UNSUPPORTED;
   const int ntiles = (a.N + LF_TM - 1) / LF_TM;
   const int grid = min(ntiles, PERT_NUM_SMS * per_sm);
-  const cudaError_t e = launch_pdl(k_bn_linear_fwd_planes<K, MODE>, grid, LF_THREADS, LfLayout<K>::SMEM, st, a);
+  LfArgs b = a;
+  b.l2 = pert_pdl_chain;
+  const cudaError_t e = launch_pdl(k_bn_linear_fwd_planes<K, MODE>, grid, LF_THREADS, LfLayout<K>::SMEM, st, b);
   return e == cudaSuccess ? PERT_OK : (int)e;
 }
 

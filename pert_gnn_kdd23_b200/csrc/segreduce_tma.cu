@@ -10,6 +10,7 @@
 // Algorithmic bytes: 4*E*H (msg, read once) + 4*(N+1) (rowptr) + 4*N*H (out).  A tile whose rows exceed the stage
 // capacity (very high in-degree) is reduced straight from global memory instead.
 #include "common.cuh"
+#include "sm90.cuh"
 #include <type_traits>
 
 namespace {
@@ -25,33 +26,6 @@ struct Ring {
 };
 constexpr int CONS_WARPS = 8;
 constexpr int THREADS = (CONS_WARPS + 1) * 32;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(phase)
-        : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
 
 struct StageHdr {
   int ptr[TN + 1];   // rowptr slice of the tile
@@ -76,7 +50,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_segreduce_stream(const float* __
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], CONS_WARPS);
     }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbar_init();
   }
   __syncthreads();
   if (warp == CONS_WARPS) {

@@ -1,6 +1,6 @@
-// Hopper (sm_90a) building blocks shared by the tensor-core GEMMs (gemm_tc.cu, linear_bwd.cu, linear_fwd.cu): wgmma
-// (m64nNk8, kind tf32) with the 3xTF32 hi / lo split, shared-memory matrix descriptors, mbarriers, bulk copies and
-// cluster barriers.
+// Hopper (sm_90a) building blocks shared by the tensor-core GEMMs (gemm_tc.cu, linear_bwd.cu, linear_fwd.cu) and the
+// bulk-copy kernels (tconv_tile.cu, segreduce_tma.cu): wgmma (m64nNk8, kind tf32) with the 3xTF32 hi / lo split,
+// shared-memory matrix descriptors, mbarriers, bulk copies, L2 eviction policies and cluster barriers.
 //
 // Operand conventions (see gemm_tc.cu for how each kernel stages its operands):
 //   A: registers in the wgmma A-fragment layout: a thread of warp w holds rows 16w + g and 16w + g + 8 (g = lane / 4)
@@ -198,11 +198,65 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
         : "memory");
   } while (!ok);
 }
+// dst / src 16-byte aligned, bytes % 16 == 0
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                    smem_u32(dst)),
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
+}
+
+// ---- L2 eviction priority.  A policy (createpolicy) gives the lines an access touches an eviction priority in L2:
+// evict_last lines are replaced after every other line, evict_first lines before them, evict_normal is what an access
+// without a hint gets.  A fraction f < 1 marks only that share of the lines (chosen by address).  A hinted access
+// re-marks a line that is already in L2, so a consumer's last read of a handoff demotes it again.
+__device__ __forceinline__ uint64_t l2_evict_last(float f = 1.f) {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, %1;" : "=l"(p) : "f"(f));
+  return p;
+}
+__device__ __forceinline__ uint64_t l2_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ uint64_t l2_evict_normal() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+// the policy of a hinted access in a kernel whose hints are switched on by `on`, else the default policy
+__device__ __forceinline__ uint64_t l2_keep(int on, float f = 1.f) { return on ? l2_evict_last(f) : l2_evict_normal(); }
+__device__ __forceinline__ uint64_t l2_stream(int on) { return on ? l2_evict_first() : l2_evict_normal(); }
+// hinted forms of the accesses of the conv chain: 16-byte read-only load, 16- and 8-byte stores, 1-D bulk copy
+__device__ __forceinline__ float4 ldg4_hint(const float* p, uint64_t pol) {
+  float4 v;
+  asm volatile("ld.global.nc.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ void st4_hint(float* p, float4 v, uint64_t pol) {
+  asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z),
+               "f"(v.w), "l"(pol)
+               : "memory");
+}
+__device__ __forceinline__ void st2_hint(float* p, float2 v, uint64_t pol) {
+  asm volatile("st.global.L2::cache_hint.v2.f32 [%0], {%1, %2}, %3;" ::"l"(p), "f"(v.x), "f"(v.y), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void bulk_g2s_hint(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t pol) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+          smem_u32(dst)),
+      "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
+      : "memory");
+}
+// Drops the 128-byte L2 line that starts at p without writing it back: its contents are undefined afterwards.  Only for
+// dead scratch, after its last read has completed.  It counts as a global write (pdl_wait first, common.cuh).  A p that
+// is not 128-byte aligned does nothing: the line would hold bytes of a live neighbour (a workspace the caller aligned to
+// 16 bytes only).
+__device__ __forceinline__ void discard_l2(const void* p) {
+  if (((uintptr_t)p & 127) == 0) asm volatile("discard.global.L2 [%0], 128;" ::"l"(p) : "memory");
 }
 
 // ---- thread-block clusters and distributed shared memory

@@ -17,6 +17,7 @@
 // sized graphs the tile is a whole number of graphs (no cut edges).
 #include "bn.cuh"
 #include "common.cuh"
+#include "sm90.cuh"
 #include <type_traits>
 
 namespace {
@@ -24,35 +25,6 @@ namespace {
 // CTA size: 512 threads when two CTAs share an SM (tiles <= ~113 KB), 1024 when a tile needs the whole SM's shared memory
 // (the same 32 resident warps per SM either way; 64 registers per thread in both)
 
-// ---------------------------------------------------------------- mbarrier / bulk-copy PTX
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(phase)
-        : "memory");
-  } while (!ok);
-}
-// global -> shared bulk copy (TMA, 1-D): dst/src 16-byte aligned, bytes % 16 == 0
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ float ex2(float x) {
   float y;
@@ -82,6 +54,8 @@ struct TileArgs {
   int pdl;             // launched as a dependent of a chain kernel (launch_pdl inside a PdlChain, common.cuh): the
                        // index set-up runs before the plane copies, which wait for the predecessor.  Else the copies
                        // are issued first and overlap the set-up.
+  int l2;              // the step engine's chain (PdlChain, common.cuh): L2 eviction hints on the handoffs between the
+                       // chain's kernels, and discards of dead scratch (see l2_keep / l2_stream)
   float* g_out;        // bwd_dst with BN: g rows, written (the plane `g` of the source pass)
 };
 
@@ -173,21 +147,28 @@ __device__ __forceinline__ void stage_index(const Smem& S, const int* nodeptr, i
     S.ord[atomicAdd(&s_hist[32 - min(S.ptr[x + 1] - S.ptr[x], 32)], 1)] = (unsigned short)x;
   __syncthreads();
 }
+// L2 policies of the chain's handoffs (TileArgs::l2): l2_keep on rows the next kernel reads (out in the forward; dq, g,
+// dk, dv in the backward), l2_stream on a last read (the planes in the forward's conv, the forward activations in the
+// backward).  The four backward planes together (52 MB at cfg2) exceed the 50 MB L2, so only a share KEEP_DPLANES of
+// their lines is kept; the node-linear backward reads them with evict_first.
+constexpr float KEEP_DPLANES = 0.6f;
+
 // the two operand tiles (planes the preceding kernels wrote: after pdl_wait), completion on S.bar (the caller's
-// mbar_wait).  The mbarrier is initialised by the caller.
+// mbar_wait), with L2 policies pol_a / pol_b.  The mbarrier is initialised by the caller.
 template <int H>
-__device__ __forceinline__ void stage_tiles(const Smem& S, const float* pa, const float* pb, int n0, int nt, int tid) {
+__device__ __forceinline__ void stage_tiles(const Smem& S, const float* pa, const float* pb, int n0, int nt, int tid,
+                                            uint64_t pol_a, uint64_t pol_b) {
   if (tid == 0) {
     const uint32_t tile_bytes = (uint32_t)nt * H * 4;
-    mbar_expect_tx(S.bar, 2 * tile_bytes);
-    bulk_g2s(S.ta, pa + (size_t)n0 * H, tile_bytes, S.bar);
-    bulk_g2s(S.tb, pb + (size_t)n0 * H, tile_bytes, S.bar);
+    mbar_arrive_tx(S.bar, 2 * tile_bytes);
+    bulk_g2s_hint(S.ta, pa + (size_t)n0 * H, tile_bytes, S.bar, pol_a);
+    bulk_g2s_hint(S.tb, pb + (size_t)n0 * H, tile_bytes, S.bar, pol_b);
   }
 }
 __device__ __forceinline__ void tile_barrier_init(const Smem& S, int tid) {
   if (tid == 0) {
     mbar_init(S.bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbar_init();
   }
   __syncthreads();
 }
@@ -260,11 +241,18 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
 #pragma unroll
     for (int u = 0; u < VPL; ++u) v[u] = ldg4(base + row * H + (lig + u * LPR) * 4);
   };
+  // q and skip rows: read once here.  The backward's next read of q comes after the rest of the forward, when the row
+  // would have left L2 anyway.
+  auto ldrow_stream = [&](const float* base, size_t row, float4 (&v)[VPL]) {
+    const uint64_t pol = l2_stream(a.l2);
+#pragma unroll
+    for (int u = 0; u < VPL; ++u) v[u] = ldg4_hint(base + row * H + (lig + u * LPR) * 4, pol);
+  };
   int n0, nt;
   cta_tile(a, n0, nt);
   if (nt <= 0) return;                         // uniform across the CTA
   tile_barrier_init(S, tid);
-  if (!a.pdl) stage_tiles<H>(S, a.k, a.v, n0, nt, tid);
+  if (!a.pdl) stage_tiles<H>(S, a.k, a.v, n0, nt, tid, l2_stream(a.l2), l2_stream(a.l2));
   stage_index<NT>(S, a.rowptr, n0, nt, tid);
   const int e_lo = S.ptr[0];
   const int ne_c = min(S.ptr[nt] - e_lo, a.edge_cap);
@@ -289,7 +277,7 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
   // the set-up above read the graph index only; the planes are the node linear's output
   pdl_wait();
   pdl_trigger();
-  if (a.pdl) stage_tiles<H>(S, a.k, a.v, n0, nt, tid);
+  if (a.pdl) stage_tiles<H>(S, a.k, a.v, n0, nt, tid, l2_stream(a.l2), l2_stream(a.l2));
   mbar_wait(S.bar, 0);
 
   // node slots are handed out in descending-degree order (S.ord); the q row is requested one node ahead, the skip row
@@ -299,7 +287,7 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
   float4 q_n[VPL];
 #pragma unroll
   for (int u = 0; u < VPL; ++u) q_n[u] = f4zero();
-  if (slot < nt) ldrow(a.q, (size_t)(n0 + loc), q_n);
+  if (slot < nt) ldrow_stream(a.q, (size_t)(n0 + loc), q_n);
   auto run = [&](auto fast_c) {
     constexpr bool FAST = decltype(fast_c)::value;
     for (; slot - grp < nt; slot += GPC) {   // warp-uniform: the warp's first group still has a node
@@ -311,12 +299,12 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
         q[u] = f4scale(qscale, q_n[u]);
         skip[u] = f4zero();
       }
-      if (valid && a.s) ldrow(a.s, (size_t)i, skip);
+      if (valid && a.s) ldrow_stream(a.s, (size_t)i, skip);
       const int p0 = valid ? ldsi(sa.ptr + loc * 4) : 0;
       const int p1 = valid ? ldsi(sa.ptr + loc * 4 + 4) : 0;
       if (slot + GPC < nt) {
         loc = ldsu16(sa.ord + (slot + GPC) * 2);
-        ldrow(a.q, (size_t)(n0 + loc), q_n);
+        ldrow_stream(a.q, (size_t)(n0 + loc), q_n);
       }
       const int deg = p1 - p0;
       const int degmax = __reduce_max_sync(0xffffffffu, deg);
@@ -408,14 +396,19 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
         // padded batch: only the real nodes (below live[0]) enter the statistics.  Read per node, not kept in a
         // register across the edge loop (a volatile load is not hoisted; it hits L1 after the first node)
         const bool counted = !a.live || i < *reinterpret_cast<const volatile long long*>(a.live);
+        // the next node linear reads out, and demotes it.  Without bn_acc (the last conv, or eval) the reader is the
+        // pool, which gives no hint: the default policy, so that no evict_last line outlives the step.
+        const uint64_t keep = l2_keep(a.l2 && a.bn_acc);
 #pragma unroll
         for (int u = 0; u < VPL; ++u) {
           const float4 o = f4add(f4scale(invZ, acc[u]), skip[u]);
-          st4(a.out + (size_t)i * H + (lig + u * LPR) * 4, o);
+          st4_hint(a.out + (size_t)i * H + (lig + u * LPR) * 4, o, keep);
           if (counted) bsum[u] = f4add(bsum[u], o);
         }
       }
       __syncwarp();
+      // the skip row is dead once the node's group has used it (the backward never reads it: its gradient is g)
+      if (a.l2 && valid && a.s && lig < H / 32) discard_l2(a.s + (size_t)i * H + lig * 32);
       for (int p = p0 + lig; p < p1; p += LPR) {
         const int le = p - e_lo;
         const float s = (FAST || le < ne_s) ? ldsf(sa.f0 + le * 4) : a.alpha[p];
@@ -483,9 +476,9 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_fwd(TileArgs a)
 // BN: g is not read but computed from the rows of dx, y and x of the node (the expressions of k_bn_bwd_apply, bn.cuh)
 // and written to g_out for the source pass and the node-linear backward.  The dx row is fetched one node ahead in
 // registers as g is otherwise, the y and x rows one node ahead into L2 only: three register rows held through the edge
-// loop spill 76 bytes per thread at 64 registers, this form 20 (nvcc 12.9, -Xptxas -v), and it measured 3 us faster
-// per launch at cfg2.  This replaces the k_bn_bwd_apply pass; CTA 0 adds the column sums into dgamma / dbeta as that
-// pass's block 0 did.
+// loop spill 76 bytes per thread at 64 registers, this form 20 (0 with the L2-hinted loads; nvcc 12.9, -Xptxas -v), and
+// it measured 3 us faster per launch at cfg2.  This replaces the k_bn_bwd_apply pass; CTA 0 adds the column sums into
+// dgamma / dbeta as that pass's block 0 did.
 template <int LPR, int VPL, bool HAS_E, int NT, bool BN>
 __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArgs a) {
   constexpr int H = 4 * LPR * VPL;
@@ -505,7 +498,8 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
   cta_tile(a, n0, nt);
   if (nt <= 0) return;                         // uniform across the CTA
   tile_barrier_init(S, tid);
-  stage_tiles<H>(S, a.k, a.v, n0, nt, tid);    // the forward's k and v planes: no need to wait for them
+  // the forward's k and v planes: no need to wait for them.  Their last read.
+  stage_tiles<H>(S, a.k, a.v, n0, nt, tid, l2_stream(a.l2), l2_stream(a.l2));
   stage_index<NT>(S, a.rowptr, n0, nt, tid);
   const int e_lo = S.ptr[0];
   const int ne_c = min(S.ptr[nt] - e_lo, a.edge_cap);
@@ -546,7 +540,9 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
   for (int u = 0; u < VPL; ++u) g_n[u] = f4zero();
   // BN: the dx row of the next node into g_n, its y and x rows only into L2; they are read where g is formed
   auto fetch_bn = [&](int row) {
-    ldrow(fresh(a.bn.dx), (size_t)row, g_n);
+    const uint64_t pol = l2_stream(a.l2);   // dx: its last read
+#pragma unroll
+    for (int u = 0; u < VPL; ++u) g_n[u] = ldg4_hint(fresh(a.bn.dx) + (size_t)row * H + (lig + u * LPR) * 4, pol);
 #pragma unroll
     for (int u = 0; u < VPL; ++u) {
       prefetch_l2(fresh(a.bn.y) + (size_t)row * H + (lig + u * LPR) * 4);
@@ -573,7 +569,9 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
         for (int u = 0; u < VPL; ++u) {
           const int c = (lig + u * LPR) * 4;
           if (i < n_live) {
-            const float4 y = ldg4(fresh(a.bn.y) + (size_t)i * H + c), x = ldg4(fresh(a.bn.x) + (size_t)i * H + c);
+            const uint64_t pol = l2_stream(a.l2);   // forward activations: their last read
+            const float4 y = ldg4_hint(fresh(a.bn.y) + (size_t)i * H + c, pol);
+            const float4 x = ldg4_hint(fresh(a.bn.x) + (size_t)i * H + c, pol);
             const double2* sp = reinterpret_cast<const double2*>(fresh(a.bn.sums) + c);
             const double2 a0 = __ldg(sp), a1 = __ldg(sp + 1), b0 = __ldg(sp + H / 2), b1 = __ldg(sp + H / 2 + 1);
             g[u] = bn_bwd_dx4(bn_bwd_dz4(g[u], y, a.bn.relu_scale), x, ldg4(fresh(a.bn.mean) + c),
@@ -583,7 +581,7 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
           } else {
             g[u] = f4zero();
           }
-          if (valid) st4(const_cast<float*>(fresh(a.g_out)) + (size_t)i * H + c, g[u]);
+          if (valid) st4_hint(const_cast<float*>(fresh(a.g_out)) + (size_t)i * H + c, g[u], l2_keep(a.l2, KEEP_DPLANES));
         }
       }
       const int p0 = valid ? ldsi(sa.ptr + loc * 4) : 0;
@@ -681,6 +679,9 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
       }
       const float sumS = (sumW - dot * sumA) * a.inv_sqrt_c;
       __syncwarp();
+      // BN: the group has formed g from the node's dx row, which nothing reads after this pass (dX0, which the
+      // embedding backward reads, never comes here)
+      if (BN && a.l2 && valid && lig < H / 32) discard_l2(a.bn.dx + (size_t)i * H + lig * 32);
       for (int p = p0 + lig; p < p1; p += LPR) {
         const int le = p - e_lo;
         const float dc = (FAST || le < ne_s) ? ldsf(sa.f1 + le * 4) : a.dsp[p];
@@ -688,12 +689,13 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_dst(TileArg
         a.dsp[p] = al * (dc - dot) * a.inv_sqrt_c;
       }
       if (valid) {
+        const uint64_t keep = l2_keep(a.l2, KEEP_DPLANES);
 #pragma unroll
         for (int u = 0; u < VPL; ++u) {
           float4 dq;
           dq.x = (P[u].x - dot * Q[u].x) * a.inv_sqrt_c; dq.y = (P[u].y - dot * Q[u].y) * a.inv_sqrt_c;
           dq.z = (P[u].z - dot * Q[u].z) * a.inv_sqrt_c; dq.w = (P[u].w - dot * Q[u].w) * a.inv_sqrt_c;
-          st4(a.out + (size_t)i * H + (lig + u * LPR) * 4, dq);
+          st4_hint(a.out + (size_t)i * H + (lig + u * LPR) * 4, dq, keep);
         }
       }
       if (HAS_E && a.rpc_ws && valid && lig < RPC_FAST) {
@@ -733,7 +735,8 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
   cta_tile(a, n0, nt);
   if (nt <= 0) return;                         // uniform across the CTA
   tile_barrier_init(S, tid);
-  if (!a.pdl) stage_tiles<H>(S, a.g, a.q, n0, nt, tid);
+  // g stays for the node-linear backward; this is q's last read
+  if (!a.pdl) stage_tiles<H>(S, a.g, a.q, n0, nt, tid, l2_keep(a.l2, KEEP_DPLANES), l2_stream(a.l2));
   stage_index<NT>(S, a.colptr, n0, nt, tid);   // targets of a node's out-edges live in the same graph
   const int c_lo = S.ptr[0];
   const int ne_c = min(S.ptr[nt] - c_lo, a.edge_cap);
@@ -763,7 +766,7 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
   pdl_wait();
   pdl_trigger();
   if (a.pdl) {
-    stage_tiles<H>(S, a.g, a.q, n0, nt, tid);
+    stage_tiles<H>(S, a.g, a.q, n0, nt, tid, l2_keep(a.l2, KEEP_DPLANES), l2_stream(a.l2));
     for (int x = tid; x < ne_c; x += NT) S.f1[x] = __ldg(a.dsp + __float_as_int(S.f1[x]));   // this thread's slots
     __syncthreads();
   }
@@ -834,10 +837,11 @@ __global__ void __launch_bounds__(NT, NT == 1024 ? 1 : 2) k_tile_bwd_src(TileArg
         }
       }
       if (valid) {
+        const uint64_t keep = l2_keep(a.l2, KEEP_DPLANES);
 #pragma unroll
         for (int u = 0; u < VPL; ++u) {
-          st4(a.dk + (size_t)jn * H + (lig + u * LPR) * 4, dk[u]);
-          st4(a.dv + (size_t)jn * H + (lig + u * LPR) * 4, dv[u]);
+          st4_hint(a.dk + (size_t)jn * H + (lig + u * LPR) * 4, dk[u], keep);
+          st4_hint(a.dv + (size_t)jn * H + (lig + u * LPR) * 4, dv[u], keep);
         }
       }
     }
@@ -944,6 +948,7 @@ int launch_k(K kernel, int grid, int threads, size_t bytes, const TileArgs& a, c
   if (rc) return rc;
   TileArgs b = a;
   b.pdl = pert_pdl_chain;
+  b.l2 = pert_pdl_chain;
   const cudaError_t e = launch_pdl(kernel, grid, threads, bytes, st, b);
   return e == cudaSuccess ? PERT_OK : (int)e;
 }

@@ -58,7 +58,8 @@ extern "C" {
  * (the conv forward with the BatchNorm statistics of its output); pert_flat_grow (relayout of the flat parameter and
  * optimizer buffers when embedding tables grow); pert_model_workspace_bytes_q, pert_model_packed_bytes_q,
  * pert_model_workspace_offset_q, pert_model_forward_q, pert_model_backward_q, pert_pinball_loss_q, pert_eval_metrics_q
- * (a global head with several quantile outputs).  An additive entry point leaves the version as it is. */
+ * (a global head with several quantile outputs); pert_calib_workspace_bytes, pert_calib_offsets, pert_calib_apply
+ * (conformal calibration of the quantile levels).  An additive entry point leaves the version as it is. */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -317,6 +318,34 @@ int pert_pinball_loss_q(const int64_t* y, const float* yhat, const float* taus, 
                         float* loss, float* dyhat, const long long* live, void* stream);
 int pert_eval_metrics_q(const int64_t* y, const float* yhat, const float* taus, int T, long long B, double* acc,
                         const long long* live, void* stream);
+
+/* ---- conformal calibration of the quantile levels (csrc/calib.cu) ------------------------------------------------
+ * Split-conformal offsets per group (entry id) and level from n held-out graphs: labels y [n] int64, predictions
+ * yhat [n, T] fp32 row-major, group [n] int64 (NULL: every graph in the global group only).  taus is a HOST array of T
+ * doubles, read during the call.  Outputs, G + 1 rows (G = n_groups), row G the global group of all n graphs:
+ *   off [(G+1) T] fp32, count [G+1] int32 (graphs per group), own [(G+1) T] int8 (1: the group's own offset).
+ * Score s = (float)y - yhat in fp32 (the conversion of pert_eval_metrics_q's coverage test), -0 canonicalised to +0.
+ * For a group of n_g graphs at level tau, k = max(1, ceil((n_g + 1) tau)) in double; the group's own offset is used iff
+ * k <= n_g and n_g >= min_count, and is then exactly the k-th smallest score of the group (an element of the score
+ * array, bit for bit); otherwise the group gets row G's offset.  Row G follows the rule over all n graphs (min_count
+ * does not apply to it).  Deterministic: integer histograms only, no device-to-host read inside the call.
+ * On the device, a NaN or infinite score or a group id outside [0, G) writes PERT_ERR_RANGE to status (the outputs
+ * are then undefined).  PERT_ERR_BADARG, before any CUDA call, for NULL pointers (group excepted), n < 1, n T >= 2^31,
+ * T outside 1..PERT_MAX_QUANTILES, taus NaN, outside [0, 1] or not strictly increasing, n_groups < 0 or >= INT_MAX,
+ * min_count < 1, a level at which row G cannot be formed (k > n, e.g. tau = 1) and a workspace below
+ * pert_calib_workspace_bytes(n, T, n_groups) (-1 for sizes the fit refuses). */
+long long pert_calib_workspace_bytes(long long n, int T, long long n_groups);
+int pert_calib_offsets(const int64_t* y, const float* yhat, const int64_t* group, long long n, int T,
+                       const double* taus, long long n_groups, long long min_count, float* off, int* count,
+                       int8_t* own, void* workspace, long long workspace_bytes, int* status, void* stream);
+/* In place on yhat [Q, T]: yhat[q, t] += off[g, t] in fp32, g = group[q]; an id outside [0, n_rows - 1) (an entry the
+ * calibration never saw) or group = NULL reads the global row n_rows - 1.  off = NULL adds nothing.  monotone != 0 then
+ * replaces each row by its running max over t (removes crossing levels; it only raises predictions).  live as in
+ * pert_eval_metrics_q: rows q >= live[1] (ghost graphs of a padded batch) are left untouched.  PERT_ERR_BADARG, before
+ * any CUDA call, for Q < 0, Q T >= 2^31, T outside 1..PERT_MAX_QUANTILES, yhat NULL with Q > 0, and off with n_rows
+ * outside 1..INT_MAX.  Nothing is launched when Q = 0 or when off = NULL and monotone = 0. */
+int pert_calib_apply(float* yhat, const int64_t* group, long long Q, int T, const float* off, long long n_rows,
+                     int monotone, const long long* live, void* stream);
 
 /* torch.optim.Adam step (pert_gnn.py:343,247) over one flat parameter buffer; g is scaled by grad_scale, weight_decay
  * is L2 added to the scaled gradient (not AdamW's decoupled decay).  The bias corrections lr / (1 - beta1^step) and

@@ -144,6 +144,10 @@ SIGNATURES = {
                                   P, P]),
     "pert_pinball_loss_q": (I, [P, P, P, I, LL, F, P, P, P, P]),
     "pert_eval_metrics_q": (I, [P, P, P, I, LL, P, P, P]),
+    # conformal calibration of the quantile levels (csrc/calib.cu; taus: host array of doubles)
+    "pert_calib_workspace_bytes": (LL, [LL, I, LL]),
+    "pert_calib_offsets": (I, [P, P, P, LL, I, P, LL, LL, P, P, P, P, LL, P, P]),
+    "pert_calib_apply": (I, [P, P, LL, I, P, LL, I, P, P]),
 }
 MAX_QUANTILES = 8                                       # PERT_MAX_QUANTILES
 

@@ -8,6 +8,7 @@ Every step, metric and evaluation takes ``tau=None``: the levels of a quantile m
 from __future__ import annotations
 
 import ctypes as C
+import math
 import operator
 import weakref
 
@@ -930,13 +931,18 @@ class EvalMetrics:
 
 
 @torch.no_grad()
-def eval_step(model, data, tau=None, metrics: EvalMetrics | None = None):
+def eval_step(model, data, tau=None, metrics: EvalMetrics | None = None, calibration=None, monotone=False):
     """Loop body of reference pert_gnn.py:260-289 on a device-resident Batch: engine forward (eval mode: BatchNorm
     running statistics), then the sums on the device.  With ``metrics`` the sums are accumulated there and nothing is
     returned to the host; without, returns the device tensor ``EvalMetrics.acc`` (at T = 1: mae, mape, quantile loss
-    * B, coverage count, crossing count)."""
-    levels = resolve_tau(model, tau)
+    * B, coverage count, crossing count).  ``calibration`` / ``monotone``: as in ``predict``, applied to the predictions
+    before the sums."""
+    levels = _calibrated_levels(model, tau, calibration)
+    _calibration_on(calibration, data.entry_id.device)
     global_pred, _ = model(*model_inputs(data))
+    if calibration is not None or monotone:
+        global_pred = global_pred.contiguous()
+        _calib_apply(global_pred, data.entry_id, calibration.offsets if calibration is not None else None, monotone)
     m = metrics if metrics is not None else EvalMetrics(global_pred.device, levels)
     m.update(data.y, global_pred)
     return m.acc if metrics is None else None
@@ -968,30 +974,48 @@ def _padded_forward(model, eng, buf):
 
 
 @torch.no_grad()
-def evaluate_bucketed(model, loader, device, tau=None, max_graphs=32):
+def evaluate_bucketed(model, loader, device, tau=None, max_graphs=32, calibration=None, monotone=False):
     """``evaluate`` (same return) with every batch padded into its capacity bucket and the engine forward + metric sums
     replayed from one CUDA graph per bucket (eager on the first visit, captured on the second; graphs persist across
     calls on the same model, and a graph captured over an engine or workspace that has since been replaced is captured
     again).  Buckets beyond ``max_graphs`` and failed captures run the padded forward eagerly; a batch
-    ``PaddedBatch`` cannot pad (per-pattern probabilities only) runs through ``eval_step``."""
-    levels = resolve_tau(model, tau)
-    was_training = model.training
-    model.eval()
+    ``PaddedBatch`` cannot pad (per-pattern probabilities only) runs through ``eval_step``.
+
+    ``calibration`` / ``monotone``: as in ``predict``, applied inside the graph before the metric sums.  The graph reads
+    a persistent copy of the offset table, one per table shape, refreshed before the loop: calibrations of one shape
+    share the graphs and a replay never reads stale offsets.  The table shape and ``monotone`` are part of the key;
+    the calls without them keep their own state and graphs."""
+    levels = _calibrated_levels(model, tau, calibration)
+    calibrated = calibration is not None or monotone
     device = torch.device(device)
     if device.type == "cuda" and device.index is None:      # "cuda" -> "cuda:<current>": the state is kept per device
         device = torch.device("cuda", torch.cuda.current_device())
-    st = model.__dict__.get("_bucketed_eval")
+    _calibration_on(calibration, device)
+    was_training = model.training
+    model.eval()
+    name = "_bucketed_eval_calibrated" if calibrated else "_bucketed_eval"
+    st = model.__dict__.get(name)
     if st is None or st.metrics.acc.device != device or st.metrics.levels != levels:
         # the graphs add into these metric sums (and hold the levels by value): new sums, new graphs
-        st = model.__dict__["_bucketed_eval"] = _GraphCache()
+        st = model.__dict__[name] = _GraphCache()
         st.metrics = EvalMetrics(device, levels)
+        st.tables = {}                                       # offset-table shape -> the table the graphs read
     st.max_graphs = max_graphs
     m = st.metrics
     m.reset()
     eng = model.engine()
+    table, shape = None, None
+    if calibration is not None:
+        shape = tuple(calibration.offsets.shape)
+        table = st.tables.get(shape)
+        if table is None:
+            table = st.tables[shape] = torch.empty(shape, dtype=torch.float32, device=device)
+        table.copy_(calibration.offsets)
 
     def run(buf):
         out = _padded_forward(model, eng, buf)
+        if calibrated:
+            _calib_apply(out[0], buf.entry_id, table, monotone, live=buf.live)
         m.add(buf.y, out[0], live=buf.live)
         return out
 
@@ -999,18 +1023,29 @@ def evaluate_bucketed(model, loader, device, tau=None, max_graphs=32):
         for data in loader:
             data = data.to(device)
             if not PaddedBatch.accepts(data):
-                eval_step(model, data, levels, m)
+                eval_step(model, data, levels, m, calibration, monotone)
                 continue
             m.count += int(data.num_graphs)
             bucket, buf = st.pad(data)
-            st.cache(bucket, eng, buf.caps, lambda: run(buf), pin=buf)
+            key = bucket + ((shape, bool(monotone)) if calibrated else ())
+            st.cache(key, eng, buf.caps, lambda: run(buf), pin=buf)
     model.train(was_training)
     return m.result()
 
 
+def _predict_cache(model, dev, max_graphs):
+    """The graph cache of ``predict`` and ``calibrate``: one graph of the padded eval forward per capacity bucket."""
+    st = model.__dict__.get("_bucketed_predict")
+    if st is None or st.zero_y.device != dev:
+        st = model.__dict__["_bucketed_predict"] = _GraphCache()
+        st.zero_y = torch.zeros(0, dtype=torch.int64, device=dev)
+    st.max_graphs = max_graphs
+    return st
+
+
 @torch.no_grad()
 def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, local=False, max_graphs=32, mixes=None,
-            overrides=None, scenario_ids=None):
+            overrides=None, scenario_ids=None, calibration=None, monotone=False):
     """Predicted latency of every request (entry ``entry_ids[q]`` at time ``timestamps[q]``, ms) of a pattern store's
     entries: float32 device tensor [Q], in request order (duplicates and any order allowed).  With ``local``, also the
     local (per-node) predictions [sum of the requests' node counts] and ``node_ptr`` [Q+1] (int64), request q owning
@@ -1029,7 +1064,13 @@ def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, lo
     request pattern mixes, resource override rows and each request's scenario, -1 for none), checked on the host and
     uploaded once per call (the override table sorted once); every slice assembles from slices of them.  The slices
     are sized, and ``node_ptr`` set, from the mixes' node counts.  A what-if slice pads into the same capacity buckets
-    as a plain one, so it replays the graphs plain calls captured."""
+    as a plain one, so it replays the graphs plain calls captured.
+
+    ``calibration`` (a ``Calibration`` of the model's levels, else ``ValueError``) adds each request's entry offsets
+    to its levels; ``monotone`` then replaces each row by its running max over the levels, so they never cross.  Either
+    runs one ``pert_calib_apply`` launch over the whole result after the slices; without them nothing more is
+    launched."""
+    _calibrated_levels(model, None, calibration)
     what_if = mixes is not None or overrides is not None or scenario_ids is not None
     bs = int(batch_size)
     if what_if:
@@ -1047,17 +1088,14 @@ def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, lo
     dev = store.device
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
+    _calibration_on(calibration, dev)
     node_ptr = np.zeros(Q + 1, dtype=np.int64)
     np.cumsum(nodes, out=node_ptr[1:])
     was_training = model.training
     model.eval()
     try:
         with torch.cuda.device(dev):
-            st = model.__dict__.get("_bucketed_predict")
-            if st is None or st.zero_y.device != dev:
-                st = model.__dict__["_bucketed_predict"] = _GraphCache()
-                st.zero_y = torch.zeros(0, dtype=torch.int64, device=dev)
-            st.max_graphs = max_graphs
+            st = _predict_cache(model, dev, max_graphs)
             if st.zero_y.numel() < min(bs, Q):
                 # requests have no label: the pad kernel, which runs eagerly in front of every replay, is the only
                 # reader of this zero column, so one buffer serves every bucket
@@ -1083,8 +1121,208 @@ def predict(model, store, entry_ids, timestamps, batch_size=1024, asof=False, lo
                 gpred[i:j].copy_(g[:j - i] if T > 1 else g[:j - i, 0])
                 if local:
                     lpred[node_ptr[i]:node_ptr[j]].copy_(loc[:node_ptr[j] - node_ptr[i], 0])
+            if Q and (calibration is not None or monotone):
+                _calib_apply(gpred, w.ent_d if what_if else ent_d,
+                             calibration.offsets if calibration is not None else None, monotone)
     finally:
         model.train(was_training)
     if not local:
         return gpred
     return gpred, lpred, torch.from_numpy(node_ptr).to(dev)
+
+
+# ------------------------------------------------------------------------------------------ conformal calibration
+CALIBRATION_GROUPINGS = ("entry", "global")
+
+
+def _calibrated_levels(model, tau, calibration):
+    """``resolve_tau(model, tau)``; with a calibration, ``tau`` None means the calibration's levels, and the levels
+    must equal them (``ValueError``)."""
+    if calibration is None:
+        return resolve_tau(model, tau)
+    if not isinstance(calibration, Calibration):
+        raise TypeError(f"calibration must be a Calibration, got {type(calibration).__name__}")
+    levels = resolve_tau(model, calibration.levels if tau is None else tau)
+    if levels != calibration.levels:
+        raise ValueError(f"the calibration's levels {calibration.levels} differ from the levels {levels}")
+    if not calibration.offsets.is_cuda:
+        raise _lib.PertGnnError("the calibration's tensors are on the host (no CPU fallback for the apply): move them "
+                                "with Calibration.to(device)")
+    return levels
+
+
+def _calibration_on(calibration, device):
+    """``PertGnnError`` unless ``calibration`` (or None) is on ``device``, where the predictions are."""
+    if calibration is not None and calibration.device != torch.device(device):
+        raise _lib.PertGnnError(f"the calibration is on {calibration.device}, the predictions on {device}: move it "
+                                "with Calibration.to(device)")
+
+
+def _calib_apply(yhat, group, off, monotone, live=None):
+    """``pert_calib_apply`` in place on the contiguous predictions ``yhat`` [Q, T] ([Q] at T = 1): + the offset row of
+    each group id ``group`` [Q] (ids outside the table read its last, global row), then the running max.  Every tensor
+    must be on yhat's CUDA device (``PertGnnError`` before the launch)."""
+    T = yhat.size(1) if yhat.dim() == 2 else 1
+    if off is not None and off.size(1) != T:
+        raise ValueError(f"an offset table of {off.size(1)} levels for predictions of {T}")
+    if not yhat.is_cuda or any(t is not None and t.device != yhat.device for t in (group, off, live)):
+        raise _lib.PertGnnError("pert_calib_apply: the predictions, entry ids, offsets and live word must be on one "
+                                "CUDA device")
+    _lib.call("pert_calib_apply", _lib.ptr(yhat), _lib.ptr(group), yhat.size(0), T, _lib.ptr(off),
+              off.size(0) if off is not None else 0, int(bool(monotone)), _lib.ptr(live), _lib.stream())
+    ops.LAUNCHES["n"] += 1
+
+
+def min_calibration_size(tau):
+    """The fewest graphs a split-conformal offset at level ``tau`` needs: the least n with ceil((n + 1) tau) <= n
+    (None for tau = 1, which no finite set reaches)."""
+    tau = float(tau)
+    if tau >= 1.0:
+        return None
+    n = max(1, int(tau / (1.0 - tau)) - 1)
+    while max(1, math.ceil((n + 1) * tau)) > n:
+        n += 1
+    return n
+
+
+class Calibration:
+    """Split-conformal offsets of a quantile model (conformalized quantile regression): ``offsets`` [G + 1, T] fp32,
+    ``counts`` [G + 1] int32 and ``own`` [G + 1, T] int8 on the device, row g of entry id g and the last row the global
+    group of every calibration graph.  For level tau and a group of n_g graphs, the offset is the k-th smallest score
+    y - yhat of the group, k = max(1, ceil((n_g + 1) tau)), when k <= n_g and n_g >= ``min_count`` (``own`` = 1), else
+    the global row's.  Then P(y <= yhat + offset) >= tau for a new request exchangeable with the calibration set, per
+    entry for the entries with their own offset.
+
+    Built by ``fit`` (or ``calibrate``), or from the three tensors, so that ``torch.save`` of them and of ``levels`` is
+    all a caller needs to keep one.  ``predict``, ``eval_step`` and ``evaluate_bucketed`` take it as ``calibration=``."""
+
+    def __init__(self, levels, offsets, counts, own, by="entry", min_count=1):
+        self.levels = _as_levels(levels)
+        if by not in CALIBRATION_GROUPINGS:
+            raise ValueError(f"by must be one of {CALIBRATION_GROUPINGS}, got {by!r}")
+        T = len(self.levels)
+        if offsets.dim() != 2 or offsets.size(1) != T or offsets.size(0) < 1 or offsets.dtype != torch.float32:
+            raise ValueError(f"offsets must be float32 [G + 1, {T}], got {offsets.dtype} {tuple(offsets.shape)}")
+        if tuple(counts.shape) != (offsets.size(0),) or tuple(own.shape) != tuple(offsets.shape):
+            raise ValueError(f"counts {tuple(counts.shape)} and own {tuple(own.shape)} do not match offsets "
+                             f"{tuple(offsets.shape)}")
+        if counts.device != offsets.device or own.device != offsets.device:
+            raise ValueError("offsets, counts and own must be on one device")
+        self.offsets, self.counts, self.own = offsets.contiguous(), counts, own
+        self.by, self.min_count = by, int(min_count)
+
+    def to(self, device):
+        """This calibration with its tensors on ``device`` (e.g. after ``torch.load(..., map_location="cpu")``)."""
+        return Calibration(self.levels, self.offsets.to(device), self.counts.to(device), self.own.to(device), self.by,
+                           self.min_count)
+
+    @property
+    def n_groups(self):
+        return self.offsets.size(0) - 1
+
+    @property
+    def device(self):
+        return self.offsets.device
+
+    @classmethod
+    @_lib.on_device_of
+    def fit(cls, y, yhat, entry_ids, levels, n_groups, by="entry", min_count=1):
+        """Offsets from labels ``y`` [n] (int64), predictions ``yhat`` [n, T] ([n] at T = 1) and the graphs' entry ids
+        ``entry_ids`` [n] (int64; ignored with ``by="global"``, which fits the global row only), all on one CUDA device,
+        for ``n_groups`` entry ids.  Checked on the host, one ``pert_calib_offsets`` launch sequence, then one read of
+        the status word.  ``ValueError`` for bad levels, shapes or ``by``, and for a set too small for a level (naming
+        the least n); ``PertGnnError`` for a NaN or infinite prediction or an entry id outside [0, n_groups)."""
+        levels = _as_levels(levels)
+        T = len(levels)
+        if by not in CALIBRATION_GROUPINGS:
+            raise ValueError(f"by must be one of {CALIBRATION_GROUPINGS}, got {by!r}")
+        if not 1 <= T <= _lib.MAX_QUANTILES:
+            raise ValueError(f"1 to {_lib.MAX_QUANTILES} levels, got {T}")
+        if any(not 0.0 <= t <= 1.0 for t in levels) or any(b <= a for a, b in zip(levels, levels[1:])):
+            raise ValueError(f"levels must be strictly increasing in [0, 1], got {levels}")
+        if operator.index(min_count) < 1:
+            raise ValueError(f"min_count must be >= 1, got {min_count}")
+        G = operator.index(n_groups) if by == "entry" else 0
+        if G < 0:
+            raise ValueError(f"n_groups must be >= 0, got {n_groups}")
+        n = int(y.numel())
+        if n < 1:
+            raise ValueError("no calibration graphs")
+        if yhat.numel() != n * T or (yhat.dim() == 2 and yhat.size(1) != T):
+            raise ValueError(f"predictions {tuple(yhat.shape)} for {n} labels and {T} levels")
+        for tau in levels:
+            need = min_calibration_size(tau)
+            if need is None or n < need:
+                raise ValueError(f"{n} calibration graphs cannot give a conformal offset at level {tau}: it needs "
+                                 + ("a finite set below 1" if need is None else f"at least n = {need}"))
+        if by == "entry" and (entry_ids is None or entry_ids.numel() != n):
+            raise ValueError(f"by='entry' needs one entry id per graph ({n})")
+        if not (y.is_cuda and yhat.is_cuda) or y.device != yhat.device:
+            raise _lib.PertGnnError("Calibration.fit needs the labels and predictions on one CUDA device")
+        dev = y.device
+        y = y.to(torch.int64).contiguous()
+        yhat = yhat.reshape(n, T).to(torch.float32).contiguous()
+        group = None
+        if by == "entry":
+            group = entry_ids.to(dev, torch.int64).contiguous()
+        ws_bytes = _lib.lib().pert_calib_workspace_bytes(n, T, G)
+        if ws_bytes < 0:
+            raise ValueError(f"{n} graphs, {T} levels and {G} groups exceed the fit's sizes (n T < 2^31)")
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        off = torch.empty(G + 1, T, dtype=torch.float32, device=dev)
+        counts = torch.empty(G + 1, dtype=torch.int32, device=dev)
+        own = torch.empty(G + 1, T, dtype=torch.int8, device=dev)
+        status = torch.zeros(1, dtype=torch.int32, device=dev)
+        _lib.call("pert_calib_offsets", _lib.ptr(y), _lib.ptr(yhat), _lib.ptr(group), n, T,
+                  (C.c_double * T)(*levels), G, int(min_count), _lib.ptr(off), _lib.ptr(counts), _lib.ptr(own),
+                  _lib.ptr(ws), ws_bytes, _lib.ptr(status), _lib.stream())
+        ops.LAUNCHES["n"] += 1
+        if int(status.item()) != 0:
+            # the error path only: name the cause
+            if not bool(torch.isfinite(y.float().reshape(n, 1) - yhat).all()):
+                raise _lib.PertGnnError("Calibration.fit: a NaN or infinite score y - yhat (a NaN or infinite "
+                                        "prediction)")
+            raise _lib.PertGnnError(f"Calibration.fit: an entry id outside [0, {G})")
+        return cls(levels, off, counts, own, by, min_count)
+
+
+@torch.no_grad()
+def calibrate(model, loader, device, tau=None, by="entry", min_count=1, max_graphs=32):
+    """Fits a ``Calibration`` of ``model`` on the labelled held-out batches of ``loader`` (e.g. a ``StoreLoader`` over
+    held-out trace ids): every batch runs the padded, graph-replayed eval forward of ``predict`` (the same graph
+    cache), its real rows' labels, predictions and entry ids are copied out on the device, and ``Calibration.fit``
+    runs once over all of them with ``n_groups = model.entry_embeds.num_embeddings``.  The levels are
+    ``resolve_tau(model, tau)``: a model trained at one level is calibrated at the ``tau`` it was trained with.  Runs
+    in eval mode under ``no_grad`` and restores the training flag; BatchNorm statistics, the dropout counter, parameters
+    and optimizer state are left as they were.  A batch ``PaddedBatch`` cannot pad runs the eval forward eagerly."""
+    levels = resolve_tau(model, tau)
+    device = torch.device(device)
+    if device.type == "cuda" and device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    ys, preds, ents = [], [], []
+    was_training = model.training
+    model.eval()
+    try:
+        with torch.cuda.device(device):
+            st = _predict_cache(model, device, max_graphs)
+            eng = model.engine()
+            for data in loader:
+                data = data.to(device)
+                B = int(data.num_graphs)
+                if PaddedBatch.accepts(data):
+                    bucket, buf = st.pad(data)
+                    g, _, _ = st.cache(bucket, eng, buf.caps, lambda: _padded_forward(model, eng, buf), pin=buf)
+                else:
+                    g, _ = model(*model_inputs(data))
+                preds.append(g[:B].clone())         # a replay rewrites the graph's output
+                ys.append(data.y.reshape(-1).to(torch.int64))
+                ents.append(data.entry_id.reshape(-1).to(torch.int64))
+    finally:
+        model.train(was_training)
+    if not ys:
+        raise ValueError("calibrate: the loader yielded no batches")
+    yhat = torch.cat(preds)
+    if yhat.size(1) != len(levels):
+        raise ValueError(f"{len(levels)} levels for a head of {yhat.size(1)} outputs")
+    return Calibration.fit(torch.cat(ys), yhat, torch.cat(ents), levels, model.entry_embeds.num_embeddings, by=by,
+                           min_count=min_count)

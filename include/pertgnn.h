@@ -59,7 +59,9 @@ extern "C" {
  * optimizer buffers when embedding tables grow); pert_model_workspace_bytes_q, pert_model_packed_bytes_q,
  * pert_model_workspace_offset_q, pert_model_forward_q, pert_model_backward_q, pert_pinball_loss_q, pert_eval_metrics_q
  * (a global head with several quantile outputs); pert_calib_workspace_bytes, pert_calib_offsets, pert_calib_apply
- * (conformal calibration of the quantile levels).  An additive entry point leaves the version as it is. */
+ * (conformal calibration of the quantile levels); pert_cpd_workspace_bytes, pert_cpd_fit, pert_cpd_tail,
+ * pert_cpd_quantile (the conformal predictive distribution: tail probabilities, p-values and quantiles at any level).
+ * An additive entry point leaves the version as it is. */
 int pert_version(void);
 
 /* ---- index construction (integer, bit-exact) ---------------------------------------------------
@@ -346,6 +348,46 @@ int pert_calib_offsets(const int64_t* y, const float* yhat, const int64_t* group
  * outside 1..INT_MAX.  Nothing is launched when Q = 0 or when off = NULL and monotone = 0. */
 int pert_calib_apply(float* yhat, const int64_t* group, long long Q, int T, const float* off, long long n_rows,
                      int monotone, const long long* live, void* stream);
+
+/* ---- conformal predictive distribution (csrc/cpd.cu) -------------------------------------------------------------
+ * The sorted split-conformal scores of n held-out graphs per group (entry id), around one prediction column: labels
+ * y [n] int64, predictions yhat[i ld + col] fp32 (a [n, ld] head output needs no copy), group [n] int64 (NULL: the
+ * global row only).  Score s = fl((float)y - yhat) in fp32, -0 canonicalised to +0 (the score of pert_calib_offsets).
+ * Outputs, G = n_groups:
+ *   ptr [G + 2] int64: row g (0 <= g < G) holds the scores of group g at scores[ptr[g] .. ptr[g+1]), ascending; row G,
+ *     all n scores ascending, is scores[ptr[G] .. ptr[G+1]).  ptr[G+1] = 2n with groups, n without.
+ *   scores [ptr[G+1]] fp32.
+ * Only values are kept, so the table is unique: bit-identical to a sort of every row, run to run.  No device-to-host
+ * read inside the call.  On the device, a NaN or infinite score or a group id outside [0, G) writes PERT_ERR_RANGE to
+ * status (the outputs are then undefined).  PERT_ERR_BADARG, before any CUDA call, for NULL pointers (group
+ * excepted), n < 1, n >= 2^30, n_groups < 0 or > INT_MAX - 2, ld < 1, col outside [0, ld) and a workspace below
+ * pert_cpd_workspace_bytes(n, n_groups) (-1 for sizes the fit refuses). */
+long long pert_cpd_workspace_bytes(long long n, long long n_groups);
+int pert_cpd_fit(const int64_t* y, const float* yhat, long long ld, int col, const int64_t* group, long long n,
+                 long long n_groups, float* scores, long long* ptr, void* workspace, long long workspace_bytes,
+                 int* status, void* stream);
+/* Queries of a fitted table (scores, ptr, n_groups as written by pert_cpd_fit) for Q requests with predictions
+ * yhat[q ld + col] and group ids group[q] (NULL: every request reads row G).
+ * pert_cpd_tail: request q reads row r = g iff 0 <= g < G and n_g >= min_count (>= 1), else row G (so an id outside
+ * [0, G) reads row G).  For each of its S thresholds x[q S + j] (x [Q, S] fp32), or for its label y[q] (y [Q] int64,
+ * S = 1; exactly one of x and y is non-NULL), with c = fl(x - yhat) (-0 -> +0) and m the row's size it writes
+ * ge[q S + j] = #{s >= c} and gt[q S + j] = #{s > c} (int32), and row[q] = r.  Then gt / (m + 1) and (ge + 1) / (m + 1)
+ * bracket P(latency > x) under the conformal predictive distribution, and (ge + 1) / (m + 1) at x = y is the
+ * conformal p-value of the label.
+ * pert_cpd_quantile: for each of L levels taus (a HOST array of doubles, 1 <= L <= PERT_MAX_QUANTILES, in [0, 1] and
+ * strictly increasing), k = max(1, ceil((m + 1) tau)) in double; row g iff 0 <= g < G, k <= n_g and n_g >= min_count,
+ * else row G; out[q L + l] = fl(yhat + s_(k)) fp32, the k-th smallest score of the row, or +inf where k exceeds even
+ * row G's size.  At a level pert_calib_offsets can fit, this is that offset added as pert_calib_apply adds it.
+ * Both: a NaN c (a NaN threshold or prediction, or inf - inf) or a NaN prediction writes PERT_ERR_RANGE to status.
+ * PERT_ERR_BADARG, before any CUDA call, for Q < 0, Q S (Q L) >= 2^31, n_groups < 0 or > INT_MAX - 2, min_count < 1,
+ * ld < 1, col outside [0, ld), NULL table, yhat, status or outputs with Q > 0, and for pert_cpd_tail S < 1, both or
+ * neither of x and y, or y with S != 1.  Nothing is launched when Q = 0. */
+int pert_cpd_tail(const float* scores, const long long* ptr, long long n_groups, long long min_count,
+                  const float* yhat, long long ld, int col, const int64_t* group, long long Q, const float* x, int S,
+                  const int64_t* y, int* ge, int* gt, int* row, int* status, void* stream);
+int pert_cpd_quantile(const float* scores, const long long* ptr, long long n_groups, long long min_count,
+                      const float* yhat, long long ld, int col, const int64_t* group, long long Q, const double* taus,
+                      int L, float* out, int* status, void* stream);
 
 /* torch.optim.Adam step (pert_gnn.py:343,247) over one flat parameter buffer; g is scaled by grad_scale, weight_decay
  * is L2 added to the scaled gradient (not AdamW's decoupled decay).  The bias corrections lr / (1 - beta1^step) and

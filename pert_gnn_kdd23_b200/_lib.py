@@ -148,6 +148,11 @@ SIGNATURES = {
     "pert_calib_workspace_bytes": (LL, [LL, I, LL]),
     "pert_calib_offsets": (I, [P, P, P, LL, I, P, LL, LL, P, P, P, P, LL, P, P]),
     "pert_calib_apply": (I, [P, P, LL, I, P, LL, I, P, P]),
+    # the conformal predictive distribution (csrc/cpd.cu; taus: host array of doubles)
+    "pert_cpd_workspace_bytes": (LL, [LL, LL]),
+    "pert_cpd_fit": (I, [P, P, LL, I, P, LL, LL, P, P, P, LL, P, P]),
+    "pert_cpd_tail": (I, [P, P, LL, LL, P, LL, I, P, LL, P, I, P, P, P, P, P, P]),
+    "pert_cpd_quantile": (I, [P, P, LL, LL, P, LL, I, P, LL, P, I, P, P, P]),
 }
 MAX_QUANTILES = 8                                       # PERT_MAX_QUANTILES
 

@@ -10,97 +10,14 @@
 // (k_cb_pick).  No segment above CB_SMALL is handled by a single CTA, so a set where one entry holds 90 % of the
 // graphs spreads over the whole GPU.  The host never reads the device: the large-tier grids are sized from n.
 #include <limits.h>
-#include <string.h>
 
 #include <algorithm>
 
-#include "common.cuh"
-#include "scan.cuh"
+#include "calib.cuh"
 
 #define CB_THREADS 256
-#define CB_SMALL 4096                  // largest segment one CTA selects (16 KB of keys in shared memory)
-#define CB_TILE 8192                   // keys per CTA of the large tier
 
 namespace {
-
-struct CalibTaus {
-  double v[PERT_MAX_QUANTILES];
-};
-
-__host__ __device__ __forceinline__ long long calib_k(long long m, double tau) {
-#ifdef __CUDA_ARCH__
-  const double x = __dmul_rn((double)(m + 1), tau);
-#else
-  const double x = (double)(m + 1) * tau;
-#endif
-  const long long k = (long long)ceil(x);
-  return k < 1 ? 1 : k;
-}
-
-// The group's own offset is used iff k <= n_g and n_g >= min_count; the global row (s == G) only needs k <= n.
-__device__ __forceinline__ bool calib_own(long long m, double tau, long long min_count, bool global) {
-  return m > 0 && calib_k(m, tau) <= m && (global || m >= min_count);
-}
-
-__device__ __forceinline__ uint32_t calib_key(float s) {
-  const uint32_t u = __float_as_uint(s);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
-__device__ __forceinline__ float calib_value(uint32_t k) {
-  return __uint_as_float((k & 0x80000000u) ? (k ^ 0x80000000u) : ~k);
-}
-
-// segment s of the group-sorted keys: groups 0 .. G-1 from the scanned counts, the global row G = all n
-__device__ __forceinline__ void calib_seg(const int* __restrict__ ptr, int G, int n, int s, int* start, int* len) {
-  if (s == G) {
-    *start = 0;
-    *len = n;
-  } else {
-    *start = ptr[s];
-    *len = ptr[s + 1] - ptr[s];
-  }
-}
-
-// atomicAdd(ctr + g, 1) for every calling lane, one atomic per distinct g in the warp: a hot entry (90 % of the graphs)
-// would otherwise serialise on one address.  Returns the calling lane's old value, as its own atomicAdd would.
-__device__ __forceinline__ int warp_counter_add(int* ctr, int g) {
-  const unsigned peers = __match_any_sync(__activemask(), g);
-  const int lane = threadIdx.x & 31, leader = __ffs(peers) - 1;
-  int base = 0;
-  if (lane == leader) base = atomicAdd(ctr + g, __popc(peers));
-  return __shfl_sync(peers, base, leader) + __popc(peers & ((1u << lane) - 1));
-}
-
-__global__ void k_cb_count(const int64_t* __restrict__ group, int n, int G, int* __restrict__ cnt,
-                           int* __restrict__ status) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int64_t g = group[i];
-  if (g < 0 || g >= G) *status = PERT_ERR_RANGE;
-  else warp_counter_add(cnt, (int)g);
-}
-
-// the T keys of graph i at its slot of the group order (slot i without groups); level t's keys are keys[t n ..)
-__global__ void k_cb_scatter(const int64_t* __restrict__ y, const float* __restrict__ yhat,
-                             const int64_t* __restrict__ group, int n, int T, int G, const int* __restrict__ ptr,
-                             int* __restrict__ fill, uint32_t* __restrict__ keys, int* __restrict__ status) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  int pos = i;
-  if (group) {
-    const int64_t g = group[i];
-    if (g < 0 || g >= G) return;            // k_cb_count has set the status
-    pos = ptr[g] + warp_counter_add(fill, (int)g);
-  }
-  const float yt = (float)y[i];             // the conversion k_eval_metrics_q's coverage test uses
-  for (int t = 0; t < T; ++t) {
-    float s = __fsub_rn(yt, yhat[(long long)i * T + t]);
-    if (!isfinite(s)) *status = PERT_ERR_RANGE;
-    if (s == 0.f) s = 0.f;                  // -0 -> +0: one key per value
-    keys[(long long)t * n + pos] = calib_key(s);
-  }
-}
 
 // One thread per segment: the large segments get a slot, their tiles and, per level, the select state {prefix, k}
 // (k = 0: the level keeps the global offset, nothing to select).
@@ -287,8 +204,6 @@ __global__ void k_cb_apply(float* __restrict__ yhat, const int64_t* __restrict__
     if (t < T) row[t] = v[t];
 }
 
-long long al256(long long b) { return (b + 255) / 256 * 256; }
-
 struct CalibLayout {
   long long ptr, fill, bsum, keys, sel, meta, large_seg, tiles, state, hist, total;
   long long L_max, tiles_max;
@@ -316,17 +231,6 @@ bool calib_layout(long long n, int T, long long G, CalibLayout* l) {
   l->hist = take(4 * 256 * l->L_max * T);
   l->total = o;
   return true;
-}
-
-int load_calib_taus(const double* taus, int T, CalibTaus* out) {
-  if (T < 1 || T > PERT_MAX_QUANTILES || !taus) return PERT_ERR_BADARG;
-  memset(out, 0, sizeof(*out));
-  for (int t = 0; t < T; ++t) {
-    if (!(taus[t] >= 0.0 && taus[t] <= 1.0)) return PERT_ERR_BADARG;
-    if (t > 0 && !(taus[t] > taus[t - 1])) return PERT_ERR_BADARG;
-    out->v[t] = taus[t];
-  }
-  return PERT_OK;
 }
 
 }  // namespace
@@ -366,18 +270,7 @@ int pert_calib_offsets(const int64_t* y, const float* yhat, const int64_t* group
   if ((e = cudaMemsetAsync(w + l.ptr, 0, l.keys - l.ptr, st)) != cudaSuccess) return (int)e;
   if ((e = cudaMemsetAsync(w + l.meta, 0, 16, st)) != cudaSuccess) return (int)e;
   if ((e = cudaMemsetAsync(w + l.hist, 0, l.total - l.hist, st)) != cudaSuccess) return (int)e;
-  const int nb = pert_cdiv(n, 256);
-  if (group && G > 0) {
-    k_cb_count<<<nb, 256, 0, st>>>(group, N, G, ptr + 1, status);
-    const int sb = pert_cdiv(G, SCAN_TILE);
-    int* bsum = (int*)(w + l.bsum);
-    k_scan_tile_sums<<<dim3(sb, 1), SCAN_THREADS, 0, st>>>(ptr + 1, nullptr, G, bsum, sb);
-    k_scan_block_sums<<<dim3(1, 1), SCAN_THREADS, 0, st>>>(bsum, sb);
-    k_scan_apply<<<dim3(sb, 1), SCAN_THREADS, 0, st>>>(ptr + 1, nullptr, G, bsum, sb);
-  } else if (group) {
-    k_cb_count<<<nb, 256, 0, st>>>(group, N, G, ptr + 1, status);       // every id is out of range
-  }
-  k_cb_scatter<<<nb, 256, 0, st>>>(y, yhat, group, N, T, G, ptr, fill, keys, status);
+  calib_group_scatter(y, yhat, T, group, N, T, G, ptr, fill, (int*)(w + l.bsum), keys, status, st);
   k_cb_plan<<<pert_cdiv(G + 1, 256), 256, 0, st>>>(ptr, G, N, T, tv, min_count, meta, large_seg, tiles, state);
   k_cb_small<<<dim3(G + 1, T), CB_THREADS, 0, st>>>(keys, ptr, G, N, T, tv, min_count, sel);
   for (int shift = 24; shift >= 0; shift -= 8) {

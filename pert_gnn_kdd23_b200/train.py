@@ -1286,16 +1286,11 @@ class Calibration:
         return cls(levels, off, counts, own, by, min_count)
 
 
-@torch.no_grad()
-def calibrate(model, loader, device, tau=None, by="entry", min_count=1, max_graphs=32):
-    """Fits a ``Calibration`` of ``model`` on the labelled held-out batches of ``loader`` (e.g. a ``StoreLoader`` over
-    held-out trace ids): every batch runs the padded, graph-replayed eval forward of ``predict`` (the same graph
-    cache), its real rows' labels, predictions and entry ids are copied out on the device, and ``Calibration.fit``
-    runs once over all of them with ``n_groups = model.entry_embeds.num_embeddings``.  The levels are
-    ``resolve_tau(model, tau)``: a model trained at one level is calibrated at the ``tau`` it was trained with.  Runs
-    in eval mode under ``no_grad`` and restores the training flag; BatchNorm statistics, the dropout counter, parameters
-    and optimizer state are left as they were.  A batch ``PaddedBatch`` cannot pad runs the eval forward eagerly."""
-    levels = resolve_tau(model, tau)
+def _replayed_predictions(model, loader, device, max_graphs, caller):
+    """-> the labels [n] (int64), predictions [n, T] and entry ids [n] (int64) of every batch of ``loader``, in loader
+    order, on ``device``.  Every batch runs the padded, graph-replayed eval forward of ``predict`` (the same graph
+    cache); a batch ``PaddedBatch`` cannot pad runs the eval forward eagerly.  Runs in eval mode under ``no_grad`` and
+    restores the training flag.  ``ValueError`` naming ``caller`` when the loader yields nothing."""
     device = torch.device(device)
     if device.type == "cuda" and device.index is None:
         device = torch.device("cuda", torch.cuda.current_device())
@@ -1320,9 +1315,282 @@ def calibrate(model, loader, device, tau=None, by="entry", min_count=1, max_grap
     finally:
         model.train(was_training)
     if not ys:
-        raise ValueError("calibrate: the loader yielded no batches")
-    yhat = torch.cat(preds)
+        raise ValueError(f"{caller}: the loader yielded no batches")
+    return torch.cat(ys), torch.cat(preds), torch.cat(ents)
+
+
+@torch.no_grad()
+def calibrate(model, loader, device, tau=None, by="entry", min_count=1, max_graphs=32):
+    """Fits a ``Calibration`` of ``model`` on the labelled held-out batches of ``loader`` (e.g. a ``StoreLoader`` over
+    held-out trace ids): every batch runs the padded, graph-replayed eval forward of ``predict`` (the same graph
+    cache), its real rows' labels, predictions and entry ids are copied out on the device, and ``Calibration.fit``
+    runs once over all of them with ``n_groups = model.entry_embeds.num_embeddings``.  The levels are
+    ``resolve_tau(model, tau)``: a model trained at one level is calibrated at the ``tau`` it was trained with.  Runs
+    in eval mode under ``no_grad`` and restores the training flag; BatchNorm statistics, the dropout counter, parameters
+    and optimizer state are left as they were.  A batch ``PaddedBatch`` cannot pad runs the eval forward eagerly."""
+    levels = resolve_tau(model, tau)
+    y, yhat, ents = _replayed_predictions(model, loader, device, max_graphs, "calibrate")
     if yhat.size(1) != len(levels):
         raise ValueError(f"{len(levels)} levels for a head of {yhat.size(1)} outputs")
-    return Calibration.fit(torch.cat(ys), yhat, torch.cat(ents), levels, model.entry_embeds.num_embeddings, by=by,
-                           min_count=min_count)
+    return Calibration.fit(y, yhat, ents, levels, model.entry_embeds.num_embeddings, by=by, min_count=min_count)
+
+
+# ------------------------------------------------------------------------------ conformal predictive distribution
+class ScoreDistribution:
+    """The split-conformal predictive distribution of a model's predictions around one base column (level ``level``):
+    the held-out scores s = (float)y - yhat in fp32 (-0 -> +0), sorted per entry.  ``scores`` [ptr[-1]] fp32 and
+    ``ptr`` [G + 2] int64 on the device: row g (0 <= g < G) holds entry g's scores at scores[ptr[g] .. ptr[g+1]), row
+    G all n of them.  A query of entry g reads row g iff it has at least ``min_count`` (>= 1) scores, else row G; an id
+    outside [0, G) -- an entry added after the fit -- reads row G.
+
+    For a request with prediction yhat, in the row of m scores read:
+    * ``tail``: with c = fl(x - yhat), lo = #{s > c} / (m + 1) and hi = (#{s >= c} + 1) / (m + 1) bracket
+      P(latency > x); hi is the conservative SLO-violation probability.
+    * ``pvalues``: hi at the observed latency y, the conformal p-value: for a trace exchangeable with the held-out set,
+      P(p <= alpha) <= alpha (per entry for the entries on their own row).
+    * ``quantile``: at any level tau, fl(yhat + s_(k)), k = max(1, ceil((m + 1) tau)), with the own-row rule of
+      ``Calibration`` (k <= n_g and n_g >= min_count, else row G); +inf where k exceeds even row G's n.  At a level
+      ``Calibration.fit`` accepts this equals its offset added by ``predict(calibration=...)``, bit for bit.
+
+    Built by ``fit`` (or ``fit_distribution``), or from the two tensors, so that ``torch.save`` of them, ``level``,
+    ``by``, ``min_count`` and ``column`` is all a caller needs to keep one.  ``column`` is the base column of a [Q, T]
+    prediction (the index of ``level`` among a quantile model's levels)."""
+
+    def __init__(self, level, scores, ptr, by="entry", min_count=1, column=0):
+        self.level = float(level)
+        if not 0.0 <= self.level <= 1.0:
+            raise ValueError(f"level must be in [0, 1], got {level}")
+        if by not in CALIBRATION_GROUPINGS:
+            raise ValueError(f"by must be one of {CALIBRATION_GROUPINGS}, got {by!r}")
+        if operator.index(min_count) < 1:
+            raise ValueError(f"min_count must be >= 1, got {min_count}")
+        if operator.index(column) < 0:
+            raise ValueError(f"column must be >= 0, got {column}")
+        if scores.dim() != 1 or scores.dtype != torch.float32 or scores.numel() < 1:
+            raise ValueError(f"scores must be float32 [n], got {scores.dtype} {tuple(scores.shape)}")
+        if ptr.dim() != 1 or ptr.dtype != torch.int64 or ptr.numel() < 2:
+            raise ValueError(f"ptr must be int64 [G + 2], got {ptr.dtype} {tuple(ptr.shape)}")
+        if ptr.device != scores.device:
+            raise ValueError("scores and ptr must be on one device")
+        self.scores, self.ptr = scores.contiguous(), ptr.contiguous()
+        self.by, self.min_count, self.column = by, int(min_count), int(column)
+
+    def to(self, device):
+        """This distribution with its tensors on ``device`` (e.g. after ``torch.load(..., map_location="cpu")``)."""
+        return ScoreDistribution(self.level, self.scores.to(device), self.ptr.to(device), self.by, self.min_count,
+                                 self.column)
+
+    @property
+    def n_groups(self):
+        return self.ptr.numel() - 2
+
+    @property
+    def device(self):
+        return self.scores.device
+
+    @property
+    def counts(self):
+        """int64 [G + 1]: the scores of each entry's row, then of the global row."""
+        return self.ptr[1:] - self.ptr[:-1]
+
+    @classmethod
+    @_lib.on_device_of
+    def fit(cls, y, yhat, entry_ids, n_groups, level, by="entry", min_count=1, column=None):
+        """The distribution of labels ``y`` [n] (int64) around predictions ``yhat`` [n], or column ``column`` of
+        ``yhat`` [n, T] (``column`` may be left out at T = 1), with the graphs' entry ids ``entry_ids`` [n] (int64;
+        ignored with ``by="global"``, which keeps the global row only), all on one CUDA device, for ``n_groups`` entry
+        ids.  ``level`` names the base column's level.  Checked on the host, one ``pert_cpd_fit`` launch sequence, then
+        one read of the status word.  ``ValueError`` for bad shapes, ``level``, ``by``, ``min_count`` or ``column``;
+        ``PertGnnError`` for host tensors, a NaN or infinite prediction or an entry id outside [0, n_groups)."""
+        level = float(level)
+        if not 0.0 <= level <= 1.0:
+            raise ValueError(f"level must be in [0, 1], got {level}")
+        if by not in CALIBRATION_GROUPINGS:
+            raise ValueError(f"by must be one of {CALIBRATION_GROUPINGS}, got {by!r}")
+        if operator.index(min_count) < 1:
+            raise ValueError(f"min_count must be >= 1, got {min_count}")
+        G = operator.index(n_groups) if by == "entry" else 0
+        if G < 0:
+            raise ValueError(f"n_groups must be >= 0, got {n_groups}")
+        n = int(y.numel())
+        if n < 1:
+            raise ValueError("no held-out graphs")
+        if yhat.dim() not in (1, 2) or yhat.size(0) != n:
+            raise ValueError(f"predictions {tuple(yhat.shape)} for {n} labels: [n] or [n, T]")
+        T = yhat.size(1) if yhat.dim() == 2 else 1
+        if column is None:
+            if T > 1:
+                raise ValueError(f"predictions of {T} levels: name the base column with column=")
+            column = 0
+        if not 0 <= operator.index(column) < T:
+            raise ValueError(f"column {column} outside the {T} columns of the predictions")
+        if by == "entry" and (entry_ids is None or entry_ids.numel() != n):
+            raise ValueError(f"by='entry' needs one entry id per graph ({n})")
+        if not (y.is_cuda and yhat.is_cuda) or y.device != yhat.device:
+            raise _lib.PertGnnError("ScoreDistribution.fit needs the labels and predictions on one CUDA device")
+        dev = y.device
+        y = y.to(torch.int64).contiguous()
+        yhat = yhat.reshape(n, T).to(torch.float32).contiguous()
+        group = entry_ids.to(dev, torch.int64).contiguous() if by == "entry" else None
+        ws_bytes = _lib.lib().pert_cpd_workspace_bytes(n, G)
+        if ws_bytes < 0:
+            raise ValueError(f"{n} graphs and {G} groups exceed the fit's sizes (n < 2^30)")
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        scores = torch.empty(2 * n if group is not None else n, dtype=torch.float32, device=dev)
+        ptr = torch.empty(G + 2, dtype=torch.int64, device=dev)
+        status = torch.zeros(1, dtype=torch.int32, device=dev)
+        _lib.call("pert_cpd_fit", _lib.ptr(y), _lib.ptr(yhat), T, int(column), _lib.ptr(group), n, G,
+                  _lib.ptr(scores), _lib.ptr(ptr), _lib.ptr(ws), ws_bytes, _lib.ptr(status), _lib.stream())
+        ops.LAUNCHES["n"] += 1
+        if int(status.item()) != 0:
+            # the error path only: name the cause
+            if not bool(torch.isfinite(y.float() - yhat[:, column]).all()):
+                raise _lib.PertGnnError("ScoreDistribution.fit: a NaN or infinite score y - yhat (a NaN or infinite "
+                                        "prediction)")
+            raise _lib.PertGnnError(f"ScoreDistribution.fit: an entry id outside [0, {G})")
+        return cls(level, scores, ptr, by, min_count, column)
+
+    def _operands(self, yhat, entry_ids):
+        """-> (yhat, ld, col, group, Q) for a query, or ``PertGnnError`` / ``ValueError`` before any launch."""
+        if not self.scores.is_cuda:
+            raise _lib.PertGnnError("the distribution's tensors are on the host (no CPU fallback for the queries): "
+                                    "move them with ScoreDistribution.to(device)")
+        if not torch.is_tensor(yhat) or yhat.device != self.device:
+            raise _lib.PertGnnError(f"the predictions must be a tensor on {self.device}, where the distribution is")
+        if entry_ids is not None and (not torch.is_tensor(entry_ids) or entry_ids.device != self.device):
+            raise _lib.PertGnnError(f"the entry ids must be a tensor on {self.device}, where the distribution is")
+        if yhat.dim() not in (1, 2):
+            raise ValueError(f"predictions {tuple(yhat.shape)}: [Q] or [Q, T]")
+        Q = yhat.size(0)
+        yhat = yhat.to(torch.float32)
+        if yhat.dim() == 2:
+            if self.column >= yhat.size(1):
+                raise ValueError(f"predictions of {yhat.size(1)} levels have no base column {self.column}")
+            if yhat.stride(1) != 1 or yhat.stride(0) < yhat.size(1):
+                yhat = yhat.contiguous()
+            ld, col = max(yhat.stride(0), 1), self.column
+        else:
+            if yhat.stride(0) < 1:
+                yhat = yhat.contiguous()
+            ld, col = max(yhat.stride(0), 1), 0
+        group = None
+        if entry_ids is not None:
+            if entry_ids.numel() != Q:
+                raise ValueError(f"{entry_ids.numel()} entry ids for {Q} predictions")
+            group = entry_ids.reshape(-1).to(torch.int64).contiguous()
+        return yhat, ld, col, group, Q
+
+    def _check(self, status, what):
+        if int(status.item()) != 0:
+            raise _lib.PertGnnError(f"ScoreDistribution.{what}: a NaN threshold, label or prediction")
+
+    def _tail_counts(self, yhat, entry_ids, x=None, y=None):
+        """-> (ge, gt [Q, S] int32, row [Q] int32, shape of the result) from one pert_cpd_tail launch and one status
+        read; ``x`` as in ``tail``, or the labels ``y`` [Q]."""
+        yhat, ld, col, group, Q = self._operands(yhat, entry_ids)
+        dev = self.device
+        if x is not None:
+            if not torch.is_tensor(x):
+                x = torch.tensor(float(x), dtype=torch.float32, device=dev)
+            elif x.device != dev:
+                raise _lib.PertGnnError(f"the thresholds must be on {dev}, where the distribution is")
+            if x.dim() > 2 or (x.dim() and x.size(0) != Q):
+                raise ValueError(f"thresholds {tuple(x.shape)} for {Q} predictions: a number, [Q] or [Q, S]")
+            shape = (Q,) if x.dim() < 2 else (Q, x.size(1))
+            x = (x.reshape(Q, -1) if x.dim() else x.reshape(1, 1).expand(Q, 1)).to(torch.float32).contiguous()
+            S = x.size(1)
+        else:
+            if not torch.is_tensor(y) or y.device != dev:
+                raise _lib.PertGnnError(f"the labels must be a tensor on {dev}, where the distribution is")
+            if y.numel() != Q:
+                raise ValueError(f"{y.numel()} labels for {Q} predictions")
+            y = y.reshape(-1).to(torch.int64).contiguous()
+            shape, S = (Q,), 1
+        ge = torch.empty(Q, S, dtype=torch.int32, device=dev)
+        gt = torch.empty(Q, S, dtype=torch.int32, device=dev)
+        row = torch.empty(Q, dtype=torch.int32, device=dev)
+        status = torch.zeros(1, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.call("pert_cpd_tail", _lib.ptr(self.scores), _lib.ptr(self.ptr), self.n_groups, self.min_count,
+                      _lib.ptr(yhat), ld, col, _lib.ptr(group), Q, _lib.ptr(x), S, _lib.ptr(y), _lib.ptr(ge),
+                      _lib.ptr(gt), _lib.ptr(row), _lib.ptr(status), _lib.stream())
+        ops.LAUNCHES["n"] += 1
+        self._check(status, "tail" if y is None else "pvalues")
+        return ge, gt, row, shape
+
+    def tail(self, yhat, entry_ids, x):
+        """-> (lo, hi) float64 bracketing P(latency > x) for every request: predictions ``yhat`` [Q] or [Q, T] (what
+        ``predict`` returns, plain or what-if; the base column is taken from [Q, T]), entry ids [Q] (None: every request
+        reads the global row) and thresholds ``x`` (ms): a number or 0-d tensor for all, [Q] per request (-> [Q]) or
+        [Q, S] per request and tier (-> [Q, S]).  Tensors must be on the distribution's device (``PertGnnError``)."""
+        ge, gt, row, shape = self._tail_counts(yhat, entry_ids, x=x)
+        m1 = (self.counts[row.long()] + 1).double().reshape(-1, 1)
+        return (gt.double() / m1).reshape(shape), ((ge.double() + 1) / m1).reshape(shape)
+
+    def pvalues(self, yhat, entry_ids, y):
+        """-> float64 [Q]: the conformal p-value (#{s >= fl(y - yhat)} + 1) / (m + 1) of every observed latency ``y``
+        [Q] (int64 ms) given its prediction and entry, as in ``tail``.  Small p flags an abnormally slow trace: flag at
+        p <= alpha for a false-alarm rate of at most alpha."""
+        ge, _, row, _ = self._tail_counts(yhat, entry_ids, y=y)
+        return (ge[:, 0].double() + 1) / (self.counts[row.long()] + 1).double()
+
+    def quantile(self, yhat, entry_ids, levels):
+        """-> float32 [Q, L]: the conformal quantile of every request at each of ``levels`` (1 to 8, strictly
+        increasing in [0, 1]), chosen at query time; +inf where no finite conformal bound exists."""
+        levels = _as_levels(levels)
+        if not 1 <= len(levels) <= _lib.MAX_QUANTILES:
+            raise ValueError(f"1 to {_lib.MAX_QUANTILES} levels, got {len(levels)}")
+        if any(not 0.0 <= t <= 1.0 for t in levels) or any(b <= a for a, b in zip(levels, levels[1:])):
+            raise ValueError(f"levels must be strictly increasing in [0, 1], got {levels}")
+        yhat, ld, col, group, Q = self._operands(yhat, entry_ids)
+        L = len(levels)
+        out = torch.empty(Q, L, dtype=torch.float32, device=self.device)
+        status = torch.zeros(1, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.call("pert_cpd_quantile", _lib.ptr(self.scores), _lib.ptr(self.ptr), self.n_groups, self.min_count,
+                      _lib.ptr(yhat), ld, col, _lib.ptr(group), Q, (C.c_double * L)(*levels), L, _lib.ptr(out),
+                      _lib.ptr(status), _lib.stream())
+        ops.LAUNCHES["n"] += 1
+        self._check(status, "quantile")
+        return out
+
+
+def _base_level(model, level):
+    """-> (level, column) of a distribution of ``model``'s predictions: ``level`` None is the model's only level; on a
+    model of T > 1 levels ``level`` must be one of them (``ValueError``)."""
+    q = getattr(model, "quantiles", None)
+    if q is not None and len(q) > 1:
+        if level is None or float(level) not in q:
+            raise ValueError(f"a model of levels {q} needs level= one of them, got {level}")
+        return float(level), q.index(float(level))
+    return resolve_tau(model, level)[0], 0
+
+
+@torch.no_grad()
+def fit_distribution(model, loader, device, level=None, by="entry", min_count=1, max_graphs=32):
+    """Fits a ``ScoreDistribution`` of ``model`` on the labelled held-out batches of ``loader``, through the same
+    padded, graph-replayed eval forward as ``calibrate``, with ``n_groups = model.entry_embeds.num_embeddings``.  The
+    base column is the model's only level (``level`` None; a one-level model may name the level it was trained at), or
+    on a quantile model of T > 1 levels the one ``level`` names (``ValueError`` otherwise)."""
+    level, column = _base_level(model, level)
+    y, yhat, ents = _replayed_predictions(model, loader, device, max_graphs, "fit_distribution")
+    return ScoreDistribution.fit(y, yhat, ents, model.entry_embeds.num_embeddings, level, by=by, min_count=min_count,
+                                 column=column)
+
+
+@torch.no_grad()
+def score_traces(model, loader, device, dist, max_graphs=32):
+    """-> float64 [n]: the conformal p-value (``ScoreDistribution.pvalues``) of every labelled trace ``loader`` yields,
+    in loader order, from the same graph-replayed eval forward as ``fit_distribution``.  Flag the traces with
+    p <= alpha as anomalously slow for a false-alarm rate of at most alpha.  A distribution on the host or on another
+    device than ``device`` raises ``PertGnnError`` before the forward."""
+    if not isinstance(dist, ScoreDistribution):
+        raise TypeError(f"dist must be a ScoreDistribution, got {type(dist).__name__}")
+    device = torch.device(device)
+    if device.type == "cuda" and device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    if not dist.scores.is_cuda or dist.device != device:
+        raise _lib.PertGnnError(f"the distribution is on {dist.device}, the predictions on {device}: move it with "
+                                "ScoreDistribution.to(device)")
+    y, yhat, ents = _replayed_predictions(model, loader, device, max_graphs, "score_traces")
+    return dist.pvalues(yhat, ents, y)

@@ -60,7 +60,8 @@ extern "C" {
  * pert_model_workspace_offset_q, pert_model_forward_q, pert_model_backward_q, pert_pinball_loss_q, pert_eval_metrics_q
  * (a global head with several quantile outputs); pert_calib_workspace_bytes, pert_calib_offsets, pert_calib_apply
  * (conformal calibration of the quantile levels); pert_cpd_workspace_bytes, pert_cpd_fit, pert_cpd_tail,
- * pert_cpd_quantile (the conformal predictive distribution: tail probabilities, p-values and quantiles at any level).
+ * pert_cpd_quantile (the conformal predictive distribution: tail probabilities, p-values and quantiles at any level);
+ * pert_cpd_merge_workspace_bytes, pert_cpd_merge (inserting scores into and removing them from a fitted table).
  * An additive entry point leaves the version as it is. */
 int pert_version(void);
 
@@ -388,6 +389,21 @@ int pert_cpd_tail(const float* scores, const long long* ptr, long long n_groups,
 int pert_cpd_quantile(const float* scores, const long long* ptr, long long n_groups, long long min_count,
                       const float* yhat, long long ld, int col, const int64_t* group, long long Q, const double* taus,
                       int L, float* out, int* status, void* stream);
+/* Updates of a fitted table: the old table (scores [n_old], ptr [G_old + 2], n_old = ptr[G_old + 1]) plus (sign = +1)
+ * or minus (sign = -1) a delta table written by pert_cpd_fit (d_scores [n_delta], d_ptr [G_new + 2], n_delta =
+ * d_ptr[G_new + 1], G_new >= G_old) gives out_scores [n_old + sign n_delta] and out_ptr [G_new + 2].  Output row r is
+ * old row r (r < G_old), an empty old row (G_old <= r < G_new) or old row G_old (r = G_new), merged with delta row r:
+ * a sorted merge, or the multiset difference (each value v loses c(v) copies, c(v) its count in the delta row).  The
+ * result is the table pert_cpd_fit writes for the union or difference of the two scored sets, bit for bit.  A delta
+ * row of a removal that holds a value more often than its old row (so also one longer than its old row) writes
+ * PERT_ERR_RANGE to status (out_scores is then undefined; no write leaves it).  No device-to-host read inside the
+ * call.  PERT_ERR_BADARG, before any CUDA call, for NULL pointers, G_old < 0, G_new < G_old or > INT_MAX - 2, a sign
+ * other than +-1, n_old < 1, n_delta < 1, a result below 1 or at 2^31 scores (the fit's n < 2^30 graphs) and a
+ * workspace below pert_cpd_merge_workspace_bytes(G_old, G_new, n_old, n_delta) (-1 for sizes neither sign accepts). */
+long long pert_cpd_merge_workspace_bytes(long long G_old, long long G_new, long long n_old, long long n_delta);
+int pert_cpd_merge(const float* scores, const long long* ptr, long long G_old, long long n_old, const float* d_scores,
+                   const long long* d_ptr, long long G_new, long long n_delta, int sign, float* out_scores,
+                   long long* out_ptr, void* workspace, long long workspace_bytes, int* status, void* stream);
 
 /* torch.optim.Adam step (pert_gnn.py:343,247) over one flat parameter buffer; g is scaled by grad_scale, weight_decay
  * is L2 added to the scaled gradient (not AdamW's decoupled decay).  The bias corrections lr / (1 - beta1^step) and

@@ -153,6 +153,8 @@ SIGNATURES = {
     "pert_cpd_fit": (I, [P, P, LL, I, P, LL, LL, P, P, P, LL, P, P]),
     "pert_cpd_tail": (I, [P, P, LL, LL, P, LL, I, P, LL, P, I, P, P, P, P, P, P]),
     "pert_cpd_quantile": (I, [P, P, LL, LL, P, LL, I, P, LL, P, I, P, P, P]),
+    "pert_cpd_merge_workspace_bytes": (LL, [LL, LL, LL, LL]),
+    "pert_cpd_merge": (I, [P, P, LL, LL, P, P, LL, LL, I, P, P, P, LL, P, P]),
 }
 MAX_QUANTILES = 8                                       # PERT_MAX_QUANTILES
 

@@ -230,6 +230,241 @@ __global__ void k_cpd_quantile(const float* __restrict__ scores, const long long
   out[i] = k > m ? INFINITY : __fadd_rn(yh, scores[ptr[r] + k - 1]);
 }
 
+// ---- pert_cpd_merge: old table (G_old) plus or minus a delta table (G_new >= G_old) -> new table (G_new).
+// Output row r reads old row r (r < G_old), no old row (G_old <= r < G_new) or old row G_old (r = G_new), and delta
+// row r.  Work is cut into tiles of CM_TILE elements of the output row (insert) or of the old row (remove); the tile
+// counts are scanned beside the row sizes, and tile t finds its row by a binary search in that prefix, so every grid
+// is sized from the host's sizes and no row is handled by a single CTA.
+#define CM_TILE 4096
+#define CM_ITEMS (CM_TILE / CPD_THREADS)
+
+__device__ __forceinline__ int cm_old_row(int r, int G_old, int G_new) {
+  return r < G_old ? r : (r == G_new ? G_old : -1);
+}
+
+// One thread per output row: its size (old +- delta) and its tile count, int32, scanned next.  A removal longer than
+// its old row sets the status and gives the row no elements.
+__global__ void k_cpd_merge_count(const long long* __restrict__ ptr, int G_old, const long long* __restrict__ dptr,
+                                  int G_new, int sign, int* __restrict__ cnt, int* __restrict__ ntile,
+                                  int* __restrict__ status) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r > G_new) return;
+  const int ro = cm_old_row(r, G_old, G_new);
+  const long long a = ro < 0 ? 0 : ptr[ro + 1] - ptr[ro], b = dptr[r + 1] - dptr[r];
+  long long c = a + b, work = c;
+  if (sign < 0) {
+    c = a - b;
+    work = a;
+    if (c < 0) {
+      *status = PERT_ERR_RANGE;
+      c = 0;
+      work = 0;
+    }
+  }
+  cnt[r] = (int)c;
+  ntile[r] = (int)((work + CM_TILE - 1) / CM_TILE);
+}
+
+// ptr_out from the scanned row sizes
+__global__ void k_cpd_merge_ptr(const int* __restrict__ cnt, int G_new, long long* __restrict__ out_ptr) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r > G_new) return;
+  out_ptr[r + 1] = cnt[r];
+  if (r == 0) out_ptr[0] = 0;
+}
+
+// tile t -> (row, first tile of the row) from the inclusive tile prefix; false past the last tile
+__device__ __forceinline__ bool cm_tile_row(const int* __restrict__ ntile, int G_new, int t, int* row, int* first) {
+  if (t >= ntile[G_new]) return false;
+  int lo = 0, hi = G_new;                     // the first row whose inclusive prefix exceeds t
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (ntile[mid] <= t) lo = mid + 1;
+    else hi = mid;
+  }
+  *row = lo;
+  *first = lo ? ntile[lo - 1] : 0;
+  return true;
+}
+
+// first index in a[lo, hi) whose key is >= k (upper: > k)
+__device__ __forceinline__ int cm_search_g(const float* __restrict__ a, int lo, int hi, uint32_t k, bool upper) {
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    const uint32_t v = calib_key(a[mid]);
+    if (upper ? v <= k : v < k) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+__device__ __forceinline__ int cm_search_s(const uint32_t* a, int lo, int hi, uint32_t k, bool upper) {
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    const uint32_t v = a[mid];
+    if (upper ? v <= k : v < k) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// Merge path with old elements first on ties: of the first d outputs of A (len a) merged with B (len b), how many
+// come from A.  ka / kb read the keys.
+template <class KA, class KB>
+__device__ __forceinline__ int cm_split(int d, int a, int b, KA ka, KB kb) {
+  int lo = max(0, d - b), hi = min(d, a);
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (ka(mid) <= kb(d - 1 - mid)) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// Insert: one CTA per output tile.  Its two diagonal searches bound the old and delta ranges, both are staged in
+// shared memory, every thread merges CM_ITEMS outputs from its own diagonal, and the tile is written out coalesced.
+__global__ void __launch_bounds__(CPD_THREADS) k_cpd_merge_insert(
+    const float* __restrict__ scores, const long long* __restrict__ ptr, int G_old, const float* __restrict__ dsc,
+    const long long* __restrict__ dptr, int G_new, const int* __restrict__ ntile, float* __restrict__ out,
+    const long long* __restrict__ out_ptr, long long n_out) {
+  __shared__ uint32_t sk[CM_TILE];
+  __shared__ float so[CM_TILE];
+  __shared__ int split[2];
+  int r, first;
+  if (!cm_tile_row(ntile, G_new, blockIdx.x, &r, &first)) return;
+  const int ro = cm_old_row(r, G_old, G_new);
+  const float* A = ro < 0 ? scores : scores + ptr[ro];
+  const float* B = dsc + dptr[r];
+  const int a = ro < 0 ? 0 : (int)(ptr[ro + 1] - ptr[ro]), b = (int)(dptr[r + 1] - dptr[r]);
+  const int o0 = (blockIdx.x - first) * CM_TILE, o1 = min(o0 + CM_TILE, a + b), len = o1 - o0;
+  if (threadIdx.x < 2) {
+    const int d = threadIdx.x ? o1 : o0;
+    split[threadIdx.x] = cm_split(d, a, b, [&](int i) { return calib_key(A[i]); },
+                                  [&](int j) { return calib_key(B[j]); });
+  }
+  __syncthreads();
+  const int i0 = split[0], na = split[1] - i0, j0 = o0 - i0, nb = len - na;
+  for (int i = threadIdx.x; i < na; i += CPD_THREADS) sk[i] = calib_key(A[i0 + i]);
+  for (int j = threadIdx.x; j < nb; j += CPD_THREADS) sk[na + j] = calib_key(B[j0 + j]);
+  __syncthreads();
+  const uint32_t* sa = sk;
+  const uint32_t* sb = sk + na;
+  const int d0 = threadIdx.x * CM_ITEMS;
+  if (d0 < len) {
+    int i = cm_split(d0, na, nb, [&](int x) { return sa[x]; }, [&](int x) { return sb[x]; }), j = d0 - i;
+    const int d1 = min(d0 + CM_ITEMS, len);
+    for (int d = d0; d < d1; ++d) {
+      const bool take_a = j >= nb || (i < na && sa[i] <= sb[j]);
+      so[d] = calib_value(take_a ? sa[i++] : sb[j++]);
+    }
+  }
+  __syncthreads();
+  const long long base = out_ptr[r] + o0;
+  for (int d = threadIdx.x; d < len; d += CPD_THREADS)
+    if (base + d < n_out) out[base + d] = so[d];
+}
+
+// Remove: one CTA per tile [s0, s1) of the old row.  The delta range the tile can touch, [lb(first), ub(last)), is
+// staged in shared memory when it fits (else searched in place).  A value v drops its first c(v) copies, c(v) its
+// count in the delta row, so a kept element i goes to i - ub_delta(v).  One search finds where the run of the tile's
+// first value starts in the old row.
+__global__ void __launch_bounds__(CPD_THREADS) k_cpd_merge_remove(
+    const float* __restrict__ scores, const long long* __restrict__ ptr, int G_old, const float* __restrict__ dsc,
+    const long long* __restrict__ dptr, int G_new, const int* __restrict__ ntile, float* __restrict__ out,
+    const long long* __restrict__ out_ptr, long long n_out, int* __restrict__ status) {
+  __shared__ uint32_t sa[CM_TILE];
+  __shared__ uint32_t sd[CM_TILE];
+  __shared__ int info[3];
+  int r, first;
+  if (!cm_tile_row(ntile, G_new, blockIdx.x, &r, &first)) return;
+  const int ro = cm_old_row(r, G_old, G_new);  // a row with tiles has an old row
+  const float* A = scores + ptr[ro];
+  const float* D = dsc + dptr[r];
+  const int a = (int)(ptr[ro + 1] - ptr[ro]), b = (int)(dptr[r + 1] - dptr[r]);
+  const int s0 = (blockIdx.x - first) * CM_TILE, len = min(CM_TILE, a - s0);
+  const long long out_len = out_ptr[r + 1] - out_ptr[r];
+  for (int i = threadIdx.x; i < len; i += CPD_THREADS) sa[i] = calib_key(A[s0 + i]);
+  __syncthreads();
+  if (threadIdx.x == 0) info[0] = cm_search_g(A, 0, s0, sa[0], false);            // the first value's run start
+  else if (threadIdx.x == 1) info[1] = cm_search_g(D, 0, b, sa[0], false);
+  else if (threadIdx.x == 2) info[2] = cm_search_g(D, 0, b, sa[len - 1], true);
+  __syncthreads();
+  const int run0 = info[0], dlo = info[1], dn = info[2] - info[1];
+  const bool staged = dn <= CM_TILE;
+  if (staged)
+    for (int j = threadIdx.x; j < dn; j += CPD_THREADS) sd[j] = calib_key(D[dlo + j]);
+  __syncthreads();
+  for (int i = threadIdx.x; i < len; i += CPD_THREADS) {
+    const uint32_t v = sa[i];
+    const int l = cm_search_s(sa, 0, i, v, false);
+    const int lb_a = l ? s0 + l : run0;
+    int lb_d, ub_d;
+    if (staged) {
+      lb_d = dlo + cm_search_s(sd, 0, dn, v, false);
+      ub_d = dlo + cm_search_s(sd, lb_d - dlo, dn, v, true);
+    } else {
+      lb_d = cm_search_g(D, dlo, dlo + dn, v, false);
+      ub_d = cm_search_g(D, lb_d, dlo + dn, v, true);
+    }
+    if (s0 + i - lb_a < ub_d - lb_d) continue;                                      // one of the first c(v) copies
+    const long long pos = (long long)s0 + i - ub_d;
+    if (pos < 0 || pos >= out_len || out_ptr[r] + pos >= n_out) {
+      *status = PERT_ERR_RANGE;                                                     // a corrupted delta
+      continue;
+    }
+    out[out_ptr[r] + pos] = calib_value(v);
+  }
+}
+
+// Remove: one thread per delta element; the j-th copy of v in its delta row (j from 0) needs at least j + 1 copies of
+// v in the old row.  A delta holding a value more often than the table does sets PERT_ERR_RANGE.
+__global__ void k_cpd_merge_check(const float* __restrict__ scores, const long long* __restrict__ ptr, int G_old,
+                                  const float* __restrict__ dsc, const long long* __restrict__ dptr, int G_new,
+                                  int n_delta, int* __restrict__ status) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_delta) return;
+  int lo = 0, hi = G_new;                     // the delta row holding element t: the last r with dptr[r] <= t
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (dptr[mid] <= t) lo = mid;
+    else hi = mid - 1;
+  }
+  const int r = lo, ro = cm_old_row(r, G_old, G_new);
+  if (ro < 0) {
+    *status = PERT_ERR_RANGE;
+    return;
+  }
+  const float* D = dsc + dptr[r];
+  const float* A = scores + ptr[ro];
+  const int j = t - (int)dptr[r], a = (int)(ptr[ro + 1] - ptr[ro]);
+  const uint32_t v = calib_key(D[j]);
+  const int rank = j - cm_search_g(D, 0, j, v, false);
+  const int lb = cm_search_g(A, 0, a, v, false);
+  if (cm_search_g(A, lb, a, v, true) - lb <= rank) *status = PERT_ERR_RANGE;
+}
+
+struct CmLayout {
+  long long cnt, ntile, bsum, total, tiles_max;
+};
+
+bool cm_layout(long long G_old, long long G_new, long long n_old, long long n_delta, int sign, CmLayout* l) {
+  if (G_old < 0 || G_new < G_old || G_new > INT_MAX - 2 || n_old < 1 || n_delta < 1) return false;
+  if (sign != 1 && sign != -1) return false;
+  const long long n_out = n_old + sign * n_delta;
+  if (n_out < 1 || n_out >= (1LL << 31) || n_old >= (1LL << 31)) return false;
+  l->tiles_max = std::max(n_old, n_out) / CM_TILE + G_new + 1;
+  const long long rows = G_new + 1;
+  long long o = 0;
+  l->cnt = o;
+  o += al256(4 * rows);
+  l->ntile = o;
+  o += al256(4 * rows);
+  l->bsum = o;
+  o += al256(2LL * pert_cdiv(rows, SCAN_TILE) * 4 + 16);
+  l->total = o;
+  return true;
+}
+
 struct CpdLayout {
   long long ptr, fill, bsum, buf0, buf1, meta, segs, tiles, hist, cursor, items, total;
   long long segs_max, tiles_max, items_max;
@@ -317,6 +552,45 @@ int pert_cpd_fit(const int64_t* y, const float* yhat, long long ld, int col, con
   }
   k_cpd_small<<<(unsigned)std::min<long long>(l.items_max, CPD_SMALL_GRID), CPD_THREADS, 0, st>>>(buf[0], buf[1], items,
                                                                                                  meta, scores);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+long long pert_cpd_merge_workspace_bytes(long long G_old, long long G_new, long long n_old, long long n_delta) {
+  CmLayout l;
+  if (!cm_layout(G_old, G_new, n_old, n_delta, 1, &l) && !cm_layout(G_old, G_new, n_old, n_delta, -1, &l))
+    return PERT_ERR_BADARG;
+  return l.total;
+}
+
+int pert_cpd_merge(const float* scores, const long long* ptr, long long G_old, long long n_old, const float* d_scores,
+                   const long long* d_ptr, long long G_new, long long n_delta, int sign, float* out_scores,
+                   long long* out_ptr, void* workspace, long long workspace_bytes, int* status, void* stream) {
+  CmLayout l;
+  if (!scores || !ptr || !d_scores || !d_ptr || !out_scores || !out_ptr || !workspace || !status)
+    return PERT_ERR_BADARG;
+  if (!cm_layout(G_old, G_new, n_old, n_delta, sign, &l) || workspace_bytes < l.total) return PERT_ERR_BADARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  char* w = (char*)workspace;
+  int* cnt = (int*)(w + l.cnt);
+  int* ntile = (int*)(w + l.ntile);
+  int* bsum = (int*)(w + l.bsum);
+  const int Go = (int)G_old, Gn = (int)G_new, rows = Gn + 1, sb = pert_cdiv(rows, SCAN_TILE);
+  const long long n_out = n_old + sign * n_delta;
+  k_cpd_merge_count<<<pert_cdiv(rows, 256), 256, 0, st>>>(ptr, Go, d_ptr, Gn, sign, cnt, ntile, status);
+  k_scan_tile_sums<<<dim3(sb, 2), SCAN_THREADS, 0, st>>>(cnt, ntile, rows, bsum, sb);
+  k_scan_block_sums<<<dim3(1, 2), SCAN_THREADS, 0, st>>>(bsum, sb);
+  k_scan_apply<<<dim3(sb, 2), SCAN_THREADS, 0, st>>>(cnt, ntile, rows, bsum, sb);
+  k_cpd_merge_ptr<<<pert_cdiv(rows, 256), 256, 0, st>>>(cnt, Gn, out_ptr);
+  if (sign > 0) {
+    k_cpd_merge_insert<<<(unsigned)l.tiles_max, CPD_THREADS, 0, st>>>(scores, ptr, Go, d_scores, d_ptr, Gn, ntile,
+                                                                     out_scores, out_ptr, n_out);
+  } else {
+    k_cpd_merge_check<<<pert_cdiv(n_delta, 256), 256, 0, st>>>(scores, ptr, Go, d_scores, d_ptr, Gn, (int)n_delta,
+                                                               status);
+    k_cpd_merge_remove<<<(unsigned)l.tiles_max, CPD_THREADS, 0, st>>>(scores, ptr, Go, d_scores, d_ptr, Gn, ntile,
+                                                                     out_scores, out_ptr, n_out, status);
+  }
   PERT_LAUNCH_CHECK();
   return PERT_OK;
 }

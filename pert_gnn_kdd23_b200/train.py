@@ -1354,9 +1354,18 @@ class ScoreDistribution:
 
     Built by ``fit`` (or ``fit_distribution``), or from the two tensors, so that ``torch.save`` of them, ``level``,
     ``by``, ``min_count`` and ``column`` is all a caller needs to keep one.  ``column`` is the base column of a [Q, T]
-    prediction (the index of ``level`` among a quantile model's levels)."""
+    prediction (the index of ``level`` among a quantile model's levels).
 
-    def __init__(self, level, scores, ptr, by="entry", min_count=1, column=0):
+    A sliding window: fitted with ``ts=`` (the graphs' store buckets, ``store.t["trace_ts"][ids]``), a distribution
+    keeps a log of its graphs in insertion order, ``log = (y int64, yhat float32 (the base column), entry int64, ts
+    int64)``, each [n] on the table's device (``log_y`` .. ``log_ts``; None without a log; pass ``log=`` to the
+    constructor to keep one across ``torch.save``).  ``insert`` adds labelled graphs, ``evict(before)`` drops the logged
+    graphs with ts < before (the cut of ``PatternStore.evict_traces``) and ``add_traces`` scores store traces, returns
+    their p-values and inserts them.  Each update is one fit of the change and one merge on the GPU, and after any
+    sequence of them ``scores`` and ``ptr`` equal, bit for bit, ``fit(log_y, log_yhat, log_entry, n_groups, ...)``.  The
+    window is valid for one set of model parameters: after fine-tuning, fit again."""
+
+    def __init__(self, level, scores, ptr, by="entry", min_count=1, column=0, *, log=None):
         self.level = float(level)
         if not 0.0 <= self.level <= 1.0:
             raise ValueError(f"level must be in [0, 1], got {level}")
@@ -1374,11 +1383,30 @@ class ScoreDistribution:
             raise ValueError("scores and ptr must be on one device")
         self.scores, self.ptr = scores.contiguous(), ptr.contiguous()
         self.by, self.min_count, self.column = by, int(min_count), int(column)
+        self.log = None
+        if log is not None:
+            if not isinstance(log, (tuple, list)) or len(log) != 4 or not all(torch.is_tensor(t) for t in log):
+                raise ValueError("log must be four tensors (y, yhat, entry, ts)")
+            n = log[0].numel()
+            want = (torch.int64, torch.float32, torch.int64, torch.int64)
+            if any(t.dim() != 1 or t.numel() != n or t.dtype != d for t, d in zip(log, want)):
+                raise ValueError("log must be y int64, yhat float32, entry int64 and ts int64, each [n], got "
+                                 + ", ".join(f"{t.dtype} {tuple(t.shape)}" for t in log))
+            if n * (2 if by == "entry" else 1) != self.scores.numel():
+                raise ValueError(f"a log of {n} graphs for a table of {self.scores.numel()} scores")
+            if any(t.device != self.scores.device for t in log):
+                raise ValueError("the log must be on the table's device")
+            self.log = tuple(t.contiguous() for t in log)
 
     def to(self, device):
         """This distribution with its tensors on ``device`` (e.g. after ``torch.load(..., map_location="cpu")``)."""
         return ScoreDistribution(self.level, self.scores.to(device), self.ptr.to(device), self.by, self.min_count,
-                                 self.column)
+                                 self.column, log=None if self.log is None else tuple(t.to(device) for t in self.log))
+
+    log_y = property(lambda self: None if self.log is None else self.log[0])
+    log_yhat = property(lambda self: None if self.log is None else self.log[1])
+    log_entry = property(lambda self: None if self.log is None else self.log[2])
+    log_ts = property(lambda self: None if self.log is None else self.log[3])
 
     @property
     def n_groups(self):
@@ -1395,13 +1423,15 @@ class ScoreDistribution:
 
     @classmethod
     @_lib.on_device_of
-    def fit(cls, y, yhat, entry_ids, n_groups, level, by="entry", min_count=1, column=None):
+    def fit(cls, y, yhat, entry_ids, n_groups, level, by="entry", min_count=1, column=None, ts=None):
         """The distribution of labels ``y`` [n] (int64) around predictions ``yhat`` [n], or column ``column`` of
         ``yhat`` [n, T] (``column`` may be left out at T = 1), with the graphs' entry ids ``entry_ids`` [n] (int64;
         ignored with ``by="global"``, which keeps the global row only), all on one CUDA device, for ``n_groups`` entry
         ids.  ``level`` names the base column's level.  Checked on the host, one ``pert_cpd_fit`` launch sequence, then
         one read of the status word.  ``ValueError`` for bad shapes, ``level``, ``by``, ``min_count`` or ``column``;
-        ``PertGnnError`` for host tensors, a NaN or infinite prediction or an entry id outside [0, n_groups)."""
+        ``PertGnnError`` for host tensors, a NaN or infinite prediction or an entry id outside [0, n_groups).  With
+        ``ts`` [n] (int64, the graphs' store buckets) the distribution keeps a log of its graphs, in this order, for
+        ``insert`` / ``evict``."""
         level = float(level)
         if not 0.0 <= level <= 1.0:
             raise ValueError(f"level must be in [0, 1], got {level}")
@@ -1426,29 +1456,155 @@ class ScoreDistribution:
             raise ValueError(f"column {column} outside the {T} columns of the predictions")
         if by == "entry" and (entry_ids is None or entry_ids.numel() != n):
             raise ValueError(f"by='entry' needs one entry id per graph ({n})")
+        _check_ts(ts, n)
         if not (y.is_cuda and yhat.is_cuda) or y.device != yhat.device:
             raise _lib.PertGnnError("ScoreDistribution.fit needs the labels and predictions on one CUDA device")
         dev = y.device
+        if ts is not None and ts.device != dev:
+            raise _lib.PertGnnError(f"the buckets ts must be on {dev}, with the labels")
         y = y.to(torch.int64).contiguous()
         yhat = yhat.reshape(n, T).to(torch.float32).contiguous()
         group = entry_ids.to(dev, torch.int64).contiguous() if by == "entry" else None
-        ws_bytes = _lib.lib().pert_cpd_workspace_bytes(n, G)
-        if ws_bytes < 0:
-            raise ValueError(f"{n} graphs and {G} groups exceed the fit's sizes (n < 2^30)")
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-        scores = torch.empty(2 * n if group is not None else n, dtype=torch.float32, device=dev)
-        ptr = torch.empty(G + 2, dtype=torch.int64, device=dev)
         status = torch.zeros(1, dtype=torch.int32, device=dev)
-        _lib.call("pert_cpd_fit", _lib.ptr(y), _lib.ptr(yhat), T, int(column), _lib.ptr(group), n, G,
-                  _lib.ptr(scores), _lib.ptr(ptr), _lib.ptr(ws), ws_bytes, _lib.ptr(status), _lib.stream())
+        scores, ptr = _cpd_fit(y, yhat, T, int(column), group, n, G, status)
         ops.LAUNCHES["n"] += 1
         if int(status.item()) != 0:
-            # the error path only: name the cause
-            if not bool(torch.isfinite(y.float() - yhat[:, column]).all()):
-                raise _lib.PertGnnError("ScoreDistribution.fit: a NaN or infinite score y - yhat (a NaN or infinite "
-                                        "prediction)")
-            raise _lib.PertGnnError(f"ScoreDistribution.fit: an entry id outside [0, {G})")
-        return cls(level, scores, ptr, by, min_count, column)
+            _raise_fit_error("fit", y, yhat[:, column], G)
+        log = None
+        if ts is not None:
+            ent = (entry_ids.to(dev, torch.int64).reshape(-1) if entry_ids is not None and entry_ids.numel() == n
+                   else torch.zeros(n, dtype=torch.int64, device=dev))
+            log = (y, yhat[:, column].contiguous(), ent.contiguous(), ts.reshape(-1).contiguous())
+        return cls(level, scores, ptr, by, min_count, column, log=log)
+
+    # ---------------------------------------------------------------------------------------- sliding-window updates
+    def _delta(self, y, yhat, entry_ids, ts, what):
+        """-> (y int64, yhat [k] fp32 base column, entry int64, ts int64) of graphs to insert, checked on the host as
+        ``fit`` checks them; ``PertGnnError`` for tensors on the host or on another device than the table."""
+        if self.log is None:
+            raise ValueError(f"ScoreDistribution.{what} needs a log: fit with ts=")
+        if not torch.is_tensor(y) or not torch.is_tensor(yhat):
+            raise ValueError("labels and predictions must be tensors")
+        k = int(y.numel())
+        if k < 1:
+            raise ValueError("no graphs to insert")
+        if yhat.dim() not in (1, 2) or yhat.size(0) != k:
+            raise ValueError(f"predictions {tuple(yhat.shape)} for {k} labels: [k] or [k, T]")
+        if yhat.dim() == 2 and yhat.size(1) > 1 and self.column >= yhat.size(1):
+            raise ValueError(f"predictions of {yhat.size(1)} levels have no base column {self.column}")
+        if self.by == "entry" and (entry_ids is None or entry_ids.numel() != k):
+            raise ValueError(f"by='entry' needs one entry id per graph ({k})")
+        _check_ts(ts, k, required=True)
+        dev = self.device
+        if not self.scores.is_cuda:
+            raise _lib.PertGnnError("the distribution's tensors are on the host: move them with "
+                                    "ScoreDistribution.to(device)")
+        for name, t in (("labels", y), ("predictions", yhat), ("entry ids", entry_ids), ("buckets ts", ts)):
+            if t is not None and t.device != dev:
+                raise _lib.PertGnnError(f"the {name} must be on {dev}, where the distribution is")
+        col = self.column if yhat.dim() == 2 and yhat.size(1) > 1 else 0
+        yh = yhat.reshape(k, -1)[:, col].to(torch.float32).contiguous()
+        ent = (entry_ids.reshape(-1).to(torch.int64).contiguous() if entry_ids is not None and entry_ids.numel() == k
+               else torch.zeros(k, dtype=torch.int64, device=dev))
+        return y.reshape(-1).to(torch.int64).contiguous(), yh, ent, ts.reshape(-1).contiguous()
+
+    def _merged(self, y, yh, ent, G_new, sign, status):
+        """The fit of the changed graphs (G_new groups) merged into (sign = +1) or out of (-1) the table: new
+        (scores, ptr) tensors; the table is not touched.  Two launch sequences, no read of the status."""
+        k = y.numel()
+        group = ent if self.by == "entry" else None
+        d_scores, d_ptr = _cpd_fit(y, yh, 1, 0, group, k, G_new, status)
+        n_old, n_d = self.scores.numel(), d_scores.numel()
+        ws_bytes = _lib.lib().pert_cpd_merge_workspace_bytes(self.n_groups, G_new, n_old, n_d)
+        if ws_bytes < 0:
+            raise ValueError(f"a table of {n_old} scores and {n_d} more exceed the fit's sizes (n < 2^30)")
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.device)
+        scores = torch.empty(n_old + sign * n_d, dtype=torch.float32, device=self.device)
+        ptr = torch.empty(G_new + 2, dtype=torch.int64, device=self.device)
+        _lib.call("pert_cpd_merge", _lib.ptr(self.scores), _lib.ptr(self.ptr), self.n_groups, n_old,
+                  _lib.ptr(d_scores), _lib.ptr(d_ptr), G_new, n_d, sign, _lib.ptr(scores), _lib.ptr(ptr),
+                  _lib.ptr(ws), ws_bytes, _lib.ptr(status), _lib.stream())
+        ops.LAUNCHES["n"] += 2
+        return scores, ptr
+
+    def insert(self, y, yhat, entry_ids, ts, n_groups=None):
+        """Adds labelled graphs to the window: labels ``y`` [k], predictions ``yhat`` [k] or [k, T] (the base column
+        is taken, as in the queries), entry ids [k] (ignored with ``by="global"``) and buckets ``ts`` [k] (int64), on
+        the table's device.  ``n_groups`` may grow the entry rows (ids from ``grow_embeddings``); it never shrinks them
+        (``ValueError``).  One fit of the k graphs and one merge on the GPU, one status read; the new tensors replace
+        the old ones only when it reads 0.  ``PertGnnError`` for a NaN or infinite score or an entry id outside [0,
+        n_groups), and the distribution is left as it was."""
+        G = self.n_groups
+        G_new = G if n_groups is None or self.by == "global" else operator.index(n_groups)
+        if G_new < G:
+            raise ValueError(f"n_groups {G_new} would shrink the table's {G} entry rows")
+        y, yh, ent, ts = self._delta(y, yhat, entry_ids, ts, "insert")
+        status = torch.zeros(1, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            scores, ptr = self._merged(y, yh, ent, G_new, 1, status)
+        if int(status.item()) != 0:
+            _raise_fit_error("insert", y, yh, G_new)
+        self.scores, self.ptr = scores, ptr
+        self.log = tuple(torch.cat([a, b]) for a, b in zip(self.log, (y, yh, ent, ts)))
+
+    def evict(self, before):
+        """Drops every logged graph whose bucket is ``< before`` from the log and the table (the cut of
+        ``PatternStore.evict_traces``), and returns how many.  The evicted log rows are fitted again (the same fp32
+        scores) and removed in one merge on the GPU; the kept rows keep their order.  ``ValueError`` without a log or
+        when nothing would be left; ``PertGnnError`` when the log's scores are not in the table (a log that does not
+        belong to it).  A failed evict leaves the distribution as it was."""
+        if self.log is None:
+            raise ValueError("ScoreDistribution.evict needs a log: fit with ts=")
+        y, yh, ent, ts = self.log
+        drop = ts < int(before)
+        k, n = int(drop.sum()), ts.numel()                # the one host read of the split
+        if k == 0:
+            return 0
+        if k == n:
+            raise ValueError(f"evicting all {n} logged graphs would leave the distribution without a score")
+        if not self.scores.is_cuda:
+            raise _lib.PertGnnError("the distribution's tensors are on the host: move them with "
+                                    "ScoreDistribution.to(device)")
+        status = torch.zeros(1, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            out, kept = torch.nonzero(drop).reshape(-1), torch.nonzero(~drop).reshape(-1)     # ascending: stable
+            scores, ptr = self._merged(y[out], yh[out], ent[out], self.n_groups, -1, status)
+        if int(status.item()) != 0:
+            raise _lib.PertGnnError("ScoreDistribution.evict: the evicted scores are not all in the table (a log that "
+                                    "does not belong to it)")
+        self.scores, self.ptr = scores, ptr
+        self.log = tuple(t[kept] for t in self.log)
+        return k
+
+    @torch.no_grad()
+    def add_traces(self, model, store, ids, evict_before=None, max_graphs=32, batch_size=1024):
+        """The online anomaly detector: runs the labelled store traces ``ids`` through the graph-replayed eval forward
+        of ``fit_distribution`` (an unshuffled ``StoreLoader``), returns their conformal p-values (float64 [len(ids)])
+        against the window as it stood before them, then inserts them with their buckets ``store.t["trace_ts"][ids]``
+        and ``n_groups = max(n_groups, model.entry_embeds.num_embeddings)``, and last evicts ``evict_before`` if given.
+        One forward, one ``pert_cpd_tail`` launch and one update; if the update fails the distribution is left as it
+        was.  The window is valid for one set of model parameters: after fine-tuning, fit again."""
+        from .store import StoreLoader
+
+        if self.log is None:
+            raise ValueError("ScoreDistribution.add_traces needs a log: fit with ts=")
+        if not self.scores.is_cuda:
+            raise _lib.PertGnnError("the distribution's tensors are on the host: move them with "
+                                    "ScoreDistribution.to(device)")
+        ids = np.asarray(ids, dtype=np.int64).reshape(-1)
+        y, yhat, ents = _replayed_predictions(model, StoreLoader(store, ids, batch_size), self.device, max_graphs,
+                                              "add_traces")
+        p = self.pvalues(yhat, ents, y)
+        ts = store.t["trace_ts"][torch.from_numpy(ids).to(store.t["trace_ts"].device)].to(self.device)
+        old = (self.scores, self.ptr, self.log)
+        try:
+            self.insert(y, yhat, ents, ts, n_groups=max(self.n_groups, model.entry_embeds.num_embeddings))
+            if evict_before is not None:
+                self.evict(evict_before)
+        except BaseException:
+            self.scores, self.ptr, self.log = old
+            raise
+        return p
 
     def _operands(self, yhat, entry_ids):
         """-> (yhat, ld, col, group, Q) for a query, or ``PertGnnError`` / ``ValueError`` before any launch."""
@@ -1555,6 +1711,37 @@ class ScoreDistribution:
         return out
 
 
+def _check_ts(ts, n, required=False):
+    """``ValueError`` unless ``ts`` is an int64 tensor of ``n`` buckets (or None when not ``required``)."""
+    if ts is None and not required:
+        return
+    if not torch.is_tensor(ts) or ts.dtype != torch.int64 or ts.numel() != n:
+        got = f"{ts.dtype} {tuple(ts.shape)}" if torch.is_tensor(ts) else type(ts).__name__
+        raise ValueError(f"ts must be int64 [{n}] (one store bucket per graph), got {got}")
+
+
+def _cpd_fit(y, yhat, ld, col, group, n, G, status):
+    """-> (scores, ptr): one ``pert_cpd_fit`` launch sequence into new tensors; the caller reads ``status``."""
+    dev = y.device
+    ws_bytes = _lib.lib().pert_cpd_workspace_bytes(n, G)
+    if ws_bytes < 0:
+        raise ValueError(f"{n} graphs and {G} groups exceed the fit's sizes (n < 2^30)")
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    scores = torch.empty(2 * n if group is not None else n, dtype=torch.float32, device=dev)
+    ptr = torch.empty(G + 2, dtype=torch.int64, device=dev)
+    _lib.call("pert_cpd_fit", _lib.ptr(y), _lib.ptr(yhat), ld, col, _lib.ptr(group), n, G, _lib.ptr(scores),
+              _lib.ptr(ptr), _lib.ptr(ws), ws_bytes, _lib.ptr(status), _lib.stream())
+    return scores, ptr
+
+
+def _raise_fit_error(what, y, yhat_col, G):
+    """The error path of a fit whose status is set: name the cause."""
+    if not bool(torch.isfinite(y.float() - yhat_col).all()):
+        raise _lib.PertGnnError(f"ScoreDistribution.{what}: a NaN or infinite score y - yhat (a NaN or infinite "
+                                "prediction)")
+    raise _lib.PertGnnError(f"ScoreDistribution.{what}: an entry id outside [0, {G})")
+
+
 def _base_level(model, level):
     """-> (level, column) of a distribution of ``model``'s predictions: ``level`` None is the model's only level; on a
     model of T > 1 levels ``level`` must be one of them (``ValueError``)."""
@@ -1567,15 +1754,17 @@ def _base_level(model, level):
 
 
 @torch.no_grad()
-def fit_distribution(model, loader, device, level=None, by="entry", min_count=1, max_graphs=32):
+def fit_distribution(model, loader, device, level=None, by="entry", min_count=1, max_graphs=32, ts=None):
     """Fits a ``ScoreDistribution`` of ``model`` on the labelled held-out batches of ``loader``, through the same
     padded, graph-replayed eval forward as ``calibrate``, with ``n_groups = model.entry_embeds.num_embeddings``.  The
     base column is the model's only level (``level`` None; a one-level model may name the level it was trained at), or
-    on a quantile model of T > 1 levels the one ``level`` names (``ValueError`` otherwise)."""
+    on a quantile model of T > 1 levels the one ``level`` names (``ValueError`` otherwise).  ``ts`` [n], the buckets of
+    the graphs in loader order (an unshuffled ``StoreLoader`` over ``ids`` and ``store.t["trace_ts"][ids]``), keeps a
+    log for ``insert`` / ``evict`` / ``add_traces``."""
     level, column = _base_level(model, level)
     y, yhat, ents = _replayed_predictions(model, loader, device, max_graphs, "fit_distribution")
     return ScoreDistribution.fit(y, yhat, ents, model.entry_embeds.num_embeddings, level, by=by, min_count=min_count,
-                                 column=column)
+                                 column=column, ts=ts)
 
 
 @torch.no_grad()

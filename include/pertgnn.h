@@ -1073,6 +1073,53 @@ int pert_raw_emit(const PertRawCalls* calls, long long N, const int64_t* order, 
                   const int64_t* g_ms, const PertRawOut* out, void* workspace, long long workspace_bytes,
                   void* stream);
 
+/* ---- Raw chunks of a stream: ids that stay fixed from chunk to chunk (rawtable.RawStream) ------------------------
+ * pert_raw_stream_process / pert_raw_stream_emit run pert_raw_process / pert_raw_emit over one chunk (its own
+ * dictionaries, as PertRawCalls) and continue the stream described by PertRawState: every chunk dictionary code is read
+ * through map[code] -> stream code (the host's dictionary of every value seen, one per coded column, microservices
+ * shared), and a stream code with id[code] >= 0 keeps that id.  Only values without an id are flagged at their first
+ * position, and get next + their rank (first sorted position; microservices: dictionary (name) order).  Traceid ids
+ * continue n_tr (the caller refuses a chunk repeating a traceid).  Entries are keyed by (dm, interface) stream codes
+ * (dm << 32 | interface) in an open-addressing table of ent_cap (a power of two >= 64) slots, ent_key ~0 = empty.
+ * The coverage filter reads has_res of the chunk OR the stream's has_res; the occurrence filter keeps a chunk's covered
+ * traces of entry e iff ent_cnt[e] + (this chunk's covered traces of e) > min_occurence.
+ * sizes[7] are those of pert_raw_process with every id count counting NEW ids only.  The state is only read; emit
+ * writes the new ids into PertRawStateOut, whose arrays the caller allocated fresh: ms_id / if_id / rpc_id / rty_id /
+ * has_res / ent_cnt hold the old contents followed by -1 (ids) or 0 (has_res, ent_cnt) for stream codes / entries
+ * the chunk adds; the entry table (ent_cap2 >= ent_cap, a power of two) is filled here, copied or rehashed from the
+ * old one, and gets the new keys.  resource_ms[K]: the id of every raw resource row's microservice (-1: outside the
+ * chunk dictionary).  The PertRawOut code arrays of new ids hold chunk codes; ent_if holds interface ids.
+ * has_res (chunk, from pert_raw_resource_groups) is OR-ed with the stream's in place.  One workspace of
+ * pert_raw_stream_workspace_bytes serves both calls. */
+typedef struct PertRawState {
+  const int64_t *ms_map, *if_map, *rpc_map, *rty_map;  /* [chunk dictionary] stream code of every chunk code     */
+  const int64_t *ms_id, *if_id, *rpc_id, *rty_id;      /* [n_*_codes] id of every stream code, -1: none          */
+  long long n_ms_codes, n_if_codes, n_rpc_codes, n_rty_codes;   /* lengths of the id arrays (and of has_res)   */
+  const int* has_res;                                  /* [n_ms_codes] a resource row in some earlier chunk      */
+  const unsigned long long* ent_key;                   /* [ent_cap] (dm << 32 | interface) stream codes, ~0 empty */
+  const int64_t* ent_id;                               /* [ent_cap] entry id of every key                        */
+  const int64_t* ent_cnt;                              /* [n_ent] covered traces of every entry so far            */
+  long long ent_cap;
+  long long n_tr, n_if, n_rpc, n_rty, n_ent, n_ms;     /* ids issued so far                                      */
+} PertRawState;
+typedef struct PertRawStateOut {
+  int64_t *ms_id, *if_id, *rpc_id, *rty_id;            /* fresh id arrays (old ids, then -1), new ids written    */
+  int* has_res;                                        /* fresh (old flags, then 0), this chunk's flags OR-ed in  */
+  unsigned long long* ent_key;                         /* [ent_cap2] fresh entry table, filled here               */
+  int64_t* ent_id;
+  int64_t* ent_cnt;                                    /* [n_ent + new] old counts then 0; this chunk's added    */
+  long long ent_cap2;
+  int64_t* resource_ms;                                /* [K] ms id of every raw resource row, -1: left out      */
+} PertRawStateOut;
+long long pert_raw_stream_workspace_bytes(const PertRawCalls* calls, long long N);
+int pert_raw_stream_process(const PertRawCalls* calls, long long N, const int64_t* order, int* has_res,
+                            long long min_occurence, const PertRawState* state, int64_t* sizes, void* workspace,
+                            long long workspace_bytes, void* stream);
+int pert_raw_stream_emit(const PertRawCalls* calls, long long N, const int64_t* order, long long G,
+                         const int64_t* g_ts, const int64_t* g_ms, long long K, const int64_t* r_ms,
+                         const int* has_res, const PertRawState* state, const PertRawOut* out,
+                         const PertRawStateOut* state_out, void* workspace, long long workspace_bytes, void* stream);
+
 /* ---- the open-bucket sample window: raw resource samples -> running statistics (csrc/rawtable.cu) -------------------
  * Continues preprocess.py:237-242 (groupby(["timestamp", "msname"]).agg([max, min, mean, median])) sample batch by
  * sample batch: after any sequence of batches every open key's 8 statistics are bit for bit those

@@ -113,6 +113,9 @@ SIGNATURES = {
     "pert_raw_process_workspace_bytes": (LL, [P, LL]),
     "pert_raw_process": (I, [P, LL, P, P, LL, P, P, LL, P]),
     "pert_raw_emit": (I, [P, LL, P, LL, P, P, P, P, LL, P]),
+    "pert_raw_stream_workspace_bytes": (LL, [P, LL]),
+    "pert_raw_stream_process": (I, [P, LL, P, P, LL, P, P, P, LL, P]),
+    "pert_raw_stream_emit": (I, [P, LL, P, LL, P, P, LL, P, P, P, P, P, P, LL, P]),
     # the open-bucket sample window (rawtable.ResourceSampleWindow)
     "pert_raw_window_workspace_bytes": (LL, [LL, LL, LL]),
     "pert_raw_window_count": (I, [LL, P, LL, LL, LL, P, P, P, P, LL, P]),
@@ -271,6 +274,18 @@ RAW_OUT = ("traceid", "timestamp", "rpcid", "um", "dm", "interface", "rpctype", 
 
 class PertRawOut(C.Structure):
     _fields_ = [(k, P) for k in RAW_OUT]
+
+
+class PertRawState(C.Structure):
+    _fields_ = [(k, P) for k in ("ms_map", "if_map", "rpc_map", "rty_map", "ms_id", "if_id", "rpc_id", "rty_id")] + \
+        [(k, LL) for k in ("n_ms_codes", "n_if_codes", "n_rpc_codes", "n_rty_codes")] + \
+        [(k, P) for k in ("has_res", "ent_key", "ent_id", "ent_cnt")] + \
+        [(k, LL) for k in ("ent_cap", "n_tr", "n_if", "n_rpc", "n_rty", "n_ent", "n_ms")]
+
+
+class PertRawStateOut(C.Structure):
+    _fields_ = [(k, P) for k in ("ms_id", "if_id", "rpc_id", "rty_id", "has_res", "ent_key", "ent_id", "ent_cnt")] + \
+        [("ent_cap2", LL), ("resource_ms", P)]
 
 
 def lib():

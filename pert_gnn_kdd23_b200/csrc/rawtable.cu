@@ -27,6 +27,10 @@
 //      (Kahan-compensated sum over the non-NaN count) and reads the median from the caller's per-group value sort.
 // Every atomic is a min, a max, an add or a slot claim whose winner changes no output, so results do not depend on
 // scheduling.
+// The chunks of a stream (pert_raw_stream_*, rawtable.RawStream) run the same passes, instantiated with S = true: every
+// chunk code is read through its map to a stream code, only values without an id are flagged at their first position
+// (so the scans rank the new ones), entries are looked up in a persistent (dm, interface) table, coverage and the
+// occurrence counts are cumulative, and the new ids go into fresh state arrays the host swaps in.
 #include "common.cuh"
 #include "rowhash.cuh"
 #include "scan.cuh"
@@ -115,6 +119,8 @@ struct Work {                 // carved from the caller's workspace by layout()
   unsigned long long *ekey, *pkey;                                  // [SE], [SP] entry / (trace, ms) tables
   int *efirst, *ecnt;                                               // [SE]
   int* bsum;
+  int64_t *cid_ms, *cid_if, *cid_rpc, *cid_rty;                    // stream only: [dictionary] id so far, -1 none
+  int64_t* eid;                                                     // stream only: [SE] entry id of a slot's key, -1
   long long SE, SP;
 };
 
@@ -126,8 +132,8 @@ long long pow2_at_least(long long n) {
 
 long long scan_bytes(long long L) { return 2LL * pert_cdiv(L, SCAN_TILE) * 4 + 16; }
 
-// bytes of the workspace of pert_raw_process / pert_raw_emit; w != NULL also carves it
-long long layout(const PertRawCalls& c, long long N, void* base, Work* w) {
+// bytes of the workspace of pert_raw_process / pert_raw_emit (stream: of the _stream_ pair); w != NULL also carves it
+long long layout(const PertRawCalls& c, long long N, void* base, Work* w, bool stream = false) {
   const long long SE = pow2_at_least(2 * c.n_trace), SP = pow2_at_least(4 * N);
   long long off = 0;
   auto take = [&](long long bytes) {
@@ -153,6 +159,14 @@ long long layout(const PertRawCalls& c, long long N, void* base, Work* w) {
   x.efirst = (int*)take(4 * SE);
   x.ecnt = (int*)take(4 * SE);
   x.bsum = (int*)take(scan_bytes(std::max(N, c.n_ms) + 1));
+  x.cid_ms = x.cid_if = x.cid_rpc = x.cid_rty = x.eid = nullptr;
+  if (stream) {
+    x.cid_ms = (int64_t*)take(8 * c.n_ms);
+    x.cid_if = (int64_t*)take(8 * c.n_iface);
+    x.cid_rpc = (int64_t*)take(8 * c.n_rpcid);
+    x.cid_rty = (int64_t*)take(8 * c.n_rpctype);
+    x.eid = (int64_t*)take(8 * SE);
+  }
   if (w) *w = x;
   return off;
 }
@@ -167,7 +181,58 @@ __global__ void k_first_codes(PertRawCalls c, long long N, const int64_t* order,
   atomicMax((long long*)&w.amax[tr], (long long)abs64(c.rt[r]));
 }
 
-// first-position flags of traceid / interface; entry candidates: http, the trace's first timestamp, its max |rt|
+// stream (S): the id a chunk code already has (-1: none), and the id of a code: its old one, or next + rank
+template <bool S>
+__device__ __forceinline__ int64_t id_of(const int64_t* cid, long long next, const int* fl, const int* first,
+                                         int64_t code) {
+  if (S) {
+    const int64_t k = cid[code];
+    if (k >= 0) return k;
+    return next + fl[first[code]];
+  }
+  return fl[first[code]];
+}
+
+// the entry table of a stream: open addressing, linear probing, load <= 1/2
+__device__ __forceinline__ int64_t ent_find(const unsigned long long* keys, const int64_t* ids, long long cap,
+                                            unsigned long long key) {
+  long long s = (long long)(mix64(key) & (unsigned long long)(cap - 1));
+  for (;;) {
+    const unsigned long long o = keys[s];
+    if (o == key) return ids[s];
+    if (o == RW_NOKEY) return -1;
+    s = (s + 1) & (cap - 1);
+  }
+}
+
+__device__ __forceinline__ void ent_insert(unsigned long long* keys, int64_t* ids, long long cap,
+                                           unsigned long long key, int64_t id) {
+  long long s = (long long)(mix64(key) & (unsigned long long)(cap - 1));
+  while (atomicCAS(&keys[s], RW_NOKEY, key) != RW_NOKEY) s = (s + 1) & (cap - 1);   // keys inserted are distinct
+  ids[s] = id;
+}
+
+// stream: every chunk code's id so far through its map (a stream code past the id array is new), and has_res OR-ed
+// with the stream's
+__global__ void k_stream_gather(PertRawCalls c, PertRawState s, int* has_res, Work w) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  auto old = [](const int64_t* map, const int64_t* id, long long n, long long k) -> int64_t {
+    const int64_t v = map[k];
+    return v >= 0 && v < n ? id[v] : -1;
+  };
+  if (i < c.n_ms) {
+    w.cid_ms[i] = old(s.ms_map, s.ms_id, s.n_ms_codes, i);
+    const int64_t v = s.ms_map[i];
+    if (v >= 0 && v < s.n_ms_codes && s.has_res[v]) has_res[i] = 1;
+  }
+  if (i < c.n_iface) w.cid_if[i] = old(s.if_map, s.if_id, s.n_if_codes, i);
+  if (i < c.n_rpcid) w.cid_rpc[i] = old(s.rpc_map, s.rpc_id, s.n_rpc_codes, i);
+  if (i < c.n_rpctype) w.cid_rty[i] = old(s.rty_map, s.rty_id, s.n_rty_codes, i);
+}
+
+// first-position flags of traceid / interface (S: interfaces without an id only); entry candidates: http, the trace's
+// first timestamp, its max |rt|
+template <bool S>
 __global__ void k_candidates(PertRawCalls c, long long N, const int64_t* order, Work w) {
   const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= N) return;
@@ -175,7 +240,7 @@ __global__ void k_candidates(PertRawCalls c, long long N, const int64_t* order, 
   const int64_t tr = c.traceid[r];
   const int f = w.first_tr[tr];
   w.fl_tr[p + 1] = f == p;
-  w.fl_if[p + 1] = w.first_if[c.interface[r]] == p;
+  w.fl_if[p + 1] = w.first_if[c.interface[r]] == p && (!S || w.cid_if[c.interface[r]] < 0);
   const int64_t ts = c.timestamp[r];
   if (c.rpctype[r] == c.http && ts == c.timestamp[order[f]] && abs64(c.rt[r]) == w.amax[tr]) {
     atomicAdd(&w.ncand[tr], 1);
@@ -187,8 +252,10 @@ __global__ void k_candidates(PertRawCalls c, long long N, const int64_t* order, 
   }
 }
 
-// per trace (dictionary code): its entry row, and the slot of its (dm, interface) key in the entry table
-__global__ void k_entries(PertRawCalls c, const int64_t* order, Work w) {
+// per trace (dictionary code): its entry row, and the slot of its (dm, interface) key in the entry table (S: stream
+// codes, and the id the stream's table holds for the key)
+template <bool S>
+__global__ void k_entries(PertRawCalls c, const int64_t* order, PertRawState st, Work w) {
   const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= c.n_trace) return;
   int e = -1;
@@ -200,7 +267,9 @@ __global__ void k_entries(PertRawCalls c, const int64_t* order, Work w) {
   w.eslot[k] = -1;
   if (e < 0) return;
   const long long r = order[e];
-  const unsigned long long key = ((unsigned long long)c.dm[r] << 32) | (unsigned long long)c.interface[r];
+  const unsigned long long key =
+      S ? ((unsigned long long)st.ms_map[c.dm[r]] << 32) | (unsigned long long)st.if_map[c.interface[r]]
+        : ((unsigned long long)c.dm[r] << 32) | (unsigned long long)c.interface[r];
   long long s = (long long)(mix64(key) & (unsigned long long)(w.SE - 1));
   for (;;) {
     const unsigned long long o = atomicCAS(&w.ekey[s], RW_NOKEY, key);
@@ -208,6 +277,7 @@ __global__ void k_entries(PertRawCalls c, const int64_t* order, Work w) {
     s = (s + 1) & (w.SE - 1);
   }
   w.eslot[k] = (int)s;
+  if (S) w.eid[s] = ent_find(st.ent_key, st.ent_id, st.ent_cap, key);   // every trace of the key writes the same
 }
 
 __device__ __forceinline__ void claim_pair(const Work& w, int64_t tr, int64_t ms, const int* has_res) {
@@ -238,15 +308,16 @@ __global__ void k_entry_rows(PertRawCalls c, long long N, const int64_t* order, 
   claim_pair(w, tr, c.dm[r], has_res);
 }
 
+template <bool S>
 __global__ void k_entry_flags(PertRawCalls c, long long N, const int64_t* order, Work w) {
   const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= N) return;
   const long long r = order[p];
   const int s = w.eslot[c.traceid[r]];
   const bool ok = s >= 0;
-  w.fl_ent[p + 1] = ok && w.efirst[s] == p;
-  w.fl_rpc[p + 1] = ok && w.first_rpc[c.rpcid[r]] == p;
-  w.fl_rty[p + 1] = ok && w.first_rty[c.rpctype[r]] == p;
+  w.fl_ent[p + 1] = ok && w.efirst[s] == p && (!S || w.eid[s] < 0);
+  w.fl_rpc[p + 1] = ok && w.first_rpc[c.rpcid[r]] == p && (!S || w.cid_rpc[c.rpcid[r]] < 0);
+  w.fl_rty[p + 1] = ok && w.first_rty[c.rpctype[r]] == p && (!S || w.cid_rty[c.rpctype[r]] < 0);
 }
 
 // resource coverage (IEEE double quotient, as Python's int / int) and the per-entry trace count of the survivors
@@ -259,22 +330,28 @@ __global__ void k_coverage(long long n_trace, Work w) {
   if (cov) atomicAdd(&w.ecnt[s], 1);
 }
 
+template <bool S>
 __global__ void k_ms_init(long long n_ms, const int* has_res, Work w) {
   const long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (m < n_ms) w.fl_ms[m + 1] = has_res[m] != 0;
+  if (m < n_ms) w.fl_ms[m + 1] = has_res[m] != 0 && (!S || w.cid_ms[m] < 0);
 }
 
-__global__ void k_survivors(PertRawCalls c, long long N, const int64_t* order, long long min_occurence, Work w) {
+// S: an entry's count is the stream's so far plus this chunk's, and only microservices without an id are flagged
+template <bool S>
+__global__ void k_survivors(PertRawCalls c, long long N, const int64_t* order, long long min_occurence,
+                            PertRawState st, Work w) {
   const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= N) return;
   const long long r = order[p];
   const int64_t tr = c.traceid[r];
   const int s = w.eslot[tr];
-  const bool keep = s >= 0 && w.covered[tr] && (long long)w.ecnt[s] > min_occurence;
+  long long cnt = s >= 0 ? w.ecnt[s] : 0;
+  if (S && s >= 0 && w.eid[s] >= 0) cnt += st.ent_cnt[w.eid[s]];
+  const bool keep = s >= 0 && w.covered[tr] && cnt > min_occurence;
   w.fl_row[p + 1] = keep;
   if (keep) {
-    w.fl_ms[c.um[r] + 1] = 1;
-    w.fl_ms[c.dm[r] + 1] = 1;
+    if (!S || w.cid_ms[c.um[r]] < 0) w.fl_ms[c.um[r] + 1] = 1;
+    if (!S || w.cid_ms[c.dm[r]] < 0) w.fl_ms[c.dm[r] + 1] = 1;
   }
 }
 
@@ -288,47 +365,97 @@ __global__ void k_sizes(long long N, long long n_ms, Work w, int64_t* sizes) {
   sizes[6] = w.fl_rty[N];
 }
 
-__global__ void k_emit_rows(PertRawCalls c, long long N, const int64_t* order, Work w, PertRawOut o) {
+// S: ids continue the stream's counters, new ones are written into the fresh state (so), and every entry of the chunk
+// (new or not) adds its covered traces to its count
+template <bool S>
+__global__ void k_emit_rows(PertRawCalls c, long long N, const int64_t* order, Work w, PertRawOut o, PertRawState st,
+                            PertRawStateOut so) {
   const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= N) return;
   const long long r = order[p];
   const int64_t tr = c.traceid[r], itf = c.interface[r];
   // dictionaries: the code each new id was given at its first position
   if (w.fl_tr[p + 1] != w.fl_tr[p]) o.tr_code[w.fl_tr[p]] = tr;
-  if (w.fl_if[p + 1] != w.fl_if[p]) o.if_code[w.fl_if[p]] = itf;
-  if (w.fl_rpc[p + 1] != w.fl_rpc[p]) o.rpc_code[w.fl_rpc[p]] = c.rpcid[r];
-  if (w.fl_rty[p + 1] != w.fl_rty[p]) o.rty_code[w.fl_rty[p]] = c.rpctype[r];
+  if (w.fl_if[p + 1] != w.fl_if[p]) {
+    o.if_code[w.fl_if[p]] = itf;
+    if (S) so.if_id[st.if_map[itf]] = st.n_if + w.fl_if[p];
+  }
+  if (w.fl_rpc[p + 1] != w.fl_rpc[p]) {
+    o.rpc_code[w.fl_rpc[p]] = c.rpcid[r];
+    if (S) so.rpc_id[st.rpc_map[c.rpcid[r]]] = st.n_rpc + w.fl_rpc[p];
+  }
+  if (w.fl_rty[p + 1] != w.fl_rty[p]) {
+    o.rty_code[w.fl_rty[p]] = c.rpctype[r];
+    if (S) so.rty_id[st.rty_map[c.rpctype[r]]] = st.n_rty + w.fl_rty[p];
+  }
   if (w.fl_ent[p + 1] != w.fl_ent[p]) {
     const long long er = order[w.epos[tr]];
     o.ent_dm[w.fl_ent[p]] = c.dm[er];
-    o.ent_if[w.fl_ent[p]] = w.fl_if[w.first_if[c.interface[er]]];
+    o.ent_if[w.fl_ent[p]] = id_of<S>(w.cid_if, st.n_if, w.fl_if, w.first_if, c.interface[er]);
+  }
+  const int es = w.eslot[tr];
+  if (S && es >= 0 && w.efirst[es] == p) {
+    const int64_t known = w.eid[es];
+    const int64_t e = known >= 0 ? known : st.n_ent + w.fl_ent[p];
+    so.ent_cnt[e] = (known >= 0 ? st.ent_cnt[known] : 0) + w.ecnt[es];
+    if (known < 0) ent_insert(so.ent_key, so.ent_id, so.ent_cap2, w.ekey[es], e);
   }
   const int q = w.fl_row[p];
   if (w.fl_row[p + 1] == q) return;
-  o.traceid[q] = w.fl_tr[w.first_tr[tr]];
+  o.traceid[q] = (S ? st.n_tr : 0) + w.fl_tr[w.first_tr[tr]];
   o.timestamp[q] = c.timestamp[r];
-  o.rpcid[q] = w.fl_rpc[w.first_rpc[c.rpcid[r]]];
-  o.um[q] = w.fl_ms[c.um[r]];
-  o.dm[q] = w.fl_ms[c.dm[r]];
-  o.interface[q] = w.fl_if[w.first_if[itf]];
-  o.rpctype[q] = w.fl_rty[w.first_rty[c.rpctype[r]]];
+  o.rpcid[q] = id_of<S>(w.cid_rpc, st.n_rpc, w.fl_rpc, w.first_rpc, c.rpcid[r]);
+  o.um[q] = S ? (w.cid_ms[c.um[r]] >= 0 ? w.cid_ms[c.um[r]] : st.n_ms + w.fl_ms[c.um[r]]) : w.fl_ms[c.um[r]];
+  o.dm[q] = S ? (w.cid_ms[c.dm[r]] >= 0 ? w.cid_ms[c.dm[r]] : st.n_ms + w.fl_ms[c.dm[r]]) : w.fl_ms[c.dm[r]];
+  o.interface[q] = id_of<S>(w.cid_if, st.n_if, w.fl_if, w.first_if, itf);
+  o.rpctype[q] = id_of<S>(w.cid_rty, st.n_rty, w.fl_rty, w.first_rty, c.rpctype[r]);
   o.rt[q] = c.rt[r];
-  o.entryid[q] = w.fl_ent[w.efirst[w.eslot[tr]]];
+  o.entryid[q] = S && w.eid[es] >= 0 ? w.eid[es] : (S ? st.n_ent : 0) + w.fl_ent[w.efirst[es]];
   o.row[q] = r;
 }
 
-__global__ void k_emit_ms(long long n_ms, Work w, int64_t* ms_code) {
-  const long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (m < n_ms && w.fl_ms[m + 1] != w.fl_ms[m]) ms_code[w.fl_ms[m]] = m;
+// microservice id of a valid chunk code (S: the stream's, or next + rank among the chunk's new names)
+template <bool S>
+__device__ __forceinline__ int64_t ms_id_of(const Work& w, const PertRawState& st, int64_t m) {
+  return S && w.cid_ms[m] >= 0 ? w.cid_ms[m] : (S ? st.n_ms : 0) + w.fl_ms[m];
 }
 
+template <bool S>
+__global__ void k_emit_ms(long long n_ms, Work w, int64_t* ms_code, const int* has_res, PertRawState st,
+                          PertRawStateOut so) {
+  const long long m = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= n_ms) return;
+  if (w.fl_ms[m + 1] != w.fl_ms[m]) {
+    ms_code[w.fl_ms[m]] = m;
+    if (S) so.ms_id[st.ms_map[m]] = st.n_ms + w.fl_ms[m];
+  }
+  if (S && has_res[m]) so.has_res[st.ms_map[m]] = 1;
+}
+
+template <bool S>
 __global__ void k_emit_res(long long G, long long n_ms, const int64_t* g_ts, const int64_t* g_ms, Work w,
-                           int64_t* res_index) {
+                           int64_t* res_index, PertRawState st) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= G) return;
   const int64_t m = g_ms[g];
   res_index[2 * g] = g_ts[g];
-  res_index[2 * g + 1] = in_dict(m, n_ms) ? w.fl_ms[m] : -1;   // groups hold valid codes only; guarded all the same
+  res_index[2 * g + 1] = in_dict(m, n_ms) ? ms_id_of<S>(w, st, m) : -1;   // groups hold valid codes only; guarded
+}
+
+// stream: the microservice id of every raw resource row (-1: an ms outside the chunk dictionary, left out)
+__global__ void k_resource_ms(long long K, long long n_ms, const int64_t* r_ms, Work w, PertRawState st,
+                              int64_t* out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= K) return;
+  const int64_t m = r_ms[i];
+  out[i] = in_dict(m, n_ms) ? ms_id_of<true>(w, st, m) : -1;
+}
+
+// stream: the old entry table into a larger fresh one
+__global__ void k_ent_rehash(const unsigned long long* keys, const int64_t* ids, long long cap, unsigned long long* keys2,
+                             int64_t* ids2, long long cap2) {
+  const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s < cap && keys[s] != RW_NOKEY) ent_insert(keys2, ids2, cap2, keys[s], ids[s]);
 }
 
 // ---- 9. resource groups ----------------------------------------------------------------------------------------------
@@ -669,17 +796,16 @@ long long pert_raw_process_workspace_bytes(const PertRawCalls* calls, long long 
   return layout(*calls, N, nullptr, nullptr) + 64;
 }
 
-int pert_raw_process(const PertRawCalls* calls, long long N, const int64_t* order, const int* has_res,
-                     long long min_occurence, int64_t* sizes, void* workspace, long long workspace_bytes,
-                     void* stream_) {
-  if (!calls_ok(calls) || N < 0 || N > calls->R || (N > 0 && !order) || !has_res || !sizes || !workspace)
-    return PERT_ERR_BADARG;
-  const long long need = pert_raw_process_workspace_bytes(calls, N);
-  if (need < 0 || workspace_bytes < need) return PERT_ERR_BADARG;
-  const PertRawCalls& c = *calls;
-  cudaStream_t st = (cudaStream_t)stream_;
+}  // extern "C"
+
+namespace {
+
+// pert_raw_process (S = false, ps unused) and pert_raw_stream_process (S = true) after their argument checks
+template <bool S>
+int process_chunk(const PertRawCalls& c, long long N, const int64_t* order, int* has_res, long long min_occurence,
+                  const PertRawState& ps, int64_t* sizes, void* workspace, cudaStream_t st) {
   Work w;
-  layout(c, N, workspace, &w);
+  layout(c, N, workspace, &w, S);
   cudaError_t e;
   auto fill = [&](void* p, long long bytes, int v) { return cudaMemsetAsync(p, v, (size_t)bytes, st); };
   if ((e = fill(w.ekey, 8 * w.SE, 0xff)) || (e = fill(w.pkey, 8 * w.SP, 0xff)) ||
@@ -698,24 +824,28 @@ int pert_raw_process(const PertRawCalls* calls, long long N, const int64_t* orde
   const int B = 256, gN = pert_cdiv(std::max(N, 1LL), B), gT = pert_cdiv(std::max(c.n_trace, 1LL), B);
   const int gM = pert_cdiv(std::max(c.n_ms, 1LL), B);
   int rc;
+  if (S) {                                               // the stream's ids of the chunk codes, its has_res
+    const long long n = std::max(std::max(c.n_ms, c.n_iface), std::max(c.n_rpcid, c.n_rpctype));
+    if (n > 0) k_stream_gather<<<pert_cdiv(n, B), B, 0, st>>>(c, ps, has_res, w);
+  }
   if (N > 0) {
     // 3. + 4. traceid / interface codes, entry candidates, entry keys
     k_first_codes<<<gN, B, 0, st>>>(c, N, order, w);
-    k_candidates<<<gN, B, 0, st>>>(c, N, order, w);
+    k_candidates<S><<<gN, B, 0, st>>>(c, N, order, w);
     PERT_LAUNCH_CHECK();
     if ((rc = scan(w.fl_tr, w.fl_if, N + 1, w.bsum, st)) != PERT_OK) return rc;
-    k_entries<<<gT, B, 0, st>>>(c, order, w);
+    k_entries<S><<<gT, B, 0, st>>>(c, order, ps, w);
     // entryid / rpcid / rpctype codes over the rows of traces with an entry; 5. coverage; 6. occurrences
     k_entry_rows<<<gN, B, 0, st>>>(c, N, order, has_res, w);
-    k_entry_flags<<<gN, B, 0, st>>>(c, N, order, w);
+    k_entry_flags<S><<<gN, B, 0, st>>>(c, N, order, w);
     PERT_LAUNCH_CHECK();
     if ((rc = scan(w.fl_ent, w.fl_rpc, N + 1, w.bsum, st)) != PERT_OK) return rc;
     if ((rc = scan(w.fl_rty, nullptr, N + 1, w.bsum, st)) != PERT_OK) return rc;
     k_coverage<<<gT, B, 0, st>>>(c.n_trace, w);
   }
   // 7. microservice presence (every resource msname, the surviving rows' um / dm); 8. survivor positions
-  k_ms_init<<<gM, B, 0, st>>>(c.n_ms, has_res, w);
-  if (N > 0) k_survivors<<<gN, B, 0, st>>>(c, N, order, min_occurence, w);
+  k_ms_init<S><<<gM, B, 0, st>>>(c.n_ms, has_res, w);
+  if (N > 0) k_survivors<S><<<gN, B, 0, st>>>(c, N, order, min_occurence, ps, w);
   PERT_LAUNCH_CHECK();
   if ((rc = scan(w.fl_ms, nullptr, c.n_ms + 1, w.bsum, st)) != PERT_OK) return rc;
   if ((rc = scan(w.fl_row, nullptr, N + 1, w.bsum, st)) != PERT_OK) return rc;
@@ -724,28 +854,120 @@ int pert_raw_process(const PertRawCalls* calls, long long N, const int64_t* orde
   return PERT_OK;
 }
 
+// pert_raw_emit (S = false) and pert_raw_stream_emit (S = true) after their argument checks
+template <bool S>
+int emit_chunk(const PertRawCalls& c, long long N, const int64_t* order, long long G, const int64_t* g_ts,
+               const int64_t* g_ms, long long K, const int64_t* r_ms, const int* has_res, const PertRawOut& o,
+               const PertRawState& ps, const PertRawStateOut& so, void* workspace, cudaStream_t st) {
+  Work w;
+  layout(c, N, workspace, &w, S);
+  const int B = 256;
+  if (S) {                                               // the fresh entry table: a copy, or the old keys rehashed
+    cudaError_t e;
+    if (so.ent_cap2 == ps.ent_cap) {
+      if ((e = cudaMemcpyAsync(so.ent_key, ps.ent_key, 8 * ps.ent_cap, cudaMemcpyDeviceToDevice, st)) ||
+          (e = cudaMemcpyAsync(so.ent_id, ps.ent_id, 8 * ps.ent_cap, cudaMemcpyDeviceToDevice, st)))
+        return (int)e;
+    } else {
+      if ((e = cudaMemsetAsync(so.ent_key, 0xff, 8 * so.ent_cap2, st))) return (int)e;
+      k_ent_rehash<<<pert_cdiv(ps.ent_cap, B), B, 0, st>>>(ps.ent_key, ps.ent_id, ps.ent_cap, so.ent_key, so.ent_id,
+                                                         so.ent_cap2);
+    }
+  }
+  if (N > 0) k_emit_rows<S><<<pert_cdiv(N, B), B, 0, st>>>(c, N, order, w, o, ps, so);
+  if (c.n_ms > 0) k_emit_ms<S><<<pert_cdiv(c.n_ms, B), B, 0, st>>>(c.n_ms, w, o.ms_code, has_res, ps, so);
+  if (G > 0) k_emit_res<S><<<pert_cdiv(G, B), B, 0, st>>>(G, c.n_ms, g_ts, g_ms, w, o.res_index, ps);
+  if (S && K > 0) k_resource_ms<<<pert_cdiv(K, B), B, 0, st>>>(K, c.n_ms, r_ms, w, ps, so.resource_ms);
+  PERT_LAUNCH_CHECK();
+  return PERT_OK;
+}
+
+bool out_ok(const PertRawOut& o) {
+  return o.traceid && o.timestamp && o.rpcid && o.um && o.dm && o.interface && o.rpctype && o.rt && o.entryid &&
+         o.row && o.res_index && o.ms_code && o.tr_code && o.if_code && o.rpc_code && o.rty_code && o.ent_dm && o.ent_if;
+}
+
+bool pow2(long long n) { return n > 0 && (n & (n - 1)) == 0; }
+
+constexpr long long RW_MAX_IDS = 0x7ffffff0LL;           // ids and stream codes of every column
+
+bool state_ok(const PertRawCalls& c, const PertRawState* s) {
+  if (!s) return false;
+  const long long codes[] = {s->n_ms_codes, s->n_if_codes, s->n_rpc_codes, s->n_rty_codes};
+  const long long ids[] = {s->n_tr, s->n_if, s->n_rpc, s->n_rty, s->n_ent, s->n_ms};
+  for (long long n : codes)
+    if (n < 0 || n > RW_MAX_IDS) return false;
+  for (long long n : ids)
+    if (n < 0 || n > RW_MAX_IDS) return false;
+  return (c.n_ms == 0 || s->ms_map) && (c.n_iface == 0 || s->if_map) && (c.n_rpcid == 0 || s->rpc_map) &&
+         (c.n_rpctype == 0 || s->rty_map) && (s->n_ms_codes == 0 || (s->ms_id && s->has_res)) &&
+         (s->n_if_codes == 0 || s->if_id) && (s->n_rpc_codes == 0 || s->rpc_id) && (s->n_rty_codes == 0 || s->rty_id) &&
+         s->ent_cap >= 64 && s->ent_cap <= (1LL << 40) && pow2(s->ent_cap) && s->ent_key && s->ent_id &&
+         (s->n_ent == 0 || s->ent_cnt) && 2 * s->n_ent <= s->ent_cap;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pert_raw_process(const PertRawCalls* calls, long long N, const int64_t* order, const int* has_res,
+                     long long min_occurence, int64_t* sizes, void* workspace, long long workspace_bytes,
+                     void* stream_) {
+  if (!calls_ok(calls) || N < 0 || N > calls->R || (N > 0 && !order) || !has_res || !sizes || !workspace)
+    return PERT_ERR_BADARG;
+  const long long need = pert_raw_process_workspace_bytes(calls, N);
+  if (need < 0 || workspace_bytes < need) return PERT_ERR_BADARG;
+  return process_chunk<false>(*calls, N, order, const_cast<int*>(has_res), min_occurence, PertRawState{}, sizes,
+                              workspace, (cudaStream_t)stream_);
+}
+
 int pert_raw_emit(const PertRawCalls* calls, long long N, const int64_t* order, long long G, const int64_t* g_ts,
                   const int64_t* g_ms, const PertRawOut* out, void* workspace, long long workspace_bytes,
                   void* stream_) {
   if (!calls_ok(calls) || N < 0 || N > calls->R || (N > 0 && !order) || G < 0 || (G > 0 && (!g_ts || !g_ms)) ||
-      !out || !workspace)
-    return PERT_ERR_BADARG;
-  const PertRawOut& o = *out;
-  if (!o.traceid || !o.timestamp || !o.rpcid || !o.um || !o.dm || !o.interface || !o.rpctype || !o.rt ||
-      !o.entryid || !o.row || !o.res_index || !o.ms_code || !o.tr_code || !o.if_code || !o.rpc_code || !o.rty_code ||
-      !o.ent_dm || !o.ent_if)
+      !out || !workspace || !out_ok(*out))
     return PERT_ERR_BADARG;
   const long long need = pert_raw_process_workspace_bytes(calls, N);
   if (need < 0 || workspace_bytes < need) return PERT_ERR_BADARG;
-  cudaStream_t st = (cudaStream_t)stream_;
-  Work w;
-  layout(*calls, N, workspace, &w);
-  const int B = 256;
-  if (N > 0) k_emit_rows<<<pert_cdiv(N, B), B, 0, st>>>(*calls, N, order, w, o);
-  if (calls->n_ms > 0) k_emit_ms<<<pert_cdiv(calls->n_ms, B), B, 0, st>>>(calls->n_ms, w, o.ms_code);
-  if (G > 0) k_emit_res<<<pert_cdiv(G, B), B, 0, st>>>(G, calls->n_ms, g_ts, g_ms, w, o.res_index);
-  PERT_LAUNCH_CHECK();
-  return PERT_OK;
+  return emit_chunk<false>(*calls, N, order, G, g_ts, g_ms, 0, nullptr, nullptr, *out, PertRawState{},
+                           PertRawStateOut{}, workspace, (cudaStream_t)stream_);
+}
+
+long long pert_raw_stream_workspace_bytes(const PertRawCalls* calls, long long N) {
+  if (!calls_ok(calls) || N < 0 || N > calls->R) return PERT_ERR_BADARG;
+  return layout(*calls, N, nullptr, nullptr, true) + 64;
+}
+
+int pert_raw_stream_process(const PertRawCalls* calls, long long N, const int64_t* order, int* has_res,
+                            long long min_occurence, const PertRawState* state, int64_t* sizes, void* workspace,
+                            long long workspace_bytes, void* stream_) {
+  if (!calls_ok(calls) || N < 0 || N > calls->R || (N > 0 && !order) || !has_res || !sizes || !workspace ||
+      !state_ok(*calls, state))
+    return PERT_ERR_BADARG;
+  const long long need = pert_raw_stream_workspace_bytes(calls, N);
+  if (need < 0 || workspace_bytes < need) return PERT_ERR_BADARG;
+  return process_chunk<true>(*calls, N, order, has_res, min_occurence, *state, sizes, workspace,
+                             (cudaStream_t)stream_);
+}
+
+int pert_raw_stream_emit(const PertRawCalls* calls, long long N, const int64_t* order, long long G,
+                         const int64_t* g_ts, const int64_t* g_ms, long long K, const int64_t* r_ms,
+                         const int* has_res, const PertRawState* state, const PertRawOut* out,
+                         const PertRawStateOut* state_out, void* workspace, long long workspace_bytes, void* stream_) {
+  if (!calls_ok(calls) || N < 0 || N > calls->R || (N > 0 && !order) || G < 0 || (G > 0 && (!g_ts || !g_ms)) ||
+      K < 0 || K > 0x7ffffff0LL || !out || !workspace || !out_ok(*out) || !state_ok(*calls, state) || !state_out)
+    return PERT_ERR_BADARG;
+  const PertRawCalls& c = *calls;
+  const PertRawStateOut& so = *state_out;
+  if ((c.n_ms > 0 && (!has_res || !so.ms_id || !so.has_res)) || (c.n_iface > 0 && !so.if_id) ||
+      (c.n_rpcid > 0 && !so.rpc_id) || (c.n_rpctype > 0 && !so.rty_id) || !so.ent_key || !so.ent_id ||
+      !so.ent_cnt || so.ent_cap2 < state->ent_cap || so.ent_cap2 > (1LL << 40) || !pow2(so.ent_cap2) ||
+      (K > 0 && (!r_ms || !so.resource_ms)))
+    return PERT_ERR_BADARG;
+  const long long need = pert_raw_stream_workspace_bytes(calls, N);
+  if (need < 0 || workspace_bytes < need) return PERT_ERR_BADARG;
+  return emit_chunk<true>(c, N, order, G, g_ts, g_ms, K, r_ms, has_res, *out, *state, so, workspace,
+                          (cudaStream_t)stream_);
 }
 
 long long pert_raw_resource_workspace_bytes(long long K) {

@@ -163,17 +163,21 @@ class ProcessedTables:
         entry_names (the reference's entry string dm + "_" + interface id), each built on first access.
     Call ``check()`` before trusting the result."""
 
-    def __init__(self, t, dicts, status):
+    def __init__(self, t, dicts, status, views=None, n_ms=None):
         self.status = status
         self.columns = {k: t[k] for k in COLUMNS}
         self.row = t["row"]
         self.resource_index, self.resource_values = t["res_index"], t["res_vals"]
         self._codes, self._dicts, self._names = {k: t[k] for k in _NAME_CODES}, dicts, {}
-        self.n_ms = int(t["ms_code"].shape[0])
+        self._views = views                  # RawStream results: name -> (the stream's list, its length then)
+        self.n_ms = int(t["ms_code"].shape[0]) if n_ms is None else n_ms
 
     def _lookup(self, name):
         """An id -> value list, built on first use (one device-to-host copy of its code array and a Python list as
         long as the ids: a million traces make a million-element traceid_names)."""
+        if name not in self._names and self._views is not None:
+            lst, n = self._views[name]
+            self._names[name] = lst[:n]
         if name not in self._names:
             code = lambda k: self._codes[k].cpu().numpy()    # noqa: E731
             d = self._dicts
@@ -231,6 +235,105 @@ def _code_of(values, v):
         return -1
 
 
+def _check_raw(raw, what, hash_bits):
+    if not isinstance(raw, RawTables):
+        raise TypeError(f"{what}: a RawTables expected (read_raw builds one)")
+    if not 1 <= int(hash_bits) <= 64:
+        raise _lib.PertGnnError(f"{what}: hash_bits must lie in 1..64")
+    R, K = len(raw), len(raw.resources["timestamp"])
+    if R > 1 << 30 or len(raw.dicts["traceid"]) > 1 << 30:
+        raise _lib.PertGnnError(f"{what}: {max(R, len(raw.dicts['traceid']))} call-graph rows or traceids exceed "
+                                "2^30")
+    if K > 0x7ffffff0:
+        raise _lib.PertGnnError(f"{what}: {K} resource rows exceed 2^31 - 16")
+
+
+class _Front(NamedTuple):
+    """What the resource groups, the statistics, the duplicate drop and the timestamp sort leave for the call-graph
+    passes (process_raw's steps 9, 1 and 2); cols keeps the device columns ``tab`` points into alive."""
+    status: torch.Tensor
+    G: int
+    g_ts: torch.Tensor
+    g_ms: torch.Tensor
+    res_vals: torch.Tensor
+    has_res: torch.Tensor
+    r_ms: torch.Tensor
+    tab: object
+    cols: dict
+    N: int
+    order: torch.Tensor
+
+
+def _front(raw, dev, hash_bits):
+    """Steps 9, 1 and 2 on the current device and stream: host synchronisations (1) G and (2) the distinct rows."""
+    L, st = _lib.lib(), _lib.stream()
+    R, K = len(raw), len(raw.resources["timestamp"])
+    i32, i64, f64 = (dict(dtype=d, device=dev) for d in (torch.int32, torch.int64, torch.float64))
+    status = torch.zeros(1, **i32)
+    n_ms = len(raw.dicts["ms"])
+    # ---- resources: stable sort by (timestamp, ms), groups, statistics (:227-242)
+    r_ts, r_ms = (torch.from_numpy(raw.resources[k]).to(dev) for k in ("timestamp", "msname"))
+    usage = [torch.from_numpy(raw.resources[u]).to(dev) for u in USAGE]
+    p1 = torch.sort(r_ms, stable=True).indices
+    perm = p1[torch.sort(r_ts[p1], stable=True).indices]
+    bad = ((r_ms < 0) | (r_ms >= n_ms))[perm]           # rows with an ms outside the dictionary go last
+    keep = torch.sort(bad.to(torch.uint8), stable=True).indices
+    perm, bad = perm[keep].contiguous(), bad[keep]
+    gflag, gptr = torch.empty(K + 1, **i32), torch.empty(K + 1, **i32)
+    has_res = torch.empty(max(n_ms, 1), **i32)
+    g_ts, g_ms, ng = torch.empty(max(K, 1), **i64), torch.empty(max(K, 1), **i64), torch.empty(1, **i64)
+    ws = torch.empty(int(L.pert_raw_resource_workspace_bytes(K)), dtype=torch.uint8, device=dev)
+    _lib.check(L.pert_raw_resource_groups(K, _lib.ptr(r_ts), _lib.ptr(r_ms), _lib.ptr(perm), n_ms,
+                                          gflag.data_ptr(), has_res.data_ptr(), gptr.data_ptr(), g_ts.data_ptr(),
+                                          g_ms.data_ptr(), ng.data_ptr(), ws.data_ptr(), ws.numel(),
+                                          status.data_ptr(), st), "pert_raw_resource_groups")
+    G = int(ng.item())                                                           # sync 1
+    gid = torch.where(bad, G, gflag[1:] - 1)           # the left-out rows sort after every group
+    sorted_usage = []
+    for u in usage:                      # every group's values ascending (NaN last) at the group's positions
+        s = torch.sort(u[perm], stable=True)
+        sorted_usage.append(s.values[torch.sort(gid[s.indices], stable=True).indices].contiguous())
+    res_vals = torch.empty(G, 8, **f64)
+    _lib.check(L.pert_raw_resource_stats(G, _lib.ptr(perm), gptr.data_ptr(), _lib.ptr(usage[0]),
+                                         _lib.ptr(usage[1]), _lib.ptr(sorted_usage[0]), _lib.ptr(sorted_usage[1]),
+                                         res_vals.data_ptr(), st), "pert_raw_resource_stats")
+    # ---- call graph: duplicates, stable sort by timestamp (:212-213)
+    cols = {k: torch.from_numpy(raw.calls[k]).to(dev) for k in CALL_COLUMNS}
+    n = {k: len(raw.dicts[k]) for k in CODED}
+    tab = _lib.PertRawCalls(R, n["traceid"], n["interface"], n["rpcid"], n["rpctype"], n_ms,
+                            _code_of(raw.dicts["rpctype"], "http"), _code_of(raw.dicts["ms"], "(?)"),
+                            *(cols[k].data_ptr() for k in CALL_COLUMNS))
+    rows, keys, nk = torch.empty(max(R, 1), **i32), torch.empty(max(R, 1), **i64), torch.empty(1, **i64)
+    ws = torch.empty(int(L.pert_raw_dedup_workspace_bytes(R)), dtype=torch.uint8, device=dev)
+    _lib.check(L.pert_raw_dedup(C.byref(tab), int(hash_bits), rows.data_ptr(), keys.data_ptr(), nk.data_ptr(),
+                                ws.data_ptr(), ws.numel(), status.data_ptr(), st), "pert_raw_dedup")
+    N = int(nk.item())                                                           # sync 2
+    order = rows[:N].long()[torch.sort(keys[:N], stable=True).indices].contiguous()
+    return _Front(status, G, g_ts, g_ms, res_vals, has_res, r_ms, tab, cols, N, order)
+
+
+def _alloc_out(dev, M, G, n_ids, n_tr, n_if, n_ent, n_rpc, n_rty):
+    """Output tensors of pert_raw_emit: every one at least one element, so no pointer is NULL; sliced to its size.
+    The id -> code arrays share one buffer (one device -> host copy reads them all)."""
+    alloc = lambda n, *w: torch.empty(max(n, 1), *w, dtype=torch.int64, device=dev)[:n]   # noqa: E731
+    t = {k: alloc(M) for k in COLUMNS + ("row",)}
+    t["res_index"] = alloc(G, 2)
+    sizes = {"ms_code": n_ids, "tr_code": n_tr, "if_code": n_if, "rpc_code": n_rpc, "rty_code": n_rty,
+             "ent_dm": n_ent, "ent_if": n_ent}
+    buf = torch.empty(max(sum(sizes.values()), 1), dtype=torch.int64, device=dev)
+    o = 0
+    for k, n in sizes.items():
+        t[k] = buf[o:o + n]
+        o += n
+    t["_codes"] = buf[:o]
+    return t
+
+
+def _raw_out(t, spare=None):
+    """PertRawOut of ``t``; with ``spare`` (a one-element tensor) an empty output points there instead of NULL."""
+    return _lib.PertRawOut(*(t[k].data_ptr() or (spare.data_ptr() if spare is not None else 0) for k in _lib.RAW_OUT))
+
+
 def process_raw(raw, device="cuda", min_occurence=100, hash_bits=64):
     """get_df()'s processing (:212-254) of a RawTables on the GPU -> ProcessedTables.  ``min_occurence``: an entry is
     kept with strictly more traces than this (:185).  ``hash_bits`` narrows the duplicate-row hash (1..64); only tests
@@ -243,77 +346,202 @@ def process_raw(raw, device="cuda", min_occurence=100, hash_bits=64):
     dev = torch.device(device)
     if dev.type != "cuda":
         raise _lib.PertGnnError("process_raw needs a CUDA device (no CPU fallback)")
-    if not isinstance(raw, RawTables):
-        raise TypeError("process_raw: a RawTables expected (read_raw builds one)")
-    if not 1 <= int(hash_bits) <= 64:
-        raise _lib.PertGnnError("process_raw: hash_bits must lie in 1..64")
-    R, K = len(raw), len(raw.resources["timestamp"])
-    if R > 1 << 30 or len(raw.dicts["traceid"]) > 1 << 30:
-        raise _lib.PertGnnError(f"process_raw: {max(R, len(raw.dicts['traceid']))} call-graph rows or traceids exceed "
-                                "2^30")
-    if K > 0x7ffffff0:
-        raise _lib.PertGnnError(f"process_raw: {K} resource rows exceed 2^31 - 16")
+    _check_raw(raw, "process_raw", hash_bits)
     with torch.cuda.device(dev):
         L, st = _lib.lib(), _lib.stream()
-        i32, i64, f64 = (dict(dtype=d, device=dev) for d in (torch.int32, torch.int64, torch.float64))
-        status = torch.zeros(1, **i32)
-        n_ms = len(raw.dicts["ms"])
-        # ---- resources: stable sort by (timestamp, ms), groups, statistics (:227-242)
-        r_ts, r_ms = (torch.from_numpy(raw.resources[k]).to(dev) for k in ("timestamp", "msname"))
-        usage = [torch.from_numpy(raw.resources[u]).to(dev) for u in USAGE]
-        p1 = torch.sort(r_ms, stable=True).indices
-        perm = p1[torch.sort(r_ts[p1], stable=True).indices]
-        bad = ((r_ms < 0) | (r_ms >= n_ms))[perm]           # rows with an ms outside the dictionary go last
-        keep = torch.sort(bad.to(torch.uint8), stable=True).indices
-        perm, bad = perm[keep].contiguous(), bad[keep]
-        gflag, gptr = torch.empty(K + 1, **i32), torch.empty(K + 1, **i32)
-        has_res = torch.empty(max(n_ms, 1), **i32)
-        g_ts, g_ms, ng = torch.empty(max(K, 1), **i64), torch.empty(max(K, 1), **i64), torch.empty(1, **i64)
-        ws = torch.empty(int(L.pert_raw_resource_workspace_bytes(K)), dtype=torch.uint8, device=dev)
-        _lib.check(L.pert_raw_resource_groups(K, _lib.ptr(r_ts), _lib.ptr(r_ms), _lib.ptr(perm), n_ms,
-                                              gflag.data_ptr(), has_res.data_ptr(), gptr.data_ptr(), g_ts.data_ptr(),
-                                              g_ms.data_ptr(), ng.data_ptr(), ws.data_ptr(), ws.numel(),
-                                              status.data_ptr(), st), "pert_raw_resource_groups")
-        G = int(ng.item())                                                           # sync 1
-        gid = torch.where(bad, G, gflag[1:] - 1)           # the left-out rows sort after every group
-        sorted_usage = []
-        for u in usage:                      # every group's values ascending (NaN last) at the group's positions
-            s = torch.sort(u[perm], stable=True)
-            sorted_usage.append(s.values[torch.sort(gid[s.indices], stable=True).indices].contiguous())
-        res_vals = torch.empty(G, 8, **f64)
-        _lib.check(L.pert_raw_resource_stats(G, _lib.ptr(perm), gptr.data_ptr(), _lib.ptr(usage[0]),
-                                             _lib.ptr(usage[1]), _lib.ptr(sorted_usage[0]), _lib.ptr(sorted_usage[1]),
-                                             res_vals.data_ptr(), st), "pert_raw_resource_stats")
-        # ---- call graph: duplicates, stable sort by timestamp, the filters, the processed columns (:212-254)
-        cols = {k: torch.from_numpy(raw.calls[k]).to(dev) for k in CALL_COLUMNS}
-        n = {k: len(raw.dicts[k]) for k in CODED}
-        tab = _lib.PertRawCalls(R, n["traceid"], n["interface"], n["rpcid"], n["rpctype"], n_ms,
-                                _code_of(raw.dicts["rpctype"], "http"), _code_of(raw.dicts["ms"], "(?)"),
-                                *(cols[k].data_ptr() for k in CALL_COLUMNS))
-        rows, keys, nk = torch.empty(max(R, 1), **i32), torch.empty(max(R, 1), **i64), torch.empty(1, **i64)
-        ws = torch.empty(int(L.pert_raw_dedup_workspace_bytes(R)), dtype=torch.uint8, device=dev)
-        _lib.check(L.pert_raw_dedup(C.byref(tab), int(hash_bits), rows.data_ptr(), keys.data_ptr(), nk.data_ptr(),
-                                    ws.data_ptr(), ws.numel(), status.data_ptr(), st), "pert_raw_dedup")
-        N = int(nk.item())                                                           # sync 2
-        order = rows[:N].long()[torch.sort(keys[:N], stable=True).indices].contiguous()
+        f = _front(raw, dev, hash_bits)
+        tab, N = f.tab, f.N
         nbytes = int(L.pert_raw_process_workspace_bytes(C.byref(tab), N))
         if nbytes < 0:
             raise _lib.PertGnnError("process_raw: table sizes out of range")
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        sizes = torch.empty(7, **i64)
-        _lib.check(L.pert_raw_process(C.byref(tab), N, _lib.ptr(order), has_res.data_ptr(), int(min_occurence),
+        sizes = torch.empty(7, dtype=torch.int64, device=dev)
+        _lib.check(L.pert_raw_process(C.byref(tab), N, _lib.ptr(f.order), f.has_res.data_ptr(), int(min_occurence),
                                       sizes.data_ptr(), ws.data_ptr(), ws.numel(), st), "pert_raw_process")
         M, n_ids, n_tr, n_if, n_ent, n_rpc, n_rty = (int(v) for v in sizes.cpu())   # sync 3
-        # every output at least one element, so no pointer is NULL; sliced to its size
-        alloc = lambda n, *w: torch.empty(max(n, 1), *w, **i64)[:n]           # noqa: E731
-        t = {k: alloc(M) for k in COLUMNS + ("row",)}
-        t.update(res_index=alloc(G, 2), ms_code=alloc(n_ids), tr_code=alloc(n_tr), if_code=alloc(n_if),
-                 rpc_code=alloc(n_rpc), rty_code=alloc(n_rty), ent_dm=alloc(n_ent), ent_if=alloc(n_ent))
-        out = _lib.PertRawOut(*(t[k].data_ptr() for k in _lib.RAW_OUT))
-        _lib.check(L.pert_raw_emit(C.byref(tab), N, _lib.ptr(order), G, g_ts.data_ptr(), g_ms.data_ptr(),
+        t = _alloc_out(dev, M, f.G, n_ids, n_tr, n_if, n_ent, n_rpc, n_rty)
+        out = _raw_out(t)
+        _lib.check(L.pert_raw_emit(C.byref(tab), N, _lib.ptr(f.order), f.G, f.g_ts.data_ptr(), f.g_ms.data_ptr(),
                                    C.byref(out), ws.data_ptr(), ws.numel(), st), "pert_raw_emit")
-        t["res_vals"] = res_vals
-    return ProcessedTables(t, raw.dicts, status)
+        t["res_vals"] = f.res_vals
+    return ProcessedTables(t, raw.dicts, f.status)
+
+
+_STREAM_CODED = (("ms", "ms"), ("interface", "if"), ("rpcid", "rpc"), ("rpctype", "rty"))   # (dictionary, id array)
+_STREAM_NAMES = ("ms_names", "traceid_names", "interface_names", "rpcid_values", "rpctype_names", "entry_names")
+
+
+class RawStream:
+    """``process_raw`` a chunk at a time, with ids that stay fixed for the life of the stream: what a serving loop
+    needs to turn the raw ``MSCallGraph`` / ``MSResource`` rows a cluster keeps emitting into ``append_traces`` /
+    ``ResourceSampleWindow.add`` input that agrees with a live ``PatternStore``.
+
+    ``process(raw)`` takes a ``RawTables`` with its own dictionaries (what ``read_raw`` returns) and runs
+    ``process_raw``'s steps over that chunk alone, continued from the stream's state (DESIGN.md §8p):
+      - deduplication and the timestamp sort are chunk-local; traceid ids continue a counter (next + rank of the
+        trace's first sorted position); a traceid an earlier chunk held is refused, so chunks hold whole traces;
+      - interface (all rows), rpcid and rpctype (rows of traces with an entry) values keep the id they have; a value
+        without one gets next + its rank by first sorted position among the chunk's new values;
+      - entries are keyed by (dm, interface); a known key keeps its id, new keys are numbered next + rank by first
+        position over the traces with an entry, before the filters (so gaps stay, as in process_raw);
+      - coverage reads every microservice with a resource row in this chunk or an earlier one;
+      - occurrence: a chunk's covered traces of entry e are kept iff e's covered traces over the stream so far,
+        this chunk included, are more than ``min_occurence``.  Traces dropped before their entry was admitted are
+        never revisited: the one departure from a whole-table run;
+      - a microservice gets an id the first time it appears in a surviving row's um / dm or in a chunk's resource
+        rows: next + its rank in name order among the chunk's new names.
+    The result is a ``ProcessedTables`` whose ids index the stream's name lists (each covering every id issued up to
+    that chunk), plus ``resource_ms`` (int64 CUDA [K]): each raw resource row's microservice id, -1 for a row
+    process_raw leaves out.  A fresh stream's first chunk gives process_raw's result bit for bit.
+
+    Refused with ``PertGnnError``, the stream left bit for bit as it was: a traceid of an earlier chunk (named), a
+    chunk whose new microservice ids would reach ``max_ms`` (the store's fixed ``n_ms``; None = no limit), a
+    dictionary that repeats a value or holds an unhashable one, and the sizes process_raw refuses (``TypeError`` for
+    something that is not a RawTables).  Codes outside a chunk's dictionary set the status word, as in process_raw.
+
+    Device state, O(dictionary sizes): an int64 id per stream code of the microservice, interface, rpcid and rpctype
+    dictionaries, an int32 has_res per microservice, and the entry table (two int64 per slot, load <= 1/2) with an
+    int64 count per entry.  Host state: the value -> stream code dictionaries, the id -> value lists, and a set of
+    every traceid seen -- the one part that grows with traces (about 150 bytes per trace for short string ids)."""
+
+    def __init__(self, device="cuda", min_occurence=100, max_ms=None, hash_bits=64):
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise _lib.PertGnnError("RawStream needs a CUDA device (no CPU fallback)")
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        if not 1 <= int(hash_bits) <= 64:
+            raise _lib.PertGnnError("RawStream: hash_bits must lie in 1..64")
+        self._reset(dev, min_occurence, max_ms, hash_bits)
+
+    def _reset(self, dev, min_occurence, max_ms, hash_bits):
+        self.device, self.min_occurence, self.max_ms, self.hash_bits = dev, int(min_occurence), max_ms, int(hash_bits)
+        self._codes = {k: {} for k, _ in _STREAM_CODED}          # value -> stream code
+        self._traceids = set()
+        self._names = {k: [] for k in _STREAM_NAMES}
+        self._n = dict(tr=0, **{a: 0 for _, a in _STREAM_CODED}, ent=0)   # ids issued
+        i32, i64 = (dict(dtype=d, device=dev) for d in (torch.int32, torch.int64))
+        self.t = {f"{a}_id": torch.zeros(0, **i64) for _, a in _STREAM_CODED}
+        self.t.update(has_res=torch.zeros(0, **i32), ent_key=torch.full((64,), -1, **i64),
+                      ent_id=torch.zeros(64, **i64), ent_cnt=torch.zeros(0, **i64))
+
+    n_ms = property(lambda self: self._n["ms"], doc="microservice ids issued so far")
+    ms_names = property(lambda self: list(self._names["ms_names"]))
+    traceid_names = property(lambda self: list(self._names["traceid_names"]))
+    interface_names = property(lambda self: list(self._names["interface_names"]))
+    rpcid_values = property(lambda self: list(self._names["rpcid_values"]))
+    rpctype_names = property(lambda self: list(self._names["rpctype_names"]))
+    entry_names = property(lambda self: list(self._names["entry_names"]))
+
+    def _map(self, raw):
+        """Chunk code -> stream code of every coded dictionary (new values numbered after the known ones, not yet
+        added), and the chunk's traceids; refuses repeated or unhashable values and traceids of earlier chunks."""
+        maps, new = {}, {}
+        for col, _ in _STREAM_CODED:
+            known, add = self._codes[col], {}
+            vals, n = raw.dicts[col], len(self._codes[col])
+            try:
+                m = np.fromiter((known[v] if v in known else add.setdefault(v, n + len(add)) for v in vals),
+                                np.int64, len(vals))
+            except TypeError:
+                raise _lib.PertGnnError(f"RawStream.process: a {col} dictionary value is not hashable") from None
+            if len(np.unique(m)) != len(m):
+                raise _lib.PertGnnError(f"RawStream.process: the {col} dictionary repeats a value")
+            maps[col], new[col] = m, add
+        trs = raw.dicts["traceid"]
+        try:
+            tset = set(trs)
+        except TypeError:
+            raise _lib.PertGnnError("RawStream.process: a traceid is not hashable") from None
+        if len(tset) != len(trs):
+            raise _lib.PertGnnError("RawStream.process: the traceid dictionary repeats a value")
+        if not self._traceids.isdisjoint(tset):
+            v = next(v for v in trs if v in self._traceids)
+            raise _lib.PertGnnError(f"RawStream.process: traceid {v!r} was in an earlier chunk (a chunk holds whole "
+                                    "traces)")
+        return maps, new, tset
+
+    def _state(self, maps):
+        t, n = self.t, self._n
+        p = lambda x: x.data_ptr() if x.numel() else None     # noqa: E731
+        return _lib.PertRawState(*(p(maps[c]) for c, _ in _STREAM_CODED), *(p(t[f"{a}_id"]) for _, a in _STREAM_CODED),
+                                 *(len(self._codes[c]) for c, _ in _STREAM_CODED), p(t["has_res"]),
+                                 p(t["ent_key"]), p(t["ent_id"]), p(t["ent_cnt"]), int(t["ent_key"].shape[0]),
+                                 n["tr"], n["if"], n["rpc"], n["rty"], n["ent"], n["ms"])
+
+    def process(self, raw):
+        """The next chunk -> ProcessedTables with the stream's ids (and ``resource_ms``); see the class.  Host
+        synchronisations: process_raw's three, then one copy of the new ids' codes, which extends the name lists.
+        Call ``check()`` on the result before trusting it."""
+        _check_raw(raw, "RawStream.process", self.hash_bits)
+        maps, new, tset = self._map(raw)
+        dev = self.device
+        with torch.cuda.device(dev):
+            L, st = _lib.lib(), _lib.stream()
+            i64 = dict(dtype=torch.int64, device=dev)
+            dmaps = {c: torch.from_numpy(m).to(dev) for c, m in maps.items()}
+            f = _front(raw, dev, self.hash_bits)
+            tab, N = f.tab, f.N
+            state = self._state(dmaps)
+            ws = torch.empty(int(L.pert_raw_stream_workspace_bytes(C.byref(tab), N)), dtype=torch.uint8,
+                             device=dev)
+            sizes = torch.empty(7, **i64)
+            _lib.check(L.pert_raw_stream_process(C.byref(tab), N, _lib.ptr(f.order), f.has_res.data_ptr(),
+                                                 self.min_occurence, C.byref(state), sizes.data_ptr(), ws.data_ptr(),
+                                                 ws.numel(), st), "pert_raw_stream_process")
+            M, n_ids, n_tr, n_if, n_ent, n_rpc, n_rty = (int(v) for v in sizes.cpu())   # sync 3
+            n = self._n
+            if self.max_ms is not None and n["ms"] + n_ids > int(self.max_ms):
+                raise _lib.PertGnnError(f"RawStream.process: the chunk brings {n_ids} new microservices; "
+                                        f"{n['ms']} + {n_ids} ids would reach max_ms = {int(self.max_ms)}")
+            # fresh state: the old contents, then room for the chunk's new stream codes and entries
+            old = self.t
+            fresh = {f"{a}_id": torch.cat([old[f"{a}_id"], torch.full((len(new[c]),), -1, **i64)])
+                     for c, a in _STREAM_CODED}
+            fresh["has_res"] = torch.cat([old["has_res"], torch.zeros(len(new["ms"]), dtype=torch.int32,
+                                                                      device=dev)])
+            n_ent2, cap = n["ent"] + n_ent, int(old["ent_key"].shape[0])
+            while 2 * n_ent2 > cap:
+                cap *= 2
+            fresh["ent_key"], fresh["ent_id"] = torch.empty(cap, **i64), torch.empty(cap, **i64)
+            fresh["ent_cnt"] = torch.zeros(max(n_ent2, 1), **i64)[:n_ent2]
+            fresh["ent_cnt"][:n["ent"]] = old["ent_cnt"]
+            K = len(raw.resources["timestamp"])
+            resource_ms = torch.empty(max(K, 1), **i64)[:K]
+            t = _alloc_out(dev, M, f.G, n_ids, n_tr, n_if, n_ent, n_rpc, n_rty)
+            spare = torch.empty(1, **i64)                        # an empty chunk's outputs point here
+            out = _raw_out(t, spare)
+            p = lambda x: x.data_ptr() if x.numel() else None     # noqa: E731
+            so = _lib.PertRawStateOut(*(p(fresh[k]) for k in ("ms_id", "if_id", "rpc_id", "rty_id", "has_res",
+                                                              "ent_key", "ent_id")),
+                                      fresh["ent_cnt"].data_ptr(), cap, p(resource_ms))
+            _lib.check(L.pert_raw_stream_emit(C.byref(tab), N, _lib.ptr(f.order), f.G, f.g_ts.data_ptr(),
+                                              f.g_ms.data_ptr(), K, p(f.r_ms), f.has_res.data_ptr(), C.byref(state),
+                                              C.byref(out), C.byref(so), ws.data_ptr(), ws.numel(), st),
+                       "pert_raw_stream_emit")
+            # accepted: swap the state in, then name the new ids
+            self.t = fresh
+            for c, _ in _STREAM_CODED:
+                self._codes[c].update(new[c])
+            self._traceids |= tset
+            for k, v in (("tr", n_tr), ("ms", n_ids), ("if", n_if), ("rpc", n_rpc), ("rty", n_rty), ("ent", n_ent)):
+                n[k] += v
+            h = {k: v.tolist() for k, v in zip(("ms_code", "tr_code", "if_code", "rpc_code", "rty_code", "ent_dm",
+                                                "ent_if"),
+                                               t["_codes"].cpu().split([n_ids, n_tr, n_if, n_rpc, n_rty, n_ent,
+                                                                        n_ent]))}   # sync 4
+            d, nm = raw.dicts, self._names
+            nm["ms_names"] += [d["ms"][i] for i in h["ms_code"]]
+            nm["traceid_names"] += [d["traceid"][i] for i in h["tr_code"]]
+            nm["interface_names"] += [d["interface"][i] for i in h["if_code"]]
+            nm["rpcid_values"] += [d["rpcid"][i] for i in h["rpc_code"]]
+            nm["rpctype_names"] += [d["rpctype"][i] for i in h["rty_code"]]
+            nm["entry_names"] += [f"{d['ms'][m]}_{i}" for m, i in zip(h["ent_dm"], h["ent_if"])]
+            t["res_vals"] = f.res_vals
+        views = {k: (v, len(v)) for k, v in nm.items()}
+        res = ProcessedTables(t, raw.dicts, f.status, views=views, n_ms=n["ms"])
+        res.resource_ms = resource_ms
+        return res
 
 
 def list_csvs(directory):
